@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
-"""bench.py -- haystack GB/s of the batched Aho-Corasick search on B200 (BASELINE.json metric).
+"""bench.py -- haystack GB/s of the batched Aho-Corasick search on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config C2] [--impl ours|reference] [--mode strong|weak]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic haystacks.
 
@@ -22,6 +23,11 @@ A "step" is one pass of the hot path over one batch of synthetic haystacks.
   cpu_baseline  the reference's own C extension (oracle/_ref) looping iter() over the whole batch, single thread (the
             reference holds the GIL), rank 0 at N=1; its match list is compared with the GPU's (parity_checked)
   latency   microseconds per Automaton.iter() call on ONE haystack of 256 B / 64 KiB / 16 MiB, ours vs the reference
+
+--dump-outputs DIR writes what the last timed step computed (rank 0's records) as float64 .npy files: records.npy,
+one row (hay_id, end_index, key_id) per match in ascending order -- the kernels append records in no fixed order, so
+they are sorted to make two builds comparable -- at most 64 MiB of them (beyond that a fixed, seeded sample of rows),
+and match_count.npy.  The inputs are seeded: the same arguments give the same batch on every run.
 
 --impl reference times the reference extension on the host cores (one process per core, the pool created once, each
 worker looping iter() over its slice of a bounded sample) and prints the same JSON shape.
@@ -64,7 +70,23 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-latency", action="store_true")
     ap.add_argument("--variant", default="planted", choices=["planted", "sparse"], help="sparse = pure random haystacks (diagnostic)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's records to DIR/*.npy")
     return ap.parse_args()
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, records, n_matches):
+    """records: (n, 3) int32 (hay_id, end_index, key_id) in the order the kernel appended them"""
+    os.makedirs(out_dir, exist_ok=True)
+    rec = records[np.lexsort((records[:, 2], records[:, 1], records[:, 0]))].astype(np.float64)
+    max_rows = DUMP_BYTES // (3 * 8) - 1
+    if rec.shape[0] > max_rows:
+        rng = np.random.Generator(np.random.PCG64(0))
+        rec = rec[np.sort(rng.choice(rec.shape[0], size=max_rows, replace=False))]
+    np.save(os.path.join(out_dir, "records.npy"), rec)
+    np.save(os.path.join(out_dir, "match_count.npy"), np.array([n_matches], dtype=np.float64))
 
 
 def default_scale(cfg, world):
@@ -437,6 +459,9 @@ def main():
     barrier()
     ms_total = ev0.elapsed_time(ev1)
     kernel_ms = float(np.mean([a.elapsed_time(b) for a, b in kev]))
+    if args.dump_outputs and rank == 0:
+        n_last = int(d_cnt.item())
+        dump_outputs(args.dump_outputs, d_out[:min(n_last, cap)].cpu().numpy(), n_last)
     launches = L.acb_launch_count() - launches0
     t = torch.tensor([ms_total], dtype=torch.float64, device="cuda")
     tot_bytes = torch.tensor([total], dtype=torch.int64, device="cuda")
@@ -496,7 +521,7 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
     algo_bytes = total + 12 * n_matches
     achieved = algo_bytes / (kernel_ms * 1e-3) / 1e9
     traffic = None
@@ -542,7 +567,7 @@ def main():
             "vs_baseline": None, "dtype": "u8", "data": "synthetic",
             "config": {"workload": WORKLOAD_DESC[cfg] + ("" if args.variant == "planted" else " [SPARSE variant: no planted keys]") + ("" if scale == default_scale(cfg, world) else f" [SCALED x{scale}: not a valid bench number]"),
                        "n_haystacks_per_gpu": n_hay, "haystack_bytes": stride, "n_keys": len(w.keys),
-                       "l2": f"batch {total / 1e6:.0f} MB per GPU > 126 MB L2, no flush needed" if total > 126e6 else "batch smaller than L2",
+                       "l2": f"batch {total / 1e6:.0f} MB per GPU > 50 MB L2, no flush needed" if total > 50e6 else "batch smaller than L2",
                        "algo": args.algo,
                        "parallelism": (f"one batch sharded x{world} (strong scaling)" if strong else f"one batch per rank x{world} (weak scaling)") + ", NCCL all-gather of match counts on a side stream" if world > 1 else "single GPU"},
             "matches_per_s": total_matches / (ms_step * 1e-3), "matches_per_step": total_matches,

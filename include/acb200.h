@@ -1,5 +1,5 @@
 /*
- * acb200.h -- C ABI of the B200-native Aho-Corasick batch-search path.
+ * acb200.h -- C ABI of the H100-native Aho-Corasick batch-search path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch / Python types.
  * The reference (WojciechMula/pyahocorasick v2.2.0) has no C plugin ABI of its own --
@@ -37,7 +37,7 @@ enum {
     ACB_ENOMEM    = -1,   /* -> MemoryError   (reference: PyErr_NoMemory everywhere)           */
     ACB_EINVAL    = -2,   /* -> ValueError / TypeError at the Python layer                      */
     ACB_ESTATE    = -3,   /* automaton not in the AHOCORASICK state (src/Automaton.c:886-891)   */
-    ACB_ECUDA     = -4,   /* CUDA runtime / launch failure, no device, no sm_100a image          */
+    ACB_ECUDA     = -4,   /* CUDA runtime / launch failure, no device, no sm_90a image           */
     ACB_EOVERFLOW = -5,   /* match buffer too small: *n_found holds the required capacity        */
     ACB_ERANGE    = -6    /* size beyond what int32 state ids / end_index can hold               */
 };

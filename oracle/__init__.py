@@ -1,4 +1,4 @@
-"""oracle -- the CPU checker for the B200 Aho-Corasick search path.
+"""oracle -- the CPU checker for the GPU Aho-Corasick search path.
 
 TEST INFRASTRUCTURE ONLY.  Importable from ``tests/``, ``__graft_entry__.smoke()``
 and ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs; nothing under

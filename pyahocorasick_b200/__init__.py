@@ -1,4 +1,4 @@
-"""pyahocorasick_b200 -- B200-native Aho-Corasick batch search behind the
+"""pyahocorasick_b200 -- H100-native Aho-Corasick batch search behind the
 ``ahocorasick.Automaton`` API of WojciechMula/pyahocorasick.
 
     import pyahocorasick_b200 as ahocorasick

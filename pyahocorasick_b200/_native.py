@@ -50,7 +50,7 @@ def lib() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -m pyahocorasick_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU fallback.")
+            "(nvcc, sm_90a).  There is no CPU fallback.")
     L = ctypes.CDLL(LIB_PATH)
     vp, i32, i64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64
     pi32, pi64 = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int64)

@@ -1,5 +1,5 @@
 """`Automaton` -- the reference's Python surface (src/Automaton.c:1204-1256) on top of the
-B200 C ABI (include/acb200.h).
+H100 C ABI (include/acb200.h).
 
 Host side (this file + csrc/acb_host.cpp): keys, values, state machine EMPTY -> TRIE ->
 AHOCORASICK, argument parsing and error behaviour of the reference.

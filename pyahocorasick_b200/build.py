@@ -1,9 +1,8 @@
-"""Build the native library in-tree: pyahocorasick_b200/_native/libacb200.so (sm_100a only).
+"""Build the native library in-tree: pyahocorasick_b200/_native/libacb200.so (sm_90a only).
 
     python -m pyahocorasick_b200.build [--force] [--verbose]
 
-nvcc cross-compiles without a GPU, so this runs in the CPU-only build container;
-the resulting .so travels to the GPU box with the repository snapshot.
+nvcc cross-compiles without a GPU, so the library can be built on a machine that has none.
 """
 from __future__ import annotations
 
@@ -21,7 +20,7 @@ HEADERS = ["acb_hash.h", "acb_internal.h", os.path.join("..", "..", "include", "
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-Xcompiler", "-fPIC,-O3,-Wall",
     "-shared",
@@ -32,7 +31,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found (needed to build libacb200.so for sm_100a)")
+    raise RuntimeError("nvcc not found (needed to build libacb200.so for sm_90a)")
 
 
 def needs_build() -> bool:

@@ -1,5 +1,5 @@
 /*
- * acb_device.cu -- sm_100a scan kernels and the device half of the C ABI (include/acb200.h).
+ * acb_device.cu -- sm_90a scan kernels and the device half of the C ABI (include/acb200.h).
  *
  * ACB_ALGO_FILTER (the fast path) is ONE launch per <= 2 GiB segment of the batch, of one of two streaming kernels
  * (both persistent, one CTA per SM, warp specialised):

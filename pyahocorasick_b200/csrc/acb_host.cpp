@@ -1,5 +1,5 @@
 /*
- * acb_host.cpp -- host side of the B200 Aho-Corasick path: trie arena, failure
+ * acb_host.cpp -- host side of the H100 Aho-Corasick path: trie arena, failure
  * links, flattening to int32 tables, gram-filter construction.
  *
  * Not a port of the reference's node graph (src/trienode.h:19-42: one malloc per

@@ -1,18 +1,17 @@
-"""bench.py contract, the parts that run without a GPU: the reference arm prints ONE JSON line with the keys the
-driver reads, measured through the unmodified reference extension on the host cores."""
+"""bench.py contract, the parts that run without a GPU: the reference arm prints ONE JSON line with the keys a caller
+reads, measured through the unmodified reference extension on the host cores where oracle/_ref is built, else through
+the C restatement (kind 'port')."""
 import json
 import os
 import subprocess
 import sys
 
-import pytest
 
 import oracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.mark.skipif(not oracle.ref_available("bytes"), reason="needs oracle/_ref")
 def test_reference_arm_prints_one_json_line():
     res = subprocess.run([sys.executable, "bench.py", "--impl", "reference", "--steps", "1", "--warmup", "0"],
                          cwd=ROOT, capture_output=True, text=True, timeout=300)
@@ -22,7 +21,7 @@ def test_reference_arm_prints_one_json_line():
     d = json.loads(lines[0])
     assert d["impl"] == "reference" and d["metric"] == "haystack GB/s" and d["unit"] == "GB/s"
     assert d["higher_is_better"] is True and d["vs_baseline"] is None and d["dtype"] == "u8" and d["gpu_launches"] == 0
-    assert d["value"] > 0 and d["cpu_baseline"]["kind"] == "reference" and d["cpu_baseline"]["cores"] >= 1
+    assert d["value"] > 0 and d["cpu_baseline"]["kind"] == ("reference" if oracle.ref_available("bytes") else "port") and d["cpu_baseline"]["cores"] >= 1
     assert d["cpu_baseline"]["value"] == d["value"] == d["e2e"]["value"]
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
     assert "workload" in d["config"] and d["steps"] == 1 and d["warmup"] == 0

@@ -1,9 +1,10 @@
-"""Parity of the CUDA path (through the C ABI) with the reference -- run with `-m gpu` on a B200.
+"""Parity of the CUDA path (through the C ABI) with the reference -- run with `-m gpu` on an H100.
 
 Bar: bit-exact records (integer/index work).  Sources of truth, in order:
   1. tests/golden/*.json  -- produced by the unmodified reference (both flavours);
   2. oracle.OracleAutomaton -- the pinned C restatement, on seeded random batches at sizes it
-     finishes in seconds; the compiled reference (oracle/_ref) too when it travelled along;
+     finishes in seconds; the reference too, through digests of the records it produced for the same
+     seeded batches (tests/golden/reference_digests.json, tests/refreplay.py);
   3. at BASELINE.json's full sizes: properties that need no CPU run -- every planted
      occurrence is reported, no duplicates, each reported record really is an occurrence
      (sampled), and the two independent kernels (filter / DFA) agree exactly.
@@ -14,6 +15,7 @@ import pytest
 import oracle
 import pyahocorasick_b200 as ac
 from golden_driver import all_scenarios, run_ops
+from refreplay import digest, records_digest, reference_records
 from pyahocorasick_b200 import automaton as am
 from pyahocorasick_b200 import synth
 
@@ -97,20 +99,23 @@ def test_random_batches_match_oracle(case, algo):
     assert _records(A.find_all_batch(hs, algo=algo)) == want3
 
 
-@pytest.mark.skipif(not oracle.ref_available("bytes"), reason="oracle/_ref did not travel")
+def c2_sample():
+    return synth.make("C2", scale=0.005)
+
+
+def reference_c2_sample():
+    w = c2_sample()
+    return records_digest("c2_sample", lambda: reference_records(w.keys, [row.tobytes() for row in w.haystacks]))
+
+
 def test_reference_extension_agrees_on_c2_sample():
-    """The unmodified reference (compiled into oracle/_ref) on a C2 sub-sample."""
-    ref = oracle.ref_module("bytes")
-    w = synth.make("C2", scale=0.005)
-    R = ref.Automaton(ref.STORE_INTS)
-    for i, k in enumerate(w.keys):
-        R.add_word(k, i)
-    R.make_automaton()
+    """The unmodified reference on a C2 sub-sample: the digest of its records."""
+    w = c2_sample()
+    want = reference_c2_sample()
     A = synth.build_automaton(w.keys)
-    want = oracle.ref_scan_batch(R, [row.tobytes() for row in w.haystacks])
     for algo in ("filter", "dfa"):
         m = A.find_all_batch(w.haystacks, algo=algo)
-        assert list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.values())) == want
+        assert digest(list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.values()))) == want
 
 
 def test_iter_long_batch_matches_oracle():
@@ -231,19 +236,25 @@ def _check_full(w, A, sample=20000):
     return len(got)
 
 
-def _check_reference_rows(w, A, rows):
-    """the compiled reference (oracle/_ref) over the listed haystacks: identical records in identical order"""
-    if not oracle.ref_available("bytes"):
-        pytest.skip("oracle/_ref did not travel")
-    ref = oracle.ref_module("bytes")
-    R = ref.Automaton(ref.STORE_INTS)
-    for i, k in enumerate(w.keys):
-        R.add_word(k, i)
-    R.make_automaton()
-    sub = np.ascontiguousarray(w.haystacks[rows])
-    want = [(h, e, v) for h in range(len(rows)) for e, v in R.iter(sub[h].tobytes())]
-    m = A.find_all_batch(sub)
-    assert list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.values())) == want
+def reference_rows(name, w, rows):
+    """the digest of the reference's records over the listed haystacks"""
+    return records_digest(name, lambda: reference_records(w.keys, [w.haystacks[h].tobytes() for h in rows]))
+
+
+def _check_reference_rows(name, w, A, rows):
+    """the reference over the listed haystacks: identical records in identical order"""
+    want = reference_rows(name, w, rows)
+    m = A.find_all_batch(np.ascontiguousarray(w.haystacks[rows]))
+    assert digest(list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.values()))) == want
+
+
+# the full-size workloads and the haystacks of each that are compared with the reference
+FULL_ROWS = {
+    "c2_rows": lambda w: np.arange(0, w.n_hay, 10),       # every 10th haystack: 100 k, BASELINE.md section 2
+    "c3_rows": lambda w: np.arange(0, w.n_hay, 100),      # 100 k reads
+    "c4_rows": lambda w: np.array([1]),                   # one whole 16 MiB haystack
+    "c5_rows": lambda w: np.arange(0, w.n_hay, 10),
+}
 
 
 def test_full_size_c2_properties():
@@ -251,19 +262,18 @@ def test_full_size_c2_properties():
     A = synth.build_automaton(w.keys)
     n = _check_full(w, A)
     assert n >= w.n_hay
-    _check_reference_rows(w, A, np.arange(0, w.n_hay, 10))           # every 10th haystack: 100 k, BASELINE.md section 2
+    _check_reference_rows("c2_rows", w, A, FULL_ROWS["c2_rows"](w))
 
 
 def test_full_size_c3_dna_properties():
     w = synth.make("C3", scale=1.0)          # BASELINE config 3 at its stated size: 10 M reads x 150 B, 100 k 20-mers
     A = synth.build_automaton(w.keys)
     _check_full(w, A)
-    _check_reference_rows(w, A, np.arange(0, w.n_hay, 100))          # 100 k reads through the reference
+    _check_reference_rows("c3_rows", w, A, FULL_ROWS["c3_rows"](w))
 
 
-def test_full_size_c4_long_haystacks_properties():
+def c4_with_straddlers():
     w = synth.make("C4", scale=1.0)          # BASELINE config 4 at its stated size: 64 x 16 MiB, a key across every 16 KiB
-    A = synth.build_automaton(w.keys)
     # more straddlers, one across every boundary the kernel or the host pipeline has: 512-byte slices of a tile, the
     # tiles themselves, and the 32 MiB chunks of the pipelined host scan (minus the reach of the longest key)
     flat = w.haystacks.reshape(-1)
@@ -292,15 +302,21 @@ def test_full_size_c4_long_haystacks_properties():
         ok[sel] = (got == want).all(axis=1)
     w.planted_hay, w.planted_end, w.planted_key = ph[ok], pe[ok], pk[ok]
     assert len(extra_h) > 40
+    return w
+
+
+def test_full_size_c4_long_haystacks_properties():
+    w = c4_with_straddlers()
+    A = synth.build_automaton(w.keys)
     _check_full(w, A)
-    _check_reference_rows(w, A, np.array([1]))                        # one whole 16 MiB haystack through the reference
+    _check_reference_rows("c4_rows", w, A, FULL_ROWS["c4_rows"](w))
 
 
 def test_c5_100k_keys_properties():
     w = synth.make("C5", scale=0.125)        # 1 M x 256 B (one GPU's shard of BASELINE config 5), 100 k keys
     A = synth.build_automaton(w.keys)
     _check_full(w, A)
-    _check_reference_rows(w, A, np.arange(0, w.n_hay, 10))
+    _check_reference_rows("c5_rows", w, A, FULL_ROWS["c5_rows"](w))
 
 
 def test_dense_matches_grow_the_buffers():

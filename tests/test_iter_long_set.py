@@ -6,14 +6,12 @@ import numpy as np
 import pytest
 
 import emul
-import oracle
 import pyahocorasick_b200 as pkg
-
-needs_ref = pytest.mark.skipif(not oracle.ref_available("bytes"), reason="needs oracle/_ref")
+from refreplay import reference
 
 
 def _fuzz(fl, trials, seed):
-    ref, mod = oracle.ref_module(fl), pkg.flavour(fl)
+    ref, mod = reference(fl), pkg.flavour(fl)
     rng = np.random.default_rng(seed)
     al = "abc"
 
@@ -22,7 +20,7 @@ def _fuzz(fl, trials, seed):
         return s.encode() if fl == "bytes" else s
 
     for _ in range(trials):
-        keys = list({word(1, 5) for _ in range(int(rng.integers(1, 8)))})
+        keys = list(dict.fromkeys(word(1, 5) for _ in range(int(rng.integers(1, 8)))))
         A, R = mod.Automaton(), ref.Automaton()
         for i, k in enumerate(keys):
             A.add_word(k, i), R.add_word(k, i)
@@ -46,14 +44,12 @@ def _fuzz(fl, trials, seed):
         assert got == want, (fl, keys, chunks)
 
 
-@needs_ref
 @pytest.mark.parametrize("fl", ["bytes", "unicode"])
 def test_iter_long_set_matches_the_reference_emulated(fl, monkeypatch):
     emul.install(monkeypatch, "filter")
     _fuzz(fl, 150, 11)
 
 
-@needs_ref
 @pytest.mark.gpu
 @pytest.mark.parametrize("fl", ["bytes", "unicode"])
 def test_iter_long_set_matches_the_reference_on_gpu(fl):
@@ -126,11 +122,10 @@ def test_iter_long_stream_uploads_only_the_new_chunk(monkeypatch):
     assert sizes[-5:] == [1] * 5
 
 
-@needs_ref
 @pytest.mark.gpu
 def test_iter_long_long_stream_on_gpu():
     """the same stream through the real ACB_ALGO_LONG kernel, against the reference extension"""
-    ref, mod = oracle.ref_module("bytes"), pkg.flavour("bytes")
+    ref, mod = reference("bytes"), pkg.flavour("bytes")
     A, R = _stream_case(mod), _stream_case(ref)
     rng = np.random.default_rng(5)
     ia, ir = A.iter_long(b"z" * 100), R.iter_long(b"z" * 100)

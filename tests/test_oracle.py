@@ -1,13 +1,14 @@
 """Pin the CPU oracle (oracle/ac_oracle.c) before anything trusts it.
 
 1. against the committed golden vectors (produced by the reference itself),
-2. against the compiled reference (oracle/_ref) on seeded random batches, when present.
+2. against the reference on seeded random batches (its recorded answers and record digests, tests/refreplay.py).
 """
 import numpy as np
 import pytest
 
 import oracle
 from golden_driver import all_scenarios, dec
+from refreplay import digest, records_digest, reference, reference_records
 
 STORE_INTS, STORE_LENGTH, STORE_ANY = 10, 20, 30
 
@@ -108,7 +109,6 @@ def test_oracle_matches_golden(sc):
     assert checked or not sc.get("make", True) or not sc["words"]
 
 
-@pytest.mark.skipif(not oracle.ref_available("bytes"), reason="oracle/_ref not built")
 @pytest.mark.parametrize("seed,alpha,nw,lens,nh,hl", [
     (1, b"ab", 30, (1, 8), 50, 300),
     (2, b"ACGT", 2000, (8, 12), 200, 150),
@@ -116,7 +116,9 @@ def test_oracle_matches_golden(sc):
     (4, bytes(range(256)), 500, (1, 4), 100, 1000),
 ])
 def test_oracle_matches_reference_batch(seed, alpha, nw, lens, nh, hl):
-    ref = oracle.ref_module("bytes")
+    """the C restatement against the reference: same counts, and records equal to the reference's (their digest,
+    tests/golden/reference_digests.json, recorded from the unmodified extension)"""
+    ref = reference("bytes")
     rng = np.random.Generator(np.random.PCG64(seed))
     al = np.frombuffer(alpha, dtype=np.uint8)
     R = ref.Automaton(ref.STORE_INTS)
@@ -138,6 +140,7 @@ def test_oracle_matches_reference_batch(seed, alpha, nw, lens, nh, hl):
         flat[h * hl + p:h * hl + p + len(k)] = k
     off = np.arange(nh + 1, dtype=np.int64) * hl
     got = O.scan_batch_bytes(flat, off)
-    want = oracle.ref_scan_batch(R, [flat[off[h]:off[h + 1]].tobytes() for h in range(nh)])
-    assert len(want) > 0
-    assert [tuple(r) for r in got.tolist()] == want      # same records, same order
+    hays = [flat[off[h]:off[h + 1]].tobytes() for h in range(nh)]
+    want = records_digest(f"oracle_batch_{seed}", lambda: reference_records(keys, hays))
+    assert want["records"] > 0
+    assert digest(got) == want                            # same records, same order

@@ -4,7 +4,7 @@
 set -e
 cd "$(dirname "$0")/.."
 OUT=${1:-/tmp/libacb200_asan.so}
-( cd pyahocorasick_b200/csrc && nvcc -O1 -g -std=c++17 -gencode arch=compute_100a,code=sm_100a \
+( cd pyahocorasick_b200/csrc && nvcc -O1 -g -std=c++17 -gencode arch=compute_90a,code=sm_90a \
     -Xcompiler -fPIC,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -shared \
     -o "$OUT" acb_host.cpp acb_device.cu -Xlinker -lasan -Xlinker -lubsan )
 ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1 \

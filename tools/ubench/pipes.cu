@@ -1,4 +1,4 @@
-// instruction issue-rate microbenchmark for sm_100a: N independent chains of one PTX instruction per thread,
+// instruction issue-rate microbenchmark for sm_90a: N independent chains of one PTX instruction per thread,
 // 8 warps per SM sub-partition, cycles per warp-instruction per sub-partition reported.
 #include <cstdio>
 #include <cstdint>
@@ -46,9 +46,9 @@ __global__ void k(uint32_t *out, uint32_t seed, unsigned long long *cyc) {
 }
 template <int OP> void run(const char *name, uint32_t *d, unsigned long long *dc) {
     const int threads = 1024;                       // 32 warps = 8 per sub-partition
-    k<OP><<<148, threads>>>(d, 12345u, dc);
+    k<OP><<<132, threads>>>(d, 12345u, dc);
     cudaDeviceSynchronize();
-    k<OP><<<148, threads>>>(d, 12345u, dc);
+    k<OP><<<132, threads>>>(d, 12345u, dc);
     cudaDeviceSynchronize();
     unsigned long long c = 0; cudaMemcpy(&c, dc, 8, cudaMemcpyDeviceToHost);
     double per = (double)c / ((double)ITERS * CHAINS * 8.0);      // 8 warps per sub-partition issue ITERS*CHAINS each
@@ -56,7 +56,7 @@ template <int OP> void run(const char *name, uint32_t *d, unsigned long long *dc
 }
 int main() {
     uint32_t *d; unsigned long long *dc;
-    cudaMalloc(&d, 148 * 1024 * 4); cudaMalloc(&dc, 8);
+    cudaMalloc(&d, 132 * 1024 * 4); cudaMalloc(&dc, 8);
     run<0>("mul.lo.u32", d, dc); run<1>("mad.lo.u32", d, dc); run<2>("mul.hi.u32", d, dc); run<12>("mad.hi.u32", d, dc);
     run<3>("mul.wide.u32 (+xor)", d, dc); run<4>("dp4a.u32.u32", d, dc); run<19>("dp2a.lo.u32.u32", d, dc);
     run<5>("shf.r.wrap", d, dc); run<16>("shf.l.wrap (rot)", d, dc); run<6>("lop3", d, dc); run<7>("prmt", d, dc);
