@@ -370,7 +370,7 @@ static int ceil_log2_u64(uint64_t x) {
  *     device walks the trie from the root at q-j.
  * Entry = 8 x uint32: tag (hash2|1, 0 = empty), key_id (-1 = MULTI), j | len<<8 | last<<16 (last = no
  * further entry with this tag in the probe sequence), 20 key/gram bytes. */
-static void build_filter(acb_trie *t, Flat &f) {
+static int build_filter(acb_trie *t, Flat &f) {
     PhaseTimer pt;
     const int L = t->letter_bytes;
     const int m = f.min_key_bytes;
@@ -396,8 +396,34 @@ static void build_filter(acb_trie *t, Flat &f) {
         }
     }
     pt.lap("filter: prefixes");
-    int forced_g = 0, forced_s = 0, forced_l1 = 0, forced_mode = -1;     /* ACB_FILTER=g,s,log1,mode (0 single, 1 pair) */
-    if (const char *env = getenv("ACB_FILTER")) sscanf(env, "%d,%d,%d,%d", &forced_g, &forced_s, &forced_l1, &forced_mode);
+    /* ACB_FILTER=g,s,log1,mode (mode 0 single, 1 pair) forces the shape, for tests and experiments; a field left out or
+       given as 0 (mode: -1) stays the cost model's choice.  A shape the kernels cannot run is refused here rather
+       than built: a stride that is not L * 2^k <= 16, a level 1 outside 2^13..2^20 bits, a pair placement other than
+       gram 4 / stride 1 / 1-byte letters, or a gram / stride pair that this key set does not offer. */
+    int forced_g = 0, forced_s = 0, forced_l1 = 0, forced_mode = -1;
+    const char *forced = getenv("ACB_FILTER");
+    if (forced) {
+        const int n = sscanf(forced, "%d,%d,%d,%d", &forced_g, &forced_s, &forced_l1, &forced_mode);
+        if (n < 1) { acb_set_error("ACB_FILTER=\"%s\": expected g,s,log1,mode", forced); return ACB_EINVAL; }
+        if (forced_g < 0 || forced_g > ACB_MAX_GRAM || forced_g % L) {
+            acb_set_error("ACB_FILTER: gram %d is not a multiple of %d bytes in 1..%d", forced_g, L, ACB_MAX_GRAM);
+            return ACB_EINVAL;
+        }
+        if (forced_s && (forced_s < L || forced_s > 16 || (forced_s & (forced_s - 1)))) {
+            acb_set_error("ACB_FILTER: stride %d is not %d * 2^k <= 16", forced_s, L);
+            return ACB_EINVAL;
+        }
+        if (forced_l1 && (forced_l1 < 13 || forced_l1 > 20)) {
+            acb_set_error("ACB_FILTER: log1 %d is outside 13..20", forced_l1);
+            return ACB_EINVAL;
+        }
+        if (forced_mode < -1 || forced_mode > 1) { acb_set_error("ACB_FILTER: mode %d is neither 0 (single) nor 1 (pair)", forced_mode); return ACB_EINVAL; }
+        if (forced_mode == 1 && !(forced_g == 4 && forced_s == 1 && L == 1)) {
+            acb_set_error("ACB_FILTER: the pair placement needs gram 4, stride 1 and 1-byte letters (got gram %d, stride %d, %d-byte letters)",
+                          forced_g, forced_s, L);
+            return ACB_EINVAL;
+        }
+    }
 
     /* Pick gram length g, probe stride s and the placement (single / pair) by a small cost model, in issue
      * cycles per text byte of one SM sub-partition (DESIGN.md section 4.1): a single-position probe is bound by the
@@ -455,6 +481,11 @@ static void build_filter(acb_trie *t, Flat &f) {
                 }
             }
         }
+    }
+    if (best.g == 0) {                                   /* only a forcing can leave no candidate */
+        acb_set_error("ACB_FILTER=\"%s\": gram %d / stride %d is not a candidate for keys of %d bytes and more (gram + stride <= %d)",
+                      forced ? forced : "", forced_g, forced_s, m, m + L);
+        return ACB_EINVAL;
     }
     collect_grams(prefixes, best.g, best.s, L, best_grams);
     pt.lap("filter: choose gram/stride");
@@ -619,6 +650,7 @@ static void build_filter(acb_trie *t, Flat &f) {
         memcpy(&f.anchors[i * 8], e.w, sizeof(e.w));
     }
     pt.lap("filter: anchor table");
+    return ACB_OK;
 }
 
 /* ----------------------------------------------- make_automaton + flatten */
@@ -735,8 +767,10 @@ extern "C" int acb_trie_make_automaton(acb_trie *t, int32_t *built) {
         }
 
         pt.lap("goto / fail / outputs");
-        if (f.n_keys > 0) build_filter(t, f);
-        else {                                               /* nothing can ever match */
+        if (f.n_keys > 0) {
+            const int rc = build_filter(t, f);
+            if (rc != ACB_OK) { t->flat = Flat(); return rc; }
+        } else {                                               /* nothing can ever match */
             f.gram = t->letter_bytes; f.stride = t->letter_bytes; f.log1 = 13; f.logA = 10; f.log3 = 0; f.bm3.assign(1, 0);
             f.filter_flags = acb_hash_is_wide(f.gram) ? ACB_FILTER_WIDE : 0;
             f.bm1.assign((size_t)1 << (13 - 5), 0);

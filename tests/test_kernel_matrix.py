@@ -1,0 +1,452 @@
+"""Every compiled scan kernel against the C oracle, one cell per filter shape.
+
+acb_stream_kernel<NW, STRIDE, MODE> is compiled 40 times (NW = 1..4 hash windows for grams of 1..16 bytes, STRIDE
+1..16, MODE wide iff the gram is a multiple of 4 bytes) and acb_pair_kernel<L2B> twice (a level 2 of 2^17 bits or any
+other size).  Each has its own unrolled probe loop, last-slice mask, item-list split and anchor offsets, and which one
+a scan runs on follows from the key set (build_filter's cost model).  So every cell here forces its shape
+(ACB_FILTER=g,s,log1,mode and ACB_FORCE_TAGMAP, only around make_automaton) on a key set whose shortest key is exactly
+gram + stride - one letter, checks with filter_shape() that the forcing took, and compares with the oracle:
+
+  GPU (-m gpu)  the filter and the DFA kernels on three 20 KiB tiles plus a ragged tail, with keys planted across every
+                32-byte lane run, 1 KiB slice and tile boundary and at every residue of the stride; the same bytes as a
+                ragged batch (empty haystacks, cuts through planted keys) and at two fixed strides; and text on which
+                every probe is a hit.  Records must equal the oracle's in order; unsorted, as a set.
+  CPU           the same forced tables through tests/emul.py (the kernels restated in Python) on about 2 KiB, so that
+                a failing GPU cell shows whether the tables or the kernel are wrong.
+
+The coverage tests read the shapes back and require all 42 instantiations plus the pair kernel with the tag bitmap.
+"""
+import dataclasses
+
+import numpy as np
+import pytest
+
+import emul
+import oracle
+import pyahocorasick_b200 as ac
+
+RUN = 32                          # kLaneBytes: one lane's bytes per slice
+SLICE = 32 * RUN                  # kSliceBytes: one consumer warp's slice
+TILE = 20 * SLICE                 # kTileBytes (ACB_TILE_SLICES slices)
+STRIDES = (1, 2, 4, 8, 16)
+PAIR_LOG1 = (13, 16, 19, 20)      # level 2 of 2^13 / 2^16 / 2^19 bits (acb_pair_kernel<0>), 2^17 (acb_pair_kernel<17>)
+GRAMS = {1: range(1, 17), 2: range(2, 17, 2), 4: range(4, 17, 4)}      # a gram is whole letters, at most 16 bytes
+
+
+@dataclasses.dataclass(frozen=True)
+class Cell:
+    L: int                        # letter bytes: 1 bytes, 2 bytes-flavour KEY_SEQUENCE, 4 unicode
+    g: int                        # gram bytes
+    s: int                        # probe stride in bytes
+    log1: int = 0                 # level-1 bitmap of 2^log1 bits; 0: the cost model's
+    pair: bool = False
+    tagmap: bool = False
+
+    @property
+    def env(self):
+        return f"{self.g},{self.s},{self.log1},{int(self.pair)}"
+
+    @property
+    def name(self):
+        kind = "pair" if self.pair else f"L{self.L}-g{self.g}-s{self.s}"
+        return kind + (f"-l{self.log1}" if self.log1 else "") + ("-tag" if self.tagmap else "")
+
+
+def _cells():
+    """The shapes the dispatcher accepts: a stride of L * 2^k <= 16 bytes, a gram of whole letters up to 16 bytes, the
+    pair placement only for 1-byte letters at gram 4 / stride 1; level 1 and the tag bitmap on a spread of them."""
+    stream = [Cell(L, g, s) for L in (1, 2, 4) for g in GRAMS[L] for s in STRIDES if s >= L]
+    pair = [Cell(1, 4, 1, log1, True, tag) for log1 in PAIR_LOG1 for tag in (False, True)]
+    spread = ([dataclasses.replace(c, log1=13) for c in stream[0::9]] +       # saturated level 1
+              [dataclasses.replace(c, log1=20) for c in stream[3::9]] +
+              [dataclasses.replace(c, tagmap=True) for c in stream[6::9]])
+    return stream + pair + spread
+
+
+CELLS = _cells()
+IDS = [c.name for c in CELLS]
+
+
+def _all_instantiations():
+    modes = ("narrow", "wide")
+    return ({("stream", nw, s, m) for nw in range(1, 5) for s in STRIDES for m in modes} |
+            {("pair", 0), ("pair", 17), ("pair-tagmap",)})
+
+
+# ------------------------------------------------------------------ key sets and text, in letters
+ALPHA = {1: [0x61, 0x62, 0x63], 2: [0x0061, 0x6162, 0xFFFF], 4: [0x61, 0x142, 0x1F600]}
+TOP = {1: 0xFF, 2: 0xFFFF, 4: 0x10FFFF}          # the largest letter; 0 is the smallest (the zero fill past the end)
+DTYPE = {1: np.uint8, 2: "<u2", 4: "<u4"}
+
+
+def _keys(cell, rng):
+    """Keys of at least m = (g + s - L) / L letters, at least one of exactly m: the forced gram is then the longest this
+    key set offers at the forced stride."""
+    L, alpha = cell.L, ALPHA[cell.L]
+    m, gl, sl = (cell.g + cell.s - L) // L, cell.g // L, cell.s // L
+    keys = []
+
+    def rnd(n):
+        return tuple(int(x) for x in rng.choice(alpha, size=n))
+
+    def add(k):
+        if len(k) >= m:
+            keys.append(tuple(k))
+
+    for _ in range(24):                                         # random keys, most longer than the 20 bytes an entry holds
+        add(rnd(int(rng.integers(m, m + 24 // L + 4))))
+    grm = rnd(gl)                                               # one gram at every probe offset j: anchor chains of one tag
+    for j in range(sl):
+        for _ in range(2):
+            add(rnd(j) + grm + rnd(max(0, m - j - gl) + int(rng.integers(0, 4))))
+    pre = rnd(gl + 3)                                           # a prefix longer than the gram: MULTI entries, trie walks
+    for _ in range(5):
+        add(pre + rnd(max(0, m - len(pre)) + int(rng.integers(0, 6))))
+    for nb in (70, 100):                                        # longer than the DFA's 64-byte warm-up span
+        add(rnd(max(m, nb // L)))
+    k = rnd(m + 3)                                              # nested prefixes and suffixes: order inside one end index
+    for x in (k, k + rnd(2), rnd(1) + k, k[1:], k[:m], rnd(2) + k + rnd(1), k[2:]):
+        add(x)
+    x, y = alpha[0], alpha[1]                                   # periodic keys: alternating text is all hits
+    for n in (m, m + 1, m + 5):
+        add(((x, y) * n)[:n])
+        add(((y, x) * n)[:n])
+    add(rnd(m) + (0, 0))                                        # against the zero fill of the last tile
+    add((0,) * m)
+    add((TOP[L],) * 2 + rnd(m))
+    if L == 4:                                                  # no key for the latin-1 automaton (it ignores ACB_FILTER)
+        keys = [k if max(k) > 0xFF else (0x142,) + k[1:] for k in keys]
+    keys = list(dict.fromkeys(keys))
+    assert min(map(len, keys)) == m
+    return keys
+
+
+def _pkg_key(k, L):
+    if L == 1:
+        return bytes(k)
+    if L == 2:
+        return k
+    return "".join(map(chr, k))
+
+
+def _oracle_key(k, L):
+    return bytes(k) if L == 1 else k
+
+
+def _build(cell, keys, mp):
+    mod = ac.flavour("unicode" if cell.L == 4 else "bytes")
+    A = mod.Automaton(mod.STORE_INTS, mod.KEY_SEQUENCE) if cell.L == 2 else mod.Automaton(mod.STORE_INTS)
+    for i, k in enumerate(keys):
+        A.add_word(_pkg_key(k, cell.L), i)
+    with mp.context() as m:
+        m.setenv("ACB_FILTER", cell.env)
+        if cell.tagmap:
+            m.setenv("ACB_FORCE_TAGMAP", "1")
+        else:
+            m.delenv("ACB_FORCE_TAGMAP", raising=False)
+        A.make_automaton()
+    return A
+
+
+def _instantiation(fs):
+    """the kernel template a scan with these tables launches (launch_stream / launch_pair)"""
+    if fs["filter_flags"] & emul.FILTER_PAIR:
+        return ("pair", 17 if fs["log2_bits2"] == 17 else 0)
+    return ("stream", (fs["gram_bytes"] + 3) // 4, fs["stride"], "wide" if fs["filter_flags"] & emul.FILTER_WIDE else "narrow")
+
+
+def _check_shape(A, cell):
+    fs = A.filter_shape()
+    assert (fs["gram_bytes"], fs["stride"]) == (cell.g, cell.s), fs
+    if cell.pair:
+        assert fs["filter_flags"] == emul.FILTER_PAIR and fs["log2_bits2"] == (17 if cell.log1 >= 20 else cell.log1), fs
+    else:
+        assert fs["filter_flags"] == (emul.FILTER_WIDE if cell.g % 4 == 0 else 0) and fs["log2_bits2"] == 0, fs
+    if cell.log1:
+        assert fs["log2_bits1"] == cell.log1, fs
+    if cell.tagmap:
+        assert fs["log2_bits3"] >= 16, fs
+    elif cell.pair:
+        assert fs["log2_bits3"] == 0, fs
+    return fs
+
+
+def _text(cell, keys, rng, n_bytes):
+    """n_bytes of text in the key alphabet (a few 0 and top letters), keys planted across every lane-run, slice and tile
+    boundary (coarser boundaries last, so that their keys survive) at every residue of the stride, and one key ending
+    on the last byte.  Returns the letters and the start letters of the boundary plants."""
+    L = cell.L
+    n = n_bytes // L
+    t = rng.choice(ALPHA[L], size=n).astype(np.uint32)
+    odd = rng.random(n)
+    t[odd < 0.01] = 0
+    t[odd > 0.99] = TOP[L]
+    plant = [k for k in keys if len(k) >= 2]
+    starts, i = [], 0
+    for step in (RUN, SLICE, TILE):
+        for b in range(step, n_bytes, step):
+            k = plant[(i * 7) % len(plant)]
+            d = 1 + (i >> 1) % (cell.s // L) if i % 2 == 0 else 1 + (i * 5) % (len(k) - 1)    # letters before b
+            st = b // L - d
+            if 0 <= st and st + len(k) <= n:
+                t[st:st + len(k)] = k
+                starts.append(st)
+            i += 1
+    k = plant[i % len(plant)]
+    t[n - len(k):] = k
+    return t, np.asarray(starts, dtype=np.int64)
+
+
+def _dense(cell, n_bytes):
+    """alternating letters: every probe's gram belongs to a periodic key, so every probe of a slice is pending and a
+    match ends at nearly every letter (item-list split, full candidate lists, match staging overflow)"""
+    x, y = ALPHA[cell.L][:2]
+    return np.array([x, y] * (n_bytes // cell.L // 2) + [x], dtype=np.uint32)
+
+
+def _ragged(rng, n, starts, boundaries):
+    """offsets (in letters) of a ragged batch over n letters: random cuts, cuts through planted keys and at tile
+    boundaries, runs of empty haystacks, empty haystacks first and last"""
+    cuts = [rng.integers(0, n + 1, size=120), starts[rng.integers(0, len(starts), size=80)] + 1, boundaries]
+    cuts = np.sort(np.concatenate(cuts))
+    cuts = np.concatenate([cuts, cuts[::17], cuts[::17], cuts[5::23]])           # repeated offsets: empty haystacks
+    return np.concatenate([[0, 0], np.sort(np.clip(cuts, 0, n)), [n, n]]).astype(np.int64)
+
+
+def _oracle(cell, keys):
+    O = oracle.OracleAutomaton()
+    for i, k in enumerate(keys):
+        O.add_word(_oracle_key(k, cell.L), i)
+    O.make_automaton()
+    return O
+
+
+def _want(O, cell, letters, off):
+    if cell.L == 1:
+        return [tuple(r) for r in O.scan_batch_bytes(letters.astype(np.uint8), off).tolist()]
+    return O.scan_batch_letters(letters, off)
+
+
+def _records(m):
+    return list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist()))
+
+
+def _diff(got, want):
+    """a short account of how two record lists differ (the first divergence, a few missing and extra records)"""
+    i = next((i for i, (a, b) in enumerate(zip(got, want)) if a != b), min(len(got), len(want)))
+    sg, sw = set(got), set(want)
+    return (f"{len(got)} records, want {len(want)}; first difference at {i}: got {got[i:i + 3]}, want {want[i:i + 3]}; "
+            f"missing {sorted(sw - sg)[:5]}, extra {sorted(sg - sw)[:5]}")
+
+
+def _seed(cell):
+    return sum(cell.name.encode()) * 7919 + cell.L
+
+
+# ------------------------------------------------------------------ GPU: the kernels
+def _check_gpu(A, batch, want, what):
+    for algo in ("filter", "dfa"):
+        got = _records(A.find_all_batch(batch, algo=algo))
+        if got != want:
+            pytest.fail(f"{what}, {algo}: {_diff(got, want)}")
+    got = sorted(_records(A.find_all_batch(batch, algo="filter", sort=False)))
+    if got != sorted(want):
+        pytest.fail(f"{what}, filter unsorted: {_diff(got, sorted(want))}")
+
+
+_RAN = set()                  # instantiations that went through a whole GPU cell
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("cell", CELLS, ids=IDS)
+def test_kernel_cell_matches_oracle(cell, monkeypatch):
+    rng = np.random.Generator(np.random.PCG64(_seed(cell)))
+    keys = _keys(cell, rng)
+    A = _build(cell, keys, monkeypatch)
+    fs = _check_shape(A, cell)
+    O = _oracle(cell, keys)
+    L, dt = cell.L, DTYPE[cell.L]
+    n_bytes = 3 * TILE + L * 1291                     # a ragged tail: not a multiple of 16, nor of a stride above L
+    t, starts = _text(cell, keys, rng, n_bytes)
+    n = t.size
+    flat = t.astype(dt).view(np.uint8)
+    # 1. one haystack
+    one = np.array([0, n], dtype=np.int64)
+    want = _want(O, cell, t, one)
+    assert len(want) > len(starts) // 2                # most plants survive the ones planted over them
+    _check_gpu(A, (flat, one * L), want, "one haystack")
+    # 2. ragged, with empty haystacks and cuts through planted keys
+    roff = _ragged(rng, n, starts, np.arange(TILE // L, n, TILE // L))
+    _check_gpu(A, (flat, roff * L), _want(O, cell, t, roff), "ragged batch")
+    # 3. fixed strides: a power of two (shift) and not (division)
+    for stride in (512, 3000):
+        k = flat.size // stride
+        foff = np.arange(k + 1, dtype=np.int64) * (stride // L)
+        _check_gpu(A, flat[:k * stride].reshape(k, stride), _want(O, cell, t[:k * (stride // L)], foff), f"stride {stride}")
+    # 4. every probe a hit
+    d = _dense(cell, TILE + 3 * SLICE)
+    doff = np.array([0, d.size], dtype=np.int64)
+    dwant = _want(O, cell, d, doff)
+    assert len(dwant) > 2 * d.size                     # several periodic keys end at every letter
+    _check_gpu(A, (d.astype(dt).view(np.uint8), doff * L), dwant, "dense text")
+    _RAN.add(_instantiation(fs))
+    if cell.pair and fs["log2_bits3"]:
+        _RAN.add(("pair-tagmap",))
+
+
+@pytest.mark.gpu
+def test_every_kernel_instantiation_ran(request):
+    """the cells above, as they ran on the GPU, reached every instantiation (run after them, in one session)"""
+    names = {it.name for it in request.session.items}
+    if not all(f"test_kernel_cell_matches_oracle[{i}]" in names for i in IDS):
+        pytest.skip("only part of the kernel matrix was selected")
+    assert _RAN == _all_instantiations(), sorted(_all_instantiations() - _RAN, key=str)
+
+
+# ------------------------------------------------------------------ CPU: the forced tables
+def test_cells_reach_every_kernel_instantiation(monkeypatch):
+    """the cells' tables, as filter_shape() reports them, select all 40 stream and 2 pair instantiations, and the pair
+    kernel with the tag bitmap; adding an instantiation or dropping a cell fails here"""
+    seen = set()
+    for cell in CELLS:
+        A = _build(cell, _keys(cell, np.random.Generator(np.random.PCG64(_seed(cell)))), monkeypatch)
+        fs = _check_shape(A, cell)
+        seen.add(_instantiation(fs))
+        if cell.pair and fs["log2_bits3"]:
+            seen.add(("pair-tagmap",))
+    assert seen == _all_instantiations(), sorted(_all_instantiations() ^ seen, key=str)
+
+
+@pytest.mark.parametrize("cell", CELLS, ids=IDS)
+def test_cell_tables_match_oracle_emulated(cell, monkeypatch):
+    rng = np.random.Generator(np.random.PCG64(_seed(cell)))
+    keys = _keys(cell, rng)
+    A = _build(cell, keys, monkeypatch)
+    _check_shape(A, cell)
+    f = A.flat()
+    O = _oracle(cell, keys)
+    L, dt = cell.L, DTYPE[cell.L]
+    t, starts = _text(cell, keys, rng, 2048 + L * 53)
+    n = t.size
+    flat = t.astype(dt).view(np.uint8)
+    d = _dense(cell, 160)
+    layouts = [("one haystack", t, np.array([0, n], dtype=np.int64)),
+               ("ragged batch", t, _ragged(rng, n, starts, np.arange(SLICE // L, n, SLICE // L))),
+               ("dense text", d, np.array([0, d.size], dtype=np.int64))]
+    for what, letters, off in layouts:
+        want = _want(O, cell, letters, off)
+        buf = flat if letters is t else letters.astype(dt).view(np.uint8)
+        for name, fn in (("filter", emul.emul_filter), ("dfa", emul.emul_dfa)):
+            got = fn(f, buf, off * L, 0)
+            if got != want:
+                pytest.fail(f"{what}, emulated {name}: {_diff(got, want)}")
+
+
+# ------------------------------------------------------------------ the forcing hook refuses what no kernel can run
+def _forced(monkeypatch, env, keys, flavour="bytes"):
+    mod = ac.flavour(flavour)
+    A = mod.Automaton(mod.STORE_INTS, mod.KEY_SEQUENCE) if isinstance(keys[0], tuple) else mod.Automaton(mod.STORE_INTS)
+    for i, k in enumerate(keys):
+        A.add_word(k, i)
+    with monkeypatch.context() as m:
+        m.setenv("ACB_FILTER", env)
+        A.make_automaton()
+    return A
+
+
+EIGHT = [b"abcdefgh", b"abcdefgx", b"bcdefghijk"]
+
+
+@pytest.mark.parametrize("env, flavour, keys, msg", [
+    ("16,16,0,0", "bytes", EIGHT, "not a candidate"),             # g + s would need keys of 31 bytes
+    ("8,2,0,0", "bytes", EIGHT, "not a candidate"),               # at stride 2 the grams stop at 7 bytes
+    ("6,1,0,0", "bytes", EIGHT, "not a candidate"),               # neither gmax (8) nor 4
+    ("0,0,0,0", "bytes", [b"a", b"ab"], None),                    # nothing forced: allowed
+    ("4,3,0,0", "bytes", EIGHT, "stride"),
+    ("4,32,0,0", "bytes", EIGHT, "stride"),
+    ("4,1,0,0", "bytes", [(1, 2, 3, 4), (5, 6, 7, 8)], "stride"),    # 2-byte letters: a stride of 1 byte is no letter
+    ("8,2,0,0", "unicode", ["łabcdefgh"], "stride"),
+    ("3,2,0,0", "bytes", [(1, 2, 3, 4), (5, 6, 7, 8)], "gram"),      # half a letter
+    ("4,1,22,0", "bytes", EIGHT, "log1"),                         # 2^22 bits: no room in shared memory
+    ("4,1,12,0", "bytes", EIGHT, "log1"),
+    ("8,1,0,1", "bytes", EIGHT, "pair"),
+    ("4,2,0,1", "bytes", EIGHT, "pair"),
+    ("0,0,0,1", "bytes", EIGHT, "pair"),
+    ("4,2,0,1", "bytes", [(1, 2, 3, 4), (5, 6, 7, 8)], "pair"),
+    ("4,1,0,2", "bytes", EIGHT, "mode"),
+    ("x", "bytes", EIGHT, "expected"),
+], ids=lambda v: v if isinstance(v, str) else None)
+def test_infeasible_forced_shapes_are_refused(monkeypatch, env, flavour, keys, msg):
+    if msg is None:
+        assert _forced(monkeypatch, env, keys, flavour).kind == ac.AHOCORASICK
+        return
+    with pytest.raises(ValueError, match=msg):
+        _forced(monkeypatch, env, keys, flavour)
+
+
+def test_a_refused_forcing_leaves_a_trie_that_builds_without_it(monkeypatch):
+    A = ac.flavour("bytes").Automaton(ac.STORE_INTS)
+    for i, k in enumerate(EIGHT):
+        A.add_word(k, i)
+    with monkeypatch.context() as m:
+        m.setenv("ACB_FILTER", "16,16,0,0")
+        with pytest.raises(ValueError):
+            A.make_automaton()
+    assert A.kind == ac.TRIE
+    with pytest.raises(AttributeError):
+        A.filter_shape()
+    monkeypatch.delenv("ACB_FILTER", raising=False)
+    assert A.make_automaton() is None and A.kind == ac.AHOCORASICK
+    fs = A.filter_shape()
+    assert fs["gram_bytes"] + fs["stride"] - 1 <= 8 and fs["log2_bits1"] >= 13
+    text = np.frombuffer(b"xxabcdefghx", dtype=np.uint8)
+    assert emul.emul_filter(A.flat(), text, np.array([0, text.size], dtype=np.int64), 0) == [(0, 9, 0)]
+
+
+# ------------------------------------------------------------------ the pipelined host scan on a ragged batch
+MiB = 1 << 20
+CHUNK = 32 * MiB                  # scan_host_pipelined's chunk; batches of 48 MiB and more take that path
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("cell", [Cell(1, 7, 8), Cell(1, 4, 1, 16, True)], ids=lambda c: c.name)
+def test_pipelined_scan_of_a_ragged_batch(cell, monkeypatch):
+    """about 100 MiB in (flat, offsets) form: the host scan copies, scans and sorts it in 32 MiB chunks, a start
+    position `reach` before a chunk boundary waits for the next chunk, and the runs of the haystacks a cut goes through
+    are merged on the host.  Here one haystack spans three chunk sorts, haystack boundaries lie exactly on a chunk
+    boundary and on a scan cut (the boundary minus the reach), and a run of empty haystacks sits on the chunk
+    boundary.  The filter path (pipelined) must equal the oracle and the DFA path (one launch over the batch)."""
+    rng = np.random.Generator(np.random.PCG64(_seed(cell)))
+    keys = _keys(cell, rng)
+    A = _build(cell, keys, monkeypatch)
+    _check_shape(A, cell)
+    reach = (max(map(len, keys)) + 31) & ~31
+    n = 100 * MiB + 12345
+    flat = rng.integers(ord("d"), ord("z") + 1, size=n, dtype=np.uint8)       # no key letter: the plants are the matches
+    plant = [np.frombuffer(bytes(k), dtype=np.uint8) for k in keys]
+    sites = list(range(4096, n - 256, 4093))
+    for c in (1, 2, 3):                                                       # across every chunk boundary and scan cut
+        for b in (c * CHUNK, c * CHUNK - reach):
+            sites += [b - d for d in range(1, 2 * reach, 3)]
+    for i, b in enumerate(sorted(sites)):
+        k = plant[i % len(plant)]
+        flat[b:b + len(k)] = k
+    k = plant[0]
+    flat[n - len(k):] = k
+    long_hay = (10 * MiB, 80 * MiB)                                           # spans the cuts of chunks 1 and 2
+    cuts = np.concatenate([[5 * MiB], rng.integers(5 * MiB, 10 * MiB, size=400), long_hay,
+                           rng.integers(80 * MiB, 3 * CHUNK - reach, size=300),
+                           [3 * CHUNK - reach] + [3 * CHUNK] * 5, rng.integers(3 * CHUNK + 1, n, size=200)])
+    off = np.concatenate([[0], np.sort(cuts), [n]]).astype(np.int64)
+    O = _oracle(cell, keys)
+    want = _want(O, cell, flat, off)
+    h_long = int(np.searchsorted(off, long_hay[0], side="right")) - 1
+    ends = np.array([e + long_hay[0] for h, e, _ in want if h == h_long])
+    assert off[h_long] == long_hay[0] and all(((ends >= a) & (ends < a + CHUNK)).any() for a in (0, CHUNK, 2 * CHUNK))
+    for algo in ("filter", "dfa"):
+        got = _records(A.find_all_batch((flat, off), algo=algo))
+        if got != want:
+            pytest.fail(f"{algo}: {_diff(got, want)}")
+    got = sorted(_records(A.find_all_batch((flat, off), algo="filter", sort=False)))
+    if got != sorted(want):
+        pytest.fail(f"filter unsorted: {_diff(got, sorted(want))}")
