@@ -259,7 +259,10 @@ int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int64_t n, int6
  *   shot, every other haystack and every later scan start at the root.  ACB_EINVAL for an id that is not a state.
  * acb_table_get_long_state: the state in which haystack 0 of the LAST ACB_ALGO_LONG scan ended (its text exhausted,
  *   a match still pending at the end reported: then the root).  After acb_scan_device the caller synchronises its
- *   stream first. */
+ *   stream first.
+ * An ACB_ALGO_LONG scan without text (total_bytes == 0 or n_hay == 0) or without keys consumes the state set before it
+ *   like any other: haystack 0 ends where it started, so acb_table_get_long_state returns that state, and the next
+ *   scan starts at the root. */
 int acb_table_set_long_state(acb_table *tb, int32_t state);
 int acb_table_get_long_state(acb_table *tb, int32_t *state);
 

@@ -217,6 +217,28 @@ class OracleAutomaton:
             out += [(h, e - a, v) for e, v in zip(idx[:n].tolist(), val[:n].tolist())]
         return out
 
+    def iter_long_batch_letters(self, letters: np.ndarray, offsets: np.ndarray) -> list:
+        """[(hay_id, end_index, value)] of iter_long over each haystack of a batch of letters (uint32 values as the
+        reference sees them) cut at `offsets` (counted in letters)."""
+        w = np.ascontiguousarray(letters, dtype=np.uint32)
+        out = []
+        cap = 1 << 16
+        idx = np.empty(cap, dtype=np.int64)
+        val = np.empty(cap, dtype=np.int64)
+        for h in range(len(offsets) - 1):
+            a, b = int(offsets[h]), int(offsets[h + 1])
+            while True:
+                n = self._L.orc_iter_long(self._h, _p(w, ctypes.c_uint32), a, b, _p(idx, ctypes.c_int64), _p(val, ctypes.c_int64), cap)
+                if n < 0:
+                    raise AttributeError("not an automaton")
+                if n <= cap:
+                    break
+                cap = int(n)
+                idx = np.empty(cap, dtype=np.int64)
+                val = np.empty(cap, dtype=np.int64)
+            out += [(h, e - a, v) for e, v in zip(idx[:n].tolist(), val[:n].tolist())]
+        return out
+
 
 class OracleIter:
     def __init__(self, A: OracleAutomaton, text, start, end, ignore_ws):

@@ -1221,6 +1221,7 @@ struct acb_table {
     uint2 *d_cand = nullptr;                 /* candidate lists of the stream kernel's consumer warps (kWarpCand entries each) */
     int32_t long_init = 0;                   /* iter_long streaming: start state of haystack 0 of the next ACB_ALGO_LONG scan */
     int32_t *d_long_final = nullptr;         /* ... and the state it ended in */
+    int32_t long_final_host = -1;            /* that state when the last ACB_ALGO_LONG scan launched nothing, else -1 */
     long long dev_bytes = 0;
     std::vector<int32_t> key_len;            /* host copy, for sorting records */
     /* workspace of acb_scan_host */
@@ -1453,6 +1454,13 @@ static void fill_params(const acb_table *tb, ScanParams &p, const uint8_t *d_hay
     p.letter_shift = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
 }
 
+/* an ACB_ALGO_LONG scan with no text or no keys launches nothing: haystack 0 ends in the state it starts in, and the
+ * one-shot start state is consumed as by any other scan */
+static void long_scan_without_launch(acb_table *tb) {
+    tb->long_final_host = tb->long_init;
+    tb->long_init = 0;
+}
+
 extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
                                const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
                                acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
@@ -1465,7 +1473,10 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
         }
         if (stride_bytes / tb->L > 0x7fffffffLL) { acb_set_error("haystack longer than 2^31-1 letters"); return ACB_ERANGE; }
     }
-    if (total_bytes == 0 || n_hay == 0) return ACB_OK;
+    if (total_bytes == 0 || n_hay == 0) {
+        if (algo == ACB_ALGO_LONG) long_scan_without_launch(tb);
+        return ACB_OK;
+    }
     if (reinterpret_cast<uintptr_t>(d_hay) & 15) { acb_set_error("d_hay must be 16-byte aligned"); return ACB_EINVAL; }
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -1474,7 +1485,10 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
     fill_params(tb, p, d_hay, total_bytes, d_offsets, n_hay, stride_bytes, d_out, cap, d_count);
 
     if (algo == ACB_ALGO_AUTO) algo = ACB_ALGO_FILTER;
-    if (tb->n_keys == 0) return ACB_OK;                     /* empty key set: nothing can match */
+    if (tb->n_keys == 0) {                                  /* empty key set: nothing can match */
+        if (algo == ACB_ALGO_LONG) long_scan_without_launch(tb);
+        return ACB_OK;
+    }
     const bool timing = g_timing.load() != 0;
     if (timing) {
         if (!tb->ev0) { CUDA_TRY(cudaEventCreate(&tb->ev0)); CUDA_TRY(cudaEventCreate(&tb->ev1)); }
@@ -1496,6 +1510,7 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
         p.long_init = tb->long_init;
         p.long_final = tb->d_long_final;
         tb->long_init = 0;                                      /* one shot */
+        tb->long_final_host = -1;                               /* the kernel writes the final state */
         long long grid = (n_hay + kDfaThreads - 1) / kDfaThreads;
         acb_long_kernel<<<(unsigned)grid, kDfaThreads, 0, s>>>(p);
         cudaError_t e = cudaGetLastError();
@@ -1524,6 +1539,7 @@ extern "C" int acb_table_set_long_state(acb_table *tb, int32_t state) {
 extern "C" int acb_table_get_long_state(acb_table *tb, int32_t *state) {
     if (!tb || !state) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *state = 0;
+    if (tb->long_final_host >= 0) { *state = tb->long_final_host; return ACB_OK; }
     if (!tb->d_long_final) return ACB_OK;                    /* no ACB_ALGO_LONG scan yet */
     CUDA_TRY(cudaSetDevice(tb->device));
     CUDA_TRY(cudaMemcpy(state, tb->d_long_final, sizeof(int32_t), cudaMemcpyDeviceToHost));
@@ -1600,6 +1616,8 @@ extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int6
                                        int64_t max_hay_letters, void *stream) {
     if (!tb || n < 0 || (n && !d_records)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (n <= 1) return ACB_OK;
+    /* before any allocation: scratch for this many records may not exist, and the caller sorts on the host on ERANGE */
+    if (n > 0x7fffffffLL) { acb_set_error("too many records to sort on the device"); return ACB_ERANGE; }
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const int max_len = tb->max_key_bytes / tb->L;
@@ -1616,7 +1634,6 @@ extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int6
         CUDA_TRY(cudaMalloc(&tb->d_sort, need + need / 4));
         tb->sort_cap = need + need / 4;
     }
-    if (n > 0x7fffffffLL) { acb_set_error("too many records to sort on the device"); return ACB_ERANGE; }
     char *base = reinterpret_cast<char *>(tb->d_sort);
     unsigned long long *k0 = reinterpret_cast<unsigned long long *>(base);
     unsigned long long *k1 = k0 + n;
@@ -1765,7 +1782,10 @@ extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_by
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
     tb->h_out_n = 0;
-    if (total_bytes == 0 || n_hay == 0) return ACB_OK;
+    if (total_bytes == 0 || n_hay == 0) {
+        if (algo == ACB_ALGO_LONG) long_scan_without_launch(tb);
+        return ACB_OK;
+    }
     CUDA_TRY(cudaSetDevice(tb->device));
     if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
     if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));

@@ -20,6 +20,7 @@ import pytest  # noqa: E402
 import emul  # noqa: E402
 import test_gpu_parity as gp  # noqa: E402
 import test_iter_long_set as ils  # noqa: E402
+import test_search_args_differential as sad  # noqa: E402
 from pyahocorasick_b200 import synth  # noqa: E402
 
 
@@ -38,6 +39,14 @@ def main():
         as_test(f"test_iter_long_set.py::test_iter_long_set_matches_the_reference_on_gpu[{fl}]",
                 ils.test_iter_long_set_matches_the_reference_on_gpu, fl)
     as_test("test_iter_long_set.py::test_iter_long_long_stream_on_gpu", ils.test_iter_long_long_stream_on_gpu)
+    for name in ("iter_ranges_and_white_space", "find_all_ranges", "batch_input_forms_equal_looping_the_reference",
+                 "key_sequences_iter_and_iter_long", "searches_between_random_mutations", "iter_long_ranges_and_batch"):
+        for fl in ("bytes", "unicode"):
+            as_test(f"test_search_args_differential.py::test_{name}_on_gpu[{fl}]", getattr(sad, f"test_{name}_on_gpu"), fl)
+    for fl in ("bytes", "unicode"):
+        for ws in (False, True):
+            as_test(f"test_search_args_differential.py::test_iter_set_at_random_points_on_gpu[{fl}-{ws}]",
+                    sad.test_iter_set_at_random_points_on_gpu, fl, ws)
     gp.reference_c2_sample()
     for name, make in (("c2_rows", lambda: synth.make("C2", scale=1.0)), ("c3_rows", lambda: synth.make("C3", scale=1.0)),
                        ("c4_rows", gp.c4_with_straddlers), ("c5_rows", lambda: synth.make("C5", scale=0.125))):

@@ -1,7 +1,8 @@
 """iter() / find_all() argument handling against the reference extension, randomised: start / end (negative too),
-ignore_white_space, find_all's callback form, chunked iteration with set() at random points.  The device is
-the CPU emulation (tests/emul.py); what is under test is the host layer's index arithmetic and state carry-over
-(src/Automaton.c:875-966, src/utils.c:293-359, src/AutomatonSearchIter.c:243-368)."""
+ignore_white_space, find_all's callback form, chunked iteration with set() at random points.  What is under test is
+the host layer's index arithmetic and state carry-over (src/Automaton.c:875-966, src/utils.c:293-359,
+src/AutomatonSearchIter.c:243-368): on the CPU emulation (tests/emul.py), and in the gpu-marked twins on the real
+kernels."""
 import numpy as np
 import pytest
 
@@ -34,11 +35,9 @@ def _call(fn, *a, **kw):
         return ("exc", type(e).__name__)
 
 
-@pytest.mark.parametrize("fl", ["bytes", "unicode"])
-def test_iter_ranges_and_white_space(fl, monkeypatch):
-    emul.install(monkeypatch, "filter")
-    rng = np.random.default_rng(21)
-    for _ in range(120):
+def _iter_ranges_and_white_space(fl, trials, seed):
+    rng = np.random.default_rng(seed)
+    for _ in range(trials):
         A, R, word = _pair(fl, rng, with_space=True)
         hay = word(0, 30)
         n = len(hay)
@@ -54,11 +53,9 @@ def test_iter_ranges_and_white_space(fl, monkeypatch):
             assert _call(A.iter, *args, **kw) == _call(R.iter, *args, **kw), (fl, hay, args, kw)
 
 
-@pytest.mark.parametrize("fl", ["bytes", "unicode"])
-def test_find_all_ranges(fl, monkeypatch):
-    emul.install(monkeypatch, "filter")
-    rng = np.random.default_rng(22)
-    for _ in range(100):
+def _find_all_ranges(fl, trials, seed):
+    rng = np.random.default_rng(seed)
+    for _ in range(trials):
         A, R, word = _pair(fl, rng, with_space=False)
         hay = word(0, 30)
         n = len(hay)
@@ -79,15 +76,12 @@ def test_find_all_ranges(fl, monkeypatch):
             assert (run(A, got), got) == (run(R, want), want), (fl, hay, extra)
 
 
-@pytest.mark.parametrize("ws", [False, True])
-@pytest.mark.parametrize("fl", ["bytes", "unicode"])
-def test_iter_set_at_random_points(fl, ws, monkeypatch):
+def _iter_set_at_random_points(fl, ws, trials, seed):
     """chunks shorter than the longest key (the history then holds everything seen so far), empty chunks, extra
     next() calls past exhaustion (each moves the reference's index on by one), reset, ignore_white_space"""
-    emul.install(monkeypatch, "filter")
-    rng = np.random.default_rng(23 + ws)
+    rng = np.random.default_rng(seed)
     kw = {"ignore_white_space": True} if ws else {}
-    for _ in range(150):
+    for _ in range(trials):
         A, R, word = _pair(fl, rng, with_space=ws)
         chunks = [word(0, 14) for _ in range(4)]
         ia, ir = A.iter(chunks[0], **kw), R.iter(chunks[0], **kw)
@@ -108,19 +102,17 @@ def test_iter_set_at_random_points(fl, ws, monkeypatch):
         assert got == want, (fl, chunks)
 
 
-@pytest.mark.parametrize("fl", ["bytes", "unicode"])
-def test_batch_input_forms_equal_looping_the_reference(fl, monkeypatch):
+def _batch_input_forms(fl, trials, seed):
     """find_all_batch over a list, over (flat, offsets), over a uint8 matrix == iter() of the reference per haystack"""
-    emul.install(monkeypatch, "filter")
     ref, mod = reference(fl), pkg.flavour(fl)
-    rng = np.random.default_rng(31)
+    rng = np.random.default_rng(seed)
     al = "ab\u0142" if fl == "unicode" else "abc"
 
     def word(lo, hi):
         s = "".join(al[int(j)] for j in rng.integers(0, len(al), size=int(rng.integers(lo, hi))))
         return s.encode() if fl == "bytes" else s
 
-    for _ in range(60):
+    for _ in range(trials):
         keys = list(dict.fromkeys(word(1, 6) for _ in range(int(rng.integers(1, 8)))))
         A, R = mod.Automaton(), ref.Automaton()
         for i, k in enumerate(keys):
@@ -139,13 +131,11 @@ def test_batch_input_forms_equal_looping_the_reference(fl, monkeypatch):
             assert list(A.find_all_batch(rows)) == [(h, e, v) for h in range(rows.shape[0]) for e, v in R.iter(rows[h].tobytes())]
 
 
-@pytest.mark.parametrize("fl", ["bytes", "unicode"])
-def test_key_sequences_iter_and_iter_long(fl, monkeypatch):
-    emul.install(monkeypatch, "filter")
+def _key_sequences(fl, trials, seed):
     ref, mod = reference(fl), pkg.flavour(fl)
-    rng = np.random.default_rng(32)
+    rng = np.random.default_rng(seed)
     vals = [0, 1, 97, 255, 256, 65535 if fl == "bytes" else 2 ** 32 - 1]
-    for _ in range(80):
+    for _ in range(trials):
         keys = list(dict.fromkeys(tuple(int(vals[j]) for j in rng.integers(0, len(vals), size=int(rng.integers(1, 5))))
                      for _ in range(int(rng.integers(1, 6)))))
         A, R = mod.Automaton(mod.STORE_INTS, mod.KEY_SEQUENCE), ref.Automaton(ref.STORE_INTS, ref.KEY_SEQUENCE)
@@ -157,17 +147,16 @@ def test_key_sequences_iter_and_iter_long(fl, monkeypatch):
         assert list(A.iter_long(hay)) == list(R.iter_long(hay))
 
 
-def test_streaming_over_mixed_narrow_and_wide_chunks_equals_the_oracle(monkeypatch):
+def _mixed_streaming(trials, seed):
     """unicode flavour, chunks that are latin-1 (scanned with the 1-byte automaton) and chunks that are not, set() at
     random points: against the C restatement (oracle/ac_oracle.c), which has no storage-kind special cases"""
-    emul.install(monkeypatch, "filter")
-    rng = np.random.default_rng(5)
+    rng = np.random.default_rng(seed)
     mod = pkg.flavour("unicode")
 
     def word(al, lo, hi):
         return "".join(al[int(j)] for j in rng.integers(0, len(al), size=int(rng.integers(lo, hi))))
 
-    for _ in range(250):
+    for _ in range(trials):
         kal = ["ab\xe9", "abł", "ab\xe9ł\U0001f600"][int(rng.integers(0, 3))]
         keys = list({word(kal, 1, 6) for _ in range(int(rng.integers(1, 7)))})
         A, O = mod.Automaton(mod.STORE_INTS), oracle.OracleAutomaton()
@@ -218,13 +207,11 @@ def test_ignore_white_space_uses_the_c_library_classes(fl, monkeypatch):
         assert list(A.iter(hay, ignore_white_space=True)) == list(R.iter(hay, ignore_white_space=True)), (keys, hay)
 
 
-@pytest.mark.parametrize("fl", ["bytes", "unicode"])
-def test_searches_between_random_mutations(fl, monkeypatch):
+def _random_mutations(fl, trials, seed):
     """add_word / remove_word / make_automaton in random order, searching whenever the reference can (and raising
     like it when it cannot) -- including automata from which every key has been removed again"""
-    emul.install(monkeypatch, "filter")
     ref, mod = reference(fl), pkg.flavour(fl)
-    rng = np.random.default_rng(13)
+    rng = np.random.default_rng(seed)
     al = "abc" if fl == "bytes" else "abł"
 
     def word(lo, hi):
@@ -237,7 +224,7 @@ def test_searches_between_random_mutations(fl, monkeypatch):
         except Exception as e:
             return type(e).__name__
 
-    for _ in range(120):
+    for _ in range(trials):
         A, R = mod.Automaton(), ref.Automaton()
         first = word(1, 2)
         A.add_word(first, -1), R.add_word(first, -1)            # the reference asserts on a never-filled trie
@@ -260,20 +247,18 @@ def test_searches_between_random_mutations(fl, monkeypatch):
         assert len(A) == len(R) and A.kind == R.kind
 
 
-@pytest.mark.parametrize("fl", ["bytes", "unicode"])
-def test_iter_long_ranges_and_batch(fl, monkeypatch):
+def _iter_long_ranges_and_batch(fl, trials, seed):
     """iter_long(string, [start, [end]]) uses find_all's range rules (src/Automaton.c:968-1040); find_long_batch ==
     looping it.  The unicode key sets mix latin-1 and other letters over latin-1 haystacks on purpose."""
-    emul.install(monkeypatch, "filter")
     ref, mod = reference(fl), pkg.flavour(fl)
-    rng = np.random.default_rng(17)
+    rng = np.random.default_rng(seed)
     al = "abc" if fl == "bytes" else "abł"
 
     def word(lo, hi):
         s = "".join(al[int(j)] for j in rng.integers(0, len(al), size=int(rng.integers(lo, hi))))
         return s.encode() if fl == "bytes" else s
 
-    for _ in range(120):
+    for _ in range(trials):
         keys = list(dict.fromkeys(word(1, 6) for _ in range(int(rng.integers(1, 8)))))
         A, R = mod.Automaton(), ref.Automaton()
         for i, k in enumerate(keys):
@@ -289,3 +274,106 @@ def test_iter_long_ranges_and_batch(fl, monkeypatch):
                 if rng.integers(0, 2):
                     args.append(int(rng.integers(-n - 2, n + 3)))
             assert _call(A.iter_long, *args) == _call(R.iter_long, *args), (keys, args)
+
+
+# ------------------------------------------------------------------ the tests: on the emulation, and on the real kernels
+# The CPU tests route _scan_flat through tests/emul.py; their gpu-marked twins run the same bodies, with fewer trials
+# and seeds of their own, through the real _scan_flat: acb_scan_host (device sort, overflow retry, pinned hand-over),
+# the latin-1 table of the unicode flavour, and tables uploaded again after add_word / remove_word / make_automaton.
+FL = pytest.mark.parametrize("fl", ["bytes", "unicode"])
+
+
+@FL
+def test_iter_ranges_and_white_space(fl, monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _iter_ranges_and_white_space(fl, 120, 21)
+
+
+@pytest.mark.gpu
+@FL
+def test_iter_ranges_and_white_space_on_gpu(fl):
+    _iter_ranges_and_white_space(fl, 30, 121)
+
+
+@FL
+def test_find_all_ranges(fl, monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _find_all_ranges(fl, 100, 22)
+
+
+@pytest.mark.gpu
+@FL
+def test_find_all_ranges_on_gpu(fl):
+    _find_all_ranges(fl, 25, 122)
+
+
+@pytest.mark.parametrize("ws", [False, True])
+@FL
+def test_iter_set_at_random_points(fl, ws, monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _iter_set_at_random_points(fl, ws, 150, 23 + ws)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("ws", [False, True])
+@FL
+def test_iter_set_at_random_points_on_gpu(fl, ws):
+    _iter_set_at_random_points(fl, ws, 30, 123 + ws)
+
+
+@FL
+def test_batch_input_forms_equal_looping_the_reference(fl, monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _batch_input_forms(fl, 60, 31)
+
+
+@pytest.mark.gpu
+@FL
+def test_batch_input_forms_equal_looping_the_reference_on_gpu(fl):
+    _batch_input_forms(fl, 20, 131)
+
+
+@FL
+def test_key_sequences_iter_and_iter_long(fl, monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _key_sequences(fl, 80, 32)
+
+
+@pytest.mark.gpu
+@FL
+def test_key_sequences_iter_and_iter_long_on_gpu(fl):
+    _key_sequences(fl, 20, 132)
+
+
+def test_streaming_over_mixed_narrow_and_wide_chunks_equals_the_oracle(monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _mixed_streaming(250, 5)
+
+
+@pytest.mark.gpu
+def test_streaming_over_mixed_narrow_and_wide_chunks_equals_the_oracle_on_gpu():
+    _mixed_streaming(60, 105)
+
+
+@FL
+def test_searches_between_random_mutations(fl, monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _random_mutations(fl, 120, 13)
+
+
+@pytest.mark.gpu
+@FL
+def test_searches_between_random_mutations_on_gpu(fl):
+    _random_mutations(fl, 30, 113)
+
+
+@FL
+def test_iter_long_ranges_and_batch(fl, monkeypatch):
+    emul.install(monkeypatch, "filter")
+    _iter_long_ranges_and_batch(fl, 120, 17)
+
+
+@pytest.mark.gpu
+@FL
+def test_iter_long_ranges_and_batch_on_gpu(fl):
+    _iter_long_ranges_and_batch(fl, 30, 117)
