@@ -6,8 +6,9 @@
  *
  *  acb_stream_kernel<NW,STRIDE,MODE>   SINGLE placements of the gram filter (any gram length and stride)
  *  acb_pair_kernel<L2B>                PAIR placement (gram 4, stride 1, 1-byte letters: one filter word per two positions)
- *      A producer warp claims 20 KiB tiles of the flat haystack buffer from an atomic counter and moves them
- *      into a 3-stage shared-memory ring with cp.async.bulk (the TMA engine) and mbarriers; the consumer warps take
+ *      A producer warp claims tiles of the flat haystack buffer from an atomic counter (20 KiB into a 3-stage ring;
+ *      pair kernel: 32 KiB into 2 stages) and moves them into shared memory with cp.async.bulk (the TMA engine) and
+ *      mbarriers; the consumer warps take
  *      1 KiB slices of the stages from a shared-memory counter, hash the gram at every probe position and test it
  *      against the gram bitmap held in shared memory.  Start-anchored search: the rare survivors get the second
  *      hash of their gram (read back from the stage, still resident) and are collected per warp; a warp that has 32 of
@@ -134,7 +135,7 @@ struct ScanParams {
     int32_t long_init;             /* ACB_ALGO_LONG: the state haystack 0 starts in (iter_long streaming) */
     int32_t *long_final;           /* ... and where the state it ends in goes (may be null) */
     long long seg_begin, seg_end;  /* byte range of this launch */
-    unsigned int n_tiles;          /* kTileBytes tiles in the segment */
+    unsigned int n_tiles;          /* tiles in the segment (kTileBytes, pair kernel: kPairTileBytes) */
     unsigned int *work_ctr;        /* [0] next tile, [1] CTAs done */
     uint2 *cand;                   /* candidate entries, kWarpCand per consumer warp of every CTA: {position in the segment, anchor tag} */
     int stride_shift;              /* log2(stride_bytes) when it is a power of two, else -1 */
@@ -460,10 +461,14 @@ __device__ __forceinline__ void resolve_backlog(const ScanParams &p, uint8_t *sm
 }
 
 /* The producer warp of a streaming kernel: claims tiles from the global counter and keeps the shared-memory ring full
- * (cp.async.bulk + mbarrier); `stages` = offset of the ring in the CTA's shared memory. */
-template <int NCONS>
+ * (cp.async.bulk + mbarrier); `stages` = offset of the ring in the CTA's shared memory.  The ring's geometry (TSLICES
+ * slices per tile, STAGES stages) is the kernel's: the pair kernel has its own. */
+template <int NCONS, int TSLICES, int STAGES>
 __device__ __forceinline__ void stream_producer(const ScanParams &p, uint8_t *smem_raw, uint32_t sbase, uint32_t stages,
                                                 uint32_t bar_full, uint32_t bar_empty, volatile uint32_t *s_tile, int lane) {
+    constexpr int kTileSlices = TSLICES, kStages = STAGES;
+    constexpr int kTileBytes = kTileSlices * kSliceBytes;
+    constexpr int kStageBytes = (kTileBytes + kLook + 127) / 128 * 128;
     struct { uint32_t stages; } lay = {stages};
         /* ---------------- producer warp.  Tiles come from one global counter.  A claim is a ~1 us round trip to L2, so
        kClaimDepth of them are kept in flight: claim[k] serves fills k, k + kClaimDepth, ... and is re-issued as soon
@@ -571,7 +576,7 @@ __global__ void __launch_bounds__(kFThreads, 1) acb_stream_kernel(const __grid_c
     const uint32_t seg_len = (uint32_t)(p.seg_end - p.seg_begin);        /* <= 2^31 */
 
     if (warp == kConsumers) {
-        stream_producer<kConsumers>(p, smem_raw, sbase, lay.stages, bar_full, bar_empty, s_tile, lane);
+        stream_producer<kConsumers, kTileSlices, kStages>(p, smem_raw, sbase, lay.stages, bar_full, bar_empty, s_tile, lane);
     } else {
         /* ---------------- consumer warps: slice `warp` of every fill */
         ProbeCtx c;
@@ -724,8 +729,9 @@ __global__ void __launch_bounds__(kFThreads, 1) acb_stream_kernel(const __grid_c
 }
 
 /* ------------------------------------------------------------ the pair kernel
- * acb_pair_kernel: the stream kernel of the PAIR placement (gram 4, stride 1, 1-byte letters; acb_hash.h).  Same ring,
- * same producer, same dynamic slices; what differs is everything a consumer warp does with its slice:
+ * acb_pair_kernel: the stream kernel of the PAIR placement (gram 4, stride 1, 1-byte letters; acb_hash.h).  Same
+ * producer, same dynamic slices, a ring of its own (kPairTileSlices x kPairStages); what differs is everything a
+ * consumer warp does with its slice:
  *   level 1   one shared-memory word per PAIR of positions, selected by the three bytes the pair's grams share; the
  *             word holds one bit per (role, remaining byte), so the loop leaves a per-POSITION pass mask -- 9.5
  *             instructions per pair, 2 % of the positions pass on random text against 10 k keys.  A lane owns two runs
@@ -747,9 +753,27 @@ __global__ void __launch_bounds__(kFThreads, 1) acb_stream_kernel(const __grid_c
 constexpr int kPairConsumers = ACB_PAIR_CONSUMERS;          /* consumer warps of the pair kernel: 27 + the producer = 896 threads leave 72 registers per thread,
                                                                 and the level-1 loop stops spilling (31 consumers at 64 registers: 4 % slower on C2) */
 constexpr int kPairThreads = (kPairConsumers + 1) * 32;
-static_assert((kPairConsumers + kTileSlices - 1) / kTileSlices + 2 < 2 * ACB_STAGES && kPairThreads <= 1024, "pair kernel shape");
+/* The pair kernel's ring: power-of-two tiles and stages, so that a slice number splits into fill, slice, stage and
+ * barrier phase by shifts and masks.  32 KiB tiles x 2 stages: the 27 consumer warps work inside one tile while the
+ * next one loads.  Fastest of the shapes that fit next to the 144 KiB filter on the H100 (DESIGN 4.1 has the sweep). */
+#ifndef ACB_PAIR_TILE_SLICES
+#define ACB_PAIR_TILE_SLICES 32
+#endif
+#ifndef ACB_PAIR_STAGES
+#define ACB_PAIR_STAGES 2
+#endif
+constexpr int kPairTileSlices = ACB_PAIR_TILE_SLICES;
+constexpr int kPairStages     = ACB_PAIR_STAGES;
+constexpr int kPairTileLog    = __builtin_ctz(kPairTileSlices);
+constexpr int kPairStageLog   = __builtin_ctz(kPairStages);
+constexpr int kPairTileBytes  = kPairTileSlices * kSliceBytes;
+constexpr int kPairStageBytes = (kPairTileBytes + kLook + 127) / 128 * 128;
+static_assert((kPairTileSlices & (kPairTileSlices - 1)) == 0 && (kPairStages & (kPairStages - 1)) == 0 && kSliceBytes == 1024,
+              "pair ring: power-of-two tiles and stages of 1 KiB slices");
+static_assert((kPairConsumers + kPairTileSlices - 1) / kPairTileSlices + 2 < 2 * kPairStages && kPairThreads <= 1024, "pair kernel shape");
 constexpr int kPairRing = 64;                                /* candidate ring entries per consumer warp */
-constexpr int kPairItems = 64;                               /* item list entries (uint16) per consumer warp */
+constexpr int kPairItems = 64;                               /* item list entries (uint16 byte offsets in the slice) per consumer warp */
+static_assert(kPairRing >= 31 + 32, "a one-round slice must fit the ring next to a turn not yet resolved");
 
 struct PairSmem {
     uint32_t bitmap, bitmap2, stages, ring, items, bars, tiles, next, total;
@@ -759,11 +783,11 @@ __host__ __device__ inline PairSmem pair_smem(int log1, int log2b) {
     uint32_t o = 0;
     s.bitmap = o;    o += 1u << (log1 - 3);                       /* >= 1 KiB: level 2 follows without a gap, as in bm1 */
     s.bitmap2 = o;   o += 1u << (log2b - 3);                      o = (o + 127u) & ~127u;
-    s.stages = o;    o += (uint32_t)kStages * kStageBytes;
+    s.stages = o;    o += (uint32_t)kPairStages * kPairStageBytes;
     s.ring = o;      o += (uint32_t)kPairConsumers * kPairRing * 8u;
     s.items = o;     o += (uint32_t)kPairConsumers * kPairItems * 2u;
-    s.bars = o;      o += 2u * kStages * 8u;
-    s.tiles = o;     o += (uint32_t)kStages * 4u;
+    s.bars = o;      o += 2u * kPairStages * 8u;
+    s.tiles = o;     o += (uint32_t)kPairStages * 4u;
     s.next = o;      o += 4u;
     s.total = (o + 15u) & ~15u;
     return s;
@@ -899,14 +923,14 @@ __global__ void __launch_bounds__(kPairThreads, 1) acb_pair_kernel(const __grid_
     const PairSmem lay = pair_smem(p.log1, p.log2b);
     const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t bar_full = sbase + lay.bars, bar_empty = bar_full + 8u * kStages;
+    const uint32_t bar_full = sbase + lay.bars, bar_empty = bar_full + 8u * kPairStages;
     volatile uint32_t *s_tile = reinterpret_cast<volatile uint32_t *>(smem_raw + lay.tiles);
 
     if (tid == 0) {
         *reinterpret_cast<unsigned int *>(smem_raw + lay.next) = 0u;
-        for (int s = 0; s < kStages; s++) {
+        for (int s = 0; s < kPairStages; s++) {
             mbar_init(bar_full + 8u * s, 1);
-            mbar_init(bar_empty + 8u * s, kTileSlices);
+            mbar_init(bar_empty + 8u * s, kPairTileSlices);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -916,7 +940,7 @@ __global__ void __launch_bounds__(kPairThreads, 1) acb_pair_kernel(const __grid_
 
     if (warp == kPairConsumers) {
         /* the producer starts at once: the first tiles are on their way while the consumers fetch the bitmap */
-        stream_producer<kPairConsumers>(p, smem_raw, sbase, lay.stages, bar_full, bar_empty, s_tile, lane);
+        stream_producer<kPairConsumers, kPairTileSlices, kPairStages>(p, smem_raw, sbase, lay.stages, bar_full, bar_empty, s_tile, lane);
     } else {
         {   /* both levels of the bitmap -> shared memory with cp.async, by the consumer warps (named barrier 1) */
             const int n16 = (1 << (p.log1 - 7)) + (1 << (p.log2b - 7));
@@ -938,25 +962,81 @@ __global__ void __launch_bounds__(kPairThreads, 1) acb_pair_kernel(const __grid_
         const uint32_t sring = sbase + lay.ring + (uint32_t)warp * (kPairRing * 8u);
         const uint32_t sitems = sbase + lay.items + (uint32_t)warp * (kPairItems * 2u);
         const uint32_t snext = sbase + lay.next;
-        const uint32_t lane5 = (uint32_t)lane << 5;
+        const uint32_t sstages = sbase + lay.stages;
+        const uint32_t lane16 = (uint32_t)lane << 4;
         unsigned int n_cand = 0, head = 0;                               /* warp-uniform: entries [head, head + n_cand) of the ring */
 
+        /* bit y of a lane's pending mask is position y of its first 16-byte run, or y - 16 of its second: byte
+           16 * lane + y (+ 496) of the slice */
+        auto offset_of = [&](uint32_t y) { return lane16 + y + (y & 16u) * 31u; };
+        auto top_bit = [](uint32_t m) { uint32_t y; asm("bfind.u32 %0, %1;" : "=r"(y) : "r"(m)); return y; };   /* m != 0 */
+        /* the list: every lane writes the byte offsets of its pending positions after those of the lanes below it */
+        auto list_all = [&](uint32_t pend) {
+            const unsigned int cnt = (unsigned)__popc(pend);
+            unsigned int incl = cnt;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const unsigned int v = __shfl_up_sync(kFull, incl, d);
+                if (lane >= d) incl += v;
+            }
+            uint32_t at = sitems + 2u * (incl - cnt);
+            while (pend) {
+                const uint32_t y = top_bit(pend);
+                pend ^= 1u << y;
+                sts16(at, offset_of(y));
+                at += 2u;
+            }
+        };
+        /* one round of items, list entries [base, base + take) with take <= 32, one per lane: the gram read back from
+           the stage, the anchor tag (hash 2), level 2; the survivors {position, tag} go to the candidate ring, which
+           has room for `take` more */
+        auto item_round = [&](uint32_t slice_saddr, uint32_t pos_base, unsigned int base, unsigned int take) {
+            uint32_t ok = 0, pos = 0, tag = 0;
+            if ((unsigned)lane < take) {
+                const uint32_t t = lds16(sitems + 2u * (base + (unsigned)lane));
+                const uint32_t ga = slice_saddr + t, wa = ga & ~3u;
+                const uint32_t lo = lds32(wa), hi = lds32(wa + 4u);
+                const uint32_t w = __funnelshift_r(lo, hi, ga << 3);                    /* wrap shift: (ga & 3) * 8 */
+                tag = (w * mul2) | 1u;
+                const uint32_t word = lds_bitmap((tag >> shy_w) * four + sbm2);
+                ok = __funnelshift_r(word, 0u, tag >> shy_a) & __funnelshift_r(word, 0u, tag >> shy_b) & 1u;
+                pos = pos_base + t;
+            }
+            if (p.log3) {                                                /* very large key sets: the tag bitmap in L2 as well */
+                const uint32_t i0 = (tag * ACB_TAGMAP_MIX) >> (32 - p.log3);
+                if (ok) ok = (__ldg(p.bm3 + (i0 >> 5)) >> (i0 & 31u)) & 1u;
+            }
+#ifdef ACB_EXP_NODRAIN
+            if (ok && tag == pos) s_tile[0] = 2u;
+#else
+            const unsigned mk = __ballot_sync(kFull, ok);
+            if (ok) {
+                const uint32_t at = sring + (((head + n_cand + (unsigned)__popc(mk & lt_mask)) & (kPairRing - 1u)) << 3);
+                asm volatile("st.shared.v2.u32 [%0], {%1, %2};" :: "r"(at), "r"(pos), "r"(tag) : "memory");
+            }
+            n_cand += (unsigned)__popc(mk);
+#endif
+        };
+
         for (;;) {
+            /* slice g is slice g % kPairTileSlices of fill g / kPairTileSlices.  One lane claims it; elect.sync tells
+               ptxas that one lane does, so the atomic is not wrapped in warp aggregation */
             unsigned int g = 0;
-            if (lane == 0) asm volatile("atom.shared.add.u32 %0, [%1], 1;" : "=r"(g) : "r"(snext) : "memory");
+            asm volatile("{ .reg .pred e; elect.sync _|e, 0xffffffff; @e atom.shared.add.u32 %0, [%1], 1; }"
+                         : "+r"(g) : "r"(snext) : "memory");
             g = __shfl_sync(kFull, g, 0);
-            const uint32_t fill = g / (uint32_t)kTileSlices, slice_off = (g % (uint32_t)kTileSlices) * (uint32_t)kSliceBytes;
-            const uint32_t stage = fill % (uint32_t)kStages;
-            mbar_wait(bar_full + 8u * stage, (fill / (uint32_t)kStages) & 1u);
+            const uint32_t fill = g >> kPairTileLog, stage = fill & (kPairStages - 1u);
+            const uint32_t slice_off = (g & (kPairTileSlices - 1u)) * (uint32_t)kSliceBytes;
+            mbar_wait(bar_full + 8u * stage, (fill >> kPairStageLog) & 1u);
             const uint32_t tile = s_tile[stage];
             if (tile == kNoTile) break;
-            const uint32_t tile_off = tile * (uint32_t)kTileBytes;       /* relative to the segment */
-            const uint32_t n_valid = (seg_len - tile_off < (uint32_t)kTileBytes) ? seg_len - tile_off : (uint32_t)kTileBytes;
-            const uint32_t slice_saddr = sbase + lay.stages + stage * (uint32_t)kStageBytes + slice_off;
+            const uint32_t tile_off = tile * (uint32_t)kPairTileBytes;   /* relative to the segment */
+            const uint32_t n_valid = (seg_len - tile_off < (uint32_t)kPairTileBytes) ? seg_len - tile_off : (uint32_t)kPairTileBytes;
+            const uint32_t slice_saddr = sstages + stage * (uint32_t)kPairStageBytes + slice_off;
             const uint32_t pos_base = tile_off + slice_off;
             uint32_t pend = 0;       /* bit y < 16: position 16 * lane + y of the slice passed level 1; y >= 16: position 512 + 16 * lane + y - 16 */
             if (slice_off < n_valid) {                                   /* warp-uniform */
-                const uint32_t saddr = slice_saddr + (uint32_t)lane * 16u;
+                const uint32_t saddr = slice_saddr + lane16;
                 uint32_t R0[5], R1[5];
                 {
                     const uint4 v = lds128(saddr), u = lds128(saddr + 512u);
@@ -987,83 +1067,54 @@ __global__ void __launch_bounds__(kPairThreads, 1) acb_pair_kernel(const __grid_
                 pend = 0;
 #endif
             }
-            /* items: the pending positions of all lanes go to the list -- an exclusive scan of the lanes' counts places
-               them (dense text, more than the list holds: ballot rounds, one position per lane and round, a pass at a
-               time) -- and are worked off 32 at a time */
+            /* items: the pending positions of all lanes go to the list and are worked off 32 at a time */
             unsigned int tot = __reduce_add_sync(kFull, (unsigned)__popc(pend));
-            while (tot) {
-                unsigned int n_items;
-                if (tot <= (unsigned)kPairItems) {
-                    const unsigned int cnt = (unsigned)__popc(pend);
-                    unsigned int incl = cnt;
-#pragma unroll
-                    for (int d = 1; d < 32; d <<= 1) {
-                        const unsigned int v = __shfl_up_sync(kFull, incl, d);
-                        if (lane >= d) incl += v;
+            if (tot <= 32u) {
+                /* the common case, one round: fewer than 32 candidates are waiting (they are resolved after every
+                   slice that brings them to 32), so the ring has room for all of them */
+                if (tot) {
+                    list_all(pend);
+                    __syncwarp();
+                    item_round(slice_saddr, pos_base, 0u, tot);
+                }
+            } else {
+                /* more than one round (dense text): passes of at most the list's size -- the whole list placed by the
+                   scan, or, past kPairItems, ballot rounds of one position per lane -- and rounds that never take more
+                   items than the ring has room for */
+                while (tot) {
+                    unsigned int n_items;
+                    if (tot <= (unsigned)kPairItems) {
+                        list_all(pend);
+                        n_items = tot;
+                        tot = 0;
+                    } else {
+                        n_items = 0;
+                        do {
+                            const unsigned int mp = __ballot_sync(kFull, pend != 0u);
+                            if (pend) {
+                                const uint32_t y = top_bit(pend);
+                                pend ^= 1u << y;
+                                sts16(sitems + 2u * (n_items + (unsigned)__popc(mp & lt_mask)), offset_of(y));
+                            }
+                            n_items += (unsigned)__popc(mp);
+                        } while (n_items <= (unsigned)(kPairItems - 32));
+                        tot -= n_items;
                     }
-                    uint32_t at = sitems + 2u * (incl - cnt);
-                    while (pend) {
-                        const uint32_t z = (uint32_t)__clz((int)pend);
-                        pend ^= 0x80000000u >> z;
-                        sts16(at, lane5 | (z ^ 31u));                     /* lane << 5 | bit */
-                        at += 2u;
-                    }
-                    n_items = tot;
-                    tot = 0;
-                } else {
-                    n_items = 0;
-                    do {
-                        const unsigned int mp = __ballot_sync(kFull, pend != 0u);
-                        if (pend) {
-                            const uint32_t z = (uint32_t)__clz((int)pend);
-                            pend ^= 0x80000000u >> z;
-                            sts16(sitems + 2u * (n_items + (unsigned)__popc(mp & lt_mask)), lane5 | (z ^ 31u));
+                    __syncwarp();
+                    for (unsigned int base = 0; base < n_items;) {
+                        if (n_cand == (unsigned)kPairRing) {            /* one slice alone filled the ring */
+                            __syncwarp();                                /* the entries were written by other lanes */
+                            pair_resolve(p, sring, head, 32u); head += 32u; n_cand -= 32u;
+                            continue;
                         }
-                        n_items += (unsigned)__popc(mp);
-                    } while (n_items <= (unsigned)(kPairItems - 32));
-                    tot -= n_items;
+                        unsigned int take = n_items - base;
+                        if (take > 32u) take = 32u;
+                        if (take > (unsigned)kPairRing - n_cand) take = (unsigned)kPairRing - n_cand;
+                        item_round(slice_saddr, pos_base, base, take);
+                        base += take;
+                    }
+                    __syncwarp();
                 }
-                __syncwarp();
-                for (unsigned int base = 0; base < n_items;) {
-                    if (n_cand == (unsigned)kPairRing) {                /* one slice alone filled the ring */
-                        __syncwarp();                                    /* the entries were written by other lanes */
-                        pair_resolve(p, sring, head, 32u); head += 32u; n_cand -= 32u;
-                        continue;
-                    }
-                    unsigned int take = n_items - base;
-                    if (take > 32u) take = 32u;
-                    if (take > (unsigned)kPairRing - n_cand) take = (unsigned)kPairRing - n_cand;
-                    bool ok = false;
-                    uint32_t pos = 0, tag = 0;
-                    if ((unsigned)lane < take) {
-                        const uint32_t it = lds16(sitems + 2u * (base + (unsigned)lane));
-                        const uint32_t y = it & 31u;
-                        const uint32_t t = ((it >> 1) & 0x1f0u) + ((y & 16u) * 31u + y);       /* 16 * lane + y, second run: + 496 */
-                        const uint32_t ga = slice_saddr + t, wa = ga & ~3u;
-                        const uint32_t lo = lds32(wa), hi = lds32(wa + 4u);
-                        const uint32_t w = __funnelshift_r(lo, hi, ga << 3);                    /* wrap shift: (ga & 3) * 8 */
-                        tag = (w * mul2) | 1u;
-                        const uint32_t word = lds_bitmap((tag >> shy_w) * four + sbm2);
-                        ok = (__funnelshift_r(word, 0u, tag >> shy_a) & __funnelshift_r(word, 0u, tag >> shy_b) & 1u) != 0u;
-                        pos = pos_base + t;
-                    }
-                    if (p.log3) {                                        /* very large key sets: the tag bitmap in L2 as well */
-                        const uint32_t i0 = (tag * ACB_TAGMAP_MIX) >> (32 - p.log3);
-                        if (ok) ok = ((__ldg(p.bm3 + (i0 >> 5)) >> (i0 & 31u)) & 1u) != 0u;
-                    }
-#ifdef ACB_EXP_NODRAIN
-                    if (ok && tag == pos) s_tile[0] = 2u;
-#else
-                    const unsigned mk = __ballot_sync(kFull, ok);
-                    if (ok) {
-                        const uint32_t at = sring + (((head + n_cand + (unsigned)__popc(mk & lt_mask)) & (kPairRing - 1u)) << 3);
-                        asm volatile("st.shared.v2.u32 [%0], {%1, %2};" :: "r"(at), "r"(pos), "r"(tag) : "memory");
-                    }
-                    n_cand += (unsigned)__popc(mk);
-#endif
-                    base += take;
-                }
-                __syncwarp();
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_empty + 8u * stage);          /* this warp is done with the stage */
@@ -1424,10 +1475,11 @@ static int launch_filter_range(acb_table *tb, ScanParams &p, long long begin, lo
         tb->dev_bytes += (long long)tb->sm_count * kConsumers * kWarpCand * (long long)sizeof(uint2);
     }
     p.cand = tb->d_cand;
+    const long long tile_bytes = (tb->filter_flags & ACB_FILTER_PAIR) ? kPairTileBytes : kTileBytes;   /* the kernel's ring */
     for (long long seg = begin; seg < end; seg += kSegBytes) {
         p.seg_begin = seg;
         p.seg_end = std::min<long long>(seg + kSegBytes, end);
-        p.n_tiles = (unsigned int)((p.seg_end - p.seg_begin + kTileBytes - 1) / kTileBytes);
+        p.n_tiles = (unsigned int)((p.seg_end - p.seg_begin + tile_bytes - 1) / tile_bytes);
         const int grid = (int)std::min<long long>(tb->sm_count, p.n_tiles);
         int rc = launch_stream(p, tb->filter_flags, tb->stride, grid, s);
         if (rc != ACB_OK) return rc;
