@@ -266,6 +266,49 @@ int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int64_t n, int6
 int acb_table_set_long_state(acb_table *tb, int32_t state);
 int acb_table_get_long_state(acb_table *tb, int32_t *state);
 
+/* ---- stream batches: the next chunk of many streams in one call ---------------------------------------------------
+ * The batch form of iter().set() / iter_long().set() (src/AutomatonSearchIter.c:303-368,
+ * src/AutomatonSearchIterLong.c:156-212).  An acb_streams holds, in HBM, what every stream carries from one chunk to
+ * the next: the letters consumed so far, and either its last longest_word - 1 letters (find_all semantics: a feed
+ * reports every match that ends inside the chunk, including those that start in earlier chunks) or the iter_long walk
+ * state (long_mode != 0: a feed continues each stream's longest-match walk).
+ *
+ * The table is passed to every call and not kept: acb_streams remembers the device, letter width, tail length and
+ * (long mode) state count of the table it was made for and refuses another (ACB_EINVAL).
+ *
+ * A feed takes chunks in the forms of acb_scan_device / acb_scan_host; ids[h] (int32, distinct, in [0, n_streams))
+ * names the stream chunk h continues, ids == NULL means chunk h continues stream h (then n_chunks <= n_streams).
+ * Streams without a chunk do not move.  Records: hay_id = index of the chunk in the call, end_index = letter of the
+ * chunk (add the stream's position before the feed, see acb_streams_positions, for the position in the stream).
+ * Overflow commits nothing: a host feed that returns ACB_EOVERFLOW, or a device feed that leaves *d_count > cap,
+ * changes no stream, and the same feed can be repeated with a larger buffer.
+ * Feeds of one stream batch must not overlap in time: issue them on one CUDA stream (or synchronise in between). */
+typedef struct acb_streams acb_streams;
+
+int  acb_streams_new(const acb_table *tb, int64_t n_streams, int long_mode, acb_streams **out);
+void acb_streams_free(acb_streams *ss);
+
+/* stream ids[0..n) (ids == NULL: every stream) back to position 0 with nothing carried (set(x, reset=True)).
+ * Synchronises the device. */
+int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n);
+
+/* DEVICE buffers, asynchronous on `stream`.  Zeroes *d_count itself, then counts every record (stored up to cap).
+ * d_ids is not checked: the caller guarantees distinct ids in range.  algo: ACB_ALGO_AUTO, _FILTER or _DFA for a
+ * find_all batch (the scan of the chunks; seams are always walked), ACB_ALGO_AUTO or _LONG for an iter_long batch.
+ * Records are unsorted: acb_sort_matches_device(tb, d_out, n, n_chunks, longest chunk in letters, stream). */
+int acb_streams_feed_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                            const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
+                            acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo);
+
+/* HOST buffers, like acb_scan_host (out may be NULL: acb_copy_records / acb_take_records on tb).  ids are checked:
+ * ACB_EINVAL for a duplicate or an id out of range, before anything runs. */
+int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                          const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids,
+                          acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort);
+
+/* letters consumed by every stream since its start or its last reset (cap >= n_streams).  Synchronises the device. */
+int acb_streams_positions(acb_streams *ss, int64_t *out, int64_t cap);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

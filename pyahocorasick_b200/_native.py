@@ -90,6 +90,12 @@ def lib() -> ctypes.CDLL:
         "acb_sort_matches_device": (ctypes.c_int, [vp, vp, i64, i64, i64, vp]),
         "acb_table_set_long_state": (ctypes.c_int, [vp, ctypes.c_int32]),
         "acb_table_get_long_state": (ctypes.c_int, [vp, ctypes.POINTER(ctypes.c_int32)]),
+        "acb_streams_new": (ctypes.c_int, [vp, i64, ctypes.c_int, ctypes.POINTER(vp)]),
+        "acb_streams_free": (None, [vp]),
+        "acb_streams_reset": (ctypes.c_int, [vp, vp, i64]),
+        "acb_streams_feed_device": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, vp, i64, vp, vp, ctypes.c_int]),
+        "acb_streams_feed_host": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, vp, i64, pi64, ctypes.c_int, ctypes.c_int]),
+        "acb_streams_positions": (ctypes.c_int, [vp, vp, i64]),
         "acb_launch_count": (i64, []),
         "acb_set_kernel_timing": (ctypes.c_int, [ctypes.c_int]),
         "acb_last_kernel_ms": (ctypes.c_float, []),
@@ -114,7 +120,9 @@ EXPORTED_SYMBOLS = [
     "acb_trie_content_hash", "acb_trie_flat_save", "acb_trie_flat_load",
     "acb_trie_export_nodes", "acb_trie_import_nodes", "acb_node_records_span",
     "acb_device_count", "acb_table_upload", "acb_table_free", "acb_table_device_bytes",
-    "acb_scan_device", "acb_scan_host", "acb_copy_records", "acb_take_records", "acb_release_records", "acb_sort_matches_device", "acb_table_set_long_state", "acb_table_get_long_state", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_scan_device", "acb_scan_host", "acb_copy_records", "acb_take_records", "acb_release_records", "acb_sort_matches_device", "acb_table_set_long_state", "acb_table_get_long_state",
+    "acb_streams_new", "acb_streams_free", "acb_streams_reset", "acb_streams_feed_device", "acb_streams_feed_host",
+    "acb_streams_positions", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

@@ -707,11 +707,7 @@ class Automaton:
         """Batch already resident in HBM: a C-contiguous uint8 torch CUDA tensor [n, stride].  No host copy of
         the haystacks; the scan runs on torch's current stream, only the records come back."""
         import torch
-        if t.dtype != torch.uint8 or t.dim() != 2 or not t.is_contiguous():
-            raise TypeError("device batches must be 2-D contiguous uint8 tensors [n_haystacks, stride_bytes]")
-        n, stride = int(t.shape[0]), int(t.shape[1])
-        if stride % self._L:
-            raise ValueError("row length must be a multiple of the letter width")
+        n, stride = self._device_batch_shape(t)
         if n == 0 or stride == 0:
             return np.empty(0, dtype=N.MATCH_DTYPE)
         dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
@@ -744,6 +740,16 @@ class Automaton:
             kl = np.asarray(self.flat()["key_len"])
             rec = rec[np.lexsort((-kl[rec["key_id"]], rec["end_index"], rec["hay_id"]))]
         return rec
+
+    def _device_batch_shape(self, t):
+        """(n, stride_bytes) of a device batch: a C-contiguous uint8 torch CUDA tensor [n, stride]"""
+        import torch
+        if t.dtype != torch.uint8 or t.dim() != 2 or not t.is_contiguous():
+            raise TypeError("device batches must be 2-D contiguous uint8 tensors [n_haystacks, stride_bytes]")
+        n, stride = int(t.shape[0]), int(t.shape[1])
+        if stride % self._L:
+            raise ValueError("row length must be a multiple of the letter width")
+        return n, stride
 
     def _scan_one(self, letters: np.ndarray, algo: str = "auto", long_state: Optional[int] = None) -> np.ndarray:
         narrow = self._uses_narrow() and letters.dtype == np.uint8 and algo != "long"
@@ -856,25 +862,36 @@ class Automaton:
         of the reference, returned as arrays.
         """
         self._require_automaton()
+        batch = self._batch_input(haystacks, narrow_ok=algo != "long")
+        if batch[0] == "device":
+            return Matches(self._scan_device_tensor(batch[1], algo, sort), self._values)
+        _, flat, offs, n, stride, narrow = batch
+        if not (n and flat.size):
+            return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
+        if narrow:
+            return Matches(self._scan_flat(flat, offs, n, stride, algo=algo, sort=sort, device=device, narrow=True), self._values)
+        return Matches(self._scan_flat(flat, offs, n, stride, algo=algo, sort=sort, device=device), self._values)
+
+    def _batch_input(self, haystacks, narrow_ok: bool = True):
+        """The input forms of find_all_batch, checked and laid out for a scan: ("device", tensor) for a CUDA tensor,
+        else ("host", flat uint8, int64 byte offsets or None, n, stride_bytes or 0, narrow).  narrow: the buffer holds
+        the 1-byte letters of the latin-1 automaton (unicode flavour, only where narrow_ok)."""
         L = self._L
         if type(haystacks).__module__.startswith("torch") and getattr(haystacks, "is_cuda", False):
-            return Matches(self._scan_device_tensor(haystacks, algo, sort), self._values)
+            return ("device", haystacks)
         if isinstance(haystacks, np.ndarray):
             if haystacks.dtype != np.uint8 or haystacks.ndim != 2 or not haystacks.flags.c_contiguous:
                 raise TypeError("array batches must be 2-D C-contiguous uint8 [n_haystacks, stride_bytes]")
             n, stride = haystacks.shape
             if stride % L:
                 raise ValueError("row length must be a multiple of the letter width")
-            rec = self._scan_flat(haystacks.reshape(-1), None, n, stride, algo=algo, sort=sort, device=device) if n and stride else np.empty(0, dtype=N.MATCH_DTYPE)
-            return Matches(rec, self._values)
+            return ("host", haystacks.reshape(-1), None, n, stride, False)
         if isinstance(haystacks, tuple) and len(haystacks) == 2 and isinstance(haystacks[0], np.ndarray) and isinstance(haystacks[1], np.ndarray):
             flat = np.ascontiguousarray(haystacks[0], dtype=np.uint8).reshape(-1)
             offs = np.ascontiguousarray(haystacks[1], dtype=np.int64)
             if offs.ndim != 1 or len(offs) < 1 or offs[0] != 0 or offs[-1] != flat.size or np.any(np.diff(offs) < 0) or np.any(offs % L):
                 raise ValueError("offsets must be non-decreasing multiples of the letter width, start at 0 and end at len(flat)")
-            n = len(offs) - 1
-            rec = self._scan_flat(flat, offs, n, 0, algo=algo, sort=sort, device=device) if n and flat.size else np.empty(0, dtype=N.MATCH_DTYPE)
-            return Matches(rec, self._values)
+            return ("host", flat, offs, len(offs) - 1, 0, False)
         # the latin-1 automaton finds exactly the matches of a latin-1 haystack -- all of them.  iter_long's walk is
         # different: which match it keeps depends on the whole trie (a non-latin-1 key whose prefix is latin-1 adds
         # nodes the walk passes through, src/AutomatonSearchIterLong.c:118-126), so it always runs on the full one
@@ -884,11 +901,8 @@ class Automaton:
             n = len(haystacks)
             offs = np.zeros(n + 1, dtype=np.int64)
             np.cumsum(np.fromiter(map(len, haystacks), dtype=np.int64, count=n), out=offs[1:])
-            flat = np.frombuffer(b"".join(haystacks), dtype=np.uint8)
-            if not flat.size:
-                return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
-            return Matches(self._scan_flat(flat, offs, n, 0, algo=algo, sort=sort, device=device), self._values)
-        get = self._letters if algo == "long" else self._hay_letters
+            return ("host", np.frombuffer(b"".join(haystacks), dtype=np.uint8), offs, n, 0, False)
+        get = self._hay_letters if narrow_ok else self._letters
         letters = [get(h, required=True) for h in haystacks]
         narrow = self._uses_narrow() and len(letters) > 0 and all(a.dtype == np.uint8 for a in letters)
         if self._uses_narrow() and not narrow:                   # mixed batch: everything at 4 bytes per letter
@@ -899,11 +913,207 @@ class Automaton:
         offs = np.zeros(n + 1, dtype=np.int64)
         np.cumsum(lens, out=offs[1:])
         flat = np.concatenate(parts) if n else np.empty(0, dtype=np.uint8)
-        if not (n and flat.size):
-            return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
-        if narrow:
-            return Matches(self._scan_flat(flat, offs, n, 0, algo=algo, sort=sort, device=device, narrow=True), self._values)
-        return Matches(self._scan_flat(flat, offs, n, 0, algo=algo, sort=sort, device=device), self._values)
+        return ("host", flat, offs, n, 0, narrow)
+
+    def stream_batch(self, n_streams: int, *, long: bool = False, algo: str = "auto",
+                     device: Optional[int] = None) -> "StreamBatch":
+        """`n_streams` independent streams searched chunk by chunk, the next chunk of many of them in one GPU call
+        (StreamBatch.feed).  long=False: stream s reports what the reference's ``iter(c0)`` ... ``.set(c1)`` ...
+        reports over its chunks -- every match, also those across chunk boundaries; long=True: what
+        ``iter_long(c0)`` ... ``.set(c1)`` reports.  What a stream carries from one chunk to the next stays in HBM.
+
+        Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
+        wider chunks, so the latin-1 automaton is not used)."""
+        if self.kind != AHOCORASICK:
+            raise AttributeError("Not an Aho-Corasick automaton yet: call add_word to add some keys and call "
+                                 "make_automaton to convert the trie to an automaton.")
+        n_streams = operator.index(n_streams)
+        if n_streams < 0:
+            raise ValueError("n_streams must not be negative")
+        if algo not in (("auto", "long") if long else ("auto", "filter", "dfa")):
+            raise ValueError(f"algo {algo!r} does not fit a {'long' if long else 'find_all'} stream batch")
+        return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device)
+
+
+class StreamBatch:
+    """Result of `Automaton.stream_batch()`: the carry-over of `n_streams` streams, kept on the GPU.
+
+    ``feed(chunks, ids=None)`` hands over the next chunk of some streams and returns a `Matches` whose ``hay_id`` is
+    the stream id and whose ``end_index`` (int64) is the position of the match's last letter in the whole stream,
+    counted from its start or its last `reset` -- exact past 2^31, unlike the reference's C int (SURVEY A7).  Records
+    come in chunk order, then end_index ascending, then longest key first.  ``positions`` is the number of letters
+    every stream has consumed.  A stream batch belongs to the key set it was made for: after the key set changes,
+    `feed` and `reset` raise ValueError as a stale iterator does."""
+
+    def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int):
+        self._A = A
+        self._version = A._version
+        self.n_streams = n_streams
+        self.long = long
+        self._algo = algo
+        self._device = device
+        self._pos = np.zeros(n_streams, dtype=np.int64)        # host mirror of the positions, for end_index
+        with A._gpu_lock:
+            self._ss = self._native("new")
+
+    def __del__(self):
+        try:
+            if getattr(self, "_ss", None) is not None:
+                self._native("free")
+                self._ss = None
+        except Exception:                                   # interpreter shutdown
+            pass
+
+    def _check(self):
+        if self._version != self._A._version:
+            raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
+
+    def _native(self, op: str, *args):
+        """Every call into the native stream batch (acb_streams_*) goes through here.
+          new -> handle;  free;  reset(ids int32 or None);  positions -> int64[n_streams];
+          feed(kind, data, offsets, n, stride, ids, sort) -> records (hay_id = chunk index, end_index in the chunk)"""
+        A = self._A
+        lib = A._lib
+        if op == "new":
+            ss = ctypes.c_void_p()
+            N.check(lib.acb_streams_new(A._ensure_table(self._device), self.n_streams, int(self.long), ctypes.byref(ss)))
+            return ss
+        if op == "free":
+            lib.acb_streams_free(self._ss)
+            return None
+        if op == "reset":
+            ids, = args
+            N.check(lib.acb_streams_reset(self._ss, None if ids is None else N.ptr(ids), 0 if ids is None else len(ids)))
+            return None
+        if op == "positions":
+            out = np.empty(max(self.n_streams, 1), dtype=np.int64)
+            N.check(lib.acb_streams_positions(self._ss, N.ptr(out), self.n_streams))
+            return out[:self.n_streams]
+        kind, data, offs, n, stride, ids, sort = args
+        algo = N.ALGOS[self._algo]
+        if kind == "device":
+            return self._feed_device(data, ids, sort, algo)
+        tb = A._ensure_table(self._device)
+        total = int(data.size)
+        cap = max(A._match_cap, 1 << 12, 2 * n)
+        found = ctypes.c_int64(0)
+        while True:
+            rc = lib.acb_streams_feed_host(self._ss, tb, N.ptr(data) if total else None, total,
+                                           None if offs is None else N.ptr(offs), n, stride,
+                                           None if ids is None else N.ptr(ids), None, cap, ctypes.byref(found), algo, int(sort))
+            if rc == N.ACB_EOVERFLOW:                        # nothing was committed: the same feed again, with room
+                cap = A._match_cap = int(found.value) + 1024
+                continue
+            N.check(rc)
+            break
+        if not found.value:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        ptr, got, room = ctypes.c_void_p(), ctypes.c_int64(0), ctypes.c_int64(0)
+        N.check(lib.acb_take_records(tb, ctypes.byref(ptr), ctypes.byref(got), ctypes.byref(room)))
+        if not ptr.value or got.value != found.value:
+            raise N.NativeError("acb_take_records: no records to take")
+        return np.asarray(_PinnedRecords(lib, ptr.value, got.value, room.value))
+
+    def _feed_device(self, t, ids, sort, algo):
+        import torch
+        A = self._A
+        n, stride = A._device_batch_shape(t)
+        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        if dev != self._device:
+            raise ValueError(f"chunks on cuda:{dev} for a stream batch on cuda:{self._device}")
+        tb = A._ensure_table(self._device)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream().cuda_stream
+            d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
+            cnt = torch.empty(1, dtype=torch.int64, device=t.device)
+            cap = max(A._match_cap, 1 << 12, 2 * n)
+            while True:
+                out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+                N.check(A._lib.acb_streams_feed_device(self._ss, tb, t.data_ptr() if n and stride else None, n * stride, None,
+                                                       n, stride, None if d_ids is None else d_ids.data_ptr(),
+                                                       out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
+                found = int(cnt.item())
+                if found > cap:                              # nothing was committed: the same feed again, with room
+                    cap = A._match_cap = found + 1024
+                    continue
+                break
+            sort_on_host = False
+            if sort and found > 1:
+                rc = A._lib.acb_sort_matches_device(tb, out.data_ptr(), found, n, stride // A._L, stream)
+                if rc == N.ACB_ERANGE:
+                    sort_on_host = True
+                else:
+                    N.check(rc)
+            rec = out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
+        if sort_on_host:
+            kl = np.asarray(A.flat()["key_len"])
+            rec = rec[np.lexsort((-kl[rec["key_id"]], rec["end_index"], rec["hay_id"]))]
+        return rec
+
+    def _ids(self, ids, n: int) -> Optional[np.ndarray]:
+        if ids is None:
+            if n > self.n_streams:
+                raise ValueError(f"{n} chunks for {self.n_streams} streams: pass ids")
+            return None
+        a = np.asarray(ids)
+        if a.ndim != 1 or len(a) != n or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise ValueError(f"ids must be {n} integers, one per chunk")
+        if a.size and (a.min() < 0 or a.max() >= self.n_streams):
+            raise ValueError(f"stream ids must lie in [0, {self.n_streams})")
+        if len(np.unique(a)) != len(a):
+            raise ValueError("a stream id is given twice")
+        return np.ascontiguousarray(a, dtype=np.int32)
+
+    def feed(self, chunks, ids=None, *, sort: bool = True) -> Matches:
+        """The next chunk of some streams: chunk h continues stream ids[h] (default: stream h).  `chunks` takes the
+        input forms of find_all_batch; in a list, None is an empty chunk.  Returns the matches that end inside
+        these chunks (see the class)."""
+        A = self._A
+        with A._gpu_lock:
+            self._check()
+            if isinstance(chunks, list) or (isinstance(chunks, tuple) and not (len(chunks) == 2 and isinstance(chunks[0], np.ndarray))):
+                empty = () if A._key_type == KEY_SEQUENCE else ("" if A._UNICODE else b"")
+                chunks = [empty if c is None else c for c in chunks]
+            batch = A._batch_input(chunks, narrow_ok=False)
+            if batch[0] == "device":
+                n, stride = A._device_batch_shape(batch[1])
+                lens = np.full(n, stride // A._L, dtype=np.int64)
+                args = ("device", batch[1], None, n, stride)
+            else:
+                _, flat, offs, n, stride, _ = batch
+                lens = (np.diff(offs) if offs is not None else np.full(n, stride, dtype=np.int64)) // A._L
+                args = ("host", flat, offs, n, stride)
+            ids32 = self._ids(ids, n)
+            rec = self._native("feed", *args, ids32, sort)
+            sid = np.arange(n, dtype=np.int64) if ids32 is None else ids32.astype(np.int64)
+            m = Matches(rec, A._values)
+            chunk = rec["hay_id"]
+            m.hay_id = sid[chunk]
+            m.end_index = rec["end_index"].astype(np.int64) + self._pos[m.hay_id]
+            self._pos[sid] += lens
+            return m
+
+    def reset(self, ids=None) -> None:
+        """Streams `ids` (default: all) back to their start, as ``set(x, reset=True)`` does: position 0, nothing
+        carried over."""
+        with self._A._gpu_lock:
+            self._check()
+            if ids is None:
+                self._native("reset", None)
+                self._pos[:] = 0
+                return
+            a = np.asarray(ids)
+            if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)) or (a.size and (a.min() < 0 or a.max() >= self.n_streams)):
+                raise ValueError(f"stream ids must be integers in [0, {self.n_streams})")
+            a = np.unique(a).astype(np.int32)
+            self._native("reset", a)
+            self._pos[a] = 0
+
+    @property
+    def positions(self) -> np.ndarray:
+        """int64[n_streams]: letters every stream has consumed since its start or its last reset (a copy)."""
+        with self._A._gpu_lock:
+            return self._native("positions")
 
 
 class AutomatonSearchIter:

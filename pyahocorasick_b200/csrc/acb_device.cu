@@ -140,6 +140,8 @@ struct ScanParams {
     uint2 *cand;                   /* candidate entries, kWarpCand per consumer warp of every CTA: {position in the segment, anchor tag} */
     int stride_shift;              /* log2(stride_bytes) when it is a power of two, else -1 */
     int letter_shift;              /* log2(L) */
+    const int32_t *long_start;     /* ACB_ALGO_LONG of a stream batch: the state every haystack starts in (nullptr: long_init / root) */
+    int32_t *long_end;             /* ... and where the state every haystack ends in goes (may be null) */
 };
 
 /* ---------------------------------------------------------------- helpers */
@@ -1202,7 +1204,7 @@ __global__ void __launch_bounds__(kDfaThreads) acb_long_kernel(const __grid_cons
     const long long he = p.offsets ? __ldg(p.offsets + h + 1) : hs + p.stride_bytes;
     const long long n = (he - hs) / p.L;                       /* letters */
     const uint8_t *text = p.hay + hs;
-    int32_t state = (h == 0) ? p.long_init : 0, last_node = -1;     /* the walk of a stream goes on where the last chunk left it */
+    int32_t state = p.long_start ? __ldg(p.long_start + h) : ((h == 0) ? p.long_init : 0), last_node = -1;   /* the walk of a stream goes on where the last chunk left it */
     long long index = -1, last_index = -1;
     for (;;) {
         if (last_node >= 0) {                                   /* return_output */
@@ -1245,6 +1247,7 @@ __global__ void __launch_bounds__(kDfaThreads) acb_long_kernel(const __grid_cons
         if (!emit && last_node < 0) break;                      /* StopIteration */
     }
     if (h == 0 && p.long_final) *p.long_final = state;
+    if (p.long_end) p.long_end[h] = state;
 }
 
 __global__ void acb_flag_goto_kernel(int32_t *gto, const int32_t *key_of, size_t n) {
@@ -1917,3 +1920,333 @@ extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_by
     return ACB_OK;
 }
 
+
+/* ------------------------------------------------------------ stream batches */
+/* A stream batch (acb_streams) keeps every stream's carry-over in HBM: the number of letters consumed, and either the
+ * last T = longest_word - 1 letters (find_all semantics) or the walk state (iter_long semantics).  A feed scans the
+ * chunks themselves with the ordinary scan (acb_scan_device: every match that starts and ends inside a chunk), then one
+ * lane per chunk walks the goto/fail automaton over the chunk's seam -- its stream's tail followed by the first
+ * min(T, n) letters of the chunk -- and reports only the matches that start in the tail and end in the chunk.  A match
+ * that ends in the chunk but starts before it has at most T + 1 letters, so at most T of them lie in the chunk and the
+ * seam holds all of it; a chunk shorter than T is covered by the next feed, whose tail is the last T letters of
+ * tail || chunk.  The new tails (long mode: end states) go to per-feed staging; a commit kernel copies them into the
+ * streams and advances the positions only when the feed's records fit the caller's buffer, so a feed that overflows
+ * changes no stream and can be repeated with a larger buffer. */
+namespace {
+struct StreamsArgs {
+    const int32_t *ids;           /* chunk -> stream; nullptr: chunk h continues stream h */
+    long long n_streams;
+    long long *pos;               /* [n_streams] letters consumed since the start / the last reset */
+    uint8_t *tail;                /* [n_streams][T letters]: the last min(T, pos) letters consumed, left aligned */
+    uint8_t *next_tail;           /* [n_chunks][T letters]: the tail after this feed's chunk (staged) */
+    int32_t *state;               /* long mode: [n_streams] walk state */
+    int32_t *start, *end;         /* long mode: [n_chunks] the state a chunk starts / ends in (staged) */
+    int T;                        /* tail letters; 0 in long mode */
+    int L;
+};
+
+__device__ __forceinline__ long long chunk_stream(const StreamsArgs &a, long long h) {
+    const long long s = a.ids ? (long long)__ldg(a.ids + h) : h;
+    return (s >= 0 && s < a.n_streams) ? s : -1;           /* ids are validated by the caller; never index outside */
+}
+
+__device__ __forceinline__ void chunk_span(const long long *off, long long stride, long long h, long long &hs, long long &he) {
+    hs = off ? __ldg(off + h) : h * stride;
+    he = off ? __ldg(off + h + 1) : hs + stride;
+}
+
+/* the seam of chunk h: walk tail || first min(T, n) letters from the root, report what straddles the chunk's start,
+ * stage the next tail */
+__global__ void __launch_bounds__(kDfaThreads) acb_seam_kernel(const __grid_constant__ ScanParams p, const StreamsArgs a) {
+    const long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= p.n_hay) return;
+    const long long s = chunk_stream(a, h);
+    if (s < 0) return;
+    long long hs, he;
+    chunk_span(p.offsets, p.stride_bytes, h, hs, he);
+    const int L = p.L, ls = p.letter_shift;                      /* L == 1 << ls */
+    const long long n = (he - hs) >> ls;
+    const long long t = min((long long)a.T, a.pos[s]), m = min((long long)a.T, n);
+    const uint8_t *tail = a.tail + s * a.T * L, *text = p.hay + hs;
+    const long long tb = t * L;
+    int32_t st = 0;
+    for (long long i = 0; i < (t + m) * L; ++i) {
+        const uint8_t c = i < tb ? tail[i] : text[i - tb];
+        const long long col = (long long)__ldg(p.cls + c) * p.S;
+        int32_t nx;
+        while ((nx = __ldg(p.gto + col + st)) < 0 && st != 0) st = __ldg(p.fail + st);   /* src/trie.c:182-190 */
+        st = (nx < 0) ? 0 : (nx & kIdMask);
+        if (i < tb || st == 0 || ((i + 1) & (L - 1))) continue;
+        const long long e = ((i + 1) >> ls) - 1;                 /* letter of the seam */
+        const int32_t o1 = __ldg(p.out_ptr + st + 1);
+        for (int32_t o = __ldg(p.out_ptr + st); o < o1; ++o) {
+            const int32_t k = __ldg(p.out_idx + o);
+            if (e - __ldg(p.key_len + k) + 1 >= t) break;         /* longest first: this key and the rest start in the chunk */
+            unsigned long long g = atomicAdd(p.count, 1ULL);
+            if (g < (unsigned long long)p.cap) {
+                acb_match r;
+                r.hay_id = (int32_t)h;
+                r.end_index = (int32_t)(e - t);
+                r.key_id = k;
+                p.out[g] = r;
+            }
+        }
+    }
+    const long long nt = min((long long)a.T, t + n), from = (t + n - nt) * L;
+    uint8_t *dst = a.next_tail + h * a.T * L;
+    for (long long j = 0; j < nt * L; ++j) {
+        const long long x = from + j;
+        dst[j] = x < tb ? tail[x] : text[x - tb];
+    }
+}
+
+__global__ void acb_streams_gather_kernel(const StreamsArgs a, long long n_chunks) {
+    const long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= n_chunks) return;
+    const long long s = chunk_stream(a, h);
+    a.start[h] = s < 0 ? 0 : a.state[s];
+}
+
+/* switch the fed streams to what the feed staged, only when its records fit (count == nullptr: unconditionally) */
+__global__ void acb_streams_commit_kernel(const StreamsArgs a, const long long *off, long long stride, long long n_chunks,
+                                          const unsigned long long *count, long long cap) {
+    const long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= n_chunks || (count && *count > (unsigned long long)cap)) return;
+    const long long s = chunk_stream(a, h);
+    if (s < 0) return;
+    long long hs, he;
+    chunk_span(off, stride, h, hs, he);
+    if (a.end) a.state[s] = a.end[h];
+    const long long tb = (long long)a.T * a.L;
+    for (long long j = 0; j < tb; ++j) a.tail[s * tb + j] = a.next_tail[h * tb + j];
+    a.pos[s] += (he - hs) / a.L;
+}
+
+__global__ void acb_streams_reset_kernel(const StreamsArgs a, long long n_ids) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_ids) return;
+    const long long s = chunk_stream(a, i);
+    if (s < 0) return;
+    a.pos[s] = 0;
+    if (a.state) a.state[s] = 0;
+}
+} // namespace
+
+struct acb_streams {
+    int device = 0;
+    int32_t L = 1, T = 0, S = 0;                 /* letter width, tail letters and (long mode) state count of the table */
+    int long_mode = 0;
+    long long n = 0;
+    long long *d_pos = nullptr;
+    uint8_t *d_tail = nullptr;
+    int32_t *d_state = nullptr;
+    uint8_t *d_next_tail = nullptr; size_t next_tail_cap = 0;     /* per-feed staging, grown on demand */
+    int32_t *d_start = nullptr; size_t start_cap = 0;
+    int32_t *d_end = nullptr; size_t end_cap = 0;
+    int32_t *d_ids = nullptr; size_t ids_cap = 0;                 /* ids of a host feed or a reset, uploaded */
+};
+
+static int32_t tail_letters(const acb_table *tb) { return std::max<int32_t>(tb->max_key_bytes / tb->L - 1, 0); }
+
+static int streams_check_table(const acb_streams *ss, const acb_table *tb) {
+    if (tb->device != ss->device || tb->L != ss->L || (!ss->long_mode && tail_letters(tb) != ss->T) || (ss->long_mode && tb->S != ss->S)) {
+        acb_set_error("the table does not belong to this stream batch (device %d/%d, letter bytes %d/%d, tail %d/%d, states %d/%d)",
+                      tb->device, ss->device, tb->L, ss->L, ss->long_mode ? 0 : tail_letters(tb), ss->T, tb->S, ss->S);
+        return ACB_EINVAL;
+    }
+    return ACB_OK;
+}
+
+static StreamsArgs streams_args(const acb_streams *ss, const int32_t *d_ids) {
+    StreamsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.tail = ss->d_tail; a.state = ss->d_state; a.T = ss->T; a.L = ss->L;
+    return a;
+}
+
+extern "C" void acb_streams_free(acb_streams *ss) {
+    if (!ss) return;
+    cudaSetDevice(ss->device);
+    cudaFree(ss->d_pos); cudaFree(ss->d_tail); cudaFree(ss->d_state); cudaFree(ss->d_next_tail);
+    cudaFree(ss->d_start); cudaFree(ss->d_end); cudaFree(ss->d_ids);
+    delete ss;
+}
+
+extern "C" int acb_streams_new(const acb_table *tb, int64_t n_streams, int long_mode, acb_streams **out) {
+    if (!tb || !out || n_streams < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    if (n_streams > 0x7fffffffLL) { acb_set_error("more than 2^31-1 streams"); return ACB_ERANGE; }
+    CUDA_TRY(cudaSetDevice(tb->device));
+    acb_streams *ss = new (std::nothrow) acb_streams();
+    if (!ss) { acb_set_error("out of memory"); return ACB_ENOMEM; }
+    ss->device = tb->device; ss->L = tb->L; ss->S = tb->S; ss->long_mode = long_mode ? 1 : 0;
+    ss->T = ss->long_mode ? 0 : tail_letters(tb);
+    ss->n = n_streams;
+    const size_t n = (size_t)std::max<int64_t>(n_streams, 1);
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ss->d_pos), n * sizeof(long long));
+    if (e == cudaSuccess) e = cudaMemset(ss->d_pos, 0, n * sizeof(long long));
+    if (e == cudaSuccess && ss->T) e = cudaMalloc(reinterpret_cast<void **>(&ss->d_tail), n * ss->T * ss->L);
+    if (e == cudaSuccess && ss->long_mode) e = cudaMalloc(reinterpret_cast<void **>(&ss->d_state), n * sizeof(int32_t));
+    if (e == cudaSuccess && ss->long_mode) e = cudaMemset(ss->d_state, 0, n * sizeof(int32_t));
+    if (e != cudaSuccess) {
+        acb_set_error("allocating %lld streams: %s", (long long)n_streams, cudaGetErrorString(e));
+        acb_streams_free(ss);
+        return ACB_ECUDA;
+    }
+    *out = ss;
+    return ACB_OK;
+}
+
+/* the device feed; d_count is zeroed here, on `s` */
+static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total, const int64_t *d_off,
+                        int64_t n_chunks, int64_t stride, const int32_t *d_ids, acb_match *d_out, int64_t cap,
+                        int64_t *d_count, cudaStream_t s, int algo) {
+    if (!ss || !tb || !d_count || total < 0 || n_chunks < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    int rc = streams_check_table(ss, tb);
+    if (rc != ACB_OK) return rc;
+    if (n_chunks > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, ss->n); return ACB_EINVAL; }
+    if (!d_off && n_chunks && (stride <= 0 || stride % ss->L || stride * n_chunks != total)) {
+        acb_set_error("fixed-stride feed needs stride_bytes > 0, a multiple of letter_bytes, and n_chunks*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    if (algo == ACB_ALGO_AUTO) algo = ss->long_mode ? ACB_ALGO_LONG : ACB_ALGO_FILTER;
+    if (ss->long_mode ? algo != ACB_ALGO_LONG : (algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA)) {
+        acb_set_error("algo %d does not fit a %s stream batch", algo, ss->long_mode ? "iter_long" : "find_all");
+        return ACB_EINVAL;
+    }
+    CUDA_TRY(cudaSetDevice(ss->device));
+    CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
+    if (total == 0 || n_chunks == 0) return ACB_OK;              /* empty chunks move no stream */
+    if (reinterpret_cast<uintptr_t>(d_chunks) & 15) { acb_set_error("d_chunks must be 16-byte aligned"); return ACB_EINVAL; }
+    ScanParams p;
+    fill_params(tb, p, d_chunks, total, d_off, n_chunks, stride, d_out, cap, d_count);
+    StreamsArgs a = streams_args(ss, d_ids);
+    const unsigned grid = (unsigned)((n_chunks + kDfaThreads - 1) / kDfaThreads);
+    if (ss->long_mode) {
+        if ((rc = ensure(&ss->d_start, &ss->start_cap, (size_t)n_chunks)) || (rc = ensure(&ss->d_end, &ss->end_cap, (size_t)n_chunks))) return rc;
+        a.start = ss->d_start;
+        a.end = ss->d_end;
+        acb_streams_gather_kernel<<<grid, kDfaThreads, 0, s>>>(a, n_chunks);
+        CUDA_TRY(cudaGetLastError());
+        p.long_start = a.start;
+        p.long_end = a.end;
+        acb_long_kernel<<<grid, kDfaThreads, 0, s>>>(p);
+        CUDA_TRY(cudaGetLastError());
+        g_launches.fetch_add(2);
+    } else {
+        if (tb->n_keys > 0 && (rc = acb_scan_device(tb, d_chunks, total, d_off, n_chunks, stride, d_out, cap, d_count, s, algo))) return rc;
+        if (ss->T > 0) {
+            if ((rc = ensure(&ss->d_next_tail, &ss->next_tail_cap, (size_t)n_chunks * ss->T * ss->L))) return rc;
+            a.next_tail = ss->d_next_tail;
+            acb_seam_kernel<<<grid, kDfaThreads, 0, s>>>(p, a);
+            CUDA_TRY(cudaGetLastError());
+            g_launches.fetch_add(1);
+        }
+    }
+    acb_streams_commit_kernel<<<grid, kDfaThreads, 0, s>>>(a, reinterpret_cast<const long long *>(d_off), stride, n_chunks,
+                                                          reinterpret_cast<const unsigned long long *>(d_count), cap);
+    CUDA_TRY(cudaGetLastError());
+    g_launches.fetch_add(1);
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_feed_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                                       const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
+                                       acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    return streams_feed(ss, tb, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, d_out, cap, d_count,
+                        reinterpret_cast<cudaStream_t>(stream), algo);
+}
+
+/* ids of a host call: each in [0, n_streams), no two alike */
+static int check_ids(const acb_streams *ss, const int32_t *ids, int64_t n) {
+    std::vector<uint8_t> seen;
+    try { seen.assign((size_t)ss->n, 0); } catch (const std::exception &) { acb_set_error("out of host memory"); return ACB_ENOMEM; }
+    for (int64_t i = 0; i < n; i++) {
+        if (ids[i] < 0 || ids[i] >= ss->n) { acb_set_error("stream id %d out of range [0, %lld)", ids[i], ss->n); return ACB_EINVAL; }
+        if (seen[ids[i]]++) { acb_set_error("stream id %d given twice", ids[i]); return ACB_EINVAL; }
+    }
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                                     const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids,
+                                     acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort) {
+    if (!ss || !tb || !n_found || total_bytes < 0 || n_chunks < 0 || cap < 0 || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *n_found = 0;
+    tb->h_out_n = 0;
+    int rc;
+    if (ids && (rc = check_ids(ss, ids, n_chunks))) return rc;
+    if ((rc = streams_check_table(ss, tb))) return rc;
+    if (n_chunks > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, ss->n); return ACB_EINVAL; }
+    if (total_bytes == 0 || n_chunks == 0) return ACB_OK;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
+    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_chunks + 1))) return rc;
+    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1)))) return rc;
+    if (ids && (rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)n_chunks))) return rc;
+    cudaStream_t s = tb->stream;
+    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, chunks, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
+    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_chunks + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+    if (ids) CUDA_TRY(cudaMemcpyAsync(ss->d_ids, ids, (size_t)n_chunks * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    rc = streams_feed(ss, tb, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_chunks,
+                      stride_bytes, ids ? ss->d_ids : nullptr, tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), s, algo);
+    if (rc != ACB_OK) return rc;
+    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    const unsigned long long n = *tb->h_count;
+    *n_found = (int64_t)n;
+    if (n > (unsigned long long)cap) {
+        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
+        return ACB_EOVERFLOW;
+    }
+    if (n) {
+        if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
+        bool host_sort = sort != 0;
+        const int64_t max_letters = (offsets ? total_bytes : stride_bytes) / tb->L;
+        if (sort && acb_sort_matches_device(tb, tb->w_out, (int64_t)n, n_chunks, max_letters, s) == ACB_OK) host_sort = false;
+        CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->w_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (host_sort) {
+            const int32_t *kl = tb->key_len.data();
+            std::sort(tb->h_out, tb->h_out + n, [kl](const acb_match &a, const acb_match &b) {
+                if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
+                if (a.end_index != b.end_index) return a.end_index < b.end_index;
+                return kl[a.key_id] > kl[b.key_id];
+            });
+        }
+        if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
+    }
+    tb->h_out_n = n;
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n) {
+    if (!ss || n < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    int rc;
+    if (ids && (rc = check_ids(ss, ids, n))) return rc;
+    CUDA_TRY(cudaSetDevice(ss->device));
+    CUDA_TRY(cudaDeviceSynchronize());                           /* feeds in flight on any stream see the old state */
+    if (!ids) {
+        CUDA_TRY(cudaMemset(ss->d_pos, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(long long)));
+        if (ss->d_state) CUDA_TRY(cudaMemset(ss->d_state, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(int32_t)));
+    } else if (n) {
+        if ((rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)n))) return rc;
+        CUDA_TRY(cudaMemcpy(ss->d_ids, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice));
+        acb_streams_reset_kernel<<<(unsigned)((n + 255) / 256), 256>>>(streams_args(ss, ss->d_ids), n);
+        CUDA_TRY(cudaGetLastError());
+        g_launches.fetch_add(1);
+    }
+    CUDA_TRY(cudaDeviceSynchronize());
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_positions(acb_streams *ss, int64_t *out, int64_t cap) {
+    if (!ss || cap < ss->n || (ss->n && !out)) { acb_set_error("bad argument (capacity %lld for %lld streams)", (long long)cap, ss ? ss->n : 0LL); return ACB_EINVAL; }
+    CUDA_TRY(cudaSetDevice(ss->device));
+    CUDA_TRY(cudaDeviceSynchronize());
+    if (ss->n) CUDA_TRY(cudaMemcpy(out, ss->d_pos, (size_t)ss->n * sizeof(long long), cudaMemcpyDeviceToHost));
+    return ACB_OK;
+}
