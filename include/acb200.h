@@ -214,8 +214,9 @@ enum {
  * Replaces the loop in automaton_search_iter_next (src/AutomatonSearchIter.c:243-300)
  * and automaton_find_all (src/Automaton.c:693-714) for a whole batch at once.
  *
- *   d_hay      : all haystacks back to back, total_bytes bytes
- *   d_offsets  : n_hay+1 byte offsets (int64, multiples of letter_bytes), or NULL
+ *   d_hay      : all haystacks back to back, total_bytes bytes; 16-byte aligned (the scan reads it with TMA bulk
+ *                copies), else ACB_EINVAL.  A view into a larger buffer that starts elsewhere must be copied first.
+ *   d_offsets : n_hay+1 byte offsets (int64, multiples of letter_bytes), or NULL
  *                when every haystack is `stride_bytes` long (haystack h = [h*stride, (h+1)*stride))
  *   d_out/cap  : match records; records beyond cap are counted but not stored
  *   d_count    : device int64; incremented by the number of matches found
@@ -293,7 +294,7 @@ void acb_streams_free(acb_streams *ss);
 int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n);
 
 /* DEVICE buffers, asynchronous on `stream`.  Zeroes *d_count itself, then counts every record (stored up to cap).
- * d_ids is not checked: the caller guarantees distinct ids in range.  algo: ACB_ALGO_AUTO, _FILTER or _DFA for a
+ * d_chunks must be 16-byte aligned, as d_hay of acb_scan_device, else ACB_EINVAL.  d_ids is not checked: the caller guarantees distinct ids in range.  algo: ACB_ALGO_AUTO, _FILTER or _DFA for a
  * find_all batch (the scan of the chunks; seams are always walked), ACB_ALGO_AUTO or _LONG for an iter_long batch.
  * Records are unsorted: acb_sort_matches_device(tb, d_out, n, n_chunks, longest chunk in letters, stream). */
 int acb_streams_feed_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,

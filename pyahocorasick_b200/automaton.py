@@ -710,6 +710,7 @@ class Automaton:
         n, stride = self._device_batch_shape(t)
         if n == 0 or stride == 0:
             return np.empty(0, dtype=N.MATCH_DTYPE)
+        t = _aligned(t)
         dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
         tb = self._ensure_table(dev)
         with torch.cuda.device(dev):
@@ -1021,6 +1022,8 @@ class StreamBatch:
         dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
         if dev != self._device:
             raise ValueError(f"chunks on cuda:{dev} for a stream batch on cuda:{self._device}")
+        if n and stride:
+            t = _aligned(t)
         tb = A._ensure_table(self._device)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream().cuda_stream
@@ -1311,6 +1314,13 @@ def _parse_start_end(args, i_start, i_end, lo, hi):
     if end < lo or end > hi:
         raise IndexError(f"end index not in range {lo}..{hi}")
     return start, end
+
+
+def _aligned(t):
+    """A device batch whose data starts on a 16-byte boundary, as the scan's TMA bulk copies need: `t` itself, or for
+    a view that starts elsewhere (e.g. d[1:] of a [n, 7] tensor) a copy in fresh storage on the same device, made on
+    the current stream."""
+    return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
 def _default_device() -> int:

@@ -1,7 +1,8 @@
 """The record buffer's bounds and the record sort, against the oracle and a plain numpy restatement.
 
 Record capacity.  Every kernel stores a record through `g = atomicAdd(count)` and `if (g < cap)`: the warp staging of the
-stream kernel (emit, flush_stage), the pair kernel's emit_direct and batched resolve, the DFA and the iter_long kernel.
+stream kernel (emit, flush_stage), the pair kernel's emit_direct and batched resolve, the DFA and the iter_long kernel, and in a stream-batch feed the
+seam kernel and the iter_long kernel with per-stream start states.
 The callers' retry depends on two things: the count is exact when the buffer overflows, and nothing is written at or
 past `cap`.  Each kernel here writes into an int32[cap + GUARD, 3] torch buffer filled with -1 that is passed with
 capacity `cap`, so an overrun lands in the guard rows of the same allocation.  acb_scan_host is checked the same way on
@@ -93,15 +94,70 @@ def _case(name, monkeypatch):
     return A, N.ALGO_FILTER, t, off, _tuples(O.scan_batch_bytes(t, off))
 
 
-KERNELS = ["pair", "pair_multi", "narrow", "wide", "dfa", "long"]
+def _feed_case(name):
+    """Stream-batch feeds through the C ABI (acb_streams_feed_device), after a first feed that leaves every stream
+    with a tail or inside a key.  seam: every key has 6 letters or more and the second chunks have 4, so every record is
+    written by the seam kernel; long_states: the iter_long kernel with per-stream start states.  Returns
+    (automaton, algo, first chunks, (second chunks, offsets), the second feed's records: (chunk, end in it, key))."""
+    rng = np.random.Generator(np.random.PCG64(606))
+    ab = np.frombuffer(b"ab", dtype=np.uint8)
+    if name == "seam":
+        keys = [bytes(b"ab"[(i >> j) & 1] for j in range(6)) for i in range(64)] + [b"abbabaabba"]   # T = 9
+        w0, w1, n_streams = 8, 4, 700
+    else:
+        keys = sorted({bytes(rng.choice(ab, size=int(rng.integers(3, 10)))) for _ in range(20)})
+        w0, w1, n_streams = 7, 9, 800
+    A = synth.build_automaton(keys)
+    first = rng.choice(ab, size=(n_streams, w0))
+    second = rng.choice(ab, size=(n_streams, w1))
+    want = []
+    if name == "seam":
+        O = _oracle(keys)
+        for s in range(n_streams):
+            want += [(s, e - w0, k) for e, k in O.find_all(first[s].tobytes() + second[s].tobytes()) if e >= w0]
+    else:
+        for s in range(n_streams):
+            it = A.iter_long(first[s].tobytes())
+            list(it)
+            it.set(second[s].tobytes())
+            want += [(s, e - w0, k) for e, k in it]
+    off = np.arange(n_streams + 1, dtype=np.int64) * w1
+    return A, N.ALGO_LONG if name == "long_states" else N.ALGO_FILTER, first, (second.reshape(-1).copy(), off), want
+
+
+FEED_KERNELS = ["seam", "long_states"]
+KERNELS = ["pair", "pair_multi", "narrow", "wide", "dfa", "long"] + FEED_KERNELS
 CAPS = ["0", "1", "31", "32", "33", "64", "65", "n-1", "n", "n+1"]
 _cases = {}
 
 
 def _cached(name, monkeypatch):
     if name not in _cases:
-        _cases[name] = _case(name, monkeypatch)
+        _cases[name] = _feed_case(name) if name in FEED_KERNELS else _case(name, monkeypatch)
     return _cases[name]
+
+
+def _write(kernel, A, algo, first, t, off, d_out, c, d_cnt, stream):
+    """one scan (or, for a stream-batch site, a fresh batch's second feed) into d_out with capacity c"""
+    import torch
+    lib, tb = N.lib(), A._ensure_table(0)
+    d_hay = torch.from_numpy(t).cuda()
+    d_off = torch.from_numpy(off).cuda()
+    if kernel not in FEED_KERNELS:
+        N.check(lib.acb_scan_device(tb, d_hay.data_ptr(), t.size, d_off.data_ptr(), len(off) - 1, 0,
+                                    d_out.data_ptr() if c else None, c, d_cnt.data_ptr(), stream.cuda_stream, algo))
+        return
+    ss = ctypes.c_void_p()
+    N.check(lib.acb_streams_new(tb, len(first), int(kernel == "long_states"), ctypes.byref(ss)))
+    try:
+        found = ctypes.c_int64(0)
+        N.check(lib.acb_streams_feed_host(ss, tb, N.ptr(first), first.size, None, len(first), first.shape[1], None,
+                                          None, 1 << 16, ctypes.byref(found), algo, 1))
+        N.check(lib.acb_streams_feed_device(ss, tb, d_hay.data_ptr(), t.size, d_off.data_ptr(), len(off) - 1, 0, None,
+                                            d_out.data_ptr() if c else None, c, d_cnt.data_ptr(), stream.cuda_stream, algo))
+        stream.synchronize()
+    finally:
+        lib.acb_streams_free(ss)
 
 
 @pytest.mark.gpu
@@ -110,17 +166,16 @@ def _cached(name, monkeypatch):
 def test_scan_device_never_writes_past_cap(kernel, cap, monkeypatch):
     import torch
     A, algo, t, off, want = _cached(kernel, monkeypatch)
+    first = None
+    if kernel in FEED_KERNELS:
+        first, (t, off) = t, off
     n = len(want)
     assert n > 200
     c = {"n-1": n - 1, "n": n, "n+1": n + 1}[cap] if cap.startswith("n") else int(cap)
-    tb = A._ensure_table(0)
-    d_hay = torch.from_numpy(t).cuda()
-    d_off = torch.from_numpy(off).cuda()
     d_cnt = torch.zeros(1, dtype=torch.int64, device="cuda")
     d_out = torch.full((c + GUARD, 3), -1, dtype=torch.int32, device="cuda")
     stream = torch.cuda.current_stream()
-    N.check(N.lib().acb_scan_device(tb, d_hay.data_ptr(), t.size, d_off.data_ptr(), len(off) - 1, 0,
-                                    d_out.data_ptr() if c else None, c, d_cnt.data_ptr(), stream.cuda_stream, algo))
+    _write(kernel, A, algo, first, t, off, d_out, c, d_cnt, stream)
     stream.synchronize()
     out = d_out.cpu().numpy()
     assert (out[c:] == -1).all(), f"{int((out[c:] != -1).any(axis=1).sum())} guard rows written"

@@ -304,18 +304,20 @@ def test_c_abi_refuses_a_table_of_another_key_set():
         lib.acb_streams_free(ss)
 
 
-def _overflow(device_route):
-    """caps 0, 1, n-1, n, n+1 with seam records at the boundary: exact count, no stream advanced; the retry gives what a
-    twin batch fed with room gives"""
+def _overflow(device_route, long_mode=0):
+    """caps 0, 1, n-1, n, n+1 with records of keys that began in the chunk before (long_mode: streams that enter the
+    feed inside a key, in a non-root state): exact count, no stream advanced; the retry gives what a twin batch fed with
+    room gives, and so does every later feed"""
     import torch
     rng = np.random.default_rng(77)
+    key_len = np.array([2, 2, 3, 1])
     A, _ = _automaton("bytes", [tuple(b"ab"), tuple(b"ba"), tuple(b"aba"), tuple(b"b")])
     lib, tb = _c(A)
     n_streams, stride = 64, 32
     feeds = [rng.choice(np.frombuffer(b"ab", dtype=np.uint8), size=(n_streams, stride)) for _ in range(3)]
     twin, ss = ctypes.c_void_p(), ctypes.c_void_p()
-    N.check(lib.acb_streams_new(tb, n_streams, 0, ctypes.byref(twin)))
-    N.check(lib.acb_streams_new(tb, n_streams, 0, ctypes.byref(ss)))
+    N.check(lib.acb_streams_new(tb, n_streams, long_mode, ctypes.byref(twin)))
+    N.check(lib.acb_streams_new(tb, n_streams, long_mode, ctypes.byref(ss)))
 
     def feed(h, batch, cap):
         if device_route:
@@ -346,8 +348,8 @@ def _overflow(device_route):
     try:
         for k, batch in enumerate(feeds):
             n, want = feed(twin, batch, 1 << 16)
-            if k:                                               # seam records: a two-letter key ending on a chunk's first letter
-                assert np.any((want[:, 1] == 0) & (want[:, 2] != 3))
+            if k:                                               # records of keys that began in the chunk before
+                assert np.any(want[:, 1] - key_len[want[:, 2]] + 1 < 0)
             for cap in (0, 1, n - 1):
                 got_n, got = feed(ss, batch, cap)
                 assert (got_n, got) == (n, None)
@@ -368,6 +370,16 @@ def test_overflow_commits_nothing_host_gpu():
 @pytest.mark.gpu
 def test_overflow_commits_nothing_device_gpu():
     _overflow(True)
+
+
+@pytest.mark.gpu
+def test_overflow_commits_nothing_long_host_gpu():
+    _overflow(False, long_mode=1)
+
+
+@pytest.mark.gpu
+def test_overflow_commits_nothing_long_device_gpu():
+    _overflow(True, long_mode=1)
 
 
 @pytest.mark.gpu
