@@ -310,6 +310,50 @@ int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks,
 /* letters consumed by every stream since its start or its last reset (cap >= n_streams).  Synchronises the device. */
 int acb_streams_positions(acb_streams *ss, int64_t *out, int64_t cap);
 
+/* ---- white space: iter(..., ignore_white_space=1) for a whole batch (src/AutomatonSearchIter.c:270-274) ------------
+ * A skip set is a sorted array of distinct letter values, exactly as the letters are stored in the buffer (1-, 2- or
+ * 4-byte little-endian values of the table's width; a unicode-flavour latin-1 table has 1-byte letters), at most
+ * ACB_MAX_SKIP long.  The skip scans behave as if every letter of the set were removed from each haystack before the
+ * scan, and report end_index in letters of the ORIGINAL haystack: the batch is compacted on the device, scanned by
+ * the ordinary kernels, and each stored record is mapped back.  ACB_EINVAL for ACB_ALGO_LONG (iter_long has no such
+ * option), an unsorted or too large set.  Records beyond cap are counted exactly, as by the plain scans. */
+#define ACB_MAX_SKIP 1024
+
+/* Every letter of the given width for which libc iswspace() is true under the current LC_CTYPE, in ascending order:
+ * letter_bytes 1 (with signed_bytes != 0 the predicate sees the byte widened through a signed char, as the reference's
+ * bytes build does; out receives the byte values), 2 (all 65 536 values) or 4 (0 .. 0x10FFFF).  *n is always set;
+ * ACB_EOVERFLOW when cap is smaller.  Host only, no device needed. */
+int acb_space_letters(int letter_bytes, int signed_bytes, uint32_t *out, int64_t cap, int64_t *n);
+
+/* acb_scan_device with a skip set (host array).  Zeroes *d_count itself.  Asynchronous on `stream` except that it
+ * waits once for the compaction, to learn the compacted size the scan kernels are launched for.  d_out holds the
+ * records in ORIGINAL coordinates once the stream reaches them.  The compacted batch and the map back live in a
+ * workspace of the table, reused by every skip call and skip feed on it: the next such call, on any CUDA stream, first
+ * waits (cudaStreamWaitEvent) for the work of this one that still reads it.  As for acb_scan_device, one scan at a time
+ * per table. */
+int acb_scan_device_skip(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
+                         const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
+                         acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo,
+                         const uint32_t *skip, int64_t n_skip);
+
+/* acb_scan_host with a skip set: upload, compact, scan, map back, sort, copy back in one call (no pipeline).
+ * out == NULL works as for acb_scan_host (acb_copy_records / acb_take_records). */
+int acb_scan_host_skip(acb_table *tb, const uint8_t *hay, int64_t total_bytes,
+                       const int64_t *offsets, int64_t n_hay, int64_t stride_bytes,
+                       acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort,
+                       const uint32_t *skip, int64_t n_skip);
+
+/* A find_all stream batch whose feeds skip the letters of `skip` (copied): stream s reports what iter(c0,
+ * ignore_white_space=1) ... .set(c1) ... reports.  Positions (acb_streams_positions, end_index) count ORIGINAL letters;
+ * the tail carried to the next chunk holds the last T kept letters, so a key that white space splits across a chunk
+ * boundary is found.  acb_streams_feed_*, _reset and _positions serve it unchanged. */
+int acb_streams_new_skip(const acb_table *tb, int64_t n_streams, const uint32_t *skip, int64_t n_skip, acb_streams **out);
+
+/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the compaction kernel and of the map-back kernel
+ * of the last skip scan or skip feed on this thread, from CUDA events around each launch (the call then waits for
+ * them); 0 when timing is off or the call launched none.  acb_last_kernel_ms() gives its scan kernel. */
+int acb_last_skip_ms(float *compact_ms, float *remap_ms);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

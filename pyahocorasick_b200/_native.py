@@ -14,6 +14,7 @@ ABI_VERSION = 5            # ACB_ABI_VERSION of include/acb200.h this binding wa
 ACB_OK, ACB_ENOMEM, ACB_EINVAL, ACB_ESTATE, ACB_ECUDA, ACB_EOVERFLOW, ACB_ERANGE = 0, -1, -2, -3, -4, -5, -6
 ALGO_AUTO, ALGO_FILTER, ALGO_DFA, ALGO_LONG = 0, 1, 2, 3
 ALGOS = {"auto": ALGO_AUTO, "filter": ALGO_FILTER, "dfa": ALGO_DFA, "long": ALGO_LONG}
+MAX_SKIP = 1024            # ACB_MAX_SKIP: largest skip set of the white-space scans
 
 MATCH_DTYPE = np.dtype([("hay_id", "<i4"), ("end_index", "<i4"), ("key_id", "<i4")])
 
@@ -96,6 +97,11 @@ def lib() -> ctypes.CDLL:
         "acb_streams_feed_device": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, vp, i64, vp, vp, ctypes.c_int]),
         "acb_streams_feed_host": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, vp, i64, pi64, ctypes.c_int, ctypes.c_int]),
         "acb_streams_positions": (ctypes.c_int, [vp, vp, i64]),
+        "acb_space_letters": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, vp, i64, pi64]),
+        "acb_scan_device_skip": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, i64, vp, vp, ctypes.c_int, vp, i64]),
+        "acb_scan_host_skip": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, i64, pi64, ctypes.c_int, ctypes.c_int, vp, i64]),
+        "acb_streams_new_skip": (ctypes.c_int, [vp, i64, vp, i64, ctypes.POINTER(vp)]),
+        "acb_last_skip_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]),
         "acb_launch_count": (i64, []),
         "acb_set_kernel_timing": (ctypes.c_int, [ctypes.c_int]),
         "acb_last_kernel_ms": (ctypes.c_float, []),
@@ -122,7 +128,8 @@ EXPORTED_SYMBOLS = [
     "acb_device_count", "acb_table_upload", "acb_table_free", "acb_table_device_bytes",
     "acb_scan_device", "acb_scan_host", "acb_copy_records", "acb_take_records", "acb_release_records", "acb_sort_matches_device", "acb_table_set_long_state", "acb_table_get_long_state",
     "acb_streams_new", "acb_streams_free", "acb_streams_reset", "acb_streams_feed_device", "acb_streams_feed_host",
-    "acb_streams_positions", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_streams_positions", "acb_space_letters", "acb_scan_device_skip", "acb_scan_host_skip", "acb_streams_new_skip",
+    "acb_last_skip_ms", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

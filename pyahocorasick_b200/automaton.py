@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import ctypes
 import functools
+import locale
 import os
 import operator
 import pickle
@@ -59,9 +60,29 @@ def _parse_c_int(x, name="an integer"):
     return v
 
 
-_libc = ctypes.CDLL(None)
-_libc.iswspace.argtypes = [ctypes.c_uint]
-_libc.iswspace.restype = ctypes.c_int
+_SPACE_SETS: dict = {}
+
+
+def _space_letters(letter_bytes: int, signed_bytes: bool) -> np.ndarray:
+    """The package's one definition of white space: every letter value of the given width (as stored) for which libc
+    iswspace() is true under the current LC_CTYPE (acb_space_letters), sorted -- the skip set of the white-space scans.
+    signed_bytes: 1-byte letters are widened through a signed char first, as the reference's bytes build does
+    (src/utils.c:199-202).  Cached per width, signedness and locale."""
+    key = (letter_bytes, bool(signed_bytes), locale.setlocale(locale.LC_CTYPE))
+    s = _SPACE_SETS.get(key)
+    if s is None:
+        lib, n, cap = N.lib(), ctypes.c_int64(0), 64
+        while True:
+            out = np.empty(cap, dtype=np.uint32)
+            rc = lib.acb_space_letters(letter_bytes, int(bool(signed_bytes)), N.ptr(out), cap, ctypes.byref(n))
+            if rc != N.ACB_EOVERFLOW:
+                break
+            cap = int(n.value)
+        N.check(rc)
+        s = out[:n.value].copy()
+        s.flags.writeable = False
+        _SPACE_SETS[key] = s
+    return s
 
 
 def _space_mask(letters: np.ndarray, bytes_flavour: bool) -> np.ndarray:
@@ -69,12 +90,8 @@ def _space_mask(letters: np.ndarray, bytes_flavour: bool) -> np.ndarray:
     The bytes flavour widens through a signed char first (src/utils.c:199-202)."""
     if letters.size == 0:
         return np.zeros(0, dtype=bool)
-    vals = letters.astype(np.uint32)
-    if bytes_flavour and letters.dtype == np.uint8:
-        vals = letters.astype(np.int8).astype(np.int16).astype(np.uint16).astype(np.uint32)
-    uniq = np.unique(vals)
-    spaces = np.array([u for u in uniq.tolist() if _libc.iswspace(u)], dtype=np.uint32)
-    return np.isin(vals, spaces)
+    w = letters.dtype.itemsize
+    return np.isin(letters, _space_letters(w, bytes_flavour and w == 1))
 
 
 class _PinnedRecords:
@@ -694,13 +711,7 @@ class Automaton:
                 self._long_state_out = int(st.value)
             if not found.value:
                 return np.empty(0, dtype=N.MATCH_DTYPE)
-            # no copy: the records stay in the pinned buffer the D2H landed in; it returns to the library's pool
-            # when the last array that views it is gone (_PinnedRecords.__del__)
-            ptr, n, room = ctypes.c_void_p(), ctypes.c_int64(0), ctypes.c_int64(0)
-            N.check(self._lib.acb_take_records(tb, ctypes.byref(ptr), ctypes.byref(n), ctypes.byref(room)))
-            if not ptr.value or n.value != found.value:
-                raise N.NativeError("acb_take_records: no records to take")
-            return np.asarray(_PinnedRecords(self._lib, ptr.value, n.value, room.value))
+            return _take_records(self._lib, tb, found.value)
 
     @_locked
     def _scan_device_tensor(self, t, algo: str, sort: bool) -> np.ndarray:
@@ -727,20 +738,84 @@ class Automaton:
                     cap = self._match_cap = found + 1024
                     continue
                 break
-            if sort and found > 1:
-                rc = self._lib.acb_sort_matches_device(tb, out.data_ptr(), found, n, stride // self._L, stream)
-                if rc == N.ACB_ERANGE:
-                    sort_on_host = True
-                else:
-                    N.check(rc)
-                    sort_on_host = False
+            return self._device_records(tb, out, found, n, stride // self._L, stream, sort)
+
+    def _device_records(self, tb, out, found: int, n_hay: int, max_letters: int, stream, sort: bool) -> np.ndarray:
+        """The first `found` records of the device buffer `out`, sorted on the device (on the host when the sort key
+        does not fit 64 bits), as numpy records."""
+        sort_on_host = False
+        if sort and found > 1:
+            rc = self._lib.acb_sort_matches_device(tb, out.data_ptr(), found, n_hay, max_letters, stream)
+            if rc == N.ACB_ERANGE:
+                sort_on_host = True
             else:
-                sort_on_host = False
-            rec = out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
+                N.check(rc)
+        rec = out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
         if sort_on_host:
             kl = np.asarray(self.flat()["key_len"])
             rec = rec[np.lexsort((-kl[rec["key_id"]], rec["end_index"], rec["hay_id"]))]
         return rec
+
+    def _skip_set(self, narrow: bool) -> np.ndarray:
+        """The white-space letters of a batch, as its buffer stores them: 1-byte letters of a latin-1 batch (unicode
+        flavour) or of the bytes flavour (widened through a signed char), 2-byte items of bytes-flavour sequences,
+        4-byte letters otherwise."""
+        if narrow:
+            return _space_letters(1, False)
+        return _space_letters(self._L, not self._UNICODE and self._key_type == KEY_STRING)
+
+    @_locked
+    def _scan_skip(self, batch, algo: str, sort: bool, device: Optional[int]) -> np.ndarray:
+        """Every scan with ignore_white_space: `batch` as _batch_input lays it out -> records in original letters.
+        The white space is removed on the GPU (acb_scan_host_skip / acb_scan_device_skip)."""
+        lib = self._lib
+        if batch[0] == "device":
+            import torch
+            t = batch[1]
+            n, stride = self._device_batch_shape(t)
+            if n == 0 or stride == 0:
+                return np.empty(0, dtype=N.MATCH_DTYPE)
+            t = _aligned(t)
+            dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+            tb = self._ensure_table(dev)
+            skip = self._skip_set(False)
+            with torch.cuda.device(dev):
+                stream = torch.cuda.current_stream().cuda_stream
+                cnt = torch.empty(1, dtype=torch.int64, device=t.device)
+                cap = max(self._match_cap, 1 << 12, 2 * n)
+                while True:
+                    out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+                    N.check(lib.acb_scan_device_skip(tb, t.data_ptr(), n * stride, None, n, stride, out.data_ptr(), cap,
+                                                     cnt.data_ptr(), stream, N.ALGOS[algo], N.ptr(skip), len(skip)))
+                    found = int(cnt.item())
+                    if found > cap:
+                        cap = self._match_cap = found + 1024
+                        continue
+                    break
+                return self._device_records(tb, out, found, n, stride // self._L, stream, sort)
+        _, flat, offs, n, stride, narrow = batch
+        if not (n and flat.size):
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        if narrow:
+            core = self._ensure_narrow(device)
+            if core is None:
+                return np.empty(0, dtype=N.MATCH_DTYPE)
+            tb = core[1]
+        else:
+            tb = self._ensure_table(device)
+        skip = self._skip_set(narrow)
+        cap = max(self._match_cap, 1 << 12, 2 * n)
+        found = ctypes.c_int64(0)
+        while True:
+            rc = lib.acb_scan_host_skip(tb, N.ptr(flat), int(flat.size), N.ptr(offs) if offs is not None else None, n, stride,
+                                        None, cap, ctypes.byref(found), N.ALGOS[algo], int(sort), N.ptr(skip), len(skip))
+            if rc != N.ACB_EOVERFLOW:
+                break
+            cap = self._match_cap = int(found.value) + 1024
+        N.check(rc)
+        if not found.value:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        return _take_records(lib, tb, found.value)
 
     def _device_batch_shape(self, t):
         """(n, stride_bytes) of a device batch: a C-contiguous uint8 torch CUDA tensor [n, stride]"""
@@ -851,7 +926,8 @@ class Automaton:
         return nodes, edges, fail
 
     # ------------------------------------------------------------------ the batch entry (new)
-    def find_all_batch(self, haystacks, *, algo: str = "auto", sort: bool = True, device: Optional[int] = None) -> Matches:
+    def find_all_batch(self, haystacks, *, algo: str = "auto", sort: bool = True, device: Optional[int] = None,
+                       ignore_white_space: bool = False) -> Matches:
         """Search a whole batch on the GPU.
 
         haystacks: a sequence of bytes / str / tuple objects (as `iter` accepts), or a 2-D
@@ -860,10 +936,16 @@ class Automaton:
         tensor [n, stride] that already lives in HBM (no host copy of the batch).
 
         Equivalent to ``[(h, e, v) for h, hay in enumerate(haystacks) for e, v in A.iter(hay)]``
-        of the reference, returned as arrays.
+        of the reference, returned as arrays.  ignore_white_space=True: to ``A.iter(hay, ignore_white_space=True)``
+        -- letters for which libc iswspace() is true are skipped (removed on the GPU before the scan) and end_index
+        still counts the letters of the original haystack.
         """
         self._require_automaton()
+        if ignore_white_space and algo == "long":
+            raise ValueError("iter_long has no ignore_white_space option")
         batch = self._batch_input(haystacks, narrow_ok=algo != "long")
+        if ignore_white_space:
+            return Matches(self._scan_skip(batch, algo, sort, device), self._values)
         if batch[0] == "device":
             return Matches(self._scan_device_tensor(batch[1], algo, sort), self._values)
         _, flat, offs, n, stride, narrow = batch
@@ -917,11 +999,13 @@ class Automaton:
         return ("host", flat, offs, n, 0, narrow)
 
     def stream_batch(self, n_streams: int, *, long: bool = False, algo: str = "auto",
-                     device: Optional[int] = None) -> "StreamBatch":
+                     device: Optional[int] = None, ignore_white_space: bool = False) -> "StreamBatch":
         """`n_streams` independent streams searched chunk by chunk, the next chunk of many of them in one GPU call
         (StreamBatch.feed).  long=False: stream s reports what the reference's ``iter(c0)`` ... ``.set(c1)`` ...
         reports over its chunks -- every match, also those across chunk boundaries; long=True: what
         ``iter_long(c0)`` ... ``.set(c1)`` reports.  What a stream carries from one chunk to the next stays in HBM.
+        ignore_white_space=True (find_all batches only): what ``iter(c0, ignore_white_space=True)`` ... ``.set(c1)``
+        ... reports; positions still count every letter, and a key that white space splits across chunks is found.
 
         Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
         wider chunks, so the latin-1 automaton is not used)."""
@@ -933,7 +1017,10 @@ class Automaton:
             raise ValueError("n_streams must not be negative")
         if algo not in (("auto", "long") if long else ("auto", "filter", "dfa")):
             raise ValueError(f"algo {algo!r} does not fit a {'long' if long else 'find_all'} stream batch")
-        return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device)
+        if long and ignore_white_space:
+            raise ValueError("iter_long has no ignore_white_space option")
+        skip = self._skip_set(False) if ignore_white_space else None
+        return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip)
 
 
 class StreamBatch:
@@ -946,7 +1033,7 @@ class StreamBatch:
     every stream has consumed.  A stream batch belongs to the key set it was made for: after the key set changes,
     `feed` and `reset` raise ValueError as a stale iterator does."""
 
-    def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int):
+    def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None):
         self._A = A
         self._version = A._version
         self.n_streams = n_streams
@@ -954,8 +1041,9 @@ class StreamBatch:
         self._algo = algo
         self._device = device
         self._pos = np.zeros(n_streams, dtype=np.int64)        # host mirror of the positions, for end_index
+        self.ignore_white_space = skip is not None
         with A._gpu_lock:
-            self._ss = self._native("new")
+            self._ss = self._native("new") if skip is None else self._native("new_skip", skip)
 
     def __del__(self):
         try:
@@ -971,13 +1059,18 @@ class StreamBatch:
 
     def _native(self, op: str, *args):
         """Every call into the native stream batch (acb_streams_*) goes through here.
-          new -> handle;  free;  reset(ids int32 or None);  positions -> int64[n_streams];
+          new -> handle;  new_skip(skip set uint32) -> handle of a batch that skips those letters;  free;  reset(ids int32 or None);  positions -> int64[n_streams];
           feed(kind, data, offsets, n, stride, ids, sort) -> records (hay_id = chunk index, end_index in the chunk)"""
         A = self._A
         lib = A._lib
         if op == "new":
             ss = ctypes.c_void_p()
             N.check(lib.acb_streams_new(A._ensure_table(self._device), self.n_streams, int(self.long), ctypes.byref(ss)))
+            return ss
+        if op == "new_skip":
+            skip, = args
+            ss = ctypes.c_void_p()
+            N.check(lib.acb_streams_new_skip(A._ensure_table(self._device), self.n_streams, N.ptr(skip), len(skip), ctypes.byref(ss)))
             return ss
         if op == "free":
             lib.acb_streams_free(self._ss)
@@ -1009,11 +1102,7 @@ class StreamBatch:
             break
         if not found.value:
             return np.empty(0, dtype=N.MATCH_DTYPE)
-        ptr, got, room = ctypes.c_void_p(), ctypes.c_int64(0), ctypes.c_int64(0)
-        N.check(lib.acb_take_records(tb, ctypes.byref(ptr), ctypes.byref(got), ctypes.byref(room)))
-        if not ptr.value or got.value != found.value:
-            raise N.NativeError("acb_take_records: no records to take")
-        return np.asarray(_PinnedRecords(lib, ptr.value, got.value, room.value))
+        return _take_records(lib, tb, found.value)
 
     def _feed_device(self, t, ids, sort, algo):
         import torch
@@ -1040,18 +1129,7 @@ class StreamBatch:
                     cap = A._match_cap = found + 1024
                     continue
                 break
-            sort_on_host = False
-            if sort and found > 1:
-                rc = A._lib.acb_sort_matches_device(tb, out.data_ptr(), found, n, stride // A._L, stream)
-                if rc == N.ACB_ERANGE:
-                    sort_on_host = True
-                else:
-                    N.check(rc)
-            rec = out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
-        if sort_on_host:
-            kl = np.asarray(A.flat()["key_len"])
-            rec = rec[np.lexsort((-kl[rec["key_id"]], rec["end_index"], rec["hay_id"]))]
-        return rec
+            return A._device_records(tb, out, found, n, stride // A._L, stream, sort)
 
     def _ids(self, ids, n: int) -> Optional[np.ndarray]:
         if ids is None:
@@ -1314,6 +1392,16 @@ def _parse_start_end(args, i_start, i_end, lo, hi):
     if end < lo or end > hi:
         raise IndexError(f"end index not in range {lo}..{hi}")
     return start, end
+
+
+def _take_records(lib, tb, found: int) -> np.ndarray:
+    """The records of the last host-buffer call on `tb`, without a copy: they stay in the pinned buffer the D2H landed
+    in, which returns to the library's pool when the last array that views it is gone (_PinnedRecords.__del__)."""
+    ptr, n, room = ctypes.c_void_p(), ctypes.c_int64(0), ctypes.c_int64(0)
+    N.check(lib.acb_take_records(tb, ctypes.byref(ptr), ctypes.byref(n), ctypes.byref(room)))
+    if not ptr.value or n.value != found:
+        raise N.NativeError("acb_take_records: no records to take")
+    return np.asarray(_PinnedRecords(lib, ptr.value, n.value, room.value))
 
 
 def _aligned(t):

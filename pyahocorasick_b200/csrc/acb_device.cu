@@ -102,6 +102,7 @@ enum { kModeNarrow = 0, kModeWide = 1 };                  /* how a SINGLE gram i
 
 std::atomic<long long> g_launches{0};
 thread_local float g_last_ms = 0.f;
+thread_local float g_compact_ms = 0.f, g_remap_ms = 0.f;   /* kernel timing of the last white-space scan */
 std::atomic<int> g_timing{0};
 
 struct ScanParams {
@@ -1291,6 +1292,18 @@ struct acb_table {
     acb_match *h_out = nullptr; size_t h_out_cap = 0;   /* pinned staging for the records */
     unsigned long long h_out_n = 0;                      /* records of the last scan held in h_out */
     void *d_sort = nullptr; size_t sort_cap = 0;         /* radix-sort scratch */
+    /* workspace of the white-space scans (acb_scan_*_skip, stream batches with a skip set) */
+    uint8_t *k_buf = nullptr; size_t k_buf_cap = 0;      /* the compacted letters */
+    uint32_t *k_mask = nullptr; size_t k_mask_cap = 0;   /* keep bit per letter, one word per 32-letter group */
+    uint16_t *k_gpre = nullptr; size_t k_gpre_cap = 0;   /* kept letters before the group, within its tile */
+    long long *k_tile_pre = nullptr; size_t k_tile_pre_cap = 0;   /* kept letters before the tile; [n_tiles] = all */
+    unsigned long long *k_status = nullptr; size_t k_status_cap = 0;   /* decoupled look-back */
+    long long *k_coff = nullptr; size_t k_coff_cap = 0;  /* compacted byte offsets of the haystacks */
+    uint32_t *k_set = nullptr;                           /* the skip set (ACB_MAX_SKIP) */
+    unsigned int *k_ctr = nullptr;                       /* tile counter of the compaction */
+    long long *h_kept = nullptr;                         /* pinned: kept letters of the last compaction */
+    cudaEvent_t k_done = nullptr;                        /* the last skip call's work that reads k_* has been issued before it */
+    cudaEvent_t k_t0 = nullptr, k_t1 = nullptr;          /* kernel timing of the compaction and the remap */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1328,6 +1341,12 @@ extern "C" void acb_table_free(acb_table *tb) {
     for (cudaEvent_t e : tb->ev_h2d) cudaEventDestroy(e);
     for (cudaEvent_t e : tb->ev_scan) cudaEventDestroy(e);
     if (tb->h_counts) cudaFreeHost(tb->h_counts);
+    cudaFree(tb->k_buf); cudaFree(tb->k_mask); cudaFree(tb->k_gpre); cudaFree(tb->k_tile_pre); cudaFree(tb->k_status);
+    cudaFree(tb->k_coff); cudaFree(tb->k_set); cudaFree(tb->k_ctr);
+    if (tb->h_kept) cudaFreeHost(tb->h_kept);
+    if (tb->k_done) cudaEventDestroy(tb->k_done);
+    if (tb->k_t0) cudaEventDestroy(tb->k_t0);
+    if (tb->k_t1) cudaEventDestroy(tb->k_t1);
     delete tb;
 }
 
@@ -1920,6 +1939,357 @@ extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_by
     return ACB_OK;
 }
 
+/* ------------------------------------------------------------ white space */
+/* iter(..., ignore_white_space=1) for a batch: compact, scan, map back.  acb_compact_kernel drops the letters of the
+ * skip set from the flat buffer in one pass (tile ids from a counter, decoupled look-back over per-tile kept counts,
+ * kept letters staged in shared memory so the stores are coalesced) and leaves what the map back needs: one keep mask
+ * per 32-letter group, a uint16 prefix per group within its tile and an int64 prefix per tile -- 6 bytes per 32 letters
+ * plus 16 per tile, never the text again.  The ordinary scan kernels then run on the compacted haystacks unchanged;
+ * acb_remap_kernel turns a record's compacted letter into the original one with a binary search over tiles, one over
+ * the tile's groups and __fns on one mask. */
+namespace {
+constexpr int kCmpThreads = 256;                          /* one 32-letter group per thread */
+constexpr int kCmpTile = kCmpThreads * 32;                /* letters per tile (uint16 prefixes within a tile) */
+constexpr unsigned long long kLbAgg = 1ULL << 62, kLbPre = 2ULL << 62, kLbVal = (1ULL << 62) - 1;
+
+struct CompactMeta {
+    const uint32_t *mask;
+    const uint16_t *gpre;
+    const long long *tile_pre;    /* [n_tiles + 1] */
+    long long n_tiles;
+};
+
+struct CompactParams {
+    const uint8_t *in;
+    uint8_t *out;                 /* 16-byte aligned */
+    long long n_letters;
+    uint32_t *mask;
+    uint16_t *gpre;
+    long long *tile_pre;
+    unsigned long long *status;   /* [n_tiles], zeroed */
+    unsigned int *ctr;            /* zeroed */
+    long long n_tiles;
+    const uint32_t *set;          /* L > 1: the sorted skip set */
+    int n_set;
+    uint32_t bits[8];             /* L == 1: the skip set as a 256-bit table */
+};
+
+template <typename T>
+__device__ __forceinline__ bool skip_letter(T v, const uint32_t *bits, const uint32_t *set, int n) {
+    if (sizeof(T) == 1) return (bits[v >> 5] >> (v & 31)) & 1;
+    int lo = 0, hi = n;                                    /* the set is short: a binary search in shared memory */
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (set[mid] < (uint32_t)v) lo = mid + 1; else hi = mid;
+    }
+    return lo < n && set[lo] == (uint32_t)v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kCmpThreads, 4) acb_compact_kernel(const __grid_constant__ CompactParams p) {
+    using Scan = cub::BlockScan<int, kCmpThreads>;
+    __shared__ typename Scan::TempStorage scan_tmp;
+    __shared__ __align__(16) uint8_t s_buf[kCmpTile * sizeof(T) + 16];   /* the tile's kept letters */
+    __shared__ uint32_t s_set[sizeof(T) == 1 ? 1 : ACB_MAX_SKIP];
+    __shared__ uint32_t s_bits[8];
+    __shared__ long long s_tile, s_base;
+    if (threadIdx.x == 0) s_tile = atomicAdd(p.ctr, 1u);   /* in claim order: every earlier tile is running or done */
+    if (sizeof(T) == 1) { if (threadIdx.x < 8) s_bits[threadIdx.x] = p.bits[threadIdx.x]; }
+    else for (int i = threadIdx.x; i < p.n_set; i += kCmpThreads) s_set[i] = __ldg(p.set + i);
+    __syncthreads();
+    const long long tile = s_tile, t0 = tile * kCmpTile;
+    const int n_tile = (int)min((long long)kCmpTile, p.n_letters - t0);
+    constexpr int kWords = 8 * (int)sizeof(T), kPer = 4 / (int)sizeof(T);
+    uint32_t w[kWords];                                    /* this thread's 32 letters, straight into registers */
+    const long long first = t0 + (long long)threadIdx.x * 32;
+    if (first + 32 <= p.n_letters) {                       /* 32 * sizeof(T) bytes at a 32-byte aligned offset, read once */
+        const uint4 *src = reinterpret_cast<const uint4 *>(p.in + first * (long long)sizeof(T));
+#pragma unroll
+        for (int k = 0; k < kWords / 4; k++) {
+            const uint4 v = __ldcs(src + k);
+            w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+        }
+    } else {
+        const T *src = reinterpret_cast<const T *>(p.in);
+#pragma unroll
+        for (int k = 0; k < kWords; k++) w[k] = 0;
+#pragma unroll
+        for (int j = 0; j < 32; j++)
+            if (first + j < p.n_letters) w[j / kPer] |= (uint32_t)src[first + j] << (8 * (int)sizeof(T) * (j % kPer));
+    }
+    const int valid = n_tile - (int)threadIdx.x * 32;      /* letters of this group inside the batch */
+    uint32_t keep = 0;
+#pragma unroll
+    for (int j = 0; j < 32; j++) {
+        const T v = (T)(w[j / kPer] >> (8 * (int)sizeof(T) * (j % kPer)));
+        if (j < valid && !skip_letter<T>(v, s_bits, s_set, p.n_set)) keep |= 1u << j;
+    }
+    int pre, agg;
+    Scan(scan_tmp).ExclusiveSum(__popc(keep), pre, agg);
+    const long long g = tile * kCmpThreads + threadIdx.x;
+    p.mask[g] = keep;
+    p.gpre[g] = (uint16_t)pre;
+    T *kept = reinterpret_cast<T *>(s_buf);
+    int o = pre;
+#pragma unroll
+    for (int j = 0; j < 32; j++)
+        if ((keep >> j) & 1) kept[o++] = (T)(w[j / kPer] >> (8 * (int)sizeof(T) * (j % kPer)));
+    if (threadIdx.x == 0) {                                /* decoupled look-back over the tiles before this one */
+        long long base = 0;
+        if (tile == 0) {
+            atomicExch(p.status, kLbPre | (unsigned long long)agg);
+        } else {
+            atomicExch(p.status + tile, kLbAgg | (unsigned long long)agg);
+            for (long long i = tile - 1;; --i) {
+                unsigned long long st;
+                while ((st = *reinterpret_cast<volatile unsigned long long *>(p.status + i)) == 0) {}
+                base += (long long)(st & kLbVal);
+                if (st & kLbPre) break;
+            }
+            atomicExch(p.status + tile, kLbPre | (unsigned long long)(base + agg));
+        }
+        p.tile_pre[tile] = base;
+        if (tile == p.n_tiles - 1) p.tile_pre[p.n_tiles] = base + agg;
+        s_base = base;
+    }
+    __syncthreads();
+    /* coalesced stores: bytes up to a 16-byte boundary of the destination, then 16-byte words, then the rest */
+    uint8_t *dst = p.out + s_base * (long long)sizeof(T);
+    const int nb = agg * (int)sizeof(T);
+    const int head = min(nb, (int)((16 - (reinterpret_cast<uintptr_t>(dst) & 15)) & 15)), nmid = (nb - head) >> 4;
+    if ((int)threadIdx.x < head) dst[threadIdx.x] = s_buf[threadIdx.x];
+    const int sh = (head & 3) * 8;
+    const uint32_t *sw = reinterpret_cast<const uint32_t *>(s_buf) + (head >> 2);
+    for (int i = threadIdx.x; i < nmid; i += kCmpThreads) {
+        const uint32_t *q = sw + 4 * i;                    /* unaligned by head bytes in shared memory: funnel shifts */
+        const uint32_t a0 = q[0], a1 = q[1], a2 = q[2], a3 = q[3], a4 = q[4];
+        reinterpret_cast<uint4 *>(dst + head)[i] = make_uint4(__funnelshift_r(a0, a1, sh), __funnelshift_r(a1, a2, sh),
+                                                              __funnelshift_r(a2, a3, sh), __funnelshift_r(a3, a4, sh));
+    }
+    for (int i = head + (nmid << 4) + threadIdx.x; i < nb; i += kCmpThreads) dst[i] = s_buf[i];
+}
+
+/* kept letters before letter q of the original buffer */
+__device__ __forceinline__ long long kept_before(const CompactMeta &m, long long q) {
+    const long long t = q / kCmpTile;
+    if (t >= m.n_tiles) return __ldg(m.tile_pre + m.n_tiles);
+    const long long g = q >> 5;
+    return __ldg(m.tile_pre + t) + __ldg(m.gpre + g) + __popc(__ldg(m.mask + g) & ((1u << (q & 31)) - 1u));
+}
+
+/* coff[h] = compacted byte offset of haystack h, h = 0 .. n_hay */
+__global__ void acb_compact_offsets_kernel(const CompactMeta m, const long long *off, long long stride, long long n_hay, int ls,
+                                           long long *coff) {
+    const long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h > n_hay) return;
+    const long long q = (off ? __ldg(off + h) : h * stride) >> ls;
+    coff[h] = kept_before(m, q) << ls;
+}
+
+/* the stored records (min(*count, cap)) from compacted letters of their haystack to original ones */
+__global__ void acb_remap_kernel(const CompactMeta m, const long long *coff, const long long *off, long long stride, int ls,
+                                 acb_match *rec, const unsigned long long *count, long long cap) {
+    const long long n = (long long)min(*count, (unsigned long long)cap);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        acb_match r = rec[i];
+        const long long k = (__ldg(coff + r.hay_id) >> ls) + r.end_index;     /* rank of the kept letter */
+        long long lo = 0, hi = m.n_tiles;                  /* the last tile with tile_pre <= k holds it */
+        while (hi - lo > 1) { const long long mid = (lo + hi) >> 1; if (__ldg(m.tile_pre + mid) <= k) lo = mid; else hi = mid; }
+        const long long kt = k - __ldg(m.tile_pre + lo);
+        int a = 0, b = kCmpThreads;                        /* ... and its last group with gpre <= kt */
+        const uint16_t *gp = m.gpre + lo * kCmpThreads;
+        while (b - a > 1) { const int mid = (a + b) >> 1; if ((long long)__ldg(gp + mid) <= kt) a = mid; else b = mid; }
+        const long long g = lo * kCmpThreads + a;
+        const int bit = (int)__fns(__ldg(m.mask + g), 0, (int)(kt - __ldg(gp + a)) + 1);
+        const long long hs = (off ? __ldg(off + r.hay_id) : (long long)r.hay_id * stride) >> ls;
+        r.end_index = (int32_t)(g * 32 + bit - hs);
+        rec[i] = r;
+    }
+}
+} // namespace
+
+/* kernel timing (acb_set_kernel_timing): events around one launch, waited for; *ms = 0 when timing is off */
+static int skip_timing_begin(acb_table *tb, cudaStream_t s) {
+    if (!g_timing.load()) return ACB_OK;
+    if (!tb->k_t0) { CUDA_TRY(cudaEventCreate(&tb->k_t0)); CUDA_TRY(cudaEventCreate(&tb->k_t1)); }
+    CUDA_TRY(cudaEventRecord(tb->k_t0, s));
+    return ACB_OK;
+}
+static int skip_timing_end(acb_table *tb, cudaStream_t s, float *ms) {
+    *ms = 0.f;
+    if (!g_timing.load()) return ACB_OK;
+    CUDA_TRY(cudaEventRecord(tb->k_t1, s));
+    CUDA_TRY(cudaEventSynchronize(tb->k_t1));
+    CUDA_TRY(cudaEventElapsedTime(ms, tb->k_t0, tb->k_t1));
+    return ACB_OK;
+}
+
+/* the work of the last skip call that reads the table's k_* workspace (remap, stream commit) is issued; a later skip
+ * call, on any CUDA stream, waits for it before it overwrites that workspace */
+static int skip_work_issued(acb_table *tb, cudaStream_t s) {
+    if (!tb->k_done) CUDA_TRY(cudaEventCreateWithFlags(&tb->k_done, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventRecord(tb->k_done, s));
+    return ACB_OK;
+}
+
+extern "C" int acb_last_skip_ms(float *compact_ms, float *remap_ms) {
+    if (!compact_ms || !remap_ms) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *compact_ms = g_compact_ms;
+    *remap_ms = g_remap_ms;
+    return ACB_OK;
+}
+
+static int check_skip(const uint32_t *skip, int64_t n_skip, int algo) {
+    if (algo == ACB_ALGO_LONG) { acb_set_error("iter_long has no white-space skipping"); return ACB_EINVAL; }
+    if (n_skip < 0 || n_skip > ACB_MAX_SKIP || (n_skip && !skip)) { acb_set_error("skip set of %lld letters (at most %d)", (long long)n_skip, ACB_MAX_SKIP); return ACB_EINVAL; }
+    for (int64_t i = 1; i < n_skip; i++)
+        if (skip[i] <= skip[i - 1]) { acb_set_error("skip set not sorted and distinct at %lld", (long long)i); return ACB_EINVAL; }
+    return ACB_OK;
+}
+
+/* Compact total_bytes of d_in (16-byte aligned) into tb->k_buf and the haystack offsets into tb->k_coff; *kept_bytes
+ * is the compacted size (this waits for the compaction on s).  The map-back metadata stays in tb->k_*. */
+static int compact(acb_table *tb, const uint8_t *d_in, int64_t total, const int64_t *d_off, int64_t n_hay, int64_t stride,
+                   const uint32_t *skip, int64_t n_skip, cudaStream_t s, long long *kept_bytes, CompactMeta *meta) {
+    const int L = tb->L, ls = L == 4 ? 2 : (L == 2 ? 1 : 0);
+    const long long n_letters = total / L, n_tiles = (n_letters + kCmpTile - 1) / kCmpTile;
+    int rc;
+    if ((rc = ensure(&tb->k_buf, &tb->k_buf_cap, (size_t)total + 64)) || (rc = ensure(&tb->k_mask, &tb->k_mask_cap, (size_t)n_tiles * kCmpThreads)) ||
+        (rc = ensure(&tb->k_gpre, &tb->k_gpre_cap, (size_t)n_tiles * kCmpThreads)) || (rc = ensure(&tb->k_tile_pre, &tb->k_tile_pre_cap, (size_t)n_tiles + 1)) ||
+        (rc = ensure(&tb->k_status, &tb->k_status_cap, (size_t)n_tiles)) || (rc = ensure(&tb->k_coff, &tb->k_coff_cap, (size_t)n_hay + 1)))
+        return rc;
+    if (!tb->k_set) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->k_set), ACB_MAX_SKIP * sizeof(uint32_t)));
+    if (!tb->k_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->k_ctr), sizeof(unsigned int)));
+    if (!tb->h_kept) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_kept), sizeof(long long)));
+    if (tb->k_done) CUDA_TRY(cudaStreamWaitEvent(s, tb->k_done, 0));
+    g_compact_ms = g_remap_ms = 0.f;
+    CompactParams p;
+    memset(&p, 0, sizeof(p));
+    p.in = d_in; p.out = tb->k_buf; p.n_letters = n_letters;
+    p.mask = tb->k_mask; p.gpre = tb->k_gpre; p.tile_pre = tb->k_tile_pre; p.status = tb->k_status; p.ctr = tb->k_ctr;
+    p.n_tiles = n_tiles; p.set = tb->k_set; p.n_set = (int)n_skip;
+    for (int64_t i = 0; i < n_skip; i++) if (skip[i] < 256) p.bits[skip[i] >> 5] |= 1u << (skip[i] & 31);
+    if (L > 1 && n_skip) CUDA_TRY(cudaMemcpyAsync(tb->k_set, skip, (size_t)n_skip * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemsetAsync(tb->k_status, 0, (size_t)n_tiles * sizeof(unsigned long long), s));
+    CUDA_TRY(cudaMemsetAsync(tb->k_ctr, 0, sizeof(unsigned int), s));
+    if (n_tiles > 0x7fffffffLL) { acb_set_error("batch too large to compact in one launch"); return ACB_ERANGE; }
+    if ((rc = skip_timing_begin(tb, s))) return rc;
+    if (L == 1) acb_compact_kernel<uint8_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
+    else if (L == 2) acb_compact_kernel<uint16_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
+    else acb_compact_kernel<uint32_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
+    CUDA_TRY(cudaGetLastError());
+    if ((rc = skip_timing_end(tb, s, &g_compact_ms))) return rc;
+    meta->mask = tb->k_mask; meta->gpre = tb->k_gpre; meta->tile_pre = tb->k_tile_pre; meta->n_tiles = n_tiles;
+    acb_compact_offsets_kernel<<<(unsigned)((n_hay + 1 + 255) / 256), 256, 0, s>>>(*meta, reinterpret_cast<const long long *>(d_off), stride,
+                                                                                 n_hay, ls, tb->k_coff);
+    CUDA_TRY(cudaGetLastError());
+    g_launches.fetch_add(2);
+    CUDA_TRY(cudaMemcpyAsync(tb->h_kept, tb->k_tile_pre + n_tiles, sizeof(long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    *kept_bytes = *tb->h_kept * L;
+    return ACB_OK;
+}
+
+static int launch_remap(acb_table *tb, const CompactMeta &meta, const int64_t *d_off, int64_t stride, acb_match *d_out, int64_t cap,
+                        int64_t *d_count, cudaStream_t s) {
+    if (cap <= 0) return ACB_OK;
+    const int ls = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
+    const long long grid = std::min<long long>((cap + 255) / 256, (long long)tb->sm_count * 16);
+    int rc;
+    if ((rc = skip_timing_begin(tb, s))) return rc;
+    acb_remap_kernel<<<(unsigned)grid, 256, 0, s>>>(meta, tb->k_coff, reinterpret_cast<const long long *>(d_off), stride, ls, d_out,
+                                                    reinterpret_cast<const unsigned long long *>(d_count), cap);
+    CUDA_TRY(cudaGetLastError());
+    g_launches.fetch_add(1);
+    return skip_timing_end(tb, s, &g_remap_ms);
+}
+
+extern "C" int acb_scan_device_skip(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
+                                    const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
+                                    acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo,
+                                    const uint32_t *skip, int64_t n_skip) {
+    if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    int rc = check_skip(skip, n_skip, algo);
+    if (rc != ACB_OK) return rc;
+    if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
+    if (!d_offsets && (stride_bytes <= 0 || stride_bytes % tb->L || stride_bytes * n_hay != total_bytes)) {
+        acb_set_error("fixed-stride batch needs stride_bytes > 0, a multiple of letter_bytes, and n_hay*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    CUDA_TRY(cudaSetDevice(tb->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
+    if (n_skip == 0) return acb_scan_device(tb, d_hay, total_bytes, d_offsets, n_hay, stride_bytes, d_out, cap, d_count, stream, algo);
+    if (total_bytes == 0 || n_hay == 0 || tb->n_keys == 0) return ACB_OK;
+    if (reinterpret_cast<uintptr_t>(d_hay) & 15) { acb_set_error("d_hay must be 16-byte aligned"); return ACB_EINVAL; }
+    long long kept = 0;
+    CompactMeta meta;
+    if ((rc = compact(tb, d_hay, total_bytes, d_offsets, n_hay, stride_bytes, skip, n_skip, s, &kept, &meta))) return rc;
+    if (kept == 0) return ACB_OK;
+    if ((rc = acb_scan_device(tb, tb->k_buf, kept, reinterpret_cast<const int64_t *>(tb->k_coff), n_hay, 0, d_out, cap, d_count, stream, algo))) return rc;
+    if ((rc = launch_remap(tb, meta, d_offsets, stride_bytes, d_out, cap, d_count, s))) return rc;
+    return skip_work_issued(tb, s);
+}
+
+/* n records of a host-buffer call, in tb->w_out: sorted (on the device when the key fits, else on the host) into the
+ * pinned staging buffer, and into `out` when given */
+static int records_to_host(acb_table *tb, unsigned long long n, int64_t n_hay, int64_t max_letters, int sort, acb_match *out, cudaStream_t s) {
+    int rc;
+    if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
+    bool host_sort = false;                                /* the device sort's key does not fit 64 bits: sort on the host */
+    if (sort && (rc = acb_sort_matches_device(tb, tb->w_out, (int64_t)n, n_hay, max_letters, s)) != ACB_OK) {
+        if (rc != ACB_ERANGE) return rc;
+        host_sort = true;
+    }
+    CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->w_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    if (host_sort) {
+        const int32_t *kl = tb->key_len.data();
+        std::sort(tb->h_out, tb->h_out + n, [kl](const acb_match &a, const acb_match &b) {
+            if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
+            if (a.end_index != b.end_index) return a.end_index < b.end_index;
+            return kl[a.key_id] > kl[b.key_id];
+        });
+    }
+    if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
+    return ACB_OK;
+}
+
+extern "C" int acb_scan_host_skip(acb_table *tb, const uint8_t *hay, int64_t total_bytes,
+                                  const int64_t *offsets, int64_t n_hay, int64_t stride_bytes,
+                                  acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort,
+                                  const uint32_t *skip, int64_t n_skip) {
+    if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *n_found = 0;
+    int rc = check_skip(skip, n_skip, algo);
+    if (rc != ACB_OK) return rc;
+    tb->h_out_n = 0;
+    if (total_bytes == 0 || n_hay == 0) return ACB_OK;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
+    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_hay + 1))) return rc;
+    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1)))) return rc;
+    cudaStream_t s = tb->stream;
+    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
+    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_hay + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+    rc = acb_scan_device_skip(tb, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_hay, stride_bytes,
+                              tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), s, algo, skip, n_skip);
+    if (rc != ACB_OK) return rc;
+    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    const unsigned long long n = *tb->h_count;
+    *n_found = (int64_t)n;
+    if (n > (unsigned long long)cap) {
+        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
+        return ACB_EOVERFLOW;
+    }
+    if (n && (rc = records_to_host(tb, n, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, sort, out, s))) return rc;
+    tb->h_out_n = n;
+    return ACB_OK;
+}
 
 /* ------------------------------------------------------------ stream batches */
 /* A stream batch (acb_streams) keeps every stream's carry-over in HBM: the number of letters consumed, and either the
@@ -1937,6 +2307,8 @@ struct StreamsArgs {
     const int32_t *ids;           /* chunk -> stream; nullptr: chunk h continues stream h */
     long long n_streams;
     long long *pos;               /* [n_streams] letters consumed since the start / the last reset */
+    long long *kept;              /* with a skip set: [n_streams] letters consumed that were kept (the tail counts those);
+                                     nullptr: every letter is kept, pos serves */
     uint8_t *tail;                /* [n_streams][T letters]: the last min(T, pos) letters consumed, left aligned */
     uint8_t *next_tail;           /* [n_chunks][T letters]: the tail after this feed's chunk (staged) */
     int32_t *state;               /* long mode: [n_streams] walk state */
@@ -1966,7 +2338,7 @@ __global__ void __launch_bounds__(kDfaThreads) acb_seam_kernel(const __grid_cons
     chunk_span(p.offsets, p.stride_bytes, h, hs, he);
     const int L = p.L, ls = p.letter_shift;                      /* L == 1 << ls */
     const long long n = (he - hs) >> ls;
-    const long long t = min((long long)a.T, a.pos[s]), m = min((long long)a.T, n);
+    const long long t = min((long long)a.T, a.kept ? a.kept[s] : a.pos[s]), m = min((long long)a.T, n);
     const uint8_t *tail = a.tail + s * a.T * L, *text = p.hay + hs;
     const long long tb = t * L;
     int32_t st = 0;
@@ -2007,9 +2379,10 @@ __global__ void acb_streams_gather_kernel(const StreamsArgs a, long long n_chunk
     a.start[h] = s < 0 ? 0 : a.state[s];
 }
 
-/* switch the fed streams to what the feed staged, only when its records fit (count == nullptr: unconditionally) */
+/* switch the fed streams to what the feed staged, only when its records fit (count == nullptr: unconditionally).
+ * koff: the compacted chunks' byte offsets of a feed with a skip set */
 __global__ void acb_streams_commit_kernel(const StreamsArgs a, const long long *off, long long stride, long long n_chunks,
-                                          const unsigned long long *count, long long cap) {
+                                          const unsigned long long *count, long long cap, const long long *koff) {
     const long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (h >= n_chunks || (count && *count > (unsigned long long)cap)) return;
     const long long s = chunk_stream(a, h);
@@ -2020,6 +2393,7 @@ __global__ void acb_streams_commit_kernel(const StreamsArgs a, const long long *
     const long long tb = (long long)a.T * a.L;
     for (long long j = 0; j < tb; ++j) a.tail[s * tb + j] = a.next_tail[h * tb + j];
     a.pos[s] += (he - hs) / a.L;
+    if (a.kept) a.kept[s] += (__ldg(koff + h + 1) - __ldg(koff + h)) / a.L;
 }
 
 __global__ void acb_streams_reset_kernel(const StreamsArgs a, long long n_ids) {
@@ -2028,6 +2402,7 @@ __global__ void acb_streams_reset_kernel(const StreamsArgs a, long long n_ids) {
     const long long s = chunk_stream(a, i);
     if (s < 0) return;
     a.pos[s] = 0;
+    if (a.kept) a.kept[s] = 0;
     if (a.state) a.state[s] = 0;
 }
 } // namespace
@@ -2044,6 +2419,8 @@ struct acb_streams {
     int32_t *d_start = nullptr; size_t start_cap = 0;
     int32_t *d_end = nullptr; size_t end_cap = 0;
     int32_t *d_ids = nullptr; size_t ids_cap = 0;                 /* ids of a host feed or a reset, uploaded */
+    std::vector<uint32_t> skip;                                   /* the skip set (find_all batches only), host copy */
+    long long *d_kept = nullptr;                                  /* with a skip set: kept letters consumed per stream */
 };
 
 static int32_t tail_letters(const acb_table *tb) { return std::max<int32_t>(tb->max_key_bytes / tb->L - 1, 0); }
@@ -2060,7 +2437,7 @@ static int streams_check_table(const acb_streams *ss, const acb_table *tb) {
 static StreamsArgs streams_args(const acb_streams *ss, const int32_t *d_ids) {
     StreamsArgs a;
     memset(&a, 0, sizeof(a));
-    a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.tail = ss->d_tail; a.state = ss->d_state; a.T = ss->T; a.L = ss->L;
+    a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.kept = ss->d_kept; a.tail = ss->d_tail; a.state = ss->d_state; a.T = ss->T; a.L = ss->L;
     return a;
 }
 
@@ -2068,7 +2445,7 @@ extern "C" void acb_streams_free(acb_streams *ss) {
     if (!ss) return;
     cudaSetDevice(ss->device);
     cudaFree(ss->d_pos); cudaFree(ss->d_tail); cudaFree(ss->d_state); cudaFree(ss->d_next_tail);
-    cudaFree(ss->d_start); cudaFree(ss->d_end); cudaFree(ss->d_ids);
+    cudaFree(ss->d_start); cudaFree(ss->d_end); cudaFree(ss->d_ids); cudaFree(ss->d_kept);
     delete ss;
 }
 
@@ -2133,6 +2510,22 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
         acb_long_kernel<<<grid, kDfaThreads, 0, s>>>(p);
         CUDA_TRY(cudaGetLastError());
         g_launches.fetch_add(2);
+    } else if (ss->d_kept) {                                     /* skip set: compact, scan, walk the seams, map back */
+        long long kept = 0;
+        CompactMeta meta;
+        if ((rc = compact(tb, d_chunks, total, d_off, n_chunks, stride, ss->skip.data(), (int64_t)ss->skip.size(), s, &kept, &meta))) return rc;
+        const int64_t *koff = reinterpret_cast<const int64_t *>(tb->k_coff);
+        if (kept && tb->n_keys > 0 && (rc = acb_scan_device(tb, tb->k_buf, kept, koff, n_chunks, 0, d_out, cap, d_count, s, algo))) return rc;
+        if (ss->T > 0) {
+            if ((rc = ensure(&ss->d_next_tail, &ss->next_tail_cap, (size_t)n_chunks * ss->T * ss->L))) return rc;
+            ScanParams pk;
+            fill_params(tb, pk, tb->k_buf, kept, koff, n_chunks, 0, d_out, cap, d_count);
+            a.next_tail = ss->d_next_tail;
+            acb_seam_kernel<<<grid, kDfaThreads, 0, s>>>(pk, a);
+            CUDA_TRY(cudaGetLastError());
+            g_launches.fetch_add(1);
+        }
+        if ((rc = launch_remap(tb, meta, d_off, stride, d_out, cap, d_count, s))) return rc;
     } else {
         if (tb->n_keys > 0 && (rc = acb_scan_device(tb, d_chunks, total, d_off, n_chunks, stride, d_out, cap, d_count, s, algo))) return rc;
         if (ss->T > 0) {
@@ -2144,9 +2537,11 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
         }
     }
     acb_streams_commit_kernel<<<grid, kDfaThreads, 0, s>>>(a, reinterpret_cast<const long long *>(d_off), stride, n_chunks,
-                                                          reinterpret_cast<const unsigned long long *>(d_count), cap);
+                                                          reinterpret_cast<const unsigned long long *>(d_count), cap,
+                                                          tb->k_coff);
     CUDA_TRY(cudaGetLastError());
     g_launches.fetch_add(1);
+    if (ss->d_kept && (rc = skip_work_issued(tb, s))) return rc;
     return ACB_OK;
 }
 
@@ -2231,6 +2626,7 @@ extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n)
     CUDA_TRY(cudaDeviceSynchronize());                           /* feeds in flight on any stream see the old state */
     if (!ids) {
         CUDA_TRY(cudaMemset(ss->d_pos, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(long long)));
+        if (ss->d_kept) CUDA_TRY(cudaMemset(ss->d_kept, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(long long)));
         if (ss->d_state) CUDA_TRY(cudaMemset(ss->d_state, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(int32_t)));
     } else if (n) {
         if ((rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)n))) return rc;
@@ -2248,5 +2644,32 @@ extern "C" int acb_streams_positions(acb_streams *ss, int64_t *out, int64_t cap)
     CUDA_TRY(cudaSetDevice(ss->device));
     CUDA_TRY(cudaDeviceSynchronize());
     if (ss->n) CUDA_TRY(cudaMemcpy(out, ss->d_pos, (size_t)ss->n * sizeof(long long), cudaMemcpyDeviceToHost));
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_new_skip(const acb_table *tb, int64_t n_streams, const uint32_t *skip, int64_t n_skip, acb_streams **out) {
+    if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    int rc = check_skip(skip, n_skip, ACB_ALGO_FILTER);
+    if (rc != ACB_OK) return rc;
+    if ((rc = acb_streams_new(tb, n_streams, 0, out))) return rc;
+    acb_streams *ss = *out;
+    const size_t n = (size_t)std::max<int64_t>(n_streams, 1);
+    try {
+        ss->skip.assign(skip, skip + n_skip);
+    } catch (const std::exception &) {
+        acb_streams_free(ss);
+        *out = nullptr;
+        acb_set_error("out of host memory");
+        return ACB_ENOMEM;
+    }
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ss->d_kept), n * sizeof(long long));
+    if (e == cudaSuccess) e = cudaMemset(ss->d_kept, 0, n * sizeof(long long));
+    if (e != cudaSuccess) {
+        acb_set_error("allocating %lld streams: %s", (long long)n_streams, cudaGetErrorString(e));
+        acb_streams_free(ss);
+        *out = nullptr;
+        return ACB_ECUDA;
+    }
     return ACB_OK;
 }

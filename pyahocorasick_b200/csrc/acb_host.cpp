@@ -23,6 +23,7 @@
 #include <exception>
 #include <new>
 #include <vector>
+#include <wctype.h>
 
 /* ------------------------------------------------------------------ errors */
 static thread_local char g_err[512] = "";
@@ -1246,5 +1247,23 @@ extern "C" int acb_node_records_span(const uint8_t *buf, int64_t len, int64_t n_
         pos += (int64_t)n * pair_bytes;
     }
     *span = pos;
+    return ACB_OK;
+}
+
+/* ------------------------------------------------------------- white space */
+/* The letters iter(..., ignore_white_space=True) skips (src/AutomatonSearchIter.c:270-274): libc iswspace() under the
+ * current LC_CTYPE, of the letter as the reference widens it (src/utils.c:199-202 for the bytes build). */
+extern "C" int acb_space_letters(int letter_bytes, int signed_bytes, uint32_t *out, int64_t cap, int64_t *n) {
+    if (!n || cap < 0 || (cap && !out) || (letter_bytes != 1 && letter_bytes != 2 && letter_bytes != 4)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    const uint32_t last = letter_bytes == 1 ? 0xffu : (letter_bytes == 2 ? 0xffffu : 0x10ffffu);   /* no code point past U+10FFFF */
+    int64_t k = 0;
+    for (uint32_t v = 0; v <= last; v++) {
+        const uint32_t w = (letter_bytes == 1 && signed_bytes) ? (uint32_t)(uint16_t)(int16_t)(int8_t)(uint8_t)v : v;
+        if (!iswspace((wint_t)w)) continue;
+        if (k < cap) out[k] = v;
+        k++;
+    }
+    *n = k;
+    if (k > cap) { acb_set_error("%lld white-space letters, capacity %lld", (long long)k, (long long)cap); return ACB_EOVERFLOW; }
     return ACB_OK;
 }
