@@ -354,6 +354,25 @@ int acb_streams_new_skip(const acb_table *tb, int64_t n_streams, const uint32_t 
  * them); 0 when timing is off or the call launched none.  acb_last_kernel_ms() gives its scan kernel. */
 int acb_last_skip_ms(float *compact_ms, float *remap_ms);
 
+/* ---- dictionary lookups: exists / match / longest_prefix / get for many keys at once -------------------------------
+ * trie_find / trie_longest (src/trie.c:139-174) for n_keys queries at once.  key_id[i]: id of the key equal to query i
+ * or -1 (always -1 for an empty query); prefix[i]: leading LETTERS of query i that follow trie edges (a letter walked
+ * only in part does not count), so query i is a prefix of some key exactly when prefix[i] equals its length in letters.
+ * prefix never exceeds the longest key.  Queries as acb_scan_device's haystacks (d_offsets: n_keys+1 int64 byte
+ * offsets, multiples of letter_bytes, or NULL and stride_bytes >= 0 for keys of one length); unlike the scans, the
+ * keys need no alignment.  One lane per query walks the goto table of the uploaded automaton from the root.
+ *
+ * DEVICE buffers, asynchronous on `stream`.  d_offsets is not checked.  With kernel timing on (acb_set_kernel_timing)
+ * the call waits for its kernel and acb_last_kernel_ms() gives its time. */
+int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t total_bytes, const int64_t *d_offsets,
+                      int64_t n_keys, int64_t stride_bytes, int32_t *d_key_id, int32_t *d_prefix, void *stream);
+
+/* HOST buffers: upload, kernel, copy back, synchronous.  The offsets are checked (ACB_EINVAL) before anything runs.
+ * The scratch buffers belong to the table: one call at a time per table, as for the scans.  Without a device:
+ * ACB_ECUDA (there is no CPU fallback). */
+int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total_bytes, const int64_t *offsets,
+                    int64_t n_keys, int64_t stride_bytes, int32_t *key_id, int32_t *prefix);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

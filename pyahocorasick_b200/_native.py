@@ -102,6 +102,8 @@ def lib() -> ctypes.CDLL:
         "acb_scan_host_skip": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, i64, pi64, ctypes.c_int, ctypes.c_int, vp, i64]),
         "acb_streams_new_skip": (ctypes.c_int, [vp, i64, vp, i64, ctypes.POINTER(vp)]),
         "acb_last_skip_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]),
+        "acb_lookup_device": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, vp, vp]),
+        "acb_lookup_host": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, vp]),
         "acb_launch_count": (i64, []),
         "acb_set_kernel_timing": (ctypes.c_int, [ctypes.c_int]),
         "acb_last_kernel_ms": (ctypes.c_float, []),
@@ -129,7 +131,7 @@ EXPORTED_SYMBOLS = [
     "acb_scan_device", "acb_scan_host", "acb_copy_records", "acb_take_records", "acb_release_records", "acb_sort_matches_device", "acb_table_set_long_state", "acb_table_get_long_state",
     "acb_streams_new", "acb_streams_free", "acb_streams_reset", "acb_streams_feed_device", "acb_streams_feed_host",
     "acb_streams_positions", "acb_space_letters", "acb_scan_device_skip", "acb_scan_host_skip", "acb_streams_new_skip",
-    "acb_last_skip_ms", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_last_skip_ms", "acb_lookup_device", "acb_lookup_host", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

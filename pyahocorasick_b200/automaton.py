@@ -955,10 +955,11 @@ class Automaton:
             return Matches(self._scan_flat(flat, offs, n, stride, algo=algo, sort=sort, device=device, narrow=True), self._values)
         return Matches(self._scan_flat(flat, offs, n, stride, algo=algo, sort=sort, device=device), self._values)
 
-    def _batch_input(self, haystacks, narrow_ok: bool = True):
+    def _batch_input(self, haystacks, narrow_ok: bool = True, required: bool = True):
         """The input forms of find_all_batch, checked and laid out for a scan: ("device", tensor) for a CUDA tensor,
         else ("host", flat uint8, int64 byte offsets or None, n, stride_bytes or 0, narrow).  narrow: the buffer holds
-        the 1-byte letters of the latin-1 automaton (unicode flavour, only where narrow_ok)."""
+        the 1-byte letters of the latin-1 automaton (unicode flavour, only where narrow_ok).  required=False: an item
+        of the wrong type raises the TypeError of the dict-like methods instead of iter()'s."""
         L = self._L
         if type(haystacks).__module__.startswith("torch") and getattr(haystacks, "is_cuda", False):
             return ("device", haystacks)
@@ -978,15 +979,23 @@ class Automaton:
         # the latin-1 automaton finds exactly the matches of a latin-1 haystack -- all of them.  iter_long's walk is
         # different: which match it keeps depends on the whole trie (a non-latin-1 key whose prefix is latin-1 adds
         # nodes the walk passes through, src/AutomatonSearchIterLong.c:118-126), so it always runs on the full one
-        if not self._UNICODE and self._key_type == KEY_STRING and isinstance(haystacks, (list, tuple)) and haystacks \
-                and set(map(type, haystacks)) == {bytes}:       # C-level pass, 3 x faster than a generator with all()
-            # the common drop-in input, a list of bytes objects: one join instead of an array per haystack
+        # the common drop-in inputs, a list of bytes objects or (4-byte letters only) of str objects: one join instead
+        # of an array per haystack.  utf-32 encodes every code point by itself, so the joined buffer holds exactly the
+        # bytes of the items encoded one by one
+        wide_str = self._UNICODE and not narrow_ok
+        if self._key_type == KEY_STRING and (wide_str or not self._UNICODE) and isinstance(haystacks, (list, tuple)) \
+                and haystacks and set(map(type, haystacks)) == {str if wide_str else bytes}:   # C-level pass, 3 x faster than all()
             n = len(haystacks)
             offs = np.zeros(n + 1, dtype=np.int64)
             np.cumsum(np.fromiter(map(len, haystacks), dtype=np.int64, count=n), out=offs[1:])
-            return ("host", np.frombuffer(b"".join(haystacks), dtype=np.uint8), offs, n, 0, False)
+            if wide_str:
+                offs *= 4
+                flat = "".join(haystacks).encode("utf-32-le", "surrogatepass")
+            else:
+                flat = b"".join(haystacks)
+            return ("host", np.frombuffer(flat, dtype=np.uint8), offs, n, 0, False)
         get = self._hay_letters if narrow_ok else self._letters
-        letters = [get(h, required=True) for h in haystacks]
+        letters = [get(h, required=required) for h in haystacks]
         narrow = self._uses_narrow() and len(letters) > 0 and all(a.dtype == np.uint8 for a in letters)
         if self._uses_narrow() and not narrow:                   # mixed batch: everything at 4 bytes per letter
             letters = [a.astype("<u4") if a.dtype == np.uint8 else a for a in letters]
@@ -1021,6 +1030,100 @@ class Automaton:
             raise ValueError("iter_long has no ignore_white_space option")
         skip = self._skip_set(False) if ignore_white_space else None
         return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip)
+
+    # ------------------------------------------------------------------ batch lookups (new)
+    # exists / match / longest_prefix / get for a whole batch of keys, in one GPU call (acb_lookup_*).  `keys` takes the
+    # input forms of find_all_batch.  The walk always runs on the full table: a latin-1 key can be a prefix of a key
+    # that is not latin-1, and the latin-1 automaton lacks those nodes.
+    def exists_batch(self, keys, *, device: Optional[int] = None):
+        """``[A.exists(k) for k in keys]`` as bool[n] (a bool CUDA tensor, not synchronised, for a CUDA tensor batch)."""
+        key_id, _, _ = self._lookup_batch(keys, device)
+        return key_id >= 0
+
+    def match_batch(self, keys, *, device: Optional[int] = None):
+        """``[A.match(k) for k in keys]`` as bool[n] (a bool CUDA tensor, not synchronised, for a CUDA tensor batch)."""
+        _, prefix, lens = self._lookup_batch(keys, device)
+        return prefix == lens
+
+    def longest_prefix_batch(self, keys, *, device: Optional[int] = None):
+        """``[A.longest_prefix(k) for k in keys]`` as int64[n] (an int64 CUDA tensor, not synchronised, for a CUDA
+        tensor batch)."""
+        _, prefix, _ = self._lookup_batch(keys, device)
+        return prefix.astype(np.int64) if isinstance(prefix, np.ndarray) else prefix.long()
+
+    def get_batch(self, keys, default=_MISSING, *, device: Optional[int] = None) -> list:
+        """``[A.get(k[, default]) for k in keys]``: a list of values, read when the call returns.  Without a default,
+        KeyError of the first key that is missing."""
+        if not isinstance(keys, (list, tuple, np.ndarray)) and not type(keys).__module__.startswith("torch"):
+            keys = list(keys)                                   # an iterator: kept, for the KeyError
+        key_id, _, _ = self._lookup_batch(keys, device)
+        if not isinstance(key_id, np.ndarray):
+            key_id = key_id.cpu().numpy()                      # synchronises torch's current stream
+        values = self._values
+        if default is Automaton._MISSING:
+            miss = np.flatnonzero(key_id < 0)
+            if miss.size:
+                raise KeyError(self._batch_key(keys, int(miss[0])))
+        else:
+            values = values + [default]                         # key_id -1 picks it
+        return list(map(values.__getitem__, key_id.tolist()))
+
+    @_locked
+    def _lookup_batch(self, keys, device: Optional[int]):
+        """(key_id int32[n], prefix int32[n], length of every key in letters) of a batch of keys: numpy arrays, or for
+        a CUDA tensor int32 CUDA tensors computed on torch's current stream and one length for all rows."""
+        self._require_automaton()
+        batch = self._batch_input(keys, narrow_ok=False, required=False)
+        if batch[0] == "device":
+            import torch
+            t = batch[1]
+            n, stride = self._device_batch_shape(t)
+            key_id = torch.empty(n, dtype=torch.int32, device=t.device)
+            prefix = torch.empty(n, dtype=torch.int32, device=t.device)
+            if n:
+                dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+                tb = self._ensure_table(dev)
+                with torch.cuda.device(dev):
+                    N.check(self._lib.acb_lookup_device(tb, t.data_ptr() if stride else None, n * stride, None, n, stride,
+                                                        key_id.data_ptr(), prefix.data_ptr(),
+                                                        torch.cuda.current_stream().cuda_stream))
+            return key_id, prefix, stride // self._L
+        _, flat, offs, n, stride, _ = batch
+        key_id, prefix = self._lookup_host(flat, offs, n, stride, device)
+        lens = (np.diff(offs) if offs is not None else np.full(n, stride, dtype=np.int64)) // self._L
+        return key_id, prefix, lens
+
+    def _lookup_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n: int, stride_bytes: int,
+                     device: Optional[int]):
+        """acb_lookup_host over a host batch -> (key_id int32[n], prefix int32[n])"""
+        key_id = np.empty(n, dtype=np.int32)
+        prefix = np.empty(n, dtype=np.int32)
+        if n:
+            tb = self._ensure_table(device)
+            N.check(self._lib.acb_lookup_host(tb, N.ptr(flat) if flat.size else None, int(flat.size),
+                                              N.ptr(offsets) if offsets is not None else None, n, stride_bytes,
+                                              N.ptr(key_id), N.ptr(prefix)))
+        return key_id, prefix
+
+    def _batch_key(self, keys, i: int):
+        """key i of a batch as the dict-like methods take it (for KeyError)"""
+        if isinstance(keys, tuple) and len(keys) == 2 and isinstance(keys[0], np.ndarray) and isinstance(keys[1], np.ndarray):
+            flat, offs = keys
+            raw = np.ascontiguousarray(flat, dtype=np.uint8).reshape(-1)[int(offs[i]):int(offs[i + 1])].tobytes()
+        elif isinstance(keys, (list, tuple)):
+            return keys[i]
+        elif isinstance(keys, np.ndarray):
+            raw = keys[i].tobytes()
+        else:
+            raw = keys[i].cpu().numpy().tobytes()
+        if self._key_type == KEY_SEQUENCE:
+            return tuple(np.frombuffer(raw, dtype=_LETTER_DTYPE[self._L]).tolist())
+        if self._UNICODE:
+            try:
+                return raw.decode("utf-32-le", "surrogatepass")
+            except UnicodeDecodeError:                          # letters beyond U+10FFFF: no str holds them
+                return raw
+        return raw
 
 
 class StreamBatch:

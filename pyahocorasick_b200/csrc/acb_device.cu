@@ -1304,6 +1304,8 @@ struct acb_table {
     long long *h_kept = nullptr;                         /* pinned: kept letters of the last compaction */
     cudaEvent_t k_done = nullptr;                        /* the last skip call's work that reads k_* has been issued before it */
     cudaEvent_t k_t0 = nullptr, k_t1 = nullptr;          /* kernel timing of the compaction and the remap */
+    /* workspace of acb_lookup_host (keys and offsets go to w_hay / w_off) */
+    int32_t *w_lk = nullptr; size_t w_lk_cap = 0;        /* key_id[n] then prefix[n] */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1343,6 +1345,7 @@ extern "C" void acb_table_free(acb_table *tb) {
     if (tb->h_counts) cudaFreeHost(tb->h_counts);
     cudaFree(tb->k_buf); cudaFree(tb->k_mask); cudaFree(tb->k_gpre); cudaFree(tb->k_tile_pre); cudaFree(tb->k_status);
     cudaFree(tb->k_coff); cudaFree(tb->k_set); cudaFree(tb->k_ctr);
+    cudaFree(tb->w_lk);
     if (tb->h_kept) cudaFreeHost(tb->h_kept);
     if (tb->k_done) cudaEventDestroy(tb->k_done);
     if (tb->k_t0) cudaEventDestroy(tb->k_t0);
@@ -2671,5 +2674,127 @@ extern "C" int acb_streams_new_skip(const acb_table *tb, int64_t n_streams, cons
         *out = nullptr;
         return ACB_ECUDA;
     }
+    return ACB_OK;
+}
+
+/* ------------------------------------------------------------ dictionary lookups */
+/* exists / match / longest_prefix / get for a whole batch of keys (trie_find / trie_longest, src/trie.c:139-174): one
+ * lane per query walks the trie edges of the flattened table from the root, byte by byte, and stops at the first
+ * missing edge.  Flattening keeps only nodes with a live key below them, so the walk takes exactly the edges the host
+ * trie's walk takes.  Every step is a dependent load from the goto table (gigabytes for a million keys): the kernel is
+ * bound by the latency of those loads, so it only keeps the byte classes in shared memory and many lanes in flight. */
+namespace {
+constexpr int kLookupThreads = 256;
+
+struct LookupParams {
+    const uint8_t *keys;
+    const long long *offsets;      /* nullptr => fixed stride */
+    long long n, stride;
+    const uint8_t *cls;
+    const int32_t *gto;            /* flagged goto (kTermBit) */
+    const int32_t *key_of;
+    long long S;
+    int32_t letter_shift;
+    int32_t *key_id, *prefix;
+};
+
+__global__ void __launch_bounds__(kLookupThreads) acb_lookup_kernel(const __grid_constant__ LookupParams p) {
+    __shared__ uint8_t cls[256];
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) cls[i] = p.cls[i];
+    __syncthreads();
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < p.n; q += (long long)gridDim.x * blockDim.x) {
+        const long long b0 = p.offsets ? __ldg(p.offsets + q) : q * p.stride;
+        const long long b1 = p.offsets ? __ldg(p.offsets + q + 1) : b0 + p.stride;
+        int32_t s = 0;
+        long long i = b0;
+        for (; i < b1; ++i) {                      /* class 0 needs no test: its column is all -1 unless K == 256 */
+            const int32_t nx = __ldg(p.gto + (long long)cls[__ldg(p.keys + i)] * p.S + s);
+            if (nx < 0) break;
+            s = nx & kIdMask;                      /* drop kTermBit */
+        }
+        p.key_id[q] = (i == b1 && b1 > b0) ? __ldg(p.key_of + s) : -1;
+        p.prefix[q] = (int32_t)((i - b0) >> p.letter_shift);   /* whole letters only; at most the longest key */
+    }
+}
+} // namespace
+
+/* fixed stride: stride >= 0, a multiple of the letter width, n * stride == total (without overflow) */
+static bool lookup_stride_ok(const acb_table *tb, int64_t total_bytes, int64_t n_keys, int64_t stride_bytes) {
+    if (stride_bytes < 0 || stride_bytes % tb->L) return false;
+    if (stride_bytes == 0) return total_bytes == 0;
+    return n_keys <= total_bytes / stride_bytes && n_keys * stride_bytes == total_bytes;
+}
+
+extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t total_bytes, const int64_t *d_offsets,
+                                 int64_t n_keys, int64_t stride_bytes, int32_t *d_key_id, int32_t *d_prefix, void *stream) {
+    if (!tb || total_bytes < 0 || n_keys < 0 || (total_bytes && !d_keys) || (n_keys && (!d_key_id || !d_prefix))) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    if (!d_offsets && !lookup_stride_ok(tb, total_bytes, n_keys, stride_bytes)) {
+        acb_set_error("fixed-stride keys need stride_bytes >= 0, a multiple of letter_bytes, and n_keys*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    if (n_keys == 0) return ACB_OK;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    LookupParams p;
+    p.keys = d_keys; p.offsets = reinterpret_cast<const long long *>(d_offsets); p.n = n_keys; p.stride = stride_bytes;
+    p.cls = tb->d_cls; p.gto = tb->d_goto; p.key_of = tb->d_keyof; p.S = tb->S;
+    p.letter_shift = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
+    p.key_id = d_key_id; p.prefix = d_prefix;
+    const long long grid = std::min<long long>((n_keys + kLookupThreads - 1) / kLookupThreads, (long long)tb->sm_count * 8);
+    const bool timing = g_timing.load() != 0;
+    if (timing) {
+        if (!tb->ev0) { CUDA_TRY(cudaEventCreate(&tb->ev0)); CUDA_TRY(cudaEventCreate(&tb->ev1)); }
+        CUDA_TRY(cudaEventRecord(tb->ev0, s));
+    }
+    acb_lookup_kernel<<<(unsigned)grid, kLookupThreads, 0, s>>>(p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { acb_set_error("lookup kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
+    g_launches.fetch_add(1);
+    if (timing) {
+        CUDA_TRY(cudaEventRecord(tb->ev1, s));
+        CUDA_TRY(cudaEventSynchronize(tb->ev1));
+        float ms = 0.f;
+        CUDA_TRY(cudaEventElapsedTime(&ms, tb->ev0, tb->ev1));
+        g_last_ms = ms;
+    }
+    return ACB_OK;
+}
+
+extern "C" int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total_bytes, const int64_t *offsets,
+                               int64_t n_keys, int64_t stride_bytes, int32_t *key_id, int32_t *prefix) {
+    if (!tb || total_bytes < 0 || n_keys < 0 || (total_bytes && !keys) || (n_keys && (!key_id || !prefix))) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (offsets) {                                  /* the kernel reads keys[offsets[i] .. offsets[i+1]) unchecked */
+        bool ok = offsets[0] == 0 && offsets[n_keys] == total_bytes;
+        for (int64_t i = 0; ok && i < n_keys; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % tb->L == 0;
+        if (!ok) {
+            acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes");
+            return ACB_EINVAL;
+        }
+    } else if (!lookup_stride_ok(tb, total_bytes, n_keys, stride_bytes)) {
+        acb_set_error("fixed-stride keys need stride_bytes >= 0, a multiple of letter_bytes, and n_keys*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    if (n_keys == 0) return ACB_OK;
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    int rc;
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_keys + 1))) return rc;
+    if ((rc = ensure(&tb->w_lk, &tb->w_lk_cap, 2 * (size_t)n_keys))) return rc;
+    cudaStream_t s = tb->stream;
+    if (total_bytes) CUDA_TRY(cudaMemcpyAsync(tb->w_hay, keys, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
+    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_keys + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+    rc = acb_lookup_device(tb, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_keys,
+                           stride_bytes, tb->w_lk, tb->w_lk + n_keys, s);
+    if (rc != ACB_OK) return rc;
+    CUDA_TRY(cudaMemcpyAsync(key_id, tb->w_lk, (size_t)n_keys * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(prefix, tb->w_lk + n_keys, (size_t)n_keys * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
     return ACB_OK;
 }
