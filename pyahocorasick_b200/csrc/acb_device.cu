@@ -155,7 +155,9 @@ __device__ __forceinline__ uint32_t load_word(const uint8_t *hay, long long a, l
     return v;
 }
 
-__device__ __forceinline__ void find_haystack(const ScanParams &p, long long q, long long &h, long long &hs, long long &he) {
+/* P: ScanParams, or the pair kernel's PairTurnArgs (the same fields, held in shared memory) */
+template <class P>
+__device__ __forceinline__ void find_haystack(const P &p, long long q, long long &h, long long &hs, long long &he) {
     if (p.offsets == nullptr) {
         if (p.stride_shift >= 0) h = q >> p.stride_shift;
         else if (p.total <= 0xffffffffLL) h = (long long)((uint32_t)q / (uint32_t)p.stride_bytes);
@@ -230,7 +232,8 @@ __device__ __forceinline__ void walk_from(const ScanParams &p, const WarpStage &
 }
 
 /* six aligned words covering the 20 text bytes from x on (zero fill past the end of the buffer) */
-__device__ __forceinline__ void load_text(const ScanParams &p, long long x, uint32_t (&w)[6]) {
+template <class P>
+__device__ __forceinline__ void load_text(const P &p, long long x, uint32_t (&w)[6]) {
     const long long x0 = x & ~3LL;
     if (x0 + 24 <= p.total) {
         const uint32_t *a = reinterpret_cast<const uint32_t *>(p.hay + x0);
@@ -778,8 +781,27 @@ constexpr int kPairRing = 64;                                /* candidate ring e
 constexpr int kPairItems = 64;                               /* item list entries (uint16 byte offsets in the slice) per consumer warp */
 static_assert(kPairRing >= 31 + 32, "a one-round slice must fit the ring next to a turn not yet resolved");
 
+/* The fields of ScanParams a resolve turn reads, copied to shared memory once per CTA.  pair_resolve is not inlined,
+ * so it would see the parameter block only through a generic pointer: every field a generic load (LD.E), several of
+ * them one after another on the turn's critical path.  From shared memory they are LDS.128 of 16-byte groups, in the
+ * order the turn needs them: the text and the anchor slot, attributing a hit, storing the records. */
+struct PairTurnArgs {
+    const uint8_t *hay;                                   /* group 0 */
+    long long total;
+    long long seg_begin;                                  /* group 1 */
+    const uint4 *anchors;
+    int logA, stride_shift, letter_shift, pad;            /* group 2 */
+    const long long *offsets;                             /* group 3 */
+    long long n_hay;
+    long long stride_bytes;                               /* group 4 */
+    long long cap;
+    acb_match *out;                                       /* group 5 */
+    unsigned long long *count;
+};
+static_assert(sizeof(PairTurnArgs) == 96, "PairTurnArgs is six 16-byte groups");
+
 struct PairSmem {
-    uint32_t bitmap, bitmap2, stages, ring, items, bars, tiles, next, total;
+    uint32_t bitmap, bitmap2, stages, ring, items, args, bars, tiles, next, total;
 };
 __host__ __device__ inline PairSmem pair_smem(int log1, int log2b) {
     PairSmem s;
@@ -791,8 +813,11 @@ __host__ __device__ inline PairSmem pair_smem(int log1, int log2b) {
     s.items = o;     o += (uint32_t)kPairConsumers * kPairItems * 2u;
     s.bars = o;      o += 2u * kPairStages * 8u;
     s.tiles = o;     o += (uint32_t)kPairStages * 4u;
-    s.next = o;      o += 4u;
-    s.total = (o + 15u) & ~15u;
+    s.next = o;      o += 4u;                                     o = (o + 15u) & ~15u;
+    /* last, so that pair_resolve finds it from the launch's dynamic shared memory size, without an argument (at offset
+       0 it moved the bitmap and the stages by 128 bytes, which cost the streaming skeleton 1.6 us per C2 launch) */
+    s.args = o;      o += (uint32_t)sizeof(PairTurnArgs);
+    s.total = o;
     return s;
 }
 
@@ -839,48 +864,76 @@ __device__ __noinline__ void pair_resolve_general(const ScanParams &p, long long
     }
 }
 
+/* groups [g0, g1) of the pair kernel's PairTurnArgs (the last bytes of its shared memory), loaded where the turn needs
+ * them: all of them at once would hold 24 registers through the turn, more than the streaming loop leaves a callee.
+ * The block is written once, before the kernel's first __syncthreads. */
+union PairTurnRegs {
+    uint4 v[sizeof(PairTurnArgs) / 16];
+    PairTurnArgs a;
+};
+__device__ __forceinline__ void load_turn_args(PairTurnRegs &u, int g0, int g1) {
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    uint32_t dyn;
+    asm("mov.u32 %0, %%dynamic_smem_size;" : "=r"(dyn));
+    const uint32_t saddr = (uint32_t)__cvta_generic_to_shared(smem_raw) + dyn - (uint32_t)sizeof(PairTurnArgs);
+#pragma unroll
+    for (int i = g0; i < g1; i++)
+        asm("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(u.v[i].x), "=r"(u.v[i].y), "=r"(u.v[i].z), "=r"(u.v[i].w) : "r"(saddr + 16u * i));
+}
+
 /* one turn of a warp's candidates (ring entries head .. head + n - 1, n <= 32, one per lane) through the anchor table.
- * Not inlined: the streaming loop keeps its registers and its schedule, and this runs once per five slices or so. */
+ * Not inlined: the streaming loop keeps its registers and its schedule, and this runs once per five slices or so.
+ * Its fields come from the PairTurnArgs in shared memory; `p` is only handed on to the general path. */
 __device__ __noinline__ void pair_resolve(const ScanParams &p, uint32_t sring, unsigned int head, unsigned int n) {
     const int lane = threadIdx.x & 31;
     const uint32_t lt_mask = (1u << lane) - 1u;
+    PairTurnRegs u;
+    const PairTurnArgs &a = u.a;
     bool hit = false;
     int32_t rh = 0, re = 0, rk = 0;
     if ((unsigned)lane < n) {
-        const uint32_t amask = (1u << p.logA) - 1u;
+        load_turn_args(u, 0, 3);
+        const uint32_t amask = (1u << a.logA) - 1u;
         const uint2 e = lds64(sring + (((head + (unsigned)lane) & (kPairRing - 1u)) << 3));
-        const long long q = p.seg_begin + (long long)e.x;
+        const long long q = a.seg_begin + (long long)e.x;
+        /* one round trip for both: the anchor slot and the text are issued before either is used */
+        uint32_t slot = e.y >> (32 - a.logA);
+        uint4 e0 = __ldg(a.anchors + 2 * (size_t)slot), e1 = __ldg(a.anchors + 2 * (size_t)slot + 1);
         uint32_t tq[6];
-        load_text(p, q, tq);
-        uint32_t slot = e.y >> (32 - p.logA);
-        uint4 e0 = __ldg(p.anchors + 2 * (size_t)slot), e1 = __ldg(p.anchors + 2 * (size_t)slot + 1);
+        load_text(a, q, tq);
         while (e0.x != 0u && e0.x != e.y) {                      /* a foreign tag in the way: linear probing */
             slot = (slot + 1) & amask;
-            e0 = __ldg(p.anchors + 2 * (size_t)slot);
-            e1 = __ldg(p.anchors + 2 * (size_t)slot + 1);
+            e0 = __ldg(a.anchors + 2 * (size_t)slot);
+            e1 = __ldg(a.anchors + 2 * (size_t)slot + 1);
         }
         if (e0.x != 0u) {
             if ((int32_t)e0.y >= 0 && (e0.z & 0x100ffu) == 0x10000u) {   /* the tag's ONE entry: UNIQUE, anchored at its first byte */
                 const uint32_t kw[5] = {e0.w, e1.x, e1.y, e1.z, e1.w};
                 const int len = (int)((e0.z >> 8) & 0xffu);
                 long long h, hs, he;
-                find_haystack(p, q, h, hs, he);
+                load_turn_args(u, 3, 5);
+                find_haystack(a, q, h, hs, he);
                 hit = q + len <= he && text_equals(tq, q, len, kw);
                 rh = (int32_t)h;
-                re = (int32_t)(((q + len - hs) >> p.letter_shift) - 1);
+                re = (int32_t)(((q + len - hs) >> a.letter_shift) - 1);
                 rk = (int32_t)e0.y;
             } else {
                 pair_resolve_general(p, q, e.y, slot, e0, e1);
             }
         }
     }
-    /* the hits of the warp: ONE atomicAdd on the record counter, records stored straight to the record buffer */
+    /* the hits of the warp: ONE atomic on the record counter, records stored straight to the record buffer (both
+       global-space operations: a.count and a.out are generic pointers to the compiler) */
+    load_turn_args(u, 4, 6);
     const unsigned mh = __ballot_sync(kFull, hit);
     if (mh) {
         unsigned long long base = 0;
-        if (lane == 0) base = atomicAdd(p.count, (unsigned long long)__popc(mh));
+        if (lane == 0)
+            asm volatile("atom.global.add.u64 %0, [%1], %2;" : "=l"(base) : "l"(__cvta_generic_to_global(a.count)), "l"((unsigned long long)__popc(mh)) : "memory");
         base = __shfl_sync(kFull, base, 0) + (unsigned long long)__popc(mh & lt_mask);
-        if (hit && base < (unsigned long long)p.cap) { acb_match m; m.hay_id = rh; m.end_index = re; m.key_id = rk; p.out[base] = m; }
+        if (hit && base < (unsigned long long)a.cap)
+            asm volatile("st.global.u32 [%0], %1;\n\tst.global.u32 [%0+4], %2;\n\tst.global.u32 [%0+8], %3;"   /* 12-byte records: 4-byte aligned */
+                         :: "l"(__cvta_generic_to_global(a.out + base)), "r"(rh), "r"(re), "r"(rk) : "memory");
     }
 }
 
@@ -931,6 +984,12 @@ __global__ void __launch_bounds__(kPairThreads, 1) acb_pair_kernel(const __grid_
 
     if (tid == 0) {
         *reinterpret_cast<unsigned int *>(smem_raw + lay.next) = 0u;
+        /* the resolve turn's fields (written in the consumers' prologue instead, the copy measured 0.9 us slower per C2 launch) */
+        PairTurnArgs &a = *reinterpret_cast<PairTurnArgs *>(smem_raw + lay.args);
+        a.hay = p.hay; a.total = p.total; a.seg_begin = p.seg_begin; a.anchors = p.anchors;
+        a.logA = p.logA; a.stride_shift = p.stride_shift; a.letter_shift = p.letter_shift; a.pad = 0;
+        a.offsets = p.offsets; a.n_hay = p.n_hay; a.stride_bytes = p.stride_bytes; a.cap = p.cap;
+        a.out = p.out; a.count = p.count;
         for (int s = 0; s < kPairStages; s++) {
             mbar_init(bar_full + 8u * s, 1);
             mbar_init(bar_empty + 8u * s, kPairTileSlices);
