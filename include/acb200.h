@@ -102,6 +102,15 @@ int64_t acb_trie_host_bytes(const acb_trie *t);    /* bytes of the node arena + 
  * the last, src/AutomatonItemsIter.c:125-288).  *n = number of live keys; ACB_EOVERFLOW when cap is smaller. */
 int acb_trie_key_order(const acb_trie *t, int32_t *out, int64_t cap, int64_t *n);
 
+/* That order as ranges over the flattened automaton (acb_trie_flat_view; ACB_ESTATE before it is built).  In a pre-order
+ * walk the keys at or under a node are one run, so for every state s that ends a whole letter (every state for 1-byte
+ * letters): the run is order[lo[s] .. lo[s] + cnt[s]) -- the node's own key first, if it ends one -- and its
+ * letter-children are child[child_ptr[s] .. child_ptr[s+1]), youngest first, which is by ascending lo.  States inside a
+ * letter have cnt 0 and no children.  Sizes: order acb_trie_count(t); lo, cnt n_states; child_ptr n_states + 1; child
+ * n_states (always enough); *n_edges = the entries of child used. */
+int acb_trie_key_ranges(const acb_trie *t, int32_t *order, int32_t *lo, int32_t *cnt, int32_t *child_ptr, int32_t *child,
+                        int64_t *n_edges);
+
 /* Read-only view of the flattened automaton (valid until the trie changes).
  * State ids are BFS order, root = 0.  Used for upload and for white-box tests. */
 typedef struct acb_flat_view {
@@ -372,6 +381,38 @@ int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t total_bytes,
  * ACB_ECUDA (there is no CPU fallback). */
 int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total_bytes, const int64_t *offsets,
                     int64_t n_keys, int64_t stride_bytes, int32_t *key_id, int32_t *prefix);
+
+/* ---- dictionary selection: keys / values / items (prefix, wildcard, how) for many patterns at once ------------------
+ * The ranges of acb_trie_key_ranges go to the device once, before the first select call: t is the trie the table was
+ * uploaded from, unchanged since.  A repeated call returns at once; the table frees them.  About 12 bytes per state plus
+ * 4 per key and per letter edge.  The scans and lookups do not need them. */
+int acb_table_upload_key_ranges(acb_table *tb, const acb_trie *t);
+
+/* how, as the reference's MATCH_* constants (src/AutomatonItemsIter.h) */
+#define ACB_MATCH_EXACT_LENGTH     0
+#define ACB_MATCH_AT_MOST_PREFIX   1
+#define ACB_MATCH_AT_LEAST_PREFIX  2
+
+/* keys(pattern, wildcard, how) (src/AutomatonItemsIter.c:125-288) for n patterns at once: the ids of pattern i's keys
+ * are key_id[out_offsets[i] .. out_offsets[i+1]), in the order acb_trie_key_order gives them.  wildcard: a letter value
+ * that matches any letter, or -1 for none; without one, `how` is ignored and the keys are those that start with the
+ * pattern (the reference's prefix query).  With one, how = EXACT_LENGTH: keys of the pattern's length that match it
+ * letter by letter; AT_MOST_PREFIX: keys that match a prefix of the pattern; AT_LEAST_PREFIX: keys whose prefix matches
+ * the pattern.  Patterns are laid out as acb_lookup_device's keys (no alignment needed).  ACB_ESTATE before
+ * acb_table_upload_key_ranges.
+ *
+ * DEVICE buffers, asynchronous on `stream`: d_out_offsets (n+1 int64) and *d_total are always written; d_key_id only
+ * when the total is at most cap (the kernel checks it on the device).  Two passes: one counts the keys of every
+ * pattern, an exclusive scan gives the offsets, the other writes the ids.  d_offsets is not checked. */
+int acb_select_device(acb_table *tb, const uint8_t *d_patterns, int64_t total_bytes, const int64_t *d_offsets, int64_t n,
+                      int64_t stride_bytes, int64_t wildcard, int how, int64_t *d_out_offsets, int32_t *d_key_id,
+                      int64_t cap, int64_t *d_total, void *stream);
+
+/* HOST buffers, synchronous.  The offsets and the arguments are checked (ACB_EINVAL) before anything runs.  out_offsets
+ * and *total are always written; key_id when *total <= cap, else ACB_EOVERFLOW.  Without a device: ACB_ECUDA. */
+int acb_select_host(acb_table *tb, const uint8_t *patterns, int64_t total_bytes, const int64_t *offsets, int64_t n,
+                    int64_t stride_bytes, int64_t wildcard, int how, int64_t *out_offsets, int32_t *key_id, int64_t cap,
+                    int64_t *total);
 
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);

@@ -71,6 +71,7 @@ def lib() -> ctypes.CDLL:
         "acb_trie_links": (i64, [vp]),
         "acb_trie_host_bytes": (i64, [vp]),
         "acb_trie_key_order": (ctypes.c_int, [vp, vp, i64, pi64]),
+        "acb_trie_key_ranges": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, pi64]),
         "acb_trie_content_hash": (ctypes.c_uint64, [vp]),
         "acb_trie_flat_save": (ctypes.c_int, [vp, vp, i64, ctypes.POINTER(i64)]),
         "acb_trie_flat_load": (ctypes.c_int, [vp, vp, i64]),
@@ -104,6 +105,9 @@ def lib() -> ctypes.CDLL:
         "acb_last_skip_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]),
         "acb_lookup_device": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, vp, vp]),
         "acb_lookup_host": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, vp]),
+        "acb_table_upload_key_ranges": (ctypes.c_int, [vp, vp]),
+        "acb_select_device": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, i64, ctypes.c_int, vp, vp, i64, vp, vp]),
+        "acb_select_host": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, i64, ctypes.c_int, vp, vp, i64, pi64]),
         "acb_launch_count": (i64, []),
         "acb_set_kernel_timing": (ctypes.c_int, [ctypes.c_int]),
         "acb_last_kernel_ms": (ctypes.c_float, []),
@@ -124,14 +128,15 @@ def lib() -> ctypes.CDLL:
 EXPORTED_SYMBOLS = [
     "acb_trie_new", "acb_trie_free", "acb_trie_clear", "acb_trie_add_word", "acb_trie_remove_word",
     "acb_trie_find", "acb_trie_longest_prefix", "acb_trie_make_automaton", "acb_trie_kind",
-    "acb_trie_count", "acb_trie_longest_word", "acb_trie_nodes", "acb_trie_links", "acb_trie_host_bytes", "acb_trie_key_order", "acb_trie_flat_view",
+    "acb_trie_count", "acb_trie_longest_word", "acb_trie_nodes", "acb_trie_links", "acb_trie_host_bytes", "acb_trie_key_order", "acb_trie_key_ranges", "acb_trie_flat_view",
     "acb_trie_content_hash", "acb_trie_flat_save", "acb_trie_flat_load",
     "acb_trie_export_nodes", "acb_trie_import_nodes", "acb_node_records_span",
     "acb_device_count", "acb_table_upload", "acb_table_free", "acb_table_device_bytes",
     "acb_scan_device", "acb_scan_host", "acb_copy_records", "acb_take_records", "acb_release_records", "acb_sort_matches_device", "acb_table_set_long_state", "acb_table_get_long_state",
     "acb_streams_new", "acb_streams_free", "acb_streams_reset", "acb_streams_feed_device", "acb_streams_feed_host",
     "acb_streams_positions", "acb_space_letters", "acb_scan_device_skip", "acb_scan_host_skip", "acb_streams_new_skip",
-    "acb_last_skip_ms", "acb_lookup_device", "acb_lookup_host", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_last_skip_ms", "acb_lookup_device", "acb_lookup_host", "acb_table_upload_key_ranges", "acb_select_device",
+    "acb_select_host", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

@@ -402,8 +402,9 @@ class Automaton:
         self._version += 1
         self._drop_table()
 
-    # keys / values / items (src/AutomatonItemsIter.c) -- host-only enumeration
-    def _select(self, args):
+    # keys / values / items (src/AutomatonItemsIter.c) -- host enumeration; keys_batch & co. run on the GPU
+    def _select_args(self, args):
+        """(prefix or None, wildcard letter value or None, how) of keys / values / items, checked in this order"""
         prefix = None
         wildcard = None
         how = MATCH_EXACT_LENGTH
@@ -411,15 +412,19 @@ class Automaton:
             prefix = args[0]
             self._letters(prefix)
         if len(args) >= 2 and args[1] is not None:
-            wildcard = args[1]
-            wl = self._letters(wildcard)
+            wl = self._letters(args[1])
             if len(wl) != 1:
                 raise ValueError("Wildcard must be a single character.")
+            wildcard = int(wl[0])
         if len(args) >= 3:
             how = args[2]
             if how not in (MATCH_EXACT_LENGTH, MATCH_AT_MOST_PREFIX, MATCH_AT_LEAST_PREFIX):
                 raise ValueError("The optional how third argument must be one of: "
                                  "MATCH_EXACT_LENGTH, MATCH_AT_LEAST_PREFIX or MATCH_AT_LEAST_PREFIX")
+        return prefix, wildcard, how
+
+    def _select(self, args):
+        prefix, w, how = self._select_args(args)
         version = self._version
         # the reference's order: a pre-order walk of the trie that takes a node's youngest child first
         # (src/AutomatonItemsIter.c:125-288); the host trie knows it (acb_trie_key_order)
@@ -433,7 +438,6 @@ class Automaton:
             sel = live
         else:
             p = list(self._letters(prefix).tolist())
-            w = None if wildcard is None else int(self._letters(wildcard)[0])
             sel = []
             for k, v in live:
                 kl = self._letters(k).tolist()
@@ -1124,6 +1128,109 @@ class Automaton:
             except UnicodeDecodeError:                          # letters beyond U+10FFFF: no str holds them
                 return raw
         return raw
+
+    # ------------------------------------------------------------------ batch keys / values / items (new)
+    # keys(pattern, wildcard, how) for a whole batch of patterns, in one GPU call (acb_select_*).  `patterns` takes the
+    # input forms of find_all_batch; wildcard and how are those of keys() and apply to every pattern.  The walk runs on
+    # the full table, as the lookups do: the latin-1 table lacks the nodes of keys that are not latin-1.
+    def keys_batch(self, patterns, wildcard=None, how=MATCH_EXACT_LENGTH, *, device: Optional[int] = None) -> list:
+        """``[list(A.keys(p, wildcard, how)) for p in patterns]``, read when the call returns."""
+        ko = self._key_objs
+        return [list(map(ko.__getitem__, ids)) for ids in self._select_lists(patterns, wildcard, how, device)]
+
+    def values_batch(self, patterns, wildcard=None, how=MATCH_EXACT_LENGTH, *, device: Optional[int] = None) -> list:
+        """``[list(A.values(p, wildcard, how)) for p in patterns]``, read when the call returns."""
+        vals = self._values
+        return [list(map(vals.__getitem__, ids)) for ids in self._select_lists(patterns, wildcard, how, device)]
+
+    def items_batch(self, patterns, wildcard=None, how=MATCH_EXACT_LENGTH, *, device: Optional[int] = None) -> list:
+        """``[list(A.items(p, wildcard, how)) for p in patterns]``, read when the call returns."""
+        ko, vals = self._key_objs, self._values
+        return [[(ko[k], vals[k]) for k in ids] for ids in self._select_lists(patterns, wildcard, how, device)]
+
+    def _select_lists(self, patterns, wildcard, how, device):
+        """the key ids of every pattern, as lists"""
+        offs, key_id = self.select_batch(patterns, wildcard, how, device=device)
+        if not isinstance(key_id, np.ndarray):
+            offs, key_id = offs.cpu().numpy(), key_id.cpu().numpy()
+        ids = key_id.tolist()
+        bounds = offs.tolist()
+        return [ids[bounds[i]:bounds[i + 1]] for i in range(len(bounds) - 1)]
+
+    @_locked
+    def select_batch(self, patterns, wildcard=None, how=MATCH_EXACT_LENGTH, *, device: Optional[int] = None):
+        """The keys of every pattern as (offsets int64[n+1], key_id int32[m]): the ids of the keys that
+        ``A.keys(patterns[i], wildcard, how)`` yields are ``key_id[offsets[i]:offsets[i+1]]``, in its order.  numpy
+        arrays for a host batch; for a CUDA tensor batch, CUDA tensors computed on torch's current stream.  The size of
+        the output depends on the data, so the call synchronises once to learn it.  Arguments are checked as keys()
+        checks them: the first pattern, then wildcard, then how, then the other patterns."""
+        self._require_automaton()
+        flat_pair = isinstance(patterns, tuple) and len(patterns) == 2 and all(isinstance(x, np.ndarray) for x in patterns)
+        first = patterns[0] if isinstance(patterns, (list, tuple)) and patterns and not flat_pair else None
+        _, w, how = self._select_args((first, wildcard, how))
+        w = -1 if w is None else w
+        batch = self._batch_input(patterns, narrow_ok=False, required=False)
+        if batch[0] == "device":
+            return self._select_device(batch[1], w, how)
+        _, flat, offs, n, stride, _ = batch
+        return self._select_host(flat, offs, n, stride, w, how, device)
+
+    def _select_device(self, t, wildcard: int, how: int):
+        import torch
+        n, stride = self._device_batch_shape(t)
+        out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+        total = torch.empty(1, dtype=torch.int64, device=t.device)
+        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        tb = self._select_table(dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream().cuda_stream
+            args = (tb, t.data_ptr() if n * stride else None, n * stride, None, n, stride, wildcard, how, out_offs.data_ptr())
+            N.check(self._lib.acb_select_device(*args, None, 0, total.data_ptr(), stream))
+            m = int(total.item())                               # the one synchronisation: the size of the output
+            key_id = torch.empty(m, dtype=torch.int32, device=t.device)
+            if m:
+                N.check(self._lib.acb_select_device(*args, key_id.data_ptr(), m, total.data_ptr(), stream))
+        return out_offs, key_id
+
+    def _select_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n: int, stride_bytes: int, wildcard: int,
+                     how: int, device: Optional[int]):
+        """acb_select_host over a host batch -> (offsets int64[n+1], key_id int32[m])"""
+        out_offs = np.zeros(n + 1, dtype=np.int64)
+        if n == 0:
+            return out_offs, np.empty(0, dtype=np.int32)
+        tb = self._select_table(device)
+        total = ctypes.c_int64(0)
+        args = (tb, N.ptr(flat) if flat.size else None, int(flat.size), N.ptr(offsets) if offsets is not None else None,
+                n, stride_bytes, wildcard, how, N.ptr(out_offs))
+        rc = self._lib.acb_select_host(*args, None, 0, ctypes.byref(total))
+        if rc == N.ACB_EOVERFLOW:                               # the ids are written by a second call of the right size
+            key_id = np.empty(total.value, dtype=np.int32)
+            rc = self._lib.acb_select_host(*args, N.ptr(key_id), total.value, ctypes.byref(total))
+        else:
+            key_id = np.empty(0, dtype=np.int32)
+        N.check(rc)
+        return out_offs, key_id
+
+    def _select_table(self, device: Optional[int]):
+        """the full table of `device`, with the key ranges of the select calls on it"""
+        tb = self._ensure_table(device)
+        N.check(self._lib.acb_table_upload_key_ranges(tb, self._trie))
+        return tb
+
+    @_locked
+    def key_ranges(self) -> dict:
+        """White-box view of the key order as ranges over the flat tables (acb_trie_key_ranges), numpy copies: order
+        (key ids in keys() order), lo / cnt per state, child_ptr / child (letter-children, youngest first)."""
+        fv = N.FlatView()
+        N.check(self._lib.acb_trie_flat_view(self._trie, ctypes.byref(fv)))
+        S = fv.n_states
+        order = np.empty(max(len(self), 1), dtype=np.int32)
+        lo, cnt, child = (np.empty(S, dtype=np.int32) for _ in range(3))
+        child_ptr = np.empty(S + 1, dtype=np.int32)
+        e = ctypes.c_int64(0)
+        N.check(self._lib.acb_trie_key_ranges(self._trie, N.ptr(order), N.ptr(lo), N.ptr(cnt), N.ptr(child_ptr),
+                                              N.ptr(child), ctypes.byref(e)))
+        return dict(order=order[:len(self)], lo=lo, cnt=cnt, child_ptr=child_ptr, child=child[:e.value])
 
 
 class StreamBatch:

@@ -35,6 +35,7 @@
 
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -1365,6 +1366,12 @@ struct acb_table {
     cudaEvent_t k_t0 = nullptr, k_t1 = nullptr;          /* kernel timing of the compaction and the remap */
     /* workspace of acb_lookup_host (keys and offsets go to w_hay / w_off) */
     int32_t *w_lk = nullptr; size_t w_lk_cap = 0;        /* key_id[n] then prefix[n] */
+    /* dictionary view of the select calls (acb_table_upload_key_ranges), uploaded on first use */
+    int32_t *d_order = nullptr, *d_lo = nullptr, *d_cnt = nullptr, *d_child_ptr = nullptr, *d_child = nullptr;
+    /* workspace of the select calls */
+    uint8_t *w_scan = nullptr; size_t w_scan_cap = 0;    /* the offsets' prefix sum */
+    long long *w_sel_off = nullptr; size_t w_sel_off_cap = 0;   /* acb_select_host: out offsets[n+1] then the total */
+    int32_t *w_sel_id = nullptr; size_t w_sel_id_cap = 0;       /* acb_select_host: key ids */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1405,6 +1412,8 @@ extern "C" void acb_table_free(acb_table *tb) {
     cudaFree(tb->k_buf); cudaFree(tb->k_mask); cudaFree(tb->k_gpre); cudaFree(tb->k_tile_pre); cudaFree(tb->k_status);
     cudaFree(tb->k_coff); cudaFree(tb->k_set); cudaFree(tb->k_ctr);
     cudaFree(tb->w_lk);
+    cudaFree(tb->d_order); cudaFree(tb->d_lo); cudaFree(tb->d_cnt); cudaFree(tb->d_child_ptr); cudaFree(tb->d_child);
+    cudaFree(tb->w_scan); cudaFree(tb->w_sel_off); cudaFree(tb->w_sel_id);
     if (tb->h_kept) cudaFreeHost(tb->h_kept);
     if (tb->k_done) cudaEventDestroy(tb->k_done);
     if (tb->k_t0) cudaEventDestroy(tb->k_t0);
@@ -2757,6 +2766,13 @@ struct LookupParams {
     int32_t *key_id, *prefix;
 };
 
+/* one byte of the dictionary walks: the child of state s along `byte`, or -1.  Class 0 needs no test: its column is all
+ * -1 unless K == 256, when it is a real byte.  The goto table can pass 2^31 entries, hence the 64-bit index. */
+__device__ __forceinline__ int32_t trie_step(const int32_t *gto, const uint8_t *cls, long long S, uint8_t byte, int32_t s) {
+    const int32_t nx = __ldg(gto + (long long)cls[byte] * S + s);
+    return nx < 0 ? -1 : (nx & kIdMask);           /* drop kTermBit */
+}
+
 __global__ void __launch_bounds__(kLookupThreads) acb_lookup_kernel(const __grid_constant__ LookupParams p) {
     __shared__ uint8_t cls[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) cls[i] = p.cls[i];
@@ -2766,10 +2782,10 @@ __global__ void __launch_bounds__(kLookupThreads) acb_lookup_kernel(const __grid
         const long long b1 = p.offsets ? __ldg(p.offsets + q + 1) : b0 + p.stride;
         int32_t s = 0;
         long long i = b0;
-        for (; i < b1; ++i) {                      /* class 0 needs no test: its column is all -1 unless K == 256 */
-            const int32_t nx = __ldg(p.gto + (long long)cls[__ldg(p.keys + i)] * p.S + s);
+        for (; i < b1; ++i) {
+            const int32_t nx = trie_step(p.gto, cls, p.S, __ldg(p.keys + i), s);
             if (nx < 0) break;
-            s = nx & kIdMask;                      /* drop kTermBit */
+            s = nx;
         }
         p.key_id[q] = (i == b1 && b1 > b0) ? __ldg(p.key_of + s) : -1;
         p.prefix[q] = (int32_t)((i - b0) >> p.letter_shift);   /* whole letters only; at most the longest key */
@@ -2854,6 +2870,314 @@ extern "C" int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total
     if (rc != ACB_OK) return rc;
     CUDA_TRY(cudaMemcpyAsync(key_id, tb->w_lk, (size_t)n_keys * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(prefix, tb->w_lk + n_keys, (size_t)n_keys * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return ACB_OK;
+}
+
+/* ------------------------------------------------------------ dictionary selection */
+/* keys / values / items (prefix, wildcard, how) for a whole batch of patterns (src/AutomatonItemsIter.c:125-288).  The
+ * reference walks the trie under the pattern with a stack, youngest child first.  In that pre-order the keys at or
+ * under a node are one run of the key order, order[lo[s] .. lo[s] + cnt[s]), and a node's letter-children sorted by lo
+ * are the order its stack pops them (acb_trie_key_ranges).  One lane per pattern:
+ *  - without a wildcard the query is one walk down the goto table and one run;
+ *  - with one, the lane walks the tree of nodes the pattern can reach depth first, taking the children of a wildcard
+ *    letter from the child list.  It emits keys in rank order, so no sort is needed.
+ * The walk is driven by a rank cursor r (every key of rank < r is dealt with).  At every node the lane takes the first
+ * child that can still match and whose run ends after r: the goto child for a plain letter, a binary search by lo in
+ * the child list for a wildcard.  A node without one is done; r moves to the end of its run and the lane goes back to
+ * its parent.  The lane keeps the last kSelectPath nodes of its path; a deeper parent is found again by the same
+ * descent from the deepest one kept, since the cursor leads it to the same node.  So there is no limit on the length
+ * of a pattern or on its wildcard letters. */
+namespace {
+constexpr int kSelectThreads = 128;
+constexpr int kSelectPath = 16;
+
+struct SelectParams {
+    const uint8_t *pat;
+    const long long *offsets;      /* nullptr => fixed stride */
+    long long n, stride;
+    const uint8_t *cls;
+    const int32_t *gto;            /* flagged goto (kTermBit) */
+    long long S;
+    const int32_t *key_of, *order, *lo, *cnt, *child_ptr, *child;
+    long long wildcard;            /* letter value, -1: none */
+    int32_t how, L;
+    long long *out_off;            /* pass 1: the count of pattern q goes to [q + 1]; pass 2: its slice starts at [q] */
+    int32_t *key_id;
+    const long long *total;        /* pass 2 writes nothing when *total > cap */
+    long long cap;
+};
+
+/* the state one whole letter below s, or -1 */
+__device__ __forceinline__ int32_t select_letter(const SelectParams &p, const uint8_t *cls, const uint8_t *b, int32_t s) {
+    for (int d = 0; d < p.L && s >= 0; ++d) s = trie_step(p.gto, cls, p.S, __ldg(b + d), s);
+    return s;
+}
+
+/* the keys of one pattern of m letters at pat: counted, or (kWrite) their ids written to out; returns the count */
+template <bool kWrite>
+__device__ long long select_walk(const SelectParams &p, const uint8_t *cls, const uint8_t *pat, long long m, int32_t *out) {
+    long long n_out = 0;
+    auto emit = [&](int32_t r0, int32_t r1) {                  /* the keys of ranks r0 .. r1 */
+        if (kWrite)
+            for (int32_t r = r0; r < r1; ++r) out[n_out + (r - r0)] = __ldg(p.order + r);
+        n_out += r1 - r0;
+    };
+    if (p.wildcard < 0) {                                      /* every key that starts with the pattern */
+        int32_t x = 0;
+        for (long long j = 0; j < m && x >= 0; ++j) x = select_letter(p, cls, pat + j * p.L, x);
+        if (x >= 0) {
+            const int32_t xlo = __ldg(p.lo + x);
+            emit(xlo, xlo + __ldg(p.cnt + x));
+        }
+        return n_out;
+    }
+    int32_t path[kSelectPath];                                 /* path[j]: the node at depth j, for j < kSelectPath */
+    path[0] = 0;
+    int32_t x = 0, r = 0;
+    long long j = 0;
+    for (;;) {
+        const int32_t xlo = __ldg(p.lo + x), xend = xlo + __ldg(p.cnt + x);
+        /* the node's own key has rank xlo; ranks below r were emitted or rejected before */
+        if (j > 0 && xlo >= r && (p.how == ACB_MATCH_AT_MOST_PREFIX || (p.how == ACB_MATCH_EXACT_LENGTH && j == m)) &&
+            __ldg(p.key_of + x) >= 0) {
+            emit(xlo, xlo + 1);
+            r = xlo + 1;
+        }
+        int32_t c = -1;
+        if (j == m) {
+            if (p.how == ACB_MATCH_AT_LEAST_PREFIX) emit(max(r, xlo), xend);
+        } else {
+            const uint8_t *b = pat + j * p.L;
+            uint32_t letter = 0;
+            for (int d = 0; d < p.L; ++d) letter |= (uint32_t)__ldg(b + d) << (8 * d);
+            if ((long long)letter == p.wildcard) {             /* the first child whose run ends after r */
+                const int32_t c0 = __ldg(p.child_ptr + x), c1 = __ldg(p.child_ptr + x + 1);
+                int32_t a = c0, z = c1;                        /* a: the first child with lo > r */
+                while (a < z) {
+                    const int32_t mid = (a + z) >> 1;
+                    if (__ldg(p.lo + __ldg(p.child + mid)) > r) z = mid; else a = mid + 1;
+                }
+                if (a > c0) {
+                    const int32_t y = __ldg(p.child + a - 1);
+                    if (__ldg(p.lo + y) + __ldg(p.cnt + y) > r) c = y;
+                }
+                if (c < 0 && a < c1) c = __ldg(p.child + a);
+            } else {                                           /* a letter walked in part matches nothing */
+                c = select_letter(p, cls, b, x);
+                if (c >= 0 && __ldg(p.lo + c) + __ldg(p.cnt + c) <= r) c = -1;
+            }
+        }
+        if (c < 0) {                                           /* x is done: back to its parent */
+            r = max(r, xend);
+            if (j == 0) break;
+            j = min(j - 1, (long long)kSelectPath - 1);
+            x = path[j];
+            continue;
+        }
+        x = c;
+        if (++j < kSelectPath) path[j] = x;
+    }
+    return n_out;
+}
+
+template <bool kWrite>
+__global__ void __launch_bounds__(kSelectThreads) acb_select_kernel(const __grid_constant__ SelectParams p) {
+    __shared__ uint8_t cls[256];
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) cls[i] = p.cls[i];
+    __syncthreads();
+    if (kWrite && *p.total > p.cap) return;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < p.n; q += (long long)gridDim.x * blockDim.x) {
+        const long long b0 = p.offsets ? __ldg(p.offsets + q) : q * p.stride;
+        const long long b1 = p.offsets ? __ldg(p.offsets + q + 1) : b0 + p.stride;
+        const long long m = (b1 - b0) / p.L;
+        if (kWrite) select_walk<true>(p, cls, p.pat + b0, m, p.key_id + p.out_off[q]);
+        else p.out_off[q + 1] = select_walk<false>(p, cls, p.pat + b0, m, nullptr);
+    }
+}
+} // namespace
+
+extern "C" int acb_table_upload_key_ranges(acb_table *tb, const acb_trie *t) {
+    if (!tb || !t) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (tb->d_order) return ACB_OK;
+    acb_flat_view f;
+    int rc = acb_trie_flat_view(t, &f);
+    if (rc != ACB_OK) return rc;
+    if (f.n_states != tb->S || f.n_keys != tb->n_keys || f.letter_bytes != tb->L) {
+        acb_set_error("the trie is not the one this table was uploaded from");
+        return ACB_EINVAL;
+    }
+    const size_t S = (size_t)f.n_states, n_live = (size_t)acb_trie_count(t);
+    std::vector<int32_t> order, lo, cnt, child_ptr, child;
+    try {
+        order.resize(std::max<size_t>(n_live, 1)); lo.resize(S); cnt.resize(S); child_ptr.resize(S + 1); child.resize(S);
+    } catch (const std::exception &) {
+        acb_set_error("out of host memory while staging the key ranges");
+        return ACB_ENOMEM;
+    }
+    int64_t n_edges = 0;
+    if ((rc = acb_trie_key_ranges(t, order.data(), lo.data(), cnt.data(), child_ptr.data(), child.data(), &n_edges))) return rc;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    do {
+        if ((rc = upload(&tb->d_lo, lo.data(), S, tb->dev_bytes))) break;
+        if ((rc = upload(&tb->d_cnt, cnt.data(), S, tb->dev_bytes))) break;
+        if ((rc = upload(&tb->d_child_ptr, child_ptr.data(), S + 1, tb->dev_bytes))) break;
+        if ((rc = upload(&tb->d_child, child.data(), (size_t)n_edges, tb->dev_bytes))) break;
+        rc = upload(&tb->d_order, order.data(), n_live, tb->dev_bytes);   /* last: it marks the view complete */
+    } while (0);
+    if (rc != ACB_OK) {
+        cudaFree(tb->d_lo); cudaFree(tb->d_cnt); cudaFree(tb->d_child_ptr); cudaFree(tb->d_child); cudaFree(tb->d_order);
+        tb->d_lo = tb->d_cnt = tb->d_child_ptr = tb->d_child = tb->d_order = nullptr;
+    }
+    return rc;
+}
+
+static int select_args_ok(const acb_table *tb, int64_t wildcard, int how) {
+    if (how != ACB_MATCH_EXACT_LENGTH && how != ACB_MATCH_AT_MOST_PREFIX && how != ACB_MATCH_AT_LEAST_PREFIX) {
+        acb_set_error("how must be ACB_MATCH_EXACT_LENGTH, ACB_MATCH_AT_MOST_PREFIX or ACB_MATCH_AT_LEAST_PREFIX");
+        return ACB_EINVAL;
+    }
+    if (wildcard < -1 || wildcard >= ((int64_t)1 << (8 * tb->L))) {
+        acb_set_error("wildcard must be -1 or a %d-byte letter value", tb->L);
+        return ACB_EINVAL;
+    }
+    return ACB_OK;
+}
+
+static void fill_select_params(const acb_table *tb, SelectParams &p, const uint8_t *d_pat, const int64_t *d_offsets,
+                               int64_t n, int64_t stride, int64_t wildcard, int how, int64_t *d_out_off,
+                               int32_t *d_key_id, int64_t cap, const int64_t *d_total) {
+    p.pat = d_pat; p.offsets = reinterpret_cast<const long long *>(d_offsets); p.n = n; p.stride = stride;
+    p.cls = tb->d_cls; p.gto = tb->d_goto; p.S = tb->S;
+    p.key_of = tb->d_keyof; p.order = tb->d_order; p.lo = tb->d_lo; p.cnt = tb->d_cnt;
+    p.child_ptr = tb->d_child_ptr; p.child = tb->d_child;
+    p.wildcard = wildcard; p.how = how; p.L = tb->L;
+    p.out_off = reinterpret_cast<long long *>(d_out_off); p.key_id = d_key_id;
+    p.total = reinterpret_cast<const long long *>(d_total); p.cap = cap;
+}
+
+/* pass 1 and the scan: d_out_off[0..n] and *d_total, on s */
+static int select_count(acb_table *tb, const SelectParams &p, int64_t n, int64_t *d_out_off, int64_t *d_total, cudaStream_t s) {
+    CUDA_TRY(cudaMemsetAsync(d_out_off, 0, sizeof(int64_t), s));
+    if (n == 0) {
+        CUDA_TRY(cudaMemsetAsync(d_total, 0, sizeof(int64_t), s));
+        return ACB_OK;
+    }
+    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, (long long)tb->sm_count * 16);
+    acb_select_kernel<false><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { acb_set_error("select kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
+    g_launches.fetch_add(1);
+    long long *cnt = reinterpret_cast<long long *>(d_out_off) + 1;     /* in place: counts -> inclusive sums */
+    size_t temp = 0;
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, temp, cnt, cnt, (long long)n, s));
+    int rc;
+    if ((rc = ensure(&tb->w_scan, &tb->w_scan_cap, temp))) return rc;
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(tb->w_scan, temp, cnt, cnt, (long long)n, s));
+    CUDA_TRY(cudaMemcpyAsync(d_total, d_out_off + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+    return ACB_OK;
+}
+
+/* pass 2: the ids, when *p.total <= p.cap */
+static int select_fill(acb_table *tb, const SelectParams &p, int64_t n, cudaStream_t s) {
+    if (n == 0 || p.cap == 0) return ACB_OK;
+    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, (long long)tb->sm_count * 16);
+    acb_select_kernel<true><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { acb_set_error("select kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
+    g_launches.fetch_add(1);
+    return ACB_OK;
+}
+
+static int select_common_checks(const acb_table *tb, const void *pat, int64_t total_bytes, int64_t n, const void *out_off,
+                                const void *key_id, int64_t cap, const void *total, int64_t wildcard, int how) {
+    if (!tb || total_bytes < 0 || n < 0 || (total_bytes && !pat) || !out_off || !total || cap < 0 || (cap && !key_id)) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    return select_args_ok(tb, wildcard, how);
+}
+
+static int select_view_ok(const acb_table *tb) {
+    if (tb->d_order) return ACB_OK;
+    acb_set_error("the key ranges are not on the device yet (acb_table_upload_key_ranges)");
+    return ACB_ESTATE;
+}
+
+extern "C" int acb_select_device(acb_table *tb, const uint8_t *d_patterns, int64_t total_bytes, const int64_t *d_offsets,
+                                 int64_t n, int64_t stride_bytes, int64_t wildcard, int how, int64_t *d_out_offsets,
+                                 int32_t *d_key_id, int64_t cap, int64_t *d_total, void *stream) {
+    int rc = select_common_checks(tb, d_patterns, total_bytes, n, d_out_offsets, d_key_id, cap, d_total, wildcard, how);
+    if (rc != ACB_OK) return rc;
+    if (!d_offsets && !lookup_stride_ok(tb, total_bytes, n, stride_bytes)) {
+        acb_set_error("fixed-stride patterns need stride_bytes >= 0, a multiple of letter_bytes, and n*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    if ((rc = select_view_ok(tb))) return rc;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    SelectParams p;
+    fill_select_params(tb, p, d_patterns, d_offsets, n, stride_bytes, wildcard, how, d_out_offsets, d_key_id, cap, d_total);
+    const bool timing = g_timing.load() != 0;
+    if (timing) {
+        if (!tb->ev0) { CUDA_TRY(cudaEventCreate(&tb->ev0)); CUDA_TRY(cudaEventCreate(&tb->ev1)); }
+        CUDA_TRY(cudaEventRecord(tb->ev0, s));
+    }
+    if ((rc = select_count(tb, p, n, d_out_offsets, d_total, s))) return rc;
+    if ((rc = select_fill(tb, p, n, s))) return rc;
+    if (timing) {
+        CUDA_TRY(cudaEventRecord(tb->ev1, s));
+        CUDA_TRY(cudaEventSynchronize(tb->ev1));
+        float ms = 0.f;
+        CUDA_TRY(cudaEventElapsedTime(&ms, tb->ev0, tb->ev1));
+        g_last_ms = ms;
+    }
+    return ACB_OK;
+}
+
+extern "C" int acb_select_host(acb_table *tb, const uint8_t *patterns, int64_t total_bytes, const int64_t *offsets,
+                               int64_t n, int64_t stride_bytes, int64_t wildcard, int how, int64_t *out_offsets,
+                               int32_t *key_id, int64_t cap, int64_t *total) {
+    int rc = select_common_checks(tb, patterns, total_bytes, n, out_offsets, key_id, cap, total, wildcard, how);
+    if (rc != ACB_OK) return rc;
+    if (offsets) {                                  /* the kernels read patterns[offsets[i] .. offsets[i+1]) unchecked */
+        bool ok = offsets[0] == 0 && offsets[n] == total_bytes;
+        for (int64_t i = 0; ok && i < n; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % tb->L == 0;
+        if (!ok) {
+            acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes");
+            return ACB_EINVAL;
+        }
+    } else if (!lookup_stride_ok(tb, total_bytes, n, stride_bytes)) {
+        acb_set_error("fixed-stride patterns need stride_bytes >= 0, a multiple of letter_bytes, and n*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    if ((rc = select_view_ok(tb))) return rc;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n + 1))) return rc;
+    if ((rc = ensure(&tb->w_sel_off, &tb->w_sel_off_cap, (size_t)n + 2))) return rc;
+    cudaStream_t s = tb->stream;
+    if (total_bytes) CUDA_TRY(cudaMemcpyAsync(tb->w_hay, patterns, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
+    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+    int64_t *d_out = reinterpret_cast<int64_t *>(tb->w_sel_off), *d_total = d_out + n + 1;
+    SelectParams p;
+    fill_select_params(tb, p, tb->w_hay, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n, stride_bytes,
+                       wildcard, how, d_out, nullptr, 0, d_total);
+    if ((rc = select_count(tb, p, n, d_out, d_total, s))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(out_offsets, d_out, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    *total = out_offsets[n];
+    if (*total > cap) {
+        acb_set_error("select: room for %lld ids, %lld selected", (long long)cap, (long long)*total);
+        return ACB_EOVERFLOW;
+    }
+    if (*total == 0) return ACB_OK;
+    if ((rc = ensure(&tb->w_sel_id, &tb->w_sel_id_cap, (size_t)*total))) return rc;
+    p.key_id = tb->w_sel_id;
+    p.cap = *total;
+    if ((rc = select_fill(tb, p, n, s))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(key_id, tb->w_sel_id, (size_t)*total * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     return ACB_OK;
 }

@@ -984,32 +984,91 @@ static void letter_children(const acb_trie *t, int32_t a, std::vector<LetterEdge
         std::sort(out.begin(), out.end(), [t](const LetterEdge &x, const LetterEdge &y) { return t->nodes[x.node].birth < t->nodes[y.node].birth; });
 }
 
+/* The walk of the reference's keys() / values() / items(): its iterator keeps a stack, pushes a node's children in array
+ * order and pops the last one first (src/AutomatonItemsIter.c:125-288) -- a pre-order walk that takes the youngest
+ * child first.  visit(a, tag, kids, kid_tags) sees every live letter node a in that order, with the tag its parent gave
+ * it (the root's is 0) and its letter-children oldest first; it sets kid_tags[i], the tag of kids[i]. */
+template <typename Visit>
+static void key_order_walk(const acb_trie *t, Visit &&visit) {
+    std::vector<std::pair<int32_t, int32_t>> stack;
+    std::vector<LetterEdge> kids, tmp;
+    std::vector<int32_t> tags;
+    stack.push_back({0, 0});
+    while (!stack.empty()) {
+        const auto [a, tag] = stack.back();
+        stack.pop_back();
+        letter_children(t, a, kids, tmp);
+        tags.assign(kids.size(), 0);
+        visit(a, tag, kids, tags);
+        for (size_t i = 0; i < kids.size(); i++) stack.push_back({kids[i].node, tags[i]});   /* the youngest ends up on top */
+    }
+}
+
 } // namespace
 
-/* Key ids in the order in which the reference's keys() / values() / items() yield them: its iterator keeps a stack, pushes
- * a node's children in array order and pops the last one first (src/AutomatonItemsIter.c:125-288) -- a pre-order walk
- * that takes the youngest child first. */
+/* Key ids in the order in which the reference's keys() / values() / items() yield them (key_order_walk). */
 extern "C" int acb_trie_key_order(const acb_trie *t, int32_t *out, int64_t cap, int64_t *n) {
     if (!t || !n || cap < 0 || (cap && !out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n = 0;
     if (t->nodes.empty() || t->count == 0) return ACB_OK;
     try {
-        std::vector<int32_t> stack;
-        std::vector<LetterEdge> kids, tmp;
-        stack.push_back(0);
         int64_t k = 0;
-        while (!stack.empty()) {
-            const int32_t a = stack.back();
-            stack.pop_back();
+        key_order_walk(t, [&](int32_t a, int32_t, const std::vector<LetterEdge> &, std::vector<int32_t> &) {
             if (t->nodes[a].key_id >= 0) {
                 if (k < cap) out[k] = t->nodes[a].key_id;
                 k++;
             }
-            letter_children(t, a, kids, tmp);
-            for (const LetterEdge &e : kids) stack.push_back(e.node);          /* the youngest ends up on top */
-        }
+        });
         *n = k;
         if (k > cap) { acb_set_error("key order: room for %lld ids, %lld keys", (long long)cap, (long long)k); return ACB_EOVERFLOW; }
+        return ACB_OK;
+    } catch (const std::exception &) {
+        acb_set_error("out of memory");
+        return ACB_ENOMEM;
+    }
+}
+
+/* The key order as ranges over the flat tables (include/acb200.h).  The same walk as acb_trie_key_order; each letter
+ * node's state is found by stepping the flat goto table from its parent's state over the letter's bytes, so the arrays
+ * fit the tables also when they came from the flat-table cache. */
+extern "C" int acb_trie_key_ranges(const acb_trie *t, int32_t *order, int32_t *lo, int32_t *cnt, int32_t *child_ptr,
+                                   int32_t *child, int64_t *n_edges) {
+    if (!t || !order || !lo || !cnt || !child_ptr || !child || !n_edges) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (t->kind != ACB_AHOCORASICK || !t->flat.valid) { acb_set_error("not an Aho-Corasick automaton yet"); return ACB_ESTATE; }
+    const Flat &f = t->flat;
+    const int L = t->letter_bytes;
+    const size_t S = (size_t)f.S;
+    *n_edges = 0;
+    try {
+        std::fill(lo, lo + S, 0);
+        std::fill(cnt, cnt + S, 0);
+        std::vector<int32_t> deg(S, 0), at(S, 0), kid_states;    /* letter-children of state s: kid_states[at[s] ..][:deg[s]] */
+        kid_states.reserve(S);
+        int64_t k = 0;
+        bool ok = true;
+        if (t->count > 0) key_order_walk(t, [&](int32_t a, int32_t s, const std::vector<LetterEdge> &kids, std::vector<int32_t> &tags) {
+            const Node &nd = t->nodes[a];
+            lo[s] = (int32_t)k;
+            cnt[s] = nd.live_below;
+            if (nd.key_id >= 0 && k < t->count) order[k++] = nd.key_id;
+            at[s] = (int32_t)kid_states.size();
+            deg[s] = (int32_t)kids.size();
+            for (size_t i = kids.size(); i-- > 0;) {             /* youngest first, the order of the walk: by ascending lo */
+                int32_t x = s;
+                for (int d = 0; d < L && x >= 0; d++)
+                    x = f.goto_cm[(size_t)f.byte_class[(kids[i].letter >> (8 * d)) & 0xffu] * S + (size_t)x];
+                if (x <= 0) { ok = false; x = 0; }
+                tags[i] = x;
+                kid_states.push_back(x);
+            }
+        });
+        if (!ok || k != t->count) { acb_set_error("internal: the flat tables do not fit the trie"); return ACB_EINVAL; }
+        child_ptr[0] = 0;
+        for (size_t s = 0; s < S; s++) {
+            child_ptr[s + 1] = child_ptr[s] + deg[s];
+            std::copy(kid_states.begin() + at[s], kid_states.begin() + at[s] + deg[s], child + child_ptr[s]);
+        }
+        *n_edges = (int64_t)kid_states.size();
         return ACB_OK;
     } catch (const std::exception &) {
         acb_set_error("out of memory");
