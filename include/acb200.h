@@ -414,6 +414,31 @@ int acb_select_host(acb_table *tb, const uint8_t *patterns, int64_t total_bytes,
                     int64_t stride_bytes, int64_t wildcard, int how, int64_t *out_offsets, int32_t *key_id, int64_t cap,
                     int64_t *total);
 
+/* ---- leftmost-longest non-overlapping matches ----------------------------------------------------------------------
+ * From the full match list of each haystack (what iter() reports, start = end_index - len + 1): p = 0; while some match
+ * starts at or after p, take the smallest such start, the longest match there, and continue at its end_index + 1.  This
+ * is not iter_long (src/AutomatonSearchIterLong.c:89-153), whose restart rule depends on the trie's inner nodes.
+ *
+ * DEVICE buffers, asynchronous on `stream`: d_records holds the full list of n records of a batch of n_hay haystacks,
+ * in any order (what acb_scan_device leaves); max_hay_letters bounds end_index.  The chosen records go to d_out in
+ * haystack order, then end_index ascending; *d_count is increased by their number and only the first cap are stored.
+ * d_records is not changed.  The scratch space belongs to the table: the next call waits (cudaStreamWaitEvent) for the
+ * work of this one, also on another CUDA stream.  ACB_ERANGE for more than 2^31-1 records. */
+int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay, int64_t max_hay_letters,
+                                acb_match *d_out, int64_t cap, int64_t *d_count, void *stream);
+
+/* HOST buffers: upload, scan (algo ACB_ALGO_AUTO, _FILTER or _DFA; monolithic, as for ACB_ALGO_DFA), select, copy back,
+ * synchronous.  *n_found is the exact number of chosen records; ACB_EOVERFLOW when it exceeds cap.  The full list is
+ * kept in a device buffer of the table grown to fit.  out == NULL works as for acb_scan_host (acb_copy_records /
+ * acb_take_records).  Without a device: ACB_ECUDA. */
+int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                           int64_t stride_bytes, acb_match *out, int64_t cap, int64_t *n_found, int algo);
+
+/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last selection's stages on this thread: sort,
+ * candidates, successors, chain, emit (the first n of them, n <= 5), from CUDA events between the stages (the call then
+ * waits for them); 0 when timing is off. */
+int acb_last_leftmost_ms(float *ms, int32_t n);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

@@ -915,6 +915,80 @@ class Automaton:
         """iter_long() over a whole batch (same input forms and result type as find_all_batch)."""
         return self.find_all_batch(haystacks, algo="long", sort=sort, device=device)
 
+    def find_leftmost_longest_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None) -> "Matches":
+        """Leftmost-longest non-overlapping matches of a whole batch, selected on the GPU (input forms and result type
+        of find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or
+        after p, take the smallest such start, the longest match there, and continue after its end.  Records come in
+        haystack order, then end_index ascending.  This is the leftmost-longest rule of keyword extractors, not
+        iter_long's: iter_long restarts from the root after every match and misses keys its walk does not pass.
+        algo ("auto", "filter", "dfa") only picks the scan that finds every match; the result does not depend on it."""
+        self._require_automaton()
+        if algo not in ("auto", "filter", "dfa"):
+            raise ValueError(f"algo {algo!r}: leftmost-longest takes 'auto', 'filter' or 'dfa'")
+        batch = self._batch_input(haystacks)
+        if batch[0] == "device":
+            return Matches(self._leftmost_device(batch[1], algo), self._values)
+        _, flat, offs, n, stride, narrow = batch
+        if not (n and flat.size):
+            return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
+        return Matches(self._leftmost_host(flat, offs, n, stride, algo, device, narrow), self._values)
+
+    @_locked
+    def _leftmost_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str,
+                       device: Optional[int], narrow: bool) -> np.ndarray:
+        """acb_scan_host_leftmost: upload, scan, select, copy back; the capacity grows on overflow."""
+        if narrow:
+            core = self._ensure_narrow(device)
+            if core is None:
+                return np.empty(0, dtype=N.MATCH_DTYPE)
+            tb = core[1]
+        else:
+            tb = self._ensure_table(device)
+        cap = max(self._match_cap, 1 << 12, 2 * n_hay)
+        found = ctypes.c_int64(0)
+        while True:
+            rc = self._lib.acb_scan_host_leftmost(tb, N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None,
+                                                  n_hay, stride_bytes, None, cap, ctypes.byref(found), N.ALGOS[algo])
+            if rc != N.ACB_EOVERFLOW:
+                break
+            cap = self._match_cap = int(found.value) + 1024
+        N.check(rc)
+        if not found.value:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        return _take_records(self._lib, tb, found.value)
+
+    @_locked
+    def _leftmost_device(self, t, algo: str) -> np.ndarray:
+        """A CUDA tensor batch: the full scan into a device buffer, then acb_leftmost_longest_device, both on torch's
+        current stream; only the chosen records come back."""
+        import torch
+        n, stride = self._device_batch_shape(t)
+        if n == 0 or stride == 0:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        t = _aligned(t)
+        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        tb = self._ensure_table(dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream().cuda_stream
+            cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
+            cap = max(self._match_cap, 1 << 12, 2 * n)
+            while True:
+                full = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+                cnt.zero_()
+                N.check(self._lib.acb_scan_device(tb, t.data_ptr(), n * stride, None, n, stride, full.data_ptr(), cap,
+                                                  cnt.data_ptr(), stream, N.ALGOS[algo]))
+                m = int(cnt.item())
+                if m <= cap:
+                    break
+                cap = self._match_cap = m + 1024
+            cap = max(m, 1)
+            out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+            cnt.zero_()
+            N.check(self._lib.acb_leftmost_longest_device(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap,
+                                                          cnt.data_ptr(), stream))
+            found = int(cnt.item())
+            return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
+
     def dump(self):
         """(nodes, edges, fail) in the spirit of src/Automaton.c:1100-1180, with int state ids."""
         f = self.flat()

@@ -36,6 +36,7 @@
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -1372,6 +1373,12 @@ struct acb_table {
     uint8_t *w_scan = nullptr; size_t w_scan_cap = 0;    /* the offsets' prefix sum */
     long long *w_sel_off = nullptr; size_t w_sel_off_cap = 0;   /* acb_select_host: out offsets[n+1] then the total */
     int32_t *w_sel_id = nullptr; size_t w_sel_id_cap = 0;       /* acb_select_host: key ids */
+    /* workspace of the leftmost-longest selection (acb_leftmost_longest_device), sized by the full record count */
+    void *l_buf = nullptr; size_t l_buf_cap = 0;         /* sort keys, sorted records, candidates, flags, successors, cub scratch */
+    unsigned long long *l_ctr = nullptr;                 /* [0] candidates, [1] chain tile counter, [2] chosen count (host route) */
+    acb_match *l_out = nullptr; size_t l_out_cap = 0;    /* acb_scan_host_leftmost: the chosen records */
+    cudaEvent_t l_done = nullptr;                        /* the last selection's work on l_buf has been issued before it */
+    cudaEvent_t l_ev[6] = {};                            /* kernel timing of its stages */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1414,6 +1421,9 @@ extern "C" void acb_table_free(acb_table *tb) {
     cudaFree(tb->w_lk);
     cudaFree(tb->d_order); cudaFree(tb->d_lo); cudaFree(tb->d_cnt); cudaFree(tb->d_child_ptr); cudaFree(tb->d_child);
     cudaFree(tb->w_scan); cudaFree(tb->w_sel_off); cudaFree(tb->w_sel_id);
+    cudaFree(tb->l_buf); cudaFree(tb->l_ctr); cudaFree(tb->l_out);
+    if (tb->l_done) cudaEventDestroy(tb->l_done);
+    for (cudaEvent_t e : tb->l_ev) if (e) cudaEventDestroy(e);
     if (tb->h_kept) cudaFreeHost(tb->h_kept);
     if (tb->k_done) cudaEventDestroy(tb->k_done);
     if (tb->k_t0) cudaEventDestroy(tb->k_t0);
@@ -1744,15 +1754,24 @@ extern "C" void acb_release_records(acb_match *ptr, int64_t cap) {
 
 /* ------------------------------------------------------------ record sort */
 /* Reference order (SURVEY 3.3): haystack, then end_index ascending, then longest key first.  One
- * 64-bit radix key per record: hay_id | end_index | (max_len - len), packed into the fewest bits. */
+ * 64-bit radix key per record: hay_id | end_index | (max_len - len), packed into the fewest bits.
+ * The leftmost-longest selection sorts by start letter instead (kKeyStart), and when that key needs more than 64 bits
+ * in two stable passes: start | (max_len - len) first (kKeyStartLow), then hay_id (kKeyHay). */
 namespace {
+enum { kKeyEnd, kKeyStart, kKeyStartLow, kKeyHay };
+
+template <int kMode>
 __global__ void acb_sortkey_kernel(const acb_match *rec, long long n, const int32_t *key_len, int be, int bl,
                                    int max_len, unsigned long long *keys) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const acb_match m = rec[i];
-    const unsigned long long inv = (unsigned long long)(max_len - __ldg(key_len + m.key_id));
-    keys[i] = ((unsigned long long)(uint32_t)m.hay_id << (be + bl)) | ((unsigned long long)(uint32_t)m.end_index << bl) | inv;
+    if (kMode == kKeyHay) { keys[i] = (uint32_t)m.hay_id; return; }
+    const int len = __ldg(key_len + m.key_id);
+    const unsigned long long inv = (unsigned long long)(max_len - len);
+    const uint32_t pos = kMode == kKeyEnd ? (uint32_t)m.end_index : (uint32_t)(m.end_index - len + 1);
+    const unsigned long long hay = kMode == kKeyStartLow ? 0ULL : (unsigned long long)(uint32_t)m.hay_id << (be + bl);
+    keys[i] = hay | ((unsigned long long)pos << bl) | inv;
 }
 int bits_for(unsigned long long v) { int b = 1; while (b < 64 && (v >> b)) b++; return b; }
 } // namespace
@@ -1784,7 +1803,7 @@ extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int6
     unsigned long long *k1 = k0 + n;
     acb_match *r1 = reinterpret_cast<acb_match *>(k1 + n);
     void *tmp = reinterpret_cast<void *>((reinterpret_cast<uintptr_t>(r1 + n) + 255) & ~(uintptr_t)255);
-    acb_sortkey_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
+    acb_sortkey_kernel<kKeyEnd><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
     CUDA_TRY(cudaGetLastError());
     g_launches.fetch_add(1);
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, temp, k0, k1, d_records, r1, (int)n, 0, bh + be + bl, s));
@@ -3179,5 +3198,335 @@ extern "C" int acb_select_host(acb_table *tb, const uint8_t *patterns, int64_t t
     if ((rc = select_fill(tb, p, n, s))) return rc;
     CUDA_TRY(cudaMemcpyAsync(key_id, tb->w_sel_id, (size_t)*total * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
+    return ACB_OK;
+}
+
+/* ------------------------------------------------------------ leftmost-longest selection */
+/* Leftmost-longest non-overlapping matches (p = 0; take the smallest start >= p, the longest match there, continue after
+ * it) are a function of the full match list alone, so they are selected from the records a scan left, in five
+ * data-parallel steps: (1) radix sort by hay | start | (max_len - len); (2) the first record of every (hay, start) run is
+ * the longest match starting there: a candidate, compacted with DeviceSelect; (3) next[i] = the first candidate of the
+ * same haystack that starts at or after the end of candidate i (a binary search over the next len_i candidates);
+ * (4) a candidate is chosen iff it lies on the next-chain from its haystack's first candidate: acb_ll_chain_kernel
+ * below; (5) the chosen candidates, already in the final order, are stream-compacted into the caller's buffer. */
+namespace {
+constexpr int kLlTile = 2048;                             /* candidates per chain tile */
+constexpr int kLlThreads = 256;
+thread_local float g_ll_ms[5] = {};                       /* kernel timing: sort, candidates, successor, chain, emit */
+
+__device__ __forceinline__ long long ll_start(const acb_match &m, const int32_t *key_len) {
+    return (long long)m.end_index - __ldg(key_len + m.key_id) + 1;
+}
+
+/* flag[i] = 1 for the first record of every (hay, start) run of the sorted list */
+__global__ void acb_ll_cand_kernel(const acb_match *rec, long long n, const int32_t *key_len, uint8_t *flag) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const acb_match m = rec[i];
+        bool first = i == 0;
+        if (!first) {
+            const acb_match q = rec[i - 1];
+            first = q.hay_id != m.hay_id || ll_start(q, key_len) != ll_start(m, key_len);
+        }
+        flag[i] = first;
+    }
+}
+
+/* next[i]: the first candidate of the same haystack with start >= start_i + len_i, or -1.  A haystack's candidates have
+ * distinct ascending starts, so candidate i + len_i (when it is of the same haystack) already qualifies: the search
+ * covers [i + 1, i + len_i]. */
+__global__ void acb_ll_next_kernel(const acb_match *cand, const unsigned long long *d_m, const int32_t *key_len, int32_t *nxt) {
+    const long long M = (long long)*d_m;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < M; i += (long long)gridDim.x * blockDim.x) {
+        const acb_match c = cand[i];
+        const long long target = (long long)c.end_index + 1;
+        long long lo = i + 1, hi = min(M, i + __ldg(key_len + c.key_id) + 1);
+        while (lo < hi) {
+            const long long mid = (lo + hi) >> 1;
+            const acb_match q = cand[mid];
+            if (q.hay_id != c.hay_id || ll_start(q, key_len) >= target) hi = mid; else lo = mid + 1;
+        }
+        bool ok = false;
+        if (lo < M) { const acb_match q = cand[lo]; ok = q.hay_id == c.hay_id && ll_start(q, key_len) >= target; }
+        nxt[i] = ok ? (int32_t)lo : -1;
+    }
+}
+
+/* Chain marking over tiles of kLlTile candidates, one block per tile, tiles claimed in order from a counter.
+ *  - The speculative walk (one thread, shared memory): from the tile's first candidate and from every haystack's first
+ *    candidate in the tile, the chain through next[].  Every haystack that starts in the tile is exact; only the one
+ *    continuing from the previous tile (candidates [0, fh)) depends on the entry the previous tile hands over.
+ *  - The exit (the chain's first candidate past the tile, or -1) is published to status[t] as soon as it is known.  It
+ *    does not depend on the entry when a haystack starts in the tile, or when the tile holds at least W = longest_word
+ *    candidates and the chain from each of the first W joins the speculative chain inside the tile: the entry is the
+ *    successor of a candidate of an earlier tile, so it lies among the first W candidates, and chains that meet stay
+ *    together.  Otherwise the tile publishes after its entry is known.
+ *  - The entry comes from status[t - 1] (a look-back of one tile: every tile publishes its exit itself).  The tile walks
+ *    from it until it lands on the speculative chain; the speculative nodes before that point are dropped. */
+__global__ void __launch_bounds__(kLlThreads) acb_ll_chain_kernel(const acb_match *cand, const unsigned long long *d_m,
+                                                                  const int32_t *nxt, int W, unsigned long long *ctr,
+                                                                  unsigned long long *status, uint8_t *chosen, int32_t *pos) {
+    __shared__ int32_t s_next[kLlTile];
+    __shared__ int32_t s_hay[kLlTile + 1];                 /* s_hay[j] = hay of candidate base + j - 1 */
+    __shared__ uint8_t s_spec[kLlTile], s_fin[kLlTile];
+    __shared__ long long s_tile, s_exit;
+    __shared__ int s_fh;
+    __shared__ volatile int s_dep;
+    if (threadIdx.x == 0) s_tile = (long long)atomicAdd(ctr, 1ULL);   /* in claim order: every earlier tile is running or done */
+    __syncthreads();
+    const long long M = (long long)*d_m, t = s_tile, base = t * kLlTile;
+    if (base >= M) return;
+    const int n_tile = (int)min((long long)kLlTile, M - base);
+    for (int j = threadIdx.x; j <= n_tile; j += kLlThreads) {
+        s_hay[j] = base + j - 1 < 0 ? -1 : cand[base + j - 1].hay_id;
+        if (j < n_tile) s_next[j] = nxt[base + j];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        long long want = base;
+        int fh = n_tile;
+        for (int j = 0; j < n_tile; j++) {
+            if (s_hay[j + 1] != s_hay[j]) { want = base + j; if (fh == n_tile) fh = j; }
+            const bool on = want == base + j;
+            s_spec[j] = on;
+            if (on) want = s_next[j];
+        }
+        s_exit = want;
+        s_fh = fh;
+        s_dep = fh == n_tile && n_tile < W;
+    }
+    __syncthreads();
+    const int fh = s_fh;
+    const long long spec_exit = s_exit;
+    for (int j = threadIdx.x; j < n_tile; j += kLlThreads) s_fin[j] = s_spec[j];
+    if (fh == n_tile && !s_dep) {                          /* one haystack fills the tile: does every possible entry join? */
+        for (int j = threadIdx.x; j < W; j += kLlThreads) {
+            long long e = base + j;
+            while (e >= base && e < base + n_tile && !s_spec[e - base] && !s_dep) e = s_next[e - base];
+            const bool joined = e >= base && e < base + n_tile && s_spec[e - base];
+            if (!joined && e != spec_exit) s_dep = 1;
+        }
+    }
+    __syncthreads();
+    const bool indep = !s_dep;
+    if (threadIdx.x == 0) {
+        if (indep) atomicExch(status + t, (unsigned long long)(spec_exit + 2));
+        long long entry = base, exit = spec_exit;
+        if (fh > 0 && t > 0) {
+            unsigned long long st;
+            while ((st = *reinterpret_cast<volatile unsigned long long *>(status + t - 1)) == 0) {}
+            entry = (long long)st - 2;
+        }
+        if (entry != base) {                               /* merge on entry */
+            long long e = entry;
+            while (e >= base && e < base + fh && !s_spec[e - base]) { s_fin[e - base] = 1; e = s_next[e - base]; }
+            const bool joined = e >= base && e < base + fh;
+            const long long stop = joined ? e : base + fh;
+            for (long long q = base; q >= base && q < stop; q = s_next[q - base]) s_fin[q - base] = 0;
+            if (fh == n_tile && !joined) exit = e;
+        }
+        if (!indep) atomicExch(status + t, (unsigned long long)(exit + 2));
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < n_tile; j += kLlThreads) {
+        chosen[base + j] = s_fin[j];
+        pos[base + j] = s_fin[j];
+    }
+}
+
+/* the chosen candidates (pos: their exclusive prefix count) to out[*count + pos], those past cap counted, not stored */
+__global__ void acb_ll_emit_kernel(const acb_match *cand, const unsigned long long *d_m, const uint8_t *chosen, const int32_t *pos,
+                                   acb_match *out, long long cap, const unsigned long long *count) {
+    const long long M = (long long)*d_m;
+    const unsigned long long first = *count;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < M; i += (long long)gridDim.x * blockDim.x) {
+        if (!chosen[i]) continue;
+        const unsigned long long p = first + (unsigned long long)pos[i];
+        if (p < (unsigned long long)cap) out[p] = cand[i];
+    }
+}
+
+__global__ void acb_ll_count_kernel(const unsigned long long *d_m, const uint8_t *chosen, const int32_t *pos, unsigned long long *count) {
+    const long long M = (long long)*d_m;
+    if (M > 0) *count += (unsigned long long)pos[M - 1] + chosen[M - 1];
+}
+
+char *carve(char *&p, size_t bytes) { char *r = p; p += (bytes + 255) & ~(size_t)255; return r; }
+} // namespace
+
+static int ll_stage(acb_table *tb, int k, cudaStream_t s) {
+    if (!g_timing.load()) return ACB_OK;
+    if (!tb->l_ev[k]) CUDA_TRY(cudaEventCreate(&tb->l_ev[k]));
+    CUDA_TRY(cudaEventRecord(tb->l_ev[k], s));
+    return ACB_OK;
+}
+
+extern "C" int acb_last_leftmost_ms(float *ms, int32_t n) {
+    if (!ms || n < 0 || n > 5) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    for (int i = 0; i < n; i++) ms[i] = g_ll_ms[i];
+    return ACB_OK;
+}
+
+extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay,
+                                           int64_t max_hay_letters, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+    if (!tb || n < 0 || (n && !d_records) || n_hay < 0 || max_hay_letters < 0 || cap < 0 || (cap > 0 && !d_out) || !d_count) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    if (n > 0x7fffffffLL) { acb_set_error("more than 2^31-1 records to select from"); return ACB_ERANGE; }
+    for (float &v : g_ll_ms) v = 0.f;
+    if (n == 0) return ACB_OK;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const int max_len = tb->max_key_bytes / tb->L;
+    const int bh = bits_for((unsigned long long)std::max<int64_t>(n_hay - 1, 1));
+    const int be = bits_for((unsigned long long)std::max<int64_t>(max_hay_letters, 1));
+    const int bl = bits_for((unsigned long long)max_len);
+    const bool one_pass = bh + be + bl <= 64;
+    const int ni = (int)n;
+    const long long n_tiles = (n + kLlTile - 1) / kLlTile;
+    size_t t_sort = 0, t_sel = 0, t_scan = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
+                                             (const acb_match *)nullptr, (acb_match *)nullptr, ni, 0, 64, s));
+    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, t_sel, (const acb_match *)nullptr, (const uint8_t *)nullptr, (acb_match *)nullptr,
+                                        (unsigned long long *)nullptr, ni, s));
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int32_t *)nullptr, (int32_t *)nullptr, ni, s));
+    const size_t temp = std::max(t_sort, std::max(t_sel, t_scan));
+    const size_t N = (size_t)n;
+    const size_t need = 8 * 256 + 2 * N * sizeof(unsigned long long) + 2 * N * sizeof(acb_match) + N + 2 * N * sizeof(int32_t) +
+                        (size_t)n_tiles * sizeof(unsigned long long) + temp;
+    if (tb->l_done) CUDA_TRY(cudaStreamWaitEvent(s, tb->l_done, 0));
+    if (tb->l_buf_cap < need) {
+        if (tb->l_buf) { CUDA_TRY(cudaStreamSynchronize(s)); cudaFree(tb->l_buf); tb->l_buf = nullptr; tb->l_buf_cap = 0; }
+        CUDA_TRY(cudaMalloc(&tb->l_buf, need + need / 4));
+        tb->l_buf_cap = need + need / 4;
+    }
+    if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
+    char *p = reinterpret_cast<char *>(tb->l_buf);
+    unsigned long long *k0 = reinterpret_cast<unsigned long long *>(carve(p, N * 8)), *k1 = reinterpret_cast<unsigned long long *>(carve(p, N * 8));
+    acb_match *ra = reinterpret_cast<acb_match *>(carve(p, N * sizeof(acb_match))), *rb = reinterpret_cast<acb_match *>(carve(p, N * sizeof(acb_match)));
+    uint8_t *flag = reinterpret_cast<uint8_t *>(carve(p, N));
+    int32_t *nxt = reinterpret_cast<int32_t *>(carve(p, N * 4)), *pos = reinterpret_cast<int32_t *>(carve(p, N * 4));
+    unsigned long long *status = reinterpret_cast<unsigned long long *>(carve(p, (size_t)n_tiles * 8));
+    void *tmp = carve(p, temp);
+    size_t tb_temp = temp;
+    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, (long long)tb->sm_count * 16);
+    int rc;
+    if ((rc = ll_stage(tb, 0, s))) return rc;
+    /* 1. re-key by start and sort */
+    if (one_pass) {
+        acb_sortkey_kernel<kKeyStart><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, d_records, ra, ni, 0, bh + be + bl, s));
+        g_launches.fetch_add(1);
+    } else {                                               /* two stable passes: start | (max_len - len), then hay */
+        acb_sortkey_kernel<kKeyStartLow><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, d_records, rb, ni, 0, be + bl, s));
+        acb_sortkey_kernel<kKeyHay><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(rb, n, tb->d_keylen, be, bl, max_len, k0);
+        CUDA_TRY(cudaGetLastError());
+        tb_temp = temp;
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, rb, ra, ni, 0, bh, s));
+        g_launches.fetch_add(2);
+    }
+    if ((rc = ll_stage(tb, 1, s))) return rc;
+    /* 2. candidates: the longest match at every (hay, start) */
+    acb_ll_cand_kernel<<<grid, 256, 0, s>>>(ra, n, tb->d_keylen, flag);
+    CUDA_TRY(cudaGetLastError());
+    tb_temp = temp;
+    CUDA_TRY(cub::DeviceSelect::Flagged(tmp, tb_temp, ra, flag, rb, tb->l_ctr, ni, s));
+    g_launches.fetch_add(1);
+    if ((rc = ll_stage(tb, 2, s))) return rc;
+    /* 3. successors */
+    acb_ll_next_kernel<<<grid, 256, 0, s>>>(rb, tb->l_ctr, tb->d_keylen, nxt);
+    CUDA_TRY(cudaGetLastError());
+    g_launches.fetch_add(1);
+    if ((rc = ll_stage(tb, 3, s))) return rc;
+    /* 4. chain marking */
+    CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)n_tiles * sizeof(unsigned long long), s));
+    CUDA_TRY(cudaMemsetAsync(pos, 0, N * sizeof(int32_t), s));
+    CUDA_TRY(cudaMemsetAsync(tb->l_ctr + 1, 0, sizeof(unsigned long long), s));
+    acb_ll_chain_kernel<<<(unsigned)n_tiles, kLlThreads, 0, s>>>(rb, tb->l_ctr, nxt, std::max(max_len, 1), tb->l_ctr + 1, status, flag, pos);
+    CUDA_TRY(cudaGetLastError());
+    g_launches.fetch_add(1);
+    if ((rc = ll_stage(tb, 4, s))) return rc;
+    /* 5. emit */
+    tb_temp = temp;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb_temp, pos, pos, ni, s));
+    acb_ll_emit_kernel<<<grid, 256, 0, s>>>(rb, tb->l_ctr, flag, pos, d_out, cap, reinterpret_cast<const unsigned long long *>(d_count));
+    CUDA_TRY(cudaGetLastError());
+    acb_ll_count_kernel<<<1, 1, 0, s>>>(tb->l_ctr, flag, pos, reinterpret_cast<unsigned long long *>(d_count));
+    CUDA_TRY(cudaGetLastError());
+    g_launches.fetch_add(2);
+    if ((rc = ll_stage(tb, 5, s))) return rc;
+    if (!tb->l_done) CUDA_TRY(cudaEventCreateWithFlags(&tb->l_done, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventRecord(tb->l_done, s));
+    if (g_timing.load()) {
+        CUDA_TRY(cudaEventSynchronize(tb->l_ev[5]));
+        for (int k = 0; k < 5; k++) CUDA_TRY(cudaEventElapsedTime(&g_ll_ms[k], tb->l_ev[k], tb->l_ev[k + 1]));
+    }
+    return ACB_OK;
+}
+
+extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                                      int64_t stride_bytes, acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *n_found = 0;
+    if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("leftmost-longest takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
+    if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
+    if (!offsets && (stride_bytes <= 0 || stride_bytes % tb->L || stride_bytes * n_hay != total_bytes)) {
+        acb_set_error("fixed-stride batch needs stride_bytes > 0, a multiple of letter_bytes, and n_hay*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    tb->h_out_n = 0;
+    if (total_bytes == 0 || n_hay == 0) return ACB_OK;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
+    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
+    if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
+    int rc;
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_hay + 1))) return rc;
+    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(2 * n_hay, 4096)))) return rc;
+    cudaStream_t s = tb->stream;
+    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
+    const int64_t *d_off = nullptr;
+    if (offsets) {
+        CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_hay + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+        d_off = reinterpret_cast<const int64_t *>(tb->w_off);
+    }
+    unsigned long long full = 0;
+    for (;;) {                                             /* the full list: an intermediate, in a buffer grown to fit */
+        CUDA_TRY(cudaMemsetAsync(tb->w_count, 0, sizeof(unsigned long long), s));
+        if ((rc = acb_scan_device(tb, tb->w_hay, total_bytes, d_off, n_hay, stride_bytes, tb->w_out, (int64_t)tb->w_out_cap,
+                                  reinterpret_cast<int64_t *>(tb->w_count), s, algo)))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        full = *tb->h_count;
+        if (full <= tb->w_out_cap) break;
+        if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)full))) return rc;
+    }
+    if (full == 0) return ACB_OK;
+    const int64_t kept_cap = std::min<int64_t>(cap, (int64_t)full);
+    if ((rc = ensure(&tb->l_out, &tb->l_out_cap, (size_t)std::max<int64_t>(kept_cap, 1)))) return rc;
+    unsigned long long *d_n = tb->l_ctr + 2;
+    CUDA_TRY(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s));
+    if ((rc = acb_leftmost_longest_device(tb, tb->w_out, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, tb->l_out,
+                                          kept_cap, reinterpret_cast<int64_t *>(d_n), s)))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(tb->h_count, d_n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    const unsigned long long n = *tb->h_count;
+    *n_found = (int64_t)n;
+    if (n > (unsigned long long)cap) {
+        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
+        return ACB_EOVERFLOW;
+    }
+    if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->l_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
+    tb->h_out_n = n;
     return ACB_OK;
 }
