@@ -439,6 +439,41 @@ int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_byte
  * waits for them); 0 when timing is off. */
 int acb_last_leftmost_ms(float *ms, int32_t n);
 
+/* ---- leftmost-longest replacement ----------------------------------------------------------------------------------
+ * Each haystack with the letters [end_index - len + 1, end_index] of every match the leftmost-longest selection chose
+ * replaced by that key's replacement, every other letter copied.  A replacer holds the replacement of every key id on
+ * the device: rep[rep_offsets[k] .. rep_offsets[k+1]) (bytes, letters of the table's width; ids of removed keys get
+ * empty entries).  It records the table's device and letter width and n_ids; the calls refuse (ACB_EINVAL) a table of
+ * another device or width, or with more key ids.  The table is passed to every call and not kept, as for stream
+ * batches.  The offsets are checked (ACB_EINVAL) before anything runs.  Without a device: ACB_ECUDA. */
+typedef struct acb_replacer acb_replacer;
+
+int  acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets, int64_t n_ids,
+                      acb_replacer **out);
+void acb_replacer_free(acb_replacer *r);
+
+/* DEVICE buffers, asynchronous on `stream`.  The batch is laid out as for acb_scan_device; d_chosen holds the
+ * *d_n_chosen <= chosen_cap records acb_leftmost_longest_device wrote for it (haystack order, then end_index ascending,
+ * non-overlapping; not checked).  d_out_offsets (n_hay+1 int64 byte offsets of the output haystacks) and *d_total
+ * (their total) are always written; d_out only when the total is at most out_cap, which the device checks.  d_hay and
+ * d_out must be 16-byte aligned (ACB_EINVAL): the write pass reads and stores whole aligned 16-byte blocks, and may
+ * read the rest of an aligned block that holds a haystack byte.  The scratch space belongs to the table: the next
+ * call waits (cudaStreamWaitEvent) for the work of this one, also on another CUDA stream. */
+int acb_replace_device(acb_replacer *r, acb_table *tb, const uint8_t *d_hay, int64_t total_bytes, const int64_t *d_offsets,
+                       int64_t n_hay, int64_t stride_bytes, const acb_match *d_chosen, int64_t chosen_cap,
+                       const int64_t *d_n_chosen, int64_t *d_out_offsets, uint8_t *d_out, int64_t out_cap, int64_t *d_total,
+                       void *stream);
+
+/* HOST buffers: upload, scan (algo ACB_ALGO_AUTO, _FILTER or _DFA) into a full list grown to fit, select, rewrite, copy
+ * back, synchronous.  out_offsets and *total are always written; out when *total <= out_cap, else ACB_EOVERFLOW. */
+int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
+                     int64_t n_hay, int64_t stride_bytes, int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap,
+                     int64_t *total);
+
+/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last replacement's offsets pass and write pass
+ * on this thread (the first n of them, n <= 2), from CUDA events (the call then waits for them); 0 when timing is off. */
+int acb_last_replace_ms(float *ms, int32_t n);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

@@ -969,25 +969,40 @@ class Automaton:
         dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
         tb = self._ensure_table(dev)
         with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream().cuda_stream
-            cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
-            cap = max(self._match_cap, 1 << 12, 2 * n)
-            while True:
-                full = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-                cnt.zero_()
-                N.check(self._lib.acb_scan_device(tb, t.data_ptr(), n * stride, None, n, stride, full.data_ptr(), cap,
-                                                  cnt.data_ptr(), stream, N.ALGOS[algo]))
-                m = int(cnt.item())
-                if m <= cap:
-                    break
-                cap = self._match_cap = m + 1024
-            cap = max(m, 1)
-            out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-            cnt.zero_()
-            N.check(self._lib.acb_leftmost_longest_device(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap,
-                                                          cnt.data_ptr(), stream))
+            out, cnt, _ = self._leftmost_chosen(tb, t, n, stride, algo, torch.cuda.current_stream().cuda_stream)
             found = int(cnt.item())
             return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
+
+    def _leftmost_chosen(self, tb, t, n: int, stride: int, algo: str, stream):
+        """The chosen records of an aligned device batch, left on the device: (records [cap, 3] int32 CUDA tensor,
+        their count as an int64 CUDA tensor, cap).  Synchronises once, to size the full list."""
+        import torch
+        cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
+        cap = max(self._match_cap, 1 << 12, 2 * n)
+        while True:
+            full = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+            cnt.zero_()
+            N.check(self._lib.acb_scan_device(tb, t.data_ptr(), n * stride, None, n, stride, full.data_ptr(), cap,
+                                              cnt.data_ptr(), stream, N.ALGOS[algo]))
+            m = int(cnt.item())
+            if m <= cap:
+                break
+            cap = self._match_cap = m + 1024
+        cap = max(m, 1)
+        out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+        cnt.zero_()
+        N.check(self._lib.acb_leftmost_longest_device(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap,
+                                                      cnt.data_ptr(), stream))
+        return out, cnt, cap
+
+    def replacer(self, replacements=None, *, device: Optional[int] = None) -> "Replacer":
+        """A `Replacer` that rewrites whole batches with the leftmost-longest matches replaced (Replacer.replace_batch).
+        replacements=None: every key is replaced by its value (STORE_ANY only); else a mapping from every key to its
+        replacement, of the haystack type (bytes, str, or a tuple for KEY_SEQUENCE).  The replacements are taken when the
+        replacer is made: giving a key a new value (add_word of a key already present) does not change it or make it
+        stale, while adding or removing keys, or make_automaton, does."""
+        self._require_automaton()
+        return Replacer(self, replacements, _default_device() if device is None else device)
 
     def dump(self):
         """(nodes, edges, fail) in the spirit of src/Automaton.c:1100-1180, with int state ids."""
@@ -1479,6 +1494,166 @@ class StreamBatch:
         """int64[n_streams]: letters every stream has consumed since its start or its last reset (a copy)."""
         with self._A._gpu_lock:
             return self._native("positions")
+
+
+class Replacer:
+    """Result of `Automaton.replacer()`: the replacement of every key, kept on the GPU, for rewriting whole batches.
+
+    ``replace_batch(haystacks)`` takes, per haystack, exactly the matches `find_leftmost_longest_batch` chooses, replaces
+    the letters of each by its key's replacement and copies every other letter; a replacement is never scanned again.
+    The replacements are a snapshot taken when the replacer is made.  A replacer belongs to the key set it was made
+    for: after keys are added or removed, `replace_batch` raises ValueError as a stale iterator does."""
+
+    def __init__(self, A: Automaton, replacements, device: int):
+        self._A = A
+        self._version = A._version
+        self._device = device
+        self._native = {}                                   # (narrow, device) -> acb_replacer*, uploaded on first use
+        if replacements is None and A._store != STORE_ANY:
+            raise ValueError("replacer() without replacements takes each key's value: the automaton must be STORE_ANY")
+        n_ids = len(A._key_objs)
+        reps = [None] * n_ids
+        for kid, key in enumerate(A._key_objs):             # ids ascend in insertion order
+            if key is None:
+                continue
+            if replacements is None:
+                rep = A._values[kid]
+            else:
+                if key not in replacements:
+                    raise KeyError(key)
+                rep = replacements[key]
+            reps[kid] = A._letters(rep)
+        L = A._L
+        empty = np.empty(0, dtype=_LETTER_DTYPE[L])
+        self._tables = {False: self._layout([empty if r is None else r for r in reps], L)}
+        if A._uses_narrow() and all(r is None or r.size == 0 or int(r.max()) < 256 for r in reps):
+            self._tables[True] = self._layout([np.empty(0, np.uint8) if r is None else r.astype(np.uint8) for r in reps], 1)
+
+    @staticmethod
+    def _layout(letters: list, width: int) -> Tuple[np.ndarray, np.ndarray]:
+        """(bytes uint8, byte offsets int64[n_ids+1]) of the replacements at `width` bytes per letter"""
+        offs = np.zeros(len(letters) + 1, dtype=np.int64)
+        np.cumsum(np.fromiter((a.size * width for a in letters), dtype=np.int64, count=len(letters)), out=offs[1:])
+        flat = np.concatenate([np.ascontiguousarray(a, dtype=_LETTER_DTYPE[width]).view(np.uint8) for a in letters]) \
+            if letters else np.empty(0, dtype=np.uint8)
+        return flat, offs
+
+    def __del__(self):
+        try:
+            for r in self._native.values():
+                self._A._lib.acb_replacer_free(r)
+            self._native = {}
+        except Exception:                                   # interpreter shutdown
+            pass
+
+    def _replacer(self, tb, narrow: bool, device: int):
+        """the native replacer for this table (letter width, device), uploaded on first use"""
+        r = self._native.get((narrow, device))
+        if r is None:
+            flat, offs = self._tables[narrow]
+            r = ctypes.c_void_p()
+            N.check(self._A._lib.acb_replacer_new(tb, N.ptr(flat) if flat.size else None, int(flat.size), N.ptr(offs),
+                                                  len(offs) - 1, ctypes.byref(r)))
+            self._native[(narrow, device)] = r
+        return r
+
+    def replace_batch(self, haystacks, *, algo: str = "auto"):
+        """The batch with every leftmost-longest match replaced.  `haystacks` takes the input forms of find_all_batch;
+        a list gives a list of the same item type, uint8[n, stride] or (flat, offsets) gives (flat uint8, offsets
+        int64[n+1]), a CUDA tensor gives that pair as CUDA tensors computed on torch's current stream (the call
+        synchronises once to size the output).  algo ("auto", "filter", "dfa") only picks the scan."""
+        A = self._A
+        with A._gpu_lock:
+            if self._version != A._version:
+                raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
+            A._require_automaton()
+            if algo not in ("auto", "filter", "dfa"):
+                raise ValueError(f"algo {algo!r}: replace_batch takes 'auto', 'filter' or 'dfa'")
+            pair = isinstance(haystacks, np.ndarray) or (isinstance(haystacks, tuple) and len(haystacks) == 2 and
+                                                         all(isinstance(x, np.ndarray) for x in haystacks))
+            batch = A._batch_input(haystacks)
+            if batch[0] == "device":
+                return self._run_device(batch[1], algo)
+            _, flat, offs, n, stride, narrow = batch
+            if narrow and True not in self._tables:         # a replacement outside latin-1: 4 bytes per letter
+                flat = flat.astype("<u4").view(np.uint8)
+                offs = offs * 4
+                narrow = False
+            if offs is None:
+                offs = np.arange(n + 1, dtype=np.int64) * stride
+            if n == 0 or flat.size == 0:
+                out, out_offs = flat[:0].copy(), np.zeros(n + 1, dtype=np.int64)
+            else:
+                out, out_offs = self._run_host(flat, offs, n, narrow, algo)
+            if pair:
+                return out, out_offs
+            return self._items(out, out_offs, narrow)
+
+    def _items(self, out: np.ndarray, offs: np.ndarray, narrow: bool) -> list:
+        """the output haystacks as objects of the input's type"""
+        A = self._A
+        b = offs.tolist()
+        if A._key_type == KEY_SEQUENCE:
+            v = out.view(_LETTER_DTYPE[A._L]).tolist()
+            L = A._L
+            return [tuple(v[b[i] // L:b[i + 1] // L]) for i in range(len(b) - 1)]
+        raw = out.tobytes()
+        if not A._UNICODE:
+            return [raw[b[i]:b[i + 1]] for i in range(len(b) - 1)]
+        if narrow:
+            s = raw.decode("latin-1")
+            return [s[b[i]:b[i + 1]] for i in range(len(b) - 1)]
+        s = raw.decode("utf-32-le", "surrogatepass")
+        return [s[b[i] // 4:b[i + 1] // 4] for i in range(len(b) - 1)]
+
+    def _run_host(self, flat: np.ndarray, offs: np.ndarray, n: int, narrow: bool, algo: str):
+        """acb_replace_host -> (output bytes, output offsets int64[n+1]); a second call when the first guess of the
+        output size was too small"""
+        A = self._A
+        if narrow:
+            core = A._ensure_narrow(self._device)
+            if core is None:                                # no latin-1 key: nothing matches
+                return flat.copy(), offs.copy()
+            tb = core[1]
+        else:
+            tb = A._ensure_table(self._device)
+        r = self._replacer(tb, narrow, self._device)
+        out_offs = np.empty(n + 1, dtype=np.int64)
+        total = ctypes.c_int64(0)
+        cap = int(flat.size) + int(flat.size) // 4 + 4096
+        for _ in range(2):
+            out = np.empty(cap, dtype=np.uint8)
+            rc = A._lib.acb_replace_host(r, tb, N.ptr(flat), int(flat.size), N.ptr(offs), n, 0, N.ALGOS[algo],
+                                         N.ptr(out_offs), N.ptr(out), cap, ctypes.byref(total))
+            if rc != N.ACB_EOVERFLOW:
+                break
+            cap = int(total.value)
+        N.check(rc)
+        return out[:total.value], out_offs
+
+    def _run_device(self, t, algo: str):
+        """A CUDA tensor batch: scan, select and rewrite on torch's current stream; (flat, offsets) CUDA tensors"""
+        import torch
+        A = self._A
+        n, stride = A._device_batch_shape(t)
+        if n == 0 or stride == 0:
+            return torch.empty(0, dtype=torch.uint8, device=t.device), torch.zeros(n + 1, dtype=torch.int64, device=t.device)
+        t = _aligned(t)
+        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        tb = A._ensure_table(dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream().cuda_stream
+            chosen, cnt, cap = A._leftmost_chosen(tb, t, n, stride, algo, stream)
+            r = self._replacer(tb, False, dev)
+            out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+            total = torch.empty(1, dtype=torch.int64, device=t.device)
+            args = (r, tb, t.data_ptr(), n * stride, None, n, stride, chosen.data_ptr(), cap, cnt.data_ptr(), out_offs.data_ptr())
+            N.check(A._lib.acb_replace_device(*args, None, 0, total.data_ptr(), stream))
+            m = int(total.item())                           # the one synchronisation: the size of the output
+            out = torch.empty(m, dtype=torch.uint8, device=t.device)
+            if m:
+                N.check(A._lib.acb_replace_device(*args, out.data_ptr(), m, total.data_ptr(), stream))
+        return out, out_offs
 
 
 class AutomatonSearchIter:

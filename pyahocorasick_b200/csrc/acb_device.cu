@@ -1379,6 +1379,13 @@ struct acb_table {
     acb_match *l_out = nullptr; size_t l_out_cap = 0;    /* acb_scan_host_leftmost: the chosen records */
     cudaEvent_t l_done = nullptr;                        /* the last selection's work on l_buf has been issued before it */
     cudaEvent_t l_ev[6] = {};                            /* kernel timing of its stages */
+    /* workspace of the leftmost-longest replacement (acb_replace_device), sized by the chosen records' capacity */
+    void *r_buf = nullptr; size_t r_buf_cap = 0;         /* shifts, per-record positions, cub scratch */
+    long long *r_ts = nullptr; size_t r_ts_cap = 0;      /* the last record that starts at or before each tile start */
+    uint8_t *r_out = nullptr; size_t r_out_cap = 0;      /* acb_replace_host: the output bytes */
+    long long *r_off = nullptr; size_t r_off_cap = 0;    /* acb_replace_host: output offsets[n+1] then the total */
+    cudaEvent_t r_done = nullptr;                        /* the last replacement's work on r_buf / r_ts has been issued before it */
+    cudaEvent_t r_ev[4] = {};                            /* kernel timing of the offsets pass and the write pass */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1424,6 +1431,9 @@ extern "C" void acb_table_free(acb_table *tb) {
     cudaFree(tb->l_buf); cudaFree(tb->l_ctr); cudaFree(tb->l_out);
     if (tb->l_done) cudaEventDestroy(tb->l_done);
     for (cudaEvent_t e : tb->l_ev) if (e) cudaEventDestroy(e);
+    cudaFree(tb->r_buf); cudaFree(tb->r_ts); cudaFree(tb->r_out); cudaFree(tb->r_off);
+    if (tb->r_done) cudaEventDestroy(tb->r_done);
+    for (cudaEvent_t e : tb->r_ev) if (e) cudaEventDestroy(e);
     if (tb->h_kept) cudaFreeHost(tb->h_kept);
     if (tb->k_done) cudaEventDestroy(tb->k_done);
     if (tb->k_t0) cudaEventDestroy(tb->k_t0);
@@ -3467,6 +3477,40 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     return ACB_OK;
 }
 
+/* The host routes' first step: the batch to tb->w_hay (and offsets to tb->w_off, *d_off), and its full match list into
+ * tb->w_out, grown until it fits; *full is its length.  On tb->stream, which it leaves synchronised. */
+static int upload_and_scan_full(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                                int64_t stride_bytes, int algo, const int64_t **d_off, unsigned long long *full) {
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
+    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
+    if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
+    int rc;
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_hay + 1))) return rc;
+    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(2 * n_hay, 4096)))) return rc;
+    cudaStream_t s = tb->stream;
+    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
+    *d_off = nullptr;
+    if (offsets) {
+        CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_hay + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+        *d_off = reinterpret_cast<const int64_t *>(tb->w_off);
+    }
+    for (;;) {                                             /* the full list: an intermediate, in a buffer grown to fit */
+        CUDA_TRY(cudaMemsetAsync(tb->w_count, 0, sizeof(unsigned long long), s));
+        if ((rc = acb_scan_device(tb, tb->w_hay, total_bytes, *d_off, n_hay, stride_bytes, tb->w_out, (int64_t)tb->w_out_cap,
+                                  reinterpret_cast<int64_t *>(tb->w_count), s, algo)))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        *full = *tb->h_count;
+        if (*full <= tb->w_out_cap) break;
+        if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)*full))) return rc;
+    }
+    return ACB_OK;
+}
+
 extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
                                       int64_t stride_bytes, acb_match *out, int64_t cap, int64_t *n_found, int algo) {
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
@@ -3479,34 +3523,11 @@ extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t
     }
     tb->h_out_n = 0;
     if (total_bytes == 0 || n_hay == 0) return ACB_OK;
-    CUDA_TRY(cudaSetDevice(tb->device));
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
-    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
-    if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
-    int rc;
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_hay + 1))) return rc;
-    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(2 * n_hay, 4096)))) return rc;
-    cudaStream_t s = tb->stream;
-    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
     const int64_t *d_off = nullptr;
-    if (offsets) {
-        CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_hay + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
-        d_off = reinterpret_cast<const int64_t *>(tb->w_off);
-    }
     unsigned long long full = 0;
-    for (;;) {                                             /* the full list: an intermediate, in a buffer grown to fit */
-        CUDA_TRY(cudaMemsetAsync(tb->w_count, 0, sizeof(unsigned long long), s));
-        if ((rc = acb_scan_device(tb, tb->w_hay, total_bytes, d_off, n_hay, stride_bytes, tb->w_out, (int64_t)tb->w_out_cap,
-                                  reinterpret_cast<int64_t *>(tb->w_count), s, algo)))
-            return rc;
-        CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaStreamSynchronize(s));
-        full = *tb->h_count;
-        if (full <= tb->w_out_cap) break;
-        if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)full))) return rc;
-    }
+    int rc;
+    if ((rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, &d_off, &full))) return rc;
+    cudaStream_t s = tb->stream;
     if (full == 0) return ACB_OK;
     const int64_t kept_cap = std::min<int64_t>(cap, (int64_t)full);
     if ((rc = ensure(&tb->l_out, &tb->l_out_cap, (size_t)std::max<int64_t>(kept_cap, 1)))) return rc;
@@ -3528,5 +3549,402 @@ extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t
     CUDA_TRY(cudaStreamSynchronize(s));
     if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
     tb->h_out_n = n;
+    return ACB_OK;
+}
+
+/* ------------------------------------------------------------ leftmost-longest replacement */
+/* The chosen records of a batch (acb_leftmost_longest_device's order) rewrite it: the letters of every chosen match
+ * become the key's replacement, every other letter is copied.  Two passes:
+ *  - offsets: D = exclusive scan of (rep_len - key_len * L) over the records.  Record i starts at input byte S_i (batch
+ *    coordinates) and its replacement at output byte P_i = S_i + D[i]; it ends at E_i = P_i + rep_len, where the input
+ *    resumes at IE_i = S_i + key_len * L.  Haystack h starts at out_off[h] = in_off[h] + D[lo_h], lo_h its first record
+ *    (a binary search on hay_id); out_off[n_hay] is the total.
+ *  - write: the output is cut into tiles of kRpTile bytes, whatever the haystacks.  ts[t] = the last record with
+ *    P <= t * kRpTile (a binary search per tile), so the records that touch tile t are ts[t] .. ts[t+1]; a block stages
+ *    them in shared memory (when they fit) and each thread writes one 16-byte chunk.  For an output byte o, k = the last
+ *    record with P_k <= o: o < E_k is replacement byte RS_k + o - P_k, else o is copied from input byte IE_k + o - E_k
+ *    (o itself before the first record).  A chunk inside one copy run or one replacement is one aligned 16-byte store
+ *    of two aligned 16-byte loads merged by funnel shifts; only chunks that straddle a boundary go byte by byte. */
+struct acb_replacer {
+    int device = 0;
+    int32_t L = 1;
+    int64_t n_ids = 0;
+    uint8_t *d_rep = nullptr;                                /* replacement bytes, 32 bytes of padding behind */
+    long long *d_rep_off = nullptr;                          /* n_ids + 1 byte offsets */
+};
+
+namespace {
+constexpr int kRpThreads = 256;
+constexpr int kRpTile = kRpThreads * 16;                   /* output bytes per tile: one 16-byte chunk per thread */
+constexpr int kRpStage = 512;                              /* records a tile stages in shared memory */
+thread_local float g_rp_ms[2] = {};                        /* kernel timing: offsets pass, write pass */
+
+struct RpArgs {
+    const acb_match *chosen; const unsigned long long *n_chosen; long long cap;   /* records: min(*n_chosen, cap) */
+    const int32_t *key_len; const long long *rep_off; const uint8_t *rep; int L;
+    const uint8_t *hay; const long long *in_off; long long stride, n_hay, total_bytes;
+    long long *D, *P, *E, *IE, *RS;                        /* D[cap + 1]; the others per record */
+    long long *ts; long long out_cap;
+    long long *out_off, *total; uint8_t *out;
+};
+
+__device__ __forceinline__ long long rp_n(const RpArgs &a) { return min((long long)*a.n_chosen, a.cap); }
+__device__ __forceinline__ long long rp_in_off(const RpArgs &a, long long h) { return a.in_off ? a.in_off[h] : h * a.stride; }
+
+/* D[i] = rep_len - key_len * L of record i, 0 for i in [n, cap] (the exclusive scan then leaves the sum in D[cap]) */
+__global__ void acb_rp_delta_kernel(const __grid_constant__ RpArgs a) {
+    const long long n = rp_n(a);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= a.cap; i += (long long)gridDim.x * blockDim.x) {
+        long long d = 0;
+        if (i < n) {
+            const int k = a.chosen[i].key_id;
+            d = a.rep_off[k + 1] - a.rep_off[k] - (long long)__ldg(a.key_len + k) * a.L;
+        }
+        a.D[i] = d;
+    }
+}
+
+__global__ void acb_rp_records_kernel(const __grid_constant__ RpArgs a) {
+    const long long n = rp_n(a);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const acb_match m = a.chosen[i];
+        const long long len = __ldg(a.key_len + m.key_id);
+        const long long s = rp_in_off(a, m.hay_id) + ((long long)m.end_index - len + 1) * a.L;
+        const long long p = s + a.D[i], rs = a.rep_off[m.key_id];
+        a.P[i] = p;
+        a.E[i] = p + a.rep_off[m.key_id + 1] - rs;
+        a.IE[i] = s + len * a.L;
+        a.RS[i] = rs;
+    }
+}
+
+/* out_off[h] = in_off[h] + D[first record of a haystack >= h], for h in [0, n_hay]; the last one is the total */
+__global__ void acb_rp_offsets_kernel(const __grid_constant__ RpArgs a) {
+    const long long n = rp_n(a);
+    for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h <= a.n_hay; h += (long long)gridDim.x * blockDim.x) {
+        long long lo = 0, hi = n;
+        while (lo < hi) {
+            const long long mid = (lo + hi) >> 1;
+            if ((long long)a.chosen[mid].hay_id < h) lo = mid + 1; else hi = mid;
+        }
+        const long long o = (h == a.n_hay ? a.total_bytes : rp_in_off(a, h)) + a.D[lo];
+        a.out_off[h] = o;
+        if (h == a.n_hay) *a.total = o;
+    }
+}
+
+/* last j in [lo, hi] with P[j - base] <= o, or lo - 1 */
+__device__ __forceinline__ long long rp_find(const long long *P, long long base, long long lo, long long hi, long long o) {
+    while (lo <= hi) {
+        const long long mid = (lo + hi) >> 1;
+        if (P[mid - base] <= o) lo = mid + 1; else hi = mid - 1;
+    }
+    return hi;
+}
+
+/* ts[t] = the last record with P <= t * kRpTile, for t in [0, n_tiles]; nothing when the output does not fit */
+__global__ void acb_rp_tiles_kernel(const __grid_constant__ RpArgs a) {
+    const long long total = *a.total;
+    if (total > a.out_cap) return;
+    const long long n = rp_n(a), n_tiles = (total + kRpTile - 1) / kRpTile;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t <= n_tiles; t += (long long)gridDim.x * blockDim.x)
+        a.ts[t] = rp_find(a.P, 0, 0, n - 1, t * kRpTile);
+}
+
+/* 16 bytes from p + x, p 16-byte aligned: two aligned loads (one when x is aligned) merged by funnel shifts.  The
+ * second block holds byte x + 15 - (x & 15) + 16 > x + 15 only when x is not aligned, so it always holds a byte of [x, x + 16) */
+__device__ __forceinline__ uint4 rp_load16(const uint8_t *p, long long x) {
+    const uint4 v0 = __ldg(reinterpret_cast<const uint4 *>(p + (x & ~15LL)));
+    const int off = (int)(x & 15);
+    if (off == 0) return v0;
+    const uint4 v1 = __ldg(reinterpret_cast<const uint4 *>(p + (x & ~15LL) + 16));
+    const uint32_t w[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+    const int q = off >> 2, r = (off & 3) * 8;
+    uint32_t s[5];
+#pragma unroll
+    for (int j = 0; j < 5; j++) s[j] = q == 0 ? w[j] : q == 1 ? w[j + 1] : q == 2 ? w[j + 2] : (j + 3 < 8 ? w[j + 3] : 0u);
+    return make_uint4(__funnelshift_r(s[0], s[1], r), __funnelshift_r(s[1], s[2], r), __funnelshift_r(s[2], s[3], r),
+                      __funnelshift_r(s[3], s[4], r));
+}
+
+__global__ void __launch_bounds__(kRpThreads) acb_rp_write_kernel(const __grid_constant__ RpArgs a) {
+    __shared__ long long sP[kRpStage], sE[kRpStage], sIE[kRpStage], sRS[kRpStage];
+    const long long total = *a.total;
+    if (total > a.out_cap) return;
+    const long long n_tiles = (total + kRpTile - 1) / kRpTile;
+    for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const long long lo = max(a.ts[t], 0LL), hi = a.ts[t + 1], m = hi - lo + 1;
+        const bool staged = m > 0 && m <= kRpStage;
+        __syncthreads();                                   /* the previous tile's readers are done */
+        if (staged) {
+            for (int j = threadIdx.x; j < m; j += kRpThreads) {
+                sP[j] = a.P[lo + j]; sE[j] = a.E[lo + j]; sIE[j] = a.IE[lo + j]; sRS[j] = a.RS[lo + j];
+            }
+        }
+        __syncthreads();
+        const long long *P = staged ? sP : a.P, *E = staged ? sE : a.E, *IE = staged ? sIE : a.IE, *RS = staged ? sRS : a.RS;
+        const long long base = staged ? lo : 0;
+        const long long c = t * kRpTile + (long long)threadIdx.x * 16;
+        if (c >= total) continue;
+        long long k = rp_find(P, base, lo, hi, c);
+        const bool in_rep = k >= lo && c < E[k - base];
+        if (in_rep && c + 16 <= E[k - base]) {
+            *reinterpret_cast<uint4 *>(a.out + c) = rp_load16(a.rep, RS[k - base] + (c - P[k - base]));
+            continue;
+        }
+        if (!in_rep && c + 16 <= total && (k == hi || c + 16 <= P[k + 1 - base])) {
+            *reinterpret_cast<uint4 *>(a.out + c) = rp_load16(a.hay, k >= lo ? IE[k - base] + (c - E[k - base]) : c);
+            continue;
+        }
+        uint32_t w[4] = {0u, 0u, 0u, 0u};                 /* a chunk across a boundary: byte by byte */
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const long long o = c + j;
+            if (o < total) {
+                k = rp_find(P, base, max(k, lo), hi, o);
+                uint32_t b;
+                if (k >= lo && o < E[k - base]) b = __ldg(a.rep + RS[k - base] + (o - P[k - base]));
+                else b = __ldg(a.hay + (k >= lo ? IE[k - base] + (o - E[k - base]) : o));
+                w[j >> 2] |= b << (8 * (j & 3));
+            }
+        }
+        if (c + 16 <= total) {
+            *reinterpret_cast<uint4 *>(a.out + c) = make_uint4(w[0], w[1], w[2], w[3]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 16; j++)
+                if (c + j < total) a.out[c + j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+        }
+    }
+}
+} // namespace
+
+static int rp_fits(const acb_replacer *r, const acb_table *tb) {
+    if (r->device != tb->device || r->L != tb->L || r->n_ids < tb->n_keys) {
+        acb_set_error("replacer made for device %d, %d-byte letters and %lld key ids; table: device %d, %d-byte letters, %d key ids",
+                      r->device, r->L, (long long)r->n_ids, tb->device, tb->L, tb->n_keys);
+        return ACB_EINVAL;
+    }
+    return ACB_OK;
+}
+
+extern "C" int acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets,
+                                int64_t n_ids, acb_replacer **out) {
+    if (!tb || !out || rep_bytes < 0 || (rep_bytes && !rep) || !rep_offsets || n_ids < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    if (tb->L != 1 && tb->L != 2 && tb->L != 4) { acb_set_error("not a table"); return ACB_EINVAL; }
+    if (n_ids < tb->n_keys) { acb_set_error("%lld replacements for %d key ids", (long long)n_ids, tb->n_keys); return ACB_EINVAL; }
+    bool ok = rep_offsets[0] == 0 && rep_offsets[n_ids] == rep_bytes;
+    for (int64_t i = 0; ok && i < n_ids; i++) ok = rep_offsets[i + 1] >= rep_offsets[i] && rep_offsets[i + 1] % tb->L == 0;
+    if (!ok) {
+        acb_set_error("replacement offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at rep_bytes");
+        return ACB_EINVAL;
+    }
+    CUDA_TRY(cudaSetDevice(tb->device));
+    acb_replacer *r = new (std::nothrow) acb_replacer();
+    if (!r) { acb_set_error("out of memory"); return ACB_ENOMEM; }
+    r->device = tb->device; r->L = tb->L; r->n_ids = n_ids;
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&r->d_rep), (size_t)rep_bytes + 32);
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&r->d_rep_off), (size_t)(n_ids + 1) * sizeof(long long));
+    if (e == cudaSuccess && rep_bytes) e = cudaMemcpy(r->d_rep, rep, (size_t)rep_bytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(r->d_rep_off, rep_offsets, (size_t)(n_ids + 1) * sizeof(long long), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        acb_set_error("CUDA error %s uploading the replacements: %s", cudaGetErrorName(e), cudaGetErrorString(e));
+        acb_replacer_free(r);
+        return ACB_ECUDA;
+    }
+    *out = r;
+    return ACB_OK;
+}
+
+extern "C" void acb_replacer_free(acb_replacer *r) {
+    if (!r) return;
+    cudaSetDevice(r->device);
+    cudaFree(r->d_rep);
+    cudaFree(r->d_rep_off);
+    delete r;
+}
+
+extern "C" int acb_last_replace_ms(float *ms, int32_t n) {
+    if (!ms || n < 0 || n > 2) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    for (int i = 0; i < n; i++) ms[i] = g_rp_ms[i];
+    return ACB_OK;
+}
+
+static int rp_event(acb_table *tb, int k, cudaStream_t s) {
+    if (!g_timing.load()) return ACB_OK;
+    if (!tb->r_ev[k]) CUDA_TRY(cudaEventCreate(&tb->r_ev[k]));
+    CUDA_TRY(cudaEventRecord(tb->r_ev[k], s));
+    return ACB_OK;
+}
+
+static int rp_launch(const char *what) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { acb_set_error("%s launch failed: %s", what, cudaGetErrorString(e)); return ACB_ECUDA; }
+    g_launches.fetch_add(1);
+    return ACB_OK;
+}
+
+/* The offsets pass on s: a.out_off[0..n_hay] and *a.total.  Carves the per-record arrays from tb->r_buf. */
+static int rp_offsets(acb_table *tb, RpArgs &a, cudaStream_t s) {
+    const size_t C = (size_t)a.cap;
+    size_t temp = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, (long long *)nullptr, (long long *)nullptr, a.cap + 1, s));
+    const size_t need = 6 * 256 + (C + 1) * 8 + 4 * C * 8 + temp;
+    if (tb->r_done) CUDA_TRY(cudaStreamWaitEvent(s, tb->r_done, 0));
+    if (tb->r_buf_cap < need) {
+        if (tb->r_buf) { CUDA_TRY(cudaStreamSynchronize(s)); cudaFree(tb->r_buf); tb->r_buf = nullptr; tb->r_buf_cap = 0; }
+        CUDA_TRY(cudaMalloc(&tb->r_buf, need + need / 4));
+        tb->r_buf_cap = need + need / 4;
+    }
+    char *p = reinterpret_cast<char *>(tb->r_buf);
+    a.D = reinterpret_cast<long long *>(carve(p, (C + 1) * 8));
+    a.P = reinterpret_cast<long long *>(carve(p, C * 8));
+    a.E = reinterpret_cast<long long *>(carve(p, C * 8));
+    a.IE = reinterpret_cast<long long *>(carve(p, C * 8));
+    a.RS = reinterpret_cast<long long *>(carve(p, C * 8));
+    void *tmp = carve(p, temp);
+    const long long most = (long long)tb->sm_count * 16;
+    int rc;
+    if ((rc = rp_event(tb, 0, s))) return rc;
+    acb_rp_delta_kernel<<<(unsigned)std::min<long long>((a.cap + 256) / 256, most), 256, 0, s>>>(a);
+    if ((rc = rp_launch("replacement delta"))) return rc;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, temp, a.D, a.D, a.cap + 1, s));
+    if (a.cap) {
+        acb_rp_records_kernel<<<(unsigned)std::min<long long>((a.cap + 255) / 256, most), 256, 0, s>>>(a);
+        if ((rc = rp_launch("replacement records"))) return rc;
+    }
+    acb_rp_offsets_kernel<<<(unsigned)std::min<long long>((a.n_hay + 256) / 256, most), 256, 0, s>>>(a);
+    if ((rc = rp_launch("replacement offsets"))) return rc;
+    return rp_event(tb, 1, s);
+}
+
+/* The write pass on s: a.out, when *a.total <= a.out_cap (checked on the device).  Then the scratch event and timing. */
+static int rp_write(acb_table *tb, RpArgs &a, cudaStream_t s) {
+    int rc;
+    if ((rc = rp_event(tb, 2, s))) return rc;
+    if (a.out_cap > 0) {
+        const long long max_tiles = (a.out_cap + kRpTile - 1) / kRpTile;
+        if (tb->r_ts_cap < (size_t)max_tiles + 1) {
+            CUDA_TRY(cudaStreamSynchronize(s));
+            if ((rc = ensure(&tb->r_ts, &tb->r_ts_cap, (size_t)max_tiles + 1))) return rc;
+        }
+        a.ts = tb->r_ts;
+        const long long most = (long long)tb->sm_count * 16;
+        acb_rp_tiles_kernel<<<(unsigned)std::min<long long>((max_tiles + 256) / 256, most), 256, 0, s>>>(a);
+        if ((rc = rp_launch("replacement tiles"))) return rc;
+        acb_rp_write_kernel<<<(unsigned)std::min<long long>(max_tiles, (long long)tb->sm_count * 8), kRpThreads, 0, s>>>(a);
+        if ((rc = rp_launch("replacement write"))) return rc;
+    }
+    if ((rc = rp_event(tb, 3, s))) return rc;
+    if (!tb->r_done) CUDA_TRY(cudaEventCreateWithFlags(&tb->r_done, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventRecord(tb->r_done, s));
+    if (g_timing.load()) {
+        CUDA_TRY(cudaEventSynchronize(tb->r_ev[3]));
+        CUDA_TRY(cudaEventElapsedTime(&g_rp_ms[0], tb->r_ev[0], tb->r_ev[1]));
+        CUDA_TRY(cudaEventElapsedTime(&g_rp_ms[1], tb->r_ev[2], tb->r_ev[3]));
+    }
+    return ACB_OK;
+}
+
+static int rp_check(const acb_replacer *r, const acb_table *tb, int64_t total_bytes, int64_t n_hay, int64_t stride_bytes,
+                    bool has_offsets, int64_t out_cap) {
+    if (!r || !tb || total_bytes < 0 || n_hay < 0 || out_cap < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    int rc = rp_fits(r, tb);
+    if (rc) return rc;
+    if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
+    if (!has_offsets && (stride_bytes < 0 || stride_bytes % tb->L || stride_bytes * n_hay != total_bytes)) {
+        acb_set_error("fixed-stride batch needs stride_bytes >= 0, a multiple of letter_bytes, and n_hay*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    return ACB_OK;
+}
+
+static void rp_args(RpArgs &a, const acb_replacer *r, const acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
+                    const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes, const acb_match *d_chosen, int64_t chosen_cap,
+                    const int64_t *d_n_chosen, int64_t *d_out_offsets, uint8_t *d_out, int64_t out_cap, int64_t *d_total) {
+    a = RpArgs{};
+    a.chosen = d_chosen; a.n_chosen = reinterpret_cast<const unsigned long long *>(d_n_chosen); a.cap = chosen_cap;
+    a.key_len = tb->d_keylen; a.rep_off = r->d_rep_off; a.rep = r->d_rep; a.L = tb->L;
+    a.hay = d_hay; a.in_off = reinterpret_cast<const long long *>(d_offsets); a.stride = stride_bytes; a.n_hay = n_hay;
+    a.total_bytes = total_bytes; a.out_cap = out_cap;
+    a.out_off = reinterpret_cast<long long *>(d_out_offsets); a.total = reinterpret_cast<long long *>(d_total); a.out = d_out;
+}
+
+extern "C" int acb_replace_device(acb_replacer *r, acb_table *tb, const uint8_t *d_hay, int64_t total_bytes, const int64_t *d_offsets,
+                                  int64_t n_hay, int64_t stride_bytes, const acb_match *d_chosen, int64_t chosen_cap,
+                                  const int64_t *d_n_chosen, int64_t *d_out_offsets, uint8_t *d_out, int64_t out_cap,
+                                  int64_t *d_total, void *stream) {
+    int rc = rp_check(r, tb, total_bytes, n_hay, stride_bytes, d_offsets != nullptr, out_cap);
+    if (rc) return rc;
+    if ((total_bytes && !d_hay) || chosen_cap < 0 || (chosen_cap && !d_chosen) || !d_n_chosen || !d_out_offsets || !d_total ||
+        (out_cap && !d_out)) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    if ((reinterpret_cast<uintptr_t>(d_hay) | reinterpret_cast<uintptr_t>(d_out)) & 15) {
+        acb_set_error("d_hay and d_out must be 16-byte aligned");
+        return ACB_EINVAL;
+    }
+    for (float &v : g_rp_ms) v = 0.f;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    RpArgs a;
+    rp_args(a, r, tb, d_hay, total_bytes, d_offsets, n_hay, stride_bytes, d_chosen, chosen_cap, d_n_chosen, d_out_offsets, d_out,
+            out_cap, d_total);
+    if ((rc = rp_offsets(tb, a, s))) return rc;
+    return rp_write(tb, a, s);
+}
+
+extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
+                                int64_t n_hay, int64_t stride_bytes, int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap,
+                                int64_t *total) {
+    int rc = rp_check(r, tb, total_bytes, n_hay, stride_bytes, offsets != nullptr, out_cap);
+    if (rc) return rc;
+    if ((total_bytes && !hay) || !out_offsets || !total || (out_cap && !out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("replacement takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
+    if (offsets) {                                          /* the kernels read hay[offsets[h] .. offsets[h+1]) unchecked */
+        bool ok = offsets[0] == 0 && offsets[n_hay] == total_bytes;
+        for (int64_t i = 0; ok && i < n_hay; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % tb->L == 0;
+        if (!ok) {
+            acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes");
+            return ACB_EINVAL;
+        }
+    }
+    *total = 0;
+    for (float &v : g_rp_ms) v = 0.f;
+    if (n_hay == 0) { out_offsets[0] = 0; return ACB_OK; }
+    const int64_t *d_off = nullptr;
+    unsigned long long full = 0;
+    if (total_bytes && (rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, &d_off, &full))) return rc;
+    if (!total_bytes) {                                     /* only empty haystacks: nothing to scan, nothing to write */
+        for (int64_t i = 0; i <= n_hay; i++) out_offsets[i] = 0;
+        return ACB_OK;
+    }
+    cudaStream_t s = tb->stream;
+    if ((rc = ensure(&tb->r_off, &tb->r_off_cap, (size_t)n_hay + 2))) return rc;
+    unsigned long long *d_n = tb->l_ctr + 2;
+    CUDA_TRY(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s));
+    if (full && (rc = ensure(&tb->l_out, &tb->l_out_cap, (size_t)full))) return rc;
+    if (full && (rc = acb_leftmost_longest_device(tb, tb->w_out, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L,
+                                                  tb->l_out, (int64_t)full, reinterpret_cast<int64_t *>(d_n), s)))
+        return rc;
+    RpArgs a;
+    rp_args(a, r, tb, tb->w_hay, total_bytes, d_off, n_hay, stride_bytes, tb->l_out, (int64_t)full, reinterpret_cast<int64_t *>(d_n),
+            reinterpret_cast<int64_t *>(tb->r_off), nullptr, 0, reinterpret_cast<int64_t *>(tb->r_off + n_hay + 1));
+    if ((rc = rp_offsets(tb, a, s))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(out_offsets, tb->r_off, (size_t)(n_hay + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    *total = out_offsets[n_hay];
+    if (*total > out_cap) {
+        acb_set_error("replacement: room for %lld bytes, output %lld", (long long)out_cap, (long long)*total);
+        return ACB_EOVERFLOW;
+    }
+    if ((rc = ensure(&tb->r_out, &tb->r_out_cap, (size_t)std::max<int64_t>(*total, 16)))) return rc;
+    a.out = tb->r_out;
+    a.out_cap = *total;
+    if ((rc = rp_write(tb, a, s))) return rc;
+    if (*total) CUDA_TRY(cudaMemcpyAsync(out, tb->r_out, (size_t)*total, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
     return ACB_OK;
 }
