@@ -474,6 +474,51 @@ int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t
  * on this thread (the first n of them, n <= 2), from CUDA events (the call then waits for them); 0 when timing is off. */
 int acb_last_replace_ms(float *ms, int32_t n);
 
+/* ---- leftmost-longest stream batches: selection and replacement chunk by chunk ------------------------------------
+ * A stream's text is the concatenation of its chunks since its start, its last reset or its last final feed.  What the
+ * feeds of a stream return, concatenated, is exactly what acb_leftmost_longest_device / acb_replace_device return for
+ * that whole text.  Per stream the batch keeps X, the position up to which every match is decided and emitted, and the
+ * pos - X <= T = longest_word - 1 letters after it; a feed reports the chosen matches that start before
+ * pos_new - T (and releases the output up to the same point), because those are the ones no later letter can change.
+ * A final feed (final != 0) decides everything and returns the stream to its start: position 0, nothing held.
+ * acb_streams_reset and acb_streams_positions serve these batches; acb_streams_feed_* refuse them (ACB_EINVAL), and
+ * these feeds refuse the other batches.  Chunks, ids and the overflow contract are those of acb_streams_feed_*: a feed
+ * that does not fit commits nothing and can be repeated.  The device feeds are asynchronous on `stream` except that
+ * they wait for the staged size, the full match list's size (the full list lives in a buffer of the batch, grown to
+ * fit) and, replacing, the decided windows' size.  Feeds of one batch must not overlap in time.  algo: ACB_ALGO_AUTO,
+ * _FILTER or _DFA. */
+int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out);
+
+/* The chosen records in chunk order, then end_index ascending; end_index is relative to the chunk (>= -T: a match may
+ * start in letters held back from earlier chunks).  Zeroes *d_count itself, counts every chosen record, stores the
+ * first cap. */
+int acb_streams_feed_leftmost_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                                     const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
+                                     int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo);
+
+/* HOST buffers: ids and offsets checked (ACB_EINVAL) before anything runs; ACB_EOVERFLOW with the exact count when the
+ * records do not fit cap.  out == NULL works as for acb_scan_host (acb_copy_records / acb_take_records). */
+int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                                   const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
+                                   acb_match *out, int64_t cap, int64_t *n_found, int algo);
+
+/* The replacing feed: per chunk, the stream's decided text [X, X_new) with every chosen match replaced as by
+ * acb_replace_device.  d_out_offsets (n_chunks+1 int64) and *d_total are always written; d_out only when the total is at
+ * most out_cap (checked on the device), and only then does the feed commit.  d_out must be 16-byte aligned. */
+int acb_streams_replace_device(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                               const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids, int final,
+                               int64_t *d_out_offsets, uint8_t *d_out, int64_t out_cap, int64_t *d_total, void *stream, int algo);
+
+/* HOST buffers: out_offsets and *total are always written; out when *total <= out_cap, else ACB_EOVERFLOW. */
+int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                             const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final, int algo,
+                             int64_t *out_offsets, uint8_t *out, int64_t out_cap, int64_t *total);
+
+/* With kernel timing on, the milliseconds of the last leftmost feed's stages on this thread: staging gather, scan,
+ * frontier filter, selection, window gather (replacing feeds), commit (the first n, n <= 6); 0 when timing is off.
+ * acb_last_replace_ms gives a replacing feed's offsets and write passes. */
+int acb_last_stream_leftmost_ms(float *ms, int32_t n);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

@@ -1101,13 +1101,16 @@ class Automaton:
         return ("host", flat, offs, n, 0, narrow)
 
     def stream_batch(self, n_streams: int, *, long: bool = False, algo: str = "auto",
-                     device: Optional[int] = None, ignore_white_space: bool = False) -> "StreamBatch":
+                     device: Optional[int] = None, ignore_white_space: bool = False,
+                     leftmost_longest: bool = False) -> "StreamBatch":
         """`n_streams` independent streams searched chunk by chunk, the next chunk of many of them in one GPU call
         (StreamBatch.feed).  long=False: stream s reports what the reference's ``iter(c0)`` ... ``.set(c1)`` ...
         reports over its chunks -- every match, also those across chunk boundaries; long=True: what
         ``iter_long(c0)`` ... ``.set(c1)`` reports.  What a stream carries from one chunk to the next stays in HBM.
         ignore_white_space=True (find_all batches only): what ``iter(c0, ignore_white_space=True)`` ... ``.set(c1)``
         ... reports; positions still count every letter, and a key that white space splits across chunks is found.
+        leftmost_longest=True: what `find_leftmost_longest_batch` reports for each stream's whole text, delivered as
+        soon as no later letter can change it (see StreamBatch.finish).
 
         Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
         wider chunks, so the latin-1 automaton is not used)."""
@@ -1117,12 +1120,15 @@ class Automaton:
         n_streams = operator.index(n_streams)
         if n_streams < 0:
             raise ValueError("n_streams must not be negative")
+        if leftmost_longest and (long or ignore_white_space):
+            raise ValueError("leftmost_longest stream batches take neither long=True nor ignore_white_space=True")
         if algo not in (("auto", "long") if long else ("auto", "filter", "dfa")):
             raise ValueError(f"algo {algo!r} does not fit a {'long' if long else 'find_all'} stream batch")
         if long and ignore_white_space:
             raise ValueError("iter_long has no ignore_white_space option")
         skip = self._skip_set(False) if ignore_white_space else None
-        return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip)
+        return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip,
+                           bool(leftmost_longest))
 
     # ------------------------------------------------------------------ batch lookups (new)
     # exists / match / longest_prefix / get for a whole batch of keys, in one GPU call (acb_lookup_*).  `keys` takes the
@@ -1330,19 +1336,29 @@ class StreamBatch:
     counted from its start or its last `reset` -- exact past 2^31, unlike the reference's C int (SURVEY A7).  Records
     come in chunk order, then end_index ascending, then longest key first.  ``positions`` is the number of letters
     every stream has consumed.  A stream batch belongs to the key set it was made for: after the key set changes,
-    `feed` and `reset` raise ValueError as a stale iterator does."""
+    `feed` and `reset` raise ValueError as a stale iterator does.
 
-    def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None):
+    A leftmost_longest batch reports, over all feeds and `finish` of a stream, exactly what
+    `find_leftmost_longest_batch` reports for its whole text, each match once, in chunk order then end_index
+    ascending.  A match is reported by the first feed after which it starts before ``position - (longest_word - 1)``:
+    from then on no later letter can change it.  `finish` reports the rest and returns those streams to their start."""
+
+    def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None,
+                 leftmost_longest: bool = False):
         self._A = A
         self._version = A._version
         self.n_streams = n_streams
         self.long = long
+        self.leftmost_longest = leftmost_longest
         self._algo = algo
         self._device = device
         self._pos = np.zeros(n_streams, dtype=np.int64)        # host mirror of the positions, for end_index
         self.ignore_white_space = skip is not None
         with A._gpu_lock:
-            self._ss = self._native("new") if skip is None else self._native("new_skip", skip)
+            if leftmost_longest:
+                self._ss = self._native("new_leftmost")
+            else:
+                self._ss = self._native("new") if skip is None else self._native("new_skip", skip)
 
     def __del__(self):
         try:
@@ -1359,13 +1375,19 @@ class StreamBatch:
     def _native(self, op: str, *args):
         """Every call into the native stream batch (acb_streams_*) goes through here.
           new -> handle;  new_skip(skip set uint32) -> handle of a batch that skips those letters;  free;  reset(ids int32 or None);  positions -> int64[n_streams];
-          feed(kind, data, offsets, n, stride, ids, sort) -> records (hay_id = chunk index, end_index in the chunk)"""
+          feed(kind, data, offsets, n, stride, ids, sort) -> records (hay_id = chunk index, end_index in the chunk);
+          new_leftmost -> handle of a leftmost-longest batch;
+          feed_leftmost(kind, data, offsets, n, stride, ids, final) -> its chosen records, as feed's"""
         A = self._A
         lib = A._lib
         if op == "new":
             ss = ctypes.c_void_p()
             N.check(lib.acb_streams_new(A._ensure_table(self._device), self.n_streams, int(self.long), ctypes.byref(ss)))
             return ss
+        if op == "new_leftmost":
+            return _new_leftmost_streams(A, self.n_streams, self._device)
+        if op == "feed_leftmost":
+            return self._feed_leftmost(*args)
         if op == "new_skip":
             skip, = args
             ss = ctypes.c_void_p()
@@ -1444,33 +1466,84 @@ class StreamBatch:
             raise ValueError("a stream id is given twice")
         return np.ascontiguousarray(a, dtype=np.int32)
 
+    def _feed_leftmost(self, kind, data, offs, n, stride, ids, final):
+        """acb_streams_feed_leftmost_*: the chosen records (hay_id = chunk index, end_index relative to the chunk)"""
+        A = self._A
+        lib = A._lib
+        tb = A._ensure_table(self._device)
+        algo = N.ALGOS[self._algo]
+        cap = max(A._match_cap, 1 << 12, 2 * n)
+        if kind == "device":
+            import torch
+            t = _stream_tensor(data, n, stride, self._device)
+            with torch.cuda.device(t.device):
+                stream = torch.cuda.current_stream().cuda_stream
+                d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
+                cnt = torch.empty(1, dtype=torch.int64, device=t.device)
+                for _ in range(2):
+                    out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+                    N.check(lib.acb_streams_feed_leftmost_device(self._ss, tb, t.data_ptr() if n and stride else None, n * stride,
+                                                                 None, n, stride, None if d_ids is None else d_ids.data_ptr(),
+                                                                 int(final), out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
+                    found = int(cnt.item())
+                    if found <= cap:
+                        break
+                    cap = A._match_cap = found + 1024            # nothing was committed: the same feed again, with room
+                return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
+        total = int(data.size)
+        found = ctypes.c_int64(0)
+        for _ in range(2):
+            rc = lib.acb_streams_feed_leftmost_host(self._ss, tb, N.ptr(data) if total else None, total,
+                                                    None if offs is None else N.ptr(offs), n, stride,
+                                                    None if ids is None else N.ptr(ids), int(final), None, cap,
+                                                    ctypes.byref(found), algo)
+            if rc != N.ACB_EOVERFLOW:
+                break
+            cap = A._match_cap = int(found.value) + 1024
+        N.check(rc)
+        if not found.value:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        return _take_records(lib, tb, found.value)
+
     def feed(self, chunks, ids=None, *, sort: bool = True) -> Matches:
         """The next chunk of some streams: chunk h continues stream ids[h] (default: stream h).  `chunks` takes the
         input forms of find_all_batch; in a list, None is an empty chunk.  Returns the matches that end inside
-        these chunks (see the class)."""
+        these chunks (see the class); a leftmost_longest batch returns the matches this feed settles, already in
+        order (`sort` has no effect)."""
         A = self._A
         with A._gpu_lock:
             self._check()
-            if isinstance(chunks, list) or (isinstance(chunks, tuple) and not (len(chunks) == 2 and isinstance(chunks[0], np.ndarray))):
-                empty = () if A._key_type == KEY_SEQUENCE else ("" if A._UNICODE else b"")
-                chunks = [empty if c is None else c for c in chunks]
-            batch = A._batch_input(chunks, narrow_ok=False)
-            if batch[0] == "device":
-                n, stride = A._device_batch_shape(batch[1])
-                lens = np.full(n, stride // A._L, dtype=np.int64)
-                args = ("device", batch[1], None, n, stride)
-            else:
-                _, flat, offs, n, stride, _ = batch
-                lens = (np.diff(offs) if offs is not None else np.full(n, stride, dtype=np.int64)) // A._L
-                args = ("host", flat, offs, n, stride)
+            args, lens = _stream_chunks(A, chunks)
+            n = args[3]
             ids32 = self._ids(ids, n)
-            rec = self._native("feed", *args, ids32, sort)
+            if self.leftmost_longest:
+                rec = self._native("feed_leftmost", *args, ids32, False)
+            else:
+                rec = self._native("feed", *args, ids32, sort)
             sid = np.arange(n, dtype=np.int64) if ids32 is None else ids32.astype(np.int64)
             m = Matches(rec, A._values)
             chunk = rec["hay_id"]
             m.hay_id = sid[chunk]
             m.end_index = rec["end_index"].astype(np.int64) + self._pos[m.hay_id]
             self._pos[sid] += lens
+            return m
+
+    def finish(self, ids=None) -> Matches:
+        """leftmost_longest batches: the matches streams `ids` (default: all) still hold back, as if their text ended
+        here; those streams then start again at position 0 with nothing held.  Other stream batches: ValueError."""
+        if not self.leftmost_longest:
+            raise ValueError("finish() belongs to leftmost_longest stream batches")
+        A = self._A
+        with A._gpu_lock:
+            self._check()
+            n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
+            ids32 = self._ids(ids, n)
+            rec = self._native("feed_leftmost", "host", np.empty(0, np.uint8), np.zeros(n + 1, np.int64), n, 0, ids32, True)
+            sid = np.arange(n, dtype=np.int64) if ids32 is None else ids32.astype(np.int64)
+            m = Matches(rec, A._values)
+            m.hay_id = sid[rec["hay_id"]]
+            m.end_index = rec["end_index"].astype(np.int64) + self._pos[m.hay_id]
+            self._pos[sid] = 0
             return m
 
     def reset(self, ids=None) -> None:
@@ -1589,6 +1662,21 @@ class Replacer:
                 return out, out_offs
             return self._items(out, out_offs, narrow)
 
+    def stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None) -> "ReplaceStream":
+        """`n_streams` streams rewritten chunk by chunk (ReplaceStream.feed): over all feeds and `finish` of a stream,
+        the output is exactly what `replace_batch` gives for its whole text.  Streams run at the automaton's full letter
+        width (unicode: 4 bytes per letter), as every stream batch does."""
+        A = self._A
+        if self._version != A._version:
+            raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
+        A._require_automaton()
+        n_streams = operator.index(n_streams)
+        if n_streams < 0:
+            raise ValueError("n_streams must not be negative")
+        if algo not in ("auto", "filter", "dfa"):
+            raise ValueError(f"algo {algo!r}: a replacing stream batch takes 'auto', 'filter' or 'dfa'")
+        return ReplaceStream(self, n_streams, algo, self._device if device is None else device)
+
     def _items(self, out: np.ndarray, offs: np.ndarray, narrow: bool) -> list:
         """the output haystacks as objects of the input's type"""
         A = self._A
@@ -1654,6 +1742,142 @@ class Replacer:
             if m:
                 N.check(A._lib.acb_replace_device(*args, out.data_ptr(), m, total.data_ptr(), stream))
         return out, out_offs
+
+
+class ReplaceStream:
+    """Result of `Replacer.stream_batch()`: `n_streams` streams rewritten chunk by chunk, what they hold back kept on the
+    GPU.  ``feed(chunks, ids=None)`` returns, per chunk, the stream's output that no later letter can change (every
+    letter before ``position - (longest_word - 1)`` and every replacement that starts there); ``finish(ids=None)``
+    returns the rest and returns those streams to their start.  Concatenated, a stream's outputs are what
+    `Replacer.replace_batch` gives for its whole text.  Stale (ValueError) when the replacer is."""
+
+    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int):
+        self._R = R
+        self._A = R._A
+        self._version = R._version
+        self.n_streams = n_streams
+        self._algo = algo
+        self._device = device
+        with self._A._gpu_lock:
+            self._ss = self._native("new")
+
+    def __del__(self):
+        try:
+            if getattr(self, "_ss", None) is not None:
+                self._native("free")
+                self._ss = None
+        except Exception:                                   # interpreter shutdown
+            pass
+
+    def _check(self):
+        if self._version != self._A._version:
+            raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
+
+    def _native(self, op: str, *args):
+        """Every call into the native batch goes through here.  new -> handle;  free;  reset(ids int32 or None);
+        positions -> int64[n_streams];  feed(kind, data, offsets, n, stride, ids, final) -> (output bytes, output
+        offsets int64[n+1]), numpy arrays for host chunks, CUDA tensors for a CUDA tensor"""
+        A = self._A
+        lib = A._lib
+        if op == "new":
+            return _new_leftmost_streams(A, self.n_streams, self._device)
+        if op == "free":
+            lib.acb_streams_free(self._ss)
+            return None
+        if op == "reset":
+            ids, = args
+            N.check(lib.acb_streams_reset(self._ss, None if ids is None else N.ptr(ids), 0 if ids is None else len(ids)))
+            return None
+        if op == "positions":
+            out = np.empty(max(self.n_streams, 1), dtype=np.int64)
+            N.check(lib.acb_streams_positions(self._ss, N.ptr(out), self.n_streams))
+            return out[:self.n_streams]
+        kind, data, offs, n, stride, ids, final = args
+        tb = A._ensure_table(self._device)
+        r = self._R._replacer(tb, False, self._device)
+        algo = N.ALGOS[self._algo]
+        held = n * max(int(lib.acb_trie_longest_word(A._trie)) - 1, 0) * A._L     # at most what the streams hold back
+        if kind == "device":
+            import torch
+            t = _stream_tensor(data, n, stride, self._device)
+            with torch.cuda.device(t.device):
+                stream = torch.cuda.current_stream().cuda_stream
+                d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
+                out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+                total = torch.empty(1, dtype=torch.int64, device=t.device)
+                cap = (n * stride + held) * 5 // 4 + 4096
+                for _ in range(2):
+                    out = torch.empty(cap, dtype=torch.uint8, device=t.device)
+                    N.check(lib.acb_streams_replace_device(self._ss, r, tb, t.data_ptr() if n and stride else None, n * stride,
+                                                           None, n, stride, None if d_ids is None else d_ids.data_ptr(),
+                                                           int(final), out_offs.data_ptr(), out.data_ptr(), cap,
+                                                           total.data_ptr(), stream, algo))
+                    m = int(total.item())                   # the size of the output
+                    if m <= cap:
+                        break
+                    cap = m                                 # nothing was committed: the same feed again, with room
+                return out[:m], out_offs
+        size = int(data.size)
+        out_offs = np.empty(n + 1, dtype=np.int64)
+        total = ctypes.c_int64(0)
+        cap = (size + held) * 5 // 4 + 4096
+        for _ in range(2):
+            out = np.empty(cap, dtype=np.uint8)
+            rc = lib.acb_streams_replace_host(self._ss, r, tb, N.ptr(data) if size else None, size,
+                                              None if offs is None else N.ptr(offs), n, stride,
+                                              None if ids is None else N.ptr(ids), int(final), algo, N.ptr(out_offs),
+                                              N.ptr(out), cap, ctypes.byref(total))
+            if rc != N.ACB_EOVERFLOW:
+                break
+            cap = int(total.value)
+        N.check(rc)
+        return out[:total.value], out_offs
+
+    def _ids(self, ids, n: int) -> Optional[np.ndarray]:
+        return StreamBatch._ids(self, ids, n)
+
+    def feed(self, chunks, ids=None):
+        """The next chunk of some streams (chunk h continues stream ids[h], default stream h), in the input forms of
+        find_all_batch; in a list, None is an empty chunk.  Returns the output each chunk releases: a list gives a list
+        of the same item type, uint8[n, stride] or (flat, offsets) gives (flat uint8, offsets int64[n+1]), a CUDA
+        tensor gives that pair as CUDA tensors computed on torch's current stream."""
+        A = self._A
+        with A._gpu_lock:
+            self._check()
+            as_list = not (isinstance(chunks, np.ndarray) or (isinstance(chunks, tuple) and len(chunks) == 2 and
+                                                              all(isinstance(x, np.ndarray) for x in chunks))
+                           or (type(chunks).__module__.startswith("torch") and getattr(chunks, "is_cuda", False)))
+            args, _ = _stream_chunks(A, chunks)
+            out, offs = self._native("feed", *args, self._ids(ids, args[3]), False)
+            return self._R._items(out, offs, False) if as_list else (out, offs)
+
+    def finish(self, ids=None) -> list:
+        """The output streams `ids` (default: all) still hold back, one item of the haystack type per id; those streams
+        then start again at position 0 with nothing held."""
+        A = self._A
+        with A._gpu_lock:
+            self._check()
+            n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
+            out, offs = self._native("feed", "host", np.empty(0, np.uint8), np.zeros(n + 1, np.int64), n, 0, self._ids(ids, n), True)
+            return self._R._items(out, offs, False)
+
+    def reset(self, ids=None) -> None:
+        """Streams `ids` (default: all) back to their start, dropping what they hold back."""
+        with self._A._gpu_lock:
+            self._check()
+            if ids is None:
+                self._native("reset", None)
+                return
+            a = np.asarray(ids)
+            if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)) or (a.size and (a.min() < 0 or a.max() >= self.n_streams)):
+                raise ValueError(f"stream ids must be integers in [0, {self.n_streams})")
+            self._native("reset", np.unique(a).astype(np.int32))
+
+    @property
+    def positions(self) -> np.ndarray:
+        """int64[n_streams]: letters every stream has consumed since its start, its last reset or its last finish."""
+        with self._A._gpu_lock:
+            return self._native("positions")
 
 
 class AutomatonSearchIter:
@@ -1861,6 +2085,36 @@ def _take_records(lib, tb, found: int) -> np.ndarray:
     if not ptr.value or n.value != found:
         raise N.NativeError("acb_take_records: no records to take")
     return np.asarray(_PinnedRecords(lib, ptr.value, n.value, room.value))
+
+
+def _stream_chunks(A: Automaton, chunks):
+    """A stream feed's chunks in the input forms of find_all_batch (in a list, None is an empty chunk) at the
+    automaton's full letter width -> ((kind, data, offsets, n, stride), letters per chunk int64[n])"""
+    if isinstance(chunks, list) or (isinstance(chunks, tuple) and not (len(chunks) == 2 and isinstance(chunks[0], np.ndarray))):
+        empty = () if A._key_type == KEY_SEQUENCE else ("" if A._UNICODE else b"")
+        chunks = [empty if c is None else c for c in chunks]
+    batch = A._batch_input(chunks, narrow_ok=False)
+    if batch[0] == "device":
+        n, stride = A._device_batch_shape(batch[1])
+        return ("device", batch[1], None, n, stride), np.full(n, stride // A._L, dtype=np.int64)
+    _, flat, offs, n, stride, _ = batch
+    lens = (np.diff(offs) if offs is not None else np.full(n, stride, dtype=np.int64)) // A._L
+    return ("host", flat, offs, n, stride), lens
+
+
+def _stream_tensor(t, n: int, stride: int, device: int):
+    """a CUDA tensor of chunks for a stream batch on `device`, 16-byte aligned"""
+    import torch
+    dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+    if dev != device:
+        raise ValueError(f"chunks on cuda:{dev} for a stream batch on cuda:{device}")
+    return _aligned(t) if n and stride else t
+
+
+def _new_leftmost_streams(A: Automaton, n_streams: int, device: int):
+    ss = ctypes.c_void_p()
+    N.check(A._lib.acb_streams_new_leftmost(A._ensure_table(device), n_streams, ctypes.byref(ss)))
+    return ss
 
 
 def _aligned(t):

@@ -2521,6 +2521,22 @@ struct acb_streams {
     int32_t *d_ids = nullptr; size_t ids_cap = 0;                 /* ids of a host feed or a reset, uploaded */
     std::vector<uint32_t> skip;                                   /* the skip set (find_all batches only), host copy */
     long long *d_kept = nullptr;                                  /* with a skip set: kept letters consumed per stream */
+    /* leftmost-longest batches (acb_streams_new_leftmost): the tail holds the letters after X, the position up to which
+     * every match is decided and emitted; d_hold[s] = pos - X of stream s (<= T).  Per-feed scratch, grown on demand. */
+    int leftmost = 0;
+    long long *d_hold = nullptr;
+    long long *d_soff = nullptr; size_t soff_cap = 0;             /* staged byte offsets [n_chunks + 1] */
+    long long *d_aux = nullptr; size_t aux_cap = 0;               /* per chunk: last chosen end, new X, window offsets */
+    uint8_t *d_stage = nullptr; size_t stage_cap = 0;             /* held || chunk, per chunk */
+    uint8_t *d_win = nullptr; size_t win_cap = 0;                 /* replacing feeds: the decided windows [X, X_new) */
+    long long *d_ts = nullptr; size_t ts_cap = 0;                 /* first haystack of every gather tile */
+    acb_match *d_full = nullptr; size_t full_cap = 0;             /* the full list of the staged batch */
+    acb_match *d_settled = nullptr; size_t settled_cap = 0;       /* ... the records that start before the frontier */
+    uint8_t *d_flag = nullptr; size_t flag_cap = 0;
+    acb_match *d_chosen = nullptr; size_t chosen_cap = 0;         /* replacing feeds: the chosen records */
+    void *d_tmp = nullptr; size_t tmp_cap = 0;                    /* cub scratch */
+    unsigned long long *d_ctr = nullptr, *h_ctr = nullptr;        /* [0] full, [1] settled, [2] chosen, [3] sizes; h_ctr pinned */
+    cudaEvent_t ev[12] = {};                                      /* kernel timing, a pair per stage */
 };
 
 static int32_t tail_letters(const acb_table *tb) { return std::max<int32_t>(tb->max_key_bytes / tb->L - 1, 0); }
@@ -2546,6 +2562,11 @@ extern "C" void acb_streams_free(acb_streams *ss) {
     cudaSetDevice(ss->device);
     cudaFree(ss->d_pos); cudaFree(ss->d_tail); cudaFree(ss->d_state); cudaFree(ss->d_next_tail);
     cudaFree(ss->d_start); cudaFree(ss->d_end); cudaFree(ss->d_ids); cudaFree(ss->d_kept);
+    cudaFree(ss->d_hold); cudaFree(ss->d_soff); cudaFree(ss->d_aux); cudaFree(ss->d_stage); cudaFree(ss->d_win); cudaFree(ss->d_ts);
+    cudaFree(ss->d_full); cudaFree(ss->d_settled); cudaFree(ss->d_flag); cudaFree(ss->d_chosen); cudaFree(ss->d_tmp);
+    cudaFree(ss->d_ctr);
+    if (ss->h_ctr) cudaFreeHost(ss->h_ctr);
+    for (cudaEvent_t e : ss->ev) if (e) cudaEventDestroy(e);
     delete ss;
 }
 
@@ -2579,10 +2600,11 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
                         int64_t n_chunks, int64_t stride, const int32_t *d_ids, acb_match *d_out, int64_t cap,
                         int64_t *d_count, cudaStream_t s, int algo) {
     if (!ss || !tb || !d_count || total < 0 || n_chunks < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (ss->leftmost) { acb_set_error("a leftmost-longest stream batch takes acb_streams_feed_leftmost_* or acb_streams_replace_*"); return ACB_EINVAL; }
     int rc = streams_check_table(ss, tb);
     if (rc != ACB_OK) return rc;
     if (n_chunks > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, ss->n); return ACB_EINVAL; }
-    if (!d_off && n_chunks && (stride <= 0 || stride % ss->L || stride * n_chunks != total)) {
+    if (!d_off && n_chunks && (stride <= 0|| stride % ss->L || stride * n_chunks != total)) {
         acb_set_error("fixed-stride feed needs stride_bytes > 0, a multiple of letter_bytes, and n_chunks*stride == total_bytes");
         return ACB_EINVAL;
     }
@@ -2669,6 +2691,7 @@ extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8
     if (!ss || !tb || !n_found || total_bytes < 0 || n_chunks < 0 || cap < 0 || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
     tb->h_out_n = 0;
+    if (ss->leftmost) { acb_set_error("a leftmost-longest stream batch takes acb_streams_feed_leftmost_* or acb_streams_replace_*"); return ACB_EINVAL; }
     int rc;
     if (ids && (rc = check_ids(ss, ids, n_chunks))) return rc;
     if ((rc = streams_check_table(ss, tb))) return rc;
@@ -2731,10 +2754,13 @@ extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n)
     } else if (n) {
         if ((rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)n))) return rc;
         CUDA_TRY(cudaMemcpy(ss->d_ids, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice));
-        acb_streams_reset_kernel<<<(unsigned)((n + 255) / 256), 256>>>(streams_args(ss, ss->d_ids), n);
+        StreamsArgs a = streams_args(ss, ss->d_ids);
+        if (ss->d_hold) a.kept = ss->d_hold;                     /* leftmost (no skip set): nothing held back either */
+        acb_streams_reset_kernel<<<(unsigned)((n + 255) / 256), 256>>>(a, n);
         CUDA_TRY(cudaGetLastError());
         g_launches.fetch_add(1);
     }
+    if (!ids && ss->d_hold) CUDA_TRY(cudaMemset(ss->d_hold, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(long long)));
     CUDA_TRY(cudaDeviceSynchronize());
     return ACB_OK;
 }
@@ -3944,6 +3970,525 @@ extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *h
     a.out = tb->r_out;
     a.out_cap = *total;
     if ((rc = rp_write(tb, a, s))) return rc;
+    if (*total) CUDA_TRY(cudaMemcpyAsync(out, tb->r_out, (size_t)*total, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return ACB_OK;
+}
+
+/* ------------------------------------------------------------ leftmost-longest stream batches */
+/* A leftmost-longest stream batch keeps, per stream, X: the position up to which every match is decided and emitted,
+ * and in its tail the pos - X <= T letters after it.  A feed:
+ *  1. stages held || chunk per chunk (a length kernel, an exclusive scan, a tiled gather);
+ *  2. scans the staged batch with acb_scan_device: from the root at X it finds exactly the matches that start at or
+ *     after X, since the greedy chain has no match starting in [last chosen end + 1, X);
+ *  3. keeps the records that start before the frontier F = pos_new - T (all of them on a final feed): they end before
+ *     pos_new, so every match that can decide a choice among them is known;
+ *  4. selects with acb_leftmost_longest_device;
+ *  5. computes X_new = max(X, F, end of the last chosen record + 1) (pos_new on a final feed) and, for a replacing
+ *     feed, rewrites the windows [X, X_new) with acb_replace_device;
+ *  6. commits the new held letters, X and the position, only when everything fit the caller's buffers.
+ * DESIGN section 4.13 gives the exactness argument. */
+namespace {
+constexpr int kSlTile = 4096;                              /* output bytes per block turn of the ragged gather */
+constexpr int kSlHays = 512;                               /* haystack offsets a gather block keeps in shared memory */
+constexpr int kSlLanes = 8;                                /* lanes per chunk of the commit's tail copy */
+thread_local float g_sl_ms[6] = {};                        /* kernel timing: stage, scan, filter, selection, window, commit */
+
+struct SlArgs {
+    const int32_t *ids; long long n_streams;               /* chunk -> stream, as StreamsArgs */
+    long long *pos, *hold; uint8_t *tail; int T, L;
+    const uint8_t *chunks; const long long *off; long long stride;   /* the caller's chunks */
+    long long n;                                           /* chunks */
+    long long *soff;                                       /* staged byte offsets [n + 1] */
+    uint8_t *stage;
+    long long *last, *xn, *woff;                           /* per chunk: last chosen end (staged letters) or -1, new X
+                                                              (staged letters), window byte offsets [n + 1] */
+    int final;
+};
+
+__device__ __forceinline__ long long sl_stream(const SlArgs &a, long long h) {
+    const long long s = a.ids ? (long long)__ldg(a.ids + h) : h;
+    return (s >= 0 && s < a.n_streams) ? s : -1;
+}
+
+__device__ __forceinline__ long long sl_chunk_bytes(const SlArgs &a, long long h, long long &begin) {
+    begin = a.off ? a.off[h] : h * a.stride;
+    return a.off ? a.off[h + 1] - begin : a.stride;
+}
+
+/* soff[h] = bytes of held || chunk h (soff[n] = 0), for the exclusive scan that makes them offsets */
+__global__ void acb_sl_len_kernel(const __grid_constant__ SlArgs a) {
+    for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h <= a.n; h += (long long)gridDim.x * blockDim.x) {
+        long long b = 0, len = 0;
+        if (h < a.n) {
+            const long long s = sl_stream(a, h);
+            len = sl_chunk_bytes(a, h, b) + (s < 0 ? 0 : a.hold[s] * a.L);
+        }
+        a.soff[h] = len;
+    }
+}
+
+/* last j in [lo, hi] with o(j) <= x, o(lo) <= x */
+template <class O>
+__device__ __forceinline__ long long sl_find(const O &o, long long lo, long long hi, long long x) {
+    while (lo < hi) {
+        const long long mid = (lo + hi + 1) >> 1;
+        if (o(mid) <= x) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+/* ts[t] = the haystack that holds output byte t * kSlTile (the last h with doff[h] <= it), one lane per tile */
+__global__ void acb_sl_tiles_kernel(const long long *doff, long long n, long long total, long long *ts) {
+    const long long n_tiles = (total + kSlTile - 1) / kSlTile;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n_tiles; t += (long long)gridDim.x * blockDim.x)
+        ts[t] = sl_find([&](long long j) { return doff[j]; }, 0, n - 1, t * kSlTile);
+}
+
+/* A ragged gather: output haystack h = [doff[h], doff[h+1]) is its first `head` bytes from the tail of its stream, then
+ * the rest from a source haystack.  kStage: held || chunk (head = held letters, source = the caller's chunk); else the
+ * window [X, X_new) (head = 0, source = the staged haystack).  Blocks take tiles of kSlTile output bytes, start at the
+ * tile's first haystack ts[t] and keep the following offsets in shared memory; each thread writes one 16-byte chunk,
+ * from two aligned 16-byte loads when it lies in one source run, else byte by byte. */
+template <bool kStage>
+__global__ void __launch_bounds__(256) acb_sl_gather_kernel(const __grid_constant__ SlArgs a, const long long *doff, const long long *ts,
+                                                             uint8_t *dst, long long total) {
+    __shared__ long long s_off[kSlHays + 1];
+    const long long n_tiles = (total + kSlTile - 1) / kSlTile;
+    const uint8_t *base = kStage ? a.chunks : a.stage;
+    for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const long long c0 = t * kSlTile, h0 = ts[t];
+        const int nh = (int)min((long long)kSlHays, a.n - h0);
+        __syncthreads();                                   /* the previous tile's readers are done */
+        for (int j = threadIdx.x; j <= nh; j += blockDim.x) s_off[j] = doff[h0 + j];
+        __syncthreads();
+        const auto O = [&](long long j) { return j - h0 <= nh ? s_off[j - h0] : doff[j]; };
+        const auto F = [&](long long from, long long x) {  /* within the shared offsets when x lies before their end */
+            return sl_find(O, from, x < s_off[nh] ? h0 + nh - 1 : a.n - 1, x);
+        };
+        const long long c = c0 + (long long)threadIdx.x * 16;
+        if (c >= total) continue;
+        long long h = F(h0, c), lo = O(h), hi = O(h + 1), hd = 0;
+        const uint8_t *tp = nullptr, *sp;                  /* the held letters; sp[o - lo] = source byte of output o */
+        const auto enter = [&]() {
+            long long b;
+            if (kStage) {
+                const long long s = sl_stream(a, h);
+                hd = s < 0 ? 0 : a.hold[s] * a.L;
+                tp = a.tail + (s < 0 ? 0 : s) * a.T * a.L;
+                sl_chunk_bytes(a, h, b);
+            } else {
+                b = a.soff[h];
+            }
+            sp = base + b - hd;
+        };
+        enter();
+        if (c - lo >= hd && c + 16 <= hi) {
+            *reinterpret_cast<uint4 *>(dst + c) = rp_load16(base, (sp - base) + (c - lo));
+            continue;
+        }
+        uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const long long o = c + j;
+            if (o < total) {
+                if (o >= hi) { h = F(h + 1, o); lo = O(h); hi = O(h + 1); enter(); }
+                const long long rel = o - lo;
+                const uint32_t b = rel < hd ? tp[rel] : sp[rel];
+                w[j >> 2] |= b << (8 * (j & 3));
+            }
+        }
+        if (c + 16 <= total) {
+            *reinterpret_cast<uint4 *>(dst + c) = make_uint4(w[0], w[1], w[2], w[3]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 16; j++)
+                if (c + j < total) dst[c + j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+        }
+    }
+}
+
+/* flag[i]: record i of the full list starts before its chunk's frontier (every record on a final feed) */
+__global__ void acb_sl_flag_kernel(const __grid_constant__ SlArgs a, const acb_match *full, const unsigned long long *count,
+                                   long long cap, const int32_t *key_len, uint8_t *flag) {
+    const long long m = min((long long)*count, cap);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (long long)gridDim.x * blockDim.x) {
+        bool keep = false;
+        if (i < m) {
+            const acb_match r = full[i];
+            const long long staged = (a.soff[r.hay_id + 1] - a.soff[r.hay_id]) / a.L;
+            keep = a.final || (long long)r.end_index - __ldg(key_len + r.key_id) + 1 < staged - a.T;
+        }
+        flag[i] = keep;
+    }
+}
+
+/* last[h] = end of chunk h's last chosen record (staged letters); rebase: end_index relative to the chunk */
+__global__ void acb_sl_last_kernel(const __grid_constant__ SlArgs a, acb_match *rec, const unsigned long long *count, long long cap,
+                                   int rebase) {
+    const long long m = min((long long)*count, cap);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (long long)gridDim.x * blockDim.x) {
+        const int32_t h = rec[i].hay_id, e = rec[i].end_index;
+        if (i + 1 == m || rec[i + 1].hay_id != h) a.last[h] = e;
+        if (rebase) {
+            const long long s = sl_stream(a, h);
+            rec[i].end_index = (int32_t)(e - (s < 0 ? 0 : a.hold[s]));
+        }
+    }
+}
+
+/* xn[h] = X_new - X in letters; woff[h] = its bytes (woff[n] = 0), for the exclusive scan that makes the window offsets */
+__global__ void acb_sl_frontier_kernel(const __grid_constant__ SlArgs a) {
+    for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h <= a.n; h += (long long)gridDim.x * blockDim.x) {
+        if (h == a.n) { a.woff[h] = 0; continue; }
+        const long long staged = (a.soff[h + 1] - a.soff[h]) / a.L;
+        const long long x = a.final ? staged : max(max(0LL, staged - a.T), a.last[h] + 1);
+        a.xn[h] = x;
+        a.woff[h] = x * a.L;
+    }
+}
+
+/* kSlLanes lanes per chunk: when the feed's records (count <= cap) and output (*total <= out_cap) fit, the letters after the
+ * new X become the stream's tail, and X and the position move (a final feed leaves the stream at its start) */
+__global__ void acb_sl_commit_kernel(const __grid_constant__ SlArgs a, const unsigned long long *count, long long cap,
+                                     const long long *total, long long out_cap) {
+    if ((count && *count > (unsigned long long)cap) || (total && *total > out_cap)) return;
+    const long long h = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / kSlLanes;
+    const int lane = threadIdx.x % kSlLanes;
+    if (h >= a.n) return;
+    const long long s = sl_stream(a, h);
+    if (s < 0) return;
+    const long long staged = (a.soff[h + 1] - a.soff[h]) / a.L, x = a.xn[h], keep = staged - x;
+    const uint8_t *from = a.stage + a.soff[h] + x * a.L;
+    uint8_t *to = a.tail + s * a.T * a.L;
+    for (long long j = lane; j < keep * a.L; j += kSlLanes) to[j] = from[j];
+    if (lane == 0) {
+        long long b;
+        const long long n = sl_chunk_bytes(a, h, b) / a.L;
+        a.pos[s] = a.final ? 0 : a.pos[s] + n;
+        a.hold[s] = a.final ? 0 : keep;
+    }
+}
+} // namespace
+
+extern "C" int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out) {
+    if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    int rc = acb_streams_new(tb, n_streams, 0, out);
+    if (rc != ACB_OK) return rc;
+    acb_streams *ss = *out;
+    ss->leftmost = 1;
+    const size_t n = (size_t)std::max<int64_t>(n_streams, 1);
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ss->d_hold), n * sizeof(long long));
+    if (e == cudaSuccess) e = cudaMemset(ss->d_hold, 0, n * sizeof(long long));
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ss->d_ctr), 4 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void **>(&ss->h_ctr), 4 * sizeof(unsigned long long));
+    if (e != cudaSuccess) {
+        acb_set_error("allocating %lld streams: %s", (long long)n_streams, cudaGetErrorString(e));
+        acb_streams_free(ss);
+        *out = nullptr;
+        return ACB_ECUDA;
+    }
+    return ACB_OK;
+}
+
+extern "C" int acb_last_stream_leftmost_ms(float *ms, int32_t n) {
+    if (!ms || n < 0 || n > 6) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    for (int i = 0; i < n; i++) ms[i] = g_sl_ms[i];
+    return ACB_OK;
+}
+
+static int sl_event(acb_streams *ss, int k, cudaStream_t s) {
+    if (!g_timing.load()) return ACB_OK;
+    if (!ss->ev[k]) CUDA_TRY(cudaEventCreate(&ss->ev[k]));
+    CUDA_TRY(cudaEventRecord(ss->ev[k], s));
+    return ACB_OK;
+}
+
+static int sl_launch(const char *what) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { acb_set_error("%s launch failed: %s", what, cudaGetErrorString(e)); return ACB_ECUDA; }
+    g_launches.fetch_add(1);
+    return ACB_OK;
+}
+
+/* the arguments every leftmost feed checks before anything runs */
+static int sl_check(const acb_streams *ss, const acb_table *tb, int64_t total, const void *offsets, int64_t n, int64_t stride,
+                    int *algo) {
+    if (!ss || !tb || total < 0 || n < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (!ss->leftmost) { acb_set_error("not a leftmost-longest stream batch (acb_streams_new_leftmost)"); return ACB_EINVAL; }
+    int rc = streams_check_table(ss, tb);
+    if (rc != ACB_OK) return rc;
+    if (n > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n, ss->n); return ACB_EINVAL; }
+    if (n >= 0x7fffffffLL) { acb_set_error("2^31-1 or more chunks in one feed"); return ACB_ERANGE; }
+    if (!offsets && (stride < 0|| stride % ss->L || stride * n != total)) {
+        acb_set_error("fixed-stride feed needs stride_bytes >= 0, a multiple of letter_bytes, and n_chunks*stride == total_bytes");
+        return ACB_EINVAL;
+    }
+    if (*algo == ACB_ALGO_AUTO) *algo = ACB_ALGO_FILTER;
+    if (*algo != ACB_ALGO_FILTER && *algo != ACB_ALGO_DFA) { acb_set_error("a leftmost-longest feed takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
+    return ACB_OK;
+}
+
+/* cub scratch of at least `bytes` */
+static int sl_tmp(acb_streams *ss, size_t bytes) {
+    uint8_t *p = static_cast<uint8_t *>(ss->d_tmp);
+    int rc = ensure(&p, &ss->tmp_cap, bytes);
+    ss->d_tmp = p;
+    return rc;
+}
+
+/* d_soff[0..n] <- exclusive scan of d_soff[0..n] in place; the total to the host (the one wait of the staging) */
+static int sl_offsets(acb_streams *ss, long long *d, int64_t n, cudaStream_t s, long long *total) {
+    size_t temp = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, d, d, (int)(n + 1), s));
+    int rc = sl_tmp(ss, temp);
+    if (rc) return rc;
+    temp = ss->tmp_cap;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(ss->d_tmp, temp, d, d, (int)(n + 1), s));
+    CUDA_TRY(cudaMemcpyAsync(ss->h_ctr + 3, d + n, sizeof(long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    *total = (long long)ss->h_ctr[3];
+    return ACB_OK;
+}
+
+static int sl_gather(acb_streams *ss, acb_table *tb, const SlArgs &a, bool stage, const long long *doff, uint8_t *dst, long long total,
+                     cudaStream_t s) {
+    if (total == 0) return ACB_OK;
+    const long long n_tiles = (total + kSlTile - 1) / kSlTile;
+    int rc = ensure(&ss->d_ts, &ss->ts_cap, (size_t)n_tiles);
+    if (rc) return rc;
+    acb_sl_tiles_kernel<<<(unsigned)std::min<long long>((n_tiles + 255) / 256, (long long)tb->sm_count * 16), 256, 0, s>>>(doff, a.n, total,
+                                                                                                                   ss->d_ts);
+    if ((rc = sl_launch("stream gather tiles"))) return rc;
+    const unsigned grid = (unsigned)std::min<long long>(n_tiles, (long long)tb->sm_count * 8);
+    if (stage) acb_sl_gather_kernel<true><<<grid, 256, 0, s>>>(a, doff, ss->d_ts, dst, total);
+    else acb_sl_gather_kernel<false><<<grid, 256, 0, s>>>(a, doff, ss->d_ts, dst, total);
+    return sl_launch("stream gather");
+}
+
+/* The leftmost feed on DEVICE buffers, both forms.  r == nullptr: the chosen records go to d_out (cap, *d_count,
+ * end_index relative to the chunk); else the decided windows are rewritten into d_rout (d_rout_off, *d_rtotal,
+ * out_cap).  Waits for the staged size, for the full list's size, and (replacing) for the windows' size. */
+static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_t *d_chunks, int64_t total, const int64_t *d_off,
+                   int64_t n, int64_t stride, const int32_t *d_ids, int final, acb_match *d_out, int64_t cap, int64_t *d_count,
+                   int64_t *d_rout_off, uint8_t *d_rout, int64_t out_cap, int64_t *d_rtotal, cudaStream_t s, int algo) {
+    int rc;
+    for (float &v : g_sl_ms) v = 0.f;
+    CUDA_TRY(cudaSetDevice(ss->device));
+    if (!r) CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
+    if (n == 0) {
+        if (r) CUDA_TRY(cudaMemsetAsync(d_rout_off, 0, sizeof(int64_t), s));
+        if (r) CUDA_TRY(cudaMemsetAsync(d_rtotal, 0, sizeof(int64_t), s));
+        return ACB_OK;
+    }
+    if (total && (reinterpret_cast<uintptr_t>(d_chunks) & 15)) { acb_set_error("d_chunks must be 16-byte aligned"); return ACB_EINVAL; }
+    const size_t N = (size_t)n;
+    if ((rc = ensure(&ss->d_soff, &ss->soff_cap, N + 1)) || (rc = ensure(&ss->d_aux, &ss->aux_cap, 3 * N + 1))) return rc;
+    SlArgs a;
+    memset(&a, 0, sizeof(a));
+    a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.hold = ss->d_hold; a.tail = ss->d_tail; a.T = ss->T; a.L = ss->L;
+    a.chunks = d_chunks; a.off = reinterpret_cast<const long long *>(d_off); a.stride = stride; a.n = n;
+    a.soff = ss->d_soff; a.last = ss->d_aux; a.xn = ss->d_aux + N; a.woff = ss->d_aux + 2 * N; a.final = final ? 1 : 0;
+    const long long most = (long long)tb->sm_count * 16;
+    const unsigned g_chunks = (unsigned)std::min<long long>((n + 256) / 256, most);
+    /* 1. stage */
+    acb_sl_len_kernel<<<g_chunks, 256, 0, s>>>(a);
+    if ((rc = sl_launch("stream staged lengths"))) return rc;
+    long long staged = 0;
+    if ((rc = sl_offsets(ss, ss->d_soff, n, s, &staged))) return rc;
+    if ((rc = ensure(&ss->d_stage, &ss->stage_cap, (size_t)staged + 64))) return rc;
+    a.stage = ss->d_stage;
+    if ((rc = sl_event(ss, 0, s)) || (rc = sl_gather(ss, tb, a, true, ss->d_soff, ss->d_stage, staged, s)) || (rc = sl_event(ss, 1, s))) return rc;
+    /* 2. scan and 3. the frontier filter; the full list grows until it fits */
+    const int64_t *soff = reinterpret_cast<const int64_t *>(ss->d_soff);
+    unsigned long long m = 0;
+    for (;;) {
+        size_t fcap = std::max<size_t>(ss->full_cap, 4096);
+        if (fcap > 0x7fffffffULL) fcap = 0x7fffffffULL;
+        if ((rc = ensure(&ss->d_full, &ss->full_cap, fcap)) || (rc = ensure(&ss->d_settled, &ss->settled_cap, fcap)) ||
+            (rc = ensure(&ss->d_flag, &ss->flag_cap, fcap)))
+            return rc;
+        fcap = std::min<size_t>(ss->full_cap, 0x7fffffffULL);
+        CUDA_TRY(cudaMemsetAsync(ss->d_ctr, 0, 4 * sizeof(unsigned long long), s));
+        if ((rc = sl_event(ss, 2, s))) return rc;
+        if (staged && (rc = acb_scan_device(tb, ss->d_stage, staged, soff, n, 0, ss->d_full, (int64_t)fcap,
+                                            reinterpret_cast<int64_t *>(ss->d_ctr), s, algo)))
+            return rc;
+        if ((rc = sl_event(ss, 3, s)) || (rc = sl_event(ss, 4, s))) return rc;
+        acb_sl_flag_kernel<<<(unsigned)std::min<long long>(((long long)fcap + 255) / 256, most), 256, 0, s>>>(a, ss->d_full, ss->d_ctr,
+                                                                                                       (long long)fcap, tb->d_keylen, ss->d_flag);
+        if ((rc = sl_launch("stream frontier flags"))) return rc;
+        size_t temp = 0;
+        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, temp, ss->d_full, ss->d_flag, ss->d_settled, ss->d_ctr + 1, (int)fcap, s));
+        if ((rc = sl_tmp(ss, temp))) return rc;
+        temp = ss->tmp_cap;
+        CUDA_TRY(cub::DeviceSelect::Flagged(ss->d_tmp, temp, ss->d_full, ss->d_flag, ss->d_settled, ss->d_ctr + 1, (int)fcap, s));
+        if ((rc = sl_event(ss, 5, s))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(ss->h_ctr, ss->d_ctr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (ss->h_ctr[0] <= fcap) { m = ss->h_ctr[1]; break; }
+        if (ss->h_ctr[0] > 0x7fffffffULL) { acb_set_error("more than 2^31-1 matches in one feed"); return ACB_ERANGE; }
+        if ((rc = ensure(&ss->d_full, &ss->full_cap, (size_t)ss->h_ctr[0]))) return rc;
+    }
+    if (g_timing.load()) {
+        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[0], ss->ev[0], ss->ev[1]));
+        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[1], ss->ev[2], ss->ev[3]));
+        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[2], ss->ev[4], ss->ev[5]));
+    }
+    /* 4. select */
+    acb_match *chosen = d_out;
+    int64_t ccap = cap;
+    unsigned long long *ccount = reinterpret_cast<unsigned long long *>(d_count);
+    if (r) {
+        if ((rc = ensure(&ss->d_chosen, &ss->chosen_cap, (size_t)std::max<unsigned long long>(m, 1)))) return rc;
+        chosen = ss->d_chosen; ccap = (int64_t)m; ccount = ss->d_ctr + 2;
+    }
+    const int64_t max_letters = std::max<int64_t>(staged / ss->L, 1);
+    if ((rc = sl_event(ss, 6, s))) return rc;
+    if (m && (rc = acb_leftmost_longest_device(tb, ss->d_settled, (int64_t)m, n, max_letters, chosen, ccap,
+                                               reinterpret_cast<int64_t *>(ccount), s)))
+        return rc;
+    if ((rc = sl_event(ss, 7, s))) return rc;
+    /* 5. the new X per chunk, and the windows of a replacing feed */
+    CUDA_TRY(cudaMemsetAsync(a.last, 0xff, N * sizeof(long long), s));
+    if (m) {
+        acb_sl_last_kernel<<<(unsigned)std::min<long long>(((long long)m + 255) / 256, most), 256, 0, s>>>(a, chosen, ccount, ccap, r ? 0 : 1);
+        if ((rc = sl_launch("stream last chosen"))) return rc;
+    }
+    acb_sl_frontier_kernel<<<g_chunks, 256, 0, s>>>(a);
+    if ((rc = sl_launch("stream frontier"))) return rc;
+    if (r) {
+        long long wtotal = 0;
+        if ((rc = sl_offsets(ss, a.woff, n, s, &wtotal))) return rc;
+        if ((rc = ensure(&ss->d_win, &ss->win_cap, (size_t)wtotal + 64))) return rc;
+        if ((rc = sl_event(ss, 8, s)) || (rc = sl_gather(ss, tb, a, false, a.woff, ss->d_win, wtotal, s)) || (rc = sl_event(ss, 9, s))) return rc;
+        if ((rc = acb_replace_device(r, tb, ss->d_win, wtotal, reinterpret_cast<const int64_t *>(a.woff), n, 0, chosen, ccap,
+                                     reinterpret_cast<const int64_t *>(ccount), d_rout_off, d_rout, out_cap, d_rtotal, s)))
+            return rc;
+    }
+    /* 6. commit */
+    if ((rc = sl_event(ss, 10, s))) return rc;
+    acb_sl_commit_kernel<<<(unsigned)((n * kSlLanes + 255) / 256), 256, 0, s>>>(a, r ? nullptr : ccount, ccap,
+                                                                          r ? reinterpret_cast<const long long *>(d_rtotal) : nullptr, out_cap);
+    if ((rc = sl_launch("stream commit"))) return rc;
+    if ((rc = sl_event(ss, 11, s))) return rc;
+    if (g_timing.load()) {
+        CUDA_TRY(cudaEventSynchronize(ss->ev[11]));
+        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[3], ss->ev[6], ss->ev[7]));
+        if (r) CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[4], ss->ev[8], ss->ev[9]));
+        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[5], ss->ev[10], ss->ev[11]));
+    }
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_feed_leftmost_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                                                const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
+                                                int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    int rc = sl_check(ss, tb, total_bytes, d_offsets, n_chunks, stride_bytes, &algo);
+    if (rc) return rc;
+    if (!d_count || cap < 0 || (cap > 0 && !d_out) || (total_bytes && !d_chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    return sl_feed(ss, tb, nullptr, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, d_out, cap, d_count,
+                   nullptr, nullptr, 0, nullptr, reinterpret_cast<cudaStream_t>(stream), algo);
+}
+
+extern "C" int acb_streams_replace_device(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                                          const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids, int final,
+                                          int64_t *d_out_offsets, uint8_t *d_out, int64_t out_cap, int64_t *d_total, void *stream, int algo) {
+    int rc = sl_check(ss, tb, total_bytes, d_offsets, n_chunks, stride_bytes, &algo);
+    if (rc) return rc;
+    if (!r || !d_out_offsets || !d_total || out_cap < 0 || (out_cap && !d_out) || (total_bytes && !d_chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if ((rc = rp_fits(r, tb))) return rc;
+    if (reinterpret_cast<uintptr_t>(d_out) & 15) { acb_set_error("d_out must be 16-byte aligned"); return ACB_EINVAL; }
+    return sl_feed(ss, tb, r, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, nullptr, 0, nullptr,
+                   d_out_offsets, d_out, out_cap, d_total, reinterpret_cast<cudaStream_t>(stream), algo);
+}
+
+/* a host feed's first step: ids and offsets checked, chunks (+ offsets, ids) uploaded to the table's workspace */
+static int sl_upload(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total, const int64_t *offsets, int64_t n,
+                     const int32_t *ids) {
+    int rc;
+    if (ids && (rc = check_ids(ss, ids, n))) return rc;
+    if (offsets) {                                          /* the kernels read chunks[offsets[h] .. offsets[h+1]) unchecked */
+        bool ok = offsets[0] == 0 && offsets[n] == total;
+        for (int64_t i = 0; ok && i < n; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % ss->L == 0;
+        if (!ok) { acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes"); return ACB_EINVAL; }
+    }
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
+    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n + 1))) return rc;
+    if (ids && (rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)std::max<int64_t>(n, 1)))) return rc;
+    cudaStream_t s = tb->stream;
+    if (total) CUDA_TRY(cudaMemcpyAsync(tb->w_hay, chunks, (size_t)total, cudaMemcpyHostToDevice, s));
+    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+    if (ids && n) CUDA_TRY(cudaMemcpyAsync(ss->d_ids, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                                              const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
+                                              acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    int rc = sl_check(ss, tb, total_bytes, offsets, n_chunks, stride_bytes, &algo);
+    if (rc) return rc;
+    if (!n_found || cap < 0 || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *n_found = 0;
+    tb->h_out_n = 0;
+    if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids))) return rc;
+    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1)))) return rc;
+    cudaStream_t s = tb->stream;
+    if ((rc = sl_feed(ss, tb, nullptr, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_chunks,
+                      stride_bytes, ids ? ss->d_ids : nullptr, final, tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), nullptr,
+                      nullptr, 0, nullptr, s, algo)))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    const unsigned long long n = *tb->h_count;
+    *n_found = (int64_t)n;
+    if (n > (unsigned long long)cap) {
+        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
+        return ACB_EOVERFLOW;
+    }
+    if (n) {
+        if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->w_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
+    }
+    tb->h_out_n = n;
+    return ACB_OK;
+}
+
+extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                                        const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
+                                        int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap, int64_t *total) {
+    int rc = sl_check(ss, tb, total_bytes, offsets, n_chunks, stride_bytes, &algo);
+    if (rc) return rc;
+    if (!r || !out_offsets || !total || out_cap < 0 || (out_cap && !out) || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if ((rc = rp_fits(r, tb))) return rc;
+    *total = 0;
+    if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids))) return rc;
+    cudaStream_t s = tb->stream;
+    if ((rc = ensure(&tb->r_off, &tb->r_off_cap, (size_t)n_chunks + 2))) return rc;
+    const int64_t guess = total_bytes + total_bytes / 4 + n_chunks * (int64_t)ss->T * ss->L + 4096;
+    if ((rc = ensure(&tb->r_out, &tb->r_out_cap, (size_t)std::max<int64_t>(std::min(out_cap, guess), 16)))) return rc;
+    for (;;) {                                             /* an output that fits out_cap but not the device buffer: grow, repeat */
+        const int64_t dev_cap = std::min<int64_t>(out_cap, (int64_t)tb->r_out_cap);
+        if ((rc = sl_feed(ss, tb, r, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_chunks,
+                          stride_bytes, ids ? ss->d_ids : nullptr, final, nullptr, 0, nullptr, reinterpret_cast<int64_t *>(tb->r_off),
+                          tb->r_out, dev_cap, reinterpret_cast<int64_t *>(tb->r_off + n_chunks + 1), s, algo)))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(out_offsets, tb->r_off, (size_t)(n_chunks + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(total, tb->r_off + n_chunks + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (*total > out_cap) {
+            acb_set_error("replacement: room for %lld bytes, output %lld", (long long)out_cap, (long long)*total);
+            return ACB_EOVERFLOW;
+        }
+        if (*total <= dev_cap) break;
+        if ((rc = ensure(&tb->r_out, &tb->r_out_cap, (size_t)*total))) return rc;
+    }
     if (*total) CUDA_TRY(cudaMemcpyAsync(out, tb->r_out, (size_t)*total, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     return ACB_OK;
