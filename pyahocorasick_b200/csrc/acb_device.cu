@@ -1502,6 +1502,41 @@ extern "C" int64_t acb_launch_count(void) { return g_launches.load(); }
 extern "C" int acb_set_kernel_timing(int enabled) { g_timing.store(enabled ? 1 : 0); return ACB_OK; }
 extern "C" float acb_last_kernel_ms(void) { return g_last_ms; }
 
+/* ----------------------------------------------------- shared host checks */
+
+/* after a launch (acb_launch_count): its error, naming the kernel, or n more launches; n > 1 counts a group once */
+static int launched(const char *what, int n = 1) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { acb_set_error("%s launch failed: %s", what, cudaGetErrorString(e)); return ACB_ECUDA; }
+    g_launches.fetch_add(n);
+    return ACB_OK;
+}
+
+/* kernel timing (acb_set_kernel_timing): event *ev recorded on s, created on first use; nothing while timing is off */
+static int timing_mark(cudaEvent_t *ev, cudaStream_t s) {
+    if (!g_timing.load()) return ACB_OK;
+    if (!*ev) CUDA_TRY(cudaEventCreate(ev));
+    CUDA_TRY(cudaEventRecord(*ev, s));
+    return ACB_OK;
+}
+
+/* *ms = the time from mark a to mark b, waiting for b; *ms untouched while timing is off */
+static int timing_ms(cudaEvent_t a, cudaEvent_t b, float *ms) {
+    if (!g_timing.load()) return ACB_OK;
+    CUDA_TRY(cudaEventSynchronize(b));
+    CUDA_TRY(cudaEventElapsedTime(ms, a, b));
+    return ACB_OK;
+}
+
+/* a fixed-stride batch: stride >= min_stride (0 or 1), a multiple of the letter width, and n * stride == total, checked
+ * without overflowing n * stride */
+static int check_stride(int32_t L, int64_t total, int64_t n, int64_t stride, int64_t min_stride) {
+    if (stride >= min_stride && stride % L == 0 && (stride == 0 ? total == 0 : n <= total / stride && n * stride == total)) return ACB_OK;
+    acb_set_error("a fixed-stride batch needs stride_bytes >= %lld, a multiple of letter_bytes, and n*stride_bytes == total_bytes",
+                  (long long)min_stride);
+    return ACB_EINVAL;
+}
+
 /* ------------------------------------------------------------- launching */
 
 constexpr int kMaxDevices = 64;                              /* opt-in caches below are per device */
@@ -1519,9 +1554,7 @@ static int launch_stream_m(const ScanParams &p, int grid, cudaStream_t s) {
         opted.store(smem, std::memory_order_relaxed);
     }
     kern<<<grid, kFThreads, smem, s>>>(p);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-    return ACB_OK;
+    return launched("stream kernel");
 }
 
 static int launch_pair(const ScanParams &p, int grid, cudaStream_t s) {
@@ -1537,9 +1570,7 @@ static int launch_pair(const ScanParams &p, int grid, cudaStream_t s) {
     }
     if (p.log2b == 17) acb_pair_kernel<17><<<grid, kPairThreads, smem, s>>>(p);      /* the 2^20-bit level 1 of 10 k keys and more */
     else acb_pair_kernel<0><<<grid, kPairThreads, smem, s>>>(p);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-    return ACB_OK;
+    return launched("pair kernel");
 }
 
 /* the placement mode follows from the table's filter_flags */
@@ -1632,10 +1663,8 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
     if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
     if (!d_offsets) {
-        if (stride_bytes <= 0 || stride_bytes % tb->L || stride_bytes * n_hay != total_bytes) {
-            acb_set_error("fixed-stride batch needs stride_bytes > 0, a multiple of letter_bytes, and n_hay*stride == total_bytes");
-            return ACB_EINVAL;
-        }
+        int rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1);
+        if (rc != ACB_OK) return rc;
         if (stride_bytes / tb->L > 0x7fffffffLL) { acb_set_error("haystack longer than 2^31-1 letters"); return ACB_ERANGE; }
     }
     if (total_bytes == 0 || n_hay == 0) {
@@ -1654,22 +1683,16 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
         if (algo == ACB_ALGO_LONG) long_scan_without_launch(tb);
         return ACB_OK;
     }
-    const bool timing = g_timing.load() != 0;
-    if (timing) {
-        if (!tb->ev0) { CUDA_TRY(cudaEventCreate(&tb->ev0)); CUDA_TRY(cudaEventCreate(&tb->ev1)); }
-        CUDA_TRY(cudaEventRecord(tb->ev0, s));
-    }
+    int rc = timing_mark(&tb->ev0, s);
+    if (rc != ACB_OK) return rc;
     if (algo == ACB_ALGO_FILTER) {
-        int rc = launch_filter_range(tb, p, 0, total_bytes, s);
-        if (rc != ACB_OK) return rc;
+        if ((rc = launch_filter_range(tb, p, 0, total_bytes, s))) return rc;
     } else if (algo == ACB_ALGO_DFA) {
         long long spans = (total_bytes + kDfaSpan - 1) / kDfaSpan;
         long long grid = (spans + kDfaThreads - 1) / kDfaThreads;
         if (grid > 0x7fffffffLL) { acb_set_error("batch too large for one launch"); return ACB_ERANGE; }
         acb_dfa_kernel<<<(unsigned)grid, kDfaThreads, 0, s>>>(p);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) { acb_set_error("DFA kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
-        g_launches.fetch_add(1);
+        if ((rc = launched("DFA kernel"))) return rc;
     } else if (algo == ACB_ALGO_LONG) {
         if (!tb->d_long_final) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->d_long_final), sizeof(int32_t)));
         p.long_init = tb->long_init;
@@ -1678,21 +1701,13 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
         tb->long_final_host = -1;                               /* the kernel writes the final state */
         long long grid = (n_hay + kDfaThreads - 1) / kDfaThreads;
         acb_long_kernel<<<(unsigned)grid, kDfaThreads, 0, s>>>(p);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) { acb_set_error("iter_long kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
-        g_launches.fetch_add(1);
+        if ((rc = launched("iter_long kernel"))) return rc;
     } else {
         acb_set_error("unknown algo %d", algo);
         return ACB_EINVAL;
     }
-    if (timing) {
-        CUDA_TRY(cudaEventRecord(tb->ev1, s));
-        CUDA_TRY(cudaEventSynchronize(tb->ev1));
-        float ms = 0.f;
-        CUDA_TRY(cudaEventElapsedTime(&ms, tb->ev0, tb->ev1));
-        g_last_ms = ms;
-    }
-    return ACB_OK;
+    if ((rc = timing_mark(&tb->ev1, s))) return rc;
+    return timing_ms(tb->ev0, tb->ev1, &g_last_ms);
 }
 
 extern "C" int acb_table_set_long_state(acb_table *tb, int32_t state) {
@@ -1814,8 +1829,8 @@ extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int6
     acb_match *r1 = reinterpret_cast<acb_match *>(k1 + n);
     void *tmp = reinterpret_cast<void *>((reinterpret_cast<uintptr_t>(r1 + n) + 255) & ~(uintptr_t)255);
     acb_sortkey_kernel<kKeyEnd><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
+    int rc = launched("sort key");
+    if (rc != ACB_OK) return rc;
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, temp, k0, k1, d_records, r1, (int)n, 0, bh + be + bl, s));
     CUDA_TRY(cudaMemcpyAsync(d_records, r1, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToDevice, s));
     return ACB_OK;
@@ -1846,6 +1861,102 @@ static int ensure_pinned_out(acb_table *tb, size_t n) {
         CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_out), want * sizeof(acb_match)));
         tb->h_out_cap = want;
     }
+    return ACB_OK;
+}
+
+/* Scratch that the last call's work, on any CUDA stream, may still read: a call waits on s for that work before it
+ * overwrites the scratch (scratch_wait), and marks its own last reader (scratch_done).  Growing it frees the old
+ * buffer only after s has drained (grow_synced). */
+static int scratch_wait(cudaEvent_t done, cudaStream_t s) {
+    if (done) CUDA_TRY(cudaStreamWaitEvent(s, done, 0));
+    return ACB_OK;
+}
+static int scratch_done(cudaEvent_t *done, cudaStream_t s) {
+    if (!*done) CUDA_TRY(cudaEventCreateWithFlags(done, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventRecord(*done, s));
+    return ACB_OK;
+}
+static int grow_synced(void **buf, size_t *cap, size_t need, cudaStream_t s) {
+    if (*cap >= need) return ACB_OK;
+    if (*buf) { CUDA_TRY(cudaStreamSynchronize(s)); cudaFree(*buf); *buf = nullptr; *cap = 0; }
+    CUDA_TRY(cudaMalloc(buf, need + need / 4));
+    *cap = need + need / 4;
+    return ACB_OK;
+}
+
+/* host offsets of n haystacks: non-decreasing multiples of the letter width, from 0 to total.  The kernels read
+ * hay[offsets[i] .. offsets[i+1]) unchecked. */
+static int check_offsets(int32_t L, const int64_t *offsets, int64_t n, int64_t total) {
+    bool ok = offsets[0] == 0 && offsets[n] == total;
+    for (int64_t i = 0; ok && i < n; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % L == 0;
+    if (ok) return ACB_OK;
+    acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at the total byte count");
+    return ACB_EINVAL;
+}
+
+/* The host routes' workspace on tb->stream: the device set, the stream and the count words made, tb->w_hay grown for
+ * total bytes and tb->w_off for the offsets of n haystacks when there are offsets. */
+static int host_workspace(acb_table *tb, int64_t total, const int64_t *offsets, int64_t n) {
+    CUDA_TRY(cudaSetDevice(tb->device));
+    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
+    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
+    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
+    int rc;
+    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total + 64))) return rc;
+    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n + 1))) return rc;
+    return ACB_OK;
+}
+
+/* ... and the batch and its offsets on their way up, asynchronously; *d_off = the device offsets, or nullptr */
+static int upload_batch(acb_table *tb, const uint8_t *hay, int64_t total, const int64_t *offsets, int64_t n, const int64_t **d_off) {
+    int rc = host_workspace(tb, total, offsets, n);
+    if (rc != ACB_OK) return rc;
+    *d_off = nullptr;
+    if (total) CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total, cudaMemcpyHostToDevice, tb->stream));
+    if (offsets) {
+        CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, tb->stream));
+        *d_off = reinterpret_cast<const int64_t *>(tb->w_off);
+    }
+    return ACB_OK;
+}
+
+/* the reference order of records (SURVEY 3.3): haystack, then end_index ascending, then longest key first (fail-chain order) */
+struct RefOrder {
+    const int32_t *key_len;
+    bool operator()(const acb_match &a, const acb_match &b) const {
+        if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
+        if (a.end_index != b.end_index) return a.end_index < b.end_index;
+        return key_len[a.key_id] > key_len[b.key_id];
+    }
+};
+
+/* The host routes' last step, on s: the record count at d_n to the host (a wait), ACB_EOVERFLOW with the exact count
+ * past cap, then the records of d_rec into the pinned staging buffer and into `out` when given.  With sort they are put
+ * into the reference order first: on the device, or on the host when the device sort's key does not fit 64 bits. */
+static int read_back(acb_table *tb, const unsigned long long *d_n, acb_match *d_rec, int64_t cap, int sort, int64_t n_hay,
+                     int64_t max_letters, acb_match *out, int64_t *n_found, cudaStream_t s) {
+    CUDA_TRY(cudaMemcpyAsync(tb->h_count, d_n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    const unsigned long long n = *tb->h_count;
+    *n_found = (int64_t)n;
+    if (n > (unsigned long long)cap) {
+        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
+        return ACB_EOVERFLOW;
+    }
+    if (n) {
+        int rc;
+        if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
+        bool host_sort = false;
+        if (sort && (rc = acb_sort_matches_device(tb, d_rec, (int64_t)n, n_hay, max_letters, s)) != ACB_OK) {
+            if (rc != ACB_ERANGE) return rc;
+            host_sort = true;
+        }
+        CUDA_TRY(cudaMemcpyAsync(tb->h_out, d_rec, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (host_sort) std::sort(tb->h_out, tb->h_out + n, RefOrder{tb->key_len.data()});
+        if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));   /* out == NULL: fetch with acb_copy_records */
+    }
+    tb->h_out_n = n;
     return ACB_OK;
 }
 
@@ -1928,12 +2039,6 @@ static int scan_host_pipelined(acb_table *tb, const uint8_t *hay, int64_t total,
         return ACB_EOVERFLOW;
     }
     if (sort) {                                                 /* the haystack every cut goes through: merge its two runs */
-        const int32_t *kl = tb->key_len.data();
-        auto less = [kl](const acb_match &a, const acb_match &b) {
-            if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
-            if (a.end_index != b.end_index) return a.end_index < b.end_index;
-            return kl[a.key_id] > kl[b.key_id];
-        };
         for (int c = 0; c + 1 < nch; c++) {
             const unsigned long long mid = tb->h_counts[c];
             if (mid == 0 || mid >= n) continue;
@@ -1943,7 +2048,7 @@ static int scan_host_pipelined(acb_table *tb, const uint8_t *hay, int64_t total,
             while (lo > 0 && tb->h_out[lo - 1].hay_id == h) lo--;
             const unsigned long long stop = std::min<unsigned long long>(n, tb->h_counts[c + 1]);   /* this cut's run ends with chunk c+1; a longer haystack meets the next cut */
             while (hi < stop && tb->h_out[hi].hay_id == h) hi++;
-            std::inplace_merge(tb->h_out + lo, tb->h_out + mid, tb->h_out + hi, less);
+            std::inplace_merge(tb->h_out + lo, tb->h_out + mid, tb->h_out + hi, RefOrder{tb->key_len.data()});
         }
     }
     tb->h_out_n = n;
@@ -1960,17 +2065,11 @@ extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_by
         if (algo == ACB_ALGO_LONG) long_scan_without_launch(tb);
         return ACB_OK;
     }
-    CUDA_TRY(cudaSetDevice(tb->device));
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
-    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
     int rc;
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_hay + 1))) return rc;
-    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1)))) return rc;
-    cudaStream_t s = tb->stream;
+    if ((rc = host_workspace(tb, total_bytes, offsets, n_hay)) || (rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1))))
+        return rc;
+    const int64_t max_letters = (offsets ? total_bytes : stride_bytes) / tb->L;
     {   /* large batches on the fast path: copy, scan, sort and copy-back as a pipeline over chunks */
-        const int64_t max_letters = (offsets ? total_bytes : stride_bytes) / tb->L;
         const int bits = bits_for((unsigned long long)std::max<int64_t>(n_hay - 1, 1)) + bits_for((unsigned long long)std::max<int64_t>(max_letters, 1)) +
                          bits_for((unsigned long long)(tb->max_key_bytes / tb->L));
         static const bool no_pipe = getenv("ACB_NO_PIPELINE") != nullptr;
@@ -1982,61 +2081,20 @@ extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_by
     }
     static const bool trace = getenv("ACB_TRACE") != nullptr;          /* phase timing to stderr (adds syncs) */
     auto now = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-    double t0 = trace ? now() : 0, t1 = 0, t2 = 0, t3 = 0, t4 = 0;
-    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
-    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_hay + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+    double t0 = trace ? now() : 0, t1 = 0, t2 = 0;
+    const int64_t *d_off = nullptr;
+    if ((rc = upload_batch(tb, hay, total_bytes, offsets, n_hay, &d_off))) return rc;
+    cudaStream_t s = tb->stream;
     CUDA_TRY(cudaMemsetAsync(tb->w_count, 0, sizeof(unsigned long long), s));
     if (trace) { cudaStreamSynchronize(s); t1 = now(); }
-    rc = acb_scan_device(tb, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr,
-                         n_hay, stride_bytes, tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), s, algo);
+    rc = acb_scan_device(tb, tb->w_hay, total_bytes, d_off, n_hay, stride_bytes, tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), s, algo);
     if (rc != ACB_OK) return rc;
-    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    if (trace) t2 = now();
-    unsigned long long n = *tb->h_count;
-    *n_found = (int64_t)n;
-    if (n > (unsigned long long)cap) {
-        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
-        return ACB_EOVERFLOW;
-    }
-    if (n) {
-        if (tb->h_out_cap < n) {                               /* pinned staging: D2H at full PCIe rate */
-            if (tb->h_out) { acb_release_records(tb->h_out, (int64_t)tb->h_out_cap); tb->h_out = nullptr; tb->h_out_cap = 0; }
-            size_t got = 0;
-            if (acb_match *p = pool_take((size_t)n, &got)) {  /* a buffer some caller has given back */
-                tb->h_out = p;
-                tb->h_out_cap = got;
-            } else {
-                size_t want = (size_t)n + (size_t)n / 4 + 1024;
-                CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_out), want * sizeof(acb_match)));
-                tb->h_out_cap = want;
-            }
-        }
-        bool host_sort = sort != 0;
-        if (sort) {                                            /* radix sort on the device when the key fits 64 bits */
-            const int64_t max_letters = (offsets ? total_bytes : stride_bytes) / tb->L;
-            if (acb_sort_matches_device(tb, tb->w_out, (int64_t)n, n_hay, max_letters, s) == ACB_OK) host_sort = false;
-        }
-        if (trace) { cudaStreamSynchronize(s); t3 = now(); }
-        CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->w_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaStreamSynchronize(s));
-        if (host_sort) {
-            const int32_t *kl = tb->key_len.data();
-            std::sort(tb->h_out, tb->h_out + n, [kl](const acb_match &a, const acb_match &b) {
-                if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
-                if (a.end_index != b.end_index) return a.end_index < b.end_index;
-                return kl[a.key_id] > kl[b.key_id];            /* longest first: fail-chain order */
-            });
-        }
-        if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));   /* out == NULL: fetch with acb_copy_records */
-    }
-    tb->h_out_n = n;
-    if (trace) {
-        t4 = now();
-        fprintf(stderr, "[acb_scan_host] %lld B: h2d %.3f ms, scan %.3f ms, sort %.3f ms, d2h+copy %.3f ms (%llu records)\n",
-                (long long)total_bytes, t1 - t0, t2 - t1, t3 ? t3 - t2 : 0.0, t3 ? t4 - t3 : t4 - t2, n);
-    }
-    return ACB_OK;
+    if (trace) { cudaStreamSynchronize(s); t2 = now(); }
+    rc = read_back(tb, tb->w_count, tb->w_out, cap, sort, n_hay, max_letters, out, n_found, s);
+    if (trace && rc == ACB_OK)
+        fprintf(stderr, "[acb_scan_host] %lld B: h2d %.3f ms, scan %.3f ms, sort+d2h+copy %.3f ms (%lld records)\n",
+                (long long)total_bytes, t1 - t0, t2 - t1, now() - t2, (long long)*n_found);
+    return rc;
 }
 
 /* ------------------------------------------------------------ white space */
@@ -2208,30 +2266,6 @@ __global__ void acb_remap_kernel(const CompactMeta m, const long long *coff, con
 }
 } // namespace
 
-/* kernel timing (acb_set_kernel_timing): events around one launch, waited for; *ms = 0 when timing is off */
-static int skip_timing_begin(acb_table *tb, cudaStream_t s) {
-    if (!g_timing.load()) return ACB_OK;
-    if (!tb->k_t0) { CUDA_TRY(cudaEventCreate(&tb->k_t0)); CUDA_TRY(cudaEventCreate(&tb->k_t1)); }
-    CUDA_TRY(cudaEventRecord(tb->k_t0, s));
-    return ACB_OK;
-}
-static int skip_timing_end(acb_table *tb, cudaStream_t s, float *ms) {
-    *ms = 0.f;
-    if (!g_timing.load()) return ACB_OK;
-    CUDA_TRY(cudaEventRecord(tb->k_t1, s));
-    CUDA_TRY(cudaEventSynchronize(tb->k_t1));
-    CUDA_TRY(cudaEventElapsedTime(ms, tb->k_t0, tb->k_t1));
-    return ACB_OK;
-}
-
-/* the work of the last skip call that reads the table's k_* workspace (remap, stream commit) is issued; a later skip
- * call, on any CUDA stream, waits for it before it overwrites that workspace */
-static int skip_work_issued(acb_table *tb, cudaStream_t s) {
-    if (!tb->k_done) CUDA_TRY(cudaEventCreateWithFlags(&tb->k_done, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventRecord(tb->k_done, s));
-    return ACB_OK;
-}
-
 extern "C" int acb_last_skip_ms(float *compact_ms, float *remap_ms) {
     if (!compact_ms || !remap_ms) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *compact_ms = g_compact_ms;
@@ -2261,7 +2295,7 @@ static int compact(acb_table *tb, const uint8_t *d_in, int64_t total, const int6
     if (!tb->k_set) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->k_set), ACB_MAX_SKIP * sizeof(uint32_t)));
     if (!tb->k_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->k_ctr), sizeof(unsigned int)));
     if (!tb->h_kept) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_kept), sizeof(long long)));
-    if (tb->k_done) CUDA_TRY(cudaStreamWaitEvent(s, tb->k_done, 0));
+    if ((rc = scratch_wait(tb->k_done, s))) return rc;
     g_compact_ms = g_remap_ms = 0.f;
     CompactParams p;
     memset(&p, 0, sizeof(p));
@@ -2273,17 +2307,16 @@ static int compact(acb_table *tb, const uint8_t *d_in, int64_t total, const int6
     CUDA_TRY(cudaMemsetAsync(tb->k_status, 0, (size_t)n_tiles * sizeof(unsigned long long), s));
     CUDA_TRY(cudaMemsetAsync(tb->k_ctr, 0, sizeof(unsigned int), s));
     if (n_tiles > 0x7fffffffLL) { acb_set_error("batch too large to compact in one launch"); return ACB_ERANGE; }
-    if ((rc = skip_timing_begin(tb, s))) return rc;
+    if ((rc = timing_mark(&tb->k_t0, s))) return rc;
     if (L == 1) acb_compact_kernel<uint8_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
     else if (L == 2) acb_compact_kernel<uint16_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
     else acb_compact_kernel<uint32_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
     CUDA_TRY(cudaGetLastError());
-    if ((rc = skip_timing_end(tb, s, &g_compact_ms))) return rc;
+    if ((rc = timing_mark(&tb->k_t1, s)) || (rc = timing_ms(tb->k_t0, tb->k_t1, &g_compact_ms))) return rc;
     meta->mask = tb->k_mask; meta->gpre = tb->k_gpre; meta->tile_pre = tb->k_tile_pre; meta->n_tiles = n_tiles;
     acb_compact_offsets_kernel<<<(unsigned)((n_hay + 1 + 255) / 256), 256, 0, s>>>(*meta, reinterpret_cast<const long long *>(d_off), stride,
                                                                                  n_hay, ls, tb->k_coff);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(2);
+    if ((rc = launched("compaction offsets", 2))) return rc;
     CUDA_TRY(cudaMemcpyAsync(tb->h_kept, tb->k_tile_pre + n_tiles, sizeof(long long), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     *kept_bytes = *tb->h_kept * L;
@@ -2296,12 +2329,11 @@ static int launch_remap(acb_table *tb, const CompactMeta &meta, const int64_t *d
     const int ls = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
     const long long grid = std::min<long long>((cap + 255) / 256, (long long)tb->sm_count * 16);
     int rc;
-    if ((rc = skip_timing_begin(tb, s))) return rc;
+    if ((rc = timing_mark(&tb->k_t0, s))) return rc;
     acb_remap_kernel<<<(unsigned)grid, 256, 0, s>>>(meta, tb->k_coff, reinterpret_cast<const long long *>(d_off), stride, ls, d_out,
                                                     reinterpret_cast<const unsigned long long *>(d_count), cap);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-    return skip_timing_end(tb, s, &g_remap_ms);
+    if ((rc = launched("remap kernel")) || (rc = timing_mark(&tb->k_t1, s))) return rc;
+    return timing_ms(tb->k_t0, tb->k_t1, &g_remap_ms);
 }
 
 extern "C" int acb_scan_device_skip(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
@@ -2312,10 +2344,7 @@ extern "C" int acb_scan_device_skip(acb_table *tb, const uint8_t *d_hay, int64_t
     int rc = check_skip(skip, n_skip, algo);
     if (rc != ACB_OK) return rc;
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
-    if (!d_offsets && (stride_bytes <= 0 || stride_bytes % tb->L || stride_bytes * n_hay != total_bytes)) {
-        acb_set_error("fixed-stride batch needs stride_bytes > 0, a multiple of letter_bytes, and n_hay*stride == total_bytes");
-        return ACB_EINVAL;
-    }
+    if (!d_offsets && (rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1))) return rc;
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
@@ -2328,31 +2357,7 @@ extern "C" int acb_scan_device_skip(acb_table *tb, const uint8_t *d_hay, int64_t
     if (kept == 0) return ACB_OK;
     if ((rc = acb_scan_device(tb, tb->k_buf, kept, reinterpret_cast<const int64_t *>(tb->k_coff), n_hay, 0, d_out, cap, d_count, stream, algo))) return rc;
     if ((rc = launch_remap(tb, meta, d_offsets, stride_bytes, d_out, cap, d_count, s))) return rc;
-    return skip_work_issued(tb, s);
-}
-
-/* n records of a host-buffer call, in tb->w_out: sorted (on the device when the key fits, else on the host) into the
- * pinned staging buffer, and into `out` when given */
-static int records_to_host(acb_table *tb, unsigned long long n, int64_t n_hay, int64_t max_letters, int sort, acb_match *out, cudaStream_t s) {
-    int rc;
-    if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
-    bool host_sort = false;                                /* the device sort's key does not fit 64 bits: sort on the host */
-    if (sort && (rc = acb_sort_matches_device(tb, tb->w_out, (int64_t)n, n_hay, max_letters, s)) != ACB_OK) {
-        if (rc != ACB_ERANGE) return rc;
-        host_sort = true;
-    }
-    CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->w_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    if (host_sort) {
-        const int32_t *kl = tb->key_len.data();
-        std::sort(tb->h_out, tb->h_out + n, [kl](const acb_match &a, const acb_match &b) {
-            if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
-            if (a.end_index != b.end_index) return a.end_index < b.end_index;
-            return kl[a.key_id] > kl[b.key_id];
-        });
-    }
-    if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
-    return ACB_OK;
+    return scratch_done(&tb->k_done, s);                   /* the remap was the last reader of the k_* workspace */
 }
 
 extern "C" int acb_scan_host_skip(acb_table *tb, const uint8_t *hay, int64_t total_bytes,
@@ -2365,30 +2370,14 @@ extern "C" int acb_scan_host_skip(acb_table *tb, const uint8_t *hay, int64_t tot
     if (rc != ACB_OK) return rc;
     tb->h_out_n = 0;
     if (total_bytes == 0 || n_hay == 0) return ACB_OK;
-    CUDA_TRY(cudaSetDevice(tb->device));
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
-    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_hay + 1))) return rc;
-    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1)))) return rc;
+    const int64_t *d_off = nullptr;
+    if ((rc = upload_batch(tb, hay, total_bytes, offsets, n_hay, &d_off)) || (rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1))))
+        return rc;
     cudaStream_t s = tb->stream;
-    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
-    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_hay + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
-    rc = acb_scan_device_skip(tb, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_hay, stride_bytes,
-                              tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), s, algo, skip, n_skip);
-    if (rc != ACB_OK) return rc;
-    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    const unsigned long long n = *tb->h_count;
-    *n_found = (int64_t)n;
-    if (n > (unsigned long long)cap) {
-        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
-        return ACB_EOVERFLOW;
-    }
-    if (n && (rc = records_to_host(tb, n, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, sort, out, s))) return rc;
-    tb->h_out_n = n;
-    return ACB_OK;
+    if ((rc = acb_scan_device_skip(tb, tb->w_hay, total_bytes, d_off, n_hay, stride_bytes, tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), s,
+                                   algo, skip, n_skip)))
+        return rc;
+    return read_back(tb, tb->w_count, tb->w_out, cap, sort, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, out, n_found, s);
 }
 
 /* ------------------------------------------------------------ stream batches */
@@ -2604,10 +2593,7 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
     int rc = streams_check_table(ss, tb);
     if (rc != ACB_OK) return rc;
     if (n_chunks > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, ss->n); return ACB_EINVAL; }
-    if (!d_off && n_chunks && (stride <= 0|| stride % ss->L || stride * n_chunks != total)) {
-        acb_set_error("fixed-stride feed needs stride_bytes > 0, a multiple of letter_bytes, and n_chunks*stride == total_bytes");
-        return ACB_EINVAL;
-    }
+    if (!d_off && n_chunks && (rc = check_stride(ss->L, total, n_chunks, stride, 1))) return rc;
     if (algo == ACB_ALGO_AUTO) algo = ss->long_mode ? ACB_ALGO_LONG : ACB_ALGO_FILTER;
     if (ss->long_mode ? algo != ACB_ALGO_LONG : (algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA)) {
         acb_set_error("algo %d does not fit a %s stream batch", algo, ss->long_mode ? "iter_long" : "find_all");
@@ -2630,8 +2616,7 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
         p.long_start = a.start;
         p.long_end = a.end;
         acb_long_kernel<<<grid, kDfaThreads, 0, s>>>(p);
-        CUDA_TRY(cudaGetLastError());
-        g_launches.fetch_add(2);
+        if ((rc = launched("stream iter_long kernel", 2))) return rc;
     } else if (ss->d_kept) {                                     /* skip set: compact, scan, walk the seams, map back */
         long long kept = 0;
         CompactMeta meta;
@@ -2644,8 +2629,7 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
             fill_params(tb, pk, tb->k_buf, kept, koff, n_chunks, 0, d_out, cap, d_count);
             a.next_tail = ss->d_next_tail;
             acb_seam_kernel<<<grid, kDfaThreads, 0, s>>>(pk, a);
-            CUDA_TRY(cudaGetLastError());
-            g_launches.fetch_add(1);
+            if ((rc = launched("seam kernel"))) return rc;
         }
         if ((rc = launch_remap(tb, meta, d_off, stride, d_out, cap, d_count, s))) return rc;
     } else {
@@ -2654,16 +2638,14 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
             if ((rc = ensure(&ss->d_next_tail, &ss->next_tail_cap, (size_t)n_chunks * ss->T * ss->L))) return rc;
             a.next_tail = ss->d_next_tail;
             acb_seam_kernel<<<grid, kDfaThreads, 0, s>>>(p, a);
-            CUDA_TRY(cudaGetLastError());
-            g_launches.fetch_add(1);
+            if ((rc = launched("seam kernel"))) return rc;
         }
     }
     acb_streams_commit_kernel<<<grid, kDfaThreads, 0, s>>>(a, reinterpret_cast<const long long *>(d_off), stride, n_chunks,
                                                           reinterpret_cast<const unsigned long long *>(d_count), cap,
                                                           tb->k_coff);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-    if (ss->d_kept && (rc = skip_work_issued(tb, s))) return rc;
+    if ((rc = launched("stream commit"))) return rc;
+    if (ss->d_kept && (rc = scratch_done(&tb->k_done, s))) return rc;    /* the commit read tb->k_coff */
     return ACB_OK;
 }
 
@@ -2685,6 +2667,15 @@ static int check_ids(const acb_streams *ss, const int32_t *ids, int64_t n) {
     return ACB_OK;
 }
 
+/* the ids of a host feed, when given, to ss->d_ids on s (after the chunks and their offsets) */
+static int upload_ids(acb_streams *ss, const int32_t *ids, int64_t n, cudaStream_t s) {
+    if (!ids) return ACB_OK;
+    int rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)n);
+    if (rc != ACB_OK) return rc;
+    if (n) CUDA_TRY(cudaMemcpyAsync(ss->d_ids, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    return ACB_OK;
+}
+
 extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
                                      const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids,
                                      acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort) {
@@ -2697,48 +2688,15 @@ extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8
     if ((rc = streams_check_table(ss, tb))) return rc;
     if (n_chunks > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, ss->n); return ACB_EINVAL; }
     if (total_bytes == 0 || n_chunks == 0) return ACB_OK;
-    CUDA_TRY(cudaSetDevice(tb->device));
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
-    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_chunks + 1))) return rc;
-    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1)))) return rc;
-    if (ids && (rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)n_chunks))) return rc;
+    const int64_t *d_off = nullptr;
+    if ((rc = upload_batch(tb, chunks, total_bytes, offsets, n_chunks, &d_off)) || (rc = upload_ids(ss, ids, n_chunks, tb->stream)) ||
+        (rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1))))
+        return rc;
     cudaStream_t s = tb->stream;
-    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, chunks, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
-    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_chunks + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
-    if (ids) CUDA_TRY(cudaMemcpyAsync(ss->d_ids, ids, (size_t)n_chunks * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    rc = streams_feed(ss, tb, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_chunks,
-                      stride_bytes, ids ? ss->d_ids : nullptr, tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), s, algo);
-    if (rc != ACB_OK) return rc;
-    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    const unsigned long long n = *tb->h_count;
-    *n_found = (int64_t)n;
-    if (n > (unsigned long long)cap) {
-        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
-        return ACB_EOVERFLOW;
-    }
-    if (n) {
-        if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
-        bool host_sort = sort != 0;
-        const int64_t max_letters = (offsets ? total_bytes : stride_bytes) / tb->L;
-        if (sort && acb_sort_matches_device(tb, tb->w_out, (int64_t)n, n_chunks, max_letters, s) == ACB_OK) host_sort = false;
-        CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->w_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaStreamSynchronize(s));
-        if (host_sort) {
-            const int32_t *kl = tb->key_len.data();
-            std::sort(tb->h_out, tb->h_out + n, [kl](const acb_match &a, const acb_match &b) {
-                if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
-                if (a.end_index != b.end_index) return a.end_index < b.end_index;
-                return kl[a.key_id] > kl[b.key_id];
-            });
-        }
-        if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
-    }
-    tb->h_out_n = n;
-    return ACB_OK;
+    if ((rc = streams_feed(ss, tb, tb->w_hay, total_bytes, d_off, n_chunks, stride_bytes, ids ? ss->d_ids : nullptr, tb->w_out, cap,
+                           reinterpret_cast<int64_t *>(tb->w_count), s, algo)))
+        return rc;
+    return read_back(tb, tb->w_count, tb->w_out, cap, sort, n_chunks, (offsets ? total_bytes : stride_bytes) / tb->L, out, n_found, s);
 }
 
 extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n) {
@@ -2757,8 +2715,7 @@ extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n)
         StreamsArgs a = streams_args(ss, ss->d_ids);
         if (ss->d_hold) a.kept = ss->d_hold;                     /* leftmost (no skip set): nothing held back either */
         acb_streams_reset_kernel<<<(unsigned)((n + 255) / 256), 256>>>(a, n);
-        CUDA_TRY(cudaGetLastError());
-        g_launches.fetch_add(1);
+        if ((rc = launched("stream reset"))) return rc;
     }
     if (!ids && ss->d_hold) CUDA_TRY(cudaMemset(ss->d_hold, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(long long)));
     CUDA_TRY(cudaDeviceSynchronize());
@@ -2848,23 +2805,14 @@ __global__ void __launch_bounds__(kLookupThreads) acb_lookup_kernel(const __grid
 }
 } // namespace
 
-/* fixed stride: stride >= 0, a multiple of the letter width, n * stride == total (without overflow) */
-static bool lookup_stride_ok(const acb_table *tb, int64_t total_bytes, int64_t n_keys, int64_t stride_bytes) {
-    if (stride_bytes < 0 || stride_bytes % tb->L) return false;
-    if (stride_bytes == 0) return total_bytes == 0;
-    return n_keys <= total_bytes / stride_bytes && n_keys * stride_bytes == total_bytes;
-}
-
 extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t total_bytes, const int64_t *d_offsets,
                                  int64_t n_keys, int64_t stride_bytes, int32_t *d_key_id, int32_t *d_prefix, void *stream) {
     if (!tb || total_bytes < 0 || n_keys < 0 || (total_bytes && !d_keys) || (n_keys && (!d_key_id || !d_prefix))) {
         acb_set_error("bad argument");
         return ACB_EINVAL;
     }
-    if (!d_offsets && !lookup_stride_ok(tb, total_bytes, n_keys, stride_bytes)) {
-        acb_set_error("fixed-stride keys need stride_bytes >= 0, a multiple of letter_bytes, and n_keys*stride == total_bytes");
-        return ACB_EINVAL;
-    }
+    int rc;
+    if (!d_offsets && (rc = check_stride(tb->L, total_bytes, n_keys, stride_bytes, 0))) return rc;
     if (n_keys == 0) return ACB_OK;
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -2874,23 +2822,10 @@ extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t t
     p.letter_shift = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
     p.key_id = d_key_id; p.prefix = d_prefix;
     const long long grid = std::min<long long>((n_keys + kLookupThreads - 1) / kLookupThreads, (long long)tb->sm_count * 8);
-    const bool timing = g_timing.load() != 0;
-    if (timing) {
-        if (!tb->ev0) { CUDA_TRY(cudaEventCreate(&tb->ev0)); CUDA_TRY(cudaEventCreate(&tb->ev1)); }
-        CUDA_TRY(cudaEventRecord(tb->ev0, s));
-    }
+    if ((rc = timing_mark(&tb->ev0, s))) return rc;
     acb_lookup_kernel<<<(unsigned)grid, kLookupThreads, 0, s>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { acb_set_error("lookup kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
-    g_launches.fetch_add(1);
-    if (timing) {
-        CUDA_TRY(cudaEventRecord(tb->ev1, s));
-        CUDA_TRY(cudaEventSynchronize(tb->ev1));
-        float ms = 0.f;
-        CUDA_TRY(cudaEventElapsedTime(&ms, tb->ev0, tb->ev1));
-        g_last_ms = ms;
-    }
-    return ACB_OK;
+    if ((rc = launched("lookup kernel")) || (rc = timing_mark(&tb->ev1, s))) return rc;
+    return timing_ms(tb->ev0, tb->ev1, &g_last_ms);
 }
 
 extern "C" int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total_bytes, const int64_t *offsets,
@@ -2900,29 +2835,13 @@ extern "C" int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total
         return ACB_EINVAL;
     }
     CUDA_TRY(cudaSetDevice(tb->device));
-    if (offsets) {                                  /* the kernel reads keys[offsets[i] .. offsets[i+1]) unchecked */
-        bool ok = offsets[0] == 0 && offsets[n_keys] == total_bytes;
-        for (int64_t i = 0; ok && i < n_keys; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % tb->L == 0;
-        if (!ok) {
-            acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes");
-            return ACB_EINVAL;
-        }
-    } else if (!lookup_stride_ok(tb, total_bytes, n_keys, stride_bytes)) {
-        acb_set_error("fixed-stride keys need stride_bytes >= 0, a multiple of letter_bytes, and n_keys*stride == total_bytes");
-        return ACB_EINVAL;
-    }
-    if (n_keys == 0) return ACB_OK;
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    int rc;
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_keys + 1))) return rc;
-    if ((rc = ensure(&tb->w_lk, &tb->w_lk_cap, 2 * (size_t)n_keys))) return rc;
-    cudaStream_t s = tb->stream;
-    if (total_bytes) CUDA_TRY(cudaMemcpyAsync(tb->w_hay, keys, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
-    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_keys + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
-    rc = acb_lookup_device(tb, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_keys,
-                           stride_bytes, tb->w_lk, tb->w_lk + n_keys, s);
+    int rc = offsets ? check_offsets(tb->L, offsets, n_keys, total_bytes) : check_stride(tb->L, total_bytes, n_keys, stride_bytes, 0);
     if (rc != ACB_OK) return rc;
+    if (n_keys == 0) return ACB_OK;
+    const int64_t *d_off = nullptr;
+    if ((rc = upload_batch(tb, keys, total_bytes, offsets, n_keys, &d_off)) || (rc = ensure(&tb->w_lk, &tb->w_lk_cap, 2 * (size_t)n_keys))) return rc;
+    cudaStream_t s = tb->stream;
+    if ((rc = acb_lookup_device(tb, tb->w_hay, total_bytes, d_off, n_keys, stride_bytes, tb->w_lk, tb->w_lk + n_keys, s))) return rc;
     CUDA_TRY(cudaMemcpyAsync(key_id, tb->w_lk, (size_t)n_keys * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(prefix, tb->w_lk + n_keys, (size_t)n_keys * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
@@ -3120,13 +3039,11 @@ static int select_count(acb_table *tb, const SelectParams &p, int64_t n, int64_t
     }
     const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, (long long)tb->sm_count * 16);
     acb_select_kernel<false><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { acb_set_error("select kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
-    g_launches.fetch_add(1);
+    int rc = launched("select kernel");
+    if (rc != ACB_OK) return rc;
     long long *cnt = reinterpret_cast<long long *>(d_out_off) + 1;     /* in place: counts -> inclusive sums */
     size_t temp = 0;
     CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, temp, cnt, cnt, (long long)n, s));
-    int rc;
     if ((rc = ensure(&tb->w_scan, &tb->w_scan_cap, temp))) return rc;
     CUDA_TRY(cub::DeviceScan::InclusiveSum(tb->w_scan, temp, cnt, cnt, (long long)n, s));
     CUDA_TRY(cudaMemcpyAsync(d_total, d_out_off + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
@@ -3138,10 +3055,7 @@ static int select_fill(acb_table *tb, const SelectParams &p, int64_t n, cudaStre
     if (n == 0 || p.cap == 0) return ACB_OK;
     const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, (long long)tb->sm_count * 16);
     acb_select_kernel<true><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { acb_set_error("select kernel launch failed: %s", cudaGetErrorString(e)); return ACB_ECUDA; }
-    g_launches.fetch_add(1);
-    return ACB_OK;
+    return launched("select kernel");
 }
 
 static int select_common_checks(const acb_table *tb, const void *pat, int64_t total_bytes, int64_t n, const void *out_off,
@@ -3164,30 +3078,16 @@ extern "C" int acb_select_device(acb_table *tb, const uint8_t *d_patterns, int64
                                  int32_t *d_key_id, int64_t cap, int64_t *d_total, void *stream) {
     int rc = select_common_checks(tb, d_patterns, total_bytes, n, d_out_offsets, d_key_id, cap, d_total, wildcard, how);
     if (rc != ACB_OK) return rc;
-    if (!d_offsets && !lookup_stride_ok(tb, total_bytes, n, stride_bytes)) {
-        acb_set_error("fixed-stride patterns need stride_bytes >= 0, a multiple of letter_bytes, and n*stride == total_bytes");
-        return ACB_EINVAL;
-    }
+    if (!d_offsets && (rc = check_stride(tb->L, total_bytes, n, stride_bytes, 0))) return rc;
     if ((rc = select_view_ok(tb))) return rc;
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     SelectParams p;
     fill_select_params(tb, p, d_patterns, d_offsets, n, stride_bytes, wildcard, how, d_out_offsets, d_key_id, cap, d_total);
-    const bool timing = g_timing.load() != 0;
-    if (timing) {
-        if (!tb->ev0) { CUDA_TRY(cudaEventCreate(&tb->ev0)); CUDA_TRY(cudaEventCreate(&tb->ev1)); }
-        CUDA_TRY(cudaEventRecord(tb->ev0, s));
-    }
-    if ((rc = select_count(tb, p, n, d_out_offsets, d_total, s))) return rc;
-    if ((rc = select_fill(tb, p, n, s))) return rc;
-    if (timing) {
-        CUDA_TRY(cudaEventRecord(tb->ev1, s));
-        CUDA_TRY(cudaEventSynchronize(tb->ev1));
-        float ms = 0.f;
-        CUDA_TRY(cudaEventElapsedTime(&ms, tb->ev0, tb->ev1));
-        g_last_ms = ms;
-    }
-    return ACB_OK;
+    if ((rc = timing_mark(&tb->ev0, s)) || (rc = select_count(tb, p, n, d_out_offsets, d_total, s)) || (rc = select_fill(tb, p, n, s)) ||
+        (rc = timing_mark(&tb->ev1, s)))
+        return rc;
+    return timing_ms(tb->ev0, tb->ev1, &g_last_ms);
 }
 
 extern "C" int acb_select_host(acb_table *tb, const uint8_t *patterns, int64_t total_bytes, const int64_t *offsets,
@@ -3195,30 +3095,14 @@ extern "C" int acb_select_host(acb_table *tb, const uint8_t *patterns, int64_t t
                                int32_t *key_id, int64_t cap, int64_t *total) {
     int rc = select_common_checks(tb, patterns, total_bytes, n, out_offsets, key_id, cap, total, wildcard, how);
     if (rc != ACB_OK) return rc;
-    if (offsets) {                                  /* the kernels read patterns[offsets[i] .. offsets[i+1]) unchecked */
-        bool ok = offsets[0] == 0 && offsets[n] == total_bytes;
-        for (int64_t i = 0; ok && i < n; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % tb->L == 0;
-        if (!ok) {
-            acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes");
-            return ACB_EINVAL;
-        }
-    } else if (!lookup_stride_ok(tb, total_bytes, n, stride_bytes)) {
-        acb_set_error("fixed-stride patterns need stride_bytes >= 0, a multiple of letter_bytes, and n*stride == total_bytes");
-        return ACB_EINVAL;
-    }
+    if ((rc = offsets ? check_offsets(tb->L, offsets, n, total_bytes) : check_stride(tb->L, total_bytes, n, stride_bytes, 0))) return rc;
     if ((rc = select_view_ok(tb))) return rc;
-    CUDA_TRY(cudaSetDevice(tb->device));
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n + 1))) return rc;
-    if ((rc = ensure(&tb->w_sel_off, &tb->w_sel_off_cap, (size_t)n + 2))) return rc;
+    const int64_t *d_off = nullptr;
+    if ((rc = upload_batch(tb, patterns, total_bytes, offsets, n, &d_off)) || (rc = ensure(&tb->w_sel_off, &tb->w_sel_off_cap, (size_t)n + 2))) return rc;
     cudaStream_t s = tb->stream;
-    if (total_bytes) CUDA_TRY(cudaMemcpyAsync(tb->w_hay, patterns, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
-    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
     int64_t *d_out = reinterpret_cast<int64_t *>(tb->w_sel_off), *d_total = d_out + n + 1;
     SelectParams p;
-    fill_select_params(tb, p, tb->w_hay, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n, stride_bytes,
-                       wildcard, how, d_out, nullptr, 0, d_total);
+    fill_select_params(tb, p, tb->w_hay, d_off, n, stride_bytes, wildcard, how, d_out, nullptr, 0, d_total);
     if ((rc = select_count(tb, p, n, d_out, d_total, s))) return rc;
     CUDA_TRY(cudaMemcpyAsync(out_offsets, d_out, (size_t)(n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
@@ -3389,13 +3273,6 @@ __global__ void acb_ll_count_kernel(const unsigned long long *d_m, const uint8_t
 char *carve(char *&p, size_t bytes) { char *r = p; p += (bytes + 255) & ~(size_t)255; return r; }
 } // namespace
 
-static int ll_stage(acb_table *tb, int k, cudaStream_t s) {
-    if (!g_timing.load()) return ACB_OK;
-    if (!tb->l_ev[k]) CUDA_TRY(cudaEventCreate(&tb->l_ev[k]));
-    CUDA_TRY(cudaEventRecord(tb->l_ev[k], s));
-    return ACB_OK;
-}
-
 extern "C" int acb_last_leftmost_ms(float *ms, int32_t n) {
     if (!ms || n < 0 || n > 5) { acb_set_error("bad argument"); return ACB_EINVAL; }
     for (int i = 0; i < n; i++) ms[i] = g_ll_ms[i];
@@ -3430,12 +3307,8 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     const size_t N = (size_t)n;
     const size_t need = 8 * 256 + 2 * N * sizeof(unsigned long long) + 2 * N * sizeof(acb_match) + N + 2 * N * sizeof(int32_t) +
                         (size_t)n_tiles * sizeof(unsigned long long) + temp;
-    if (tb->l_done) CUDA_TRY(cudaStreamWaitEvent(s, tb->l_done, 0));
-    if (tb->l_buf_cap < need) {
-        if (tb->l_buf) { CUDA_TRY(cudaStreamSynchronize(s)); cudaFree(tb->l_buf); tb->l_buf = nullptr; tb->l_buf_cap = 0; }
-        CUDA_TRY(cudaMalloc(&tb->l_buf, need + need / 4));
-        tb->l_buf_cap = need + need / 4;
-    }
+    int rc;
+    if ((rc = scratch_wait(tb->l_done, s)) || (rc = grow_synced(&tb->l_buf, &tb->l_buf_cap, need, s))) return rc;
     if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
     char *p = reinterpret_cast<char *>(tb->l_buf);
     unsigned long long *k0 = reinterpret_cast<unsigned long long *>(carve(p, N * 8)), *k1 = reinterpret_cast<unsigned long long *>(carve(p, N * 8));
@@ -3446,60 +3319,46 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     void *tmp = carve(p, temp);
     size_t tb_temp = temp;
     const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, (long long)tb->sm_count * 16);
-    int rc;
-    if ((rc = ll_stage(tb, 0, s))) return rc;
+    if ((rc = timing_mark(&tb->l_ev[0], s))) return rc;
     /* 1. re-key by start and sort */
     if (one_pass) {
         acb_sortkey_kernel<kKeyStart><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
-        CUDA_TRY(cudaGetLastError());
+        if ((rc = launched("leftmost sort key"))) return rc;
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, d_records, ra, ni, 0, bh + be + bl, s));
-        g_launches.fetch_add(1);
     } else {                                               /* two stable passes: start | (max_len - len), then hay */
         acb_sortkey_kernel<kKeyStartLow><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, d_records, rb, ni, 0, be + bl, s));
         acb_sortkey_kernel<kKeyHay><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(rb, n, tb->d_keylen, be, bl, max_len, k0);
-        CUDA_TRY(cudaGetLastError());
+        if ((rc = launched("leftmost sort keys", 2))) return rc;
         tb_temp = temp;
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, rb, ra, ni, 0, bh, s));
-        g_launches.fetch_add(2);
     }
-    if ((rc = ll_stage(tb, 1, s))) return rc;
+    if ((rc = timing_mark(&tb->l_ev[1], s))) return rc;
     /* 2. candidates: the longest match at every (hay, start) */
     acb_ll_cand_kernel<<<grid, 256, 0, s>>>(ra, n, tb->d_keylen, flag);
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = launched("leftmost candidates"))) return rc;
     tb_temp = temp;
     CUDA_TRY(cub::DeviceSelect::Flagged(tmp, tb_temp, ra, flag, rb, tb->l_ctr, ni, s));
-    g_launches.fetch_add(1);
-    if ((rc = ll_stage(tb, 2, s))) return rc;
+    if ((rc = timing_mark(&tb->l_ev[2], s))) return rc;
     /* 3. successors */
     acb_ll_next_kernel<<<grid, 256, 0, s>>>(rb, tb->l_ctr, tb->d_keylen, nxt);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-    if ((rc = ll_stage(tb, 3, s))) return rc;
+    if ((rc = launched("leftmost successors")) || (rc = timing_mark(&tb->l_ev[3], s))) return rc;
     /* 4. chain marking */
     CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)n_tiles * sizeof(unsigned long long), s));
     CUDA_TRY(cudaMemsetAsync(pos, 0, N * sizeof(int32_t), s));
     CUDA_TRY(cudaMemsetAsync(tb->l_ctr + 1, 0, sizeof(unsigned long long), s));
     acb_ll_chain_kernel<<<(unsigned)n_tiles, kLlThreads, 0, s>>>(rb, tb->l_ctr, nxt, std::max(max_len, 1), tb->l_ctr + 1, status, flag, pos);
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-    if ((rc = ll_stage(tb, 4, s))) return rc;
+    if ((rc = launched("leftmost chain")) || (rc = timing_mark(&tb->l_ev[4], s))) return rc;
     /* 5. emit */
     tb_temp = temp;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb_temp, pos, pos, ni, s));
     acb_ll_emit_kernel<<<grid, 256, 0, s>>>(rb, tb->l_ctr, flag, pos, d_out, cap, reinterpret_cast<const unsigned long long *>(d_count));
     CUDA_TRY(cudaGetLastError());
     acb_ll_count_kernel<<<1, 1, 0, s>>>(tb->l_ctr, flag, pos, reinterpret_cast<unsigned long long *>(d_count));
-    CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(2);
-    if ((rc = ll_stage(tb, 5, s))) return rc;
-    if (!tb->l_done) CUDA_TRY(cudaEventCreateWithFlags(&tb->l_done, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventRecord(tb->l_done, s));
-    if (g_timing.load()) {
-        CUDA_TRY(cudaEventSynchronize(tb->l_ev[5]));
-        for (int k = 0; k < 5; k++) CUDA_TRY(cudaEventElapsedTime(&g_ll_ms[k], tb->l_ev[k], tb->l_ev[k + 1]));
-    }
+    if ((rc = launched("leftmost emit", 2)) || (rc = timing_mark(&tb->l_ev[5], s)) || (rc = scratch_done(&tb->l_done, s))) return rc;
+    for (int k = 0; k < 5; k++)
+        if ((rc = timing_ms(tb->l_ev[k], tb->l_ev[k + 1], &g_ll_ms[k]))) return rc;
     return ACB_OK;
 }
 
@@ -3507,22 +3366,12 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
  * tb->w_out, grown until it fits; *full is its length.  On tb->stream, which it leaves synchronised. */
 static int upload_and_scan_full(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
                                 int64_t stride_bytes, int algo, const int64_t **d_off, unsigned long long *full) {
-    CUDA_TRY(cudaSetDevice(tb->device));
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
-    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
-    if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
     int rc;
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total_bytes + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n_hay + 1))) return rc;
-    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(2 * n_hay, 4096)))) return rc;
+    if ((rc = upload_batch(tb, hay, total_bytes, offsets, n_hay, d_off)) ||
+        (rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(2 * n_hay, 4096))))
+        return rc;
+    if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
     cudaStream_t s = tb->stream;
-    CUDA_TRY(cudaMemcpyAsync(tb->w_hay, hay, (size_t)total_bytes, cudaMemcpyHostToDevice, s));
-    *d_off = nullptr;
-    if (offsets) {
-        CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n_hay + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
-        *d_off = reinterpret_cast<const int64_t *>(tb->w_off);
-    }
     for (;;) {                                             /* the full list: an intermediate, in a buffer grown to fit */
         CUDA_TRY(cudaMemsetAsync(tb->w_count, 0, sizeof(unsigned long long), s));
         if ((rc = acb_scan_device(tb, tb->w_hay, total_bytes, *d_off, n_hay, stride_bytes, tb->w_out, (int64_t)tb->w_out_cap,
@@ -3543,15 +3392,12 @@ extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t
     *n_found = 0;
     if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("leftmost-longest takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
-    if (!offsets && (stride_bytes <= 0 || stride_bytes % tb->L || stride_bytes * n_hay != total_bytes)) {
-        acb_set_error("fixed-stride batch needs stride_bytes > 0, a multiple of letter_bytes, and n_hay*stride == total_bytes");
-        return ACB_EINVAL;
-    }
+    int rc;
+    if (!offsets && (rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1))) return rc;
     tb->h_out_n = 0;
     if (total_bytes == 0 || n_hay == 0) return ACB_OK;
     const int64_t *d_off = nullptr;
     unsigned long long full = 0;
-    int rc;
     if ((rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, &d_off, &full))) return rc;
     cudaStream_t s = tb->stream;
     if (full == 0) return ACB_OK;
@@ -3562,20 +3408,7 @@ extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t
     if ((rc = acb_leftmost_longest_device(tb, tb->w_out, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, tb->l_out,
                                           kept_cap, reinterpret_cast<int64_t *>(d_n), s)))
         return rc;
-    CUDA_TRY(cudaMemcpyAsync(tb->h_count, d_n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    const unsigned long long n = *tb->h_count;
-    *n_found = (int64_t)n;
-    if (n > (unsigned long long)cap) {
-        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
-        return ACB_EOVERFLOW;
-    }
-    if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->l_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
-    tb->h_out_n = n;
-    return ACB_OK;
+    return read_back(tb, d_n, tb->l_out, cap, 0, n_hay, 0, out, n_found, s);
 }
 
 /* ------------------------------------------------------------ leftmost-longest replacement */
@@ -3760,12 +3593,8 @@ extern "C" int acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t
     *out = nullptr;
     if (tb->L != 1 && tb->L != 2 && tb->L != 4) { acb_set_error("not a table"); return ACB_EINVAL; }
     if (n_ids < tb->n_keys) { acb_set_error("%lld replacements for %d key ids", (long long)n_ids, tb->n_keys); return ACB_EINVAL; }
-    bool ok = rep_offsets[0] == 0 && rep_offsets[n_ids] == rep_bytes;
-    for (int64_t i = 0; ok && i < n_ids; i++) ok = rep_offsets[i + 1] >= rep_offsets[i] && rep_offsets[i + 1] % tb->L == 0;
-    if (!ok) {
-        acb_set_error("replacement offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at rep_bytes");
-        return ACB_EINVAL;
-    }
+    int rc = check_offsets(tb->L, rep_offsets, n_ids, rep_bytes);
+    if (rc != ACB_OK) return rc;
     CUDA_TRY(cudaSetDevice(tb->device));
     acb_replacer *r = new (std::nothrow) acb_replacer();
     if (!r) { acb_set_error("out of memory"); return ACB_ENOMEM; }
@@ -3797,32 +3626,14 @@ extern "C" int acb_last_replace_ms(float *ms, int32_t n) {
     return ACB_OK;
 }
 
-static int rp_event(acb_table *tb, int k, cudaStream_t s) {
-    if (!g_timing.load()) return ACB_OK;
-    if (!tb->r_ev[k]) CUDA_TRY(cudaEventCreate(&tb->r_ev[k]));
-    CUDA_TRY(cudaEventRecord(tb->r_ev[k], s));
-    return ACB_OK;
-}
-
-static int rp_launch(const char *what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { acb_set_error("%s launch failed: %s", what, cudaGetErrorString(e)); return ACB_ECUDA; }
-    g_launches.fetch_add(1);
-    return ACB_OK;
-}
-
 /* The offsets pass on s: a.out_off[0..n_hay] and *a.total.  Carves the per-record arrays from tb->r_buf. */
 static int rp_offsets(acb_table *tb, RpArgs &a, cudaStream_t s) {
     const size_t C = (size_t)a.cap;
     size_t temp = 0;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, (long long *)nullptr, (long long *)nullptr, a.cap + 1, s));
     const size_t need = 6 * 256 + (C + 1) * 8 + 4 * C * 8 + temp;
-    if (tb->r_done) CUDA_TRY(cudaStreamWaitEvent(s, tb->r_done, 0));
-    if (tb->r_buf_cap < need) {
-        if (tb->r_buf) { CUDA_TRY(cudaStreamSynchronize(s)); cudaFree(tb->r_buf); tb->r_buf = nullptr; tb->r_buf_cap = 0; }
-        CUDA_TRY(cudaMalloc(&tb->r_buf, need + need / 4));
-        tb->r_buf_cap = need + need / 4;
-    }
+    int rc;
+    if ((rc = scratch_wait(tb->r_done, s)) || (rc = grow_synced(&tb->r_buf, &tb->r_buf_cap, need, s))) return rc;
     char *p = reinterpret_cast<char *>(tb->r_buf);
     a.D = reinterpret_cast<long long *>(carve(p, (C + 1) * 8));
     a.P = reinterpret_cast<long long *>(carve(p, C * 8));
@@ -3831,24 +3642,23 @@ static int rp_offsets(acb_table *tb, RpArgs &a, cudaStream_t s) {
     a.RS = reinterpret_cast<long long *>(carve(p, C * 8));
     void *tmp = carve(p, temp);
     const long long most = (long long)tb->sm_count * 16;
-    int rc;
-    if ((rc = rp_event(tb, 0, s))) return rc;
+    if ((rc = timing_mark(&tb->r_ev[0], s))) return rc;
     acb_rp_delta_kernel<<<(unsigned)std::min<long long>((a.cap + 256) / 256, most), 256, 0, s>>>(a);
-    if ((rc = rp_launch("replacement delta"))) return rc;
+    if ((rc = launched("replacement delta"))) return rc;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, temp, a.D, a.D, a.cap + 1, s));
     if (a.cap) {
         acb_rp_records_kernel<<<(unsigned)std::min<long long>((a.cap + 255) / 256, most), 256, 0, s>>>(a);
-        if ((rc = rp_launch("replacement records"))) return rc;
+        if ((rc = launched("replacement records"))) return rc;
     }
     acb_rp_offsets_kernel<<<(unsigned)std::min<long long>((a.n_hay + 256) / 256, most), 256, 0, s>>>(a);
-    if ((rc = rp_launch("replacement offsets"))) return rc;
-    return rp_event(tb, 1, s);
+    if ((rc = launched("replacement offsets"))) return rc;
+    return timing_mark(&tb->r_ev[1], s);
 }
 
 /* The write pass on s: a.out, when *a.total <= a.out_cap (checked on the device).  Then the scratch event and timing. */
 static int rp_write(acb_table *tb, RpArgs &a, cudaStream_t s) {
     int rc;
-    if ((rc = rp_event(tb, 2, s))) return rc;
+    if ((rc = timing_mark(&tb->r_ev[2], s))) return rc;
     if (a.out_cap > 0) {
         const long long max_tiles = (a.out_cap + kRpTile - 1) / kRpTile;
         if (tb->r_ts_cap < (size_t)max_tiles + 1) {
@@ -3858,19 +3668,13 @@ static int rp_write(acb_table *tb, RpArgs &a, cudaStream_t s) {
         a.ts = tb->r_ts;
         const long long most = (long long)tb->sm_count * 16;
         acb_rp_tiles_kernel<<<(unsigned)std::min<long long>((max_tiles + 256) / 256, most), 256, 0, s>>>(a);
-        if ((rc = rp_launch("replacement tiles"))) return rc;
+        if ((rc = launched("replacement tiles"))) return rc;
         acb_rp_write_kernel<<<(unsigned)std::min<long long>(max_tiles, (long long)tb->sm_count * 8), kRpThreads, 0, s>>>(a);
-        if ((rc = rp_launch("replacement write"))) return rc;
+        if ((rc = launched("replacement write"))) return rc;
     }
-    if ((rc = rp_event(tb, 3, s))) return rc;
-    if (!tb->r_done) CUDA_TRY(cudaEventCreateWithFlags(&tb->r_done, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventRecord(tb->r_done, s));
-    if (g_timing.load()) {
-        CUDA_TRY(cudaEventSynchronize(tb->r_ev[3]));
-        CUDA_TRY(cudaEventElapsedTime(&g_rp_ms[0], tb->r_ev[0], tb->r_ev[1]));
-        CUDA_TRY(cudaEventElapsedTime(&g_rp_ms[1], tb->r_ev[2], tb->r_ev[3]));
-    }
-    return ACB_OK;
+    if ((rc = timing_mark(&tb->r_ev[3], s)) || (rc = scratch_done(&tb->r_done, s)) || (rc = timing_ms(tb->r_ev[0], tb->r_ev[1], &g_rp_ms[0])))
+        return rc;
+    return timing_ms(tb->r_ev[2], tb->r_ev[3], &g_rp_ms[1]);
 }
 
 static int rp_check(const acb_replacer *r, const acb_table *tb, int64_t total_bytes, int64_t n_hay, int64_t stride_bytes,
@@ -3879,11 +3683,7 @@ static int rp_check(const acb_replacer *r, const acb_table *tb, int64_t total_by
     int rc = rp_fits(r, tb);
     if (rc) return rc;
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
-    if (!has_offsets && (stride_bytes < 0 || stride_bytes % tb->L || stride_bytes * n_hay != total_bytes)) {
-        acb_set_error("fixed-stride batch needs stride_bytes >= 0, a multiple of letter_bytes, and n_hay*stride == total_bytes");
-        return ACB_EINVAL;
-    }
-    return ACB_OK;
+    return has_offsets ? ACB_OK : check_stride(tb->L, total_bytes, n_hay, stride_bytes, 0);
 }
 
 static void rp_args(RpArgs &a, const acb_replacer *r, const acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
@@ -3929,14 +3729,7 @@ extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *h
     if (rc) return rc;
     if ((total_bytes && !hay) || !out_offsets || !total || (out_cap && !out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("replacement takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
-    if (offsets) {                                          /* the kernels read hay[offsets[h] .. offsets[h+1]) unchecked */
-        bool ok = offsets[0] == 0 && offsets[n_hay] == total_bytes;
-        for (int64_t i = 0; ok && i < n_hay; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % tb->L == 0;
-        if (!ok) {
-            acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes");
-            return ACB_EINVAL;
-        }
-    }
+    if (offsets && (rc = check_offsets(tb->L, offsets, n_hay, total_bytes))) return rc;
     *total = 0;
     for (float &v : g_rp_ms) v = 0.f;
     if (n_hay == 0) { out_offsets[0] = 0; return ACB_OK; }
@@ -4197,20 +3990,6 @@ extern "C" int acb_last_stream_leftmost_ms(float *ms, int32_t n) {
     return ACB_OK;
 }
 
-static int sl_event(acb_streams *ss, int k, cudaStream_t s) {
-    if (!g_timing.load()) return ACB_OK;
-    if (!ss->ev[k]) CUDA_TRY(cudaEventCreate(&ss->ev[k]));
-    CUDA_TRY(cudaEventRecord(ss->ev[k], s));
-    return ACB_OK;
-}
-
-static int sl_launch(const char *what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { acb_set_error("%s launch failed: %s", what, cudaGetErrorString(e)); return ACB_ECUDA; }
-    g_launches.fetch_add(1);
-    return ACB_OK;
-}
-
 /* the arguments every leftmost feed checks before anything runs */
 static int sl_check(const acb_streams *ss, const acb_table *tb, int64_t total, const void *offsets, int64_t n, int64_t stride,
                     int *algo) {
@@ -4220,10 +3999,7 @@ static int sl_check(const acb_streams *ss, const acb_table *tb, int64_t total, c
     if (rc != ACB_OK) return rc;
     if (n > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n, ss->n); return ACB_EINVAL; }
     if (n >= 0x7fffffffLL) { acb_set_error("2^31-1 or more chunks in one feed"); return ACB_ERANGE; }
-    if (!offsets && (stride < 0|| stride % ss->L || stride * n != total)) {
-        acb_set_error("fixed-stride feed needs stride_bytes >= 0, a multiple of letter_bytes, and n_chunks*stride == total_bytes");
-        return ACB_EINVAL;
-    }
+    if (!offsets && (rc = check_stride(ss->L, total, n, stride, 0))) return rc;
     if (*algo == ACB_ALGO_AUTO) *algo = ACB_ALGO_FILTER;
     if (*algo != ACB_ALGO_FILTER && *algo != ACB_ALGO_DFA) { acb_set_error("a leftmost-longest feed takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
     return ACB_OK;
@@ -4259,11 +4035,11 @@ static int sl_gather(acb_streams *ss, acb_table *tb, const SlArgs &a, bool stage
     if (rc) return rc;
     acb_sl_tiles_kernel<<<(unsigned)std::min<long long>((n_tiles + 255) / 256, (long long)tb->sm_count * 16), 256, 0, s>>>(doff, a.n, total,
                                                                                                                    ss->d_ts);
-    if ((rc = sl_launch("stream gather tiles"))) return rc;
+    if ((rc = launched("stream gather tiles"))) return rc;
     const unsigned grid = (unsigned)std::min<long long>(n_tiles, (long long)tb->sm_count * 8);
     if (stage) acb_sl_gather_kernel<true><<<grid, 256, 0, s>>>(a, doff, ss->d_ts, dst, total);
     else acb_sl_gather_kernel<false><<<grid, 256, 0, s>>>(a, doff, ss->d_ts, dst, total);
-    return sl_launch("stream gather");
+    return launched("stream gather");
 }
 
 /* The leftmost feed on DEVICE buffers, both forms.  r == nullptr: the chosen records go to d_out (cap, *d_count,
@@ -4293,12 +4069,12 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     const unsigned g_chunks = (unsigned)std::min<long long>((n + 256) / 256, most);
     /* 1. stage */
     acb_sl_len_kernel<<<g_chunks, 256, 0, s>>>(a);
-    if ((rc = sl_launch("stream staged lengths"))) return rc;
+    if ((rc = launched("stream staged lengths"))) return rc;
     long long staged = 0;
     if ((rc = sl_offsets(ss, ss->d_soff, n, s, &staged))) return rc;
     if ((rc = ensure(&ss->d_stage, &ss->stage_cap, (size_t)staged + 64))) return rc;
     a.stage = ss->d_stage;
-    if ((rc = sl_event(ss, 0, s)) || (rc = sl_gather(ss, tb, a, true, ss->d_soff, ss->d_stage, staged, s)) || (rc = sl_event(ss, 1, s))) return rc;
+    if ((rc = timing_mark(&ss->ev[0], s)) || (rc = sl_gather(ss, tb, a, true, ss->d_soff, ss->d_stage, staged, s)) || (rc = timing_mark(&ss->ev[1], s))) return rc;
     /* 2. scan and 3. the frontier filter; the full list grows until it fits */
     const int64_t *soff = reinterpret_cast<const int64_t *>(ss->d_soff);
     unsigned long long m = 0;
@@ -4310,31 +4086,29 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
             return rc;
         fcap = std::min<size_t>(ss->full_cap, 0x7fffffffULL);
         CUDA_TRY(cudaMemsetAsync(ss->d_ctr, 0, 4 * sizeof(unsigned long long), s));
-        if ((rc = sl_event(ss, 2, s))) return rc;
+        if ((rc = timing_mark(&ss->ev[2], s))) return rc;
         if (staged && (rc = acb_scan_device(tb, ss->d_stage, staged, soff, n, 0, ss->d_full, (int64_t)fcap,
                                             reinterpret_cast<int64_t *>(ss->d_ctr), s, algo)))
             return rc;
-        if ((rc = sl_event(ss, 3, s)) || (rc = sl_event(ss, 4, s))) return rc;
+        if ((rc = timing_mark(&ss->ev[3], s)) || (rc = timing_mark(&ss->ev[4], s))) return rc;
         acb_sl_flag_kernel<<<(unsigned)std::min<long long>(((long long)fcap + 255) / 256, most), 256, 0, s>>>(a, ss->d_full, ss->d_ctr,
                                                                                                        (long long)fcap, tb->d_keylen, ss->d_flag);
-        if ((rc = sl_launch("stream frontier flags"))) return rc;
+        if ((rc = launched("stream frontier flags"))) return rc;
         size_t temp = 0;
         CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, temp, ss->d_full, ss->d_flag, ss->d_settled, ss->d_ctr + 1, (int)fcap, s));
         if ((rc = sl_tmp(ss, temp))) return rc;
         temp = ss->tmp_cap;
         CUDA_TRY(cub::DeviceSelect::Flagged(ss->d_tmp, temp, ss->d_full, ss->d_flag, ss->d_settled, ss->d_ctr + 1, (int)fcap, s));
-        if ((rc = sl_event(ss, 5, s))) return rc;
+        if ((rc = timing_mark(&ss->ev[5], s))) return rc;
         CUDA_TRY(cudaMemcpyAsync(ss->h_ctr, ss->d_ctr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
         CUDA_TRY(cudaStreamSynchronize(s));
         if (ss->h_ctr[0] <= fcap) { m = ss->h_ctr[1]; break; }
         if (ss->h_ctr[0] > 0x7fffffffULL) { acb_set_error("more than 2^31-1 matches in one feed"); return ACB_ERANGE; }
         if ((rc = ensure(&ss->d_full, &ss->full_cap, (size_t)ss->h_ctr[0]))) return rc;
     }
-    if (g_timing.load()) {
-        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[0], ss->ev[0], ss->ev[1]));
-        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[1], ss->ev[2], ss->ev[3]));
-        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[2], ss->ev[4], ss->ev[5]));
-    }
+    if ((rc = timing_ms(ss->ev[0], ss->ev[1], &g_sl_ms[0])) || (rc = timing_ms(ss->ev[2], ss->ev[3], &g_sl_ms[1])) ||
+        (rc = timing_ms(ss->ev[4], ss->ev[5], &g_sl_ms[2])))
+        return rc;
     /* 4. select */
     acb_match *chosen = d_out;
     int64_t ccap = cap;
@@ -4344,41 +4118,36 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
         chosen = ss->d_chosen; ccap = (int64_t)m; ccount = ss->d_ctr + 2;
     }
     const int64_t max_letters = std::max<int64_t>(staged / ss->L, 1);
-    if ((rc = sl_event(ss, 6, s))) return rc;
+    if ((rc = timing_mark(&ss->ev[6], s))) return rc;
     if (m && (rc = acb_leftmost_longest_device(tb, ss->d_settled, (int64_t)m, n, max_letters, chosen, ccap,
                                                reinterpret_cast<int64_t *>(ccount), s)))
         return rc;
-    if ((rc = sl_event(ss, 7, s))) return rc;
+    if ((rc = timing_mark(&ss->ev[7], s))) return rc;
     /* 5. the new X per chunk, and the windows of a replacing feed */
     CUDA_TRY(cudaMemsetAsync(a.last, 0xff, N * sizeof(long long), s));
     if (m) {
         acb_sl_last_kernel<<<(unsigned)std::min<long long>(((long long)m + 255) / 256, most), 256, 0, s>>>(a, chosen, ccount, ccap, r ? 0 : 1);
-        if ((rc = sl_launch("stream last chosen"))) return rc;
+        if ((rc = launched("stream last chosen"))) return rc;
     }
     acb_sl_frontier_kernel<<<g_chunks, 256, 0, s>>>(a);
-    if ((rc = sl_launch("stream frontier"))) return rc;
+    if ((rc = launched("stream frontier"))) return rc;
     if (r) {
         long long wtotal = 0;
         if ((rc = sl_offsets(ss, a.woff, n, s, &wtotal))) return rc;
         if ((rc = ensure(&ss->d_win, &ss->win_cap, (size_t)wtotal + 64))) return rc;
-        if ((rc = sl_event(ss, 8, s)) || (rc = sl_gather(ss, tb, a, false, a.woff, ss->d_win, wtotal, s)) || (rc = sl_event(ss, 9, s))) return rc;
+        if ((rc = timing_mark(&ss->ev[8], s)) || (rc = sl_gather(ss, tb, a, false, a.woff, ss->d_win, wtotal, s)) || (rc = timing_mark(&ss->ev[9], s))) return rc;
         if ((rc = acb_replace_device(r, tb, ss->d_win, wtotal, reinterpret_cast<const int64_t *>(a.woff), n, 0, chosen, ccap,
                                      reinterpret_cast<const int64_t *>(ccount), d_rout_off, d_rout, out_cap, d_rtotal, s)))
             return rc;
     }
     /* 6. commit */
-    if ((rc = sl_event(ss, 10, s))) return rc;
+    if ((rc = timing_mark(&ss->ev[10], s))) return rc;
     acb_sl_commit_kernel<<<(unsigned)((n * kSlLanes + 255) / 256), 256, 0, s>>>(a, r ? nullptr : ccount, ccap,
                                                                           r ? reinterpret_cast<const long long *>(d_rtotal) : nullptr, out_cap);
-    if ((rc = sl_launch("stream commit"))) return rc;
-    if ((rc = sl_event(ss, 11, s))) return rc;
-    if (g_timing.load()) {
-        CUDA_TRY(cudaEventSynchronize(ss->ev[11]));
-        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[3], ss->ev[6], ss->ev[7]));
-        if (r) CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[4], ss->ev[8], ss->ev[9]));
-        CUDA_TRY(cudaEventElapsedTime(&g_sl_ms[5], ss->ev[10], ss->ev[11]));
-    }
-    return ACB_OK;
+    if ((rc = launched("stream commit")) || (rc = timing_mark(&ss->ev[11], s)) || (rc = timing_ms(ss->ev[6], ss->ev[7], &g_sl_ms[3])) ||
+        (r && (rc = timing_ms(ss->ev[8], ss->ev[9], &g_sl_ms[4]))))
+        return rc;
+    return timing_ms(ss->ev[10], ss->ev[11], &g_sl_ms[5]);
 }
 
 extern "C" int acb_streams_feed_leftmost_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
@@ -4405,26 +4174,12 @@ extern "C" int acb_streams_replace_device(acb_streams *ss, acb_replacer *r, acb_
 
 /* a host feed's first step: ids and offsets checked, chunks (+ offsets, ids) uploaded to the table's workspace */
 static int sl_upload(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total, const int64_t *offsets, int64_t n,
-                     const int32_t *ids) {
+                     const int32_t *ids, const int64_t **d_off) {
     int rc;
     if (ids && (rc = check_ids(ss, ids, n))) return rc;
-    if (offsets) {                                          /* the kernels read chunks[offsets[h] .. offsets[h+1]) unchecked */
-        bool ok = offsets[0] == 0 && offsets[n] == total;
-        for (int64_t i = 0; ok && i < n; i++) ok = offsets[i + 1] >= offsets[i] && offsets[i + 1] % ss->L == 0;
-        if (!ok) { acb_set_error("offsets must be non-decreasing multiples of letter_bytes, start at 0 and end at total_bytes"); return ACB_EINVAL; }
-    }
-    CUDA_TRY(cudaSetDevice(tb->device));
-    if (!tb->stream) CUDA_TRY(cudaStreamCreateWithFlags(&tb->stream, cudaStreamNonBlocking));
-    if (!tb->w_count) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->w_count), sizeof(unsigned long long)));
-    if (!tb->h_count) CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_count), sizeof(unsigned long long)));
-    if ((rc = ensure(&tb->w_hay, &tb->w_hay_cap, (size_t)total + 64))) return rc;
-    if (offsets && (rc = ensure(&tb->w_off, &tb->w_off_cap, (size_t)n + 1))) return rc;
-    if (ids && (rc = ensure(&ss->d_ids, &ss->ids_cap, (size_t)std::max<int64_t>(n, 1)))) return rc;
-    cudaStream_t s = tb->stream;
-    if (total) CUDA_TRY(cudaMemcpyAsync(tb->w_hay, chunks, (size_t)total, cudaMemcpyHostToDevice, s));
-    if (offsets) CUDA_TRY(cudaMemcpyAsync(tb->w_off, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
-    if (ids && n) CUDA_TRY(cudaMemcpyAsync(ss->d_ids, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    return ACB_OK;
+    if (offsets && (rc = check_offsets(ss->L, offsets, n, total))) return rc;
+    if ((rc = upload_batch(tb, chunks, total, offsets, n, d_off))) return rc;
+    return upload_ids(ss, ids, n, tb->stream);
 }
 
 extern "C" int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
@@ -4435,29 +4190,15 @@ extern "C" int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, co
     if (!n_found || cap < 0 || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
     tb->h_out_n = 0;
-    if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids))) return rc;
-    if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1)))) return rc;
-    cudaStream_t s = tb->stream;
-    if ((rc = sl_feed(ss, tb, nullptr, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_chunks,
-                      stride_bytes, ids ? ss->d_ids : nullptr, final, tb->w_out, cap, reinterpret_cast<int64_t *>(tb->w_count), nullptr,
-                      nullptr, 0, nullptr, s, algo)))
+    const int64_t *d_off = nullptr;
+    if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids, &d_off)) ||
+        (rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(cap, 1))))
         return rc;
-    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    const unsigned long long n = *tb->h_count;
-    *n_found = (int64_t)n;
-    if (n > (unsigned long long)cap) {
-        acb_set_error("match buffer too small: %llu matches, capacity %lld", n, (long long)cap);
-        return ACB_EOVERFLOW;
-    }
-    if (n) {
-        if ((rc = ensure_pinned_out(tb, (size_t)n))) return rc;
-        CUDA_TRY(cudaMemcpyAsync(tb->h_out, tb->w_out, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaStreamSynchronize(s));
-        if (out) memcpy(out, tb->h_out, (size_t)n * sizeof(acb_match));
-    }
-    tb->h_out_n = n;
-    return ACB_OK;
+    cudaStream_t s = tb->stream;
+    if ((rc = sl_feed(ss, tb, nullptr, tb->w_hay, total_bytes, d_off, n_chunks, stride_bytes, ids ? ss->d_ids : nullptr, final, tb->w_out, cap,
+                      reinterpret_cast<int64_t *>(tb->w_count), nullptr, nullptr, 0, nullptr, s, algo)))
+        return rc;
+    return read_back(tb, tb->w_count, tb->w_out, cap, 0, n_chunks, 0, out, n_found, s);
 }
 
 extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
@@ -4468,16 +4209,17 @@ extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_ta
     if (!r || !out_offsets || !total || out_cap < 0 || (out_cap && !out) || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if ((rc = rp_fits(r, tb))) return rc;
     *total = 0;
-    if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids))) return rc;
+    const int64_t *d_off = nullptr;
+    if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids, &d_off))) return rc;
     cudaStream_t s = tb->stream;
     if ((rc = ensure(&tb->r_off, &tb->r_off_cap, (size_t)n_chunks + 2))) return rc;
     const int64_t guess = total_bytes + total_bytes / 4 + n_chunks * (int64_t)ss->T * ss->L + 4096;
     if ((rc = ensure(&tb->r_out, &tb->r_out_cap, (size_t)std::max<int64_t>(std::min(out_cap, guess), 16)))) return rc;
     for (;;) {                                             /* an output that fits out_cap but not the device buffer: grow, repeat */
         const int64_t dev_cap = std::min<int64_t>(out_cap, (int64_t)tb->r_out_cap);
-        if ((rc = sl_feed(ss, tb, r, tb->w_hay, total_bytes, offsets ? reinterpret_cast<const int64_t *>(tb->w_off) : nullptr, n_chunks,
-                          stride_bytes, ids ? ss->d_ids : nullptr, final, nullptr, 0, nullptr, reinterpret_cast<int64_t *>(tb->r_off),
-                          tb->r_out, dev_cap, reinterpret_cast<int64_t *>(tb->r_off + n_chunks + 1), s, algo)))
+        if ((rc = sl_feed(ss, tb, r, tb->w_hay, total_bytes, d_off, n_chunks, stride_bytes, ids ? ss->d_ids : nullptr, final, nullptr, 0,
+                          nullptr, reinterpret_cast<int64_t *>(tb->r_off), tb->r_out, dev_cap, reinterpret_cast<int64_t *>(tb->r_off + n_chunks + 1),
+                          s, algo)))
             return rc;
         CUDA_TRY(cudaMemcpyAsync(out_offsets, tb->r_off, (size_t)(n_chunks + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
         CUDA_TRY(cudaMemcpyAsync(total, tb->r_off + n_chunks + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
