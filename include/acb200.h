@@ -519,6 +519,43 @@ int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_table *tb, co
  * acb_last_replace_ms gives a replacing feed's offsets and write passes. */
 int acb_last_stream_leftmost_ms(float *ms, int32_t n);
 
+/* ---- whole words: keep the matches that are not part of a longer word ---------------------------------------------
+ * A match with end e and start s = e - len + 1 (letters) is a whole-word match iff s == 0 or letter s-1 is not a word
+ * letter, and e is the haystack's last letter or letter e+1 is not a word letter.  A haystack edge counts as a non-word
+ * letter: a neighbour is never read from another haystack.  The key's own letters do not matter.  A word set is a bitmap
+ * of uint32 words over letter values, as the buffer stores them: letter v is a word letter iff v < n_bits and bit v
+ * (bits[v / 32] >> (v % 32) & 1) is set.  n_bits is at most 256, 65 536 or 0x110000 for 1-, 2- or 4-byte letters
+ * (ACB_EINVAL beyond); bits == NULL with n_bits == 0 is the set without word letters, which keeps every match. */
+
+/* DEVICE buffers, asynchronous on `stream`.  The batch is laid out as for acb_scan_device, but d_hay needs no alignment;
+ * d_records holds n records of it (what acb_scan_device leaves; hay_id, end_index and key_id are not checked), d_bits
+ * the word set.  The whole-word records go to d_out in their order in d_records, from index *d_count on; *d_count is
+ * increased by their number and only records below index cap are stored, as for acb_leftmost_longest_device.  d_records
+ * is not changed.  The scratch space belongs to the table: the next call waits (cudaStreamWaitEvent) for the work of this
+ * one, also on another CUDA stream.  ACB_ERANGE for more than 2^31-1 records. */
+int acb_word_filter_device(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                           int64_t stride_bytes, const acb_match *d_records, int64_t n, const uint32_t *d_bits, int64_t n_bits,
+                           acb_match *d_out, int64_t cap, int64_t *d_count, void *stream);
+
+/* HOST buffers, the word set a host bitmap: acb_scan_host, acb_scan_host_leftmost and acb_replace_host on the whole-word
+ * matches only.  Each uploads the batch and scans it into a full list (algo ACB_ALGO_AUTO, _FILTER or _DFA; monolithic,
+ * no pipeline), filters that list on the device, then goes on as its route does: sort (sort != 0) and copy back; select;
+ * select and rewrite.  The result contracts are those routes' (ACB_EOVERFLOW with the exact count; out == NULL as for
+ * acb_scan_host).  The offsets are checked (ACB_EINVAL) before anything runs.  Without a device: ACB_ECUDA. */
+int acb_scan_host_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                        int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap, int64_t *n_found,
+                        int algo, int sort);
+int acb_scan_host_leftmost_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                                 int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap,
+                                 int64_t *n_found, int algo);
+int acb_replace_host_words(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
+                           int64_t n_hay, int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, int algo, int64_t *out_offsets,
+                           uint8_t *out, int64_t out_cap, int64_t *total);
+
+/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last whole-word filter on this thread, from its
+ * flags to its count, from CUDA events (the call then waits for them); 0 when timing is off or it had no records. */
+int acb_last_words_ms(float *ms);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

@@ -94,6 +94,54 @@ def _space_mask(letters: np.ndarray, bytes_flavour: bool) -> np.ndarray:
     return np.isin(letters, _space_letters(w, bytes_flavour and w == 1))
 
 
+_WORD_LETTERS_BYTES = b"0123456789ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz_"
+
+
+@functools.lru_cache(maxsize=None)
+def _default_word_mask(flavour: str) -> np.ndarray:
+    """The default word letters: re's \\w -- [0-9A-Za-z_] over the 256 byte values for the bytes flavour, isalnum() or
+    "_" over every code point for the unicode flavour (about 1.1 M calls: built on first use, once per process)."""
+    if flavour == "bytes":
+        m = np.zeros(256, dtype=bool)
+        m[np.frombuffer(_WORD_LETTERS_BYTES, dtype=np.uint8)] = True
+    else:
+        m = np.fromiter((chr(c).isalnum() for c in range(0x110000)), dtype=bool, count=0x110000)
+        m[ord("_")] = True
+    m.flags.writeable = False
+    return m
+
+
+@functools.lru_cache(maxsize=64)
+def _word_bits(words: tuple, width: int) -> Tuple[np.ndarray, int]:
+    """(uint32 bitmap, n_bits) of a word set (Automaton._words) for letters of `width` bytes as a batch stores them: 1
+    for the bytes flavour and for the unicode flavour's latin-1 batches (the first 256 code points), 4 otherwise.
+    n_bits is one past the largest word letter, so a set without letters has no bitmap at all."""
+    flavour, letters = words
+    size = 256 if width == 1 else 0x110000
+    if letters is None:
+        mask = _default_word_mask(flavour)[:size]
+    else:
+        v = np.frombuffer(letters, dtype=np.uint8) if flavour == "bytes" else \
+            np.fromiter(map(ord, letters), dtype=np.int64, count=len(letters))
+        mask = np.zeros(size, dtype=bool)
+        mask[v[v < size]] = True
+    set_bits = np.flatnonzero(mask)
+    n_bits = int(set_bits[-1]) + 1 if set_bits.size else 0
+    packed = np.zeros(-(-n_bits // 32) * 4, dtype=np.uint8)
+    packed[:-(-n_bits // 8)] = np.packbits(mask[:n_bits], bitorder="little")
+    bits = packed.view("<u4")
+    bits.flags.writeable = False
+    return bits, n_bits
+
+
+@functools.lru_cache(maxsize=64)
+def _word_bits_device(words: tuple, width: int, device: int):
+    """_word_bits on a CUDA device: (int32 CUDA tensor, n_bits), uploaded once per device, width and word set"""
+    import torch
+    bits, n_bits = _word_bits(words, width)
+    return torch.from_numpy(bits.view(np.int32).copy()).to(f"cuda:{device}"), n_bits
+
+
 class _PinnedRecords:
     """Owner of one pinned record buffer taken from the library (acb_take_records): exposes it to numpy through
     the array interface, gives it back (acb_release_records) when the last view is garbage collected."""
@@ -717,10 +765,70 @@ class Automaton:
                 return np.empty(0, dtype=N.MATCH_DTYPE)
             return _take_records(self._lib, tb, found.value)
 
+    def _words(self, whole_words):
+        """The whole_words argument of the batch methods, parsed once: None for False, else the word set as
+        (flavour, letters) with letters None for the default set (see _word_bits)."""
+        if whole_words is False:
+            return None
+        if self._key_type == KEY_SEQUENCE:
+            raise ValueError("whole_words needs text: KEY_SEQUENCE letters are integers, not letters of words")
+        flavour = "unicode" if self._UNICODE else "bytes"
+        if whole_words is True:
+            return (flavour, None)
+        if isinstance(whole_words, (bytes, bytearray, str)):
+            if isinstance(whole_words, str) != self._UNICODE:
+                raise ValueError(f"whole_words of the {flavour} flavour is True or a {'str' if self._UNICODE else 'bytes'} "
+                                 "of word letters")
+            return (flavour, whole_words if isinstance(whole_words, str) else bytes(whole_words))
+        raise TypeError("whole_words must be a bool, or the word letters as bytes (bytes flavour) or str (unicode flavour)")
+
     @_locked
-    def _scan_device_tensor(self, t, algo: str, sort: bool) -> np.ndarray:
+    def _words_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str, sort: bool,
+                    device: Optional[int], narrow: bool, words: tuple, leftmost: bool) -> np.ndarray:
+        """acb_scan_host_words / acb_scan_host_leftmost_words: upload, scan, keep the whole-word matches, then sort or
+        select, copy back; the capacity grows on overflow."""
+        if narrow:
+            core = self._ensure_narrow(device)
+            if core is None:
+                return np.empty(0, dtype=N.MATCH_DTYPE)
+            tb = core[1]
+        else:
+            tb = self._ensure_table(device)
+        bits, n_bits = _word_bits(words, 1 if narrow else self._L)
+        args = (tb, N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes,
+                N.ptr(bits) if n_bits else None, n_bits, None)
+        cap = max(self._match_cap, 1 << 12, 2 * n_hay)
+        found = ctypes.c_int64(0)
+        while True:
+            if leftmost:
+                rc = self._lib.acb_scan_host_leftmost_words(*args, cap, ctypes.byref(found), N.ALGOS[algo])
+            else:
+                rc = self._lib.acb_scan_host_words(*args, cap, ctypes.byref(found), N.ALGOS[algo], int(sort))
+            if rc != N.ACB_EOVERFLOW:
+                break
+            cap = self._match_cap = int(found.value) + 1024
+        N.check(rc)
+        if not found.value:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        return _take_records(self._lib, tb, found.value)
+
+    def _filter_words_device(self, tb, t, n: int, stride: int, full, m: int, words: tuple, stream):
+        """The whole-word records among the first m of the device buffer `full` (a scan of the aligned device batch t),
+        on `stream`: (records [max(m, 1), 3] int32 CUDA tensor, their number).  Waits once, for that number."""
+        import torch
+        bits, n_bits = _word_bits_device(words, self._L, t.device.index)
+        out = torch.empty((max(m, 1), 3), dtype=torch.int32, device=t.device)
+        cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
+        N.check(self._lib.acb_word_filter_device(tb, t.data_ptr(), n * stride, None, n, stride, full.data_ptr(), m,
+                                                 bits.data_ptr() if n_bits else None, n_bits, out.data_ptr(), m, cnt.data_ptr(),
+                                                 stream))
+        return out, int(cnt.item())
+
+    @_locked
+    def _scan_device_tensor(self, t, algo: str, sort: bool, words: Optional[tuple] = None) -> np.ndarray:
         """Batch already resident in HBM: a C-contiguous uint8 torch CUDA tensor [n, stride].  No host copy of
-        the haystacks; the scan runs on torch's current stream, only the records come back."""
+        the haystacks; the scan runs on torch's current stream, only the records come back.  words: keep the
+        whole-word matches (_filter_words_device) before the sort."""
         import torch
         n, stride = self._device_batch_shape(t)
         if n == 0 or stride == 0:
@@ -742,6 +850,8 @@ class Automaton:
                     cap = self._match_cap = found + 1024
                     continue
                 break
+            if words is not None:
+                out, found = self._filter_words_device(tb, t, n, stride, out, found, words, stream)
             return self._device_records(tb, out, found, n, stride // self._L, stream, sort)
 
     def _device_records(self, tb, out, found: int, n_hay: int, max_letters: int, stream, sort: bool) -> np.ndarray:
@@ -911,26 +1021,35 @@ class Automaton:
         start, end = _parse_start_end(args, 1, 2, 0, len(letters))
         return AutomatonSearchIterLong(self, letters, start, end)
 
-    def find_long_batch(self, haystacks, *, sort: bool = True, device: Optional[int] = None) -> "Matches":
-        """iter_long() over a whole batch (same input forms and result type as find_all_batch)."""
-        return self.find_all_batch(haystacks, algo="long", sort=sort, device=device)
+    def find_long_batch(self, haystacks, *, sort: bool = True, device: Optional[int] = None, whole_words=False) -> "Matches":
+        """iter_long() over a whole batch (same input forms and result type as find_all_batch).  whole_words is refused
+        (ValueError): iter_long's walk picks its matches itself, so a filter after it has no clear meaning."""
+        return self.find_all_batch(haystacks, algo="long", sort=sort, device=device, whole_words=whole_words)
 
-    def find_leftmost_longest_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None) -> "Matches":
+    def find_leftmost_longest_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
+                                    whole_words=False) -> "Matches":
         """Leftmost-longest non-overlapping matches of a whole batch, selected on the GPU (input forms and result type
         of find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or
         after p, take the smallest such start, the longest match there, and continue after its end.  Records come in
         haystack order, then end_index ascending.  This is the leftmost-longest rule of keyword extractors, not
         iter_long's: iter_long restarts from the root after every match and misses keys its walk does not pass.
-        algo ("auto", "filter", "dfa") only picks the scan that finds every match; the result does not depend on it."""
+        algo ("auto", "filter", "dfa") only picks the scan that finds every match; the result does not depend on it.
+
+        whole_words (see find_all_batch): the same rule over the whole-word matches only, so a longer match inside a
+        word does not hide a shorter whole word: keys ``new`` and ``new york`` on ``new yorker`` give ``new``.  A CUDA
+        tensor batch then waits once more, for the number of whole-word matches."""
         self._require_automaton()
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-longest takes 'auto', 'filter' or 'dfa'")
+        words = self._words(whole_words)
         batch = self._batch_input(haystacks)
         if batch[0] == "device":
-            return Matches(self._leftmost_device(batch[1], algo), self._values)
+            return Matches(self._leftmost_device(batch[1], algo, words), self._values)
         _, flat, offs, n, stride, narrow = batch
         if not (n and flat.size):
             return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
+        if words is not None:
+            return Matches(self._words_host(flat, offs, n, stride, algo, False, device, narrow, words, True), self._values)
         return Matches(self._leftmost_host(flat, offs, n, stride, algo, device, narrow), self._values)
 
     @_locked
@@ -958,7 +1077,7 @@ class Automaton:
         return _take_records(self._lib, tb, found.value)
 
     @_locked
-    def _leftmost_device(self, t, algo: str) -> np.ndarray:
+    def _leftmost_device(self, t, algo: str, words: Optional[tuple] = None) -> np.ndarray:
         """A CUDA tensor batch: the full scan into a device buffer, then acb_leftmost_longest_device, both on torch's
         current stream; only the chosen records come back."""
         import torch
@@ -969,13 +1088,14 @@ class Automaton:
         dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
         tb = self._ensure_table(dev)
         with torch.cuda.device(dev):
-            out, cnt, _ = self._leftmost_chosen(tb, t, n, stride, algo, torch.cuda.current_stream().cuda_stream)
+            out, cnt, _ = self._leftmost_chosen(tb, t, n, stride, algo, torch.cuda.current_stream().cuda_stream, words)
             found = int(cnt.item())
             return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
 
-    def _leftmost_chosen(self, tb, t, n: int, stride: int, algo: str, stream):
+    def _leftmost_chosen(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None):
         """The chosen records of an aligned device batch, left on the device: (records [cap, 3] int32 CUDA tensor,
-        their count as an int64 CUDA tensor, cap).  Synchronises once, to size the full list."""
+        their count as an int64 CUDA tensor, cap).  Synchronises once, to size the full list; with words, the
+        selection runs on the whole-word matches and a second wait sizes them (_filter_words_device)."""
         import torch
         cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
         cap = max(self._match_cap, 1 << 12, 2 * n)
@@ -988,6 +1108,8 @@ class Automaton:
             if m <= cap:
                 break
             cap = self._match_cap = m + 1024
+        if words is not None:
+            full, m = self._filter_words_device(tb, t, n, stride, full, m, words, stream)
         cap = max(m, 1)
         out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
         cnt.zero_()
@@ -1020,7 +1142,7 @@ class Automaton:
 
     # ------------------------------------------------------------------ the batch entry (new)
     def find_all_batch(self, haystacks, *, algo: str = "auto", sort: bool = True, device: Optional[int] = None,
-                       ignore_white_space: bool = False) -> Matches:
+                       ignore_white_space: bool = False, whole_words=False) -> Matches:
         """Search a whole batch on the GPU.
 
         haystacks: a sequence of bytes / str / tuple objects (as `iter` accepts), or a 2-D
@@ -1032,11 +1154,32 @@ class Automaton:
         of the reference, returned as arrays.  ignore_white_space=True: to ``A.iter(hay, ignore_white_space=True)``
         -- letters for which libc iswspace() is true are skipped (removed on the GPU before the scan) and end_index
         still counts the letters of the original haystack.
+
+        whole_words: keep only the whole-word matches, in the same format and order: neither the letter before the
+        match nor the one after it is a word letter (a haystack edge is not one; the key's own letters do not matter,
+        so ``#tag`` or ``foo bar`` work as keys).  True: re's \\w -- [0-9A-Za-z_] for the bytes flavour (flashtext's
+        default; the bytes of a UTF-8 letter such as b"\\xc3\\xa9" are not word letters, so b"caf" is a whole word in
+        b"caf\\xc3\\xa9": give bytes 0x80-0xFF as word letters for UTF-8 text), isalnum() or "_" for the unicode
+        flavour.  bytes (bytes flavour) or str (unicode flavour): exactly these word letters; empty: none, every match
+        is kept.  The matches are filtered on the GPU after the scan; a CUDA tensor batch then waits once more, for
+        their number.  ValueError with ignore_white_space, algo="long" or a KEY_SEQUENCE automaton.
         """
         self._require_automaton()
         if ignore_white_space and algo == "long":
             raise ValueError("iter_long has no ignore_white_space option")
+        words = self._words(whole_words)
+        if words is not None and ignore_white_space:
+            raise ValueError("whole_words cannot be combined with ignore_white_space")
+        if words is not None and algo == "long":
+            raise ValueError("whole_words cannot be combined with algo='long': iter_long's walk picks its matches itself")
         batch = self._batch_input(haystacks, narrow_ok=algo != "long")
+        if words is not None:
+            if batch[0] == "device":
+                return Matches(self._scan_device_tensor(batch[1], algo, sort, words), self._values)
+            _, flat, offs, n, stride, narrow = batch
+            if not (n and flat.size):
+                return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
+            return Matches(self._words_host(flat, offs, n, stride, algo, sort, device, narrow, words, False), self._values)
         if ignore_white_space:
             return Matches(self._scan_skip(batch, algo, sort, device), self._values)
         if batch[0] == "device":
@@ -1630,11 +1773,13 @@ class Replacer:
             self._native[(narrow, device)] = r
         return r
 
-    def replace_batch(self, haystacks, *, algo: str = "auto"):
+    def replace_batch(self, haystacks, *, algo: str = "auto", whole_words=False):
         """The batch with every leftmost-longest match replaced.  `haystacks` takes the input forms of find_all_batch;
         a list gives a list of the same item type, uint8[n, stride] or (flat, offsets) gives (flat uint8, offsets
         int64[n+1]), a CUDA tensor gives that pair as CUDA tensors computed on torch's current stream (the call
-        synchronises once to size the output).  algo ("auto", "filter", "dfa") only picks the scan."""
+        synchronises once to size the output).  algo ("auto", "filter", "dfa") only picks the scan.  whole_words (see
+        find_all_batch): replace the matches that find_leftmost_longest_batch chooses with the same option, so a key
+        inside a longer word is left alone; a CUDA tensor batch then synchronises once more."""
         A = self._A
         with A._gpu_lock:
             if self._version != A._version:
@@ -1642,11 +1787,12 @@ class Replacer:
             A._require_automaton()
             if algo not in ("auto", "filter", "dfa"):
                 raise ValueError(f"algo {algo!r}: replace_batch takes 'auto', 'filter' or 'dfa'")
+            words = A._words(whole_words)
             pair = isinstance(haystacks, np.ndarray) or (isinstance(haystacks, tuple) and len(haystacks) == 2 and
                                                          all(isinstance(x, np.ndarray) for x in haystacks))
             batch = A._batch_input(haystacks)
             if batch[0] == "device":
-                return self._run_device(batch[1], algo)
+                return self._run_device(batch[1], algo, words)
             _, flat, offs, n, stride, narrow = batch
             if narrow and True not in self._tables:         # a replacement outside latin-1: 4 bytes per letter
                 flat = flat.astype("<u4").view(np.uint8)
@@ -1656,8 +1802,10 @@ class Replacer:
                 offs = np.arange(n + 1, dtype=np.int64) * stride
             if n == 0 or flat.size == 0:
                 out, out_offs = flat[:0].copy(), np.zeros(n + 1, dtype=np.int64)
-            else:
+            elif words is None:
                 out, out_offs = self._run_host(flat, offs, n, narrow, algo)
+            else:
+                out, out_offs = self._run_host(flat, offs, n, narrow, algo, words)
             if pair:
                 return out, out_offs
             return self._items(out, out_offs, narrow)
@@ -1694,9 +1842,9 @@ class Replacer:
         s = raw.decode("utf-32-le", "surrogatepass")
         return [s[b[i] // 4:b[i + 1] // 4] for i in range(len(b) - 1)]
 
-    def _run_host(self, flat: np.ndarray, offs: np.ndarray, n: int, narrow: bool, algo: str):
-        """acb_replace_host -> (output bytes, output offsets int64[n+1]); a second call when the first guess of the
-        output size was too small"""
+    def _run_host(self, flat: np.ndarray, offs: np.ndarray, n: int, narrow: bool, algo: str, words: Optional[tuple] = None):
+        """acb_replace_host (acb_replace_host_words with a word set) -> (output bytes, output offsets int64[n+1]); a
+        second call when the first guess of the output size was too small"""
         A = self._A
         if narrow:
             core = A._ensure_narrow(self._device)
@@ -1709,17 +1857,23 @@ class Replacer:
         out_offs = np.empty(n + 1, dtype=np.int64)
         total = ctypes.c_int64(0)
         cap = int(flat.size) + int(flat.size) // 4 + 4096
+        batch = (r, tb, N.ptr(flat), int(flat.size), N.ptr(offs), n, 0)
+        if words is not None:
+            bits, n_bits = _word_bits(words, 1 if narrow else A._L)
         for _ in range(2):
             out = np.empty(cap, dtype=np.uint8)
-            rc = A._lib.acb_replace_host(r, tb, N.ptr(flat), int(flat.size), N.ptr(offs), n, 0, N.ALGOS[algo],
-                                         N.ptr(out_offs), N.ptr(out), cap, ctypes.byref(total))
+            result = (N.ALGOS[algo], N.ptr(out_offs), N.ptr(out), cap, ctypes.byref(total))
+            if words is None:
+                rc = A._lib.acb_replace_host(*batch, *result)
+            else:
+                rc = A._lib.acb_replace_host_words(*batch, N.ptr(bits) if n_bits else None, n_bits, *result)
             if rc != N.ACB_EOVERFLOW:
                 break
             cap = int(total.value)
         N.check(rc)
         return out[:total.value], out_offs
 
-    def _run_device(self, t, algo: str):
+    def _run_device(self, t, algo: str, words: Optional[tuple] = None):
         """A CUDA tensor batch: scan, select and rewrite on torch's current stream; (flat, offsets) CUDA tensors"""
         import torch
         A = self._A
@@ -1731,7 +1885,7 @@ class Replacer:
         tb = A._ensure_table(dev)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream().cuda_stream
-            chosen, cnt, cap = A._leftmost_chosen(tb, t, n, stride, algo, stream)
+            chosen, cnt, cap = A._leftmost_chosen(tb, t, n, stride, algo, stream, words)
             r = self._replacer(tb, False, dev)
             out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
             total = torch.empty(1, dtype=torch.int64, device=t.device)

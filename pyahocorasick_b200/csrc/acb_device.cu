@@ -1386,6 +1386,12 @@ struct acb_table {
     long long *r_off = nullptr; size_t r_off_cap = 0;    /* acb_replace_host: output offsets[n+1] then the total */
     cudaEvent_t r_done = nullptr;                        /* the last replacement's work on r_buf / r_ts has been issued before it */
     cudaEvent_t r_ev[4] = {};                            /* kernel timing of the offsets pass and the write pass */
+    /* workspace of the whole-word filter (acb_word_filter_device), sized by the record count */
+    void *ww_buf = nullptr; size_t ww_buf_cap = 0;       /* flags, positions, the record count, cub scratch */
+    uint32_t *ww_bits = nullptr; size_t ww_bits_cap = 0; /* the host routes: their word bitmap */
+    acb_match *ww_out = nullptr; size_t ww_out_cap = 0;  /* the host routes: the whole-word records */
+    cudaEvent_t ww_done = nullptr;                       /* the last filter's work on ww_buf has been issued before it */
+    cudaEvent_t ww_ev[2] = {};                           /* kernel timing of the filter */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1434,6 +1440,9 @@ extern "C" void acb_table_free(acb_table *tb) {
     cudaFree(tb->r_buf); cudaFree(tb->r_ts); cudaFree(tb->r_out); cudaFree(tb->r_off);
     if (tb->r_done) cudaEventDestroy(tb->r_done);
     for (cudaEvent_t e : tb->r_ev) if (e) cudaEventDestroy(e);
+    cudaFree(tb->ww_buf); cudaFree(tb->ww_bits); cudaFree(tb->ww_out);
+    if (tb->ww_done) cudaEventDestroy(tb->ww_done);
+    for (cudaEvent_t e : tb->ww_ev) if (e) cudaEventDestroy(e);
     if (tb->h_kept) cudaFreeHost(tb->h_kept);
     if (tb->k_done) cudaEventDestroy(tb->k_done);
     if (tb->k_t0) cudaEventDestroy(tb->k_t0);
@@ -3362,10 +3371,138 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     return ACB_OK;
 }
 
+/* ------------------------------------------------------------ whole-word filter */
+/* A record is a whole-word match when neither the letter before its start nor the letter after its end is a word letter;
+ * a haystack edge counts as a non-word letter, so a neighbour is never read from another haystack.  acb_ww_flag_kernel
+ * flags every record (its key's length from the table, one or two neighbour letters, a bitmap lookup each); the kept
+ * records are then compacted in order by the selection's emit step: exclusive sum of the flags, acb_ll_emit_kernel,
+ * acb_ll_count_kernel. */
+namespace {
+thread_local float g_ww_ms = 0.f;                          /* kernel timing: flags to count */
+
+struct WwArgs {
+    const uint8_t *hay;
+    const long long *off;                                  /* n_hay + 1 byte offsets, or nullptr: haystack h = [h*stride, (h+1)*stride) */
+    long long stride;
+    const int32_t *key_len;
+    const uint32_t *bits;                                  /* letter v is a word letter iff v < n_bits and bit v is set */
+    long long n_bits;
+};
+
+/* the letter at p, little-endian, at any alignment */
+template <int L>
+__device__ __forceinline__ uint32_t ww_letter(const uint8_t *p) {
+    uint32_t v = __ldg(p);
+    if (L >= 2) v |= (uint32_t)__ldg(p + 1) << 8;
+    if (L == 4) v |= (uint32_t)__ldg(p + 2) << 16 | (uint32_t)__ldg(p + 3) << 24;
+    return v;
+}
+
+/* flag[i] = pos[i] = record i is a whole-word match; *d_n = n (the emit step reads the count from the device) */
+template <int L>
+__global__ void __launch_bounds__(256) acb_ww_flag_kernel(const __grid_constant__ WwArgs a, const acb_match *rec, long long n,
+                                                         uint8_t *flag, int32_t *pos, unsigned long long *d_n) {
+    __shared__ uint32_t s_bits[8];                         /* 1-byte letters: the whole set */
+    if (L == 1) {
+        if (threadIdx.x < 8) s_bits[threadIdx.x] = (long long)threadIdx.x * 32 < a.n_bits ? a.bits[threadIdx.x] : 0u;
+        __syncthreads();
+    }
+    auto word = [&](uint32_t v) {
+        if ((long long)v >= a.n_bits) return false;
+        return ((L == 1 ? s_bits[v >> 5] : __ldg(a.bits + (v >> 5))) >> (v & 31) & 1u) != 0;
+    };
+    const long long first = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (first == 0) *d_n = (unsigned long long)n;
+    for (long long i = first; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const acb_match m = rec[i];
+        long long b0, letters;
+        if (a.off) {
+            b0 = __ldg(a.off + m.hay_id);
+            letters = (__ldg(a.off + m.hay_id + 1) - b0) / L;
+        } else {
+            b0 = (long long)m.hay_id * a.stride;
+            letters = a.stride / L;
+        }
+        const long long end = m.end_index, start = end - __ldg(a.key_len + m.key_id) + 1;
+        bool keep = start == 0 || !word(ww_letter<L>(a.hay + b0 + (start - 1) * L));
+        keep = keep && (end + 1 == letters || !word(ww_letter<L>(a.hay + b0 + (end + 1) * L)));
+        flag[i] = keep;
+        pos[i] = keep;
+    }
+}
+} // namespace
+
+extern "C" int acb_last_words_ms(float *ms) {
+    if (!ms) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *ms = g_ww_ms;
+    return ACB_OK;
+}
+
+/* a word bitmap of n_bits bits for the table's letters: at most one bit per letter value, bits given unless empty */
+static int check_words(const acb_table *tb, const uint32_t *bits, int64_t n_bits) {
+    const int64_t most = tb->L == 1 ? 256 : (tb->L == 2 ? 65536 : 0x110000);
+    if (n_bits >= 0 && n_bits <= most && (bits || n_bits == 0)) return ACB_OK;
+    acb_set_error("a word set of %d-byte letters has 0 .. %lld bits, and needs a bitmap unless it has none", tb->L, (long long)most);
+    return ACB_EINVAL;
+}
+
+extern "C" int acb_word_filter_device(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                                      int64_t stride_bytes, const acb_match *d_records, int64_t n, const uint32_t *d_bits, int64_t n_bits,
+                                      acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+    if (!tb || total_bytes < 0 || (total_bytes && !d_hay) || n_hay < 0 || n < 0 || (n && !d_records) || cap < 0 || (cap > 0 && !d_out) ||
+        !d_count) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    int rc;
+    if ((rc = check_words(tb, d_bits, n_bits))) return rc;
+    if (!d_offsets && (rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 0))) return rc;
+    if (n > 0x7fffffffLL) { acb_set_error("more than 2^31-1 records to filter"); return ACB_ERANGE; }
+    g_ww_ms = 0.f;
+    if (n == 0) return ACB_OK;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const int ni = (int)n;
+    const size_t N = (size_t)n;
+    size_t temp = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, (int32_t *)nullptr, (int32_t *)nullptr, ni, s));
+    const size_t need = 3 * 256 + N + N * sizeof(int32_t) + sizeof(unsigned long long) + temp;
+    if ((rc = scratch_wait(tb->ww_done, s)) || (rc = grow_synced(&tb->ww_buf, &tb->ww_buf_cap, need, s))) return rc;
+    char *p = reinterpret_cast<char *>(tb->ww_buf);
+    uint8_t *flag = reinterpret_cast<uint8_t *>(carve(p, N));
+    int32_t *pos = reinterpret_cast<int32_t *>(carve(p, N * sizeof(int32_t)));
+    unsigned long long *d_n = reinterpret_cast<unsigned long long *>(carve(p, sizeof(unsigned long long)));
+    void *tmp = carve(p, temp);
+    WwArgs a;
+    a.hay = d_hay; a.off = reinterpret_cast<const long long *>(d_offsets); a.stride = stride_bytes; a.key_len = tb->d_keylen;
+    a.bits = d_bits; a.n_bits = n_bits;
+    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, (long long)tb->sm_count * 16);
+    if ((rc = timing_mark(&tb->ww_ev[0], s))) return rc;
+    if (tb->L == 1) acb_ww_flag_kernel<1><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
+    else if (tb->L == 2) acb_ww_flag_kernel<2><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
+    else acb_ww_flag_kernel<4><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
+    if ((rc = launched("word flags"))) return rc;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, temp, pos, pos, ni, s));
+    acb_ll_emit_kernel<<<grid, 256, 0, s>>>(d_records, d_n, flag, pos, d_out, cap, reinterpret_cast<const unsigned long long *>(d_count));
+    CUDA_TRY(cudaGetLastError());
+    acb_ll_count_kernel<<<1, 1, 0, s>>>(d_n, flag, pos, reinterpret_cast<unsigned long long *>(d_count));
+    if ((rc = launched("word filter emit", 2)) || (rc = timing_mark(&tb->ww_ev[1], s)) || (rc = scratch_done(&tb->ww_done, s))) return rc;
+    return timing_ms(tb->ww_ev[0], tb->ww_ev[1], &g_ww_ms);
+}
+
+/* The word set of a host route that filters (acb_*_words): a host bitmap */
+struct WordSet {
+    const uint32_t *bits;
+    int64_t n_bits;
+};
+
 /* The host routes' first step: the batch to tb->w_hay (and offsets to tb->w_off, *d_off), and its full match list into
- * tb->w_out, grown until it fits; *full is its length.  On tb->stream, which it leaves synchronised. */
+ * tb->w_out, grown until it fits; *full is its length.  With a word set, the whole-word records of that list go on to
+ * tb->ww_out and *full is their number.  *rec is the list the route goes on with, its length also in tb->w_count.  On
+ * tb->stream, which it leaves synchronised. */
 static int upload_and_scan_full(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
-                                int64_t stride_bytes, int algo, const int64_t **d_off, unsigned long long *full) {
+                                int64_t stride_bytes, int algo, const WordSet *ws, const int64_t **d_off, unsigned long long *full,
+                                acb_match **rec) {
     int rc;
     if ((rc = upload_batch(tb, hay, total_bytes, offsets, n_hay, d_off)) ||
         (rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)std::max<int64_t>(2 * n_hay, 4096))))
@@ -3383,32 +3520,88 @@ static int upload_and_scan_full(acb_table *tb, const uint8_t *hay, int64_t total
         if (*full <= tb->w_out_cap) break;
         if ((rc = ensure(&tb->w_out, &tb->w_out_cap, (size_t)*full))) return rc;
     }
+    *rec = tb->w_out;
+    if (!ws || *full == 0) return ACB_OK;
+    const size_t words = ((size_t)ws->n_bits + 31) / 32;
+    if ((rc = ensure(&tb->ww_bits, &tb->ww_bits_cap, std::max<size_t>(words, 1))) || (rc = ensure(&tb->ww_out, &tb->ww_out_cap, (size_t)*full)))
+        return rc;
+    if (words) CUDA_TRY(cudaMemcpyAsync(tb->ww_bits, ws->bits, words * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemsetAsync(tb->w_count, 0, sizeof(unsigned long long), s));
+    if ((rc = acb_word_filter_device(tb, tb->w_hay, total_bytes, *d_off, n_hay, stride_bytes, tb->w_out, (int64_t)*full, tb->ww_bits,
+                                     ws->n_bits, tb->ww_out, (int64_t)*full, reinterpret_cast<int64_t *>(tb->w_count), s)))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    *full = *tb->h_count;
+    *rec = tb->ww_out;
     return ACB_OK;
 }
 
-extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
-                                      int64_t stride_bytes, acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+/* the argument checks of the host routes that filter: the word set, and offsets, which the filter reads unchecked */
+static int check_words_route(const acb_table *tb, const uint32_t *bits, int64_t n_bits, const int64_t *offsets, int64_t n_hay,
+                             int64_t total_bytes) {
+    int rc = check_words(tb, bits, n_bits);
+    if (rc == ACB_OK && offsets) rc = check_offsets(tb->L, offsets, n_hay, total_bytes);
+    return rc;
+}
+
+extern "C" int acb_scan_host_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                                   int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap,
+                                   int64_t *n_found, int algo, int sort) {
+    if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *n_found = 0;
+    if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("a whole-word scan takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
+    if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
+    int rc;
+    if ((rc = check_words_route(tb, bits, n_bits, offsets, n_hay, total_bytes))) return rc;
+    if (!offsets && (rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1))) return rc;
+    tb->h_out_n = 0;
+    if (total_bytes == 0 || n_hay == 0) return ACB_OK;
+    const WordSet ws{bits, n_bits};
+    const int64_t *d_off = nullptr;
+    unsigned long long full = 0;
+    acb_match *rec = nullptr;
+    if ((rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, &ws, &d_off, &full, &rec))) return rc;
+    return read_back(tb, tb->w_count, rec, cap, sort, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, out, n_found, tb->stream);
+}
+
+static int scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                              int64_t stride_bytes, const WordSet *ws, acb_match *out, int64_t cap, int64_t *n_found, int algo) {
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
     if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("leftmost-longest takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
     int rc;
+    if (ws && (rc = check_words_route(tb, ws->bits, ws->n_bits, offsets, n_hay, total_bytes))) return rc;
     if (!offsets && (rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1))) return rc;
     tb->h_out_n = 0;
     if (total_bytes == 0 || n_hay == 0) return ACB_OK;
     const int64_t *d_off = nullptr;
     unsigned long long full = 0;
-    if ((rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, &d_off, &full))) return rc;
+    acb_match *rec = nullptr;
+    if ((rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, ws, &d_off, &full, &rec))) return rc;
     cudaStream_t s = tb->stream;
     if (full == 0) return ACB_OK;
     const int64_t kept_cap = std::min<int64_t>(cap, (int64_t)full);
     if ((rc = ensure(&tb->l_out, &tb->l_out_cap, (size_t)std::max<int64_t>(kept_cap, 1)))) return rc;
     unsigned long long *d_n = tb->l_ctr + 2;
     CUDA_TRY(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s));
-    if ((rc = acb_leftmost_longest_device(tb, tb->w_out, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, tb->l_out,
+    if ((rc = acb_leftmost_longest_device(tb, rec, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, tb->l_out,
                                           kept_cap, reinterpret_cast<int64_t *>(d_n), s)))
         return rc;
     return read_back(tb, d_n, tb->l_out, cap, 0, n_hay, 0, out, n_found, s);
+}
+
+extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                                      int64_t stride_bytes, acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    return scan_host_leftmost(tb, hay, total_bytes, offsets, n_hay, stride_bytes, nullptr, out, cap, n_found, algo);
+}
+
+extern "C" int acb_scan_host_leftmost_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                                            int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap,
+                                            int64_t *n_found, int algo) {
+    const WordSet ws{bits, n_bits};
+    return scan_host_leftmost(tb, hay, total_bytes, offsets, n_hay, stride_bytes, &ws, out, cap, n_found, algo);
 }
 
 /* ------------------------------------------------------------ leftmost-longest replacement */
@@ -3722,20 +3915,21 @@ extern "C" int acb_replace_device(acb_replacer *r, acb_table *tb, const uint8_t 
     return rp_write(tb, a, s);
 }
 
-extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
-                                int64_t n_hay, int64_t stride_bytes, int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap,
-                                int64_t *total) {
+static int replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                        int64_t stride_bytes, const WordSet *ws, int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap, int64_t *total) {
     int rc = rp_check(r, tb, total_bytes, n_hay, stride_bytes, offsets != nullptr, out_cap);
     if (rc) return rc;
     if ((total_bytes && !hay) || !out_offsets || !total || (out_cap && !out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("replacement takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
     if (offsets && (rc = check_offsets(tb->L, offsets, n_hay, total_bytes))) return rc;
+    if (ws && (rc = check_words(tb, ws->bits, ws->n_bits))) return rc;
     *total = 0;
     for (float &v : g_rp_ms) v = 0.f;
     if (n_hay == 0) { out_offsets[0] = 0; return ACB_OK; }
     const int64_t *d_off = nullptr;
     unsigned long long full = 0;
-    if (total_bytes && (rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, &d_off, &full))) return rc;
+    acb_match *rec = nullptr;
+    if (total_bytes && (rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, ws, &d_off, &full, &rec))) return rc;
     if (!total_bytes) {                                     /* only empty haystacks: nothing to scan, nothing to write */
         for (int64_t i = 0; i <= n_hay; i++) out_offsets[i] = 0;
         return ACB_OK;
@@ -3745,7 +3939,7 @@ extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *h
     unsigned long long *d_n = tb->l_ctr + 2;
     CUDA_TRY(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s));
     if (full && (rc = ensure(&tb->l_out, &tb->l_out_cap, (size_t)full))) return rc;
-    if (full && (rc = acb_leftmost_longest_device(tb, tb->w_out, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L,
+    if (full && (rc = acb_leftmost_longest_device(tb, rec, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L,
                                                   tb->l_out, (int64_t)full, reinterpret_cast<int64_t *>(d_n), s)))
         return rc;
     RpArgs a;
@@ -3766,6 +3960,19 @@ extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *h
     if (*total) CUDA_TRY(cudaMemcpyAsync(out, tb->r_out, (size_t)*total, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     return ACB_OK;
+}
+
+extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
+                                int64_t n_hay, int64_t stride_bytes, int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap,
+                                int64_t *total) {
+    return replace_host(r, tb, hay, total_bytes, offsets, n_hay, stride_bytes, nullptr, algo, out_offsets, out, out_cap, total);
+}
+
+extern "C" int acb_replace_host_words(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
+                                      int64_t n_hay, int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, int algo, int64_t *out_offsets,
+                                      uint8_t *out, int64_t out_cap, int64_t *total) {
+    const WordSet ws{bits, n_bits};
+    return replace_host(r, tb, hay, total_bytes, offsets, n_hay, stride_bytes, &ws, algo, out_offsets, out, out_cap, total);
 }
 
 /* ------------------------------------------------------------ leftmost-longest stream batches */
