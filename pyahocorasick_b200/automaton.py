@@ -10,6 +10,7 @@ Reference semantics are cited as file:line relative to /root/reference.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import functools
 import locale
@@ -17,7 +18,7 @@ import os
 import operator
 import pickle
 import threading
-from typing import Any, Iterable, List, Optional, Sequence, Tuple
+from typing import Any, Iterable, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -687,6 +688,14 @@ class Automaton:
         self._table_device = device
         return tb
 
+    def _table_for(self, device: Optional[int], narrow: bool):
+        """The table a batch runs on: the latin-1 one for a narrow batch, else the full one.  None when the batch is narrow
+        and no key is latin-1: then nothing matches."""
+        if not narrow:
+            return self._ensure_table(device)
+        core = self._ensure_narrow(device)
+        return None if core is None else core[1]
+
     @_locked
     def filter_shape(self) -> dict:
         """The prefilter the host chose for this key set (no table copies): gram length, probe stride, bitmap sizes
@@ -736,34 +745,60 @@ class Automaton:
         narrow=True: the buffer holds 1-byte letters of a unicode-flavour automaton (latin-1 path).
         long_state (algo "long", one haystack): the state the walk starts in; the state it ends in is left in
         self._long_state_out (iter_long streaming, acb_table_set_long_state / acb_table_get_long_state)."""
-        if narrow:
-            core = self._ensure_narrow(device)
-            if core is None:
-                return np.empty(0, dtype=N.MATCH_DTYPE)
-            tb = core[1]
-        else:
-            tb = self._ensure_table(device)
-        total = int(flat.size)
-        cap = max(self._match_cap, 1 << 12, 2 * n_hay)        # device-side capacity; grown on overflow
-        found = ctypes.c_int64(0)
-        while True:
+        lib, total = self._lib, int(flat.size)
+
+        def scan(tb, cap, found_ref):
             if long_state is not None:
-                N.check(self._lib.acb_table_set_long_state(tb, int(long_state)))      # one shot: again before a retry
-            rc = self._lib.acb_scan_host(tb, N.ptr(flat) if total else None, total,
-                                         N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes,
-                                         None, cap, ctypes.byref(found), N.ALGOS[algo], 1 if sort else 0)
-            if rc == N.ACB_EOVERFLOW:
-                cap = int(found.value) + 1024
-                self._match_cap = cap
-                continue
-            N.check(rc)
-            if long_state is not None:
+                N.check(lib.acb_table_set_long_state(tb, int(long_state)))      # one shot: again before a retry
+            rc = lib.acb_scan_host(tb, N.ptr(flat) if total else None, total, N.ptr(offsets) if offsets is not None else None,
+                                   n_hay, stride_bytes, None, cap, found_ref, N.ALGOS[algo], 1 if sort else 0)
+            if rc == N.ACB_OK and long_state is not None:
                 st = ctypes.c_int32(0)
-                N.check(self._lib.acb_table_get_long_state(tb, ctypes.byref(st)))
+                N.check(lib.acb_table_get_long_state(tb, ctypes.byref(st)))
                 self._long_state_out = int(st.value)
-            if not found.value:
-                return np.empty(0, dtype=N.MATCH_DTYPE)
-            return _take_records(self._lib, tb, found.value)
+            return rc
+        return self._host_records(device, narrow, n_hay, scan)
+
+    def _record_room(self, n_hay: int) -> int:
+        """The first guess of the records a batch of n_hay haystacks gives; _match_cap remembers the largest overflow."""
+        return max(self._match_cap, 1 << 12, 2 * n_hay)
+
+    def _host_records(self, device: Optional[int], narrow: bool, n_hay: int, call) -> np.ndarray:
+        """The records of one host-buffer call, which leaves them in its table's pinned buffer.  call(tb, cap, found_ref)
+        makes the native call with room for cap records and returns its status.  On ACB_EOVERFLOW it runs once more with
+        room for the exact count (+1024, kept in _match_cap); a second overflow raises.  The records are handed over
+        without a copy (_take_records)."""
+        tb = self._table_for(device, narrow)
+        if tb is None:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        found = ctypes.c_int64(0)
+        rc = call(tb, self._record_room(n_hay), ctypes.byref(found))
+        if rc == N.ACB_EOVERFLOW:
+            self._match_cap = int(found.value) + 1024
+            rc = call(tb, self._match_cap, ctypes.byref(found))
+        N.check(rc)
+        if not found.value:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        return _take_records(self._lib, tb, found.value)
+
+    def _device_scan(self, t, n_hay: int, call):
+        """The records of one device call on torch's current stream, left on the device: (int32 [cap, 3] CUDA tensor,
+        their number).  call(out, cap, cnt) makes the native call into out with its int64 count cnt, zeroed before each
+        try.  When the count exceeds cap (nothing was committed), it runs once more with room for it (+1024, kept in
+        _match_cap); a second overflow raises."""
+        import torch
+        cnt = torch.empty(1, dtype=torch.int64, device=t.device)
+        cap = self._record_room(n_hay)
+        for retry in (False, True):
+            out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
+            cnt.zero_()
+            call(out, cap, cnt)
+            found = int(cnt.item())
+            if found <= cap:
+                return out, found
+            if retry:
+                raise N.NativeError(f"{found} records after a retry with room for {cap}")
+            cap = self._match_cap = found + 1024
 
     def _words(self, whole_words):
         """The whole_words argument of the batch methods, parsed once: None for False, else the word set as
@@ -786,31 +821,17 @@ class Automaton:
     def _words_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str, sort: bool,
                     device: Optional[int], narrow: bool, words: tuple, leftmost: bool) -> np.ndarray:
         """acb_scan_host_words / acb_scan_host_leftmost_words: upload, scan, keep the whole-word matches, then sort or
-        select, copy back; the capacity grows on overflow."""
-        if narrow:
-            core = self._ensure_narrow(device)
-            if core is None:
-                return np.empty(0, dtype=N.MATCH_DTYPE)
-            tb = core[1]
-        else:
-            tb = self._ensure_table(device)
+        select, copy back (_host_records)."""
+        lib = self._lib
         bits, n_bits = _word_bits(words, 1 if narrow else self._L)
-        args = (tb, N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes,
+        args = (N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes,
                 N.ptr(bits) if n_bits else None, n_bits, None)
-        cap = max(self._match_cap, 1 << 12, 2 * n_hay)
-        found = ctypes.c_int64(0)
-        while True:
+
+        def scan(tb, cap, found_ref):
             if leftmost:
-                rc = self._lib.acb_scan_host_leftmost_words(*args, cap, ctypes.byref(found), N.ALGOS[algo])
-            else:
-                rc = self._lib.acb_scan_host_words(*args, cap, ctypes.byref(found), N.ALGOS[algo], int(sort))
-            if rc != N.ACB_EOVERFLOW:
-                break
-            cap = self._match_cap = int(found.value) + 1024
-        N.check(rc)
-        if not found.value:
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        return _take_records(self._lib, tb, found.value)
+                return lib.acb_scan_host_leftmost_words(tb, *args, cap, found_ref, N.ALGOS[algo])
+            return lib.acb_scan_host_words(tb, *args, cap, found_ref, N.ALGOS[algo], int(sort))
+        return self._host_records(device, narrow, n_hay, scan)
 
     def _filter_words_device(self, tb, t, n: int, stride: int, full, m: int, words: tuple, stream):
         """The whole-word records among the first m of the device buffer `full` (a scan of the aligned device batch t),
@@ -825,34 +846,33 @@ class Automaton:
         return out, int(cnt.item())
 
     @_locked
-    def _scan_device_tensor(self, t, algo: str, sort: bool, words: Optional[tuple] = None) -> np.ndarray:
+    def _scan_device_tensor(self, batch, algo: str, sort: bool, words: Optional[tuple] = None,
+                            white_space: bool = False) -> np.ndarray:
         """Batch already resident in HBM: a C-contiguous uint8 torch CUDA tensor [n, stride].  No host copy of
         the haystacks; the scan runs on torch's current stream, only the records come back.  words: keep the
-        whole-word matches (_filter_words_device) before the sort."""
-        import torch
-        n, stride = self._device_batch_shape(t)
-        if n == 0 or stride == 0:
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        t = _aligned(t)
-        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        whole-word matches (_filter_words_device) before the sort.  white_space: the scan skips the white space
+        (acb_scan_device_skip)."""
+        t = _aligned(batch.data)
+        dev = _device_of(t)
         tb = self._ensure_table(dev)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream().cuda_stream
-            cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
-            cap = max(self._match_cap, 1 << 12, 2 * n)
-            while True:
-                out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-                cnt.zero_()
-                N.check(self._lib.acb_scan_device(tb, t.data_ptr(), n * stride, None, n, stride, out.data_ptr(), cap,
-                                                  cnt.data_ptr(), stream, N.ALGOS[algo]))
-                found = int(cnt.item())
-                if found > cap:
-                    cap = self._match_cap = found + 1024
-                    continue
-                break
-            if words is not None:
-                out, found = self._filter_words_device(tb, t, n, stride, out, found, words, stream)
-            return self._device_records(tb, out, found, n, stride // self._L, stream, sort)
+        skip = self._skip_set(False) if white_space else None
+        with _on_device(dev) as stream:
+            out, found = self._device_matches(tb, t, batch.n, batch.stride, algo, stream, words, skip)
+            return self._device_records(tb, out, found, batch.n, batch.stride // self._L, stream, sort)
+
+    def _device_matches(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None,
+                        skip: Optional[np.ndarray] = None):
+        """Every match of the aligned device batch t, left on the device (_device_scan): (int32 [cap, 3] CUDA tensor,
+        their number).  skip: the scan skips these letters; words: only the whole-word matches (_filter_words_device)."""
+        lib = self._lib
+
+        def scan(out, cap, cnt):
+            args = (tb, t.data_ptr(), n * stride, None, n, stride, out.data_ptr(), cap, cnt.data_ptr(), stream, N.ALGOS[algo])
+            N.check(lib.acb_scan_device(*args) if skip is None else lib.acb_scan_device_skip(*args, N.ptr(skip), len(skip)))
+        out, found = self._device_scan(t, n, scan)
+        if words is not None:
+            out, found = self._filter_words_device(tb, t, n, stride, out, found, words, stream)
+        return out, found
 
     def _device_records(self, tb, out, found: int, n_hay: int, max_letters: int, stream, sort: bool) -> np.ndarray:
         """The first `found` records of the device buffer `out`, sorted on the device (on the host when the sort key
@@ -880,56 +900,16 @@ class Automaton:
 
     @_locked
     def _scan_skip(self, batch, algo: str, sort: bool, device: Optional[int]) -> np.ndarray:
-        """Every scan with ignore_white_space: `batch` as _batch_input lays it out -> records in original letters.
-        The white space is removed on the GPU (acb_scan_host_skip / acb_scan_device_skip)."""
+        """Every host scan with ignore_white_space: `batch`, a host batch as _batch_input lays it out -> records in
+        original letters.  The white space is removed on the GPU (acb_scan_host_skip)."""
         lib = self._lib
-        if batch[0] == "device":
-            import torch
-            t = batch[1]
-            n, stride = self._device_batch_shape(t)
-            if n == 0 or stride == 0:
-                return np.empty(0, dtype=N.MATCH_DTYPE)
-            t = _aligned(t)
-            dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
-            tb = self._ensure_table(dev)
-            skip = self._skip_set(False)
-            with torch.cuda.device(dev):
-                stream = torch.cuda.current_stream().cuda_stream
-                cnt = torch.empty(1, dtype=torch.int64, device=t.device)
-                cap = max(self._match_cap, 1 << 12, 2 * n)
-                while True:
-                    out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-                    N.check(lib.acb_scan_device_skip(tb, t.data_ptr(), n * stride, None, n, stride, out.data_ptr(), cap,
-                                                     cnt.data_ptr(), stream, N.ALGOS[algo], N.ptr(skip), len(skip)))
-                    found = int(cnt.item())
-                    if found > cap:
-                        cap = self._match_cap = found + 1024
-                        continue
-                    break
-                return self._device_records(tb, out, found, n, stride // self._L, stream, sort)
         _, flat, offs, n, stride, narrow = batch
-        if not (n and flat.size):
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        if narrow:
-            core = self._ensure_narrow(device)
-            if core is None:
-                return np.empty(0, dtype=N.MATCH_DTYPE)
-            tb = core[1]
-        else:
-            tb = self._ensure_table(device)
         skip = self._skip_set(narrow)
-        cap = max(self._match_cap, 1 << 12, 2 * n)
-        found = ctypes.c_int64(0)
-        while True:
-            rc = lib.acb_scan_host_skip(tb, N.ptr(flat), int(flat.size), N.ptr(offs) if offs is not None else None, n, stride,
-                                        None, cap, ctypes.byref(found), N.ALGOS[algo], int(sort), N.ptr(skip), len(skip))
-            if rc != N.ACB_EOVERFLOW:
-                break
-            cap = self._match_cap = int(found.value) + 1024
-        N.check(rc)
-        if not found.value:
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        return _take_records(lib, tb, found.value)
+
+        def scan(tb, cap, found_ref):
+            return lib.acb_scan_host_skip(tb, N.ptr(flat), int(flat.size), N.ptr(offs) if offs is not None else None, n,
+                                          stride, None, cap, found_ref, N.ALGOS[algo], int(sort), N.ptr(skip), len(skip))
+        return self._host_records(device, narrow, n, scan)
 
     def _device_batch_shape(self, t):
         """(n, stride_bytes) of a device batch: a C-contiguous uint8 torch CUDA tensor [n, stride]"""
@@ -948,11 +928,7 @@ class Automaton:
         flat = np.ascontiguousarray(letters).view(np.uint8)
         if flat.size == 0:
             return np.empty(0, dtype=N.MATCH_DTYPE)
-        if narrow:
-            return self._scan_flat(flat, None, 1, int(flat.size), algo=algo, narrow=True)
-        if long_state is not None:
-            return self._scan_flat(flat, None, 1, int(flat.size), algo=algo, long_state=long_state)
-        return self._scan_flat(flat, None, 1, int(flat.size), algo=algo)
+        return self._scan_flat(flat, None, 1, int(flat.size), algo=algo, narrow=narrow, long_state=long_state)
 
     def _require_automaton(self):
         if self.kind != AHOCORASICK:
@@ -1042,77 +1018,46 @@ class Automaton:
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-longest takes 'auto', 'filter' or 'dfa'")
         words = self._words(whole_words)
-        batch = self._batch_input(haystacks)
-        if batch[0] == "device":
-            return Matches(self._leftmost_device(batch[1], algo, words), self._values)
-        _, flat, offs, n, stride, narrow = batch
-        if not (n and flat.size):
-            return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
-        if words is not None:
-            return Matches(self._words_host(flat, offs, n, stride, algo, False, device, narrow, words, True), self._values)
-        return Matches(self._leftmost_host(flat, offs, n, stride, algo, device, narrow), self._values)
+        b = self._batch_input(haystacks)
+        if b.empty:
+            rec = np.empty(0, dtype=N.MATCH_DTYPE)
+        elif b.kind == "device":
+            rec = self._leftmost_device(b, algo, words)
+        elif words is not None:
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True)
+        else:
+            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow)
+        return Matches(rec, self._values)
 
     @_locked
     def _leftmost_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str,
                        device: Optional[int], narrow: bool) -> np.ndarray:
-        """acb_scan_host_leftmost: upload, scan, select, copy back; the capacity grows on overflow."""
-        if narrow:
-            core = self._ensure_narrow(device)
-            if core is None:
-                return np.empty(0, dtype=N.MATCH_DTYPE)
-            tb = core[1]
-        else:
-            tb = self._ensure_table(device)
-        cap = max(self._match_cap, 1 << 12, 2 * n_hay)
-        found = ctypes.c_int64(0)
-        while True:
-            rc = self._lib.acb_scan_host_leftmost(tb, N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None,
-                                                  n_hay, stride_bytes, None, cap, ctypes.byref(found), N.ALGOS[algo])
-            if rc != N.ACB_EOVERFLOW:
-                break
-            cap = self._match_cap = int(found.value) + 1024
-        N.check(rc)
-        if not found.value:
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        return _take_records(self._lib, tb, found.value)
+        """acb_scan_host_leftmost: upload, scan, select, copy back (_host_records)."""
+        return self._host_records(device, narrow, n_hay, lambda tb, cap, found_ref: self._lib.acb_scan_host_leftmost(
+            tb, N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes, None, cap,
+            found_ref, N.ALGOS[algo]))
 
     @_locked
-    def _leftmost_device(self, t, algo: str, words: Optional[tuple] = None) -> np.ndarray:
+    def _leftmost_device(self, batch, algo: str, words: Optional[tuple] = None) -> np.ndarray:
         """A CUDA tensor batch: the full scan into a device buffer, then acb_leftmost_longest_device, both on torch's
         current stream; only the chosen records come back."""
-        import torch
-        n, stride = self._device_batch_shape(t)
-        if n == 0 or stride == 0:
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        t = _aligned(t)
-        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        t = _aligned(batch.data)
+        dev = _device_of(t)
         tb = self._ensure_table(dev)
-        with torch.cuda.device(dev):
-            out, cnt, _ = self._leftmost_chosen(tb, t, n, stride, algo, torch.cuda.current_stream().cuda_stream, words)
+        with _on_device(dev) as stream:
+            out, cnt, _ = self._leftmost_chosen(tb, t, batch.n, batch.stride, algo, stream, words)
             found = int(cnt.item())
             return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
 
     def _leftmost_chosen(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None):
         """The chosen records of an aligned device batch, left on the device: (records [cap, 3] int32 CUDA tensor,
         their count as an int64 CUDA tensor, cap).  Synchronises once, to size the full list; with words, the
-        selection runs on the whole-word matches and a second wait sizes them (_filter_words_device)."""
+        selection runs on the whole-word matches and a second wait sizes them (_device_matches)."""
         import torch
-        cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
-        cap = max(self._match_cap, 1 << 12, 2 * n)
-        while True:
-            full = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-            cnt.zero_()
-            N.check(self._lib.acb_scan_device(tb, t.data_ptr(), n * stride, None, n, stride, full.data_ptr(), cap,
-                                              cnt.data_ptr(), stream, N.ALGOS[algo]))
-            m = int(cnt.item())
-            if m <= cap:
-                break
-            cap = self._match_cap = m + 1024
-        if words is not None:
-            full, m = self._filter_words_device(tb, t, n, stride, full, m, words, stream)
+        full, m = self._device_matches(tb, t, n, stride, algo, stream, words)
         cap = max(m, 1)
         out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-        cnt.zero_()
+        cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
         N.check(self._lib.acb_leftmost_longest_device(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap,
                                                       cnt.data_ptr(), stream))
         return out, cnt, cap
@@ -1172,46 +1117,39 @@ class Automaton:
             raise ValueError("whole_words cannot be combined with ignore_white_space")
         if words is not None and algo == "long":
             raise ValueError("whole_words cannot be combined with algo='long': iter_long's walk picks its matches itself")
-        batch = self._batch_input(haystacks, narrow_ok=algo != "long")
-        if words is not None:
-            if batch[0] == "device":
-                return Matches(self._scan_device_tensor(batch[1], algo, sort, words), self._values)
-            _, flat, offs, n, stride, narrow = batch
-            if not (n and flat.size):
-                return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
-            return Matches(self._words_host(flat, offs, n, stride, algo, sort, device, narrow, words, False), self._values)
-        if ignore_white_space:
-            return Matches(self._scan_skip(batch, algo, sort, device), self._values)
-        if batch[0] == "device":
-            return Matches(self._scan_device_tensor(batch[1], algo, sort), self._values)
-        _, flat, offs, n, stride, narrow = batch
-        if not (n and flat.size):
-            return Matches(np.empty(0, dtype=N.MATCH_DTYPE), self._values)
-        if narrow:
-            return Matches(self._scan_flat(flat, offs, n, stride, algo=algo, sort=sort, device=device, narrow=True), self._values)
-        return Matches(self._scan_flat(flat, offs, n, stride, algo=algo, sort=sort, device=device), self._values)
+        b = self._batch_input(haystacks, narrow_ok=algo != "long")
+        if b.empty:
+            rec = np.empty(0, dtype=N.MATCH_DTYPE)
+        elif b.kind == "device":
+            rec = self._scan_device_tensor(b, algo, sort, words, ignore_white_space)
+        elif words is not None:
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, sort, device, b.narrow, words, False)
+        elif ignore_white_space:
+            rec = self._scan_skip(b, algo, sort, device)
+        else:
+            rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow)
+        return Matches(rec, self._values)
 
-    def _batch_input(self, haystacks, narrow_ok: bool = True, required: bool = True):
-        """The input forms of find_all_batch, checked and laid out for a scan: ("device", tensor) for a CUDA tensor,
-        else ("host", flat uint8, int64 byte offsets or None, n, stride_bytes or 0, narrow).  narrow: the buffer holds
-        the 1-byte letters of the latin-1 automaton (unicode flavour, only where narrow_ok).  required=False: an item
-        of the wrong type raises the TypeError of the dict-like methods instead of iter()'s."""
+    def _batch_input(self, haystacks, narrow_ok: bool = True, required: bool = True) -> "_Batch":
+        """The input forms of find_all_batch, checked and laid out for a scan (_Batch).  narrow: the buffer holds the
+        1-byte letters of the latin-1 automaton (unicode flavour, only where narrow_ok).  required=False: an item of the
+        wrong type raises the TypeError of the dict-like methods instead of iter()'s."""
         L = self._L
         if type(haystacks).__module__.startswith("torch") and getattr(haystacks, "is_cuda", False):
-            return ("device", haystacks)
+            return _Batch("device", haystacks, None, *self._device_batch_shape(haystacks), False)
         if isinstance(haystacks, np.ndarray):
             if haystacks.dtype != np.uint8 or haystacks.ndim != 2 or not haystacks.flags.c_contiguous:
                 raise TypeError("array batches must be 2-D C-contiguous uint8 [n_haystacks, stride_bytes]")
             n, stride = haystacks.shape
             if stride % L:
                 raise ValueError("row length must be a multiple of the letter width")
-            return ("host", haystacks.reshape(-1), None, n, stride, False)
-        if isinstance(haystacks, tuple) and len(haystacks) == 2 and isinstance(haystacks[0], np.ndarray) and isinstance(haystacks[1], np.ndarray):
+            return _Batch("host", haystacks.reshape(-1), None, n, stride, False)
+        if _is_pair(haystacks):
             flat = np.ascontiguousarray(haystacks[0], dtype=np.uint8).reshape(-1)
             offs = np.ascontiguousarray(haystacks[1], dtype=np.int64)
             if offs.ndim != 1 or len(offs) < 1 or offs[0] != 0 or offs[-1] != flat.size or np.any(np.diff(offs) < 0) or np.any(offs % L):
                 raise ValueError("offsets must be non-decreasing multiples of the letter width, start at 0 and end at len(flat)")
-            return ("host", flat, offs, len(offs) - 1, 0, False)
+            return _Batch("host", flat, offs, len(offs) - 1, 0, False)
         # the latin-1 automaton finds exactly the matches of a latin-1 haystack -- all of them.  iter_long's walk is
         # different: which match it keeps depends on the whole trie (a non-latin-1 key whose prefix is latin-1 adds
         # nodes the walk passes through, src/AutomatonSearchIterLong.c:118-126), so it always runs on the full one
@@ -1229,7 +1167,7 @@ class Automaton:
                 flat = "".join(haystacks).encode("utf-32-le", "surrogatepass")
             else:
                 flat = b"".join(haystacks)
-            return ("host", np.frombuffer(flat, dtype=np.uint8), offs, n, 0, False)
+            return _Batch("host", np.frombuffer(flat, dtype=np.uint8), offs, n, 0, False)
         get = self._hay_letters if narrow_ok else self._letters
         letters = [get(h, required=required) for h in haystacks]
         narrow = self._uses_narrow() and len(letters) > 0 and all(a.dtype == np.uint8 for a in letters)
@@ -1241,7 +1179,7 @@ class Automaton:
         offs = np.zeros(n + 1, dtype=np.int64)
         np.cumsum(lens, out=offs[1:])
         flat = np.concatenate(parts) if n else np.empty(0, dtype=np.uint8)
-        return ("host", flat, offs, n, 0, narrow)
+        return _Batch("host", flat, offs, n, 0, narrow)
 
     def stream_batch(self, n_streams: int, *, long: bool = False, algo: str = "auto",
                      device: Optional[int] = None, ignore_white_space: bool = False,
@@ -1257,9 +1195,7 @@ class Automaton:
 
         Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
         wider chunks, so the latin-1 automaton is not used)."""
-        if self.kind != AHOCORASICK:
-            raise AttributeError("Not an Aho-Corasick automaton yet: call add_word to add some keys and call "
-                                 "make_automaton to convert the trie to an automaton.")
+        self._require_automaton()
         n_streams = operator.index(n_streams)
         if n_streams < 0:
             raise ValueError("n_streams must not be negative")
@@ -1315,23 +1251,20 @@ class Automaton:
         """(key_id int32[n], prefix int32[n], length of every key in letters) of a batch of keys: numpy arrays, or for
         a CUDA tensor int32 CUDA tensors computed on torch's current stream and one length for all rows."""
         self._require_automaton()
-        batch = self._batch_input(keys, narrow_ok=False, required=False)
-        if batch[0] == "device":
+        kind, data, offs, n, stride, _ = self._batch_input(keys, narrow_ok=False, required=False)
+        if kind == "device":
             import torch
-            t = batch[1]
-            n, stride = self._device_batch_shape(t)
+            t = data
             key_id = torch.empty(n, dtype=torch.int32, device=t.device)
             prefix = torch.empty(n, dtype=torch.int32, device=t.device)
             if n:
-                dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+                dev = _device_of(t)
                 tb = self._ensure_table(dev)
-                with torch.cuda.device(dev):
+                with _on_device(dev) as stream:
                     N.check(self._lib.acb_lookup_device(tb, t.data_ptr() if stride else None, n * stride, None, n, stride,
-                                                        key_id.data_ptr(), prefix.data_ptr(),
-                                                        torch.cuda.current_stream().cuda_stream))
+                                                        key_id.data_ptr(), prefix.data_ptr(), stream))
             return key_id, prefix, stride // self._L
-        _, flat, offs, n, stride, _ = batch
-        key_id, prefix = self._lookup_host(flat, offs, n, stride, device)
+        key_id, prefix = self._lookup_host(data, offs, n, stride, device)
         lens = (np.diff(offs) if offs is not None else np.full(n, stride, dtype=np.int64)) // self._L
         return key_id, prefix, lens
 
@@ -1349,7 +1282,7 @@ class Automaton:
 
     def _batch_key(self, keys, i: int):
         """key i of a batch as the dict-like methods take it (for KeyError)"""
-        if isinstance(keys, tuple) and len(keys) == 2 and isinstance(keys[0], np.ndarray) and isinstance(keys[1], np.ndarray):
+        if _is_pair(keys):
             flat, offs = keys
             raw = np.ascontiguousarray(flat, dtype=np.uint8).reshape(-1)[int(offs[i]):int(offs[i + 1])].tobytes()
         elif isinstance(keys, (list, tuple)):
@@ -1403,25 +1336,21 @@ class Automaton:
         the output depends on the data, so the call synchronises once to learn it.  Arguments are checked as keys()
         checks them: the first pattern, then wildcard, then how, then the other patterns."""
         self._require_automaton()
-        flat_pair = isinstance(patterns, tuple) and len(patterns) == 2 and all(isinstance(x, np.ndarray) for x in patterns)
-        first = patterns[0] if isinstance(patterns, (list, tuple)) and patterns and not flat_pair else None
+        first = patterns[0] if isinstance(patterns, (list, tuple)) and patterns and not _is_pair(patterns) else None
         _, w, how = self._select_args((first, wildcard, how))
         w = -1 if w is None else w
-        batch = self._batch_input(patterns, narrow_ok=False, required=False)
-        if batch[0] == "device":
-            return self._select_device(batch[1], w, how)
-        _, flat, offs, n, stride, _ = batch
-        return self._select_host(flat, offs, n, stride, w, how, device)
+        kind, data, offs, n, stride, _ = self._batch_input(patterns, narrow_ok=False, required=False)
+        if kind == "device":
+            return self._select_device(data, n, stride, w, how)
+        return self._select_host(data, offs, n, stride, w, how, device)
 
-    def _select_device(self, t, wildcard: int, how: int):
+    def _select_device(self, t, n: int, stride: int, wildcard: int, how: int):
         import torch
-        n, stride = self._device_batch_shape(t)
         out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
         total = torch.empty(1, dtype=torch.int64, device=t.device)
-        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        dev = _device_of(t)
         tb = self._select_table(dev)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream().cuda_stream
+        with _on_device(dev) as stream:
             args = (tb, t.data_ptr() if n * stride else None, n * stride, None, n, stride, wildcard, how, out_offs.data_ptr())
             N.check(self._lib.acb_select_device(*args, None, 0, total.data_ptr(), stream))
             m = int(total.item())                               # the one synchronisation: the size of the output
@@ -1471,7 +1400,76 @@ class Automaton:
         return dict(order=order[:len(self)], lo=lo, cnt=cnt, child_ptr=child_ptr, child=child[:e.value])
 
 
-class StreamBatch:
+class _Streams:
+    """What StreamBatch and ReplaceStream share: the native stream batch `_ss`, reached only through `_native`, the
+    check that the key set has not changed, stream ids, `reset` and `positions`."""
+
+    def __del__(self):
+        try:
+            if getattr(self, "_ss", None) is not None:
+                self._native("free")
+                self._ss = None
+        except Exception:                                   # interpreter shutdown
+            pass
+
+    def _check(self):
+        if self._version != self._A._version:
+            raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
+
+    def _native(self, op: str, *args):
+        """The calls both kinds of native stream batch take: free;  reset(ids int32 or None);  positions ->
+        int64[n_streams]"""
+        lib = self._A._lib
+        if op == "free":
+            lib.acb_streams_free(self._ss)
+            return None
+        if op == "reset":
+            ids, = args
+            N.check(lib.acb_streams_reset(self._ss, None if ids is None else N.ptr(ids), 0 if ids is None else len(ids)))
+            return None
+        out = np.empty(max(self.n_streams, 1), dtype=np.int64)                  # positions
+        N.check(lib.acb_streams_positions(self._ss, N.ptr(out), self.n_streams))
+        return out[:self.n_streams]
+
+    def _ids(self, ids, n: int) -> Optional[np.ndarray]:
+        if ids is None:
+            if n > self.n_streams:
+                raise ValueError(f"{n} chunks for {self.n_streams} streams: pass ids")
+            return None
+        a = np.asarray(ids)
+        if a.ndim != 1 or len(a) != n or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise ValueError(f"ids must be {n} integers, one per chunk")
+        if a.size and (a.min() < 0 or a.max() >= self.n_streams):
+            raise ValueError(f"stream ids must lie in [0, {self.n_streams})")
+        if len(np.unique(a)) != len(a):
+            raise ValueError("a stream id is given twice")
+        return np.ascontiguousarray(a, dtype=np.int32)
+
+    def reset(self, ids=None) -> None:
+        """Streams `ids` (default: all) back to their start, as ``set(x, reset=True)`` does: position 0, nothing carried
+        over or held back."""
+        with self._A._gpu_lock:
+            self._check()
+            if ids is not None:
+                a = np.asarray(ids)
+                if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)) or (a.size and (a.min() < 0 or a.max() >= self.n_streams)):
+                    raise ValueError(f"stream ids must be integers in [0, {self.n_streams})")
+                ids = np.unique(a).astype(np.int32)
+            self._native("reset", ids)
+            self._restart(slice(None) if ids is None else ids)
+
+    def _restart(self, streams) -> None:
+        """`streams` (an index into the streams) are back at position 0: for what the Python side keeps per stream"""
+
+    @property
+    def positions(self) -> np.ndarray:
+        """int64[n_streams]: letters every stream has consumed since its start, its last reset or its last finish (a
+        copy)."""
+        with self._A._gpu_lock:
+            return self._native("positions")
+
+
+class StreamBatch(_Streams):
     """Result of `Automaton.stream_batch()`: the carry-over of `n_streams` streams, kept on the GPU.
 
     ``feed(chunks, ids=None)`` hands over the next chunk of some streams and returns a `Matches` whose ``hay_id`` is
@@ -1503,18 +1501,6 @@ class StreamBatch:
             else:
                 self._ss = self._native("new") if skip is None else self._native("new_skip", skip)
 
-    def __del__(self):
-        try:
-            if getattr(self, "_ss", None) is not None:
-                self._native("free")
-                self._ss = None
-        except Exception:                                   # interpreter shutdown
-            pass
-
-    def _check(self):
-        if self._version != self._A._version:
-            raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
-
     def _native(self, op: str, *args):
         """Every call into the native stream batch (acb_streams_*) goes through here.
           new -> handle;  new_skip(skip set uint32) -> handle of a batch that skips those letters;  free;  reset(ids int32 or None);  positions -> int64[n_streams];
@@ -1522,131 +1508,63 @@ class StreamBatch:
           new_leftmost -> handle of a leftmost-longest batch;
           feed_leftmost(kind, data, offsets, n, stride, ids, final) -> its chosen records, as feed's"""
         A = self._A
-        lib = A._lib
         if op == "new":
             ss = ctypes.c_void_p()
-            N.check(lib.acb_streams_new(A._ensure_table(self._device), self.n_streams, int(self.long), ctypes.byref(ss)))
+            N.check(A._lib.acb_streams_new(A._ensure_table(self._device), self.n_streams, int(self.long), ctypes.byref(ss)))
             return ss
         if op == "new_leftmost":
             return _new_leftmost_streams(A, self.n_streams, self._device)
-        if op == "feed_leftmost":
-            return self._feed_leftmost(*args)
         if op == "new_skip":
             skip, = args
             ss = ctypes.c_void_p()
-            N.check(lib.acb_streams_new_skip(A._ensure_table(self._device), self.n_streams, N.ptr(skip), len(skip), ctypes.byref(ss)))
+            N.check(A._lib.acb_streams_new_skip(A._ensure_table(self._device), self.n_streams, N.ptr(skip), len(skip), ctypes.byref(ss)))
             return ss
-        if op == "free":
-            lib.acb_streams_free(self._ss)
-            return None
-        if op == "reset":
-            ids, = args
-            N.check(lib.acb_streams_reset(self._ss, None if ids is None else N.ptr(ids), 0 if ids is None else len(ids)))
-            return None
-        if op == "positions":
-            out = np.empty(max(self.n_streams, 1), dtype=np.int64)
-            N.check(lib.acb_streams_positions(self._ss, N.ptr(out), self.n_streams))
-            return out[:self.n_streams]
-        kind, data, offs, n, stride, ids, sort = args
-        algo = N.ALGOS[self._algo]
-        if kind == "device":
-            return self._feed_device(data, ids, sort, algo)
-        tb = A._ensure_table(self._device)
-        total = int(data.size)
-        cap = max(A._match_cap, 1 << 12, 2 * n)
-        found = ctypes.c_int64(0)
-        while True:
-            rc = lib.acb_streams_feed_host(self._ss, tb, N.ptr(data) if total else None, total,
-                                           None if offs is None else N.ptr(offs), n, stride,
-                                           None if ids is None else N.ptr(ids), None, cap, ctypes.byref(found), algo, int(sort))
-            if rc == N.ACB_EOVERFLOW:                        # nothing was committed: the same feed again, with room
-                cap = A._match_cap = int(found.value) + 1024
-                continue
-            N.check(rc)
-            break
-        if not found.value:
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        return _take_records(lib, tb, found.value)
+        if op in ("feed", "feed_leftmost"):
+            return self._feed(op == "feed_leftmost", *args)
+        return super()._native(op, *args)
 
-    def _feed_device(self, t, ids, sort, algo):
+    def _feed(self, leftmost: bool, kind: str, data, offs, n: int, stride: int, ids, flag: bool) -> np.ndarray:
+        """acb_streams_feed_* (flag: sort) or, leftmost, acb_streams_feed_leftmost_* (flag: final) -> the records (hay_id =
+        chunk index, end_index in the chunk).  Overflow commits nothing: the retry is the same feed again, with room."""
+        A = self._A
+        lib, algo = A._lib, N.ALGOS[self._algo]
+        if kind == "host":
+            def feed(tb, cap, found_ref):
+                args = (self._ss, tb, N.ptr(data) if data.size else None, int(data.size), None if offs is None else N.ptr(offs),
+                        n, stride, None if ids is None else N.ptr(ids))
+                if leftmost:
+                    return lib.acb_streams_feed_leftmost_host(*args, int(flag), None, cap, found_ref, algo)
+                return lib.acb_streams_feed_host(*args, None, cap, found_ref, algo, int(flag))
+            return A._host_records(self._device, False, n, feed)
         import torch
-        A = self._A
-        n, stride = A._device_batch_shape(t)
-        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
-        if dev != self._device:
-            raise ValueError(f"chunks on cuda:{dev} for a stream batch on cuda:{self._device}")
-        if n and stride:
-            t = _aligned(t)
+        t = _stream_tensor(data, n, stride, self._device)
         tb = A._ensure_table(self._device)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream().cuda_stream
+        with _on_device(self._device) as stream:
             d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
-            cnt = torch.empty(1, dtype=torch.int64, device=t.device)
-            cap = max(A._match_cap, 1 << 12, 2 * n)
-            while True:
-                out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-                N.check(A._lib.acb_streams_feed_device(self._ss, tb, t.data_ptr() if n and stride else None, n * stride, None,
-                                                       n, stride, None if d_ids is None else d_ids.data_ptr(),
-                                                       out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
-                found = int(cnt.item())
-                if found > cap:                              # nothing was committed: the same feed again, with room
-                    cap = A._match_cap = found + 1024
-                    continue
-                break
-            return A._device_records(tb, out, found, n, stride // A._L, stream, sort)
+            args = (self._ss, tb, t.data_ptr() if n and stride else None, n * stride, None, n, stride,
+                    None if d_ids is None else d_ids.data_ptr())
 
-    def _ids(self, ids, n: int) -> Optional[np.ndarray]:
-        if ids is None:
-            if n > self.n_streams:
-                raise ValueError(f"{n} chunks for {self.n_streams} streams: pass ids")
-            return None
-        a = np.asarray(ids)
-        if a.ndim != 1 or len(a) != n or (a.size and not np.issubdtype(a.dtype, np.integer)):
-            raise ValueError(f"ids must be {n} integers, one per chunk")
-        if a.size and (a.min() < 0 or a.max() >= self.n_streams):
-            raise ValueError(f"stream ids must lie in [0, {self.n_streams})")
-        if len(np.unique(a)) != len(a):
-            raise ValueError("a stream id is given twice")
-        return np.ascontiguousarray(a, dtype=np.int32)
-
-    def _feed_leftmost(self, kind, data, offs, n, stride, ids, final):
-        """acb_streams_feed_leftmost_*: the chosen records (hay_id = chunk index, end_index relative to the chunk)"""
-        A = self._A
-        lib = A._lib
-        tb = A._ensure_table(self._device)
-        algo = N.ALGOS[self._algo]
-        cap = max(A._match_cap, 1 << 12, 2 * n)
-        if kind == "device":
-            import torch
-            t = _stream_tensor(data, n, stride, self._device)
-            with torch.cuda.device(t.device):
-                stream = torch.cuda.current_stream().cuda_stream
-                d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
-                cnt = torch.empty(1, dtype=torch.int64, device=t.device)
-                for _ in range(2):
-                    out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
-                    N.check(lib.acb_streams_feed_leftmost_device(self._ss, tb, t.data_ptr() if n and stride else None, n * stride,
-                                                                 None, n, stride, None if d_ids is None else d_ids.data_ptr(),
-                                                                 int(final), out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
-                    found = int(cnt.item())
-                    if found <= cap:
-                        break
-                    cap = A._match_cap = found + 1024            # nothing was committed: the same feed again, with room
+            def feed(out, cap, cnt):
+                if leftmost:
+                    N.check(lib.acb_streams_feed_leftmost_device(*args, int(flag), out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
+                else:
+                    N.check(lib.acb_streams_feed_device(*args, out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
+            out, found = A._device_scan(t, n, feed)
+            if leftmost:
                 return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
-        total = int(data.size)
-        found = ctypes.c_int64(0)
-        for _ in range(2):
-            rc = lib.acb_streams_feed_leftmost_host(self._ss, tb, N.ptr(data) if total else None, total,
-                                                    None if offs is None else N.ptr(offs), n, stride,
-                                                    None if ids is None else N.ptr(ids), int(final), None, cap,
-                                                    ctypes.byref(found), algo)
-            if rc != N.ACB_EOVERFLOW:
-                break
-            cap = A._match_cap = int(found.value) + 1024
-        N.check(rc)
-        if not found.value:
-            return np.empty(0, dtype=N.MATCH_DTYPE)
-        return _take_records(lib, tb, found.value)
+            return A._device_records(tb, out, found, n, stride // A._L, stream, flag)
+
+    def _stream_matches(self, rec: np.ndarray, n: int, ids32) -> Tuple[Matches, np.ndarray]:
+        """A feed's records (hay_id = chunk index, end_index in the chunk) -> (Matches with stream ids and positions in
+        the whole stream, the stream of every chunk)"""
+        sid = np.arange(n, dtype=np.int64) if ids32 is None else ids32.astype(np.int64)
+        m = Matches(rec, self._A._values)
+        m.hay_id = sid[rec["hay_id"]]
+        m.end_index = rec["end_index"].astype(np.int64) + self._pos[m.hay_id]
+        return m, sid
+
+    def _restart(self, streams) -> None:
+        self._pos[streams] = 0
 
     def feed(self, chunks, ids=None, *, sort: bool = True) -> Matches:
         """The next chunk of some streams: chunk h continues stream ids[h] (default: stream h).  `chunks` takes the
@@ -1656,18 +1574,13 @@ class StreamBatch:
         A = self._A
         with A._gpu_lock:
             self._check()
-            args, lens = _stream_chunks(A, chunks)
-            n = args[3]
-            ids32 = self._ids(ids, n)
+            b, lens = _stream_chunks(A, chunks)
+            ids32 = self._ids(ids, b.n)
             if self.leftmost_longest:
-                rec = self._native("feed_leftmost", *args, ids32, False)
+                rec = self._native("feed_leftmost", *b[:5], ids32, False)
             else:
-                rec = self._native("feed", *args, ids32, sort)
-            sid = np.arange(n, dtype=np.int64) if ids32 is None else ids32.astype(np.int64)
-            m = Matches(rec, A._values)
-            chunk = rec["hay_id"]
-            m.hay_id = sid[chunk]
-            m.end_index = rec["end_index"].astype(np.int64) + self._pos[m.hay_id]
+                rec = self._native("feed", *b[:5], ids32, sort)
+            m, sid = self._stream_matches(rec, b.n, ids32)
             self._pos[sid] += lens
             return m
 
@@ -1682,34 +1595,9 @@ class StreamBatch:
             n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
             ids32 = self._ids(ids, n)
             rec = self._native("feed_leftmost", "host", np.empty(0, np.uint8), np.zeros(n + 1, np.int64), n, 0, ids32, True)
-            sid = np.arange(n, dtype=np.int64) if ids32 is None else ids32.astype(np.int64)
-            m = Matches(rec, A._values)
-            m.hay_id = sid[rec["hay_id"]]
-            m.end_index = rec["end_index"].astype(np.int64) + self._pos[m.hay_id]
-            self._pos[sid] = 0
+            m, sid = self._stream_matches(rec, n, ids32)
+            self._restart(sid)
             return m
-
-    def reset(self, ids=None) -> None:
-        """Streams `ids` (default: all) back to their start, as ``set(x, reset=True)`` does: position 0, nothing
-        carried over."""
-        with self._A._gpu_lock:
-            self._check()
-            if ids is None:
-                self._native("reset", None)
-                self._pos[:] = 0
-                return
-            a = np.asarray(ids)
-            if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)) or (a.size and (a.min() < 0 or a.max() >= self.n_streams)):
-                raise ValueError(f"stream ids must be integers in [0, {self.n_streams})")
-            a = np.unique(a).astype(np.int32)
-            self._native("reset", a)
-            self._pos[a] = 0
-
-    @property
-    def positions(self) -> np.ndarray:
-        """int64[n_streams]: letters every stream has consumed since its start or its last reset (a copy)."""
-        with self._A._gpu_lock:
-            return self._native("positions")
 
 
 class Replacer:
@@ -1788,11 +1676,10 @@ class Replacer:
             if algo not in ("auto", "filter", "dfa"):
                 raise ValueError(f"algo {algo!r}: replace_batch takes 'auto', 'filter' or 'dfa'")
             words = A._words(whole_words)
-            pair = isinstance(haystacks, np.ndarray) or (isinstance(haystacks, tuple) and len(haystacks) == 2 and
-                                                         all(isinstance(x, np.ndarray) for x in haystacks))
+            pair = isinstance(haystacks, np.ndarray) or _is_pair(haystacks)
             batch = A._batch_input(haystacks)
-            if batch[0] == "device":
-                return self._run_device(batch[1], algo, words)
+            if batch.kind == "device":
+                return self._run_device(batch, algo, words)
             _, flat, offs, n, stride, narrow = batch
             if narrow and True not in self._tables:         # a replacement outside latin-1: 4 bytes per letter
                 flat = flat.astype("<u4").view(np.uint8)
@@ -1800,7 +1687,7 @@ class Replacer:
                 narrow = False
             if offs is None:
                 offs = np.arange(n + 1, dtype=np.int64) * stride
-            if n == 0 or flat.size == 0:
+            if batch.empty:
                 out, out_offs = flat[:0].copy(), np.zeros(n + 1, dtype=np.int64)
             elif words is None:
                 out, out_offs = self._run_host(flat, offs, n, narrow, algo)
@@ -1844,47 +1731,35 @@ class Replacer:
 
     def _run_host(self, flat: np.ndarray, offs: np.ndarray, n: int, narrow: bool, algo: str, words: Optional[tuple] = None):
         """acb_replace_host (acb_replace_host_words with a word set) -> (output bytes, output offsets int64[n+1]); a
-        second call when the first guess of the output size was too small"""
+        second call when the first guess of the output size was too small (_host_bytes)"""
         A = self._A
-        if narrow:
-            core = A._ensure_narrow(self._device)
-            if core is None:                                # no latin-1 key: nothing matches
-                return flat.copy(), offs.copy()
-            tb = core[1]
-        else:
-            tb = A._ensure_table(self._device)
+        tb = A._table_for(self._device, narrow)
+        if tb is None:                                      # no latin-1 key: nothing matches
+            return flat.copy(), offs.copy()
         r = self._replacer(tb, narrow, self._device)
         out_offs = np.empty(n + 1, dtype=np.int64)
-        total = ctypes.c_int64(0)
-        cap = int(flat.size) + int(flat.size) // 4 + 4096
         batch = (r, tb, N.ptr(flat), int(flat.size), N.ptr(offs), n, 0)
         if words is not None:
             bits, n_bits = _word_bits(words, 1 if narrow else A._L)
-        for _ in range(2):
-            out = np.empty(cap, dtype=np.uint8)
-            result = (N.ALGOS[algo], N.ptr(out_offs), N.ptr(out), cap, ctypes.byref(total))
-            if words is None:
-                rc = A._lib.acb_replace_host(*batch, *result)
-            else:
-                rc = A._lib.acb_replace_host_words(*batch, N.ptr(bits) if n_bits else None, n_bits, *result)
-            if rc != N.ACB_EOVERFLOW:
-                break
-            cap = int(total.value)
-        N.check(rc)
-        return out[:total.value], out_offs
 
-    def _run_device(self, t, algo: str, words: Optional[tuple] = None):
+        def replace(out, total_ref):
+            result = (N.ALGOS[algo], N.ptr(out_offs), N.ptr(out), out.size, total_ref)
+            if words is None:
+                return A._lib.acb_replace_host(*batch, *result)
+            return A._lib.acb_replace_host_words(*batch, N.ptr(bits) if n_bits else None, n_bits, *result)
+        return _host_bytes(int(flat.size) * 5 // 4 + 4096, replace), out_offs
+
+    def _run_device(self, batch, algo: str, words: Optional[tuple] = None):
         """A CUDA tensor batch: scan, select and rewrite on torch's current stream; (flat, offsets) CUDA tensors"""
         import torch
         A = self._A
-        n, stride = A._device_batch_shape(t)
-        if n == 0 or stride == 0:
+        t, n, stride = batch.data, batch.n, batch.stride
+        if batch.empty:
             return torch.empty(0, dtype=torch.uint8, device=t.device), torch.zeros(n + 1, dtype=torch.int64, device=t.device)
         t = _aligned(t)
-        dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+        dev = _device_of(t)
         tb = A._ensure_table(dev)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream().cuda_stream
+        with _on_device(dev) as stream:
             chosen, cnt, cap = A._leftmost_chosen(tb, t, n, stride, algo, stream, words)
             r = self._replacer(tb, False, dev)
             out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
@@ -1898,7 +1773,7 @@ class Replacer:
         return out, out_offs
 
 
-class ReplaceStream:
+class ReplaceStream(_Streams):
     """Result of `Replacer.stream_batch()`: `n_streams` streams rewritten chunk by chunk, what they hold back kept on the
     GPU.  ``feed(chunks, ids=None)`` returns, per chunk, the stream's output that no later letter can change (every
     letter before ``position - (longest_word - 1)`` and every replacement that starts there); ``finish(ids=None)``
@@ -1915,18 +1790,6 @@ class ReplaceStream:
         with self._A._gpu_lock:
             self._ss = self._native("new")
 
-    def __del__(self):
-        try:
-            if getattr(self, "_ss", None) is not None:
-                self._native("free")
-                self._ss = None
-        except Exception:                                   # interpreter shutdown
-            pass
-
-    def _check(self):
-        if self._version != self._A._version:
-            raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
-
     def _native(self, op: str, *args):
         """Every call into the native batch goes through here.  new -> handle;  free;  reset(ids int32 or None);
         positions -> int64[n_streams];  feed(kind, data, offsets, n, stride, ids, final) -> (output bytes, output
@@ -1935,60 +1798,39 @@ class ReplaceStream:
         lib = A._lib
         if op == "new":
             return _new_leftmost_streams(A, self.n_streams, self._device)
-        if op == "free":
-            lib.acb_streams_free(self._ss)
-            return None
-        if op == "reset":
-            ids, = args
-            N.check(lib.acb_streams_reset(self._ss, None if ids is None else N.ptr(ids), 0 if ids is None else len(ids)))
-            return None
-        if op == "positions":
-            out = np.empty(max(self.n_streams, 1), dtype=np.int64)
-            N.check(lib.acb_streams_positions(self._ss, N.ptr(out), self.n_streams))
-            return out[:self.n_streams]
+        if op != "feed":
+            return super()._native(op, *args)
         kind, data, offs, n, stride, ids, final = args
         tb = A._ensure_table(self._device)
         r = self._R._replacer(tb, False, self._device)
         algo = N.ALGOS[self._algo]
         held = n * max(int(lib.acb_trie_longest_word(A._trie)) - 1, 0) * A._L     # at most what the streams hold back
-        if kind == "device":
-            import torch
-            t = _stream_tensor(data, n, stride, self._device)
-            with torch.cuda.device(t.device):
-                stream = torch.cuda.current_stream().cuda_stream
-                d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
-                out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
-                total = torch.empty(1, dtype=torch.int64, device=t.device)
-                cap = (n * stride + held) * 5 // 4 + 4096
-                for _ in range(2):
-                    out = torch.empty(cap, dtype=torch.uint8, device=t.device)
-                    N.check(lib.acb_streams_replace_device(self._ss, r, tb, t.data_ptr() if n and stride else None, n * stride,
-                                                           None, n, stride, None if d_ids is None else d_ids.data_ptr(),
-                                                           int(final), out_offs.data_ptr(), out.data_ptr(), cap,
-                                                           total.data_ptr(), stream, algo))
-                    m = int(total.item())                   # the size of the output
-                    if m <= cap:
-                        break
-                    cap = m                                 # nothing was committed: the same feed again, with room
-                return out[:m], out_offs
-        size = int(data.size)
-        out_offs = np.empty(n + 1, dtype=np.int64)
-        total = ctypes.c_int64(0)
-        cap = (size + held) * 5 // 4 + 4096
-        for _ in range(2):
-            out = np.empty(cap, dtype=np.uint8)
-            rc = lib.acb_streams_replace_host(self._ss, r, tb, N.ptr(data) if size else None, size,
-                                              None if offs is None else N.ptr(offs), n, stride,
-                                              None if ids is None else N.ptr(ids), int(final), algo, N.ptr(out_offs),
-                                              N.ptr(out), cap, ctypes.byref(total))
-            if rc != N.ACB_EOVERFLOW:
-                break
-            cap = int(total.value)
-        N.check(rc)
-        return out[:total.value], out_offs
-
-    def _ids(self, ids, n: int) -> Optional[np.ndarray]:
-        return StreamBatch._ids(self, ids, n)
+        if kind == "host":
+            size = int(data.size)
+            out_offs = np.empty(n + 1, dtype=np.int64)
+            out = _host_bytes((size + held) * 5 // 4 + 4096, lambda out, total_ref: lib.acb_streams_replace_host(
+                self._ss, r, tb, N.ptr(data) if size else None, size, None if offs is None else N.ptr(offs), n, stride,
+                None if ids is None else N.ptr(ids), int(final), algo, N.ptr(out_offs), N.ptr(out), out.size, total_ref))
+            return out, out_offs
+        import torch
+        t = _stream_tensor(data, n, stride, self._device)
+        with _on_device(self._device) as stream:
+            d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
+            out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+            total = torch.empty(1, dtype=torch.int64, device=t.device)
+            cap = (n * stride + held) * 5 // 4 + 4096
+            for retry in (False, True):
+                out = torch.empty(cap, dtype=torch.uint8, device=t.device)
+                N.check(lib.acb_streams_replace_device(self._ss, r, tb, t.data_ptr() if n and stride else None, n * stride,
+                                                       None, n, stride, None if d_ids is None else d_ids.data_ptr(),
+                                                       int(final), out_offs.data_ptr(), out.data_ptr(), cap,
+                                                       total.data_ptr(), stream, algo))
+                m = int(total.item())                       # the size of the output
+                if m <= cap:
+                    return out[:m], out_offs
+                if retry:
+                    raise N.NativeError(f"{m} output bytes after a retry with room for {cap}")
+                cap = m                                     # nothing was committed: the same feed again, with room
 
     def feed(self, chunks, ids=None):
         """The next chunk of some streams (chunk h continues stream ids[h], default stream h), in the input forms of
@@ -1998,12 +1840,11 @@ class ReplaceStream:
         A = self._A
         with A._gpu_lock:
             self._check()
-            as_list = not (isinstance(chunks, np.ndarray) or (isinstance(chunks, tuple) and len(chunks) == 2 and
-                                                              all(isinstance(x, np.ndarray) for x in chunks))
-                           or (type(chunks).__module__.startswith("torch") and getattr(chunks, "is_cuda", False)))
-            args, _ = _stream_chunks(A, chunks)
-            out, offs = self._native("feed", *args, self._ids(ids, args[3]), False)
-            return self._R._items(out, offs, False) if as_list else (out, offs)
+            b, _ = _stream_chunks(A, chunks)
+            out, offs = self._native("feed", *b[:5], self._ids(ids, b.n), False)
+            if isinstance(chunks, np.ndarray) or _is_pair(chunks) or b.kind == "device":
+                return out, offs
+            return self._R._items(out, offs, False)
 
     def finish(self, ids=None) -> list:
         """The output streams `ids` (default: all) still hold back, one item of the haystack type per id; those streams
@@ -2014,24 +1855,6 @@ class ReplaceStream:
             n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
             out, offs = self._native("feed", "host", np.empty(0, np.uint8), np.zeros(n + 1, np.int64), n, 0, self._ids(ids, n), True)
             return self._R._items(out, offs, False)
-
-    def reset(self, ids=None) -> None:
-        """Streams `ids` (default: all) back to their start, dropping what they hold back."""
-        with self._A._gpu_lock:
-            self._check()
-            if ids is None:
-                self._native("reset", None)
-                return
-            a = np.asarray(ids)
-            if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)) or (a.size and (a.min() < 0 or a.max() >= self.n_streams)):
-                raise ValueError(f"stream ids must be integers in [0, {self.n_streams})")
-            self._native("reset", np.unique(a).astype(np.int32))
-
-    @property
-    def positions(self) -> np.ndarray:
-        """int64[n_streams]: letters every stream has consumed since its start, its last reset or its last finish."""
-        with self._A._gpu_lock:
-            return self._native("positions")
 
 
 class AutomatonSearchIter:
@@ -2241,28 +2064,73 @@ def _take_records(lib, tb, found: int) -> np.ndarray:
     return np.asarray(_PinnedRecords(lib, ptr.value, n.value, room.value))
 
 
+class _Batch(NamedTuple):
+    """A batch as _batch_input lays it out.  kind "device": data is the CUDA tensor [n, stride] itself; kind "host": data
+    is the flat uint8 buffer and offsets its int64 byte offsets, or None for rows of a fixed stride (else stride is 0).
+    narrow: the buffer holds the 1-byte letters of the latin-1 automaton."""
+    kind: str
+    data: Any
+    offsets: Optional[np.ndarray]
+    n: int
+    stride: int
+    narrow: bool
+
+    @property
+    def empty(self) -> bool:
+        """no haystack or no letter at all: nothing can match"""
+        return self.n == 0 or (self.stride if self.kind == "device" else self.data.size) == 0
+
+
+def _is_pair(x) -> bool:
+    """x is the (flat, offsets) input form of the batch methods"""
+    return isinstance(x, tuple) and len(x) == 2 and isinstance(x[0], np.ndarray) and isinstance(x[1], np.ndarray)
+
+
 def _stream_chunks(A: Automaton, chunks):
     """A stream feed's chunks in the input forms of find_all_batch (in a list, None is an empty chunk) at the
-    automaton's full letter width -> ((kind, data, offsets, n, stride), letters per chunk int64[n])"""
-    if isinstance(chunks, list) or (isinstance(chunks, tuple) and not (len(chunks) == 2 and isinstance(chunks[0], np.ndarray))):
+    automaton's full letter width -> (_Batch, letters per chunk int64[n])"""
+    if isinstance(chunks, list) or (isinstance(chunks, tuple) and not _is_pair(chunks)):
         empty = () if A._key_type == KEY_SEQUENCE else ("" if A._UNICODE else b"")
         chunks = [empty if c is None else c for c in chunks]
-    batch = A._batch_input(chunks, narrow_ok=False)
-    if batch[0] == "device":
-        n, stride = A._device_batch_shape(batch[1])
-        return ("device", batch[1], None, n, stride), np.full(n, stride // A._L, dtype=np.int64)
-    _, flat, offs, n, stride, _ = batch
-    lens = (np.diff(offs) if offs is not None else np.full(n, stride, dtype=np.int64)) // A._L
-    return ("host", flat, offs, n, stride), lens
+    b = A._batch_input(chunks, narrow_ok=False)
+    if b.kind == "device":
+        return b, np.full(b.n, b.stride // A._L, dtype=np.int64)
+    return b, (np.diff(b.offsets) if b.offsets is not None else np.full(b.n, b.stride, dtype=np.int64)) // A._L
 
 
 def _stream_tensor(t, n: int, stride: int, device: int):
     """a CUDA tensor of chunks for a stream batch on `device`, 16-byte aligned"""
-    import torch
-    dev = t.device.index if t.device.index is not None else torch.cuda.current_device()
+    dev = _device_of(t)
     if dev != device:
         raise ValueError(f"chunks on cuda:{dev} for a stream batch on cuda:{device}")
     return _aligned(t) if n and stride else t
+
+
+def _device_of(t) -> int:
+    """the index of the CUDA device a tensor lives on"""
+    import torch
+    return t.device.index if t.device.index is not None else torch.cuda.current_device()
+
+
+@contextlib.contextmanager
+def _on_device(dev: int):
+    """CUDA device `dev` made current for the block, which gets torch's current stream on it (a cudaStream_t)"""
+    import torch
+    with torch.cuda.device(dev):
+        yield torch.cuda.current_stream().cuda_stream
+
+
+def _host_bytes(cap: int, call) -> np.ndarray:
+    """The output of one host call that writes bytes: call(out, total_ref) writes into out, a fresh uint8[cap], and
+    returns its status.  On ACB_EOVERFLOW it runs once more with room for the exact total; a second overflow raises."""
+    total = ctypes.c_int64(0)
+    out = np.empty(cap, dtype=np.uint8)
+    rc = call(out, ctypes.byref(total))
+    if rc == N.ACB_EOVERFLOW:
+        out = np.empty(int(total.value), dtype=np.uint8)
+        rc = call(out, ctypes.byref(total))
+    N.check(rc)
+    return out[:total.value]
 
 
 def _new_leftmost_streams(A: Automaton, n_streams: int, device: int):
