@@ -14,6 +14,7 @@ import pytest
 
 import oracle
 import pyahocorasick_b200 as ac
+from batch_cases import triples
 from golden_driver import all_scenarios, run_ops
 from refreplay import digest, records_digest, reference_records
 from pyahocorasick_b200 import automaton as am
@@ -43,10 +44,6 @@ def _oracle_for(keys):
         O.add_word(k, i)
     O.make_automaton()
     return O
-
-
-def _records(m):
-    return list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist()))
 
 
 def _want_sorted(O, keys, flat, off):
@@ -82,21 +79,21 @@ def test_random_batches_match_oracle(case, algo):
     off = np.arange(nh + 1, dtype=np.int64) * hl
     want = _want_sorted(O, keys, hay.reshape(-1), off)
     assert len(want) > 0
-    got = _records(A.find_all_batch(hay, algo=algo))
+    got = triples(A.find_all_batch(hay, algo=algo))
     assert got == want
     # ragged offsets, with empty haystacks and odd alignment
     cuts = np.sort(rng.integers(0, hay.size + 1, size=nh))
     cuts[5::7] = cuts[4::7][:len(cuts[5::7])]                 # repeated offsets = empty haystacks
     roff = np.concatenate([[0, 0], np.sort(cuts), [hay.size, hay.size]]).astype(np.int64)
     want2 = _want_sorted(O, keys, hay.reshape(-1), roff)
-    got2 = _records(A.find_all_batch((hay.reshape(-1), roff), algo=algo))
+    got2 = triples(A.find_all_batch((hay.reshape(-1), roff), algo=algo))
     assert got2 == want2
     # list-of-bytes entry point
     hs = [hay[i, : int(rng.integers(0, hl + 1))].tobytes() for i in range(0, min(nh, 200))]
     loff = np.concatenate([[0], np.cumsum([len(h) for h in hs])]).astype(np.int64)
     lflat = np.frombuffer(b"".join(hs), dtype=np.uint8)
     want3 = _want_sorted(O, keys, lflat, loff) if lflat.size else []
-    assert _records(A.find_all_batch(hs, algo=algo)) == want3
+    assert triples(A.find_all_batch(hs, algo=algo)) == want3
 
 
 def c2_sample():
@@ -141,7 +138,7 @@ def test_pathological_overlaps():
     off = np.array([0, hay.size], dtype=np.int64)
     want = _want_sorted(O, keys, hay.reshape(-1), off)
     for algo in ("filter", "dfa"):
-        assert _records(A.find_all_batch(hay, algo=algo)) == want
+        assert triples(A.find_all_batch(hay, algo=algo)) == want
 
 
 def test_pair_kernel_boundaries_and_dense_text():
@@ -167,9 +164,9 @@ def test_pair_kernel_boundaries_and_dense_text():
     off = np.array([0, n], dtype=np.int64)
     want = _want_sorted(O, keys, hay, off)
     assert len(want) > 3000
-    assert _records(A.find_all_batch((hay, off), algo="filter")) == want
+    assert triples(A.find_all_batch((hay, off), algo="filter")) == want
     roff = np.concatenate([[0], np.sort(rng.integers(0, n, size=300)), [n]]).astype(np.int64)
-    assert _records(A.find_all_batch((hay, roff), algo="filter")) == _want_sorted(O, keys, hay, roff)
+    assert triples(A.find_all_batch((hay, roff), algo="filter")) == _want_sorted(O, keys, hay, roff)
     # dense text: one short key back to back -- every position of a slice is pending, every one is a candidate
     dense_keys = [b"abab", b"baba", b"ababab", b"abcd"]
     D = synth.build_automaton(dense_keys)
@@ -177,7 +174,7 @@ def test_pair_kernel_boundaries_and_dense_text():
     OD = _oracle_for(dense_keys)
     dh = np.frombuffer(b"ab" * 30000 + b"abcd" * 100 + b"ab" * 5000, dtype=np.uint8).copy()
     doff = np.array([0, 1000, 1001, 40000, dh.size], dtype=np.int64)
-    assert _records(D.find_all_batch((dh, doff), algo="filter")) == _want_sorted(OD, dense_keys, dh, doff)
+    assert triples(D.find_all_batch((dh, doff), algo="filter")) == _want_sorted(OD, dense_keys, dh, doff)
 
 
 def test_unicode_and_sequence_flavours_on_gpu():
@@ -331,20 +328,20 @@ def test_dense_matches_grow_the_buffers():
     want = _want_sorted(O, keys, hay.reshape(-1), off)
     assert len(want) > 2 * hay.size * 0.9
     for algo in ("filter", "dfa"):
-        assert _records(A.find_all_batch(hay, algo=algo)) == want
+        assert triples(A.find_all_batch(hay, algo=algo)) == want
     import torch
-    assert _records(A.find_all_batch(torch.from_numpy(hay).cuda())) == want       # device-resident entry, same growth path
+    assert triples(A.find_all_batch(torch.from_numpy(hay).cuda())) == want       # device-resident entry, same growth path
 
 
 def test_torch_cuda_tensor_batches():
     import torch
     w = synth.make("C2", scale=0.01)
     A = synth.build_automaton(w.keys)
-    want = _records(A.find_all_batch(w.haystacks))
+    want = triples(A.find_all_batch(w.haystacks))
     d = torch.from_numpy(w.haystacks).cuda()
     for algo in ("filter", "dfa"):
-        assert _records(A.find_all_batch(d, algo=algo)) == want
-    assert sorted(_records(A.find_all_batch(d, sort=False))) == sorted(want)
+        assert triples(A.find_all_batch(d, algo=algo)) == want
+    assert sorted(triples(A.find_all_batch(d, sort=False))) == sorted(want)
 
 
 def test_batch_larger_than_one_segment():
@@ -382,7 +379,7 @@ def test_device_resident_entry_and_overflow_retry():
     from pyahocorasick_b200 import _native as N
     w = synth.make("C2", scale=0.01)
     A = synth.build_automaton(w.keys)
-    want = _records(A.find_all_batch(w.haystacks))
+    want = triples(A.find_all_batch(w.haystacks))
     tb = A._ensure_table(0)
     d_hay = torch.from_numpy(w.haystacks).cuda()
     d_cnt = torch.zeros(1, dtype=torch.int64, device="cuda")

@@ -24,32 +24,12 @@ import pytest
 import emul
 import oracle
 import pyahocorasick_b200 as ac
+from batch_cases import DT, triples
+from kernel_cells import ALPHA, RUN, SLICE, TILE, TOP, Cell, _build, _check_shape, _dense, _keys, _seed
 
-RUN = 32                          # kLaneBytes: one lane's bytes per slice
-SLICE = 32 * RUN                  # kSliceBytes: one consumer warp's slice
-TILE = 20 * SLICE                 # kTileBytes (ACB_TILE_SLICES slices)
 STRIDES = (1, 2, 4, 8, 16)
 PAIR_LOG1 = (13, 16, 19, 20)      # level 2 of 2^13 / 2^16 / 2^19 bits (acb_pair_kernel<0>), 2^17 (acb_pair_kernel<17>)
 GRAMS = {1: range(1, 17), 2: range(2, 17, 2), 4: range(4, 17, 4)}      # a gram is whole letters, at most 16 bytes
-
-
-@dataclasses.dataclass(frozen=True)
-class Cell:
-    L: int                        # letter bytes: 1 bytes, 2 bytes-flavour KEY_SEQUENCE, 4 unicode
-    g: int                        # gram bytes
-    s: int                        # probe stride in bytes
-    log1: int = 0                 # level-1 bitmap of 2^log1 bits; 0: the cost model's
-    pair: bool = False
-    tagmap: bool = False
-
-    @property
-    def env(self):
-        return f"{self.g},{self.s},{self.log1},{int(self.pair)}"
-
-    @property
-    def name(self):
-        kind = "pair" if self.pair else f"L{self.L}-g{self.g}-s{self.s}"
-        return kind + (f"-l{self.log1}" if self.log1 else "") + ("-tag" if self.tagmap else "")
 
 
 def _cells():
@@ -73,81 +53,6 @@ def _all_instantiations():
             {("pair", 0), ("pair", 17), ("pair-tagmap",)})
 
 
-# ------------------------------------------------------------------ key sets and text, in letters
-ALPHA = {1: [0x61, 0x62, 0x63], 2: [0x0061, 0x6162, 0xFFFF], 4: [0x61, 0x142, 0x1F600]}
-TOP = {1: 0xFF, 2: 0xFFFF, 4: 0x10FFFF}          # the largest letter; 0 is the smallest (the zero fill past the end)
-DTYPE = {1: np.uint8, 2: "<u2", 4: "<u4"}
-
-
-def _keys(cell, rng):
-    """Keys of at least m = (g + s - L) / L letters, at least one of exactly m: the forced gram is then the longest this
-    key set offers at the forced stride."""
-    L, alpha = cell.L, ALPHA[cell.L]
-    m, gl, sl = (cell.g + cell.s - L) // L, cell.g // L, cell.s // L
-    keys = []
-
-    def rnd(n):
-        return tuple(int(x) for x in rng.choice(alpha, size=n))
-
-    def add(k):
-        if len(k) >= m:
-            keys.append(tuple(k))
-
-    for _ in range(24):                                         # random keys, most longer than the 20 bytes an entry holds
-        add(rnd(int(rng.integers(m, m + 24 // L + 4))))
-    grm = rnd(gl)                                               # one gram at every probe offset j: anchor chains of one tag
-    for j in range(sl):
-        for _ in range(2):
-            add(rnd(j) + grm + rnd(max(0, m - j - gl) + int(rng.integers(0, 4))))
-    pre = rnd(gl + 3)                                           # a prefix longer than the gram: MULTI entries, trie walks
-    for _ in range(5):
-        add(pre + rnd(max(0, m - len(pre)) + int(rng.integers(0, 6))))
-    for nb in (70, 100):                                        # longer than the DFA's 64-byte warm-up span
-        add(rnd(max(m, nb // L)))
-    k = rnd(m + 3)                                              # nested prefixes and suffixes: order inside one end index
-    for x in (k, k + rnd(2), rnd(1) + k, k[1:], k[:m], rnd(2) + k + rnd(1), k[2:]):
-        add(x)
-    x, y = alpha[0], alpha[1]                                   # periodic keys: alternating text is all hits
-    for n in (m, m + 1, m + 5):
-        add(((x, y) * n)[:n])
-        add(((y, x) * n)[:n])
-    add(rnd(m) + (0, 0))                                        # against the zero fill of the last tile
-    add((0,) * m)
-    add((TOP[L],) * 2 + rnd(m))
-    if L == 4:                                                  # no key for the latin-1 automaton (it ignores ACB_FILTER)
-        keys = [k if max(k) > 0xFF else (0x142,) + k[1:] for k in keys]
-    keys = list(dict.fromkeys(keys))
-    assert min(map(len, keys)) == m
-    return keys
-
-
-def _pkg_key(k, L):
-    if L == 1:
-        return bytes(k)
-    if L == 2:
-        return k
-    return "".join(map(chr, k))
-
-
-def _oracle_key(k, L):
-    return bytes(k) if L == 1 else k
-
-
-def _build(cell, keys, mp):
-    mod = ac.flavour("unicode" if cell.L == 4 else "bytes")
-    A = mod.Automaton(mod.STORE_INTS, mod.KEY_SEQUENCE) if cell.L == 2 else mod.Automaton(mod.STORE_INTS)
-    for i, k in enumerate(keys):
-        A.add_word(_pkg_key(k, cell.L), i)
-    with mp.context() as m:
-        m.setenv("ACB_FILTER", cell.env)
-        if cell.tagmap:
-            m.setenv("ACB_FORCE_TAGMAP", "1")
-        else:
-            m.delenv("ACB_FORCE_TAGMAP", raising=False)
-        A.make_automaton()
-    return A
-
-
 def _instantiation(fs):
     """the kernel template a scan with these tables launches (launch_stream / launch_pair)"""
     if fs["filter_flags"] & emul.FILTER_PAIR:
@@ -155,22 +60,7 @@ def _instantiation(fs):
     return ("stream", (fs["gram_bytes"] + 3) // 4, fs["stride"], "wide" if fs["filter_flags"] & emul.FILTER_WIDE else "narrow")
 
 
-def _check_shape(A, cell):
-    fs = A.filter_shape()
-    assert (fs["gram_bytes"], fs["stride"]) == (cell.g, cell.s), fs
-    if cell.pair:
-        assert fs["filter_flags"] == emul.FILTER_PAIR and fs["log2_bits2"] == (17 if cell.log1 >= 20 else cell.log1), fs
-    else:
-        assert fs["filter_flags"] == (emul.FILTER_WIDE if cell.g % 4 == 0 else 0) and fs["log2_bits2"] == 0, fs
-    if cell.log1:
-        assert fs["log2_bits1"] == cell.log1, fs
-    if cell.tagmap:
-        assert fs["log2_bits3"] >= 16, fs
-    elif cell.pair:
-        assert fs["log2_bits3"] == 0, fs
-    return fs
-
-
+# ------------------------------------------------------------------ text, in letters
 def _text(cell, keys, rng, n_bytes):
     """n_bytes of text in the key alphabet (a few 0 and top letters), keys planted across every lane-run, slice and tile
     boundary (coarser boundaries last, so that their keys survive) at every residue of the stride, and one key ending
@@ -197,13 +87,6 @@ def _text(cell, keys, rng, n_bytes):
     return t, np.asarray(starts, dtype=np.int64)
 
 
-def _dense(cell, n_bytes):
-    """alternating letters: every probe's gram belongs to a periodic key, so every probe of a slice is pending and a
-    match ends at nearly every letter (item-list split, full candidate lists, match staging overflow)"""
-    x, y = ALPHA[cell.L][:2]
-    return np.array([x, y] * (n_bytes // cell.L // 2) + [x], dtype=np.uint32)
-
-
 def _ragged(rng, n, starts, boundaries):
     """offsets (in letters) of a ragged batch over n letters: random cuts, cuts through planted keys and at tile
     boundaries, runs of empty haystacks, empty haystacks first and last"""
@@ -211,6 +94,10 @@ def _ragged(rng, n, starts, boundaries):
     cuts = np.sort(np.concatenate(cuts))
     cuts = np.concatenate([cuts, cuts[::17], cuts[::17], cuts[5::23]])           # repeated offsets: empty haystacks
     return np.concatenate([[0, 0], np.sort(np.clip(cuts, 0, n)), [n, n]]).astype(np.int64)
+
+
+def _oracle_key(k, L):
+    return bytes(k) if L == 1 else k
 
 
 def _oracle(cell, keys):
@@ -227,10 +114,6 @@ def _want(O, cell, letters, off):
     return O.scan_batch_letters(letters, off)
 
 
-def _records(m):
-    return list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist()))
-
-
 def _diff(got, want):
     """a short account of how two record lists differ (the first divergence, a few missing and extra records)"""
     i = next((i for i, (a, b) in enumerate(zip(got, want)) if a != b), min(len(got), len(want)))
@@ -239,17 +122,13 @@ def _diff(got, want):
             f"missing {sorted(sw - sg)[:5]}, extra {sorted(sg - sw)[:5]}")
 
 
-def _seed(cell):
-    return sum(cell.name.encode()) * 7919 + cell.L
-
-
 # ------------------------------------------------------------------ GPU: the kernels
 def _check_gpu(A, batch, want, what):
     for algo in ("filter", "dfa"):
-        got = _records(A.find_all_batch(batch, algo=algo))
+        got = triples(A.find_all_batch(batch, algo=algo))
         if got != want:
             pytest.fail(f"{what}, {algo}: {_diff(got, want)}")
-    got = sorted(_records(A.find_all_batch(batch, algo="filter", sort=False)))
+    got = sorted(triples(A.find_all_batch(batch, algo="filter", sort=False)))
     if got != sorted(want):
         pytest.fail(f"{what}, filter unsorted: {_diff(got, sorted(want))}")
 
@@ -265,7 +144,7 @@ def test_kernel_cell_matches_oracle(cell, monkeypatch):
     A = _build(cell, keys, monkeypatch)
     fs = _check_shape(A, cell)
     O = _oracle(cell, keys)
-    L, dt = cell.L, DTYPE[cell.L]
+    L, dt = cell.L, DT[cell.L]
     n_bytes = 3 * TILE + L * 1291                     # a ragged tail: not a multiple of 16, nor of a stride above L
     t, starts = _text(cell, keys, rng, n_bytes)
     n = t.size
@@ -325,7 +204,7 @@ def test_cell_tables_match_oracle_emulated(cell, monkeypatch):
     _check_shape(A, cell)
     f = A.flat()
     O = _oracle(cell, keys)
-    L, dt = cell.L, DTYPE[cell.L]
+    L, dt = cell.L, DT[cell.L]
     t, starts = _text(cell, keys, rng, 2048 + L * 53)
     n = t.size
     flat = t.astype(dt).view(np.uint8)
@@ -444,9 +323,9 @@ def test_pipelined_scan_of_a_ragged_batch(cell, monkeypatch):
     ends = np.array([e + long_hay[0] for h, e, _ in want if h == h_long])
     assert off[h_long] == long_hay[0] and all(((ends >= a) & (ends < a + CHUNK)).any() for a in (0, CHUNK, 2 * CHUNK))
     for algo in ("filter", "dfa"):
-        got = _records(A.find_all_batch((flat, off), algo=algo))
+        got = triples(A.find_all_batch((flat, off), algo=algo))
         if got != want:
             pytest.fail(f"{algo}: {_diff(got, want)}")
-    got = sorted(_records(A.find_all_batch((flat, off), algo="filter", sort=False)))
+    got = sorted(triples(A.find_all_batch((flat, off), algo="filter", sort=False)))
     if got != sorted(want):
         pytest.fail(f"filter unsorted: {_diff(got, sorted(want))}")

@@ -12,122 +12,34 @@ import pytest
 import emul_leftmost
 import oracle
 import pyahocorasick_b200 as pkg
+from batch_cases import (CASES, DT, automaton, check_device_capacities, check_host_capacities, fake_table, forms,
+                         got_values, key_len, leftmost_random_case, leftmost_structured_cases, np_greedy, obj, oracle_full,
+                         rows, skip_if_device, table_and_batch)
 from pyahocorasick_b200 import _native as N
 
 TILES = [1, 2, 3, 7]
 
-# (flavour, key type, text alphabet): latin-1, wide and mixed unicode; bytes-flavour sequences are 2-byte letters,
-# unicode-flavour sequences 4-byte ones
-CASES = {
-    "bytes": ("bytes", False, [0x61, 0x62, 0xE9]),
-    "latin1": ("unicode", False, [0x61, 0x62, 0xE9]),
-    "wide": ("unicode", False, [0x61, 0x142, 0x1F600]),
-    "mixed": ("unicode", False, [0x61, 0x62, 0x1F600]),
-    "seq2": ("bytes", True, [0x61, 0x6162, 0xFF20]),
-    "seq4": ("unicode", True, [0x61, 0x1F600, 0x10FFFF]),
-}
-
-
-def _obj(case, letters):
-    fl, seq, _ = CASES[case]
-    if seq:
-        return tuple(letters)
-    return bytes(letters) if fl == "bytes" else "".join(map(chr, letters))
-
-
-def _automaton(case, keys):
-    fl, seq, _ = CASES[case]
-    mod = pkg.flavour(fl)
-    A = mod.Automaton(mod.STORE_INTS, mod.KEY_SEQUENCE) if seq else mod.Automaton(mod.STORE_INTS)
-    O = oracle.OracleAutomaton()
-    for i, k in enumerate(keys):
-        A.add_word(_obj(case, k), i)
-        O.add_word(_obj(case, k), i)
-    A.make_automaton()
-    O.make_automaton()
-    return A, O
-
-
-def _full(O, hays, case="bytes"):
-    """the C oracle's full list [(hay, end, value)]; bytes-flavour text letters as the reference widens them"""
-    fl, seq, _ = CASES[case]
-    letters = np.array([x for h in hays for x in h], dtype=np.uint32)
-    if fl == "bytes" and not seq:
-        letters = oracle._letters(letters.astype(np.uint8).tobytes())
-    offs = np.zeros(len(hays) + 1, dtype=np.int64)
-    np.cumsum([len(h) for h in hays], out=offs[1:])
-    return O.scan_batch_letters(letters, offs)
-
 
 def _want(O, keys, hays, case="bytes"):
-    return emul_leftmost.greedy(_full(O, hays, case), [len(k) for k in keys])
-
-
-def _got(m):
-    return list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.values()))
-
-
-def _random_case(case, rng):
-    _, _, al = CASES[case]
-    keys = sorted({tuple(int(x) for x in rng.choice(al[:2] if rng.integers(0, 2) else al, size=int(rng.integers(1, 7))))
-                   for _ in range(int(rng.integers(1, 9)))})
-    hays = []
-    for _ in range(int(rng.integers(1, 10))):
-        r = int(rng.integers(0, 6))
-        if r == 0:
-            hays.append([])
-        elif r == 1:
-            hays.append([0x63] * int(rng.integers(1, 5)) if case != "seq2" else [0x7A])          # no match
-        else:
-            hays.append([int(x) for x in rng.choice(al, size=int(rng.integers(1, 50)))])
-    if case == "mixed" and all(max(h, default=0) < 256 for h in hays):
-        hays.append([0x1F600, 0x61, 0x62])
-    return keys, hays
-
-
-def _forms(case, A, hays):
-    """the input forms of find_all_batch for this case"""
-    yield "list", [_obj(case, h) for h in hays]
-    if case in ("latin1", "mixed"):
-        return
-    dt = {1: np.uint8, 2: "<u2", 4: "<u4"}[A._L]
-    parts = [np.asarray(h, dtype=dt).view(np.uint8) for h in hays]
-    offs = np.zeros(len(parts) + 1, dtype=np.int64)
-    np.cumsum([p.size for p in parts], out=offs[1:])
-    yield "flat", (np.concatenate(parts), offs)
-    width = max(len(h) for h in hays)
-    if width and all(len(h) == width for h in hays):
-        yield "array", np.stack(parts)
+    return emul_leftmost.greedy(oracle_full(O, hays, case), [len(k) for k in keys])
 
 
 # ------------------------------------------------------------------ the restatement against the definition (CPU)
-NESTED = [[0x61] * k for k in range(1, 17)]                               # a ... a^16
-
-
-def _structured_cases():
-    """nested keys, prefixes and suffixes of others, adjacent and abutting matches, empty haystacks, no match"""
-    a, b, c = 0x61, 0x62, 0x63
-    yield NESTED, [[a] * 40, [a] * 16 + [b] + [a] * 17, [], [b, b], [a, b] * 9, [a]]
-    yield [[a, b], [a, b, c], [b, c], [c], [b, c, a, b]], [[a, b, c, a, b, c], [a, b, a, b, a, b], [c, c, c], [], [b, c, a, b, c]]
-    yield [[a, b, c, 0x64, 0x65], [b, c, 0x64, 0x78], [c, 0x64]], [[a, b, c, 0x64, 0x79]]      # the documented example
-    yield [[a, b], [b, a]], [[a, b, a, b, a], [b, a, b], [a], [b]]
-
-
 @pytest.mark.parametrize("tile", TILES + [2048])
 def test_restatement_equals_the_definition_on_the_oracle(tile):
     rng = np.random.default_rng(tile)
-    for case in CASES:
+    for case, (fl, seq, _) in CASES.items():
         for _ in range(12):
-            keys, hays = _random_case(case, rng)
-            _, O = _automaton(case, keys)
-            full = _full(O, hays, case)
+            keys, hays = leftmost_random_case(case, rng)
+            _, O = automaton(fl, seq, keys)
+            full = oracle_full(O, hays, case)
             kl = np.array([len(k) for k in keys])
             raw = np.array(full, dtype=np.int64).reshape(-1, 3)
             got = emul_leftmost.select(raw[rng.permutation(len(raw))], kl, int(kl.max()), tile)
             assert [tuple(r) for r in got.tolist()] == emul_leftmost.greedy(full, kl), (case, keys, hays)
-    for keys, hays in _structured_cases():
-        _, O = _automaton("bytes", keys)
-        full = _full(O, hays)
+    for keys, hays in leftmost_structured_cases():
+        _, O = automaton("bytes", False, keys)
+        full = oracle_full(O, hays)
         kl = np.array([len(k) for k in keys])
         got = emul_leftmost.select(np.array(full, dtype=np.int64).reshape(-1, 3), kl, int(kl.max()), tile)
         assert [tuple(r) for r in got.tolist()] == emul_leftmost.greedy(full, kl)
@@ -140,11 +52,11 @@ def test_chains_enter_tiles_at_every_offset(tile):
     rng = np.random.default_rng(100 + tile)
     for W in (1, 2, 5, 16):
         keys = [[0x61] * k for k in range(1, W + 1)]
-        _, O = _automaton("bytes", keys)
+        _, O = automaton("bytes", False, keys)
         hay = []
         for _ in range(30):
             hay += [0x61] * int(rng.integers(1, 3 * W + 2)) + [0x62]
-        full = _full(O, [hay, hay[:17], hay])
+        full = oracle_full(O, [hay, hay[:17], hay])
         kl = np.array([len(k) for k in keys])
         got = emul_leftmost.select(np.array(full, dtype=np.int64).reshape(-1, 3), kl, W, tile)
         assert [tuple(r) for r in got.tolist()] == emul_leftmost.greedy(full, kl)
@@ -154,16 +66,16 @@ def test_chains_enter_tiles_at_every_offset(tile):
 def test_python_layer_on_the_restatement(monkeypatch, tile):
     emul_leftmost.install(monkeypatch, tile)
     rng = np.random.default_rng(7 + tile)
-    for case in CASES:
+    for case, (fl, seq, _) in CASES.items():
         for _ in range(4):
-            keys, hays = _random_case(case, rng)
-            A, O = _automaton(case, keys)
+            keys, hays = leftmost_random_case(case, rng)
+            A, O = automaton(fl, seq, keys)
             want = _want(O, keys, hays, case)
-            for form, batch in _forms(case, A, hays):
-                assert _got(A.find_leftmost_longest_batch(batch)) == want, (case, form)
-    for keys, hays in _structured_cases():
-        A, O = _automaton("bytes", keys)
-        assert _got(A.find_leftmost_longest_batch([bytes(h) for h in hays])) == _want(O, keys, hays)
+            for form, batch in forms([obj(fl, seq, h) for h in hays], hays, A._L, case in ("latin1", "mixed")):
+                assert got_values(A.find_leftmost_longest_batch(batch)) == want, (case, form)
+    for keys, hays in leftmost_structured_cases():
+        A, O = automaton("bytes", False, keys)
+        assert got_values(A.find_leftmost_longest_batch([bytes(h) for h in hays])) == _want(O, keys, hays)
 
 
 def test_abcde_example_differs_from_iter_long(monkeypatch):
@@ -171,7 +83,7 @@ def test_abcde_example_differs_from_iter_long(monkeypatch):
     direct fail link), iter reports (3, cd), and leftmost-longest takes cd"""
     emul_leftmost.install(monkeypatch)
     keys = [b"abcde", b"bcdx", b"cd"]
-    A, O = _automaton("bytes", [list(k) for k in keys])
+    A, O = automaton("bytes", False, keys)
     assert list(O.iter_long(b"abcdy")) == []
     assert list(O.iter(b"abcdy")) == [(3, 2)]
     if oracle.ref_available("bytes"):
@@ -181,7 +93,7 @@ def test_abcde_example_differs_from_iter_long(monkeypatch):
         R.make_automaton()
         assert list(R.iter_long(b"abcdy")) == []
         assert list(R.iter(b"abcdy")) == [(3, 2)]
-    assert _got(A.find_leftmost_longest_batch([b"abcdy"])) == [(0, 3, 2)]
+    assert got_values(A.find_leftmost_longest_batch([b"abcdy"])) == [(0, 3, 2)]
 
 
 def test_argument_errors():
@@ -197,7 +109,7 @@ def test_argument_errors():
         with pytest.raises(ValueError):
             A.find_leftmost_longest_batch([b"ab"], algo=algo)
     L = N.lib()
-    fake = ctypes.create_string_buffer(1 << 16)                # zeroed: device 0; never used past the checks
+    fake = fake_table()                                         # device 0; never used past the checks
     n = ctypes.c_int64(0)
     hay = np.zeros(16, dtype=np.uint8)
     assert L.acb_scan_host_leftmost(None, N.ptr(hay), 16, None, 1, 16, None, 8, ctypes.byref(n), N.ALGO_AUTO) == N.ACB_EINVAL
@@ -213,10 +125,8 @@ def test_argument_errors():
 
 
 def test_host_route_fails_loudly_without_a_device():
-    import torch
-    if torch.cuda.is_available():
-        pytest.skip("a device is present")
-    fake = ctypes.create_string_buffer(1 << 16)
+    skip_if_device()
+    fake = fake_table()
     n = ctypes.c_int64(0)
     hay = np.frombuffer(b"abcd" * 4, dtype=np.uint8)
     offs = np.array([0, 8, 16], dtype=np.int64)
@@ -225,58 +135,22 @@ def test_host_route_fails_loudly_without_a_device():
 
 
 # ------------------------------------------------------------------ the real kernels
-def _np_greedy(full: np.ndarray, key_len: np.ndarray) -> np.ndarray:
-    """the definition over a full record array (hay_id, end_index, key_id), vectorised but for the walk itself"""
-    if len(full) == 0:
-        return np.empty((0, 3), dtype=np.int64)
-    hay, end, key = (full[f].astype(np.int64) for f in ("hay_id", "end_index", "key_id"))
-    ln = key_len[key]
-    start = end - ln + 1
-    o = np.lexsort((-ln, start, hay))
-    hay, start, ln, end, key = hay[o], start[o], ln[o], end[o], key[o]
-    first = np.ones(len(o), dtype=bool)
-    first[1:] = (hay[1:] != hay[:-1]) | (start[1:] != start[:-1])
-    hay, start, ln, end, key = hay[first], start[first], ln[first], end[first], key[first]
-    big = np.int64(1) << 32                                 # start + len < 2^32: one sortable number per (hay, start)
-    flat = hay * big + start
-    nxt = np.searchsorted(flat, flat + ln)
-    nxt_ok = nxt < len(flat)
-    nxt_ok[nxt_ok] = hay[nxt[nxt_ok]] == hay[nxt_ok]
-    heads = np.nonzero(np.r_[True, hay[1:] != hay[:-1]])[0].tolist()
-    nx = np.where(nxt_ok, nxt, -1).tolist()
-    chosen = []
-    for i in heads:
-        while i >= 0:
-            chosen.append(i)
-            i = nx[i]
-    chosen = np.array(sorted(chosen), dtype=np.int64)
-    return np.stack([hay[chosen], end[chosen], key[chosen]], axis=1)
-
-
-def _rec(m):
-    return np.stack([m.hay_id.astype(np.int64), m.end_index.astype(np.int64), m.key_id.astype(np.int64)], axis=1)
-
-
-def _key_len(A):
-    return np.asarray(A.flat()["key_len"], dtype=np.int64)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("algo", ["filter", "dfa"])
 def test_gpu_fuzz_against_the_definition(algo):
     rng = np.random.default_rng(11)
-    for case in CASES:
+    for case, (fl, seq, _) in CASES.items():
         for _ in range(6):
-            keys, hays = _random_case(case, rng)
-            A, O = _automaton(case, keys)
+            keys, hays = leftmost_random_case(case, rng)
+            A, O = automaton(fl, seq, keys)
             want = _want(O, keys, hays, case)
-            for form, batch in _forms(case, A, hays):
-                assert _got(A.find_leftmost_longest_batch(batch, algo=algo)) == want, (case, form, keys, hays)
-    for keys, hays in _structured_cases():
-        A, O = _automaton("bytes", keys)
-        assert _got(A.find_leftmost_longest_batch([bytes(h) for h in hays], algo=algo)) == _want(O, keys, hays)
-    A, _ = _automaton("bytes", [list(b"abcde"), list(b"bcdx"), list(b"cd")])
-    assert _got(A.find_leftmost_longest_batch([b"abcdy"], algo=algo)) == [(0, 3, 2)]
+            for form, batch in forms([obj(fl, seq, h) for h in hays], hays, A._L, case in ("latin1", "mixed")):
+                assert got_values(A.find_leftmost_longest_batch(batch, algo=algo)) == want, (case, form, keys, hays)
+    for keys, hays in leftmost_structured_cases():
+        A, O = automaton("bytes", False, keys)
+        assert got_values(A.find_leftmost_longest_batch([bytes(h) for h in hays], algo=algo)) == _want(O, keys, hays)
+    A, _ = automaton("bytes", False, [list(b"abcde"), list(b"bcdx"), list(b"cd")])
+    assert got_values(A.find_leftmost_longest_batch([b"abcdy"], algo=algo)) == [(0, 3, 2)]
     assert list(A.iter_long(b"abcdy")) == []
 
 
@@ -293,10 +167,10 @@ def test_gpu_filter_and_dfa_identical_and_ragged():
     for batch in (w.haystacks, (flat, offs)):
         f = A.find_leftmost_longest_batch(batch, algo="filter")
         d = A.find_leftmost_longest_batch(batch, algo="dfa")
-        assert np.array_equal(_rec(f), _rec(d))
+        assert np.array_equal(rows(f), rows(d))
         full = A.find_all_batch(batch, algo="filter")
-        assert np.array_equal(_rec(f), _np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id],
-                                                                    names="hay_id,end_index,key_id"), _key_len(A)))
+        assert np.array_equal(rows(f), np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id],
+                                                                    names="hay_id,end_index,key_id"), key_len(A)))
     assert (np.diff(offs) == 0).any()
 
 
@@ -307,12 +181,12 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
     rng = np.random.default_rng(5)
     case = "bytes" if fl == "bytes" else "wide"
     keys = [list(k) for k in ({tuple(rng.choice(CASES[case][2][:2], size=int(rng.integers(1, 6)))) for _ in range(12)})]
-    A, O = _automaton(case, keys)
+    A, O = automaton(*CASES[case][:2], keys)
     L = A._L
     hays = [[int(x) for x in rng.choice(CASES[case][2], size=7)] for _ in range(300)]
-    host = np.stack([np.asarray(h, dtype={1: np.uint8, 4: "<u4"}[L]).view(np.uint8) for h in hays])
+    host = np.stack([np.asarray(h, dtype=DT[L]).view(np.uint8) for h in hays])
     d = torch.from_numpy(host).cuda()
-    want = _got(A.find_leftmost_longest_batch(host))
+    want = got_values(A.find_leftmost_longest_batch(host))
     assert want == _want(O, keys, hays, case)
     views = {"whole": (d, hays)}
     if L == 1:
@@ -323,53 +197,29 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
     for name, (t, hs) in views.items():
         with torch.cuda.stream(side):
             m = A.find_leftmost_longest_batch(t)
-        assert _got(m) == _want(O, keys, hs, case), name
-
-
-def _table_and_batch(A, hays):
-    flat = np.frombuffer(b"".join(hays), dtype=np.uint8)
-    offs = np.zeros(len(hays) + 1, dtype=np.int64)
-    np.cumsum([len(h) for h in hays], out=offs[1:])
-    return A._ensure_table(0), flat, offs
+        assert got_values(m) == _want(O, keys, hs, case), name
 
 
 @pytest.mark.gpu
 def test_gpu_exact_counts_at_every_capacity():
     import torch
     keys = [b"a" * k for k in range(1, 6)] + [b"ab", b"ba"]
-    A, _ = _automaton("bytes", [list(k) for k in keys])
+    A, _ = automaton("bytes", False, keys)
     hays = [b"aaaaaaaabaaab" * 30, b"", b"ba" * 40, b"c"]
-    want = _rec(A.find_leftmost_longest_batch(hays))
+    want = rows(A.find_leftmost_longest_batch(hays))
     n = len(want)
     assert n > 10
     L = N.lib()
-    tb, flat, offs = _table_and_batch(A, hays)
-    found = ctypes.c_int64(0)
-    for cap in (0, 1, n - 1, n):
-        out = np.zeros(max(cap, 1), dtype=N.MATCH_DTYPE)
-        rc = L.acb_scan_host_leftmost(tb, N.ptr(flat), flat.size, N.ptr(offs), len(hays), 0, N.ptr(out), cap, ctypes.byref(found), N.ALGO_AUTO)
-        assert found.value == n
-        assert rc == (N.ACB_OK if cap >= n else N.ACB_EOVERFLOW)
-        if cap >= n:
-            assert np.array_equal(_rec(np.rec.fromarrays([out["hay_id"][:n], out["end_index"][:n], out["key_id"][:n]],
-                                                        names="hay_id,end_index,key_id")), want)
-    # the device entry: the full list in any order, guard rows behind the capacity stay untouched
+    tb, flat, offs = table_and_batch(A, hays)
+    check_host_capacities(lambda out, cap, found: L.acb_scan_host_leftmost(
+        tb, N.ptr(flat), flat.size, N.ptr(offs), len(hays), 0, out, cap, found, N.ALGO_AUTO), want)
+    # the device entry: the full list in any order
     full = A.find_all_batch(hays)
     rec = np.stack([full.hay_id, full.end_index, full.key_id], axis=1).astype(np.int32)
     rec = rec[np.random.default_rng(0).permutation(len(rec))]
     d_rec = torch.from_numpy(np.ascontiguousarray(rec)).cuda()
-    for cap in (0, 1, n - 1, n):
-        out = torch.full((cap + 4, 3), -7, dtype=torch.int32, device="cuda")
-        cnt = torch.tensor([5], dtype=torch.int64, device="cuda")             # the count is added to
-        assert L.acb_leftmost_longest_device(tb, d_rec.data_ptr(), len(rec), len(hays), int(flat.size), out.data_ptr(), cap,
-                                             cnt.data_ptr(), torch.cuda.current_stream().cuda_stream) == N.ACB_OK
-        assert int(cnt.item()) == 5 + n
-        o = out.cpu().numpy()
-        assert (o[cap:] == -7).all()
-        if cap > 5:
-            assert np.array_equal(o[5:cap].astype(np.int64), want[:cap - 5])
-        assert (o[:min(cap, 5)] == -7).all()                                     # slots before *d_count are not written
-    assert np.array_equal(rec, d_rec.cpu().numpy())                             # d_records is not changed
+    check_device_capacities(lambda out, cap, cnt, s: L.acb_leftmost_longest_device(
+        tb, d_rec.data_ptr(), len(rec), len(hays), int(flat.size), out, cap, cnt, s), want, d_rec)
 
 
 @pytest.mark.gpu
@@ -379,15 +229,15 @@ def test_gpu_one_haystack_over_many_tiles():
     rng = np.random.default_rng(9)
     for W in (1, 3, 16, 64):
         keys = [b"a" * k for k in range(1, W + 1)] + [b"ab", b"ba" * 3]
-        A, _ = _automaton("bytes", [list(k) for k in keys])
+        A, _ = automaton("bytes", False, keys)
         runs = rng.integers(1, 3 * W + 2, size=40000 // W + 2000)
         hay = b"b".join(b"a" * int(r) for r in runs)
         hays = [hay, b"", hay[: len(hay) // 3], b"ab" * 5000]
         got = A.find_leftmost_longest_batch(hays)
         full = A.find_all_batch(hays)
-        want = _np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), _key_len(A))
+        want = np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), key_len(A))
         assert len(want) > 3 * 2048
-        assert np.array_equal(_rec(got), want), W
+        assert np.array_equal(rows(got), want), W
 
 
 def _windows_agree(O, text: bytes, got: np.ndarray, key_len, max_len, rng, n=40, span=1 << 16):
@@ -412,14 +262,14 @@ def test_gpu_single_haystack_of_256_mib():
     numpy pass of the definition over find_all_batch's list and on sampled windows against the C oracle"""
     rng = np.random.default_rng(21)
     keys = sorted({bytes(rng.choice(list(b"acgt"), size=int(rng.integers(3, 7))).tolist()) for _ in range(24)})
-    A, O = _automaton("bytes", [list(k) for k in keys])
+    A, O = automaton("bytes", False, keys)
     text = rng.choice(np.frombuffer(b"acgt", dtype=np.uint8), size=256 << 20)
     offs = np.array([0, text.size], dtype=np.int64)
     m = A.find_leftmost_longest_batch((text, offs))
-    got = _rec(m)
+    got = rows(m)
     full = A.find_all_batch((text, offs))
-    kl = _key_len(A)
-    want = _np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), kl)
+    kl = key_len(A)
+    want = np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), kl)
     assert len(want) > 2_000_000
     assert np.array_equal(got, want)
     by_value = np.stack([got[:, 0], got[:, 1], np.array(m.values(), dtype=np.int64)], axis=1)
@@ -431,21 +281,21 @@ def test_gpu_batch_past_2_gib():
     """a CUDA tensor of 2^31 + 2^24 bytes in 2 080 rows, keys planted near the end of rows and across 2^31"""
     import torch
     keys = [b"qzqzx", b"zqzx", b"qzq", b"xqzqzxq"]
-    A, _ = _automaton("bytes", [list(k) for k in keys])
-    rows, stride = 2080, ((1 << 31) + (1 << 24)) // 2080 // 16 * 16
-    d = torch.randint(0, 16, (rows, stride), dtype=torch.uint8, device="cuda")
+    A, _ = automaton("bytes", False, keys)
+    n_rows, stride = 2080, ((1 << 31) + (1 << 24)) // 2080 // 16 * 16
+    d = torch.randint(0, 16, (n_rows, stride), dtype=torch.uint8, device="cuda")
     d += ord("a")                                                            # a..p: no key letter but for planted ones
     rng = np.random.default_rng(2)
-    for r in rng.integers(0, rows, size=400).tolist():
+    for r in rng.integers(0, n_rows, size=400).tolist():
         c = int(rng.integers(0, stride - 8))
         for j, b in enumerate(b"xqzqzxq"[: int(rng.integers(3, 8))]):
             d[r, c + j] = b
     d[-1, -8:] = torch.tensor(list(b"qzqzxqzq"), dtype=torch.uint8)
     got = A.find_leftmost_longest_batch(d)
     full = A.find_all_batch(d)
-    want = _np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), _key_len(A))
-    assert rows * stride > (1 << 31) and len(want) > 300
-    assert np.array_equal(_rec(got), want)
+    want = np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), key_len(A))
+    assert n_rows * stride > (1 << 31) and len(want) > 300
+    assert np.array_equal(rows(got), want)
 
 
 @pytest.mark.gpu
@@ -455,13 +305,13 @@ def test_gpu_sort_key_of_64_and_65_bits(log_len):
     len) takes 16 + 28 + 20 = 64 bits (one radix sort) or 65 (two stable passes)"""
     rng = np.random.default_rng(log_len)
     short = [b"ab", b"abc", b"bca", b"cab", b"abcab"]
-    A, _ = _automaton("bytes", [list(k) for k in short + [b"d" * (1 << log_len)]])
+    A, _ = automaton("bytes", False, [list(k) for k in short + [b"d" * (1 << log_len)]])
     n = (128 << 20) + 4096
     text = rng.choice(np.frombuffer(b"abc", dtype=np.uint8), size=n)
     off = np.concatenate([[0], np.sort(rng.integers(0, n, size=65535)), [n]]).astype(np.int64)
     bits = sum(int(v).bit_length() or 1 for v in (len(off) - 2, n, 1 << log_len))
     assert bits == (64 if log_len == 19 else 65)
-    got = _rec(A.find_leftmost_longest_batch((text, off)))
+    got = rows(A.find_leftmost_longest_batch((text, off)))
     full = A.find_all_batch((text, off))
-    want = _np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), _key_len(A))
+    want = np_greedy(np.rec.fromarrays([full.hay_id, full.end_index, full.key_id], names="hay_id,end_index,key_id"), key_len(A))
     assert np.array_equal(got, want)

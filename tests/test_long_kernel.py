@@ -28,6 +28,7 @@ import pytest
 import emul
 import oracle
 import pyahocorasick_b200 as ac
+from batch_cases import DT, triples
 from pyahocorasick_b200 import _native as N
 
 # name -> (letter bytes, flavour, KEY_SEQUENCE, alphabet a b c d, a letter in no key)
@@ -37,7 +38,6 @@ WIDTHS = {
     "L4": (4, "unicode", False, (0x42, 0x142, 0x4242, 0x1F642), 0x7A),
     "L4seq": (4, "unicode", True, (0x42, 0x10042, 0x4242, 0xFFFF0042), 0x7A7A7A7A),
 }
-DTYPE = {1: np.uint8, 2: "<u2", 4: "<u4"}
 
 # key sets over the alphabet's indices
 KEYSETS = {
@@ -123,11 +123,7 @@ def _ragged(width, keys, rng, n_hay):
 
 
 def _flat(width, letters):
-    return np.ascontiguousarray(letters.astype(DTYPE[WIDTHS[width][0]])).view(np.uint8)
-
-
-def _records(m):
-    return list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist()))
+    return np.ascontiguousarray(letters.astype(DT[WIDTHS[width][0]])).view(np.uint8)
 
 
 def _diff(got, want):
@@ -181,11 +177,11 @@ def test_long_kernel_matches_oracle(width, keyset):
     assert any(e == off[h + 1] - off[h] - 1 for h, e, _ in want)                 # ... and at the last
     assert any(e == len(keys[v]) - 1 == off[h + 1] - off[h] - 1 for h, e, v in want)   # a key as long as its haystack
     batch = (_flat(width, t), off * L)
-    _check(_records(A.find_long_batch(batch)), want, "ragged")
-    _check(sorted(_records(A.find_long_batch(batch, sort=False))), sorted(want), "ragged, unsorted")
+    _check(triples(A.find_long_batch(batch)), want, "ragged")
+    _check(sorted(triples(A.find_long_batch(batch, sort=False))), sorted(want), "ragged, unsorted")
     # the list entry point
     hays = _hay_objects(width, t, off[:301])
-    _check(_records(A.find_long_batch(hays)), [r for r in want if r[0] < 300], "list")
+    _check(triples(A.find_long_batch(hays)), [r for r in want if r[0] < 300], "list")
     # fixed strides: a power of two and not
     for stride in (64, 37):
         n_hay = 300
@@ -193,7 +189,7 @@ def test_long_kernel_matches_oracle(width, keyset):
         foff = np.arange(n_hay + 1, dtype=np.int64) * stride
         fw = O.iter_long_batch_letters(ft, foff)
         rows = _flat(width, ft).reshape(n_hay, stride * L)
-        _check(_records(A.find_long_batch(rows)), fw, f"stride {stride}")
+        _check(triples(A.find_long_batch(rows)), fw, f"stride {stride}")
 
 
 @pytest.mark.gpu
@@ -208,7 +204,7 @@ def test_long_kernel_long_haystack(width):
     t = _text(width, keys, rng, n + 200)
     off = np.array([0, 100, 100 + n, n + 200], dtype=np.int64)
     want = O.iter_long_batch_letters(t, off)
-    _check(_records(A.find_long_batch((_flat(width, t), off * L))), want, "3 MiB haystack")
+    _check(triples(A.find_long_batch((_flat(width, t), off * L))), want, "3 MiB haystack")
 
 
 def _stream(A):

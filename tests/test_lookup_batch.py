@@ -14,6 +14,7 @@ import pytest
 import emul_lookup
 import oracle
 import pyahocorasick_b200 as pkg
+from batch_cases import DT, fake_table, obj, skip_if_device
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200 import automaton as am
 
@@ -27,14 +28,6 @@ CASES = {
     "seq4": ("unicode", True, [0x61, 0x1F600, 0x10FFFF, 0x62], [0x00, 0x162, 0x7FFFFFFF]),
 }
 STORES = ["any", "ints", "length"]
-_DT = {1: np.uint8, 2: "<u2", 4: "<u4"}
-
-
-def _obj(case, letters):
-    fl, seq = CASES[case][:2]
-    if seq:
-        return tuple(letters)
-    return bytes(letters) if fl == "bytes" else "".join(map(chr, letters))
 
 
 def _add(A, store, k, i):
@@ -86,8 +79,8 @@ def _queries(case, keys, rng):
 
 def _forms(case, A, queries):
     """every input form the batch methods take (list, (flat, offsets), and uint8[n, stride] for equal lengths)"""
-    yield "list", [_obj(case, x) for x in queries]
-    parts = [np.asarray(x, dtype=_DT[A._L]).view(np.uint8) for x in queries]
+    yield "list", [obj(*CASES[case][:2], x) for x in queries]
+    parts = [np.asarray(x, dtype=DT[A._L]).view(np.uint8) for x in queries]
     offs = np.zeros(len(parts) + 1, dtype=np.int64)
     np.cumsum([p.size for p in parts], out=offs[1:])
     yield "flat", (np.concatenate(parts) if parts else np.empty(0, np.uint8), offs)
@@ -96,7 +89,7 @@ def _forms(case, A, queries):
 
 
 def _check(A, R, case, queries):
-    objs = [_obj(case, x) for x in queries]
+    objs = [obj(*CASES[case][:2], x) for x in queries]
     want = dict(exists=[A.exists(k) for k in objs], match=[A.match(k) for k in objs],
                 lp=[A.longest_prefix(k) for k in objs], get=[A.get(k, "dflt") for k in objs])
     if R is not None:
@@ -125,7 +118,7 @@ def _fuzz(case, store, seed, trials):
         for i, k in enumerate(keys):
             for X in (A, R):
                 if X is not None:
-                    _add(X, store, _obj(case, k), i)
+                    _add(X, store, obj(*CASES[case][:2], k), i)
             live[tuple(k)] = i
         for X in (A, R):
             if X is not None:
@@ -138,11 +131,11 @@ def _fuzz(case, store, seed, trials):
             for k in keys[:len(keys) // 2]:
                 for X in (A, R):
                     if X is not None:
-                        X.remove_word(_obj(case, k))
+                        X.remove_word(obj(*CASES[case][:2], k))
             back = keys[0]
             for X in (A, R):
                 if X is not None:
-                    _add(X, store, _obj(case, back), 99)
+                    _add(X, store, obj(*CASES[case][:2], back), 99)
         elif op == 1:
             for X in (A, R):
                 if X is not None:
@@ -151,11 +144,11 @@ def _fuzz(case, store, seed, trials):
             for i, k in enumerate(keys):
                 for X in (A, R):
                     if X is not None:
-                        _add(X, store, _obj(case, k), 50 + i)
+                        _add(X, store, obj(*CASES[case][:2], k), 50 + i)
         else:
             for X in (A, R):
                 if X is not None:
-                    _add(X, store, _obj(case, keys[-1]), 77)
+                    _add(X, store, obj(*CASES[case][:2], keys[-1]), 77)
         for X in (A, R):
             if X is not None:
                 X.make_automaton()
@@ -181,9 +174,9 @@ def _root_only(case, store):
     A, _ = _pair(case, store, with_ref=False)
     al = CASES[case][2]
     for i, k in enumerate(([al[0]], [al[0], al[1]])):
-        _add(A, store, _obj(case, k), i)
+        _add(A, store, obj(*CASES[case][:2], k), i)
     for k in ([al[0]], [al[0], al[1]]):
-        A.remove_word(_obj(case, k))
+        A.remove_word(obj(*CASES[case][:2], k))
     A.make_automaton()
     assert A.kind == pkg.AHOCORASICK and A.flat()["n_states"] == 1
     _check(A, None, case, [[], [al[0]], [al[0], al[1]], [], [CASES[case][3][0]]])
@@ -296,11 +289,9 @@ def test_str_lists_take_one_join_with_the_bytes_of_the_per_item_path():
 
 
 def test_lookup_host_fails_loudly_without_a_device():
-    import torch
-    if torch.cuda.is_available():
-        pytest.skip("a device is present")
+    skip_if_device()
     L = N.lib()
-    fake = ctypes.create_string_buffer(1 << 16)           # zeroed: device 0, and no device to select
+    fake = fake_table()                                   # device 0, and no device to select
     keys = np.frombuffer(b"abcd", dtype=np.uint8)
     offs = np.array([0, 2, 4], dtype=np.int64)
     kid, pre = np.empty(2, np.int32), np.empty(2, np.int32)
@@ -413,9 +404,9 @@ def test_cuda_tensors_on_a_side_stream(fl):
     letters = [0x61, 0x62, 0x163] if fl == "unicode" else [0x61, 0x62]
     keys = {tuple(int(x) for x in rng.choice(letters[:2], size=int(rng.integers(1, 4)))) for _ in range(12)}
     for i, k in enumerate(sorted(keys)):
-        A.add_word(_obj("unicode" if fl == "unicode" else "bytes", list(k)), i)
+        A.add_word(obj(fl, False, list(k)), i)
     A.make_automaton()
-    rows = rng.choice(letters, size=(2001, 7 if L == 1 else 2)).astype(_DT[L])
+    rows = rng.choice(letters, size=(2001, 7 if L == 1 else 2)).astype(DT[L])
     host = np.ascontiguousarray(rows.view(np.uint8).reshape(2001, -1))
     d = torch.from_numpy(host).cuda()
     views = {"whole": (d, host), "misaligned": (d[1:], host[1:])}

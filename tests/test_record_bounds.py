@@ -23,7 +23,8 @@ import oracle
 import pyahocorasick_b200 as ac
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200 import synth
-from test_kernel_matrix import TILE, SLICE, Cell, _build, _check_shape, _dense, _keys, _seed
+from batch_cases import triples
+from kernel_cells import TILE, SLICE, Cell, _big_batch, _build, _check_shape, _dense, _keys, _seed
 
 GUARD = 64
 MiB = 1 << 20
@@ -219,17 +220,6 @@ def test_scan_host_overflow_is_exact_monolithic(kernel, monkeypatch):
     _check_host_bounds(A, algo, t, off, want)
 
 
-def _big_batch(rng, keys, n):
-    """n bytes of text in no key's letters with keys planted every few KiB, cut into a ragged batch"""
-    flat = rng.choice(np.frombuffer(b"#%&*+-", dtype=np.uint8), size=n)
-    for i, b in enumerate(range(100, n - 64, 4093)):
-        k = keys[i % len(keys)]
-        flat[b:b + len(k)] = np.frombuffer(k, dtype=np.uint8)
-    cuts = np.sort(rng.integers(0, n, size=600))
-    off = np.concatenate([[0, 0], cuts, [32 * MiB] * 3, [n, n]]).astype(np.int64)
-    return flat, np.sort(off)
-
-
 @pytest.mark.gpu
 def test_scan_host_overflow_is_exact_pipelined():
     """64 MiB: the host scan runs as a pipeline over 32 MiB chunks, each sorted by itself"""
@@ -248,7 +238,7 @@ def test_scan_host_overflow_is_exact_pipelined():
     fresh = synth.build_automaton(keys)                                     # 4096 records: the first attempt overflows
     m = fresh.find_all_batch((flat, off))
     assert fresh._match_cap > 4096
-    assert list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist())) == want
+    assert triples(m) == want
 
 
 # ------------------------------------------------------------------ the record sort, called directly
@@ -365,7 +355,7 @@ def test_sort_key_width_selects_the_host_route(log_len):
     m = A.find_all_batch((flat, off), algo="filter")
     launches = lib.acb_launch_count() - before
     assert launches == (8 if log_len == 19 else 1)          # 4 chunks: scan + sort each / one scan, sorted on the host
-    got = list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist()))
+    got = triples(m)
     assert got == want
 
 
@@ -387,4 +377,4 @@ def test_device_tensor_entry_sorts_on_the_host_when_the_device_sort_refuses(monk
     monkeypatch.setattr(N.lib(), "acb_sort_matches_device", refuse)
     m = A.find_all_batch(torch.from_numpy(rows).cuda())
     assert calls == [len(want)]
-    assert list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist())) == want
+    assert triples(m) == want

@@ -12,61 +12,31 @@ import pytest
 import emul_leftmost
 import emul_replace
 import pyahocorasick_b200 as pkg
+from batch_cases import (CASES, DT, NESTED, automaton, fake_table, forms, layout, leftmost_random_case,
+                         leftmost_structured_cases, obj, oracle_full, replace_reps, rows, skip_if_device, split,
+                         table_and_batch)
 from pyahocorasick_b200 import _native as N
-from test_leftmost_longest import CASES, NESTED, _automaton, _forms, _full, _obj, _random_case, _structured_cases
 
 TILES = [1, 3, 16, 64]
 WIDTH = {"bytes": 1, "latin1": 1, "wide": 4, "mixed": 4, "seq2": 2, "seq4": 4}
 
 
-def _reps(case, keys, rng):
-    """a replacement per key: empty, shorter, equal (the key itself), longer, or text that holds other keys"""
-    al = CASES[case][2]
-    out = []
-    for k in keys:
-        r = int(rng.integers(0, 5))
-        if r == 0:
-            out.append([])
-        elif r == 1:
-            out.append(list(k[: max(len(k) - 1, 0)]))
-        elif r == 2:
-            out.append(list(k))
-        elif r == 3:
-            out.append([int(x) for x in rng.choice(al, size=len(k) + int(rng.integers(1, 5)))])
-        else:
-            out.append(list(keys[int(rng.integers(0, len(keys)))]) * 2)
-    return out
-
-
 def _want(O, keys, hays, reps, case="bytes"):
     """per haystack, the definition over the selection's definition over the oracle's full list"""
     chosen = [[] for _ in hays]
-    for h, e, k in emul_leftmost.greedy(_full(O, hays, case), [len(k) for k in keys]):
+    for h, e, k in emul_leftmost.greedy(oracle_full(O, hays, case), [len(k) for k in keys]):
         chosen[h].append((e, k))
     return [emul_replace.definition(h, c, [len(k) for k in keys], reps) for h, c in zip(hays, chosen)]
 
 
-def _layout(seqs, width):
-    dt = {1: np.uint8, 2: "<u2", 4: "<u4"}[width]
-    parts = [np.asarray(s, dtype=dt).view(np.uint8) for s in seqs]
-    offs = np.zeros(len(parts) + 1, dtype=np.int64)
-    np.cumsum([p.size for p in parts], out=offs[1:])
-    return (np.concatenate(parts) if parts else np.empty(0, np.uint8)), offs
-
-
-def _split(out, offs, width):
-    dt = {1: np.uint8, 2: "<u2", 4: "<u4"}[width]
-    return [np.asarray(out[offs[i]:offs[i + 1]]).view(dt).tolist() for i in range(len(offs) - 1)]
-
-
 def _restated(O, keys, hays, reps, case, tile):
     w = WIDTH[case]
-    flat, offs = _layout(hays, w)
+    flat, offs = layout(hays, w)
     kl = np.array([len(k) for k in keys])
-    chosen = np.array(emul_leftmost.greedy(_full(O, hays, case), kl), dtype=np.int64).reshape(-1, 3)
-    rep, rep_off = _layout(reps, w)
+    chosen = np.array(emul_leftmost.greedy(oracle_full(O, hays, case), kl), dtype=np.int64).reshape(-1, 3)
+    rep, rep_off = layout(reps, w)
     out, out_off = emul_replace.replace(flat, offs, chosen, kl, rep, rep_off, w, tile)
-    return _split(out, out_off, w)
+    return split(out, out_off, w)
 
 
 # ------------------------------------------------------------------ the restatement against the definition (CPU)
@@ -78,14 +48,14 @@ def _structured_reps(keys):
 @pytest.mark.parametrize("tile", TILES)
 def test_restatement_equals_the_definition_on_the_oracle(tile):
     rng = np.random.default_rng(tile)
-    for case in CASES:
+    for case, (fl, seq, _) in CASES.items():
         for _ in range(10):
-            keys, hays = _random_case(case, rng)
-            _, O = _automaton(case, keys)
-            reps = _reps(case, keys, rng)
+            keys, hays = leftmost_random_case(case, rng)
+            _, O = automaton(fl, seq, keys)
+            reps = replace_reps(case, keys, rng)
             assert _restated(O, keys, hays, reps, case, tile) == _want(O, keys, hays, reps, case), (case, keys, hays, reps)
-    for keys, hays in list(_structured_cases()) + [(NESTED, [[0x61] * 100, [], [], [0x62] * 40, [0x61, 0x62] * 30])]:
-        _, O = _automaton("bytes", keys)
+    for keys, hays in list(leftmost_structured_cases()) + [(NESTED, [[0x61] * 100, [], [], [0x62] * 40, [0x61, 0x62] * 30])]:
+        _, O = automaton("bytes", False, keys)
         reps = _structured_reps(keys)[:len(keys)]
         assert _restated(O, keys, hays, reps, "bytes", tile) == _want(O, keys, hays, reps)
 
@@ -95,27 +65,26 @@ def test_python_layer_on_the_restatement(monkeypatch, tile):
     """every input form, the mapping mode on STORE_INTS, the values mode on STORE_ANY"""
     emul_replace.install(monkeypatch, tile)
     rng = np.random.default_rng(30 + tile)
-    for case in CASES:
-        fl, seq, _ = CASES[case]
+    for case, (fl, seq, _) in CASES.items():
         for _ in range(4):
-            keys, hays = _random_case(case, rng)
-            A, O = _automaton(case, keys)
-            reps = _reps(case, keys, rng)
+            keys, hays = leftmost_random_case(case, rng)
+            A, O = automaton(fl, seq, keys)
+            reps = replace_reps(case, keys, rng)
             want = _want(O, keys, hays, reps, case)
-            R = A.replacer({_obj(case, k): _obj(case, r) for k, r in zip(keys, reps)})
-            for form, batch in _forms(case, A, hays):
+            R = A.replacer({obj(fl, seq, k): obj(fl, seq, r) for k, r in zip(keys, reps)})
+            for form, batch in forms([obj(fl, seq, h) for h in hays], hays, A._L, case in ("latin1", "mixed")):
                 got = R.replace_batch(batch)
                 if form == "list":
-                    assert got == [_obj(case, h) for h in want], (case, form)
+                    assert got == [obj(fl, seq, h) for h in want], (case, form)
                 else:
                     out, offs = got
-                    assert offs.dtype == np.int64 and _split(out, offs, A._L) == want, (case, form)
+                    assert offs.dtype == np.int64 and split(out, offs, A._L) == want, (case, form)
             mod = pkg.flavour(fl)
             B = mod.Automaton(mod.STORE_ANY, mod.KEY_SEQUENCE) if seq else mod.Automaton(mod.STORE_ANY)
             for k, r in zip(keys, reps):
-                B.add_word(_obj(case, k), _obj(case, r))
+                B.add_word(obj(fl, seq, k), obj(fl, seq, r))
             B.make_automaton()
-            assert B.replacer().replace_batch([_obj(case, h) for h in hays]) == [_obj(case, h) for h in want], case
+            assert B.replacer().replace_batch([obj(fl, seq, h) for h in hays]) == [obj(fl, seq, h) for h in want], case
 
 
 def test_latin1_table_only_when_every_replacement_is_latin1(monkeypatch):
@@ -202,29 +171,21 @@ def test_every_key_removed_gives_the_input(monkeypatch):
     assert A.replacer().replace_batch(hays) == hays
 
 
-def _fake_table(L):
-    """a zeroed stand-in for acb_table (device 0) with the letter width set: acb_table starts with int device, int
-    sm_count, int32 S, K, L"""
-    fake = ctypes.create_string_buffer(1 << 16)
-    ctypes.c_int32.from_buffer(fake, 16).value = L
-    return fake
-
-
 def test_c_entries_check_arguments_first():
     L = N.lib()
-    tb = _fake_table(1)
+    tb = fake_table(1)
     rep = np.frombuffer(b"xyz", dtype=np.uint8)
     r = ctypes.c_void_p()
     bad_offsets = ([1, 3], [0, 2], [0, 4], [0, 2, 1, 3])
     assert L.acb_replacer_new(None, N.ptr(rep), 3, N.ptr(np.array([0, 3], np.int64)), 1, ctypes.byref(r)) == N.ACB_EINVAL
-    assert L.acb_replacer_new(ctypes.addressof(_fake_table(0)), N.ptr(rep), 3, N.ptr(np.array([0, 3], np.int64)), 1,
+    assert L.acb_replacer_new(ctypes.addressof(fake_table(0)), N.ptr(rep), 3, N.ptr(np.array([0, 3], np.int64)), 1,
                               ctypes.byref(r)) == N.ACB_EINVAL
     for offs in bad_offsets:
         o = np.array(offs, dtype=np.int64)
         assert L.acb_replacer_new(ctypes.addressof(tb), N.ptr(rep), 3, N.ptr(o), len(o) - 1, ctypes.byref(r)) == N.ACB_EINVAL, offs
     o = np.array([0, 2, 4], np.int64)
-    assert L.acb_replacer_new(ctypes.addressof(_fake_table(2)), N.ptr(rep), 3, N.ptr(o), 2, ctypes.byref(r)) == N.ACB_EINVAL
-    fake_r = _fake_table(0)                                     # a zeroed replacer: letter width 0 does not fit the table
+    assert L.acb_replacer_new(ctypes.addressof(fake_table(2)), N.ptr(rep), 3, N.ptr(o), 2, ctypes.byref(r)) == N.ACB_EINVAL
+    fake_r = fake_table(0)                                     # a zeroed replacer: letter width 0 does not fit the table
     hay = np.zeros(32, dtype=np.uint8)
     offs = np.array([0, 16, 32], np.int64)
     out_offs = np.zeros(3, np.int64)
@@ -240,10 +201,8 @@ def test_c_entries_check_arguments_first():
 
 
 def test_c_entries_fail_loudly_without_a_device():
-    import torch
-    if torch.cuda.is_available():
-        pytest.skip("a device is present")
-    tb = _fake_table(1)
+    skip_if_device()
+    tb = fake_table(1)
     rep = np.frombuffer(b"xyz", dtype=np.uint8)
     r = ctypes.c_void_p()
     assert N.lib().acb_replacer_new(ctypes.addressof(tb), N.ptr(rep), 3, N.ptr(np.array([0, 3], np.int64)), 1,
@@ -256,21 +215,21 @@ def test_c_entries_fail_loudly_without_a_device():
 @pytest.mark.parametrize("algo", ["filter", "dfa"])
 def test_gpu_fuzz_against_the_definition(algo):
     rng = np.random.default_rng(41)
-    for case in CASES:
+    for case, (fl, seq, _) in CASES.items():
         for _ in range(6):
-            keys, hays = _random_case(case, rng)
-            A, O = _automaton(case, keys)
-            reps = _reps(case, keys, rng)
+            keys, hays = leftmost_random_case(case, rng)
+            A, O = automaton(fl, seq, keys)
+            reps = replace_reps(case, keys, rng)
             want = _want(O, keys, hays, reps, case)
-            R = A.replacer({_obj(case, k): _obj(case, r) for k, r in zip(keys, reps)})
-            for form, batch in _forms(case, A, hays):
+            R = A.replacer({obj(fl, seq, k): obj(fl, seq, r) for k, r in zip(keys, reps)})
+            for form, batch in forms([obj(fl, seq, h) for h in hays], hays, A._L, case in ("latin1", "mixed")):
                 got = R.replace_batch(batch, algo=algo)
                 if form == "list":
-                    assert got == [_obj(case, h) for h in want], (case, form, keys, hays)
+                    assert got == [obj(fl, seq, h) for h in want], (case, form, keys, hays)
                 else:
-                    assert _split(*got, A._L) == want, (case, form)
-    for keys, hays in _structured_cases():
-        A, O = _automaton("bytes", keys)
+                    assert split(*got, A._L) == want, (case, form)
+    for keys, hays in leftmost_structured_cases():
+        A, O = automaton("bytes", False, keys)
         reps = _structured_reps(keys)[:len(keys)]
         R = A.replacer({bytes(k): bytes(r) for k, r in zip(keys, reps)})
         assert R.replace_batch([bytes(h) for h in hays], algo=algo) == [bytes(h) for h in _want(O, keys, hays, reps)]
@@ -297,16 +256,12 @@ def _np_replace(flat, in_off, chosen, key_len, rep, rep_off):
     return out, pos[in_off]
 
 
-def _rec(m):
-    return np.stack([m.hay_id.astype(np.int64), m.end_index.astype(np.int64), m.key_id.astype(np.int64)], axis=1)
-
-
 def _check_batch(A, table, flat, offs, tensor=None):
     """replace_batch from the host pair (and from a CUDA tensor) against _np_replace over the selection's records"""
     import torch
     kl = np.asarray(A.flat()["key_len"], dtype=np.int64)
     rep, rep_off = emul_replace_layout(A, table)
-    chosen = _rec(A.find_leftmost_longest_batch((flat, offs)))
+    chosen = rows(A.find_leftmost_longest_batch((flat, offs)))
     want, want_off = _np_replace(flat, offs, chosen, kl, rep, rep_off)
     R = A.replacer(table)
     out, out_off = R.replace_batch((flat, offs))
@@ -357,7 +312,7 @@ def test_gpu_tile_and_segment_boundaries():
     haystacks across a tile"""
     rng = np.random.default_rng(12)
     keys = [bytes([0x41 + i]) * (i + 1) for i in range(33)] + [b"#big#"]
-    A, _ = _automaton("bytes", [list(k) for k in keys])
+    A, _ = automaton("bytes", False, keys)
     table = {k: bytes(rng.integers(0x61, 0x7B, size=int(rng.integers(0, 34)), dtype=np.uint8)) for k in keys[:33]}
     table[keys[0]] = b""
     table[b"#big#"] = bytes(rng.integers(0, 256, size=200 << 10, dtype=np.uint8))
@@ -375,7 +330,7 @@ def test_gpu_output_past_2_gib():
     """a CUDA batch whose output passes 2^31 bytes (32 x 4 MiB of 'ab' -> 40 bytes each), and one haystack whose own
     output does (64 MiB of 'ab' -> 72 bytes each); checked on the device"""
     import torch
-    A, _ = _automaton("bytes", [list(b"ab"), list(b"zz")])
+    A, _ = automaton("bytes", False, [list(b"ab"), list(b"zz")])
     for rows, stride, rl in ((32, 4 << 20, 40), (1, 64 << 20, 72)):
         rep = bytes(range(1, rl + 1))
         d = torch.tensor(list(b"ab"), dtype=torch.uint8, device="cuda").repeat(rows * stride // 2).view(rows, stride)
@@ -392,17 +347,14 @@ def test_gpu_output_past_2_gib():
 def test_gpu_capacity_contract():
     import torch
     keys = [b"ab", b"b", b"abc"]
-    A, _ = _automaton("bytes", [list(k) for k in keys])
+    A, _ = automaton("bytes", False, keys)
     table = {b"ab": b"XYZW", b"b": b"", b"abc": b"q"}
     hays = [b"abcabxbab" * 20, b"", b"bbbb", b"zzz"]
-    flat = np.frombuffer(b"".join(hays), dtype=np.uint8)
-    offs = np.zeros(len(hays) + 1, dtype=np.int64)
-    np.cumsum([len(h) for h in hays], out=offs[1:])
+    tb, flat, offs = table_and_batch(A, hays)
     want, want_off = _check_batch(A, table, flat, offs)
     total = int(want_off[-1])
     L = N.lib()
     R = A.replacer(table)
-    tb = A._ensure_table(0)
     r = R._replacer(tb, False, 0)
     got_off = np.zeros(len(hays) + 1, dtype=np.int64)
     t = ctypes.c_int64(0)
@@ -418,7 +370,7 @@ def test_gpu_capacity_contract():
     # the device entry, on records the selection left on the device
     d = torch.from_numpy(flat.copy()).cuda()
     d_off = torch.from_numpy(offs).cuda()
-    chosen = torch.from_numpy(_rec(A.find_leftmost_longest_batch((flat, offs))).astype(np.int32)).cuda()
+    chosen = torch.from_numpy(rows(A.find_leftmost_longest_batch((flat, offs))).astype(np.int32)).cuda()
     n = torch.tensor([chosen.shape[0]], dtype=torch.int64, device="cuda")
     s = torch.cuda.current_stream().cuda_stream
     for cap in (0, total - 1, total):
@@ -445,11 +397,11 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
     case = "bytes" if fl == "bytes" else "wide"
     al = CASES[case][2]
     keys = sorted({tuple(int(x) for x in rng.choice(al[:2], size=int(rng.integers(1, 5)))) for _ in range(10)})
-    A, O = _automaton(case, keys)
-    reps = _reps(case, keys, rng)
-    R = A.replacer({_obj(case, k): _obj(case, r) for k, r in zip(keys, reps)})
+    A, O = automaton(*CASES[case][:2], keys)
+    reps = replace_reps(case, keys, rng)
+    R = A.replacer({obj(*CASES[case][:2], k): obj(*CASES[case][:2], r) for k, r in zip(keys, reps)})
     hays = [[int(x) for x in rng.choice(al, size=7)] for _ in range(300)]
-    host = np.stack([np.asarray(h, dtype={1: np.uint8, 4: "<u4"}[A._L]).view(np.uint8) for h in hays])
+    host = np.stack([np.asarray(h, dtype=DT[A._L]).view(np.uint8) for h in hays])
     d = torch.from_numpy(host).cuda()
     views = {"whole": (d, hays)}
     if A._L == 1:
@@ -461,4 +413,4 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
         with torch.cuda.stream(side):
             out, offs = R.replace_batch(t)
         side.synchronize()
-        assert _split(out.cpu().numpy(), offs.cpu().numpy(), A._L) == _want(O, keys, hs, reps, case), name
+        assert split(out.cpu().numpy(), offs.cpu().numpy(), A._L) == _want(O, keys, hs, reps, case), name

@@ -16,6 +16,7 @@ import pytest
 import emul_select
 import oracle
 import pyahocorasick_b200 as pkg
+from batch_cases import DT, fake_table, obj, skip_if_device
 from pyahocorasick_b200 import _native as N
 
 EXACT, AT_MOST, AT_LEAST = pkg.MATCH_EXACT_LENGTH, pkg.MATCH_AT_MOST_PREFIX, pkg.MATCH_AT_LEAST_PREFIX
@@ -30,14 +31,6 @@ CASES = {
     "seq4": ("unicode", True, [0x61, 0x1F600, 0x10FFFF, 0x62], [0x00, 0x162, 0x7FFFFFFF]),
 }
 STORES = ["any", "ints", "length"]
-_DT = {1: np.uint8, 2: "<u2", 4: "<u4"}
-
-
-def _obj(case, letters):
-    fl, seq = CASES[case][:2]
-    if seq:
-        return tuple(letters)
-    return bytes(letters) if fl == "bytes" else "".join(map(chr, letters))
 
 
 def _add(A, store, k, i):
@@ -95,8 +88,8 @@ def _patterns(case, keys, rng, w):
 
 def _forms(case, A, patterns):
     """every input form the batch methods take (list, (flat, offsets), and uint8[n, stride] for equal lengths)"""
-    yield "list", [_obj(case, x) for x in patterns]
-    parts = [np.asarray(x, dtype=_DT[A._L]).view(np.uint8) for x in patterns]
+    yield "list", [obj(*CASES[case][:2], x) for x in patterns]
+    parts = [np.asarray(x, dtype=DT[A._L]).view(np.uint8) for x in patterns]
     offs = np.zeros(len(parts) + 1, dtype=np.int64)
     np.cumsum([p.size for p in parts], out=offs[1:])
     yield "flat", (np.concatenate(parts) if parts else np.empty(0, np.uint8), offs)
@@ -114,11 +107,11 @@ def _rows(case, A, x):
         raw = [flat[offs[i]:offs[i + 1]].tobytes() for i in range(len(offs) - 1)]
     else:
         raw = [r.tobytes() for r in x]
-    return [_obj(case, np.frombuffer(r, dtype=_DT[A._L]).tolist()) for r in raw]
+    return [obj(*CASES[case][:2], np.frombuffer(r, dtype=DT[A._L]).tolist()) for r in raw]
 
 
 def _check(A, R, case, patterns, w, how):
-    wobj = None if w is None else _obj(case, [w])
+    wobj = None if w is None else obj(*CASES[case][:2], [w])
     for form, x in _forms(case, A, patterns):
         objs = _rows(case, A, x)
         want_k = [list(A.keys(p, wobj, how)) for p in objs]
@@ -157,7 +150,7 @@ def _fuzz(case, store, seed, trials):
         for i, k in enumerate(keys):
             for X in (A, R):
                 if X is not None:
-                    _add(X, store, _obj(case, k), i)
+                    _add(X, store, obj(*CASES[case][:2], k), i)
         for X in (A, R):
             if X is not None:
                 X.make_automaton()
@@ -168,11 +161,11 @@ def _fuzz(case, store, seed, trials):
             for k in gone:
                 for X in (A, R):
                     if X is not None:
-                        X.remove_word(_obj(case, k))
+                        X.remove_word(obj(*CASES[case][:2], k))
             for k in gone[::-1][:2]:
                 for X in (A, R):
                     if X is not None:
-                        _add(X, store, _obj(case, k), 90)
+                        _add(X, store, obj(*CASES[case][:2], k), 90)
             keys = keys[len(keys) // 2:] + gone[::-1][:2]
         for X in (A, R):
             if X is not None:
@@ -202,11 +195,11 @@ def test_key_ranges_restate_the_key_order(case):
     A, _ = _pair(case, "ints", with_ref=False)
     keys = _random_keys(case, rng) + _random_keys(case, rng)
     for i, k in enumerate(keys):
-        _add(A, "ints", _obj(case, k), i)
+        _add(A, "ints", obj(*CASES[case][:2], k), i)
     for k in keys[::3]:
-        A.remove_word(_obj(case, k))
+        A.remove_word(obj(*CASES[case][:2], k))
     for k in keys[::6]:
-        _add(A, "ints", _obj(case, k), 5)
+        _add(A, "ints", obj(*CASES[case][:2], k), 5)
     A.make_automaton()
     f, kr = A.flat(), A.key_ranges()
     want = [A._key_ids[k] for k in A.keys()]
@@ -286,11 +279,9 @@ def test_wrong_arguments_raise_the_per_key_errors(fl, seq, good, bad, wild, bad_
 
 
 def test_select_host_fails_loudly_without_a_device():
-    import torch
-    if torch.cuda.is_available():
-        pytest.skip("a device is present")
+    skip_if_device()
     L = N.lib()
-    fake = ctypes.create_string_buffer(1 << 16)
+    fake = fake_table()
     pats = np.frombuffer(b"abcd", dtype=np.uint8)
     offs = np.array([0, 2, 4], dtype=np.int64)
     out = np.empty(3, np.int64)
@@ -403,7 +394,7 @@ def test_cuda_tensors_on_a_side_stream(fl):
     for i, k in enumerate(sorted(keys)):
         A.add_word(bytes(k) if L == 1 else "".join(map(chr, k)), i)
     A.make_automaton()
-    rows = rng.choice(letters, size=(3001, 3)).astype(_DT[L])
+    rows = rng.choice(letters, size=(3001, 3)).astype(DT[L])
     host = np.ascontiguousarray(rows.view(np.uint8).reshape(3001, -1))
     d = torch.from_numpy(host).cuda()
     w = b"?" if L == 1 else "?"

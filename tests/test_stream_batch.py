@@ -11,40 +11,12 @@ import pytest
 
 import emul
 import emul_streams
-import oracle
 import pyahocorasick_b200 as pkg
+from batch_cases import automaton, got_values, obj, triples
 from pyahocorasick_b200 import _native as N
 
 # (flavour, key type): 1-, 2- and 4-byte letters
 KINDS = {"bytes": ("bytes", False), "seq": ("bytes", True), "unicode": ("unicode", False)}
-
-
-def _text(kind, letters):
-    if kind == "bytes":
-        return bytes(letters)
-    if kind == "seq":
-        return tuple(letters)
-    return "".join(map(chr, letters))
-
-
-def _automaton(kind, keys, mp=None, env=None, tagmap=False):
-    fl, seq = KINDS[kind]
-    mod = pkg.flavour(fl)
-    A = mod.Automaton(mod.STORE_INTS, mod.KEY_SEQUENCE) if seq else mod.Automaton(mod.STORE_INTS)
-    O = oracle.OracleAutomaton()
-    for i, k in enumerate(keys):
-        A.add_word(_text(kind, k), i)
-        O.add_word(_text(kind, k), i)
-    if env is None:
-        A.make_automaton()
-    else:
-        with mp.context() as m:
-            m.setenv("ACB_FILTER", env)
-            if tagmap:
-                m.setenv("ACB_FORCE_TAGMAP", "1")
-            A.make_automaton()
-    O.make_automaton()
-    return A, O
 
 
 ALPHA = {"bytes": [0x61, 0x62, 0x63], "seq": [0x61, 0x6162, 0xFFFF], "unicode": [0x61, 0x142, 0x1F600]}
@@ -75,15 +47,15 @@ def _run(A, O, kind, rng, n_streams, n_feeds, algo="auto"):
             ids = None
         sel = list(range(n_streams)) if ids is None else ids.tolist()
         chunks = [_chunk(kind, rng, T) for _ in sel]
-        m = S.feed([_text(kind, c) if c or rng.integers(0, 2) else None for c in chunks], ids)
+        m = S.feed([obj(*KINDS[kind], c) if c or rng.integers(0, 2) else None for c in chunks], ids)
         want = []
         for s, c in zip(sel, chunks):
             before = len(hist[s])
             hist[s] += c
-            for e, v in O.find_all(_text(kind, hist[s])) or []:
+            for e, v in O.find_all(obj(*KINDS[kind], hist[s])) or []:
                 if e >= before:
                     want.append((s, e, v))
-        got = list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist()))
+        got = triples(m)
         assert got == want
         assert S.positions.tolist() == [len(h) for h in hist]
     return S, hist
@@ -94,7 +66,7 @@ def _differential(kind, seed, n_streams, trials, algo="auto"):
     rng = np.random.default_rng(seed)
     for t in range(trials):
         hi = 1 if t == 0 else 20                                # T = 0 once
-        A, O = _automaton(kind, _keys(kind, rng, hi=hi))
+        A, O = automaton(*KINDS[kind], _keys(kind, rng, hi=hi))
         _run(A, O, kind, rng, n_streams, 6, algo=algo)
 
 
@@ -124,7 +96,7 @@ def test_streams_on_forced_filter_shapes_gpu(kind, env, tagmap, monkeypatch):
     L = 4 if kind == "unicode" else 1
     m = (g + s - L) // L                                        # the shortest key: the forced gram is the longest it allows
     keys = _keys(kind, rng, lo=m, hi=20) + [tuple([ALPHA[kind][1]] * m)]
-    A, O = _automaton(kind, sorted(set(keys)), monkeypatch, env, tagmap)
+    A, O = automaton(*KINDS[kind], sorted(set(keys)), monkeypatch, env, tagmap)
     fs = A.filter_shape()
     assert (fs["gram_bytes"], fs["stride"]) == (g, s) and bool(fs["filter_flags"] & emul.FILTER_PAIR) == env.endswith(",1")
     assert bool(fs["log2_bits3"]) == tagmap
@@ -135,7 +107,7 @@ def test_streams_equal_iter_set_chain_emulated(monkeypatch):
     """long=False is the reference's iter(c0) run to exhaustion, then set(c1), ... (the C oracle's iterator)"""
     emul_streams.install(monkeypatch)
     rng = np.random.default_rng(5)
-    A, O = _automaton("bytes", _keys("bytes", rng, hi=7))
+    A, O = automaton("bytes", False, _keys("bytes", rng, hi=7))
     S = A.stream_batch(3)
     its, got, want = [None] * 3, [[] for _ in range(3)], [[] for _ in range(3)]
     for _ in range(8):
@@ -158,7 +130,7 @@ def _planted(seed, residues, n_keys_extra):
     rng = np.random.default_rng(seed)
     key = b"qrstuvwxyzQR"
     keys = [tuple(key)] + [tuple(rng.integers(0x61, 0x65, size=int(rng.integers(5, 13))).tolist()) for _ in range(n_keys_extra)]
-    A, O = _automaton("bytes", keys)
+    A, O = automaton("bytes", False, keys)
     cases = [(r, j) for r in range(residues) for j in range(1, len(key))]
     S = A.stream_batch(len(cases))
     m0 = S.feed([b"0" * r + key[:j] for r, j in cases])
@@ -184,12 +156,12 @@ def _long_chain(kind, seed, n_streams, trials):
     """long=True: stream s equals the drop-in's own iter_long(c0) -> exhaust -> set(c1) chain"""
     rng = np.random.default_rng(seed)
     for _ in range(trials):
-        A, O = _automaton(kind, _keys(kind, rng, hi=8))
+        A, O = automaton(*KINDS[kind], _keys(kind, rng, hi=8))
         S = A.stream_batch(n_streams, long=True)
         its = [None] * n_streams
         for _ in range(6):
             ids = rng.permutation(n_streams)[:int(rng.integers(1, n_streams + 1))]
-            chunks = [_text(kind, _chunk(kind, rng, 6)) for _ in ids]
+            chunks = [obj(*KINDS[kind], _chunk(kind, rng, 6)) for _ in ids]
             m = S.feed(chunks, ids)
             want = []
             for s, c in zip(ids.tolist(), chunks):
@@ -198,7 +170,7 @@ def _long_chain(kind, seed, n_streams, trials):
                 else:
                     its[s].set(c)
                 want += [(s, e, v) for e, v in its[s]]
-            assert list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.values())) == want
+            assert got_values(m) == want
 
 
 @pytest.mark.parametrize("kind", list(KINDS))
@@ -217,7 +189,7 @@ def test_long_streams_equal_iter_long_set_gpu(kind):
 # ------------------------------------------------------------------ reset, key-set changes, independence
 def _reset_and_independence():
     rng = np.random.default_rng(8)
-    A, O = _automaton("bytes", _keys("bytes", rng, hi=6))
+    A, O = automaton("bytes", False, _keys("bytes", rng, hi=6))
     S1, S2 = A.stream_batch(4), A.stream_batch(4)
     S1.feed([b"abcab", b"ca", b"", b"bbb"])
     S1.reset([1, 3])
@@ -250,7 +222,7 @@ def test_reset_independence_and_key_set_change_gpu():
 
 def test_argument_errors(monkeypatch):
     emul_streams.install(monkeypatch)
-    A, _ = _automaton("bytes", [tuple(b"ab")])
+    A, _ = automaton("bytes", False, [tuple(b"ab")])
     S = A.stream_batch(3)
     with pytest.raises(ValueError):
         S.feed([b"a", b"b"], [1, 1])                            # duplicate
@@ -263,7 +235,7 @@ def test_argument_errors(monkeypatch):
     with pytest.raises(ValueError):
         S.feed([b"a", b"b"], [0])                               # one id per chunk
     assert S.positions.tolist() == [0, 0, 0]                    # nothing ran
-    U, _ = _automaton("unicode", [tuple(b"ab")])
+    U, _ = automaton("unicode", False, [tuple(b"ab")])
     with pytest.raises(ValueError, match="multiple of the letter width"):
         U.stream_batch(2).feed(np.zeros((2, 6), dtype=np.uint8))
     E = pkg.flavour("bytes").Automaton()
@@ -282,9 +254,9 @@ def _c(A):
 
 @pytest.mark.gpu
 def test_c_abi_refuses_a_table_of_another_key_set():
-    A, _ = _automaton("bytes", [tuple(b"abc")])
-    B, _ = _automaton("bytes", [tuple(b"abcdef")])
-    U, _ = _automaton("unicode", [tuple(b"abc")])
+    A, _ = automaton("bytes", False, [tuple(b"abc")])
+    B, _ = automaton("bytes", False, [tuple(b"abcdef")])
+    U, _ = automaton("unicode", False, [tuple(b"abc")])
     lib, ta = _c(A)
     ss = ctypes.c_void_p()
     N.check(lib.acb_streams_new(ta, 4, 0, ctypes.byref(ss)))
@@ -311,7 +283,7 @@ def _overflow(device_route, long_mode=0):
     import torch
     rng = np.random.default_rng(77)
     key_len = np.array([2, 2, 3, 1])
-    A, _ = _automaton("bytes", [tuple(b"ab"), tuple(b"ba"), tuple(b"aba"), tuple(b"b")])
+    A, _ = automaton("bytes", False, [tuple(b"ab"), tuple(b"ba"), tuple(b"aba"), tuple(b"b")])
     lib, tb = _c(A)
     n_streams, stride = 64, 32
     feeds = [rng.choice(np.frombuffer(b"ab", dtype=np.uint8), size=(n_streams, stride)) for _ in range(3)]
@@ -386,7 +358,7 @@ def test_overflow_commits_nothing_long_device_gpu():
 def test_device_tensor_feed_equals_host_feed():
     import torch
     rng = np.random.default_rng(31)
-    A, _ = _automaton("bytes", _keys("bytes", rng, hi=12))
+    A, _ = automaton("bytes", False, _keys("bytes", rng, hi=12))
     Sh, Sd = A.stream_batch(500), A.stream_batch(500)
     for k in range(4):
         batch = rng.choice(np.frombuffer(b"abc", dtype=np.uint8), size=(300, 7 + k))
@@ -402,7 +374,7 @@ def test_device_tensor_feed_equals_host_feed():
 def test_position_past_2_31_is_exact():
     """one stream, three 1 GiB device chunks, a key across 2^31"""
     import torch
-    A, _ = _automaton("bytes", [tuple(b"abcd")])
+    A, _ = automaton("bytes", False, [tuple(b"abcd")])
     S = A.stream_batch(1)
     G = 1 << 30
     d = torch.zeros((1, G), dtype=torch.uint8, device="cuda")

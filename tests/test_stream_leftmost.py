@@ -14,16 +14,16 @@ import emul_replace
 import emul_stream_leftmost
 import emul_streams
 import pyahocorasick_b200 as pkg
+from batch_cases import (CASES, DT, NESTED, automaton, fake_table, leftmost_random_case, obj, oracle_full, replace_reps,
+                         rows, skip_if_device, split, table_and_batch)
 from pyahocorasick_b200 import _native as N
-from test_leftmost_longest import CASES, NESTED, _automaton, _full, _obj, _random_case
-from test_replace import _reps
 
 ABCDE = [[0x61, 0x62, 0x63, 0x64, 0x65], [0x62, 0x63, 0x64, 0x78], [0x63, 0x64]]
 
 
 def _key_sets(case, rng):
     """random keys, nested keys a .. a^W over runs of a, the abcde / bcdx / cd example, prefixes and suffixes, T = 0"""
-    keys, _ = _random_case(case, rng)
+    keys, _ = leftmost_random_case(case, rng)
     yield keys
     if case in ("bytes", "latin1", "seq2", "seq4"):
         yield NESTED[:int(rng.integers(2, 9))]
@@ -76,7 +76,7 @@ def _drive(case, A, texts, rng, feed, finish, T, check_lag=None):
         for s in pick:
             piece = texts[s][seg[s]][off[s]:off[s] + _chunk_len(T, rng)]
             off[s] += len(piece)
-            chunks.append(None if not piece and rng.integers(0, 2) else _obj(case, piece))
+            chunks.append(None if not piece and rng.integers(0, 2) else obj(*CASES[case][:2], piece))
         for s, r in zip(pick, feed(chunks, pick)):
             got[s][seg[s]].append(r)
         if check_lag:
@@ -95,11 +95,11 @@ def _per_id(m, ids):
 
 
 def _want_matches(O, keys, text, case):
-    return [(e, k) for _, e, k in emul_leftmost.greedy(_full(O, [text], case), [len(k) for k in keys])]
+    return [(e, k) for _, e, k in emul_leftmost.greedy(oracle_full(O, [text], case), [len(k) for k in keys])]
 
 
 def _want_output(O, keys, text, reps, case):
-    chosen = [(e, k) for _, e, k in emul_leftmost.greedy(_full(O, [text], case), [len(k) for k in keys])]
+    chosen = [(e, k) for _, e, k in emul_leftmost.greedy(oracle_full(O, [text], case), [len(k) for k in keys])]
     return emul_replace.definition(text, chosen, [len(k) for k in keys], reps)
 
 
@@ -110,7 +110,8 @@ def _letters(case, item):
 
 
 def _run_case(case, keys, texts, rng, algo, emulated):
-    A, O = _automaton(case, keys)
+    fl, seq, _ = CASES[case]
+    A, O = automaton(fl, seq, keys)
     T = max(len(k) for k in keys) - 1
     B = A.stream_batch(len(texts), leftmost_longest=True, algo=algo)
 
@@ -141,8 +142,8 @@ def _run_case(case, keys, texts, rng, algo, emulated):
             assert [x for r in got[s][g] for x in r] == _want_matches(O, keys, text, case), (case, algo, keys, text)
     assert not B.positions.any()
     # the replacing form over the same texts
-    reps = _reps(case, keys, rng)
-    R = A.replacer({_obj(case, k): _obj(case, r) for k, r in zip(keys, reps)})
+    reps = replace_reps(case, keys, rng)
+    R = A.replacer({obj(fl, seq, k): obj(fl, seq, r) for k, r in zip(keys, reps)})
     S = R.stream_batch(len(texts), algo=algo)
     got = _drive(case, A, texts, rng, lambda c, i: [_letters(case, x) for x in S.feed(c, i)],
                  lambda i: [_letters(case, x) for x in S.finish(i)], T)
@@ -173,7 +174,7 @@ def test_other_input_forms_and_two_interleaved_batches(monkeypatch):
     emul_stream_leftmost.install(monkeypatch)
     emul_replace.install(monkeypatch)
     keys = [b"ab", b"abc", b"bca", b"c"]
-    A, O = _automaton("bytes", [list(k) for k in keys])
+    A, O = automaton("bytes", False, keys)
     text = b"abcabcaabcbcab" * 3
     want = [(0, e, k) for e, k in _want_matches(O, [list(k) for k in keys], list(text), "bytes")]
     B1 = A.stream_batch(4, leftmost_longest=True)
@@ -254,11 +255,8 @@ def test_c_entries_check_arguments_first():
 
 
 def test_c_entries_fail_loudly_without_a_device():
-    import torch
-    if torch.cuda.is_available():
-        pytest.skip("a device is present")
-    fake = ctypes.create_string_buffer(1 << 16)                # a zeroed stand-in for acb_table with 1-byte letters
-    ctypes.c_int32.from_buffer(fake, 16).value = 1
+    skip_if_device()
+    fake = fake_table(1)
     ss = ctypes.c_void_p()
     assert N.lib().acb_streams_new_leftmost(ctypes.addressof(fake), 4, ctypes.byref(ss)) == N.ACB_ECUDA
     assert N.last_error()
@@ -285,10 +283,6 @@ def _collect(B, feeds, n):
     recs.append(np.stack([m.hay_id, m.end_index, m.key_id.astype(np.int64)], axis=1))
     r = np.concatenate(recs)
     return r[np.lexsort((r[:, 1], r[:, 0]))]
-
-
-def _whole_records(m):
-    return np.stack([m.hay_id.astype(np.int64), m.end_index.astype(np.int64), m.key_id.astype(np.int64)], axis=1)
 
 
 def _assemble(outs, n):
@@ -322,7 +316,7 @@ def test_gpu_c2_million_streams(step):
     A = synth.build_automaton(w.keys)
     n = w.n_hay
     d = torch.from_numpy(w.haystacks).cuda()
-    want = _whole_records(A.find_leftmost_longest_batch(d))
+    want = rows(A.find_leftmost_longest_batch(d))
     feeds = [(d[:, i:i + step].contiguous(), None) for i in range(0, d.shape[1], step)]
     got = _collect(A.stream_batch(n, leftmost_longest=True), feeds, n)
     assert np.array_equal(got, want)
@@ -347,7 +341,7 @@ def test_gpu_long_keys(klen):
     rng = np.random.default_rng(klen)
     keys = sorted({bytes(rng.integers(0x61, 0x63, size=int(rng.integers(1, klen + 1)), dtype=np.uint8)) for _ in range(8)}
                   | {bytes(rng.integers(0x61, 0x63, size=klen, dtype=np.uint8))})
-    A, _ = _automaton("bytes", [list(k) for k in keys])
+    A, _ = automaton("bytes", False, keys)
     n = 6
     texts = []
     for _ in range(n):
@@ -355,7 +349,7 @@ def test_gpu_long_keys(klen):
         while len(t) < 3 * klen:
             t += keys[int(rng.integers(0, len(keys)))] if rng.integers(0, 2) else bytes(rng.integers(0x61, 0x64, size=5, dtype=np.uint8))
         texts.append(t)
-    want = _whole_records(A.find_leftmost_longest_batch(texts))
+    want = rows(A.find_leftmost_longest_batch(texts))
     R = A.replacer({k: k[: len(k) // 3] for k in keys})
     wout = R.replace_batch(texts)
     B = A.stream_batch(n, leftmost_longest=True)
@@ -384,8 +378,8 @@ def test_gpu_staged_batch_past_2_gib():
     for s in range(n):
         for j, b in enumerate(b"needle"):
             d[s, where + j + s] = b
-    A, _ = _automaton("bytes", [list(b"needle"), list(b"eed"), list(b"le\0")])
-    want = _whole_records(A.find_leftmost_longest_batch(d))
+    A, _ = automaton("bytes", False, [list(b"needle"), list(b"eed"), list(b"le\0")])
+    want = rows(A.find_leftmost_longest_batch(d))
     cut = (1 << 20) * 7 + 3                                 # inside a planted key
     feeds = [(d[:, :cut].contiguous(), None), (d[:, cut:].contiguous(), None)]
     del d
@@ -400,15 +394,12 @@ def test_gpu_capacity_contract():
     repeated feed gives the answer of a batch that never overflowed"""
     import torch
     keys = [b"ab", b"b", b"abc", b"ca"]
-    A, _ = _automaton("bytes", [list(k) for k in keys])
+    A, _ = automaton("bytes", False, keys)
     table = {b"ab": b"XYZW", b"b": b"", b"abc": b"q", b"ca": b"CA!"}
     R = A.replacer(table)
     chunks = [b"abcabxbab" * 5, b"bbbbca", b"zzab", b"c"]
-    flat = np.frombuffer(b"".join(chunks), dtype=np.uint8)
-    offs = np.zeros(len(chunks) + 1, dtype=np.int64)
-    np.cumsum([len(c) for c in chunks], out=offs[1:])
+    tb, flat, offs = table_and_batch(A, chunks)
     L = N.lib()
-    tb = A._ensure_table(0)
     r = R._replacer(tb, False, 0)
     prime = [b"a", b"", b"", b"xab"]
 
@@ -464,13 +455,13 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
     import torch
     rng = np.random.default_rng(21)
     case = "bytes" if fl == "bytes" else "wide"
-    al = CASES[case][2]
+    fl, seq, al = CASES[case]
     keys = sorted({tuple(int(x) for x in rng.choice(al[:2], size=int(rng.integers(1, 5)))) for _ in range(10)})
-    A, O = _automaton(case, keys)
-    reps = _reps(case, keys, rng)
-    R = A.replacer({_obj(case, k): _obj(case, r) for k, r in zip(keys, reps)})
+    A, O = automaton(fl, seq, keys)
+    reps = replace_reps(case, keys, rng)
+    R = A.replacer({obj(fl, seq, k): obj(fl, seq, r) for k, r in zip(keys, reps)})
     texts = [[int(x) for x in rng.choice(al, size=28)] for _ in range(300)]
-    host = np.stack([np.asarray(t, dtype={1: np.uint8, 4: "<u4"}[A._L]).view(np.uint8) for t in texts])
+    host = np.stack([np.asarray(t, dtype=DT[A._L]).view(np.uint8) for t in texts])
     d = torch.from_numpy(host).cuda()
     W = 7 * A._L
     views = {"whole": (lambda i: d[:, i * W:(i + 1) * W].contiguous(), texts)}
@@ -499,9 +490,10 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
         for h, e, v in zip(m.hay_id.tolist(), m.end_index.tolist(), m.values()):
             got[h].append((e, v))
         assert all(o.is_cuda and f.is_cuda for o, f in outs)
+        parts = [split(o.cpu().numpy(), f.cpu().numpy(), A._L) for o, f in outs]
         for s, t in enumerate(ts):
             assert got[s] == _want_matches(O, keys, t, case), name
-            out = [x for o, f in outs for x in np.asarray(o[f[s]:f[s + 1]].cpu()).view({1: np.uint8, 4: "<u4"}[A._L]).tolist()]
+            out = [x for p in parts for x in p[s]]
             assert out + _letters(case, rest[s]) == _want_output(O, keys, t, reps, case), name
 
 
@@ -510,23 +502,23 @@ def test_gpu_interleaved_with_other_calls_on_one_table():
     """feeds between find_leftmost_longest_batch, replace_batch and a find_all stream batch on the same table"""
     rng = np.random.default_rng(33)
     keys = [b"ab", b"abc", b"bc", b"cab", b"a"]
-    A, O = _automaton("bytes", [list(k) for k in keys])
+    A, O = automaton("bytes", False, keys)
     texts = [bytes(rng.choice(list(b"abc"), size=90).astype(np.uint8)) for _ in range(50)]
     R = A.replacer({k: k.upper() * 2 for k in keys})
     B = A.stream_batch(50, leftmost_longest=True)
     S = R.stream_batch(50)
     F = A.stream_batch(50)
-    whole = _whole_records(A.find_leftmost_longest_batch(texts))
+    whole = rows(A.find_leftmost_longest_batch(texts))
     wout = R.replace_batch(texts)
     recs, outs, fa = [], [b""] * 50, 0
     for i in range(0, 90, 13):
         chunks = [t[i:i + 13] for t in texts]
-        recs.append(_whole_records(B.feed(chunks)))
-        assert _whole_records(A.find_leftmost_longest_batch(texts)).tolist() == whole.tolist()
+        recs.append(rows(B.feed(chunks)))
+        assert rows(A.find_leftmost_longest_batch(texts)).tolist() == whole.tolist()
         outs = [a + b for a, b in zip(outs, S.feed(chunks))]
         assert R.replace_batch(texts) == wout
         fa += len(F.feed(chunks))
-    recs.append(_whole_records(B.finish()))
+    recs.append(rows(B.finish()))
     r = np.concatenate(recs)
     assert np.array_equal(r[np.lexsort((r[:, 1], r[:, 0]))], whole)
     assert [a + b for a, b in zip(outs, S.finish())] == wout

@@ -18,8 +18,8 @@ import emul_streams
 import pyahocorasick_b200 as pkg
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200 import synth
-from test_record_bounds import _big_batch
-from test_stream_batch import _automaton
+from batch_cases import automaton, layout
+from kernel_cells import _big_batch
 
 MiB = 1 << 20
 
@@ -219,11 +219,8 @@ def _windows(rng, base, n_streams, size):
 
 def _plain_ragged(A, kind, hist, sel, before):
     """the plain scan of the histories of streams `sel` as (flat, offsets); the records past `before`"""
-    dt = np.uint8 if kind == "bytes" else np.dtype("<u4")
-    parts = [hist[s].astype(dt).view(np.uint8) for s in sel]
-    off = np.zeros(len(parts) + 1, dtype=np.int64)
-    np.cumsum([p.size for p in parts], out=off[1:])
-    return _new_part(_arr(A.find_all_batch((np.concatenate(parts), off))), before, np.asarray(sel))
+    batch = layout([hist[s] for s in sel], 1 if kind == "bytes" else 4)
+    return _new_part(_arr(A.find_all_batch(batch)), before, np.asarray(sel))
 
 
 def _long_key_streams(kind, keys, src, width, n_feeds, seed, gpu, long=False):
@@ -231,7 +228,7 @@ def _long_key_streams(kind, keys, src, width, n_feeds, seed, gpu, long=False):
     odd ones.  Compared with the oracle per stream (long: the iter_long().set() chain) and, on the GPU, with the plain
     scan of whole streams; a twin batch gets every feed in two calls."""
     rng = np.random.default_rng(seed)
-    A, O = _automaton(kind, keys)
+    A, O = automaton(kind, False, keys)
     n = len(src)
     S, Tw = A.stream_batch(n, long=long), A.stream_batch(n, long=long)
     hist = [s[:0] for s in src]
@@ -344,7 +341,7 @@ def test_million_long_streams_equal_iter_long_chains():
     torch = _torch()
     rng = np.random.default_rng(37)
     keys = sorted({tuple(rng.choice([0x61, 0x62, 0x63], size=int(rng.integers(3, 13))).tolist()) for _ in range(16)})
-    A, _ = _automaton("bytes", keys)
+    A, _ = automaton("bytes", False, keys)
     n = 1 << 20
     S, Tw = A.stream_batch(n, long=True), A.stream_batch(n, long=True)
     g = torch.Generator(device="cuda").manual_seed(37)
@@ -467,7 +464,7 @@ def test_misaligned_device_views_equal_aligned_copies(flavour):
 def test_c_abi_still_refuses_misaligned_buffers():
     """the C entries keep their check: a device pointer off a 16-byte boundary is ACB_EINVAL"""
     torch = _torch()
-    A, _ = _automaton("bytes", [tuple(b"ab")])
+    A, _ = automaton("bytes", False, [tuple(b"ab")])
     lib, tb = A._lib, A._ensure_table(0)
     d = torch.zeros(64, dtype=torch.uint8, device="cuda")
     cnt = torch.zeros(1, dtype=torch.int64, device="cuda")

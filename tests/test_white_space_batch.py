@@ -11,8 +11,7 @@ import numpy as np
 import pytest
 
 import emul_white_space
-import oracle
-import pyahocorasick_b200 as pkg
+from batch_cases import automaton, fake_table, forms, got_values, obj, table_and_batch, triples
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200 import automaton as am
 
@@ -65,7 +64,7 @@ def test_space_mask_takes_the_same_set():
 # ------------------------------------------------------------------ argument errors
 def test_skip_argument_errors():
     L = N.lib()
-    fake = ctypes.addressof(ctypes.create_string_buffer(1 << 16))   # never used as a table: the skip set is checked first
+    fake = ctypes.addressof(fake_table())                       # never used as a table: the skip set is checked first
     n = ctypes.c_int64(0)
     ok = np.array([9, 32], dtype=np.uint32)
     bad = np.array([32, 9], dtype=np.uint32)
@@ -78,7 +77,7 @@ def test_skip_argument_errors():
     for skip in (bad, dup, big):
         ss = ctypes.c_void_p()
         assert L.acb_streams_new_skip(fake, 4, N.ptr(skip), len(skip), ctypes.byref(ss)) == N.ACB_EINVAL and not ss.value
-    A = _automaton("bytes", [b"ab"])[0]
+    A = automaton("bytes", False, [b"ab"])[0]
     with pytest.raises(ValueError):
         A.find_all_batch([b"a b"], algo="long", ignore_white_space=True)
     with pytest.raises(ValueError):
@@ -86,24 +85,8 @@ def test_skip_argument_errors():
 
 
 # ------------------------------------------------------------------ batches against the oracle
-def _automaton(fl, keys, seq=False):
-    mod = pkg.flavour(fl)
-    A = mod.Automaton(mod.STORE_INTS, mod.KEY_SEQUENCE) if seq else mod.Automaton(mod.STORE_INTS)
-    O = oracle.OracleAutomaton()
-    for i, k in enumerate(keys):
-        A.add_word(k, i)
-        O.add_word(k, i)
-    A.make_automaton()
-    O.make_automaton()
-    return A, O
-
-
 def _want(O, hays):
     return [(h, e, v) for h, hay in enumerate(hays) for e, v in O.iter(hay, ignore_white_space=True)]
-
-
-def _got(m):
-    return list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.key_id.tolist()))
 
 
 # (flavour, key type, alphabet of text letters) -- latin-1, wide and mixed unicode; bytes-flavour sequences are
@@ -118,19 +101,12 @@ CASES = {
 }
 
 
-def _obj(case, letters):
-    fl, seq, _ = CASES[case]
-    if seq:
-        return tuple(letters)
-    return bytes(letters) if fl == "bytes" else "".join(map(chr, letters))
-
-
 def _random_case(case, rng):
     fl, seq, al = CASES[case]
     words = [0x61, 0x62] if case in ("bytes", "latin1", "mixed") else al[:3]
     keys = {tuple(int(x) for x in rng.choice(words, size=int(rng.integers(1, 6)))) for _ in range(int(rng.integers(1, 8)))}
     keys |= {tuple(int(x) for x in rng.choice(al, size=int(rng.integers(1, 4)))) for _ in range(2)}   # keys with white space
-    A, O = _automaton(fl, [_obj(case, k) for k in sorted(keys)], seq)
+    A, O = automaton(fl, seq, sorted(keys))
     n = int(rng.integers(1, 12))
     hays = []
     for _ in range(n):
@@ -146,24 +122,6 @@ def _random_case(case, rng):
     return A, O, hays
 
 
-def _forms(case, A, hays):
-    """every input form find_all_batch accepts for this case"""
-    fl, seq, _ = CASES[case]
-    objs = [_obj(case, h) for h in hays]
-    yield "list", objs
-    if case in ("latin1", "mixed"):
-        return
-    L = A._L
-    dt = {1: np.uint8, 2: "<u2", 4: "<u4"}[L]
-    parts = [np.asarray(h, dtype=dt).view(np.uint8) for h in hays]
-    offs = np.zeros(len(parts) + 1, dtype=np.int64)
-    np.cumsum([p.size for p in parts], out=offs[1:])
-    yield "flat", (np.concatenate(parts), offs)
-    width = max(len(h) for h in hays)
-    if all(len(h) == width for h in hays) and width:
-        yield "array", np.stack(parts)
-
-
 def _batches(cases, seed, trials, algo="auto", sort=True):
     rng = np.random.default_rng(seed)
     for case in cases:
@@ -172,9 +130,10 @@ def _batches(cases, seed, trials, algo="auto", sort=True):
             if rng.integers(0, 3) == 0:                           # a fixed-stride batch too
                 w = int(rng.integers(1, 20))
                 hays = [(h + [0x61] * w)[:w] for h in hays]
-            want = _want(O, [_obj(case, h) for h in hays])
-            for form, x in _forms(case, A, hays):
-                got = _got(A.find_all_batch(x, algo=algo, sort=sort, ignore_white_space=True))
+            objs = [obj(*CASES[case][:2], h) for h in hays]
+            want = _want(O, objs)
+            for form, x in forms(objs, hays, A._L, case in ("latin1", "mixed")):
+                got = triples(A.find_all_batch(x, algo=algo, sort=sort, ignore_white_space=True))
                 if not sort:
                     got, want_ = sorted(got), sorted(want)
                 else:
@@ -202,10 +161,9 @@ def test_batches_equal_the_drop_in_iter(monkeypatch):
     rng = np.random.default_rng(3)
     for case in CASES:
         A, O, hays = _random_case(case, rng)
-        objs = [_obj(case, h) for h in hays]
+        objs = [obj(*CASES[case][:2], h) for h in hays]
         want = [(h, e, v) for h, o in enumerate(objs) for e, v in A.iter(o, ignore_white_space=True)]
-        m = A.find_all_batch(objs, ignore_white_space=True)
-        assert list(zip(m.hay_id.tolist(), m.end_index.tolist(), m.values())) == want
+        assert got_values(A.find_all_batch(objs, ignore_white_space=True)) == want
 
 
 # ------------------------------------------------------------------ streams against the oracle's iter().set() chain
@@ -232,18 +190,18 @@ def _streams(case, seed, n_streams, n_feeds, algo="auto"):
             n = [0, int(rng.integers(0, T + 1)), int(rng.integers(0, 3 * T + 4)), 30][r]
             pool = WS if rng.integers(0, 4) == 0 else al                  # chunks of white space only
             chunks.append([int(x) for x in rng.choice(pool, size=n)])
-        m = S.feed([_obj(case, c) for c in chunks], ids)
+        m = S.feed([obj(fl, seq, c) for c in chunks], ids)
         want = []
         for s, c in sorted(zip(ids.tolist(), chunks), key=lambda x: x[0]):
             if its[s] is None:
-                its[s] = O.iter(_obj(case, c), ignore_white_space=True)
+                its[s] = O.iter(obj(fl, seq, c), ignore_white_space=True)
             else:
-                its[s].set(_obj(case, c))
+                its[s].set(obj(fl, seq, c))
             want += [(s, e, v) for e, v in its[s]]
             pos[s] += len(c)
         order = {s: i for i, s in enumerate(ids.tolist())}
         want.sort(key=lambda r: order[r[0]])                              # records come in chunk order
-        got = _got(m)
+        got = triples(m)
         assert sorted(got) == sorted(want) and [r[0] for r in got] == [r[0] for r in want], (case, f)
         assert S.positions.tolist() == pos
 
@@ -265,14 +223,12 @@ def test_streams_match_oracle_chain_gpu(case, algo):
 @pytest.mark.gpu
 def test_overflow_counts_exactly_and_stream_feeds_commit_nothing():
     rng = np.random.default_rng(1)
-    A, O = _automaton("bytes", [b"ab", b"abc", b"b", b"ca"])
+    A, O = automaton("bytes", False, [b"ab", b"abc", b"b", b"ca"])
     hays = [bytes(rng.choice(list(b"abc \t"), size=40).tolist()) for _ in range(30)]
     want = _want(O, hays)
     n = len(want)
-    flat = np.frombuffer(b"".join(hays), dtype=np.uint8)
-    offs = np.array([0] + np.cumsum([len(h) for h in hays]).tolist(), dtype=np.int64)
     skip = A._skip_set(False)
-    tb = A._ensure_table(0)
+    tb, flat, offs = table_and_batch(A, hays)
     lib = N.lib()
     for cap in (0, 1, n - 1):
         found = ctypes.c_int64(0)
@@ -294,7 +250,7 @@ def test_overflow_counts_exactly_and_stream_feeds_commit_nothing():
         assert stored <= set(want)                             # stored records are mapped back
     S = A.stream_batch(len(hays), ignore_white_space=True)
     first = S.feed(hays)
-    assert _got(first) == want
+    assert triples(first) == want
     second = [h[::-1] for h in hays]
     its = [O.iter(h, ignore_white_space=True) for h in hays]
     want2 = []
@@ -307,7 +263,7 @@ def test_overflow_counts_exactly_and_stream_feeds_commit_nothing():
     f2 = np.frombuffer(b"".join(second), dtype=np.uint8)
     rc = lib.acb_streams_feed_host(ss, tb, N.ptr(f2), f2.size, N.ptr(offs), len(hays), 0, None, None, 1, ctypes.byref(found), N.ALGO_FILTER, 1)
     assert rc == N.ACB_EOVERFLOW and found.value == len(want2) and (S.positions == before).all()
-    assert _got(S.feed(second)) == want2                     # the same feed again, with room
+    assert triples(S.feed(second)) == want2                  # the same feed again, with room
     assert S.positions.tolist() == [2 * len(h) for h in hays]
 
 
@@ -370,24 +326,17 @@ def test_white_space_runs_and_keys_across_every_boundary(L):
     letters; several tiles each, so the look-back, later tiles' prefixes, unaligned stores and the remap's search over
     tiles all run at every width"""
     fl, seq, _, key, ws = WIDTHS[L]
-    A, O = _automaton(fl, [_obj_w(L, key), _obj_w(L, [0x7A, 0x7A])], seq)
+    A, O = automaton(fl, seq, [key, [0x7A, 0x7A]])
     assert A._L == L
     letters, n_plants, straddled = _boundary_text(L, np.random.default_rng(L))
     assert len(straddled) >= 15 and len(letters) > 20 * 8192
-    objs = [_obj_w(L, letters), _obj_w(L, letters[1:]), _obj_w(L, letters[:8191] + ws[:1] * 2 + letters[8191:])]
+    objs = [obj(fl, seq, letters), obj(fl, seq, letters[1:]), obj(fl, seq, letters[:8191] + ws[:1] * 2 + letters[8191:])]
     batch = A._batch_input(objs)
     assert batch[0] == "host" and batch[5] is False and batch[1].size == L * sum(len(o) for o in objs)   # not the latin-1 table
     want = _want(O, objs)
     assert sum(1 for r in want if r[2] == 0) >= 3 * n_plants - 1
     for algo in ("filter", "dfa"):
-        assert _got(A.find_all_batch(objs, algo=algo, ignore_white_space=True)) == want
-
-
-def _obj_w(L, letters):
-    fl, seq = WIDTHS[L][:2]
-    if seq:
-        return tuple(letters)
-    return bytes(letters) if fl == "bytes" else "".join(map(chr, letters))
+        assert triples(A.find_all_batch(objs, algo=algo, ignore_white_space=True)) == want
 
 
 def _column_reference(A, x, keep_cols, algo="auto"):
@@ -428,7 +377,7 @@ def _scale(n, stride, seed, host=True):
     x[:, ws] = ord(" ")
     want = _column_reference(A, x, cols[~ws])
     m = A.find_all_batch(x.cpu().numpy() if host else x, ignore_white_space=True)
-    assert _got(m) == want
+    assert triples(m) == want
     return len(want)
 
 
@@ -447,14 +396,14 @@ def test_batch_past_2_31_bytes_and_two_compacted_segments():
 def test_device_tensors_and_a_misaligned_view():
     import torch
     rng = np.random.default_rng(8)
-    A, O = _automaton("bytes", [b"ab", b"b c", b"ca", b"abcab"])
+    A, O = automaton("bytes", False, [b"ab", b"b c", b"ca", b"abcab"])
     x = rng.choice(np.frombuffer(b"abc \t\x85", dtype=np.uint8), size=(301, 7))
     want = _want(O, [bytes(r) for r in x])
     d = torch.from_numpy(x).cuda()
-    assert _got(A.find_all_batch(d, ignore_white_space=True)) == want
+    assert triples(A.find_all_batch(d, ignore_white_space=True)) == want
     v = d[1:]
     assert v.data_ptr() % 16
-    assert _got(A.find_all_batch(v, ignore_white_space=True)) == [(h - 1, e, k) for h, e, k in want if h]
+    assert triples(A.find_all_batch(v, ignore_white_space=True)) == [(h - 1, e, k) for h, e, k in want if h]
 
 
 @pytest.mark.gpu

@@ -15,9 +15,9 @@ import emul
 import emul_leftmost
 import emul_replace
 import emul_words
-import oracle
 import pyahocorasick_b200 as pkg
-import test_leftmost_longest as tl
+from batch_cases import (CASES, DT, automaton, check_device_capacities, check_host_capacities, fake_table, forms,
+                         got_values, key_len, np_greedy, obj, oracle_full, rows, skip_if_device, split, table_and_batch)
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200.automaton import _word_bits
 
@@ -27,7 +27,7 @@ SPACE, UNDERSCORE = 0x20, 0x5F
 
 def _is_word(case, words):
     """the word-letter predicate over letter values for a whole_words argument"""
-    bytes_fl = tl.CASES[case][0] == "bytes"
+    bytes_fl = CASES[case][0] == "bytes"
     if words is True:
         if bytes_fl:
             return lambda v: re.fullmatch(rb"\w", bytes([v])) is not None
@@ -37,7 +37,7 @@ def _is_word(case, words):
 
 
 def _word_sets(case):
-    if tl.CASES[case][0] == "bytes":
+    if CASES[case][0] == "bytes":
         return [True, b"", b"a_ "]
     return [True, "", "ał_\U0001F600"]
 
@@ -45,7 +45,7 @@ def _word_sets(case):
 def _random_case(case, rng):
     """keys and haystacks over the case's alphabet plus a space (never a word letter) and an underscore (always one, but
     for the custom sets), so keys begin and end with word and non-word letters"""
-    al = tl.CASES[case][2] + [SPACE, UNDERSCORE]
+    al = CASES[case][2] + [SPACE, UNDERSCORE]
     keys = sorted({tuple(int(x) for x in rng.choice(al, size=int(rng.integers(1, 5)))) for _ in range(int(rng.integers(1, 9)))})
     hays = []
     for _ in range(int(rng.integers(1, 10))):
@@ -64,7 +64,7 @@ def _random_case(case, rng):
 def _want(O, keys, hays, case, words):
     """(find_all, leftmost-longest) by the definition over the oracle's full list"""
     kl = [len(k) for k in keys]
-    kept = emul_words.definition(hays, tl._full(O, hays, case), kl, _is_word(case, words))
+    kept = emul_words.definition(hays, oracle_full(O, hays, case), kl, _is_word(case, words))
     return kept, emul_leftmost.greedy(kept, kl)
 
 
@@ -77,17 +77,17 @@ def _reps(keys):
     return [[0x5A] * (len(k) % 3) for k in keys]          # "", "Z" or "ZZ": latin-1, so the latin-1 table exists
 
 
-def _check_case(case, keys, hays, words, algo="auto", forms=True):
-    A, O = tl._automaton(case, keys)
+def _check_case(case, keys, hays, words, algo="auto"):
+    fl, seq, _ = CASES[case]
+    A, O = automaton(fl, seq, keys)
     want_all, want_ll = _want(O, keys, hays, case, words)
-    batches = list(tl._forms(case, A, hays)) if forms else [("list", [tl._obj(case, h) for h in hays])]
-    for form, batch in batches:
-        assert tl._got(A.find_all_batch(batch, algo=algo, whole_words=words)) == want_all, (case, form, keys, hays, words)
-        assert tl._got(A.find_leftmost_longest_batch(batch, algo=algo, whole_words=words)) == want_ll, (case, form, keys, hays, words)
+    for form, batch in forms([obj(fl, seq, h) for h in hays], hays, A._L, case in ("latin1", "mixed")):
+        assert got_values(A.find_all_batch(batch, algo=algo, whole_words=words)) == want_all, (case, form, keys, hays, words)
+        assert got_values(A.find_leftmost_longest_batch(batch, algo=algo, whole_words=words)) == want_ll, (case, form, keys, hays, words)
     reps = _reps(keys)
-    R = A.replacer({tl._obj(case, k): tl._obj(case, r) for k, r in zip(keys, reps)})
-    got = R.replace_batch([tl._obj(case, h) for h in hays], algo=algo, whole_words=words)
-    assert got == [tl._obj(case, h) for h in _want_replaced(hays, want_ll, keys, reps)], (case, keys, hays, words)
+    R = A.replacer({obj(fl, seq, k): obj(fl, seq, r) for k, r in zip(keys, reps)})
+    got = R.replace_batch([obj(fl, seq, h) for h in hays], algo=algo, whole_words=words)
+    assert got == [obj(fl, seq, h) for h in _want_replaced(hays, want_ll, keys, reps)], (case, keys, hays, words)
 
 
 # ------------------------------------------------------------------ the word sets
@@ -150,12 +150,12 @@ def test_empty_set_equals_no_option(monkeypatch):
     rng = np.random.default_rng(23)
     for case in FUZZ_CASES:
         keys, hays = _random_case(case, rng)
-        A, _ = tl._automaton(case, keys)
-        batch = [tl._obj(case, h) for h in hays]
+        A, _ = automaton(*CASES[case][:2], keys)
+        batch = [obj(*CASES[case][:2], h) for h in hays]
         for sort in (True, False):
             a, b = A.find_all_batch(batch, sort=sort), A.find_all_batch(batch, sort=sort, whole_words=_word_sets(case)[1])
-            assert (tl._got(a) == tl._got(b)) if sort else sorted(tl._got(a)) == sorted(tl._got(b))   # unsorted: any order
-        assert tl._got(A.find_leftmost_longest_batch(batch)) == tl._got(A.find_leftmost_longest_batch(batch, whole_words=_word_sets(case)[1]))
+            assert (got_values(a) == got_values(b)) if sort else sorted(got_values(a)) == sorted(got_values(b))   # unsorted: any order
+        assert got_values(A.find_leftmost_longest_batch(batch)) == got_values(A.find_leftmost_longest_batch(batch, whole_words=_word_sets(case)[1]))
 
 
 def _bytes_automaton(keys, cls_args=()):
@@ -237,17 +237,9 @@ def test_refusals():
             S.replacer({(1, 2): (3,)}).replace_batch([(1, 2)], whole_words=True)
 
 
-def _fake_table(L):
-    """a zeroed stand-in for acb_table (device 0) with the letter width set: acb_table starts with int device, int
-    sm_count, int32 S, K, L"""
-    fake = ctypes.create_string_buffer(1 << 16)
-    ctypes.c_int32.from_buffer(fake, 16).value = L
-    return fake
-
-
 def test_c_argument_checks():
     L = N.lib()
-    fake = _fake_table(1)
+    fake = fake_table(1)
     tb = ctypes.addressof(fake)
     n = ctypes.c_int64(0)
     hay = np.frombuffer(b"ab cd ab", dtype=np.uint8).copy()
@@ -282,7 +274,7 @@ def test_c_argument_checks():
     assert dev(tb, 256, N.ptr(bits), 1 << 31) == N.ACB_ERANGE
     assert dev(tb, 0, None, 0) == N.ACB_OK                                # nothing to filter: no device needed
     for width, most in ((2, 65536), (4, 0x110000)):
-        wide = _fake_table(width)
+        wide = fake_table(width)
         big = np.zeros(most // 32, dtype=np.uint32)
         assert dev(ctypes.addressof(wide), most, N.ptr(big), 0) == N.ACB_OK
         assert dev(ctypes.addressof(wide), most + 1, N.ptr(big), 0) == N.ACB_EINVAL
@@ -291,10 +283,8 @@ def test_c_argument_checks():
 
 
 def test_host_routes_fail_loudly_without_a_device():
-    import torch
-    if torch.cuda.is_available():
-        pytest.skip("a device is present")
-    fake = _fake_table(1)
+    skip_if_device()
+    fake = fake_table(1)
     n = ctypes.c_int64(0)
     hay = np.frombuffer(b"abcd" * 4, dtype=np.uint8)
     offs = np.array([0, 8, 16], dtype=np.int64)
@@ -307,16 +297,12 @@ def test_host_routes_fail_loudly_without_a_device():
 
 
 # ------------------------------------------------------------------ the real kernels
-def _rec(m):
-    return np.stack([m.hay_id.astype(np.int64), m.end_index.astype(np.int64), m.key_id.astype(np.int64)], axis=1)
-
-
 def _kept_np(A, flat, offs, stride, full, words, width=None):
     """the definition at scale: emul_words.flags over find_all_batch's records"""
     L = A._L if width is None else width
     bits, n_bits = _word_bits(A._words(words), L)
-    raw = _rec(full)
-    return raw[emul_words.flags(flat, offs, stride, L, raw, tl._key_len(A), bits, n_bits)]
+    raw = rows(full)
+    return raw[emul_words.flags(flat, offs, stride, L, raw, key_len(A), bits, n_bits)]
 
 
 @pytest.mark.gpu
@@ -347,23 +333,23 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
     import torch
     rng = np.random.default_rng(5)
     case = "bytes" if fl == "bytes" else "wide"
-    al = tl.CASES[case][2][:2] + [SPACE]
+    al = CASES[case][2][:2] + [SPACE]
     keys = [list(k) for k in {tuple(int(x) for x in rng.choice(al, size=int(rng.integers(1, 5)))) for _ in range(12)}]
-    A, O = tl._automaton(case, keys)
+    A, O = automaton(*CASES[case][:2], keys)
     L = A._L
     hays = [[int(x) for x in rng.choice(al, size=7)] for _ in range(300)]
-    host = np.stack([np.asarray(h, dtype={1: np.uint8, 4: "<u4"}[L]).view(np.uint8) for h in hays])
+    host = np.stack([np.asarray(h, dtype=DT[L]).view(np.uint8) for h in hays])
     d = torch.from_numpy(host).cuda()
     views = {"whole": (d, hays)}
     if L == 1:
         views["misaligned"] = (d[1:], hays[1:])
         assert d[1:].data_ptr() % 16 != 0
     reps = _reps(keys)
-    R = A.replacer({tl._obj(case, k): tl._obj(case, r) for k, r in zip(keys, reps)})
+    R = A.replacer({obj(*CASES[case][:2], k): obj(*CASES[case][:2], r) for k, r in zip(keys, reps)})
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
     for words in (True, _word_sets(case)[1]):
-        assert tl._got(A.find_all_batch(host, whole_words=words)) == _want(O, keys, hays, case, words)[0]
+        assert got_values(A.find_all_batch(host, whole_words=words)) == _want(O, keys, hays, case, words)[0]
         for name, (t, hs) in views.items():
             want_all, want_ll = _want(O, keys, hs, case, words)
             with torch.cuda.stream(side):
@@ -371,18 +357,10 @@ def test_gpu_cuda_tensors_on_a_side_stream(fl):
                 m_ll = A.find_leftmost_longest_batch(t, whole_words=words)
                 flat, offs = R.replace_batch(t, whole_words=words)
                 side.synchronize()
-            assert tl._got(m_all) == want_all, (name, words)
-            assert tl._got(m_ll) == want_ll, (name, words)
-            raw, o = flat.cpu().numpy(), offs.cpu().numpy()
-            got = [raw[o[i]:o[i + 1]].view({1: np.uint8, 4: "<u4"}[L]).tolist() for i in range(len(hs))]
+            assert got_values(m_all) == want_all, (name, words)
+            assert got_values(m_ll) == want_ll, (name, words)
+            got = split(flat.cpu().numpy(), offs.cpu().numpy(), L)
             assert got == _want_replaced(hs, want_ll, keys, reps), (name, words)
-
-
-def _table_and_batch(A, hays):
-    flat = np.frombuffer(b"".join(hays), dtype=np.uint8).copy()
-    offs = np.zeros(len(hays) + 1, dtype=np.int64)
-    np.cumsum([len(h) for h in hays], out=offs[1:])
-    return A._ensure_table(0), flat, offs
 
 
 @pytest.mark.gpu
@@ -392,21 +370,16 @@ def test_gpu_exact_counts_at_every_capacity():
     A = _bytes_automaton(keys)
     hays = [b"ab ba aba abab b b a" * 20, b"", b"a", b"ab_ab ba-ba"]
     L = N.lib()
-    tb, flat, offs = _table_and_batch(A, hays)
+    tb, flat, offs = table_and_batch(A, hays)
     bits, n_bits = _word_bits(("bytes", None), 1)
-    found = ctypes.c_int64(0)
+    batch = (tb, N.ptr(flat), flat.size, N.ptr(offs), len(hays), 0, N.ptr(bits), n_bits)
     for leftmost in (False, True):
-        want = _rec(A.find_leftmost_longest_batch(hays, whole_words=True) if leftmost else A.find_all_batch(hays, whole_words=True))
-        n = len(want)
-        assert n > 10
-        for cap in (0, 1, n - 1, n):
-            out = np.zeros(max(cap, 1), dtype=N.MATCH_DTYPE)
-            args = (tb, N.ptr(flat), flat.size, N.ptr(offs), len(hays), 0, N.ptr(bits), n_bits, N.ptr(out), cap, ctypes.byref(found),
-                    N.ALGO_AUTO)
-            rc = L.acb_scan_host_leftmost_words(*args) if leftmost else L.acb_scan_host_words(*args, 1)
-            assert found.value == n and rc == (N.ACB_OK if cap >= n else N.ACB_EOVERFLOW)
-            if cap >= n:
-                assert np.array_equal(np.stack([out["hay_id"], out["end_index"], out["key_id"]], axis=1)[:n].astype(np.int64), want)
+        want = rows(A.find_leftmost_longest_batch(hays, whole_words=True) if leftmost else A.find_all_batch(hays, whole_words=True))
+        assert len(want) > 10
+        if leftmost:
+            check_host_capacities(lambda out, cap, found: L.acb_scan_host_leftmost_words(*batch, out, cap, found, N.ALGO_AUTO), want)
+        else:
+            check_host_capacities(lambda out, cap, found: L.acb_scan_host_words(*batch, out, cap, found, N.ALGO_AUTO, 1), want)
     # the replacement: the exact output size past out_cap
     R = A.replacer({k: k.upper() + b"!" for k in keys})
     want = R.replace_batch(hays, whole_words=True)
@@ -421,27 +394,17 @@ def test_gpu_exact_counts_at_every_capacity():
         assert total.value == size and rc == (N.ACB_OK if cap >= size else N.ACB_EOVERFLOW)
         if cap >= size:
             assert [out[oo[i]:oo[i + 1]].tobytes() for i in range(len(hays))] == want
-    # the device entry: any record order, guard rows behind the capacity untouched, the count added to
+    # the device entry: any record order
     full = A.find_all_batch(hays)
-    rec = _rec(full).astype(np.int32)
+    rec = rows(full).astype(np.int32)
     rec = rec[np.random.default_rng(0).permutation(len(rec))]
-    want = rec[emul_words.flags(flat, offs, 0, 1, rec, tl._key_len(A), bits, n_bits)].astype(np.int64)
-    n = len(want)
+    want = rec[emul_words.flags(flat, offs, 0, 1, rec, key_len(A), bits, n_bits)].astype(np.int64)
     d_rec = torch.from_numpy(np.ascontiguousarray(rec)).cuda()
     d_hay, d_off = torch.from_numpy(flat).cuda(), torch.from_numpy(offs).cuda()
     d_bits = torch.from_numpy(bits.view(np.int32).copy()).cuda()
-    for cap in (0, 1, n - 1, n):
-        out = torch.full((cap + 4, 3), -7, dtype=torch.int32, device="cuda")
-        cnt = torch.tensor([5], dtype=torch.int64, device="cuda")
-        assert L.acb_word_filter_device(tb, d_hay.data_ptr(), flat.size, d_off.data_ptr(), len(hays), 0, d_rec.data_ptr(), len(rec),
-                                        d_bits.data_ptr(), n_bits, out.data_ptr(), cap, cnt.data_ptr(),
-                                        torch.cuda.current_stream().cuda_stream) == N.ACB_OK
-        assert int(cnt.item()) == 5 + n
-        o = out.cpu().numpy()
-        assert (o[cap:] == -7).all() and (o[:min(cap, 5)] == -7).all()
-        if cap > 5:
-            assert np.array_equal(o[5:cap].astype(np.int64), want[:cap - 5])
-    assert np.array_equal(rec, d_rec.cpu().numpy())
+    check_device_capacities(lambda out, cap, cnt, s: L.acb_word_filter_device(
+        tb, d_hay.data_ptr(), flat.size, d_off.data_ptr(), len(hays), 0, d_rec.data_ptr(), len(rec), d_bits.data_ptr(), n_bits,
+        out, cap, cnt, s), want, d_rec)
 
 
 @pytest.mark.gpu
@@ -454,13 +417,13 @@ def test_gpu_c2_planted_against_the_definition():
         for algo in ("filter", "dfa"):
             full = A.find_all_batch(w.haystacks, algo=algo)
             want = _kept_np(A, w.haystacks.reshape(-1), None, stride, full, words)
-            assert np.array_equal(_rec(A.find_all_batch(w.haystacks, algo=algo, whole_words=words)), want)
-            got = _rec(A.find_leftmost_longest_batch(w.haystacks, algo=algo, whole_words=words))
-            assert np.array_equal(got, tl._np_greedy(np.rec.fromarrays(want.T, names="hay_id,end_index,key_id"), tl._key_len(A)))
+            assert np.array_equal(rows(A.find_all_batch(w.haystacks, algo=algo, whole_words=words)), want)
+            got = rows(A.find_leftmost_longest_batch(w.haystacks, algo=algo, whole_words=words))
+            assert np.array_equal(got, np_greedy(np.rec.fromarrays(want.T, names="hay_id,end_index,key_id"), key_len(A)))
         if words == b"":
-            assert np.array_equal(_rec(A.find_all_batch(w.haystacks, whole_words=b"")), _rec(A.find_all_batch(w.haystacks)))
-            assert np.array_equal(_rec(A.find_leftmost_longest_batch(w.haystacks, whole_words=b"")),
-                                  _rec(A.find_leftmost_longest_batch(w.haystacks)))
+            assert np.array_equal(rows(A.find_all_batch(w.haystacks, whole_words=b"")), rows(A.find_all_batch(w.haystacks)))
+            assert np.array_equal(rows(A.find_leftmost_longest_batch(w.haystacks, whole_words=b"")),
+                                  rows(A.find_leftmost_longest_batch(w.haystacks)))
 
 
 @pytest.mark.gpu
@@ -473,9 +436,9 @@ def test_gpu_single_haystack_of_256_mib():
     full = A.find_all_batch((text, offs))
     want = _kept_np(A, text, offs, 0, full, True)
     assert len(want) > 200_000
-    assert np.array_equal(_rec(A.find_all_batch((text, offs), whole_words=True)), want)
-    got = _rec(A.find_leftmost_longest_batch((text, offs), whole_words=True))
-    assert np.array_equal(got, tl._np_greedy(np.rec.fromarrays(want.T, names="hay_id,end_index,key_id"), tl._key_len(A)))
+    assert np.array_equal(rows(A.find_all_batch((text, offs), whole_words=True)), want)
+    got = rows(A.find_leftmost_longest_batch((text, offs), whole_words=True))
+    assert np.array_equal(got, np_greedy(np.rec.fromarrays(want.T, names="hay_id,end_index,key_id"), key_len(A)))
 
 
 @pytest.mark.gpu
@@ -485,13 +448,13 @@ def test_gpu_batch_past_2_gib():
     import torch
     keys = [b"qzq", b"zqz", b"qzqzx"]
     A = _bytes_automaton(keys)
-    rows, stride = 2080, ((1 << 31) + (1 << 24)) // 2080 // 16 * 16
-    d = torch.randint(0, 16, (rows, stride), dtype=torch.uint8, device="cuda")
+    n_rows, stride = 2080, ((1 << 31) + (1 << 24)) // 2080 // 16 * 16
+    d = torch.randint(0, 16, (n_rows, stride), dtype=torch.uint8, device="cuda")
     d += ord("a")                                                            # a..p: no key letter but for planted ones
     d[:, ::97] = ord(" ")
     rng = np.random.default_rng(2)
     plants = [b" qzqzx ", b" qzq ", b"aqzqzx ", b" zqzb"]
-    for r in rng.integers(0, rows, size=800).tolist():
+    for r in rng.integers(0, n_rows, size=800).tolist():
         c = int(rng.integers(0, stride - 8))
         p = plants[int(rng.integers(0, len(plants)))]
         d[r, c:c + len(p)] = torch.tensor(list(p), dtype=torch.uint8)
@@ -500,8 +463,8 @@ def test_gpu_batch_past_2_gib():
     d[5, -4:] = torch.tensor(list(b" zqz"), dtype=torch.uint8)          # row 6 starts with a word letter
     d[6, :3] = torch.tensor(list(b"qzq"), dtype=torch.uint8)
     full = A.find_all_batch(d)
-    raw = _rec(full)
-    kl = tl._key_len(A)
+    raw = rows(full)
+    kl = key_len(A)
     flat = d.view(-1)
     start = raw[:, 0] * stride + raw[:, 1] - kl[raw[:, 2]] + 1
     end = raw[:, 0] * stride + raw[:, 1]
@@ -516,11 +479,11 @@ def test_gpu_batch_past_2_gib():
     word = lambda v: np.array([re.fullmatch(rb"\w", bytes([int(x)])) is not None for x in range(256)])[v]
     want = raw[~word(letters(left)) & ~word(letters(right))]
     got = A.find_all_batch(d, whole_words=True)
-    assert rows * stride > (1 << 31) and len(want) > 300 and len(want) < len(raw)
+    assert n_rows * stride > (1 << 31) and len(want) > 300 and len(want) < len(raw)
     assert (want[:, 0] * stride + want[:, 1] >= (1 << 31)).any()
-    assert np.array_equal(_rec(got), want)
+    assert np.array_equal(rows(got), want)
     ll = A.find_leftmost_longest_batch(d, whole_words=True)
-    assert np.array_equal(_rec(ll), tl._np_greedy(np.rec.fromarrays(want.T, names="hay_id,end_index,key_id"), kl))
+    assert np.array_equal(rows(ll), np_greedy(np.rec.fromarrays(want.T, names="hay_id,end_index,key_id"), kl))
 
 
 @pytest.mark.gpu
