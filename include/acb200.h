@@ -556,6 +556,36 @@ int acb_replace_host_words(acb_replacer *r, acb_table *tb, const uint8_t *hay, i
  * flags to its count, from CUDA events (the call then waits for them); 0 when timing is off or it had no records. */
 int acb_last_words_ms(float *ms);
 
+/* ---- whole-word stream batches: find_all, leftmost-longest and replacing streams, chunk by chunk ------------------
+ * A stream's text is the concatenation of its chunks since its start, its last reset or its last final feed.  Per
+ * stream the batch keeps the position, up to T + 1 held letters (T = longest_word - 1) and one byte: whether the letter
+ * just before the held ones exists and is a word letter.  The word set (host bitmap, as for acb_scan_host_words; checked
+ * against the letter width, ACB_EINVAL) is uploaded once and belongs to the batch.
+ *  - leftmost != 0: acb_streams_feed_leftmost_* and acb_streams_replace_* take the batch.  Over all feeds of a stream
+ *    they return what acb_scan_host_leftmost_words / acb_replace_host_words return for its whole text; a feed reports
+ *    the chosen whole-word matches that start before pos_new - T - 1 and releases the output up to there.
+ *  - leftmost == 0: acb_streams_feed_words_* take the batch.  Over all feeds of a stream they return what
+ *    acb_scan_host_words (sorted) returns for its whole text; a feed reports the whole-word matches that end in
+ *    [pos_old - 1, pos_new - 2] (pos_new - 1 on a final feed), because a match is a whole word only once the letter after
+ *    it is known.
+ * A final feed decides everything and returns the stream to its start.  acb_streams_reset and acb_streams_positions
+ * serve these batches; acb_streams_feed_* refuse them (ACB_EINVAL), and each feed refuses the batches of the other kind.
+ * The overflow contract, the waits and the rules on streams are those of the leftmost feeds.  Without a device:
+ * ACB_ECUDA. */
+int acb_streams_new_words(const acb_table *tb, int64_t n_streams, int leftmost, const uint32_t *bits, int64_t n_bits,
+                          acb_streams **out);
+
+/* The whole-word records in chunk order, then end_index ascending, then longest key first; end_index is relative to the
+ * chunk (>= -1: the letter after a match may arrive a feed later).  Arguments and count as acb_streams_feed_leftmost_*;
+ * the host entry checks ids and offsets (ACB_EINVAL) before anything runs, and returns ACB_EOVERFLOW with the exact
+ * count when the records do not fit cap. */
+int acb_streams_feed_words_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                                  const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
+                                  int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo);
+int acb_streams_feed_words_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                                const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
+                                acb_match *out, int64_t cap, int64_t *n_found, int algo);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

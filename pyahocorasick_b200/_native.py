@@ -131,6 +131,11 @@ def lib() -> ctypes.CDLL:
         "acb_scan_host_leftmost_words": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, i64, vp, i64, pi64, ctypes.c_int]),
         "acb_replace_host_words": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, i64, ctypes.c_int, vp, vp, i64, pi64]),
         "acb_last_words_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float)]),
+        "acb_streams_new_words": (ctypes.c_int, [vp, i64, ctypes.c_int, vp, i64, ctypes.POINTER(vp)]),
+        "acb_streams_feed_words_device": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, ctypes.c_int, vp, i64, vp, vp,
+                                                         ctypes.c_int]),
+        "acb_streams_feed_words_host": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, ctypes.c_int, vp, i64, pi64,
+                                                       ctypes.c_int]),
         "acb_launch_count": (i64, []),
         "acb_set_kernel_timing": (ctypes.c_int, [ctypes.c_int]),
         "acb_last_kernel_ms": (ctypes.c_float, []),
@@ -163,7 +168,8 @@ EXPORTED_SYMBOLS = [
     "acb_replacer_new", "acb_replacer_free", "acb_replace_device", "acb_replace_host", "acb_last_replace_ms",
     "acb_streams_new_leftmost", "acb_streams_feed_leftmost_device", "acb_streams_feed_leftmost_host", "acb_streams_replace_device",
     "acb_streams_replace_host", "acb_last_stream_leftmost_ms", "acb_word_filter_device", "acb_scan_host_words",
-    "acb_scan_host_leftmost_words", "acb_replace_host_words", "acb_last_words_ms", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_scan_host_leftmost_words", "acb_replace_host_words", "acb_last_words_ms", "acb_streams_new_words",
+    "acb_streams_feed_words_device", "acb_streams_feed_words_host", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

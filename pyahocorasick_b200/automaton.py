@@ -1183,7 +1183,7 @@ class Automaton:
 
     def stream_batch(self, n_streams: int, *, long: bool = False, algo: str = "auto",
                      device: Optional[int] = None, ignore_white_space: bool = False,
-                     leftmost_longest: bool = False) -> "StreamBatch":
+                     leftmost_longest: bool = False, whole_words=False) -> "StreamBatch":
         """`n_streams` independent streams searched chunk by chunk, the next chunk of many of them in one GPU call
         (StreamBatch.feed).  long=False: stream s reports what the reference's ``iter(c0)`` ... ``.set(c1)`` ...
         reports over its chunks -- every match, also those across chunk boundaries; long=True: what
@@ -1192,6 +1192,9 @@ class Automaton:
         ... reports; positions still count every letter, and a key that white space splits across chunks is found.
         leftmost_longest=True: what `find_leftmost_longest_batch` reports for each stream's whole text, delivered as
         soon as no later letter can change it (see StreamBatch.finish).
+        whole_words (see find_all_batch; not with long=True or ignore_white_space=True): only whole-word matches, what
+        find_all_batch or find_leftmost_longest_batch reports with the same option for each stream's whole text.  A
+        match is reported once the letter after it has arrived (or by `finish`), so a stream holds back one letter more.
 
         Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
         wider chunks, so the latin-1 automaton is not used)."""
@@ -1199,6 +1202,9 @@ class Automaton:
         n_streams = operator.index(n_streams)
         if n_streams < 0:
             raise ValueError("n_streams must not be negative")
+        words = self._words(whole_words)
+        if words is not None and (long or ignore_white_space):
+            raise ValueError("whole_words stream batches take neither long=True nor ignore_white_space=True")
         if leftmost_longest and (long or ignore_white_space):
             raise ValueError("leftmost_longest stream batches take neither long=True nor ignore_white_space=True")
         if algo not in (("auto", "long") if long else ("auto", "filter", "dfa")):
@@ -1207,7 +1213,7 @@ class Automaton:
             raise ValueError("iter_long has no ignore_white_space option")
         skip = self._skip_set(False) if ignore_white_space else None
         return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip,
-                           bool(leftmost_longest))
+                           bool(leftmost_longest), words)
 
     # ------------------------------------------------------------------ batch lookups (new)
     # exists / match / longest_prefix / get for a whole batch of keys, in one GPU call (acb_lookup_*).  `keys` takes the
@@ -1482,21 +1488,30 @@ class StreamBatch(_Streams):
     A leftmost_longest batch reports, over all feeds and `finish` of a stream, exactly what
     `find_leftmost_longest_batch` reports for its whole text, each match once, in chunk order then end_index
     ascending.  A match is reported by the first feed after which it starts before ``position - (longest_word - 1)``:
-    from then on no later letter can change it.  `finish` reports the rest and returns those streams to their start."""
+    from then on no later letter can change it.  `finish` reports the rest and returns those streams to their start.
+
+    A whole_words batch reports, over all feeds and `finish` of a stream, what find_all_batch (or, leftmost_longest,
+    find_leftmost_longest_batch) reports with the same whole_words for its whole text.  A find_all match is reported by
+    the first feed after which at least one letter follows it, so its end_index can be the last letter of an earlier
+    chunk; a leftmost_longest match by the first feed after which it starts before ``position - longest_word``."""
 
     def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None,
-                 leftmost_longest: bool = False):
+                 leftmost_longest: bool = False, words: Optional[tuple] = None):
         self._A = A
         self._version = A._version
         self.n_streams = n_streams
         self.long = long
         self.leftmost_longest = leftmost_longest
+        self._words = words
+        self.whole_words = words is not None
         self._algo = algo
         self._device = device
         self._pos = np.zeros(n_streams, dtype=np.int64)        # host mirror of the positions, for end_index
         self.ignore_white_space = skip is not None
         with A._gpu_lock:
-            if leftmost_longest:
+            if words is not None:
+                self._ss = self._native("new_words")
+            elif leftmost_longest:
                 self._ss = self._native("new_leftmost")
             else:
                 self._ss = self._native("new") if skip is None else self._native("new_skip", skip)
@@ -1506,7 +1521,9 @@ class StreamBatch(_Streams):
           new -> handle;  new_skip(skip set uint32) -> handle of a batch that skips those letters;  free;  reset(ids int32 or None);  positions -> int64[n_streams];
           feed(kind, data, offsets, n, stride, ids, sort) -> records (hay_id = chunk index, end_index in the chunk);
           new_leftmost -> handle of a leftmost-longest batch;
-          feed_leftmost(kind, data, offsets, n, stride, ids, final) -> its chosen records, as feed's"""
+          feed_leftmost(kind, data, offsets, n, stride, ids, final) -> its chosen records, as feed's;
+          new_words -> handle of a whole-word batch (leftmost-longest or find_all, with the batch's word set);
+          feed_words(kind, data, offsets, n, stride, ids, final) -> a find_all word batch's records, ordered, as feed's"""
         A = self._A
         if op == "new":
             ss = ctypes.c_void_p()
@@ -1514,26 +1531,32 @@ class StreamBatch(_Streams):
             return ss
         if op == "new_leftmost":
             return _new_leftmost_streams(A, self.n_streams, self._device)
+        if op == "new_words":
+            return _new_word_streams(A, self.n_streams, self._device, self.leftmost_longest, self._words)
         if op == "new_skip":
             skip, = args
             ss = ctypes.c_void_p()
             N.check(A._lib.acb_streams_new_skip(A._ensure_table(self._device), self.n_streams, N.ptr(skip), len(skip), ctypes.byref(ss)))
             return ss
-        if op in ("feed", "feed_leftmost"):
-            return self._feed(op == "feed_leftmost", *args)
+        if op in ("feed", "feed_leftmost", "feed_words"):
+            return self._feed(op, *args)
         return super()._native(op, *args)
 
-    def _feed(self, leftmost: bool, kind: str, data, offs, n: int, stride: int, ids, flag: bool) -> np.ndarray:
-        """acb_streams_feed_* (flag: sort) or, leftmost, acb_streams_feed_leftmost_* (flag: final) -> the records (hay_id =
-        chunk index, end_index in the chunk).  Overflow commits nothing: the retry is the same feed again, with room."""
+    def _feed(self, op: str, kind: str, data, offs, n: int, stride: int, ids, flag: bool) -> np.ndarray:
+        """acb_streams_feed_* (flag: sort), acb_streams_feed_leftmost_* or acb_streams_feed_words_* (flag: final) -> the
+        records (hay_id = chunk index, end_index in the chunk).  Overflow commits nothing: the retry is the same feed
+        again, with room."""
         A = self._A
         lib, algo = A._lib, N.ALGOS[self._algo]
+        ordered = op != "feed"                                  # the leftmost and word feeds order their records
         if kind == "host":
             def feed(tb, cap, found_ref):
                 args = (self._ss, tb, N.ptr(data) if data.size else None, int(data.size), None if offs is None else N.ptr(offs),
                         n, stride, None if ids is None else N.ptr(ids))
-                if leftmost:
+                if op == "feed_leftmost":
                     return lib.acb_streams_feed_leftmost_host(*args, int(flag), None, cap, found_ref, algo)
+                if op == "feed_words":
+                    return lib.acb_streams_feed_words_host(*args, int(flag), None, cap, found_ref, algo)
                 return lib.acb_streams_feed_host(*args, None, cap, found_ref, algo, int(flag))
             return A._host_records(self._device, False, n, feed)
         import torch
@@ -1545,12 +1568,14 @@ class StreamBatch(_Streams):
                     None if d_ids is None else d_ids.data_ptr())
 
             def feed(out, cap, cnt):
-                if leftmost:
+                if op == "feed_leftmost":
                     N.check(lib.acb_streams_feed_leftmost_device(*args, int(flag), out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
+                elif op == "feed_words":
+                    N.check(lib.acb_streams_feed_words_device(*args, int(flag), out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
                 else:
                     N.check(lib.acb_streams_feed_device(*args, out.data_ptr(), cap, cnt.data_ptr(), stream, algo))
             out, found = A._device_scan(t, n, feed)
-            if leftmost:
+            if ordered:
                 return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
             return A._device_records(tb, out, found, n, stride // A._L, stream, flag)
 
@@ -1569,15 +1594,15 @@ class StreamBatch(_Streams):
     def feed(self, chunks, ids=None, *, sort: bool = True) -> Matches:
         """The next chunk of some streams: chunk h continues stream ids[h] (default: stream h).  `chunks` takes the
         input forms of find_all_batch; in a list, None is an empty chunk.  Returns the matches that end inside
-        these chunks (see the class); a leftmost_longest batch returns the matches this feed settles, already in
-        order (`sort` has no effect)."""
+        these chunks (see the class); a leftmost_longest or whole_words batch returns the matches this feed settles,
+        already in order (`sort` has no effect)."""
         A = self._A
         with A._gpu_lock:
             self._check()
             b, lens = _stream_chunks(A, chunks)
             ids32 = self._ids(ids, b.n)
-            if self.leftmost_longest:
-                rec = self._native("feed_leftmost", *b[:5], ids32, False)
+            if self.leftmost_longest or self.whole_words:
+                rec = self._native("feed_leftmost" if self.leftmost_longest else "feed_words", *b[:5], ids32, False)
             else:
                 rec = self._native("feed", *b[:5], ids32, sort)
             m, sid = self._stream_matches(rec, b.n, ids32)
@@ -1585,16 +1610,18 @@ class StreamBatch(_Streams):
             return m
 
     def finish(self, ids=None) -> Matches:
-        """leftmost_longest batches: the matches streams `ids` (default: all) still hold back, as if their text ended
-        here; those streams then start again at position 0 with nothing held.  Other stream batches: ValueError."""
-        if not self.leftmost_longest:
-            raise ValueError("finish() belongs to leftmost_longest stream batches")
+        """leftmost_longest and whole_words batches: the matches streams `ids` (default: all) still hold back, as if their
+        text ended here; those streams then start again at position 0 with nothing held.  Other stream batches:
+        ValueError."""
+        if not (self.leftmost_longest or self.whole_words):
+            raise ValueError("finish() belongs to leftmost_longest and whole_words stream batches")
         A = self._A
         with A._gpu_lock:
             self._check()
             n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
             ids32 = self._ids(ids, n)
-            rec = self._native("feed_leftmost", "host", np.empty(0, np.uint8), np.zeros(n + 1, np.int64), n, 0, ids32, True)
+            rec = self._native("feed_leftmost" if self.leftmost_longest else "feed_words", "host", np.empty(0, np.uint8),
+                               np.zeros(n + 1, np.int64), n, 0, ids32, True)
             m, sid = self._stream_matches(rec, n, ids32)
             self._restart(sid)
             return m
@@ -1697,10 +1724,11 @@ class Replacer:
                 return out, out_offs
             return self._items(out, out_offs, narrow)
 
-    def stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None) -> "ReplaceStream":
+    def stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
+                     whole_words=False) -> "ReplaceStream":
         """`n_streams` streams rewritten chunk by chunk (ReplaceStream.feed): over all feeds and `finish` of a stream,
-        the output is exactly what `replace_batch` gives for its whole text.  Streams run at the automaton's full letter
-        width (unicode: 4 bytes per letter), as every stream batch does."""
+        the output is exactly what `replace_batch` gives for its whole text, with the same whole_words.  Streams run at
+        the automaton's full letter width (unicode: 4 bytes per letter), as every stream batch does."""
         A = self._A
         if self._version != A._version:
             raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
@@ -1710,7 +1738,8 @@ class Replacer:
             raise ValueError("n_streams must not be negative")
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: a replacing stream batch takes 'auto', 'filter' or 'dfa'")
-        return ReplaceStream(self, n_streams, algo, self._device if device is None else device)
+        words = A._words(whole_words)
+        return ReplaceStream(self, n_streams, algo, self._device if device is None else device, words)
 
     def _items(self, out: np.ndarray, offs: np.ndarray, narrow: bool) -> list:
         """the output haystacks as objects of the input's type"""
@@ -1778,15 +1807,18 @@ class ReplaceStream(_Streams):
     GPU.  ``feed(chunks, ids=None)`` returns, per chunk, the stream's output that no later letter can change (every
     letter before ``position - (longest_word - 1)`` and every replacement that starts there); ``finish(ids=None)``
     returns the rest and returns those streams to their start.  Concatenated, a stream's outputs are what
-    `Replacer.replace_batch` gives for its whole text.  Stale (ValueError) when the replacer is."""
+    `Replacer.replace_batch` gives for its whole text.  Stale (ValueError) when the replacer is.  With whole_words, a
+    stream holds back one letter more: the output before ``position - longest_word`` is released."""
 
-    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int):
+    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int, words: Optional[tuple] = None):
         self._R = R
         self._A = R._A
         self._version = R._version
         self.n_streams = n_streams
         self._algo = algo
         self._device = device
+        self._words = words
+        self.whole_words = words is not None
         with self._A._gpu_lock:
             self._ss = self._native("new")
 
@@ -1797,6 +1829,8 @@ class ReplaceStream(_Streams):
         A = self._A
         lib = A._lib
         if op == "new":
+            if self._words is not None:
+                return _new_word_streams(A, self.n_streams, self._device, True, self._words)
             return _new_leftmost_streams(A, self.n_streams, self._device)
         if op != "feed":
             return super()._native(op, *args)
@@ -1804,7 +1838,7 @@ class ReplaceStream(_Streams):
         tb = A._ensure_table(self._device)
         r = self._R._replacer(tb, False, self._device)
         algo = N.ALGOS[self._algo]
-        held = n * max(int(lib.acb_trie_longest_word(A._trie)) - 1, 0) * A._L     # at most what the streams hold back
+        held = n * max(int(lib.acb_trie_longest_word(A._trie)) - 1 + self.whole_words, 0) * A._L   # at most what is held back
         if kind == "host":
             size = int(data.size)
             out_offs = np.empty(n + 1, dtype=np.int64)
@@ -2136,6 +2170,15 @@ def _host_bytes(cap: int, call) -> np.ndarray:
 def _new_leftmost_streams(A: Automaton, n_streams: int, device: int):
     ss = ctypes.c_void_p()
     N.check(A._lib.acb_streams_new_leftmost(A._ensure_table(device), n_streams, ctypes.byref(ss)))
+    return ss
+
+
+def _new_word_streams(A: Automaton, n_streams: int, device: int, leftmost: bool, words: tuple):
+    """a whole-word stream batch (acb_streams_new_words) with the word set at the streams' full letter width"""
+    bits, n_bits = _word_bits(words, A._L)
+    ss = ctypes.c_void_p()
+    N.check(A._lib.acb_streams_new_words(A._ensure_table(device), n_streams, int(leftmost), N.ptr(bits) if n_bits else None,
+                                         n_bits, ctypes.byref(ss)))
     return ss
 
 

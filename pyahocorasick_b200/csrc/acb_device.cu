@@ -40,6 +40,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cassert>
 #include <mutex>
 #include <chrono>
 #include <cstdio>
@@ -2503,6 +2504,14 @@ __global__ void acb_streams_reset_kernel(const StreamsArgs a, long long n_ids) {
     if (a.kept) a.kept[s] = 0;
     if (a.state) a.state[s] = 0;
 }
+
+/* flag[ids[i]] = 0 (the left-neighbour flags of whole-word stream batches) */
+__global__ void acb_streams_clear_kernel(const int32_t *ids, long long n_ids, long long n_streams, uint8_t *flag) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_ids) return;
+    const long long s = ids[i];
+    if (s >= 0 && s < n_streams) flag[s] = 0;
+}
 } // namespace
 
 struct acb_streams {
@@ -2535,6 +2544,12 @@ struct acb_streams {
     void *d_tmp = nullptr; size_t tmp_cap = 0;                    /* cub scratch */
     unsigned long long *d_ctr = nullptr, *h_ctr = nullptr;        /* [0] full, [1] settled, [2] chosen, [3] sizes; h_ctr pinned */
     cudaEvent_t ev[12] = {};                                      /* kernel timing, a pair per stage */
+    /* whole-word batches (acb_streams_new_words; leftmost or find_all): the tail holds up to T + 1 letters, and d_left[s]
+     * = 1 when the letter just before them exists and is a word letter.  The word set belongs to the batch. */
+    int words = 0;
+    uint8_t *d_left = nullptr;
+    uint32_t *d_bits = nullptr; long long n_bits = 0;
+    unsigned long long *d_keys = nullptr; size_t keys_cap = 0;    /* find_all word feeds: sort keys, 2 per kept record */
 };
 
 static int32_t tail_letters(const acb_table *tb) { return std::max<int32_t>(tb->max_key_bytes / tb->L - 1, 0); }
@@ -2562,7 +2577,7 @@ extern "C" void acb_streams_free(acb_streams *ss) {
     cudaFree(ss->d_start); cudaFree(ss->d_end); cudaFree(ss->d_ids); cudaFree(ss->d_kept);
     cudaFree(ss->d_hold); cudaFree(ss->d_soff); cudaFree(ss->d_aux); cudaFree(ss->d_stage); cudaFree(ss->d_win); cudaFree(ss->d_ts);
     cudaFree(ss->d_full); cudaFree(ss->d_settled); cudaFree(ss->d_flag); cudaFree(ss->d_chosen); cudaFree(ss->d_tmp);
-    cudaFree(ss->d_ctr);
+    cudaFree(ss->d_ctr); cudaFree(ss->d_left); cudaFree(ss->d_bits); cudaFree(ss->d_keys);
     if (ss->h_ctr) cudaFreeHost(ss->h_ctr);
     for (cudaEvent_t e : ss->ev) if (e) cudaEventDestroy(e);
     delete ss;
@@ -2599,6 +2614,7 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
                         int64_t *d_count, cudaStream_t s, int algo) {
     if (!ss || !tb || !d_count || total < 0 || n_chunks < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (ss->leftmost) { acb_set_error("a leftmost-longest stream batch takes acb_streams_feed_leftmost_* or acb_streams_replace_*"); return ACB_EINVAL; }
+    if (ss->words) { acb_set_error("a whole-word stream batch takes acb_streams_feed_words_*"); return ACB_EINVAL; }
     int rc = streams_check_table(ss, tb);
     if (rc != ACB_OK) return rc;
     if (n_chunks > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, ss->n); return ACB_EINVAL; }
@@ -2692,6 +2708,7 @@ extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8
     *n_found = 0;
     tb->h_out_n = 0;
     if (ss->leftmost) { acb_set_error("a leftmost-longest stream batch takes acb_streams_feed_leftmost_* or acb_streams_replace_*"); return ACB_EINVAL; }
+    if (ss->words) { acb_set_error("a whole-word stream batch takes acb_streams_feed_words_*"); return ACB_EINVAL; }
     int rc;
     if (ids && (rc = check_ids(ss, ids, n_chunks))) return rc;
     if ((rc = streams_check_table(ss, tb))) return rc;
@@ -2725,8 +2742,13 @@ extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n)
         if (ss->d_hold) a.kept = ss->d_hold;                     /* leftmost (no skip set): nothing held back either */
         acb_streams_reset_kernel<<<(unsigned)((n + 255) / 256), 256>>>(a, n);
         if ((rc = launched("stream reset"))) return rc;
+        if (ss->d_left) {                                        /* whole words: no letter before the start */
+            acb_streams_clear_kernel<<<(unsigned)((n + 255) / 256), 256>>>(ss->d_ids, n, ss->n, ss->d_left);
+            if ((rc = launched("stream reset"))) return rc;
+        }
     }
     if (!ids && ss->d_hold) CUDA_TRY(cudaMemset(ss->d_hold, 0, (size_t)std::max<long long>(ss->n, 1) * sizeof(long long)));
+    if (!ids && ss->d_left) CUDA_TRY(cudaMemset(ss->d_left, 0, (size_t)std::max<long long>(ss->n, 1)));
     CUDA_TRY(cudaDeviceSynchronize());
     return ACB_OK;
 }
@@ -4169,6 +4191,93 @@ __global__ void acb_sl_commit_kernel(const __grid_constant__ SlArgs a, const uns
         a.hold[s] = a.final ? 0 : keep;
     }
 }
+
+/* Whole-word stream feeds (DESIGN section 4.15) run the pipeline above with T + 1 held letters (SlArgs::T) and these
+ * kernels in place of the frontier flags (and, for find_all batches, of the selection) */
+struct SwArgs {
+    SlArgs a;
+    uint8_t *left;                                         /* [n_streams] the letter before the held ones is a word letter */
+    const uint32_t *bits; long long n_bits;                /* the word set, as WwArgs */
+    const int32_t *key_len;
+    int leftmost;
+};
+
+/* letter v is in the word set; tab: the bitmap (in shared memory for 1-byte letters) */
+template <int L>
+__device__ __forceinline__ bool sw_word(const SwArgs &w, const uint32_t *tab, uint32_t v) {
+    if ((long long)v >= w.n_bits) return false;
+    return ((L == 1 ? tab[v >> 5] : __ldg(w.bits + (v >> 5))) >> (v & 31) & 1u) != 0;
+}
+
+/* flag[i]: record i of the staged full list lies in the feed's window and is a whole-word match.  Window: leftmost, it
+ * starts before the frontier staged - (T + 1) (every record on a final feed); find_all, it ends in [hold - 1, staged - 2]
+ * (staged - 1 on a final feed).  A record that starts at staged letter 0 takes its left neighbour from w.left.  A kept
+ * record of a non-final feed never ends on the last staged letter, so its right neighbour is staged. */
+template <int L>
+__global__ void __launch_bounds__(256) acb_sw_flag_kernel(const __grid_constant__ SwArgs w, const acb_match *full,
+                                                          const unsigned long long *count, long long cap, uint8_t *flag) {
+    __shared__ uint32_t s_bits[8];                         /* 1-byte letters: the whole set */
+    if (L == 1) {
+        if (threadIdx.x < 8) s_bits[threadIdx.x] = (long long)threadIdx.x * 32 < w.n_bits ? w.bits[threadIdx.x] : 0u;
+        __syncthreads();
+    }
+    const SlArgs &a = w.a;
+    const long long m = min((long long)*count, cap);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (long long)gridDim.x * blockDim.x) {
+        bool keep = false;
+        if (i < m) {
+            const acb_match r = full[i];
+            const long long b0 = a.soff[r.hay_id], staged = (a.soff[r.hay_id + 1] - b0) / L, s = sl_stream(a, r.hay_id);
+            const long long end = r.end_index, start = end - __ldg(w.key_len + r.key_id) + 1;
+            if (w.leftmost) keep = a.final || start < staged - a.T;
+            else keep = end >= (s < 0 ? 0 : a.hold[s]) - 1 && end < staged - 1 + a.final;
+#ifdef ACB_DEBUG
+            assert(!keep || a.final || end + 1 < staged);
+#endif
+            if (keep) keep = !(start == 0 ? (s >= 0 && w.left[s]) : sw_word<L>(w, s_bits, ww_letter<L>(a.stage + b0 + (start - 1) * L)));
+            if (keep && end + 1 < staged) keep = !sw_word<L>(w, s_bits, ww_letter<L>(a.stage + b0 + (end + 1) * L));
+        }
+        flag[i] = keep;
+    }
+}
+
+/* the sort key of a kept record: hay | end | (max_len - len), or without the hay when hay_shift < 0 */
+__global__ void acb_sw_key_kernel(const acb_match *rec, long long n, const int32_t *key_len, int bl, int max_len, int hay_shift,
+                                  unsigned long long *keys) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const acb_match m = rec[i];
+        const unsigned long long k = (unsigned long long)(uint32_t)m.end_index << bl | (unsigned long long)(max_len - __ldg(key_len + m.key_id));
+        keys[i] = hay_shift < 0 ? k : ((unsigned long long)(uint32_t)m.hay_id << hay_shift | k);
+    }
+}
+
+/* out[i] = rec[i] with end_index relative to its chunk, for i < cap; *count = m */
+__global__ void acb_sw_emit_kernel(const __grid_constant__ SlArgs a, const acb_match *rec, long long m, acb_match *out, long long cap,
+                                   unsigned long long *count) {
+    const long long first = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (first == 0) *count = (unsigned long long)m;
+    for (long long i = first; i < min(m, cap); i += (long long)gridDim.x * blockDim.x) {
+        acb_match r = rec[i];
+        const long long s = sl_stream(a, r.hay_id);
+        r.end_index = (int32_t)(r.end_index - (s < 0 ? 0 : a.hold[s]));
+        out[i] = r;
+    }
+}
+
+/* under the commit's condition: left[s] = staged letter X_new - 1 is a word letter (unchanged when X_new is the staged
+ * start; 0 after a final feed) */
+template <int L>
+__global__ void acb_sw_left_kernel(const __grid_constant__ SwArgs w, const unsigned long long *count, long long cap,
+                                   const long long *total, long long out_cap) {
+    if ((count && *count > (unsigned long long)cap) || (total && *total > out_cap)) return;
+    const SlArgs &a = w.a;
+    for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h < a.n; h += (long long)gridDim.x * blockDim.x) {
+        const long long s = sl_stream(a, h), x = a.xn[h];
+        if (s < 0) continue;
+        if (a.final) w.left[s] = 0;
+        else if (x > 0) w.left[s] = sw_word<L>(w, w.bits, ww_letter<L>(a.stage + a.soff[h] + (x - 1) * L));
+    }
+}
 } // namespace
 
 extern "C" int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out) {
@@ -4191,17 +4300,48 @@ extern "C" int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, 
     return ACB_OK;
 }
 
+extern "C" int acb_streams_new_words(const acb_table *tb, int64_t n_streams, int leftmost, const uint32_t *bits, int64_t n_bits,
+                                     acb_streams **out) {
+    if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    int rc = check_words(tb, bits, n_bits);
+    if (rc != ACB_OK || (rc = acb_streams_new_leftmost(tb, n_streams, out))) return rc;
+    acb_streams *ss = *out;
+    ss->leftmost = leftmost ? 1 : 0;
+    ss->words = 1;
+    ss->n_bits = n_bits;
+    const size_t n = (size_t)std::max<int64_t>(n_streams, 1), words = ((size_t)n_bits + 31) / 32;
+    cudaFree(ss->d_tail);                                  /* room for T + 1 held letters */
+    ss->d_tail = nullptr;
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ss->d_tail), n * (ss->T + 1) * ss->L);
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ss->d_left), n);
+    if (e == cudaSuccess) e = cudaMemset(ss->d_left, 0, n);
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ss->d_bits), std::max<size_t>(words, 1) * sizeof(uint32_t));
+    if (e == cudaSuccess && words) e = cudaMemcpy(ss->d_bits, bits, words * sizeof(uint32_t), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        acb_set_error("allocating %lld streams: %s", (long long)n_streams, cudaGetErrorString(e));
+        acb_streams_free(ss);
+        *out = nullptr;
+        return ACB_ECUDA;
+    }
+    return ACB_OK;
+}
+
 extern "C" int acb_last_stream_leftmost_ms(float *ms, int32_t n) {
     if (!ms || n < 0 || n > 6) { acb_set_error("bad argument"); return ACB_EINVAL; }
     for (int i = 0; i < n; i++) ms[i] = g_sl_ms[i];
     return ACB_OK;
 }
 
-/* the arguments every leftmost feed checks before anything runs */
+/* the arguments every leftmost feed (find_all_words: every find_all word feed) checks before anything runs */
 static int sl_check(const acb_streams *ss, const acb_table *tb, int64_t total, const void *offsets, int64_t n, int64_t stride,
-                    int *algo) {
+                    int *algo, bool find_all_words = false) {
     if (!ss || !tb || total < 0 || n < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
-    if (!ss->leftmost) { acb_set_error("not a leftmost-longest stream batch (acb_streams_new_leftmost)"); return ACB_EINVAL; }
+    if (find_all_words && (ss->leftmost || !ss->words)) {
+        acb_set_error("not a find_all whole-word stream batch (acb_streams_new_words with leftmost = 0)");
+        return ACB_EINVAL;
+    }
+    if (!find_all_words && !ss->leftmost) { acb_set_error("not a leftmost-longest stream batch (acb_streams_new_leftmost)"); return ACB_EINVAL; }
     int rc = streams_check_table(ss, tb);
     if (rc != ACB_OK) return rc;
     if (n > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n, ss->n); return ACB_EINVAL; }
@@ -4249,6 +4389,66 @@ static int sl_gather(acb_streams *ss, acb_table *tb, const SlArgs &a, bool stage
     return launched("stream gather");
 }
 
+static SwArgs sw_args(const acb_streams *ss, const acb_table *tb, const SlArgs &a) {
+    SwArgs w;
+    w.a = a; w.left = ss->d_left; w.bits = ss->d_bits; w.n_bits = ss->n_bits; w.key_len = tb->d_keylen; w.leftmost = ss->leftmost;
+    return w;
+}
+
+/* a word feed's window and word flags over the first min(*count, fcap) records of the full list */
+static int sw_flags(acb_streams *ss, acb_table *tb, const SlArgs &a, long long fcap, cudaStream_t s) {
+    const SwArgs w = sw_args(ss, tb, a);
+    const unsigned grid = (unsigned)std::min<long long>((fcap + 255) / 256, (long long)tb->sm_count * 16);
+    if (ss->L == 1) acb_sw_flag_kernel<1><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
+    else if (ss->L == 2) acb_sw_flag_kernel<2><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
+    else acb_sw_flag_kernel<4><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
+    return launched("stream word flags");
+}
+
+/* a find_all word feed's m kept records (ss->d_settled, staged coordinates) in the reference order -- chunk, end, longest
+ * key first -- and rebased to their chunks into d_out (the first cap of them); *d_count = m.  One radix pass when
+ * chunk | end | length fit 64 bits, else two stable ones (end | length, then chunk). */
+static int sw_order(acb_streams *ss, acb_table *tb, const SlArgs &a, unsigned long long m, long long staged, acb_match *d_out,
+                    int64_t cap, unsigned long long *d_count, cudaStream_t s) {
+    if (m == 0) return ACB_OK;                             /* *d_count is 0 already */
+    const int max_len = tb->max_key_bytes / tb->L, mi = (int)m;
+    const int bh = bits_for((unsigned long long)std::max<long long>(a.n - 1, 1));
+    const int be = bits_for((unsigned long long)std::max<long long>(staged / a.L, 1)), bl = bits_for((unsigned long long)max_len);
+    const bool one_pass = bh + be + bl <= 64;
+    int rc = ensure(&ss->d_keys, &ss->keys_cap, 2 * (size_t)m);
+    if (rc) return rc;
+    unsigned long long *k0 = ss->d_keys, *k1 = ss->d_keys + m;
+    size_t temp = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, temp, k0, k1, ss->d_settled, ss->d_full, mi, 0, 64, s));
+    if ((rc = sl_tmp(ss, temp))) return rc;
+    const unsigned grid = (unsigned)std::min<long long>(((long long)m + 255) / 256, (long long)tb->sm_count * 16);
+    acb_sw_key_kernel<<<grid, 256, 0, s>>>(ss->d_settled, (long long)m, tb->d_keylen, bl, max_len, one_pass ? be + bl : -1, k0);
+    if ((rc = launched("stream word sort key"))) return rc;
+    temp = ss->tmp_cap;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(ss->d_tmp, temp, k0, k1, ss->d_settled, ss->d_full, mi, 0, one_pass ? bh + be + bl : be + bl, s));
+    acb_match *sorted = ss->d_full;
+    if (!one_pass) {
+        acb_sortkey_kernel<kKeyHay><<<(unsigned)((m + 255) / 256), 256, 0, s>>>(ss->d_full, (long long)m, tb->d_keylen, be, bl, max_len, k0);
+        if ((rc = launched("stream word sort key"))) return rc;
+        temp = ss->tmp_cap;
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(ss->d_tmp, temp, k0, k1, ss->d_full, ss->d_settled, mi, 0, bh, s));
+        sorted = ss->d_settled;
+    }
+    acb_sw_emit_kernel<<<grid, 256, 0, s>>>(a, sorted, (long long)m, d_out, cap, d_count);
+    return launched("stream word emit");
+}
+
+/* the left-neighbour flags of the fed streams, under the commit's condition */
+static int sw_left(acb_streams *ss, acb_table *tb, const SlArgs &a, const unsigned long long *count, long long cap,
+                   const long long *total, long long out_cap, cudaStream_t s) {
+    const SwArgs w = sw_args(ss, tb, a);
+    const unsigned grid = (unsigned)std::min<long long>((a.n + 255) / 256, (long long)tb->sm_count * 16);
+    if (ss->L == 1) acb_sw_left_kernel<1><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
+    else if (ss->L == 2) acb_sw_left_kernel<2><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
+    else acb_sw_left_kernel<4><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
+    return launched("stream word edge");
+}
+
 /* The leftmost feed on DEVICE buffers, both forms.  r == nullptr: the chosen records go to d_out (cap, *d_count,
  * end_index relative to the chunk); else the decided windows are rewritten into d_rout (d_rout_off, *d_rtotal,
  * out_cap).  Waits for the staged size, for the full list's size, and (replacing) for the windows' size. */
@@ -4269,7 +4469,7 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     if ((rc = ensure(&ss->d_soff, &ss->soff_cap, N + 1)) || (rc = ensure(&ss->d_aux, &ss->aux_cap, 3 * N + 1))) return rc;
     SlArgs a;
     memset(&a, 0, sizeof(a));
-    a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.hold = ss->d_hold; a.tail = ss->d_tail; a.T = ss->T; a.L = ss->L;
+    a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.hold = ss->d_hold; a.tail = ss->d_tail; a.T = ss->T + ss->words; a.L = ss->L;
     a.chunks = d_chunks; a.off = reinterpret_cast<const long long *>(d_off); a.stride = stride; a.n = n;
     a.soff = ss->d_soff; a.last = ss->d_aux; a.xn = ss->d_aux + N; a.woff = ss->d_aux + 2 * N; a.final = final ? 1 : 0;
     const long long most = (long long)tb->sm_count * 16;
@@ -4298,9 +4498,13 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
                                             reinterpret_cast<int64_t *>(ss->d_ctr), s, algo)))
             return rc;
         if ((rc = timing_mark(&ss->ev[3], s)) || (rc = timing_mark(&ss->ev[4], s))) return rc;
-        acb_sl_flag_kernel<<<(unsigned)std::min<long long>(((long long)fcap + 255) / 256, most), 256, 0, s>>>(a, ss->d_full, ss->d_ctr,
-                                                                                                       (long long)fcap, tb->d_keylen, ss->d_flag);
-        if ((rc = launched("stream frontier flags"))) return rc;
+        if (ss->words) {
+            if ((rc = sw_flags(ss, tb, a, (long long)fcap, s))) return rc;
+        } else {
+            acb_sl_flag_kernel<<<(unsigned)std::min<long long>(((long long)fcap + 255) / 256, most), 256, 0, s>>>(a, ss->d_full, ss->d_ctr,
+                                                                                                           (long long)fcap, tb->d_keylen, ss->d_flag);
+            if ((rc = launched("stream frontier flags"))) return rc;
+        }
         size_t temp = 0;
         CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, temp, ss->d_full, ss->d_flag, ss->d_settled, ss->d_ctr + 1, (int)fcap, s));
         if ((rc = sl_tmp(ss, temp))) return rc;
@@ -4326,13 +4530,16 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     }
     const int64_t max_letters = std::max<int64_t>(staged / ss->L, 1);
     if ((rc = timing_mark(&ss->ev[6], s))) return rc;
-    if (m && (rc = acb_leftmost_longest_device(tb, ss->d_settled, (int64_t)m, n, max_letters, chosen, ccap,
-                                               reinterpret_cast<int64_t *>(ccount), s)))
+    if (!ss->leftmost) {                                   /* a find_all word feed returns every kept record, ordered */
+        if ((rc = sw_order(ss, tb, a, m, staged, d_out, cap, ccount, s))) return rc;
+    } else if (m && (rc = acb_leftmost_longest_device(tb, ss->d_settled, (int64_t)m, n, max_letters, chosen, ccap,
+                                                      reinterpret_cast<int64_t *>(ccount), s))) {
         return rc;
+    }
     if ((rc = timing_mark(&ss->ev[7], s))) return rc;
     /* 5. the new X per chunk, and the windows of a replacing feed */
     CUDA_TRY(cudaMemsetAsync(a.last, 0xff, N * sizeof(long long), s));
-    if (m) {
+    if (m && ss->leftmost) {
         acb_sl_last_kernel<<<(unsigned)std::min<long long>(((long long)m + 255) / 256, most), 256, 0, s>>>(a, chosen, ccount, ccap, r ? 0 : 1);
         if ((rc = launched("stream last chosen"))) return rc;
     }
@@ -4349,6 +4556,9 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     }
     /* 6. commit */
     if ((rc = timing_mark(&ss->ev[10], s))) return rc;
+    if (ss->words && (rc = sw_left(ss, tb, a, r ? nullptr : ccount, ccap, r ? reinterpret_cast<const long long *>(d_rtotal) : nullptr,
+                                   out_cap, s)))
+        return rc;
     acb_sl_commit_kernel<<<(unsigned)((n * kSlLanes + 255) / 256), 256, 0, s>>>(a, r ? nullptr : ccount, ccap,
                                                                           r ? reinterpret_cast<const long long *>(d_rtotal) : nullptr, out_cap);
     if ((rc = launched("stream commit")) || (rc = timing_mark(&ss->ev[11], s)) || (rc = timing_ms(ss->ev[6], ss->ev[7], &g_sl_ms[3])) ||
@@ -4357,14 +4567,28 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     return timing_ms(ss->ev[10], ss->ev[11], &g_sl_ms[5]);
 }
 
-extern "C" int acb_streams_feed_leftmost_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
-                                                const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
-                                                int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
-    int rc = sl_check(ss, tb, total_bytes, d_offsets, n_chunks, stride_bytes, &algo);
+static int sl_feed_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes, const int64_t *d_offsets,
+                          int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids, int final, acb_match *d_out, int64_t cap,
+                          int64_t *d_count, void *stream, int algo, bool find_all_words) {
+    int rc = sl_check(ss, tb, total_bytes, d_offsets, n_chunks, stride_bytes, &algo, find_all_words);
     if (rc) return rc;
     if (!d_count || cap < 0 || (cap > 0 && !d_out) || (total_bytes && !d_chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     return sl_feed(ss, tb, nullptr, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, d_out, cap, d_count,
                    nullptr, nullptr, 0, nullptr, reinterpret_cast<cudaStream_t>(stream), algo);
+}
+
+extern "C" int acb_streams_feed_leftmost_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                                                const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
+                                                int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    return sl_feed_device(ss, tb, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, d_out, cap, d_count, stream,
+                          algo, false);
+}
+
+extern "C" int acb_streams_feed_words_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
+                                             const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
+                                             int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    return sl_feed_device(ss, tb, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, d_out, cap, d_count, stream,
+                          algo, true);
 }
 
 extern "C" int acb_streams_replace_device(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
@@ -4389,10 +4613,10 @@ static int sl_upload(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int6
     return upload_ids(ss, ids, n, tb->stream);
 }
 
-extern "C" int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
-                                              const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
-                                              acb_match *out, int64_t cap, int64_t *n_found, int algo) {
-    int rc = sl_check(ss, tb, total_bytes, offsets, n_chunks, stride_bytes, &algo);
+static int sl_feed_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes, const int64_t *offsets,
+                        int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final, acb_match *out, int64_t cap, int64_t *n_found,
+                        int algo, bool find_all_words) {
+    int rc = sl_check(ss, tb, total_bytes, offsets, n_chunks, stride_bytes, &algo, find_all_words);
     if (rc) return rc;
     if (!n_found || cap < 0 || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
@@ -4408,6 +4632,18 @@ extern "C" int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, co
     return read_back(tb, tb->w_count, tb->w_out, cap, 0, n_chunks, 0, out, n_found, s);
 }
 
+extern "C" int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                                              const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
+                                              acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    return sl_feed_host(ss, tb, chunks, total_bytes, offsets, n_chunks, stride_bytes, ids, final, out, cap, n_found, algo, false);
+}
+
+extern "C" int acb_streams_feed_words_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
+                                           const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
+                                           acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    return sl_feed_host(ss, tb, chunks, total_bytes, offsets, n_chunks, stride_bytes, ids, final, out, cap, n_found, algo, true);
+}
+
 extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
                                         const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
                                         int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap, int64_t *total) {
@@ -4420,7 +4656,7 @@ extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_ta
     if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids, &d_off))) return rc;
     cudaStream_t s = tb->stream;
     if ((rc = ensure(&tb->r_off, &tb->r_off_cap, (size_t)n_chunks + 2))) return rc;
-    const int64_t guess = total_bytes + total_bytes / 4 + n_chunks * (int64_t)ss->T * ss->L + 4096;
+    const int64_t guess = total_bytes + total_bytes / 4 + n_chunks * (int64_t)(ss->T + ss->words) * ss->L + 4096;
     if ((rc = ensure(&tb->r_out, &tb->r_out_cap, (size_t)std::max<int64_t>(std::min(out_cap, guess), 16)))) return rc;
     for (;;) {                                             /* an output that fits out_cap but not the device buffer: grow, repeat */
         const int64_t dev_cap = std::min<int64_t>(out_cap, (int64_t)tb->r_out_cap);
