@@ -210,6 +210,20 @@ int  acb_table_upload(const acb_trie *t, int device, acb_table **out);
 void acb_table_free(acb_table *tb);
 int64_t acb_table_device_bytes(const acb_table *tb);
 
+/* Test hooks: the scan kernels' tile rings, and launches on fewer SMs, so that a test can make one CTA go round its
+ * ring many times on a short text.
+ * acb_scan_geometry: the ring of acb_pair_kernel (pair != 0) or of acb_stream_kernel, from the constants the kernels
+ *   are compiled with: out[0..5] = slice bytes, tile bytes, stages, consumer warps, tile claims in flight per CTA,
+ *   look-ahead bytes copied past a tile.  n is the room in out (at least 6).  Needs no device.
+ * acb_table_set_cta_limit: n = 0 (the default) launches as the device allows, one persistent scan CTA per SM; n > 0
+ *   launches as if the device had min(n, SMs) SMs: the grid of the persistent scan kernels and the bound of the
+ *   grid-stride loops (a few blocks per SM) shrink, allocations sized by the SM count stay.  Results are the same.
+ * acb_table_scan_grid: the launch of a filter scan of one segment of total_bytes (at most 2 GiB) under the current
+ *   limit: its CTAs and the tiles they claim.  The scans compute their launch shape with this very function. */
+int acb_scan_geometry(int pair, int32_t *out, int32_t n);
+int acb_table_set_cta_limit(acb_table *tb, int32_t n);
+int acb_table_scan_grid(const acb_table *tb, int64_t total_bytes, int32_t *grid, int64_t *n_tiles);
+
 /* which scan kernel to run */
 enum {
     ACB_ALGO_AUTO   = 0,

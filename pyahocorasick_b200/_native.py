@@ -84,6 +84,9 @@ def lib() -> ctypes.CDLL:
         "acb_table_upload": (ctypes.c_int, [vp, ctypes.c_int, ctypes.POINTER(vp)]),
         "acb_table_free": (None, [vp]),
         "acb_table_device_bytes": (i64, [vp]),
+        "acb_scan_geometry": (ctypes.c_int, [ctypes.c_int, pi32, i32]),          # test hooks (acb200.h)
+        "acb_table_set_cta_limit": (ctypes.c_int, [vp, i32]),
+        "acb_table_scan_grid": (ctypes.c_int, [vp, i64, pi32, pi64]),
         "acb_scan_device": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, i64, vp, vp, ctypes.c_int]),
         "acb_scan_host": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, i64, pi64, ctypes.c_int, ctypes.c_int]),
         "acb_copy_records": (ctypes.c_int, [vp, vp, i64]),
@@ -160,6 +163,7 @@ EXPORTED_SYMBOLS = [
     "acb_trie_content_hash", "acb_trie_flat_save", "acb_trie_flat_load",
     "acb_trie_export_nodes", "acb_trie_import_nodes", "acb_node_records_span",
     "acb_device_count", "acb_table_upload", "acb_table_free", "acb_table_device_bytes",
+    "acb_scan_geometry", "acb_table_set_cta_limit", "acb_table_scan_grid",
     "acb_scan_device", "acb_scan_host", "acb_copy_records", "acb_take_records", "acb_release_records", "acb_sort_matches_device", "acb_table_set_long_state", "acb_table_get_long_state",
     "acb_streams_new", "acb_streams_free", "acb_streams_reset", "acb_streams_feed_device", "acb_streams_feed_host",
     "acb_streams_positions", "acb_space_letters", "acb_scan_device_skip", "acb_scan_host_skip", "acb_streams_new_skip",

@@ -1326,7 +1326,7 @@ __global__ void acb_flag_goto_kernel(int32_t *gto, const int32_t *key_of, size_t
 
 struct acb_table {
     int device = 0;
-    int sm_count = 0;
+    int sm_count = 0;                        /* sizes the per-CTA allocations (d_cand); launches take grid_sms() */
     int32_t S = 0, K = 0, L = 1, n_keys = 0, gram = 1, stride = 1, log1 = 13, log3 = 0, logA = 10, filter_flags = 0, log2b = 0;
     int32_t min_key_bytes = 0, max_key_bytes = 0;
     uint32_t mul1[ACB_MAX_WINDOWS], mul2[ACB_MAX_WINDOWS];
@@ -1393,6 +1393,7 @@ struct acb_table {
     acb_match *ww_out = nullptr; size_t ww_out_cap = 0;  /* the host routes: the whole-word records */
     cudaEvent_t ww_done = nullptr;                       /* the last filter's work on ww_buf has been issued before it */
     cudaEvent_t ww_ev[2] = {};                           /* kernel timing of the filter */
+    int cta_limit = 0;                       /* acb_table_set_cta_limit: 0, or the SMs the launches act as if the device had */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1508,6 +1509,34 @@ extern "C" int acb_table_upload(const acb_trie *t, int device, acb_table **out) 
 }
 
 extern "C" int64_t acb_table_device_bytes(const acb_table *tb) { return tb ? tb->dev_bytes : 0; }
+
+/* the SMs a launch spreads over: one persistent CTA each, and the bound of the grid-stride loops */
+static long long grid_sms(const acb_table *tb) {
+    return tb->cta_limit > 0 ? std::min(tb->cta_limit, tb->sm_count) : tb->sm_count;
+}
+
+extern "C" int acb_table_set_cta_limit(acb_table *tb, int32_t n) {
+    if (!tb || n < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    tb->cta_limit = n;
+    return ACB_OK;
+}
+
+extern "C" int acb_scan_geometry(int pair, int32_t *out, int32_t n) {
+    if (!out || n < 6) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    const int32_t g[2][6] = {{kSliceBytes, kTileBytes, kStages, kConsumers, kClaimDepth, kLook},
+                             {kSliceBytes, kPairTileBytes, kPairStages, kPairConsumers, kClaimDepth, kLook}};
+    memcpy(out, g[pair != 0], sizeof(g[0]));
+    return ACB_OK;
+}
+
+/* the launch shape of a filter scan of one segment (<= kSegBytes): tiles of the kernel's ring, one CTA per SM */
+extern "C" int acb_table_scan_grid(const acb_table *tb, int64_t total_bytes, int32_t *grid, int64_t *n_tiles) {
+    if (!tb || !grid || !n_tiles || total_bytes < 0 || total_bytes > kSegBytes) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    const long long tile_bytes = (tb->filter_flags & ACB_FILTER_PAIR) ? kPairTileBytes : kTileBytes;
+    *n_tiles = (total_bytes + tile_bytes - 1) / tile_bytes;
+    *grid = (int32_t)std::min<long long>(grid_sms(tb), *n_tiles);
+    return ACB_OK;
+}
 extern "C" int64_t acb_launch_count(void) { return g_launches.load(); }
 extern "C" int acb_set_kernel_timing(int enabled) { g_timing.store(enabled ? 1 : 0); return ACB_OK; }
 extern "C" float acb_last_kernel_ms(void) { return g_last_ms; }
@@ -1629,13 +1658,15 @@ static int launch_filter_range(acb_table *tb, ScanParams &p, long long begin, lo
         tb->dev_bytes += (long long)tb->sm_count * kConsumers * kWarpCand * (long long)sizeof(uint2);
     }
     p.cand = tb->d_cand;
-    const long long tile_bytes = (tb->filter_flags & ACB_FILTER_PAIR) ? kPairTileBytes : kTileBytes;   /* the kernel's ring */
     for (long long seg = begin; seg < end; seg += kSegBytes) {
         p.seg_begin = seg;
         p.seg_end = std::min<long long>(seg + kSegBytes, end);
-        p.n_tiles = (unsigned int)((p.seg_end - p.seg_begin + tile_bytes - 1) / tile_bytes);
-        const int grid = (int)std::min<long long>(tb->sm_count, p.n_tiles);
-        int rc = launch_stream(p, tb->filter_flags, tb->stride, grid, s);
+        int32_t grid = 0;
+        int64_t n_tiles = 0;
+        int rc = acb_table_scan_grid(tb, p.seg_end - p.seg_begin, &grid, &n_tiles);
+        if (rc != ACB_OK) return rc;
+        p.n_tiles = (unsigned int)n_tiles;
+        rc = launch_stream(p, tb->filter_flags, tb->stride, grid, s);
         if (rc != ACB_OK) return rc;
     }
     return ACB_OK;
@@ -2337,7 +2368,7 @@ static int launch_remap(acb_table *tb, const CompactMeta &meta, const int64_t *d
                         int64_t *d_count, cudaStream_t s) {
     if (cap <= 0) return ACB_OK;
     const int ls = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
-    const long long grid = std::min<long long>((cap + 255) / 256, (long long)tb->sm_count * 16);
+    const long long grid = std::min<long long>((cap + 255) / 256, grid_sms(tb) * 16);
     int rc;
     if ((rc = timing_mark(&tb->k_t0, s))) return rc;
     acb_remap_kernel<<<(unsigned)grid, 256, 0, s>>>(meta, tb->k_coff, reinterpret_cast<const long long *>(d_off), stride, ls, d_out,
@@ -2852,7 +2883,7 @@ extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t t
     p.cls = tb->d_cls; p.gto = tb->d_goto; p.key_of = tb->d_keyof; p.S = tb->S;
     p.letter_shift = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
     p.key_id = d_key_id; p.prefix = d_prefix;
-    const long long grid = std::min<long long>((n_keys + kLookupThreads - 1) / kLookupThreads, (long long)tb->sm_count * 8);
+    const long long grid = std::min<long long>((n_keys + kLookupThreads - 1) / kLookupThreads, grid_sms(tb) * 8);
     if ((rc = timing_mark(&tb->ev0, s))) return rc;
     acb_lookup_kernel<<<(unsigned)grid, kLookupThreads, 0, s>>>(p);
     if ((rc = launched("lookup kernel")) || (rc = timing_mark(&tb->ev1, s))) return rc;
@@ -3068,7 +3099,7 @@ static int select_count(acb_table *tb, const SelectParams &p, int64_t n, int64_t
         CUDA_TRY(cudaMemsetAsync(d_total, 0, sizeof(int64_t), s));
         return ACB_OK;
     }
-    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, (long long)tb->sm_count * 16);
+    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, grid_sms(tb) * 16);
     acb_select_kernel<false><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
     int rc = launched("select kernel");
     if (rc != ACB_OK) return rc;
@@ -3084,7 +3115,7 @@ static int select_count(acb_table *tb, const SelectParams &p, int64_t n, int64_t
 /* pass 2: the ids, when *p.total <= p.cap */
 static int select_fill(acb_table *tb, const SelectParams &p, int64_t n, cudaStream_t s) {
     if (n == 0 || p.cap == 0) return ACB_OK;
-    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, (long long)tb->sm_count * 16);
+    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, grid_sms(tb) * 16);
     acb_select_kernel<true><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
     return launched("select kernel");
 }
@@ -3349,7 +3380,7 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     unsigned long long *status = reinterpret_cast<unsigned long long *>(carve(p, (size_t)n_tiles * 8));
     void *tmp = carve(p, temp);
     size_t tb_temp = temp;
-    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, (long long)tb->sm_count * 16);
+    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, grid_sms(tb) * 16);
     if ((rc = timing_mark(&tb->l_ev[0], s))) return rc;
     /* 1. re-key by start and sort */
     if (one_pass) {
@@ -3498,7 +3529,7 @@ extern "C" int acb_word_filter_device(acb_table *tb, const uint8_t *d_hay, int64
     WwArgs a;
     a.hay = d_hay; a.off = reinterpret_cast<const long long *>(d_offsets); a.stride = stride_bytes; a.key_len = tb->d_keylen;
     a.bits = d_bits; a.n_bits = n_bits;
-    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, (long long)tb->sm_count * 16);
+    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, grid_sms(tb) * 16);
     if ((rc = timing_mark(&tb->ww_ev[0], s))) return rc;
     if (tb->L == 1) acb_ww_flag_kernel<1><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
     else if (tb->L == 2) acb_ww_flag_kernel<2><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
@@ -3856,7 +3887,7 @@ static int rp_offsets(acb_table *tb, RpArgs &a, cudaStream_t s) {
     a.IE = reinterpret_cast<long long *>(carve(p, C * 8));
     a.RS = reinterpret_cast<long long *>(carve(p, C * 8));
     void *tmp = carve(p, temp);
-    const long long most = (long long)tb->sm_count * 16;
+    const long long most = grid_sms(tb) * 16;
     if ((rc = timing_mark(&tb->r_ev[0], s))) return rc;
     acb_rp_delta_kernel<<<(unsigned)std::min<long long>((a.cap + 256) / 256, most), 256, 0, s>>>(a);
     if ((rc = launched("replacement delta"))) return rc;
@@ -3881,10 +3912,10 @@ static int rp_write(acb_table *tb, RpArgs &a, cudaStream_t s) {
             if ((rc = ensure(&tb->r_ts, &tb->r_ts_cap, (size_t)max_tiles + 1))) return rc;
         }
         a.ts = tb->r_ts;
-        const long long most = (long long)tb->sm_count * 16;
+        const long long most = grid_sms(tb) * 16;
         acb_rp_tiles_kernel<<<(unsigned)std::min<long long>((max_tiles + 256) / 256, most), 256, 0, s>>>(a);
         if ((rc = launched("replacement tiles"))) return rc;
-        acb_rp_write_kernel<<<(unsigned)std::min<long long>(max_tiles, (long long)tb->sm_count * 8), kRpThreads, 0, s>>>(a);
+        acb_rp_write_kernel<<<(unsigned)std::min<long long>(max_tiles, grid_sms(tb) * 8), kRpThreads, 0, s>>>(a);
         if ((rc = launched("replacement write"))) return rc;
     }
     if ((rc = timing_mark(&tb->r_ev[3], s)) || (rc = scratch_done(&tb->r_done, s)) || (rc = timing_ms(tb->r_ev[0], tb->r_ev[1], &g_rp_ms[0])))
@@ -4380,10 +4411,10 @@ static int sl_gather(acb_streams *ss, acb_table *tb, const SlArgs &a, bool stage
     const long long n_tiles = (total + kSlTile - 1) / kSlTile;
     int rc = ensure(&ss->d_ts, &ss->ts_cap, (size_t)n_tiles);
     if (rc) return rc;
-    acb_sl_tiles_kernel<<<(unsigned)std::min<long long>((n_tiles + 255) / 256, (long long)tb->sm_count * 16), 256, 0, s>>>(doff, a.n, total,
+    acb_sl_tiles_kernel<<<(unsigned)std::min<long long>((n_tiles + 255) / 256, grid_sms(tb) * 16), 256, 0, s>>>(doff, a.n, total,
                                                                                                                    ss->d_ts);
     if ((rc = launched("stream gather tiles"))) return rc;
-    const unsigned grid = (unsigned)std::min<long long>(n_tiles, (long long)tb->sm_count * 8);
+    const unsigned grid = (unsigned)std::min<long long>(n_tiles, grid_sms(tb) * 8);
     if (stage) acb_sl_gather_kernel<true><<<grid, 256, 0, s>>>(a, doff, ss->d_ts, dst, total);
     else acb_sl_gather_kernel<false><<<grid, 256, 0, s>>>(a, doff, ss->d_ts, dst, total);
     return launched("stream gather");
@@ -4398,7 +4429,7 @@ static SwArgs sw_args(const acb_streams *ss, const acb_table *tb, const SlArgs &
 /* a word feed's window and word flags over the first min(*count, fcap) records of the full list */
 static int sw_flags(acb_streams *ss, acb_table *tb, const SlArgs &a, long long fcap, cudaStream_t s) {
     const SwArgs w = sw_args(ss, tb, a);
-    const unsigned grid = (unsigned)std::min<long long>((fcap + 255) / 256, (long long)tb->sm_count * 16);
+    const unsigned grid = (unsigned)std::min<long long>((fcap + 255) / 256, grid_sms(tb) * 16);
     if (ss->L == 1) acb_sw_flag_kernel<1><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
     else if (ss->L == 2) acb_sw_flag_kernel<2><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
     else acb_sw_flag_kernel<4><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
@@ -4421,7 +4452,7 @@ static int sw_order(acb_streams *ss, acb_table *tb, const SlArgs &a, unsigned lo
     size_t temp = 0;
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, temp, k0, k1, ss->d_settled, ss->d_full, mi, 0, 64, s));
     if ((rc = sl_tmp(ss, temp))) return rc;
-    const unsigned grid = (unsigned)std::min<long long>(((long long)m + 255) / 256, (long long)tb->sm_count * 16);
+    const unsigned grid = (unsigned)std::min<long long>(((long long)m + 255) / 256, grid_sms(tb) * 16);
     acb_sw_key_kernel<<<grid, 256, 0, s>>>(ss->d_settled, (long long)m, tb->d_keylen, bl, max_len, one_pass ? be + bl : -1, k0);
     if ((rc = launched("stream word sort key"))) return rc;
     temp = ss->tmp_cap;
@@ -4442,7 +4473,7 @@ static int sw_order(acb_streams *ss, acb_table *tb, const SlArgs &a, unsigned lo
 static int sw_left(acb_streams *ss, acb_table *tb, const SlArgs &a, const unsigned long long *count, long long cap,
                    const long long *total, long long out_cap, cudaStream_t s) {
     const SwArgs w = sw_args(ss, tb, a);
-    const unsigned grid = (unsigned)std::min<long long>((a.n + 255) / 256, (long long)tb->sm_count * 16);
+    const unsigned grid = (unsigned)std::min<long long>((a.n + 255) / 256, grid_sms(tb) * 16);
     if (ss->L == 1) acb_sw_left_kernel<1><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
     else if (ss->L == 2) acb_sw_left_kernel<2><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
     else acb_sw_left_kernel<4><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
@@ -4472,7 +4503,7 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.hold = ss->d_hold; a.tail = ss->d_tail; a.T = ss->T + ss->words; a.L = ss->L;
     a.chunks = d_chunks; a.off = reinterpret_cast<const long long *>(d_off); a.stride = stride; a.n = n;
     a.soff = ss->d_soff; a.last = ss->d_aux; a.xn = ss->d_aux + N; a.woff = ss->d_aux + 2 * N; a.final = final ? 1 : 0;
-    const long long most = (long long)tb->sm_count * 16;
+    const long long most = grid_sms(tb) * 16;
     const unsigned g_chunks = (unsigned)std::min<long long>((n + 256) / 256, most);
     /* 1. stage */
     acb_sl_len_kernel<<<g_chunks, 256, 0, s>>>(a);

@@ -1,19 +1,50 @@
-"""Forced filter shapes of the scan kernels, their key sets and texts, shared by test_kernel_matrix.py,
-test_record_bounds.py and test_stream_scale.py.  Not a test module.
+"""Forced filter shapes of the scan kernels, their key sets and texts, the kernels' ring geometry and the oracle
+comparison, shared by test_kernel_matrix.py, test_scan_ring.py, test_record_bounds.py and test_stream_scale.py.  Not a
+test module.
 
 A cell forces its shape (ACB_FILTER=g,s,log1,mode and ACB_FORCE_TAGMAP, only around make_automaton) on a key set whose
-shortest key is exactly gram + stride - one letter; _check_shape reads it back with filter_shape()."""
+shortest key is exactly gram + stride - one letter; _check_shape reads it back with filter_shape().  The tile a cell's
+text is planted at is the tile of the kernel the cell runs, as the library reports it (acb_scan_geometry)."""
+import collections
+import ctypes
 import dataclasses
+import functools
 
 import numpy as np
+import pytest
 
 import emul
+import oracle
 import pyahocorasick_b200 as ac
+from pyahocorasick_b200 import _native as N
+from batch_cases import triples
 
 RUN = 32                          # kLaneBytes: one lane's bytes per slice
-SLICE = 32 * RUN                  # kSliceBytes: one consumer warp's slice
-TILE = 20 * SLICE                 # kTileBytes (ACB_TILE_SLICES slices)
+SLICE = 32 * RUN                  # kSliceBytes: one consumer warp's slice (the pair kernel static-asserts 1 KiB)
 MiB = 1 << 20
+
+
+# ------------------------------------------------------------------ the kernels' tile rings
+Ring = collections.namedtuple("Ring", "slice tile stages consumers claim_depth look")
+
+
+@functools.lru_cache(maxsize=None)
+def geometry(pair):
+    """the tile ring of acb_pair_kernel (pair) or acb_stream_kernel, from the constants the library was compiled with"""
+    out = (ctypes.c_int32 * 6)()
+    N.check(N.lib().acb_scan_geometry(int(bool(pair)), out, 6))
+    return Ring(*out)
+
+
+def sentinels(ring):
+    """the fills the producer hands out when its claims run dry: one slice for every consumer warp"""
+    slices = ring.tile // ring.slice
+    return (ring.consumers + slices - 1) // slices
+
+
+def tile_bytes(cell):
+    """the tile of the kernel this cell runs on"""
+    return geometry(cell.pair).tile
 
 
 @dataclasses.dataclass(frozen=True)
@@ -33,6 +64,47 @@ class Cell:
     def name(self):
         kind = "pair" if self.pair else f"L{self.L}-g{self.g}-s{self.s}"
         return kind + (f"-l{self.log1}" if self.log1 else "") + ("-tag" if self.tagmap else "")
+
+
+# ------------------------------------------------------------------ the cells: every instantiation
+STRIDES = (1, 2, 4, 8, 16)
+PAIR_LOG1 = (13, 16, 19, 20)      # level 2 of 2^13 / 2^16 / 2^19 bits (acb_pair_kernel<0>), 2^17 (acb_pair_kernel<17>)
+GRAMS = {1: range(1, 17), 2: range(2, 17, 2), 4: range(4, 17, 4)}      # a gram is whole letters, at most 16 bytes
+
+
+def _cells():
+    """The shapes the dispatcher accepts: a stride of L * 2^k <= 16 bytes, a gram of whole letters up to 16 bytes, the
+    pair placement only for 1-byte letters at gram 4 / stride 1; level 1 and the tag bitmap on a spread of them."""
+    stream = [Cell(L, g, s) for L in (1, 2, 4) for g in GRAMS[L] for s in STRIDES if s >= L]
+    pair = [Cell(1, 4, 1, log1, True, tag) for log1 in PAIR_LOG1 for tag in (False, True)]
+    spread = ([dataclasses.replace(c, log1=13) for c in stream[0::9]] +       # saturated level 1
+              [dataclasses.replace(c, log1=20) for c in stream[3::9]] +
+              [dataclasses.replace(c, tagmap=True) for c in stream[6::9]])
+    return stream + pair + spread
+
+
+CELLS = _cells()
+IDS = [c.name for c in CELLS]
+
+
+def all_instantiations():
+    modes = ("narrow", "wide")
+    return ({("stream", nw, s, m) for nw in range(1, 5) for s in STRIDES for m in modes} |
+            {("pair", 0), ("pair", 17), ("pair-tagmap",)})
+
+
+def instantiation(fs):
+    """the kernel template a scan with these tables launches (launch_stream / launch_pair)"""
+    if fs["filter_flags"] & emul.FILTER_PAIR:
+        return ("pair", 17 if fs["log2_bits2"] == 17 else 0)
+    return ("stream", (fs["gram_bytes"] + 3) // 4, fs["stride"], "wide" if fs["filter_flags"] & emul.FILTER_WIDE else "narrow")
+
+
+def cell_instantiation(cell):
+    """the instantiation a cell forces, without building it (the pair cells with the tag bitmap count for it)"""
+    if cell.pair:
+        return ("pair-tagmap",) if cell.tagmap else ("pair", 17 if cell.log1 >= 20 else 0)
+    return ("stream", (cell.g + 3) // 4, cell.s, "wide" if cell.g % 4 == 0 else "narrow")
 
 
 # ------------------------------------------------------------------ key sets and text, in letters
@@ -132,6 +204,41 @@ def _seed(cell):
     return sum(cell.name.encode()) * 7919 + cell.L
 
 
+def _text(cell, keys, rng, n_bytes):
+    """n_bytes of text in the key alphabet (a few 0 and top letters), keys planted across every lane-run, slice and tile
+    boundary of the cell's kernel (coarser boundaries last, so that their keys survive) at every residue of the stride,
+    and one key ending on the last byte.  Returns the letters and the start letters of the boundary plants."""
+    L = cell.L
+    n = n_bytes // L
+    t = rng.choice(ALPHA[L], size=n).astype(np.uint32)
+    odd = rng.random(n)
+    t[odd < 0.01] = 0
+    t[odd > 0.99] = TOP[L]
+    plant = [k for k in keys if len(k) >= 2]
+    starts, i = [], 0
+    for step in (RUN, SLICE, tile_bytes(cell)):
+        for b in range(step, n_bytes, step):
+            k = plant[(i * 7) % len(plant)]
+            d = 1 + (i >> 1) % (cell.s // L) if i % 2 == 0 else 1 + (i * 5) % (len(k) - 1)    # letters before b
+            st = b // L - d
+            if 0 <= st and st + len(k) <= n:
+                t[st:st + len(k)] = k
+                starts.append(st)
+            i += 1
+    k = plant[i % len(plant)]
+    t[n - len(k):] = k
+    return t, np.asarray(starts, dtype=np.int64)
+
+
+def _ragged(rng, n, starts, boundaries):
+    """offsets (in letters) of a ragged batch over n letters: random cuts, cuts through planted keys and at tile
+    boundaries, runs of empty haystacks, empty haystacks first and last"""
+    cuts = [rng.integers(0, n + 1, size=120), starts[rng.integers(0, len(starts), size=80)] + 1, boundaries]
+    cuts = np.sort(np.concatenate(cuts))
+    cuts = np.concatenate([cuts, cuts[::17], cuts[::17], cuts[5::23]])           # repeated offsets: empty haystacks
+    return np.concatenate([[0, 0], np.sort(np.clip(cuts, 0, n)), [n, n]]).astype(np.int64)
+
+
 def _big_batch(rng, keys, n):
     """n bytes of text in no key's letters with keys planted every few KiB, cut into a ragged batch"""
     flat = rng.choice(np.frombuffer(b"#%&*+-", dtype=np.uint8), size=n)
@@ -141,3 +248,41 @@ def _big_batch(rng, keys, n):
     cuts = np.sort(rng.integers(0, n, size=600))
     off = np.concatenate([[0, 0], cuts, [32 * MiB] * 3, [n, n]]).astype(np.int64)
     return flat, np.sort(off)
+
+
+# ------------------------------------------------------------------ the oracle
+def _oracle_key(k, L):
+    return bytes(k) if L == 1 else k
+
+
+def _oracle(cell, keys):
+    O = oracle.OracleAutomaton()
+    for i, k in enumerate(keys):
+        O.add_word(_oracle_key(k, cell.L), i)
+    O.make_automaton()
+    return O
+
+
+def _want(O, cell, letters, off):
+    if cell.L == 1:
+        return [tuple(r) for r in O.scan_batch_bytes(letters.astype(np.uint8), off).tolist()]
+    return O.scan_batch_letters(letters, off)
+
+
+def _diff(got, want):
+    """a short account of how two record lists differ (the first divergence, a few missing and extra records)"""
+    i = next((i for i, (a, b) in enumerate(zip(got, want)) if a != b), min(len(got), len(want)))
+    sg, sw = set(got), set(want)
+    return (f"{len(got)} records, want {len(want)}; first difference at {i}: got {got[i:i + 3]}, want {want[i:i + 3]}; "
+            f"missing {sorted(sw - sg)[:5]}, extra {sorted(sg - sw)[:5]}")
+
+
+def _check_gpu(A, batch, want, what, dfa=True):
+    """filter (and DFA) records equal the oracle's in order; unsorted filter records equal them as a set"""
+    for algo in ("filter", "dfa") if dfa else ("filter",):
+        got = triples(A.find_all_batch(batch, algo=algo))
+        if got != want:
+            pytest.fail(f"{what}, {algo}: {_diff(got, want)}")
+    got = sorted(triples(A.find_all_batch(batch, algo="filter", sort=False)))
+    if got != sorted(want):
+        pytest.fail(f"{what}, filter unsorted: {_diff(got, sorted(want))}")

@@ -151,7 +151,7 @@ def test_pair_kernel_boundaries_and_dense_text():
     f = A.flat()
     assert f["filter_flags"] & 2 and f["gram_bytes"] == 4 and f["stride"] == 1          # PAIR placement -> acb_pair_kernel
     O = _oracle_for(keys)
-    n = 200 * 1024 + 37                                                                # ten 20 KiB tiles and a ragged tail
+    n = 200 * 1024 + 37                                                                # 200 slices: several tiles, a ragged tail
     hay = rng.choice(np.frombuffer(b"#%&*+-", dtype=np.uint8), size=n).astype(np.uint8)    # no key letter: only planted keys match
     k = 0
     for b in range(16, n - 32, 16):                                                     # every run / half / slice / tile boundary ...

@@ -7,8 +7,8 @@ a scan runs on follows from the key set (build_filter's cost model).  So every c
 (ACB_FILTER=g,s,log1,mode and ACB_FORCE_TAGMAP, only around make_automaton) on a key set whose shortest key is exactly
 gram + stride - one letter, checks with filter_shape() that the forcing took, and compares with the oracle:
 
-  GPU (-m gpu)  the filter and the DFA kernels on three 20 KiB tiles plus a ragged tail, with keys planted across every
-                32-byte lane run, 1 KiB slice and tile boundary and at every residue of the stride; the same bytes as a
+  GPU (-m gpu)  the filter and the DFA kernels on three tiles of the cell's kernel (as acb_scan_geometry reports its
+                ring) plus a ragged tail, with keys planted across every 32-byte lane run, 1 KiB slice and tile boundary and at every residue of the stride; the same bytes as a
                 ragged batch (empty haystacks, cuts through planted keys) and at two fixed strides; and text on which
                 every probe is a hit.  Records must equal the oracle's in order; unsorted, as a set.
   CPU           the same forced tables through tests/emul.py (the kernels restated in Python) on about 2 KiB, so that
@@ -16,123 +16,17 @@ gram + stride - one letter, checks with filter_shape() that the forcing took, an
 
 The coverage tests read the shapes back and require all 42 instantiations plus the pair kernel with the tag bitmap.
 """
-import dataclasses
-
 import numpy as np
 import pytest
 
 import emul
-import oracle
 import pyahocorasick_b200 as ac
 from batch_cases import DT, triples
-from kernel_cells import ALPHA, RUN, SLICE, TILE, TOP, Cell, _build, _check_shape, _dense, _keys, _seed
-
-STRIDES = (1, 2, 4, 8, 16)
-PAIR_LOG1 = (13, 16, 19, 20)      # level 2 of 2^13 / 2^16 / 2^19 bits (acb_pair_kernel<0>), 2^17 (acb_pair_kernel<17>)
-GRAMS = {1: range(1, 17), 2: range(2, 17, 2), 4: range(4, 17, 4)}      # a gram is whole letters, at most 16 bytes
-
-
-def _cells():
-    """The shapes the dispatcher accepts: a stride of L * 2^k <= 16 bytes, a gram of whole letters up to 16 bytes, the
-    pair placement only for 1-byte letters at gram 4 / stride 1; level 1 and the tag bitmap on a spread of them."""
-    stream = [Cell(L, g, s) for L in (1, 2, 4) for g in GRAMS[L] for s in STRIDES if s >= L]
-    pair = [Cell(1, 4, 1, log1, True, tag) for log1 in PAIR_LOG1 for tag in (False, True)]
-    spread = ([dataclasses.replace(c, log1=13) for c in stream[0::9]] +       # saturated level 1
-              [dataclasses.replace(c, log1=20) for c in stream[3::9]] +
-              [dataclasses.replace(c, tagmap=True) for c in stream[6::9]])
-    return stream + pair + spread
-
-
-CELLS = _cells()
-IDS = [c.name for c in CELLS]
-
-
-def _all_instantiations():
-    modes = ("narrow", "wide")
-    return ({("stream", nw, s, m) for nw in range(1, 5) for s in STRIDES for m in modes} |
-            {("pair", 0), ("pair", 17), ("pair-tagmap",)})
-
-
-def _instantiation(fs):
-    """the kernel template a scan with these tables launches (launch_stream / launch_pair)"""
-    if fs["filter_flags"] & emul.FILTER_PAIR:
-        return ("pair", 17 if fs["log2_bits2"] == 17 else 0)
-    return ("stream", (fs["gram_bytes"] + 3) // 4, fs["stride"], "wide" if fs["filter_flags"] & emul.FILTER_WIDE else "narrow")
-
-
-# ------------------------------------------------------------------ text, in letters
-def _text(cell, keys, rng, n_bytes):
-    """n_bytes of text in the key alphabet (a few 0 and top letters), keys planted across every lane-run, slice and tile
-    boundary (coarser boundaries last, so that their keys survive) at every residue of the stride, and one key ending
-    on the last byte.  Returns the letters and the start letters of the boundary plants."""
-    L = cell.L
-    n = n_bytes // L
-    t = rng.choice(ALPHA[L], size=n).astype(np.uint32)
-    odd = rng.random(n)
-    t[odd < 0.01] = 0
-    t[odd > 0.99] = TOP[L]
-    plant = [k for k in keys if len(k) >= 2]
-    starts, i = [], 0
-    for step in (RUN, SLICE, TILE):
-        for b in range(step, n_bytes, step):
-            k = plant[(i * 7) % len(plant)]
-            d = 1 + (i >> 1) % (cell.s // L) if i % 2 == 0 else 1 + (i * 5) % (len(k) - 1)    # letters before b
-            st = b // L - d
-            if 0 <= st and st + len(k) <= n:
-                t[st:st + len(k)] = k
-                starts.append(st)
-            i += 1
-    k = plant[i % len(plant)]
-    t[n - len(k):] = k
-    return t, np.asarray(starts, dtype=np.int64)
-
-
-def _ragged(rng, n, starts, boundaries):
-    """offsets (in letters) of a ragged batch over n letters: random cuts, cuts through planted keys and at tile
-    boundaries, runs of empty haystacks, empty haystacks first and last"""
-    cuts = [rng.integers(0, n + 1, size=120), starts[rng.integers(0, len(starts), size=80)] + 1, boundaries]
-    cuts = np.sort(np.concatenate(cuts))
-    cuts = np.concatenate([cuts, cuts[::17], cuts[::17], cuts[5::23]])           # repeated offsets: empty haystacks
-    return np.concatenate([[0, 0], np.sort(np.clip(cuts, 0, n)), [n, n]]).astype(np.int64)
-
-
-def _oracle_key(k, L):
-    return bytes(k) if L == 1 else k
-
-
-def _oracle(cell, keys):
-    O = oracle.OracleAutomaton()
-    for i, k in enumerate(keys):
-        O.add_word(_oracle_key(k, cell.L), i)
-    O.make_automaton()
-    return O
-
-
-def _want(O, cell, letters, off):
-    if cell.L == 1:
-        return [tuple(r) for r in O.scan_batch_bytes(letters.astype(np.uint8), off).tolist()]
-    return O.scan_batch_letters(letters, off)
-
-
-def _diff(got, want):
-    """a short account of how two record lists differ (the first divergence, a few missing and extra records)"""
-    i = next((i for i, (a, b) in enumerate(zip(got, want)) if a != b), min(len(got), len(want)))
-    sg, sw = set(got), set(want)
-    return (f"{len(got)} records, want {len(want)}; first difference at {i}: got {got[i:i + 3]}, want {want[i:i + 3]}; "
-            f"missing {sorted(sw - sg)[:5]}, extra {sorted(sg - sw)[:5]}")
+from kernel_cells import (CELLS, IDS, SLICE, Cell, _build, _check_gpu, _check_shape, _dense, _diff, _keys, _oracle, _ragged,
+                          _seed, _text, _want, all_instantiations, instantiation, tile_bytes)
 
 
 # ------------------------------------------------------------------ GPU: the kernels
-def _check_gpu(A, batch, want, what):
-    for algo in ("filter", "dfa"):
-        got = triples(A.find_all_batch(batch, algo=algo))
-        if got != want:
-            pytest.fail(f"{what}, {algo}: {_diff(got, want)}")
-    got = sorted(triples(A.find_all_batch(batch, algo="filter", sort=False)))
-    if got != sorted(want):
-        pytest.fail(f"{what}, filter unsorted: {_diff(got, sorted(want))}")
-
-
 _RAN = set()                  # instantiations that went through a whole GPU cell
 
 
@@ -145,7 +39,8 @@ def test_kernel_cell_matches_oracle(cell, monkeypatch):
     fs = _check_shape(A, cell)
     O = _oracle(cell, keys)
     L, dt = cell.L, DT[cell.L]
-    n_bytes = 3 * TILE + L * 1291                     # a ragged tail: not a multiple of 16, nor of a stride above L
+    tile = tile_bytes(cell)
+    n_bytes = 3 * tile + L * 1291                     # a ragged tail: not a multiple of 16, nor of a stride above L
     t, starts = _text(cell, keys, rng, n_bytes)
     n = t.size
     flat = t.astype(dt).view(np.uint8)
@@ -155,7 +50,7 @@ def test_kernel_cell_matches_oracle(cell, monkeypatch):
     assert len(want) > len(starts) // 2                # most plants survive the ones planted over them
     _check_gpu(A, (flat, one * L), want, "one haystack")
     # 2. ragged, with empty haystacks and cuts through planted keys
-    roff = _ragged(rng, n, starts, np.arange(TILE // L, n, TILE // L))
+    roff = _ragged(rng, n, starts, np.arange(tile // L, n, tile // L))
     _check_gpu(A, (flat, roff * L), _want(O, cell, t, roff), "ragged batch")
     # 3. fixed strides: a power of two (shift) and not (division)
     for stride in (512, 3000):
@@ -163,12 +58,12 @@ def test_kernel_cell_matches_oracle(cell, monkeypatch):
         foff = np.arange(k + 1, dtype=np.int64) * (stride // L)
         _check_gpu(A, flat[:k * stride].reshape(k, stride), _want(O, cell, t[:k * (stride // L)], foff), f"stride {stride}")
     # 4. every probe a hit
-    d = _dense(cell, TILE + 3 * SLICE)
+    d = _dense(cell, tile + 3 * SLICE)
     doff = np.array([0, d.size], dtype=np.int64)
     dwant = _want(O, cell, d, doff)
     assert len(dwant) > 2 * d.size                     # several periodic keys end at every letter
     _check_gpu(A, (d.astype(dt).view(np.uint8), doff * L), dwant, "dense text")
-    _RAN.add(_instantiation(fs))
+    _RAN.add(instantiation(fs))
     if cell.pair and fs["log2_bits3"]:
         _RAN.add(("pair-tagmap",))
 
@@ -179,7 +74,7 @@ def test_every_kernel_instantiation_ran(request):
     names = {it.name for it in request.session.items}
     if not all(f"test_kernel_cell_matches_oracle[{i}]" in names for i in IDS):
         pytest.skip("only part of the kernel matrix was selected")
-    assert _RAN == _all_instantiations(), sorted(_all_instantiations() - _RAN, key=str)
+    assert _RAN == all_instantiations(), sorted(all_instantiations() - _RAN, key=str)
 
 
 # ------------------------------------------------------------------ CPU: the forced tables
@@ -190,10 +85,10 @@ def test_cells_reach_every_kernel_instantiation(monkeypatch):
     for cell in CELLS:
         A = _build(cell, _keys(cell, np.random.Generator(np.random.PCG64(_seed(cell)))), monkeypatch)
         fs = _check_shape(A, cell)
-        seen.add(_instantiation(fs))
+        seen.add(instantiation(fs))
         if cell.pair and fs["log2_bits3"]:
             seen.add(("pair-tagmap",))
-    assert seen == _all_instantiations(), sorted(_all_instantiations() ^ seen, key=str)
+    assert seen == all_instantiations(), sorted(all_instantiations() ^ seen, key=str)
 
 
 @pytest.mark.parametrize("cell", CELLS, ids=IDS)

@@ -24,7 +24,7 @@ import pyahocorasick_b200 as ac
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200 import synth
 from batch_cases import triples
-from kernel_cells import TILE, SLICE, Cell, _big_batch, _build, _check_shape, _dense, _keys, _seed
+from kernel_cells import SLICE, Cell, _big_batch, _build, _check_shape, _dense, _keys, _seed, tile_bytes
 
 GUARD = 64
 MiB = 1 << 20
@@ -89,7 +89,7 @@ def _case(name, monkeypatch):
     A = _build(cell, keys, monkeypatch)
     fs = _check_shape(A, cell)
     assert fs["filter_flags"] == (0 if name == "narrow" else 1)   # acb_stream_kernel, narrow / wide mode
-    t = _dense(cell, TILE + 3 * SLICE).astype(np.uint8)            # every probe a hit: the 64-record staging spills
+    t = _dense(cell, tile_bytes(cell) + 3 * SLICE).astype(np.uint8)            # every probe a hit: the 64-record staging spills
     off = np.array([0, 7, 7, t.size // 2, t.size], dtype=np.int64)
     O = _oracle([bytes(k) for k in keys])
     return A, N.ALGO_FILTER, t, off, _tuples(O.scan_batch_bytes(t, off))
