@@ -48,6 +48,7 @@
 #include <cstring>
 #include <exception>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #define CUDA_TRY(expr)                                                                       \
@@ -1324,6 +1325,13 @@ __global__ void acb_flag_goto_kernel(int32_t *gto, const int32_t *key_of, size_t
 
 /* ------------------------------------------------------------- the table */
 
+/* Scratch that the last call's work, on any CUDA stream, may still read (scratch_take, carve, scratch_done) */
+struct Scratch {
+    void *buf = nullptr; size_t cap = 0;
+    cudaEvent_t done = nullptr;              /* the last call's work on buf has been issued before it */
+    void release() { cudaFree(buf); if (done) cudaEventDestroy(done); }
+};
+
 struct acb_table {
     int device = 0;
     int sm_count = 0;                        /* sizes the per-CTA allocations (d_cand); launches take grid_sms() */
@@ -1353,7 +1361,7 @@ struct acb_table {
     unsigned long long *h_count = nullptr;   /* pinned */
     acb_match *h_out = nullptr; size_t h_out_cap = 0;   /* pinned staging for the records */
     unsigned long long h_out_n = 0;                      /* records of the last scan held in h_out */
-    void *d_sort = nullptr; size_t sort_cap = 0;         /* radix-sort scratch */
+    Scratch sort_buf;                                    /* the record sort: keys, sorted records, cub scratch */
     /* workspace of the white-space scans (acb_scan_*_skip, stream batches with a skip set) */
     uint8_t *k_buf = nullptr; size_t k_buf_cap = 0;      /* the compacted letters */
     uint32_t *k_mask = nullptr; size_t k_mask_cap = 0;   /* keep bit per letter, one word per 32-letter group */
@@ -1375,23 +1383,20 @@ struct acb_table {
     long long *w_sel_off = nullptr; size_t w_sel_off_cap = 0;   /* acb_select_host: out offsets[n+1] then the total */
     int32_t *w_sel_id = nullptr; size_t w_sel_id_cap = 0;       /* acb_select_host: key ids */
     /* workspace of the leftmost-longest selection (acb_leftmost_longest_device), sized by the full record count */
-    void *l_buf = nullptr; size_t l_buf_cap = 0;         /* sort keys, sorted records, candidates, flags, successors, cub scratch */
+    Scratch l_buf;                                       /* sort keys, sorted records, candidates, flags, successors, cub scratch */
     unsigned long long *l_ctr = nullptr;                 /* [0] candidates, [1] chain tile counter, [2] chosen count (host route) */
     acb_match *l_out = nullptr; size_t l_out_cap = 0;    /* acb_scan_host_leftmost: the chosen records */
-    cudaEvent_t l_done = nullptr;                        /* the last selection's work on l_buf has been issued before it */
     cudaEvent_t l_ev[6] = {};                            /* kernel timing of its stages */
     /* workspace of the leftmost-longest replacement (acb_replace_device), sized by the chosen records' capacity */
-    void *r_buf = nullptr; size_t r_buf_cap = 0;         /* shifts, per-record positions, cub scratch */
+    Scratch r_buf;                                       /* shifts, per-record positions, cub scratch; its event also guards r_ts */
     long long *r_ts = nullptr; size_t r_ts_cap = 0;      /* the last record that starts at or before each tile start */
     uint8_t *r_out = nullptr; size_t r_out_cap = 0;      /* acb_replace_host: the output bytes */
     long long *r_off = nullptr; size_t r_off_cap = 0;    /* acb_replace_host: output offsets[n+1] then the total */
-    cudaEvent_t r_done = nullptr;                        /* the last replacement's work on r_buf / r_ts has been issued before it */
     cudaEvent_t r_ev[4] = {};                            /* kernel timing of the offsets pass and the write pass */
     /* workspace of the whole-word filter (acb_word_filter_device), sized by the record count */
-    void *ww_buf = nullptr; size_t ww_buf_cap = 0;       /* flags, positions, the record count, cub scratch */
+    Scratch ww_buf;                                      /* flags, positions, the record count, cub scratch */
     uint32_t *ww_bits = nullptr; size_t ww_bits_cap = 0; /* the host routes: their word bitmap */
     acb_match *ww_out = nullptr; size_t ww_out_cap = 0;  /* the host routes: the whole-word records */
-    cudaEvent_t ww_done = nullptr;                       /* the last filter's work on ww_buf has been issued before it */
     cudaEvent_t ww_ev[2] = {};                           /* kernel timing of the filter */
     int cta_limit = 0;                       /* acb_table_set_cta_limit: 0, or the SMs the launches act as if the device had */
 };
@@ -1420,7 +1425,7 @@ extern "C" void acb_table_free(acb_table *tb) {
     cudaSetDevice(tb->device);
     cudaFree(tb->d_lfail); cudaFree(tb->d_cls); cudaFree(tb->d_goto); cudaFree(tb->d_fail); cudaFree(tb->d_keyof);
     cudaFree(tb->d_outptr); cudaFree(tb->d_outidx); cudaFree(tb->d_keylen); cudaFree(tb->d_bm1); cudaFree(tb->d_bm3); cudaFree(tb->d_anchors);
-    cudaFree(tb->d_sort); cudaFree(tb->d_work); cudaFree(tb->d_cand); cudaFree(tb->d_long_final); cudaFree(tb->w_hay); cudaFree(tb->w_off); cudaFree(tb->w_out); cudaFree(tb->w_count);
+    tb->sort_buf.release(); cudaFree(tb->d_work); cudaFree(tb->d_cand); cudaFree(tb->d_long_final); cudaFree(tb->w_hay); cudaFree(tb->w_off); cudaFree(tb->w_out); cudaFree(tb->w_count);
     if (tb->h_count) cudaFreeHost(tb->h_count);
     if (tb->h_out) cudaFreeHost(tb->h_out);
     if (tb->ev0) cudaEventDestroy(tb->ev0);
@@ -1436,14 +1441,11 @@ extern "C" void acb_table_free(acb_table *tb) {
     cudaFree(tb->w_lk);
     cudaFree(tb->d_order); cudaFree(tb->d_lo); cudaFree(tb->d_cnt); cudaFree(tb->d_child_ptr); cudaFree(tb->d_child);
     cudaFree(tb->w_scan); cudaFree(tb->w_sel_off); cudaFree(tb->w_sel_id);
-    cudaFree(tb->l_buf); cudaFree(tb->l_ctr); cudaFree(tb->l_out);
-    if (tb->l_done) cudaEventDestroy(tb->l_done);
+    tb->l_buf.release(); cudaFree(tb->l_ctr); cudaFree(tb->l_out);
     for (cudaEvent_t e : tb->l_ev) if (e) cudaEventDestroy(e);
-    cudaFree(tb->r_buf); cudaFree(tb->r_ts); cudaFree(tb->r_out); cudaFree(tb->r_off);
-    if (tb->r_done) cudaEventDestroy(tb->r_done);
+    tb->r_buf.release(); cudaFree(tb->r_ts); cudaFree(tb->r_out); cudaFree(tb->r_off);
     for (cudaEvent_t e : tb->r_ev) if (e) cudaEventDestroy(e);
-    cudaFree(tb->ww_buf); cudaFree(tb->ww_bits); cudaFree(tb->ww_out);
-    if (tb->ww_done) cudaEventDestroy(tb->ww_done);
+    tb->ww_buf.release(); cudaFree(tb->ww_bits); cudaFree(tb->ww_out);
     for (cudaEvent_t e : tb->ww_ev) if (e) cudaEventDestroy(e);
     if (tb->h_kept) cudaFreeHost(tb->h_kept);
     if (tb->k_done) cudaEventDestroy(tb->k_done);
@@ -1513,6 +1515,24 @@ extern "C" int64_t acb_table_device_bytes(const acb_table *tb) { return tb ? tb-
 /* the SMs a launch spreads over: one persistent CTA each, and the bound of the grid-stride loops */
 static long long grid_sms(const acb_table *tb) {
     return tb->cta_limit > 0 ? std::min(tb->cta_limit, tb->sm_count) : tb->sm_count;
+}
+
+/* the grid of a grid-stride launch over `items`: a block per `threads` of them, at most 16 per SM */
+static unsigned blocks(const acb_table *tb, long long items, int threads = 256) {
+    return (unsigned)std::min<long long>((items + threads - 1) / threads, grid_sms(tb) * 16);
+}
+
+/* f(std::integral_constant<int, L>()) for the letter width L (1, 2 or 4), so f can launch the kernel templated on it */
+template <class F>
+static void with_width(int L, F &&f) {
+    if (L == 1) f(std::integral_constant<int, 1>());
+    else if (L == 2) f(std::integral_constant<int, 2>());
+    else f(std::integral_constant<int, 4>());
+}
+
+/* haystack h of a batch starts at byte off[h], or at h * stride without offsets; it ends where haystack h + 1 starts */
+static __device__ __forceinline__ long long hay_start(const long long *off, long long stride, long long h) {
+    return off ? __ldg(off + h) : h * stride;
 }
 
 extern "C" int acb_table_set_cta_limit(acb_table *tb, int32_t n) {
@@ -1818,13 +1838,42 @@ extern "C" void acb_release_records(acb_match *ptr, int64_t cap) {
     cudaFreeHost(ptr);
 }
 
+/* ------------------------------------------------------------ scratch */
+/* A call on stream s takes a Scratch (scratch_take): s waits for the work the last call issued on it, from any CUDA
+ * stream, and a buffer too small is freed only after s has drained.  The call carves its parts from the buffer and marks
+ * its own last reader (scratch_done).  scratch_wait / scratch_done also serve event-only guards (k_done). */
+static int scratch_wait(cudaEvent_t done, cudaStream_t s) {
+    if (done) CUDA_TRY(cudaStreamWaitEvent(s, done, 0));
+    return ACB_OK;
+}
+static int scratch_done(cudaEvent_t *done, cudaStream_t s) {
+    if (!*done) CUDA_TRY(cudaEventCreateWithFlags(done, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventRecord(*done, s));
+    return ACB_OK;
+}
+static int scratch_take(Scratch &sc, size_t need, cudaStream_t s) {
+    int rc = scratch_wait(sc.done, s);
+    if (rc || sc.cap >= need) return rc;
+    if (sc.buf) { CUDA_TRY(cudaStreamSynchronize(s)); cudaFree(sc.buf); sc.buf = nullptr; sc.cap = 0; }
+    CUDA_TRY(cudaMalloc(&sc.buf, need + need / 4));
+    sc.cap = need + need / 4;
+    return ACB_OK;
+}
+/* n T's from p, 256-byte aligned (a layout of k parts needs k * 256 bytes beyond their sizes) */
+template <typename T>
+static T *carve(char *&p, size_t n) {
+    T *r = reinterpret_cast<T *>(p);
+    p += (n * sizeof(T) + 255) & ~(size_t)255;
+    return r;
+}
+
 /* ------------------------------------------------------------ record sort */
-/* Reference order (SURVEY 3.3): haystack, then end_index ascending, then longest key first.  One
- * 64-bit radix key per record: hay_id | end_index | (max_len - len), packed into the fewest bits.
- * The leftmost-longest selection sorts by start letter instead (kKeyStart), and when that key needs more than 64 bits
- * in two stable passes: start | (max_len - len) first (kKeyStartLow), then hay_id (kKeyHay). */
+/* Reference order (SURVEY 3.3): haystack, then end_index ascending, then longest key first; start order: haystack, then
+ * start letter, then longest first.  One 64-bit radix key per record, hay_id | position | (max_len - len), packed into
+ * the fewest bits.  When those need more than 64 bits, two stable passes: position | (max_len - len) first (kKeyEndLow,
+ * kKeyStartLow), then hay_id (kKeyHay). */
 namespace {
-enum { kKeyEnd, kKeyStart, kKeyStartLow, kKeyHay };
+enum { kKeyEnd, kKeyStart, kKeyStartLow, kKeyHay, kKeyEndLow };
 
 template <int kMode>
 __global__ void acb_sortkey_kernel(const acb_match *rec, long long n, const int32_t *key_len, int be, int bl,
@@ -1835,12 +1884,57 @@ __global__ void acb_sortkey_kernel(const acb_match *rec, long long n, const int3
     if (kMode == kKeyHay) { keys[i] = (uint32_t)m.hay_id; return; }
     const int len = __ldg(key_len + m.key_id);
     const unsigned long long inv = (unsigned long long)(max_len - len);
-    const uint32_t pos = kMode == kKeyEnd ? (uint32_t)m.end_index : (uint32_t)(m.end_index - len + 1);
-    const unsigned long long hay = kMode == kKeyStartLow ? 0ULL : (unsigned long long)(uint32_t)m.hay_id << (be + bl);
+    const bool by_end = kMode == kKeyEnd || kMode == kKeyEndLow;
+    const uint32_t pos = by_end ? (uint32_t)m.end_index : (uint32_t)(m.end_index - len + 1);
+    const unsigned long long hay = kMode == kKeyStartLow || kMode == kKeyEndLow ? 0ULL : (unsigned long long)(uint32_t)m.hay_id << (be + bl);
     keys[i] = hay | ((unsigned long long)pos << bl) | inv;
 }
-int bits_for(unsigned long long v) { int b = 1; while (b < 64 && (v >> b)) b++; return b; }
 } // namespace
+
+/* the sort key's fields: bits of the haystack, of the position and of max_len - key length */
+struct SortKey {
+    int bh, be, bl, max_len;
+    int bits() const { return bh + be + bl; }
+};
+static SortKey sort_key(const acb_table *tb, int64_t n_hay, int64_t max_hay_letters) {
+    auto bits_for = [](unsigned long long v) { int b = 1; while (b < 64 && (v >> b)) b++; return b; };
+    const int max_len = tb->max_key_bytes / tb->L;
+    return {bits_for((unsigned long long)std::max<int64_t>(n_hay - 1, 1)), bits_for((unsigned long long)std::max<int64_t>(max_hay_letters, 1)),
+            bits_for((unsigned long long)max_len), max_len};
+}
+
+/* The n records of `in` into `out`, in reference order (kByStart: start order).  Keys in k0 and k1 (n each); tmp: cub
+ * scratch of temp bytes, enough for a 64-bit sort of n.  Two passes go through `mid`, and `out` may then be `in`. */
+template <bool kByStart>
+static int sort_records(acb_table *tb, const SortKey &k, const acb_match *in, acb_match *mid, acb_match *out, long long n,
+                        unsigned long long *k0, unsigned long long *k1, void *tmp, size_t temp, cudaStream_t s, const char *what) {
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    const int ni = (int)n;
+    size_t t = temp;
+    int rc;
+    if (k.bits() <= 64) {
+        acb_sortkey_kernel<kByStart ? kKeyStart : kKeyEnd><<<grid, 256, 0, s>>>(in, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
+        if ((rc = launched(what))) return rc;
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t, k0, k1, in, out, ni, 0, k.bits(), s));
+        return ACB_OK;
+    }
+    acb_sortkey_kernel<kByStart ? kKeyStartLow : kKeyEndLow><<<grid, 256, 0, s>>>(in, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
+    if ((rc = launched(what))) return rc;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t, k0, k1, in, mid, ni, 0, k.be + k.bl, s));
+    acb_sortkey_kernel<kKeyHay><<<grid, 256, 0, s>>>(mid, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
+    if ((rc = launched(what))) return rc;
+    t = temp;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t, k0, k1, mid, out, ni, 0, k.bh, s));
+    return ACB_OK;
+}
+
+/* bytes of acb_sort_matches_device's scratch for n records and keys of `bits` bits; *temp: cub's part */
+static size_t sort_scratch_bytes(int64_t n, int bits, cudaStream_t s, size_t *temp) {
+    *temp = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, *temp, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
+                                    (const acb_match *)nullptr, (acb_match *)nullptr, (int)n, 0, bits, s);
+    return 4 * 256 + (size_t)n * (2 * sizeof(unsigned long long) + sizeof(acb_match)) + *temp;
+}
 
 extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int64_t n, int64_t n_hay,
                                        int64_t max_hay_letters, void *stream) {
@@ -1850,31 +1944,18 @@ extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int6
     if (n > 0x7fffffffLL) { acb_set_error("too many records to sort on the device"); return ACB_ERANGE; }
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    const int max_len = tb->max_key_bytes / tb->L;
-    const int bh = bits_for((unsigned long long)std::max<int64_t>(n_hay - 1, 1));
-    const int be = bits_for((unsigned long long)std::max<int64_t>(max_hay_letters, 1));
-    const int bl = bits_for((unsigned long long)max_len);
-    if (bh + be + bl > 64) { acb_set_error("sort key does not fit 64 bits (%d+%d+%d)", bh, be, bl); return ACB_ERANGE; }
+    const SortKey k = sort_key(tb, n_hay, max_hay_letters);
+    if (k.bits() > 64) { acb_set_error("sort key does not fit 64 bits (%d+%d+%d)", k.bh, k.be, k.bl); return ACB_ERANGE; }
     size_t temp = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, temp, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
-                                    (const acb_match *)nullptr, (acb_match *)nullptr, (int)n, 0, bh + be + bl, s);
-    const size_t need = (size_t)n * (2 * sizeof(unsigned long long) + sizeof(acb_match)) + temp + 1024;
-    if (tb->sort_cap < need) {
-        if (tb->d_sort) { cudaFree(tb->d_sort); tb->d_sort = nullptr; tb->sort_cap = 0; }
-        CUDA_TRY(cudaMalloc(&tb->d_sort, need + need / 4));
-        tb->sort_cap = need + need / 4;
-    }
-    char *base = reinterpret_cast<char *>(tb->d_sort);
-    unsigned long long *k0 = reinterpret_cast<unsigned long long *>(base);
-    unsigned long long *k1 = k0 + n;
-    acb_match *r1 = reinterpret_cast<acb_match *>(k1 + n);
-    void *tmp = reinterpret_cast<void *>((reinterpret_cast<uintptr_t>(r1 + n) + 255) & ~(uintptr_t)255);
-    acb_sortkey_kernel<kKeyEnd><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
-    int rc = launched("sort key");
+    int rc = scratch_take(tb->sort_buf, sort_scratch_bytes(n, k.bits(), s, &temp), s);
     if (rc != ACB_OK) return rc;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, temp, k0, k1, d_records, r1, (int)n, 0, bh + be + bl, s));
+    char *p = static_cast<char *>(tb->sort_buf.buf);
+    unsigned long long *k0 = carve<unsigned long long>(p, n), *k1 = carve<unsigned long long>(p, n);
+    acb_match *r1 = carve<acb_match>(p, n);
+    void *tmp = carve<char>(p, temp);
+    if ((rc = sort_records<false>(tb, k, d_records, nullptr, r1, n, k0, k1, tmp, temp, s, "sort key"))) return rc;
     CUDA_TRY(cudaMemcpyAsync(d_records, r1, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToDevice, s));
-    return ACB_OK;
+    return scratch_done(&tb->sort_buf.done, s);
 }
 
 /* ------------------------------------------------------- host-buffer scan */
@@ -1902,26 +1983,6 @@ static int ensure_pinned_out(acb_table *tb, size_t n) {
         CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&tb->h_out), want * sizeof(acb_match)));
         tb->h_out_cap = want;
     }
-    return ACB_OK;
-}
-
-/* Scratch that the last call's work, on any CUDA stream, may still read: a call waits on s for that work before it
- * overwrites the scratch (scratch_wait), and marks its own last reader (scratch_done).  Growing it frees the old
- * buffer only after s has drained (grow_synced). */
-static int scratch_wait(cudaEvent_t done, cudaStream_t s) {
-    if (done) CUDA_TRY(cudaStreamWaitEvent(s, done, 0));
-    return ACB_OK;
-}
-static int scratch_done(cudaEvent_t *done, cudaStream_t s) {
-    if (!*done) CUDA_TRY(cudaEventCreateWithFlags(done, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventRecord(*done, s));
-    return ACB_OK;
-}
-static int grow_synced(void **buf, size_t *cap, size_t need, cudaStream_t s) {
-    if (*cap >= need) return ACB_OK;
-    if (*buf) { CUDA_TRY(cudaStreamSynchronize(s)); cudaFree(*buf); *buf = nullptr; *cap = 0; }
-    CUDA_TRY(cudaMalloc(buf, need + need / 4));
-    *cap = need + need / 4;
     return ACB_OK;
 }
 
@@ -2029,17 +2090,8 @@ static int scan_host_pipelined(acb_table *tb, const uint8_t *hay, int64_t total,
     int rc;
     if ((rc = ensure_pinned_out(tb, (size_t)cap))) return rc;
     const int64_t max_letters = (offsets ? total : stride_bytes) / tb->L;
-    if (sort) {                                                 /* scratch of the per-chunk sorts, once, before anything is in flight */
-        size_t temp = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, temp, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
-                                        (const acb_match *)nullptr, (acb_match *)nullptr, (int)std::min<int64_t>(cap, 0x7fffffff), 0, 64, tb->s_sort);
-        const size_t need = (size_t)cap * (2 * sizeof(unsigned long long) + sizeof(acb_match)) + temp + 1024;
-        if (tb->sort_cap < need) {
-            if (tb->d_sort) { cudaFree(tb->d_sort); tb->d_sort = nullptr; tb->sort_cap = 0; }
-            CUDA_TRY(cudaMalloc(&tb->d_sort, need));
-            tb->sort_cap = need;
-        }
-    }
+    size_t temp = 0;                                            /* scratch of the per-chunk sorts, once, before anything is in flight */
+    if (sort && (rc = scratch_take(tb->sort_buf, sort_scratch_bytes(cap, 64, tb->s_sort, &temp), tb->s_sort))) return rc;
     cudaStream_t sc = tb->stream, sh = tb->s_copy, ss = tb->s_sort;
     const int64_t *d_off = nullptr;
     if (offsets) {
@@ -2111,8 +2163,7 @@ extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_by
         return rc;
     const int64_t max_letters = (offsets ? total_bytes : stride_bytes) / tb->L;
     {   /* large batches on the fast path: copy, scan, sort and copy-back as a pipeline over chunks */
-        const int bits = bits_for((unsigned long long)std::max<int64_t>(n_hay - 1, 1)) + bits_for((unsigned long long)std::max<int64_t>(max_letters, 1)) +
-                         bits_for((unsigned long long)(tb->max_key_bytes / tb->L));
+        const int bits = sort_key(tb, n_hay, max_letters).bits();
         static const bool no_pipe = getenv("ACB_NO_PIPELINE") != nullptr;
         if (!no_pipe && (algo == ACB_ALGO_AUTO || algo == ACB_ALGO_FILTER) && tb->n_keys > 0 && total_bytes >= (48LL << 20) && bits <= 64 && cap < 0x7fffffffLL) {
             rc = scan_host_pipelined(tb, hay, total_bytes, offsets, n_hay, stride_bytes, cap, n_found, sort);
@@ -2281,8 +2332,7 @@ __global__ void acb_compact_offsets_kernel(const CompactMeta m, const long long 
                                            long long *coff) {
     const long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (h > n_hay) return;
-    const long long q = (off ? __ldg(off + h) : h * stride) >> ls;
-    coff[h] = kept_before(m, q) << ls;
+    coff[h] = kept_before(m, hay_start(off, stride, h) >> ls) << ls;
 }
 
 /* the stored records (min(*count, cap)) from compacted letters of their haystack to original ones */
@@ -2300,8 +2350,7 @@ __global__ void acb_remap_kernel(const CompactMeta m, const long long *coff, con
         while (b - a > 1) { const int mid = (a + b) >> 1; if ((long long)__ldg(gp + mid) <= kt) a = mid; else b = mid; }
         const long long g = lo * kCmpThreads + a;
         const int bit = (int)__fns(__ldg(m.mask + g), 0, (int)(kt - __ldg(gp + a)) + 1);
-        const long long hs = (off ? __ldg(off + r.hay_id) : (long long)r.hay_id * stride) >> ls;
-        r.end_index = (int32_t)(g * 32 + bit - hs);
+        r.end_index = (int32_t)(g * 32 + bit - (hay_start(off, stride, r.hay_id) >> ls));
         rec[i] = r;
     }
 }
@@ -2349,9 +2398,10 @@ static int compact(acb_table *tb, const uint8_t *d_in, int64_t total, const int6
     CUDA_TRY(cudaMemsetAsync(tb->k_ctr, 0, sizeof(unsigned int), s));
     if (n_tiles > 0x7fffffffLL) { acb_set_error("batch too large to compact in one launch"); return ACB_ERANGE; }
     if ((rc = timing_mark(&tb->k_t0, s))) return rc;
-    if (L == 1) acb_compact_kernel<uint8_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
-    else if (L == 2) acb_compact_kernel<uint16_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
-    else acb_compact_kernel<uint32_t><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
+    with_width(L, [&](auto w) {
+        using T = std::conditional_t<w.value == 1, uint8_t, std::conditional_t<w.value == 2, uint16_t, uint32_t>>;
+        acb_compact_kernel<T><<<(unsigned)n_tiles, kCmpThreads, 0, s>>>(p);
+    });
     CUDA_TRY(cudaGetLastError());
     if ((rc = timing_mark(&tb->k_t1, s)) || (rc = timing_ms(tb->k_t0, tb->k_t1, &g_compact_ms))) return rc;
     meta->mask = tb->k_mask; meta->gpre = tb->k_gpre; meta->tile_pre = tb->k_tile_pre; meta->n_tiles = n_tiles;
@@ -2368,10 +2418,9 @@ static int launch_remap(acb_table *tb, const CompactMeta &meta, const int64_t *d
                         int64_t *d_count, cudaStream_t s) {
     if (cap <= 0) return ACB_OK;
     const int ls = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
-    const long long grid = std::min<long long>((cap + 255) / 256, grid_sms(tb) * 16);
     int rc;
     if ((rc = timing_mark(&tb->k_t0, s))) return rc;
-    acb_remap_kernel<<<(unsigned)grid, 256, 0, s>>>(meta, tb->k_coff, reinterpret_cast<const long long *>(d_off), stride, ls, d_out,
+    acb_remap_kernel<<<blocks(tb, cap), 256, 0, s>>>(meta, tb->k_coff, reinterpret_cast<const long long *>(d_off), stride, ls, d_out,
                                                     reinterpret_cast<const unsigned long long *>(d_count), cap);
     if ((rc = launched("remap kernel")) || (rc = timing_mark(&tb->k_t1, s))) return rc;
     return timing_ms(tb->k_t0, tb->k_t1, &g_remap_ms);
@@ -2452,11 +2501,6 @@ __device__ __forceinline__ long long chunk_stream(const StreamsArgs &a, long lon
     return (s >= 0 && s < a.n_streams) ? s : -1;           /* ids are validated by the caller; never index outside */
 }
 
-__device__ __forceinline__ void chunk_span(const long long *off, long long stride, long long h, long long &hs, long long &he) {
-    hs = off ? __ldg(off + h) : h * stride;
-    he = off ? __ldg(off + h + 1) : hs + stride;
-}
-
 /* the seam of chunk h: walk tail || first min(T, n) letters from the root, report what straddles the chunk's start,
  * stage the next tail */
 __global__ void __launch_bounds__(kDfaThreads) acb_seam_kernel(const __grid_constant__ ScanParams p, const StreamsArgs a) {
@@ -2464,8 +2508,7 @@ __global__ void __launch_bounds__(kDfaThreads) acb_seam_kernel(const __grid_cons
     if (h >= p.n_hay) return;
     const long long s = chunk_stream(a, h);
     if (s < 0) return;
-    long long hs, he;
-    chunk_span(p.offsets, p.stride_bytes, h, hs, he);
+    const long long hs = hay_start(p.offsets, p.stride_bytes, h), he = hay_start(p.offsets, p.stride_bytes, h + 1);
     const int L = p.L, ls = p.letter_shift;                      /* L == 1 << ls */
     const long long n = (he - hs) >> ls;
     const long long t = min((long long)a.T, a.kept ? a.kept[s] : a.pos[s]), m = min((long long)a.T, n);
@@ -2517,12 +2560,10 @@ __global__ void acb_streams_commit_kernel(const StreamsArgs a, const long long *
     if (h >= n_chunks || (count && *count > (unsigned long long)cap)) return;
     const long long s = chunk_stream(a, h);
     if (s < 0) return;
-    long long hs, he;
-    chunk_span(off, stride, h, hs, he);
     if (a.end) a.state[s] = a.end[h];
     const long long tb = (long long)a.T * a.L;
     for (long long j = 0; j < tb; ++j) a.tail[s * tb + j] = a.next_tail[h * tb + j];
-    a.pos[s] += (he - hs) / a.L;
+    a.pos[s] += (hay_start(off, stride, h + 1) - hay_start(off, stride, h)) / a.L;
     if (a.kept) a.kept[s] += (__ldg(koff + h + 1) - __ldg(koff + h)) / a.L;
 }
 
@@ -2572,7 +2613,7 @@ struct acb_streams {
     acb_match *d_settled = nullptr; size_t settled_cap = 0;       /* ... the records that start before the frontier */
     uint8_t *d_flag = nullptr; size_t flag_cap = 0;
     acb_match *d_chosen = nullptr; size_t chosen_cap = 0;         /* replacing feeds: the chosen records */
-    void *d_tmp = nullptr; size_t tmp_cap = 0;                    /* cub scratch */
+    uint8_t *d_tmp = nullptr; size_t tmp_cap = 0;                 /* cub scratch */
     unsigned long long *d_ctr = nullptr, *h_ctr = nullptr;        /* [0] full, [1] settled, [2] chosen, [3] sizes; h_ctr pinned */
     cudaEvent_t ev[12] = {};                                      /* kernel timing, a pair per stage */
     /* whole-word batches (acb_streams_new_words; leftmost or find_all): the tail holds up to T + 1 letters, and d_left[s]
@@ -3099,8 +3140,7 @@ static int select_count(acb_table *tb, const SelectParams &p, int64_t n, int64_t
         CUDA_TRY(cudaMemsetAsync(d_total, 0, sizeof(int64_t), s));
         return ACB_OK;
     }
-    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, grid_sms(tb) * 16);
-    acb_select_kernel<false><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
+    acb_select_kernel<false><<<blocks(tb, n, kSelectThreads), kSelectThreads, 0, s>>>(p);
     int rc = launched("select kernel");
     if (rc != ACB_OK) return rc;
     long long *cnt = reinterpret_cast<long long *>(d_out_off) + 1;     /* in place: counts -> inclusive sums */
@@ -3115,8 +3155,7 @@ static int select_count(acb_table *tb, const SelectParams &p, int64_t n, int64_t
 /* pass 2: the ids, when *p.total <= p.cap */
 static int select_fill(acb_table *tb, const SelectParams &p, int64_t n, cudaStream_t s) {
     if (n == 0 || p.cap == 0) return ACB_OK;
-    const long long grid = std::min<long long>((n + kSelectThreads - 1) / kSelectThreads, grid_sms(tb) * 16);
-    acb_select_kernel<true><<<(unsigned)grid, kSelectThreads, 0, s>>>(p);
+    acb_select_kernel<true><<<blocks(tb, n, kSelectThreads), kSelectThreads, 0, s>>>(p);
     return launched("select kernel");
 }
 
@@ -3331,9 +3370,19 @@ __global__ void acb_ll_count_kernel(const unsigned long long *d_m, const uint8_t
     const long long M = (long long)*d_m;
     if (M > 0) *count += (unsigned long long)pos[M - 1] + chosen[M - 1];
 }
-
-char *carve(char *&p, size_t bytes) { char *r = p; p += (bytes + 255) & ~(size_t)255; return r; }
 } // namespace
+
+/* The flagged ones of the first *d_m (<= n) records of rec, in order, to d_out[*d_count ..] (those past cap counted, not
+ * stored), and *d_count += their number.  pos holds the flags and becomes their exclusive sum; tmp: cub scratch of temp
+ * bytes for it. */
+static int emit_flagged(acb_table *tb, const acb_match *rec, const unsigned long long *d_m, const uint8_t *flag, int32_t *pos, int n,
+                        void *tmp, size_t temp, acb_match *d_out, int64_t cap, int64_t *d_count, cudaStream_t s, const char *what) {
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, temp, pos, pos, n, s));
+    acb_ll_emit_kernel<<<blocks(tb, n), 256, 0, s>>>(rec, d_m, flag, pos, d_out, cap, reinterpret_cast<const unsigned long long *>(d_count));
+    CUDA_TRY(cudaGetLastError());
+    acb_ll_count_kernel<<<1, 1, 0, s>>>(d_m, flag, pos, reinterpret_cast<unsigned long long *>(d_count));
+    return launched(what, 2);
+}
 
 extern "C" int acb_last_leftmost_ms(float *ms, int32_t n) {
     if (!ms || n < 0 || n > 5) { acb_set_error("bad argument"); return ACB_EINVAL; }
@@ -3352,11 +3401,7 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     if (n == 0) return ACB_OK;
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    const int max_len = tb->max_key_bytes / tb->L;
-    const int bh = bits_for((unsigned long long)std::max<int64_t>(n_hay - 1, 1));
-    const int be = bits_for((unsigned long long)std::max<int64_t>(max_hay_letters, 1));
-    const int bl = bits_for((unsigned long long)max_len);
-    const bool one_pass = bh + be + bl <= 64;
+    const SortKey k = sort_key(tb, n_hay, max_hay_letters);
     const int ni = (int)n;
     const long long n_tiles = (n + kLlTile - 1) / kLlTile;
     size_t t_sort = 0, t_sel = 0, t_scan = 0;
@@ -3370,33 +3415,22 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     const size_t need = 8 * 256 + 2 * N * sizeof(unsigned long long) + 2 * N * sizeof(acb_match) + N + 2 * N * sizeof(int32_t) +
                         (size_t)n_tiles * sizeof(unsigned long long) + temp;
     int rc;
-    if ((rc = scratch_wait(tb->l_done, s)) || (rc = grow_synced(&tb->l_buf, &tb->l_buf_cap, need, s))) return rc;
+    if ((rc = scratch_take(tb->l_buf, need, s))) return rc;
     if (!tb->l_ctr) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->l_ctr), 4 * sizeof(unsigned long long)));
-    char *p = reinterpret_cast<char *>(tb->l_buf);
-    unsigned long long *k0 = reinterpret_cast<unsigned long long *>(carve(p, N * 8)), *k1 = reinterpret_cast<unsigned long long *>(carve(p, N * 8));
-    acb_match *ra = reinterpret_cast<acb_match *>(carve(p, N * sizeof(acb_match))), *rb = reinterpret_cast<acb_match *>(carve(p, N * sizeof(acb_match)));
-    uint8_t *flag = reinterpret_cast<uint8_t *>(carve(p, N));
-    int32_t *nxt = reinterpret_cast<int32_t *>(carve(p, N * 4)), *pos = reinterpret_cast<int32_t *>(carve(p, N * 4));
-    unsigned long long *status = reinterpret_cast<unsigned long long *>(carve(p, (size_t)n_tiles * 8));
-    void *tmp = carve(p, temp);
+    char *p = static_cast<char *>(tb->l_buf.buf);
+    unsigned long long *k0 = carve<unsigned long long>(p, N), *k1 = carve<unsigned long long>(p, N);
+    acb_match *ra = carve<acb_match>(p, N), *rb = carve<acb_match>(p, N);
+    uint8_t *flag = carve<uint8_t>(p, N);
+    int32_t *nxt = carve<int32_t>(p, N), *pos = carve<int32_t>(p, N);
+    unsigned long long *status = carve<unsigned long long>(p, (size_t)n_tiles);
+    void *tmp = carve<char>(p, temp);
     size_t tb_temp = temp;
-    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, grid_sms(tb) * 16);
+    const unsigned grid = blocks(tb, n);
     if ((rc = timing_mark(&tb->l_ev[0], s))) return rc;
-    /* 1. re-key by start and sort */
-    if (one_pass) {
-        acb_sortkey_kernel<kKeyStart><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
-        if ((rc = launched("leftmost sort key"))) return rc;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, d_records, ra, ni, 0, bh + be + bl, s));
-    } else {                                               /* two stable passes: start | (max_len - len), then hay */
-        acb_sortkey_kernel<kKeyStartLow><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_records, n, tb->d_keylen, be, bl, max_len, k0);
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, d_records, rb, ni, 0, be + bl, s));
-        acb_sortkey_kernel<kKeyHay><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(rb, n, tb->d_keylen, be, bl, max_len, k0);
-        if ((rc = launched("leftmost sort keys", 2))) return rc;
-        tb_temp = temp;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb_temp, k0, k1, rb, ra, ni, 0, bh, s));
-    }
-    if ((rc = timing_mark(&tb->l_ev[1], s))) return rc;
+    /* 1. sort by start */
+    if ((rc = sort_records<true>(tb, k, d_records, rb, ra, n, k0, k1, tmp, temp, s, "leftmost sort key")) ||
+        (rc = timing_mark(&tb->l_ev[1], s)))
+        return rc;
     /* 2. candidates: the longest match at every (hay, start) */
     acb_ll_cand_kernel<<<grid, 256, 0, s>>>(ra, n, tb->d_keylen, flag);
     if ((rc = launched("leftmost candidates"))) return rc;
@@ -3410,15 +3444,12 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)n_tiles * sizeof(unsigned long long), s));
     CUDA_TRY(cudaMemsetAsync(pos, 0, N * sizeof(int32_t), s));
     CUDA_TRY(cudaMemsetAsync(tb->l_ctr + 1, 0, sizeof(unsigned long long), s));
-    acb_ll_chain_kernel<<<(unsigned)n_tiles, kLlThreads, 0, s>>>(rb, tb->l_ctr, nxt, std::max(max_len, 1), tb->l_ctr + 1, status, flag, pos);
+    acb_ll_chain_kernel<<<(unsigned)n_tiles, kLlThreads, 0, s>>>(rb, tb->l_ctr, nxt, std::max(k.max_len, 1), tb->l_ctr + 1, status, flag, pos);
     if ((rc = launched("leftmost chain")) || (rc = timing_mark(&tb->l_ev[4], s))) return rc;
     /* 5. emit */
-    tb_temp = temp;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb_temp, pos, pos, ni, s));
-    acb_ll_emit_kernel<<<grid, 256, 0, s>>>(rb, tb->l_ctr, flag, pos, d_out, cap, reinterpret_cast<const unsigned long long *>(d_count));
-    CUDA_TRY(cudaGetLastError());
-    acb_ll_count_kernel<<<1, 1, 0, s>>>(tb->l_ctr, flag, pos, reinterpret_cast<unsigned long long *>(d_count));
-    if ((rc = launched("leftmost emit", 2)) || (rc = timing_mark(&tb->l_ev[5], s)) || (rc = scratch_done(&tb->l_done, s))) return rc;
+    if ((rc = emit_flagged(tb, rb, tb->l_ctr, flag, pos, ni, tmp, temp, d_out, cap, d_count, s, "leftmost emit")) ||
+        (rc = timing_mark(&tb->l_ev[5], s)) || (rc = scratch_done(&tb->l_buf.done, s)))
+        return rc;
     for (int k = 0; k < 5; k++)
         if ((rc = timing_ms(tb->l_ev[k], tb->l_ev[k + 1], &g_ll_ms[k]))) return rc;
     return ACB_OK;
@@ -3433,13 +3464,32 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
 namespace {
 thread_local float g_ww_ms = 0.f;                          /* kernel timing: flags to count */
 
+/* a word set: letter v is a word letter iff v < n_bits and bit v is set */
+struct WordBits {
+    const uint32_t *bits;
+    long long n_bits;
+
+    /* for 1-byte letters, the set with its bitmap copied to s[8] in shared memory; every thread of the block calls it */
+    template <int L>
+    __device__ __forceinline__ WordBits shared(uint32_t *s) const {
+        if (L != 1) return *this;
+        if (threadIdx.x < 8) s[threadIdx.x] = (long long)threadIdx.x * 32 < n_bits ? bits[threadIdx.x] : 0u;
+        __syncthreads();
+        return {s, n_bits};
+    }
+    template <int L>
+    __device__ __forceinline__ bool is_word(uint32_t v) const {
+        if ((long long)v >= n_bits) return false;
+        return ((L == 1 ? bits[v >> 5] : __ldg(bits + (v >> 5))) >> (v & 31) & 1u) != 0;
+    }
+};
+
 struct WwArgs {
     const uint8_t *hay;
-    const long long *off;                                  /* n_hay + 1 byte offsets, or nullptr: haystack h = [h*stride, (h+1)*stride) */
+    const long long *off;                                  /* n_hay + 1 byte offsets, or nullptr: fixed stride (hay_start) */
     long long stride;
     const int32_t *key_len;
-    const uint32_t *bits;                                  /* letter v is a word letter iff v < n_bits and bit v is set */
-    long long n_bits;
+    WordBits words;
 };
 
 /* the letter at p, little-endian, at any alignment */
@@ -3455,30 +3505,16 @@ __device__ __forceinline__ uint32_t ww_letter(const uint8_t *p) {
 template <int L>
 __global__ void __launch_bounds__(256) acb_ww_flag_kernel(const __grid_constant__ WwArgs a, const acb_match *rec, long long n,
                                                          uint8_t *flag, int32_t *pos, unsigned long long *d_n) {
-    __shared__ uint32_t s_bits[8];                         /* 1-byte letters: the whole set */
-    if (L == 1) {
-        if (threadIdx.x < 8) s_bits[threadIdx.x] = (long long)threadIdx.x * 32 < a.n_bits ? a.bits[threadIdx.x] : 0u;
-        __syncthreads();
-    }
-    auto word = [&](uint32_t v) {
-        if ((long long)v >= a.n_bits) return false;
-        return ((L == 1 ? s_bits[v >> 5] : __ldg(a.bits + (v >> 5))) >> (v & 31) & 1u) != 0;
-    };
+    __shared__ uint32_t s_bits[8];
+    const WordBits w = a.words.shared<L>(s_bits);
     const long long first = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (first == 0) *d_n = (unsigned long long)n;
     for (long long i = first; i < n; i += (long long)gridDim.x * blockDim.x) {
         const acb_match m = rec[i];
-        long long b0, letters;
-        if (a.off) {
-            b0 = __ldg(a.off + m.hay_id);
-            letters = (__ldg(a.off + m.hay_id + 1) - b0) / L;
-        } else {
-            b0 = (long long)m.hay_id * a.stride;
-            letters = a.stride / L;
-        }
+        const long long b0 = hay_start(a.off, a.stride, m.hay_id), letters = (hay_start(a.off, a.stride, m.hay_id + 1) - b0) / L;
         const long long end = m.end_index, start = end - __ldg(a.key_len + m.key_id) + 1;
-        bool keep = start == 0 || !word(ww_letter<L>(a.hay + b0 + (start - 1) * L));
-        keep = keep && (end + 1 == letters || !word(ww_letter<L>(a.hay + b0 + (end + 1) * L)));
+        bool keep = start == 0 || !w.is_word<L>(ww_letter<L>(a.hay + b0 + (start - 1) * L));
+        keep = keep && (end + 1 == letters || !w.is_word<L>(ww_letter<L>(a.hay + b0 + (end + 1) * L)));
         flag[i] = keep;
         pos[i] = keep;
     }
@@ -3520,26 +3556,20 @@ extern "C" int acb_word_filter_device(acb_table *tb, const uint8_t *d_hay, int64
     size_t temp = 0;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, (int32_t *)nullptr, (int32_t *)nullptr, ni, s));
     const size_t need = 3 * 256 + N + N * sizeof(int32_t) + sizeof(unsigned long long) + temp;
-    if ((rc = scratch_wait(tb->ww_done, s)) || (rc = grow_synced(&tb->ww_buf, &tb->ww_buf_cap, need, s))) return rc;
-    char *p = reinterpret_cast<char *>(tb->ww_buf);
-    uint8_t *flag = reinterpret_cast<uint8_t *>(carve(p, N));
-    int32_t *pos = reinterpret_cast<int32_t *>(carve(p, N * sizeof(int32_t)));
-    unsigned long long *d_n = reinterpret_cast<unsigned long long *>(carve(p, sizeof(unsigned long long)));
-    void *tmp = carve(p, temp);
+    if ((rc = scratch_take(tb->ww_buf, need, s))) return rc;
+    char *p = static_cast<char *>(tb->ww_buf.buf);
+    uint8_t *flag = carve<uint8_t>(p, N);
+    int32_t *pos = carve<int32_t>(p, N);
+    unsigned long long *d_n = carve<unsigned long long>(p, 1);
+    void *tmp = carve<char>(p, temp);
     WwArgs a;
     a.hay = d_hay; a.off = reinterpret_cast<const long long *>(d_offsets); a.stride = stride_bytes; a.key_len = tb->d_keylen;
-    a.bits = d_bits; a.n_bits = n_bits;
-    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, grid_sms(tb) * 16);
+    a.words = {d_bits, n_bits};
     if ((rc = timing_mark(&tb->ww_ev[0], s))) return rc;
-    if (tb->L == 1) acb_ww_flag_kernel<1><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
-    else if (tb->L == 2) acb_ww_flag_kernel<2><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
-    else acb_ww_flag_kernel<4><<<grid, 256, 0, s>>>(a, d_records, n, flag, pos, d_n);
-    if ((rc = launched("word flags"))) return rc;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, temp, pos, pos, ni, s));
-    acb_ll_emit_kernel<<<grid, 256, 0, s>>>(d_records, d_n, flag, pos, d_out, cap, reinterpret_cast<const unsigned long long *>(d_count));
-    CUDA_TRY(cudaGetLastError());
-    acb_ll_count_kernel<<<1, 1, 0, s>>>(d_n, flag, pos, reinterpret_cast<unsigned long long *>(d_count));
-    if ((rc = launched("word filter emit", 2)) || (rc = timing_mark(&tb->ww_ev[1], s)) || (rc = scratch_done(&tb->ww_done, s))) return rc;
+    with_width(tb->L, [&](auto w) { acb_ww_flag_kernel<decltype(w)::value><<<blocks(tb, n), 256, 0, s>>>(a, d_records, n, flag, pos, d_n); });
+    if ((rc = launched("word flags")) || (rc = emit_flagged(tb, d_records, d_n, flag, pos, ni, tmp, temp, d_out, cap, d_count, s, "word filter emit")) ||
+        (rc = timing_mark(&tb->ww_ev[1], s)) || (rc = scratch_done(&tb->ww_buf.done, s)))
+        return rc;
     return timing_ms(tb->ww_ev[0], tb->ww_ev[1], &g_ww_ms);
 }
 
@@ -3694,7 +3724,6 @@ struct RpArgs {
 };
 
 __device__ __forceinline__ long long rp_n(const RpArgs &a) { return min((long long)*a.n_chosen, a.cap); }
-__device__ __forceinline__ long long rp_in_off(const RpArgs &a, long long h) { return a.in_off ? a.in_off[h] : h * a.stride; }
 
 /* D[i] = rep_len - key_len * L of record i, 0 for i in [n, cap] (the exclusive scan then leaves the sum in D[cap]) */
 __global__ void acb_rp_delta_kernel(const __grid_constant__ RpArgs a) {
@@ -3714,7 +3743,7 @@ __global__ void acb_rp_records_kernel(const __grid_constant__ RpArgs a) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const acb_match m = a.chosen[i];
         const long long len = __ldg(a.key_len + m.key_id);
-        const long long s = rp_in_off(a, m.hay_id) + ((long long)m.end_index - len + 1) * a.L;
+        const long long s = hay_start(a.in_off, a.stride, m.hay_id) + ((long long)m.end_index - len + 1) * a.L;
         const long long p = s + a.D[i], rs = a.rep_off[m.key_id];
         a.P[i] = p;
         a.E[i] = p + a.rep_off[m.key_id + 1] - rs;
@@ -3732,7 +3761,7 @@ __global__ void acb_rp_offsets_kernel(const __grid_constant__ RpArgs a) {
             const long long mid = (lo + hi) >> 1;
             if ((long long)a.chosen[mid].hay_id < h) lo = mid + 1; else hi = mid;
         }
-        const long long o = (h == a.n_hay ? a.total_bytes : rp_in_off(a, h)) + a.D[lo];
+        const long long o = (h == a.n_hay ? a.total_bytes : hay_start(a.in_off, a.stride, h)) + a.D[lo];
         a.out_off[h] = o;
         if (h == a.n_hay) *a.total = o;
     }
@@ -3879,24 +3908,23 @@ static int rp_offsets(acb_table *tb, RpArgs &a, cudaStream_t s) {
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, (long long *)nullptr, (long long *)nullptr, a.cap + 1, s));
     const size_t need = 6 * 256 + (C + 1) * 8 + 4 * C * 8 + temp;
     int rc;
-    if ((rc = scratch_wait(tb->r_done, s)) || (rc = grow_synced(&tb->r_buf, &tb->r_buf_cap, need, s))) return rc;
-    char *p = reinterpret_cast<char *>(tb->r_buf);
-    a.D = reinterpret_cast<long long *>(carve(p, (C + 1) * 8));
-    a.P = reinterpret_cast<long long *>(carve(p, C * 8));
-    a.E = reinterpret_cast<long long *>(carve(p, C * 8));
-    a.IE = reinterpret_cast<long long *>(carve(p, C * 8));
-    a.RS = reinterpret_cast<long long *>(carve(p, C * 8));
-    void *tmp = carve(p, temp);
-    const long long most = grid_sms(tb) * 16;
+    if ((rc = scratch_take(tb->r_buf, need, s))) return rc;
+    char *p = static_cast<char *>(tb->r_buf.buf);
+    a.D = carve<long long>(p, C + 1);
+    a.P = carve<long long>(p, C);
+    a.E = carve<long long>(p, C);
+    a.IE = carve<long long>(p, C);
+    a.RS = carve<long long>(p, C);
+    void *tmp = carve<char>(p, temp);
     if ((rc = timing_mark(&tb->r_ev[0], s))) return rc;
-    acb_rp_delta_kernel<<<(unsigned)std::min<long long>((a.cap + 256) / 256, most), 256, 0, s>>>(a);
+    acb_rp_delta_kernel<<<blocks(tb, a.cap + 1), 256, 0, s>>>(a);
     if ((rc = launched("replacement delta"))) return rc;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, temp, a.D, a.D, a.cap + 1, s));
     if (a.cap) {
-        acb_rp_records_kernel<<<(unsigned)std::min<long long>((a.cap + 255) / 256, most), 256, 0, s>>>(a);
+        acb_rp_records_kernel<<<blocks(tb, a.cap), 256, 0, s>>>(a);
         if ((rc = launched("replacement records"))) return rc;
     }
-    acb_rp_offsets_kernel<<<(unsigned)std::min<long long>((a.n_hay + 256) / 256, most), 256, 0, s>>>(a);
+    acb_rp_offsets_kernel<<<blocks(tb, a.n_hay + 1), 256, 0, s>>>(a);
     if ((rc = launched("replacement offsets"))) return rc;
     return timing_mark(&tb->r_ev[1], s);
 }
@@ -3912,13 +3940,12 @@ static int rp_write(acb_table *tb, RpArgs &a, cudaStream_t s) {
             if ((rc = ensure(&tb->r_ts, &tb->r_ts_cap, (size_t)max_tiles + 1))) return rc;
         }
         a.ts = tb->r_ts;
-        const long long most = grid_sms(tb) * 16;
-        acb_rp_tiles_kernel<<<(unsigned)std::min<long long>((max_tiles + 256) / 256, most), 256, 0, s>>>(a);
+        acb_rp_tiles_kernel<<<blocks(tb, max_tiles + 1), 256, 0, s>>>(a);
         if ((rc = launched("replacement tiles"))) return rc;
         acb_rp_write_kernel<<<(unsigned)std::min<long long>(max_tiles, grid_sms(tb) * 8), kRpThreads, 0, s>>>(a);
         if ((rc = launched("replacement write"))) return rc;
     }
-    if ((rc = timing_mark(&tb->r_ev[3], s)) || (rc = scratch_done(&tb->r_done, s)) || (rc = timing_ms(tb->r_ev[0], tb->r_ev[1], &g_rp_ms[0])))
+    if ((rc = timing_mark(&tb->r_ev[3], s)) || (rc = scratch_done(&tb->r_buf.done, s)) || (rc = timing_ms(tb->r_ev[0], tb->r_ev[1], &g_rp_ms[0])))
         return rc;
     return timing_ms(tb->r_ev[2], tb->r_ev[3], &g_rp_ms[1]);
 }
@@ -4064,18 +4091,18 @@ __device__ __forceinline__ long long sl_stream(const SlArgs &a, long long h) {
     return (s >= 0 && s < a.n_streams) ? s : -1;
 }
 
-__device__ __forceinline__ long long sl_chunk_bytes(const SlArgs &a, long long h, long long &begin) {
-    begin = a.off ? a.off[h] : h * a.stride;
-    return a.off ? a.off[h + 1] - begin : a.stride;
+/* bytes of chunk h */
+__device__ __forceinline__ long long sl_chunk_bytes(const SlArgs &a, long long h) {
+    return hay_start(a.off, a.stride, h + 1) - hay_start(a.off, a.stride, h);
 }
 
 /* soff[h] = bytes of held || chunk h (soff[n] = 0), for the exclusive scan that makes them offsets */
 __global__ void acb_sl_len_kernel(const __grid_constant__ SlArgs a) {
     for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h <= a.n; h += (long long)gridDim.x * blockDim.x) {
-        long long b = 0, len = 0;
+        long long len = 0;
         if (h < a.n) {
             const long long s = sl_stream(a, h);
-            len = sl_chunk_bytes(a, h, b) + (s < 0 ? 0 : a.hold[s] * a.L);
+            len = sl_chunk_bytes(a, h) + (s < 0 ? 0 : a.hold[s] * a.L);
         }
         a.soff[h] = len;
     }
@@ -4124,16 +4151,12 @@ __global__ void __launch_bounds__(256) acb_sl_gather_kernel(const __grid_constan
         long long h = F(h0, c), lo = O(h), hi = O(h + 1), hd = 0;
         const uint8_t *tp = nullptr, *sp;                  /* the held letters; sp[o - lo] = source byte of output o */
         const auto enter = [&]() {
-            long long b;
             if (kStage) {
                 const long long s = sl_stream(a, h);
                 hd = s < 0 ? 0 : a.hold[s] * a.L;
                 tp = a.tail + (s < 0 ? 0 : s) * a.T * a.L;
-                sl_chunk_bytes(a, h, b);
-            } else {
-                b = a.soff[h];
             }
-            sp = base + b - hd;
+            sp = base + (kStage ? hay_start(a.off, a.stride, h) : a.soff[h]) - hd;
         };
         enter();
         if (c - lo >= hd && c + 16 <= hi) {
@@ -4216,8 +4239,7 @@ __global__ void acb_sl_commit_kernel(const __grid_constant__ SlArgs a, const uns
     uint8_t *to = a.tail + s * a.T * a.L;
     for (long long j = lane; j < keep * a.L; j += kSlLanes) to[j] = from[j];
     if (lane == 0) {
-        long long b;
-        const long long n = sl_chunk_bytes(a, h, b) / a.L;
+        const long long n = sl_chunk_bytes(a, h) / a.L;
         a.pos[s] = a.final ? 0 : a.pos[s] + n;
         a.hold[s] = a.final ? 0 : keep;
     }
@@ -4228,17 +4250,10 @@ __global__ void acb_sl_commit_kernel(const __grid_constant__ SlArgs a, const uns
 struct SwArgs {
     SlArgs a;
     uint8_t *left;                                         /* [n_streams] the letter before the held ones is a word letter */
-    const uint32_t *bits; long long n_bits;                /* the word set, as WwArgs */
+    WordBits words;
     const int32_t *key_len;
     int leftmost;
 };
-
-/* letter v is in the word set; tab: the bitmap (in shared memory for 1-byte letters) */
-template <int L>
-__device__ __forceinline__ bool sw_word(const SwArgs &w, const uint32_t *tab, uint32_t v) {
-    if ((long long)v >= w.n_bits) return false;
-    return ((L == 1 ? tab[v >> 5] : __ldg(w.bits + (v >> 5))) >> (v & 31) & 1u) != 0;
-}
 
 /* flag[i]: record i of the staged full list lies in the feed's window and is a whole-word match.  Window: leftmost, it
  * starts before the frontier staged - (T + 1) (every record on a final feed); find_all, it ends in [hold - 1, staged - 2]
@@ -4247,11 +4262,8 @@ __device__ __forceinline__ bool sw_word(const SwArgs &w, const uint32_t *tab, ui
 template <int L>
 __global__ void __launch_bounds__(256) acb_sw_flag_kernel(const __grid_constant__ SwArgs w, const acb_match *full,
                                                           const unsigned long long *count, long long cap, uint8_t *flag) {
-    __shared__ uint32_t s_bits[8];                         /* 1-byte letters: the whole set */
-    if (L == 1) {
-        if (threadIdx.x < 8) s_bits[threadIdx.x] = (long long)threadIdx.x * 32 < w.n_bits ? w.bits[threadIdx.x] : 0u;
-        __syncthreads();
-    }
+    __shared__ uint32_t s_bits[8];
+    const WordBits words = w.words.shared<L>(s_bits);
     const SlArgs &a = w.a;
     const long long m = min((long long)*count, cap);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (long long)gridDim.x * blockDim.x) {
@@ -4265,20 +4277,10 @@ __global__ void __launch_bounds__(256) acb_sw_flag_kernel(const __grid_constant_
 #ifdef ACB_DEBUG
             assert(!keep || a.final || end + 1 < staged);
 #endif
-            if (keep) keep = !(start == 0 ? (s >= 0 && w.left[s]) : sw_word<L>(w, s_bits, ww_letter<L>(a.stage + b0 + (start - 1) * L)));
-            if (keep && end + 1 < staged) keep = !sw_word<L>(w, s_bits, ww_letter<L>(a.stage + b0 + (end + 1) * L));
+            if (keep) keep = !(start == 0 ? (s >= 0 && w.left[s]) : words.is_word<L>(ww_letter<L>(a.stage + b0 + (start - 1) * L)));
+            if (keep && end + 1 < staged) keep = !words.is_word<L>(ww_letter<L>(a.stage + b0 + (end + 1) * L));
         }
         flag[i] = keep;
-    }
-}
-
-/* the sort key of a kept record: hay | end | (max_len - len), or without the hay when hay_shift < 0 */
-__global__ void acb_sw_key_kernel(const acb_match *rec, long long n, const int32_t *key_len, int bl, int max_len, int hay_shift,
-                                  unsigned long long *keys) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const acb_match m = rec[i];
-        const unsigned long long k = (unsigned long long)(uint32_t)m.end_index << bl | (unsigned long long)(max_len - __ldg(key_len + m.key_id));
-        keys[i] = hay_shift < 0 ? k : ((unsigned long long)(uint32_t)m.hay_id << hay_shift | k);
     }
 }
 
@@ -4306,7 +4308,7 @@ __global__ void acb_sw_left_kernel(const __grid_constant__ SwArgs w, const unsig
         const long long s = sl_stream(a, h), x = a.xn[h];
         if (s < 0) continue;
         if (a.final) w.left[s] = 0;
-        else if (x > 0) w.left[s] = sw_word<L>(w, w.bits, ww_letter<L>(a.stage + a.soff[h] + (x - 1) * L));
+        else if (x > 0) w.left[s] = w.words.is_word<L>(ww_letter<L>(a.stage + a.soff[h] + (x - 1) * L));
     }
 }
 } // namespace
@@ -4383,19 +4385,11 @@ static int sl_check(const acb_streams *ss, const acb_table *tb, int64_t total, c
     return ACB_OK;
 }
 
-/* cub scratch of at least `bytes` */
-static int sl_tmp(acb_streams *ss, size_t bytes) {
-    uint8_t *p = static_cast<uint8_t *>(ss->d_tmp);
-    int rc = ensure(&p, &ss->tmp_cap, bytes);
-    ss->d_tmp = p;
-    return rc;
-}
-
 /* d_soff[0..n] <- exclusive scan of d_soff[0..n] in place; the total to the host (the one wait of the staging) */
 static int sl_offsets(acb_streams *ss, long long *d, int64_t n, cudaStream_t s, long long *total) {
     size_t temp = 0;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, d, d, (int)(n + 1), s));
-    int rc = sl_tmp(ss, temp);
+    int rc = ensure(&ss->d_tmp, &ss->tmp_cap, temp);
     if (rc) return rc;
     temp = ss->tmp_cap;
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(ss->d_tmp, temp, d, d, (int)(n + 1), s));
@@ -4411,8 +4405,7 @@ static int sl_gather(acb_streams *ss, acb_table *tb, const SlArgs &a, bool stage
     const long long n_tiles = (total + kSlTile - 1) / kSlTile;
     int rc = ensure(&ss->d_ts, &ss->ts_cap, (size_t)n_tiles);
     if (rc) return rc;
-    acb_sl_tiles_kernel<<<(unsigned)std::min<long long>((n_tiles + 255) / 256, grid_sms(tb) * 16), 256, 0, s>>>(doff, a.n, total,
-                                                                                                                   ss->d_ts);
+    acb_sl_tiles_kernel<<<blocks(tb, n_tiles), 256, 0, s>>>(doff, a.n, total, ss->d_ts);
     if ((rc = launched("stream gather tiles"))) return rc;
     const unsigned grid = (unsigned)std::min<long long>(n_tiles, grid_sms(tb) * 8);
     if (stage) acb_sl_gather_kernel<true><<<grid, 256, 0, s>>>(a, doff, ss->d_ts, dst, total);
@@ -4422,50 +4415,36 @@ static int sl_gather(acb_streams *ss, acb_table *tb, const SlArgs &a, bool stage
 
 static SwArgs sw_args(const acb_streams *ss, const acb_table *tb, const SlArgs &a) {
     SwArgs w;
-    w.a = a; w.left = ss->d_left; w.bits = ss->d_bits; w.n_bits = ss->n_bits; w.key_len = tb->d_keylen; w.leftmost = ss->leftmost;
+    w.a = a; w.left = ss->d_left; w.words = {ss->d_bits, ss->n_bits}; w.key_len = tb->d_keylen; w.leftmost = ss->leftmost;
     return w;
 }
 
 /* a word feed's window and word flags over the first min(*count, fcap) records of the full list */
 static int sw_flags(acb_streams *ss, acb_table *tb, const SlArgs &a, long long fcap, cudaStream_t s) {
     const SwArgs w = sw_args(ss, tb, a);
-    const unsigned grid = (unsigned)std::min<long long>((fcap + 255) / 256, grid_sms(tb) * 16);
-    if (ss->L == 1) acb_sw_flag_kernel<1><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
-    else if (ss->L == 2) acb_sw_flag_kernel<2><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
-    else acb_sw_flag_kernel<4><<<grid, 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
+    with_width(ss->L, [&](auto l) {
+        acb_sw_flag_kernel<decltype(l)::value><<<blocks(tb, fcap), 256, 0, s>>>(w, ss->d_full, ss->d_ctr, fcap, ss->d_flag);
+    });
     return launched("stream word flags");
 }
 
 /* a find_all word feed's m kept records (ss->d_settled, staged coordinates) in the reference order -- chunk, end, longest
- * key first -- and rebased to their chunks into d_out (the first cap of them); *d_count = m.  One radix pass when
- * chunk | end | length fit 64 bits, else two stable ones (end | length, then chunk). */
+ * key first -- and rebased to their chunks into d_out (the first cap of them); *d_count = m */
 static int sw_order(acb_streams *ss, acb_table *tb, const SlArgs &a, unsigned long long m, long long staged, acb_match *d_out,
                     int64_t cap, unsigned long long *d_count, cudaStream_t s) {
     if (m == 0) return ACB_OK;                             /* *d_count is 0 already */
-    const int max_len = tb->max_key_bytes / tb->L, mi = (int)m;
-    const int bh = bits_for((unsigned long long)std::max<long long>(a.n - 1, 1));
-    const int be = bits_for((unsigned long long)std::max<long long>(staged / a.L, 1)), bl = bits_for((unsigned long long)max_len);
-    const bool one_pass = bh + be + bl <= 64;
+    const SortKey k = sort_key(tb, a.n, staged / a.L);
     int rc = ensure(&ss->d_keys, &ss->keys_cap, 2 * (size_t)m);
     if (rc) return rc;
     unsigned long long *k0 = ss->d_keys, *k1 = ss->d_keys + m;
     size_t temp = 0;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, temp, k0, k1, ss->d_settled, ss->d_full, mi, 0, 64, s));
-    if ((rc = sl_tmp(ss, temp))) return rc;
-    const unsigned grid = (unsigned)std::min<long long>(((long long)m + 255) / 256, grid_sms(tb) * 16);
-    acb_sw_key_kernel<<<grid, 256, 0, s>>>(ss->d_settled, (long long)m, tb->d_keylen, bl, max_len, one_pass ? be + bl : -1, k0);
-    if ((rc = launched("stream word sort key"))) return rc;
-    temp = ss->tmp_cap;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(ss->d_tmp, temp, k0, k1, ss->d_settled, ss->d_full, mi, 0, one_pass ? bh + be + bl : be + bl, s));
-    acb_match *sorted = ss->d_full;
-    if (!one_pass) {
-        acb_sortkey_kernel<kKeyHay><<<(unsigned)((m + 255) / 256), 256, 0, s>>>(ss->d_full, (long long)m, tb->d_keylen, be, bl, max_len, k0);
-        if ((rc = launched("stream word sort key"))) return rc;
-        temp = ss->tmp_cap;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(ss->d_tmp, temp, k0, k1, ss->d_full, ss->d_settled, mi, 0, bh, s));
-        sorted = ss->d_settled;
-    }
-    acb_sw_emit_kernel<<<grid, 256, 0, s>>>(a, sorted, (long long)m, d_out, cap, d_count);
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, temp, k0, k1, ss->d_settled, ss->d_full, (int)m, 0, 64, s));
+    if ((rc = ensure(&ss->d_tmp, &ss->tmp_cap, temp))) return rc;
+    acb_match *sorted = k.bits() <= 64 ? ss->d_full : ss->d_settled;      /* two passes go through d_full */
+    if ((rc = sort_records<false>(tb, k, ss->d_settled, ss->d_full, sorted, (long long)m, k0, k1, ss->d_tmp, ss->tmp_cap, s,
+                                  "stream word sort key")))
+        return rc;
+    acb_sw_emit_kernel<<<blocks(tb, m), 256, 0, s>>>(a, sorted, (long long)m, d_out, cap, d_count);
     return launched("stream word emit");
 }
 
@@ -4473,10 +4452,7 @@ static int sw_order(acb_streams *ss, acb_table *tb, const SlArgs &a, unsigned lo
 static int sw_left(acb_streams *ss, acb_table *tb, const SlArgs &a, const unsigned long long *count, long long cap,
                    const long long *total, long long out_cap, cudaStream_t s) {
     const SwArgs w = sw_args(ss, tb, a);
-    const unsigned grid = (unsigned)std::min<long long>((a.n + 255) / 256, grid_sms(tb) * 16);
-    if (ss->L == 1) acb_sw_left_kernel<1><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
-    else if (ss->L == 2) acb_sw_left_kernel<2><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
-    else acb_sw_left_kernel<4><<<grid, 256, 0, s>>>(w, count, cap, total, out_cap);
+    with_width(ss->L, [&](auto l) { acb_sw_left_kernel<decltype(l)::value><<<blocks(tb, a.n), 256, 0, s>>>(w, count, cap, total, out_cap); });
     return launched("stream word edge");
 }
 
@@ -4503,8 +4479,7 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     a.ids = d_ids; a.n_streams = ss->n; a.pos = ss->d_pos; a.hold = ss->d_hold; a.tail = ss->d_tail; a.T = ss->T + ss->words; a.L = ss->L;
     a.chunks = d_chunks; a.off = reinterpret_cast<const long long *>(d_off); a.stride = stride; a.n = n;
     a.soff = ss->d_soff; a.last = ss->d_aux; a.xn = ss->d_aux + N; a.woff = ss->d_aux + 2 * N; a.final = final ? 1 : 0;
-    const long long most = grid_sms(tb) * 16;
-    const unsigned g_chunks = (unsigned)std::min<long long>((n + 256) / 256, most);
+    const unsigned g_chunks = blocks(tb, n + 1);
     /* 1. stage */
     acb_sl_len_kernel<<<g_chunks, 256, 0, s>>>(a);
     if ((rc = launched("stream staged lengths"))) return rc;
@@ -4532,13 +4507,12 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
         if (ss->words) {
             if ((rc = sw_flags(ss, tb, a, (long long)fcap, s))) return rc;
         } else {
-            acb_sl_flag_kernel<<<(unsigned)std::min<long long>(((long long)fcap + 255) / 256, most), 256, 0, s>>>(a, ss->d_full, ss->d_ctr,
-                                                                                                           (long long)fcap, tb->d_keylen, ss->d_flag);
+            acb_sl_flag_kernel<<<blocks(tb, (long long)fcap), 256, 0, s>>>(a, ss->d_full, ss->d_ctr, (long long)fcap, tb->d_keylen, ss->d_flag);
             if ((rc = launched("stream frontier flags"))) return rc;
         }
         size_t temp = 0;
         CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, temp, ss->d_full, ss->d_flag, ss->d_settled, ss->d_ctr + 1, (int)fcap, s));
-        if ((rc = sl_tmp(ss, temp))) return rc;
+        if ((rc = ensure(&ss->d_tmp, &ss->tmp_cap, temp))) return rc;
         temp = ss->tmp_cap;
         CUDA_TRY(cub::DeviceSelect::Flagged(ss->d_tmp, temp, ss->d_full, ss->d_flag, ss->d_settled, ss->d_ctr + 1, (int)fcap, s));
         if ((rc = timing_mark(&ss->ev[5], s))) return rc;
@@ -4571,7 +4545,7 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     /* 5. the new X per chunk, and the windows of a replacing feed */
     CUDA_TRY(cudaMemsetAsync(a.last, 0xff, N * sizeof(long long), s));
     if (m && ss->leftmost) {
-        acb_sl_last_kernel<<<(unsigned)std::min<long long>(((long long)m + 255) / 256, most), 256, 0, s>>>(a, chosen, ccount, ccap, r ? 0 : 1);
+        acb_sl_last_kernel<<<blocks(tb, (long long)m), 256, 0, s>>>(a, chosen, ccount, ccap, r ? 0 : 1);
         if ((rc = launched("stream last chosen"))) return rc;
     }
     acb_sl_frontier_kernel<<<g_chunks, 256, 0, s>>>(a);

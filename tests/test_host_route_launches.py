@@ -12,11 +12,13 @@ import pytest
 
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200 import synth
+from pyahocorasick_b200.automaton import _word_bits
 
 KEYS = [b"he", b"she", b"his", b"hers"]
 HAYS = [b"ushers and she sells his shells", b"his hers", b"", b"hehe she said"]
 CAP = 1024
 AT_LEAST_PREFIX = 2                                           # ACB_MATCH_AT_LEAST_PREFIX
+WORD_BITS, N_WORD_BITS = _word_bits(("bytes", None), 1)        # the default word set of the acb_*_words routes
 
 
 def _batch():
@@ -115,6 +117,23 @@ def _replace_host(L, A, tb, flat, off):
                                                                      N.ALGO_FILTER, oo, o, oc, t))
 
 
+def _word_batch(tb, flat, off):
+    return tb, N.ptr(flat), flat.size, N.ptr(off), len(off) - 1, 0, N.ptr(WORD_BITS), N_WORD_BITS
+
+
+def _scan_host_words(L, A, tb, flat, off):
+    _records(L, lambda out, n: L.acb_scan_host_words(*_word_batch(tb, flat, off), out, CAP, n, N.ALGO_FILTER, 1))
+
+
+def _scan_host_leftmost_words(L, A, tb, flat, off):
+    _records(L, lambda out, n: L.acb_scan_host_leftmost_words(*_word_batch(tb, flat, off), out, CAP, n, N.ALGO_FILTER))
+
+
+def _replace_host_words(L, A, tb, flat, off):
+    _with_replacer(L, tb, lambda r, oo, o, oc, t: L.acb_replace_host_words(r, *_word_batch(tb, flat, off), N.ALGO_FILTER, oo, o,
+                                                                           oc, t))
+
+
 def _feed_leftmost(L, A, tb, flat, off):
     _with_streams(L, lambda p: L.acb_streams_new_leftmost(tb, len(HAYS), p),
                   lambda ss: _records(L, lambda out, n: L.acb_streams_feed_leftmost_host(
@@ -132,6 +151,8 @@ def _streams_replace(L, A, tb, flat, off):
 SELECTION = 1 + 1 + 1 + 1 + 2
 # the replacement (rp_offsets, rp_write): delta, records, offsets, tiles, write
 REPLACEMENT = 3 + 2
+# the whole-word filter (acb_word_filter_device): flags, emit + count
+WORD_FILTER = 1 + 2
 # a final leftmost feed up to its selection: staged lengths, gather tiles + gather, scan, frontier flags, then last chosen
 # and frontier after it
 FEED_LEFTMOST = 1 + 2 + 1 + 1 + 1 + 1
@@ -148,6 +169,9 @@ CASES = {
     "replace_host": (_replace_host, 1 + SELECTION + REPLACEMENT),              # scan, selection, replacement
     "feed_leftmost": (_feed_leftmost, FEED_LEFTMOST + SELECTION + 1),          # feed, selection, commit
     "streams_replace": (_streams_replace, FEED_LEFTMOST + SELECTION + 2 + REPLACEMENT + 1),   # ... window gather, replacement, commit
+    "scan_host_words": (_scan_host_words, 1 + WORD_FILTER + 1),                                 # scan, word filter, sort key
+    "scan_host_leftmost_words": (_scan_host_leftmost_words, 1 + WORD_FILTER + SELECTION),       # scan, word filter, selection
+    "replace_host_words": (_replace_host_words, 1 + WORD_FILTER + SELECTION + REPLACEMENT),     # ... replacement
 }
 
 

@@ -320,6 +320,28 @@ def test_sort_matches_device_zero_and_one_record():
     assert one.cpu().tolist() == [[5, 6, 1]]
 
 
+@pytest.mark.gpu
+def test_sort_matches_device_on_two_streams():
+    """two sorts of different record sets for one table, issued on two CUDA streams with no host wait between them: the
+    second waits for the first before it reuses the table's sort scratch.  Without that wait the second would overwrite
+    keys the first may still be reading; whether the first is still running then is up to the device, so the test can
+    pass without the wait too."""
+    import torch
+    A = _sort_automaton(4)
+    tb = A._ensure_table(0)
+    kl = np.asarray(A.flat()["key_len"], dtype=np.int64)
+    n_hay, max_letters = 1 << 16, (1 << 20) - 1
+    rng = np.random.Generator(np.random.PCG64(5))
+    recs = [_synthetic_records(rng, n, n_hay, max_letters, len(kl)) for n in (400_000, 300_000)]
+    ds = [torch.from_numpy(r).cuda() for r in recs]
+    torch.cuda.synchronize()
+    for d, s in zip(ds, (torch.cuda.Stream(), torch.cuda.Stream())):
+        N.check(N.lib().acb_sort_matches_device(tb, d.data_ptr(), len(d), n_hay, max_letters, s.cuda_stream))
+    torch.cuda.synchronize()
+    for d, r in zip(ds, recs):
+        assert np.array_equal(d.cpu().numpy(), r[np.lexsort((-kl[r[:, 2]], r[:, 1], r[:, 0]))])
+
+
 # ------------------------------------------------------------------ the record sort through its callers
 def _one_long_key_batch(long_letters, rng):
     """about 128 MiB in 65 536 haystacks; keys: one of `long_letters` letters (it never matches) and short keys that
