@@ -448,6 +448,23 @@ int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_records, int64
 int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
                            int64_t stride_bytes, acb_match *out, int64_t cap, int64_t *n_found, int algo);
 
+/* ---- leftmost-first: the same rule with priority by key order --------------------------------------------------
+ * Among the matches at the smallest start >= p, the one with the smallest key id (the order in which the keys were
+ * first added) instead of the longest.  One selection kind says which rule a call follows; the entries below take it
+ * where the rule is not in the name.  Every other entry selects leftmost-longest. */
+#define ACB_SELECT_LONGEST 0
+#define ACB_SELECT_FIRST   1
+
+/* acb_leftmost_longest_device's contract, the leftmost-first rule */
+int acb_leftmost_first_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay, int64_t max_hay_letters,
+                              acb_match *d_out, int64_t cap, int64_t *d_count, void *stream);
+
+/* acb_scan_host_leftmost (n_bits < 0 and bits == NULL: no word set) or acb_scan_host_leftmost_words (a word set as
+ * there) under selection kind `kind` (ACB_EINVAL for another value) */
+int acb_scan_host_leftmost_kind(acb_table *tb, int kind, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
+                                int64_t n_hay, int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out,
+                                int64_t cap, int64_t *n_found, int algo);
+
 /* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last selection's stages on this thread: sort,
  * candidates, successors, chain, emit (the first n of them, n <= 5), from CUDA events between the stages (the call then
  * waits for them); 0 when timing is off. */
@@ -465,6 +482,11 @@ typedef struct acb_replacer acb_replacer;
 int  acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets, int64_t n_ids,
                       acb_replacer **out);
 void acb_replacer_free(acb_replacer *r);
+
+/* A replacer of selection kind `kind`: acb_replace_host, acb_replace_host_words and the replacing stream feeds rewrite
+ * the matches that rule chooses.  acb_replacer_new makes one of kind ACB_SELECT_LONGEST. */
+int  acb_replacer_new_kind(const acb_table *tb, int kind, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets,
+                           int64_t n_ids, acb_replacer **out);
 
 /* DEVICE buffers, asynchronous on `stream`.  The batch is laid out as for acb_scan_device; d_chosen holds the
  * *d_n_chosen <= chosen_cap records acb_leftmost_longest_device wrote for it (haystack order, then end_index ascending,
@@ -502,6 +524,13 @@ int acb_last_replace_ms(float *ms, int32_t n);
  * fit) and, replacing, the decided windows' size.  Feeds of one batch must not overlap in time.  algo: ACB_ALGO_AUTO,
  * _FILTER or _DFA. */
 int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out);
+
+/* A leftmost stream batch of selection kind `kind`: n_bits < 0 and bits == NULL, as acb_streams_new_leftmost; else a
+ * whole-word leftmost batch with that word set, as acb_streams_new_words with leftmost != 0.  Those two make batches of
+ * kind ACB_SELECT_LONGEST.  The feeds select by the batch's kind; a replacing feed refuses (ACB_EINVAL) a replacer of
+ * another kind. */
+int acb_streams_new_leftmost_kind(const acb_table *tb, int64_t n_streams, int kind, const uint32_t *bits, int64_t n_bits,
+                                  acb_streams **out);
 
 /* The chosen records in chunk order, then end_index ascending; end_index is relative to the chunk (>= -T: a match may
  * start in letters held back from earlier chunks).  Zeroes *d_count itself, counts every chosen record, stores the

@@ -14,6 +14,7 @@ ABI_VERSION = 5            # ACB_ABI_VERSION of include/acb200.h this binding wa
 ACB_OK, ACB_ENOMEM, ACB_EINVAL, ACB_ESTATE, ACB_ECUDA, ACB_EOVERFLOW, ACB_ERANGE = 0, -1, -2, -3, -4, -5, -6
 ALGO_AUTO, ALGO_FILTER, ALGO_DFA, ALGO_LONG = 0, 1, 2, 3
 ALGOS = {"auto": ALGO_AUTO, "filter": ALGO_FILTER, "dfa": ALGO_DFA, "long": ALGO_LONG}
+SELECT_LONGEST, SELECT_FIRST = 0, 1     # ACB_SELECT_*: the match a leftmost selection takes at a start
 MAX_SKIP = 1024            # ACB_MAX_SKIP: largest skip set of the white-space scans
 
 MATCH_DTYPE = np.dtype([("hay_id", "<i4"), ("end_index", "<i4"), ("key_id", "<i4")])
@@ -114,6 +115,11 @@ def lib() -> ctypes.CDLL:
         "acb_leftmost_longest_device": (ctypes.c_int, [vp, vp, i64, i64, i64, vp, i64, vp, vp]),
         "acb_scan_host_leftmost": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, i64, pi64, ctypes.c_int]),
         "acb_last_leftmost_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), i32]),
+        "acb_leftmost_first_device": (ctypes.c_int, [vp, vp, i64, i64, i64, vp, i64, vp, vp]),
+        "acb_scan_host_leftmost_kind": (ctypes.c_int, [vp, ctypes.c_int, vp, i64, vp, i64, i64, vp, i64, vp, i64, pi64,
+                                                       ctypes.c_int]),
+        "acb_replacer_new_kind": (ctypes.c_int, [vp, ctypes.c_int, vp, i64, vp, i64, ctypes.POINTER(vp)]),
+        "acb_streams_new_leftmost_kind": (ctypes.c_int, [vp, i64, ctypes.c_int, vp, i64, ctypes.POINTER(vp)]),
         "acb_replacer_new": (ctypes.c_int, [vp, vp, i64, vp, i64, ctypes.POINTER(vp)]),
         "acb_replacer_free": (None, [vp]),
         "acb_replace_device": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, i64, vp, vp, vp, i64, vp, vp]),
@@ -173,7 +179,8 @@ EXPORTED_SYMBOLS = [
     "acb_streams_new_leftmost", "acb_streams_feed_leftmost_device", "acb_streams_feed_leftmost_host", "acb_streams_replace_device",
     "acb_streams_replace_host", "acb_last_stream_leftmost_ms", "acb_word_filter_device", "acb_scan_host_words",
     "acb_scan_host_leftmost_words", "acb_replace_host_words", "acb_last_words_ms", "acb_streams_new_words",
-    "acb_streams_feed_words_device", "acb_streams_feed_words_host", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_streams_feed_words_device", "acb_streams_feed_words_host", "acb_leftmost_first_device", "acb_scan_host_leftmost_kind",
+    "acb_replacer_new_kind", "acb_streams_new_leftmost_kind", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

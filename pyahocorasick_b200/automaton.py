@@ -819,15 +819,17 @@ class Automaton:
 
     @_locked
     def _words_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str, sort: bool,
-                    device: Optional[int], narrow: bool, words: tuple, leftmost: bool) -> np.ndarray:
-        """acb_scan_host_words / acb_scan_host_leftmost_words: upload, scan, keep the whole-word matches, then sort or
-        select, copy back (_host_records)."""
+                    device: Optional[int], narrow: bool, words: tuple, leftmost: bool, select: int = N.SELECT_LONGEST) -> np.ndarray:
+        """acb_scan_host_words / acb_scan_host_leftmost_words (acb_scan_host_leftmost_kind for leftmost-first): upload,
+        scan, keep the whole-word matches, then sort or select, copy back (_host_records)."""
         lib = self._lib
         bits, n_bits = _word_bits(words, 1 if narrow else self._L)
         args = (N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes,
                 N.ptr(bits) if n_bits else None, n_bits, None)
 
         def scan(tb, cap, found_ref):
+            if leftmost and select != N.SELECT_LONGEST:
+                return lib.acb_scan_host_leftmost_kind(tb, select, *args, cap, found_ref, N.ALGOS[algo])
             if leftmost:
                 return lib.acb_scan_host_leftmost_words(tb, *args, cap, found_ref, N.ALGOS[algo])
             return lib.acb_scan_host_words(tb, *args, cap, found_ref, N.ALGOS[algo], int(sort))
@@ -1029,47 +1031,82 @@ class Automaton:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow)
         return Matches(rec, self._values)
 
-    @_locked
-    def _leftmost_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str,
-                       device: Optional[int], narrow: bool) -> np.ndarray:
-        """acb_scan_host_leftmost: upload, scan, select, copy back (_host_records)."""
-        return self._host_records(device, narrow, n_hay, lambda tb, cap, found_ref: self._lib.acb_scan_host_leftmost(
-            tb, N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes, None, cap,
-            found_ref, N.ALGOS[algo]))
+    def find_leftmost_first_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
+                                  whole_words=False) -> "Matches":
+        """Leftmost-first non-overlapping matches of a whole batch, selected on the GPU (input forms and result type of
+        find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or after
+        p, take the smallest such start, the match there whose key was added first, and continue after its end.  This is
+        the rule of regex alternation (``sam|samwise`` finds ``sam`` in ``samwise``): keys earlier in the dictionary win
+        at a start, but a match further left always wins.  Priority is the order in which add_word first added each key:
+        add_word of a key already present keeps its place, removing a key and adding it again moves it to the end.  An
+        automaton read back from pickle or save numbers its keys afresh, so its priority can differ.  Records come in
+        haystack order, then end_index ascending; algo and whole_words as for find_leftmost_longest_batch."""
+        self._require_automaton()
+        if algo not in ("auto", "filter", "dfa"):
+            raise ValueError(f"algo {algo!r}: leftmost-first takes 'auto', 'filter' or 'dfa'")
+        words = self._words(whole_words)
+        b = self._batch_input(haystacks)
+        if b.empty:
+            rec = np.empty(0, dtype=N.MATCH_DTYPE)
+        elif b.kind == "device":
+            rec = self._leftmost_device(b, algo, words, N.SELECT_FIRST)
+        elif words is not None:
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, select=N.SELECT_FIRST)
+        else:
+            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST)
+        return Matches(rec, self._values)
 
     @_locked
-    def _leftmost_device(self, batch, algo: str, words: Optional[tuple] = None) -> np.ndarray:
-        """A CUDA tensor batch: the full scan into a device buffer, then acb_leftmost_longest_device, both on torch's
-        current stream; only the chosen records come back."""
+    def _leftmost_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str,
+                       device: Optional[int], narrow: bool, select: int = N.SELECT_LONGEST) -> np.ndarray:
+        """acb_scan_host_leftmost (acb_scan_host_leftmost_kind for leftmost-first): upload, scan, select, copy back
+        (_host_records)."""
+        lib = self._lib
+        args = (N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes)
+
+        def scan(tb, cap, found_ref):
+            if select != N.SELECT_LONGEST:
+                return lib.acb_scan_host_leftmost_kind(tb, select, *args, None, -1, None, cap, found_ref, N.ALGOS[algo])
+            return lib.acb_scan_host_leftmost(tb, *args, None, cap, found_ref, N.ALGOS[algo])
+        return self._host_records(device, narrow, n_hay, scan)
+
+    @_locked
+    def _leftmost_device(self, batch, algo: str, words: Optional[tuple] = None, select: int = N.SELECT_LONGEST) -> np.ndarray:
+        """A CUDA tensor batch: the full scan into a device buffer, then the selection, both on torch's current stream;
+        only the chosen records come back."""
         t = _aligned(batch.data)
         dev = _device_of(t)
         tb = self._ensure_table(dev)
         with _on_device(dev) as stream:
-            out, cnt, _ = self._leftmost_chosen(tb, t, batch.n, batch.stride, algo, stream, words)
+            out, cnt, _ = self._leftmost_chosen(tb, t, batch.n, batch.stride, algo, stream, words, select)
             found = int(cnt.item())
             return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
 
-    def _leftmost_chosen(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None):
+    def _leftmost_chosen(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None,
+                         select: int = N.SELECT_LONGEST):
         """The chosen records of an aligned device batch, left on the device: (records [cap, 3] int32 CUDA tensor,
         their count as an int64 CUDA tensor, cap).  Synchronises once, to size the full list; with words, the
-        selection runs on the whole-word matches and a second wait sizes them (_device_matches)."""
+        selection runs on the whole-word matches and a second wait sizes them (_device_matches).  select: the rule,
+        acb_leftmost_longest_device or acb_leftmost_first_device."""
         import torch
         full, m = self._device_matches(tb, t, n, stride, algo, stream, words)
         cap = max(m, 1)
         out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
         cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
-        N.check(self._lib.acb_leftmost_longest_device(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap,
-                                                      cnt.data_ptr(), stream))
+        fn = self._lib.acb_leftmost_longest_device if select == N.SELECT_LONGEST else self._lib.acb_leftmost_first_device
+        N.check(fn(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap, cnt.data_ptr(), stream))
         return out, cnt, cap
 
-    def replacer(self, replacements=None, *, device: Optional[int] = None) -> "Replacer":
-        """A `Replacer` that rewrites whole batches with the leftmost-longest matches replaced (Replacer.replace_batch).
+    def replacer(self, replacements=None, *, device: Optional[int] = None, leftmost_first: bool = False) -> "Replacer":
+        """A `Replacer` that rewrites whole batches with the leftmost-longest matches replaced (Replacer.replace_batch);
+        leftmost_first=True: the matches find_leftmost_first_batch chooses.
         replacements=None: every key is replaced by its value (STORE_ANY only); else a mapping from every key to its
         replacement, of the haystack type (bytes, str, or a tuple for KEY_SEQUENCE).  The replacements are taken when the
         replacer is made: giving a key a new value (add_word of a key already present) does not change it or make it
         stale, while adding or removing keys, or make_automaton, does."""
         self._require_automaton()
-        return Replacer(self, replacements, _default_device() if device is None else device)
+        return Replacer(self, replacements, _default_device() if device is None else device,
+                        N.SELECT_FIRST if leftmost_first else N.SELECT_LONGEST)
 
     def dump(self):
         """(nodes, edges, fail) in the spirit of src/Automaton.c:1100-1180, with int state ids."""
@@ -1183,7 +1220,7 @@ class Automaton:
 
     def stream_batch(self, n_streams: int, *, long: bool = False, algo: str = "auto",
                      device: Optional[int] = None, ignore_white_space: bool = False,
-                     leftmost_longest: bool = False, whole_words=False) -> "StreamBatch":
+                     leftmost_longest: bool = False, whole_words=False, leftmost_first: bool = False) -> "StreamBatch":
         """`n_streams` independent streams searched chunk by chunk, the next chunk of many of them in one GPU call
         (StreamBatch.feed).  long=False: stream s reports what the reference's ``iter(c0)`` ... ``.set(c1)`` ...
         reports over its chunks -- every match, also those across chunk boundaries; long=True: what
@@ -1191,7 +1228,8 @@ class Automaton:
         ignore_white_space=True (find_all batches only): what ``iter(c0, ignore_white_space=True)`` ... ``.set(c1)``
         ... reports; positions still count every letter, and a key that white space splits across chunks is found.
         leftmost_longest=True: what `find_leftmost_longest_batch` reports for each stream's whole text, delivered as
-        soon as no later letter can change it (see StreamBatch.finish).
+        soon as no later letter can change it (see StreamBatch.finish); leftmost_first=True: the same for
+        `find_leftmost_first_batch` (not with leftmost_longest, long or ignore_white_space).
         whole_words (see find_all_batch; not with long=True or ignore_white_space=True): only whole-word matches, what
         find_all_batch or find_leftmost_longest_batch reports with the same option for each stream's whole text.  A
         match is reported once the letter after it has arrived (or by `finish`), so a stream holds back one letter more.
@@ -1207,13 +1245,15 @@ class Automaton:
             raise ValueError("whole_words stream batches take neither long=True nor ignore_white_space=True")
         if leftmost_longest and (long or ignore_white_space):
             raise ValueError("leftmost_longest stream batches take neither long=True nor ignore_white_space=True")
+        if leftmost_first and (leftmost_longest or long or ignore_white_space):
+            raise ValueError("leftmost_first stream batches take none of leftmost_longest, long=True and ignore_white_space=True")
         if algo not in (("auto", "long") if long else ("auto", "filter", "dfa")):
             raise ValueError(f"algo {algo!r} does not fit a {'long' if long else 'find_all'} stream batch")
         if long and ignore_white_space:
             raise ValueError("iter_long has no ignore_white_space option")
         skip = self._skip_set(False) if ignore_white_space else None
         return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip,
-                           bool(leftmost_longest), words)
+                           bool(leftmost_longest), words, bool(leftmost_first))
 
     # ------------------------------------------------------------------ batch lookups (new)
     # exists / match / longest_prefix / get for a whole batch of keys, in one GPU call (acb_lookup_*).  `keys` takes the
@@ -1493,15 +1533,20 @@ class StreamBatch(_Streams):
     A whole_words batch reports, over all feeds and `finish` of a stream, what find_all_batch (or, leftmost_longest,
     find_leftmost_longest_batch) reports with the same whole_words for its whole text.  A find_all match is reported by
     the first feed after which at least one letter follows it, so its end_index can be the last letter of an earlier
-    chunk; a leftmost_longest match by the first feed after which it starts before ``position - longest_word``."""
+    chunk; a leftmost_longest match by the first feed after which it starts before ``position - longest_word``.
+
+    A leftmost_first batch is a leftmost_longest batch under the leftmost-first rule: it reports what
+    `find_leftmost_first_batch` reports (with the same whole_words), at the same points."""
 
     def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None,
-                 leftmost_longest: bool = False, words: Optional[tuple] = None):
+                 leftmost_longest: bool = False, words: Optional[tuple] = None, leftmost_first: bool = False):
         self._A = A
         self._version = A._version
         self.n_streams = n_streams
         self.long = long
         self.leftmost_longest = leftmost_longest
+        self.leftmost_first = leftmost_first
+        self._select = N.SELECT_FIRST if leftmost_first else N.SELECT_LONGEST
         self._words = words
         self.whole_words = words is not None
         self._algo = algo
@@ -1511,7 +1556,7 @@ class StreamBatch(_Streams):
         with A._gpu_lock:
             if words is not None:
                 self._ss = self._native("new_words")
-            elif leftmost_longest:
+            elif leftmost_longest or leftmost_first:
                 self._ss = self._native("new_leftmost")
             else:
                 self._ss = self._native("new") if skip is None else self._native("new_skip", skip)
@@ -1520,9 +1565,9 @@ class StreamBatch(_Streams):
         """Every call into the native stream batch (acb_streams_*) goes through here.
           new -> handle;  new_skip(skip set uint32) -> handle of a batch that skips those letters;  free;  reset(ids int32 or None);  positions -> int64[n_streams];
           feed(kind, data, offsets, n, stride, ids, sort) -> records (hay_id = chunk index, end_index in the chunk);
-          new_leftmost -> handle of a leftmost-longest batch;
+          new_leftmost -> handle of a leftmost batch (leftmost-longest or leftmost-first: self._select);
           feed_leftmost(kind, data, offsets, n, stride, ids, final) -> its chosen records, as feed's;
-          new_words -> handle of a whole-word batch (leftmost-longest or find_all, with the batch's word set);
+          new_words -> handle of a whole-word batch (leftmost or find_all, with the batch's word set);
           feed_words(kind, data, offsets, n, stride, ids, final) -> a find_all word batch's records, ordered, as feed's"""
         A = self._A
         if op == "new":
@@ -1530,9 +1575,10 @@ class StreamBatch(_Streams):
             N.check(A._lib.acb_streams_new(A._ensure_table(self._device), self.n_streams, int(self.long), ctypes.byref(ss)))
             return ss
         if op == "new_leftmost":
-            return _new_leftmost_streams(A, self.n_streams, self._device)
+            return _new_leftmost_streams(A, self.n_streams, self._device, self._select)
         if op == "new_words":
-            return _new_word_streams(A, self.n_streams, self._device, self.leftmost_longest, self._words)
+            return _new_word_streams(A, self.n_streams, self._device, self.leftmost_longest or self.leftmost_first, self._words,
+                                     self._select)
         if op == "new_skip":
             skip, = args
             ss = ctypes.c_void_p()
@@ -1601,8 +1647,9 @@ class StreamBatch(_Streams):
             self._check()
             b, lens = _stream_chunks(A, chunks)
             ids32 = self._ids(ids, b.n)
-            if self.leftmost_longest or self.whole_words:
-                rec = self._native("feed_leftmost" if self.leftmost_longest else "feed_words", *b[:5], ids32, False)
+            leftmost = self.leftmost_longest or self.leftmost_first
+            if leftmost or self.whole_words:
+                rec = self._native("feed_leftmost" if leftmost else "feed_words", *b[:5], ids32, False)
             else:
                 rec = self._native("feed", *b[:5], ids32, sort)
             m, sid = self._stream_matches(rec, b.n, ids32)
@@ -1610,17 +1657,18 @@ class StreamBatch(_Streams):
             return m
 
     def finish(self, ids=None) -> Matches:
-        """leftmost_longest and whole_words batches: the matches streams `ids` (default: all) still hold back, as if their
-        text ended here; those streams then start again at position 0 with nothing held.  Other stream batches:
-        ValueError."""
-        if not (self.leftmost_longest or self.whole_words):
-            raise ValueError("finish() belongs to leftmost_longest and whole_words stream batches")
+        """leftmost_longest, leftmost_first and whole_words batches: the matches streams `ids` (default: all) still hold
+        back, as if their text ended here; those streams then start again at position 0 with nothing held.  Other stream
+        batches: ValueError."""
+        leftmost = self.leftmost_longest or self.leftmost_first
+        if not (leftmost or self.whole_words):
+            raise ValueError("finish() belongs to leftmost_longest, leftmost_first and whole_words stream batches")
         A = self._A
         with A._gpu_lock:
             self._check()
             n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
             ids32 = self._ids(ids, n)
-            rec = self._native("feed_leftmost" if self.leftmost_longest else "feed_words", "host", np.empty(0, np.uint8),
+            rec = self._native("feed_leftmost" if leftmost else "feed_words", "host", np.empty(0, np.uint8),
                                np.zeros(n + 1, np.int64), n, 0, ids32, True)
             m, sid = self._stream_matches(rec, n, ids32)
             self._restart(sid)
@@ -1633,12 +1681,15 @@ class Replacer:
     ``replace_batch(haystacks)`` takes, per haystack, exactly the matches `find_leftmost_longest_batch` chooses, replaces
     the letters of each by its key's replacement and copies every other letter; a replacement is never scanned again.
     The replacements are a snapshot taken when the replacer is made.  A replacer belongs to the key set it was made
-    for: after keys are added or removed, `replace_batch` raises ValueError as a stale iterator does."""
+    for: after keys are added or removed, `replace_batch` raises ValueError as a stale iterator does.  A leftmost_first
+    replacer (Automaton.replacer) takes the matches `find_leftmost_first_batch` chooses instead, in both methods."""
 
-    def __init__(self, A: Automaton, replacements, device: int):
+    def __init__(self, A: Automaton, replacements, device: int, select: int = N.SELECT_LONGEST):
         self._A = A
         self._version = A._version
         self._device = device
+        self._select = select
+        self.leftmost_first = select == N.SELECT_FIRST
         self._native = {}                                   # (narrow, device) -> acb_replacer*, uploaded on first use
         if replacements is None and A._store != STORE_ANY:
             raise ValueError("replacer() without replacements takes each key's value: the automaton must be STORE_ANY")
@@ -1683,8 +1734,11 @@ class Replacer:
         if r is None:
             flat, offs = self._tables[narrow]
             r = ctypes.c_void_p()
-            N.check(self._A._lib.acb_replacer_new(tb, N.ptr(flat) if flat.size else None, int(flat.size), N.ptr(offs),
-                                                  len(offs) - 1, ctypes.byref(r)))
+            args = (N.ptr(flat) if flat.size else None, int(flat.size), N.ptr(offs), len(offs) - 1, ctypes.byref(r))
+            if self._select == N.SELECT_LONGEST:
+                N.check(self._A._lib.acb_replacer_new(tb, *args))
+            else:
+                N.check(self._A._lib.acb_replacer_new_kind(tb, self._select, *args))
             self._native[(narrow, device)] = r
         return r
 
@@ -1789,7 +1843,7 @@ class Replacer:
         dev = _device_of(t)
         tb = A._ensure_table(dev)
         with _on_device(dev) as stream:
-            chosen, cnt, cap = A._leftmost_chosen(tb, t, n, stride, algo, stream, words)
+            chosen, cnt, cap = A._leftmost_chosen(tb, t, n, stride, algo, stream, words, self._select)
             r = self._replacer(tb, False, dev)
             out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
             total = torch.empty(1, dtype=torch.int64, device=t.device)
@@ -1830,8 +1884,8 @@ class ReplaceStream(_Streams):
         lib = A._lib
         if op == "new":
             if self._words is not None:
-                return _new_word_streams(A, self.n_streams, self._device, True, self._words)
-            return _new_leftmost_streams(A, self.n_streams, self._device)
+                return _new_word_streams(A, self.n_streams, self._device, True, self._words, self._R._select)
+            return _new_leftmost_streams(A, self.n_streams, self._device, self._R._select)
         if op != "feed":
             return super()._native(op, *args)
         kind, data, offs, n, stride, ids, final = args
@@ -2167,18 +2221,28 @@ def _host_bytes(cap: int, call) -> np.ndarray:
     return out[:total.value]
 
 
-def _new_leftmost_streams(A: Automaton, n_streams: int, device: int):
+def _new_leftmost_streams(A: Automaton, n_streams: int, device: int, select: int = N.SELECT_LONGEST):
     ss = ctypes.c_void_p()
-    N.check(A._lib.acb_streams_new_leftmost(A._ensure_table(device), n_streams, ctypes.byref(ss)))
+    tb = A._ensure_table(device)
+    if select == N.SELECT_LONGEST:
+        N.check(A._lib.acb_streams_new_leftmost(tb, n_streams, ctypes.byref(ss)))
+    else:
+        N.check(A._lib.acb_streams_new_leftmost_kind(tb, n_streams, select, None, -1, ctypes.byref(ss)))
     return ss
 
 
-def _new_word_streams(A: Automaton, n_streams: int, device: int, leftmost: bool, words: tuple):
-    """a whole-word stream batch (acb_streams_new_words) with the word set at the streams' full letter width"""
+def _new_word_streams(A: Automaton, n_streams: int, device: int, leftmost: bool, words: tuple, select: int = N.SELECT_LONGEST):
+    """a whole-word stream batch (acb_streams_new_words; acb_streams_new_leftmost_kind for leftmost-first) with the
+    word set at the streams' full letter width"""
     bits, n_bits = _word_bits(words, A._L)
     ss = ctypes.c_void_p()
-    N.check(A._lib.acb_streams_new_words(A._ensure_table(device), n_streams, int(leftmost), N.ptr(bits) if n_bits else None,
-                                         n_bits, ctypes.byref(ss)))
+    tb = A._ensure_table(device)
+    if leftmost and select != N.SELECT_LONGEST:
+        N.check(A._lib.acb_streams_new_leftmost_kind(tb, n_streams, select, N.ptr(bits) if n_bits else None, n_bits,
+                                                     ctypes.byref(ss)))
+    else:
+        N.check(A._lib.acb_streams_new_words(tb, n_streams, int(leftmost), N.ptr(bits) if n_bits else None, n_bits,
+                                             ctypes.byref(ss)))
     return ss
 
 

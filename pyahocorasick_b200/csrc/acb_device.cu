@@ -1871,9 +1871,10 @@ static T *carve(char *&p, size_t n) {
 /* Reference order (SURVEY 3.3): haystack, then end_index ascending, then longest key first; start order: haystack, then
  * start letter, then longest first.  One 64-bit radix key per record, hay_id | position | (max_len - len), packed into
  * the fewest bits.  When those need more than 64 bits, two stable passes: position | (max_len - len) first (kKeyEndLow,
- * kKeyStartLow), then hay_id (kKeyHay). */
+ * kKeyStartLow), then hay_id (kKeyHay).  The leftmost-first order puts key_id where max_len - len goes: hay | start |
+ * key_id (kKeyFirst), or start | key_id (kKeyFirstLow) then hay_id. */
 namespace {
-enum { kKeyEnd, kKeyStart, kKeyStartLow, kKeyHay, kKeyEndLow };
+enum { kKeyEnd, kKeyStart, kKeyStartLow, kKeyHay, kKeyEndLow, kKeyFirst, kKeyFirstLow };
 
 template <int kMode>
 __global__ void acb_sortkey_kernel(const acb_match *rec, long long n, const int32_t *key_len, int be, int bl,
@@ -1883,29 +1884,34 @@ __global__ void acb_sortkey_kernel(const acb_match *rec, long long n, const int3
     const acb_match m = rec[i];
     if (kMode == kKeyHay) { keys[i] = (uint32_t)m.hay_id; return; }
     const int len = __ldg(key_len + m.key_id);
-    const unsigned long long inv = (unsigned long long)(max_len - len);
+    const bool by_id = kMode == kKeyFirst || kMode == kKeyFirstLow;
+    const unsigned long long inv = by_id ? (unsigned long long)(uint32_t)m.key_id : (unsigned long long)(max_len - len);
     const bool by_end = kMode == kKeyEnd || kMode == kKeyEndLow;
     const uint32_t pos = by_end ? (uint32_t)m.end_index : (uint32_t)(m.end_index - len + 1);
-    const unsigned long long hay = kMode == kKeyStartLow || kMode == kKeyEndLow ? 0ULL : (unsigned long long)(uint32_t)m.hay_id << (be + bl);
+    const bool low = kMode == kKeyStartLow || kMode == kKeyEndLow || kMode == kKeyFirstLow;
+    const unsigned long long hay = low ? 0ULL : (unsigned long long)(uint32_t)m.hay_id << (be + bl);
     keys[i] = hay | ((unsigned long long)pos << bl) | inv;
 }
 } // namespace
 
-/* the sort key's fields: bits of the haystack, of the position and of max_len - key length */
+/* the sort key's fields: bits of the haystack, of the position and of the tie-break: max_len - key length, or (the
+ * leftmost-first order) the key id, over every id of the table, removed ones included */
 struct SortKey {
     int bh, be, bl, max_len;
     int bits() const { return bh + be + bl; }
 };
-static SortKey sort_key(const acb_table *tb, int64_t n_hay, int64_t max_hay_letters) {
+static SortKey sort_key(const acb_table *tb, int64_t n_hay, int64_t max_hay_letters, int kind = ACB_SELECT_LONGEST) {
     auto bits_for = [](unsigned long long v) { int b = 1; while (b < 64 && (v >> b)) b++; return b; };
     const int max_len = tb->max_key_bytes / tb->L;
+    const unsigned long long tie = kind == ACB_SELECT_FIRST ? (unsigned long long)std::max(tb->n_keys - 1, 0) : (unsigned long long)max_len;
     return {bits_for((unsigned long long)std::max<int64_t>(n_hay - 1, 1)), bits_for((unsigned long long)std::max<int64_t>(max_hay_letters, 1)),
-            bits_for((unsigned long long)max_len), max_len};
+            bits_for(tie), max_len};
 }
 
-/* The n records of `in` into `out`, in reference order (kByStart: start order).  Keys in k0 and k1 (n each); tmp: cub
- * scratch of temp bytes, enough for a 64-bit sort of n.  Two passes go through `mid`, and `out` may then be `in`. */
-template <bool kByStart>
+/* The n records of `in` into `out`, in the order of sort-key modes kOne (one pass) / kLow (the first of two passes,
+ * then hay_id).  Keys in k0 and k1 (n each); tmp: cub scratch of temp bytes, enough for a 64-bit sort of n.  Two passes
+ * go through `mid`, and `out` may then be `in`. */
+template <int kOne, int kLow>
 static int sort_records(acb_table *tb, const SortKey &k, const acb_match *in, acb_match *mid, acb_match *out, long long n,
                         unsigned long long *k0, unsigned long long *k1, void *tmp, size_t temp, cudaStream_t s, const char *what) {
     const unsigned grid = (unsigned)((n + 255) / 256);
@@ -1913,12 +1919,12 @@ static int sort_records(acb_table *tb, const SortKey &k, const acb_match *in, ac
     size_t t = temp;
     int rc;
     if (k.bits() <= 64) {
-        acb_sortkey_kernel<kByStart ? kKeyStart : kKeyEnd><<<grid, 256, 0, s>>>(in, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
+        acb_sortkey_kernel<kOne><<<grid, 256, 0, s>>>(in, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
         if ((rc = launched(what))) return rc;
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t, k0, k1, in, out, ni, 0, k.bits(), s));
         return ACB_OK;
     }
-    acb_sortkey_kernel<kByStart ? kKeyStartLow : kKeyEndLow><<<grid, 256, 0, s>>>(in, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
+    acb_sortkey_kernel<kLow><<<grid, 256, 0, s>>>(in, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
     if ((rc = launched(what))) return rc;
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t, k0, k1, in, mid, ni, 0, k.be + k.bl, s));
     acb_sortkey_kernel<kKeyHay><<<grid, 256, 0, s>>>(mid, n, tb->d_keylen, k.be, k.bl, k.max_len, k0);
@@ -1953,7 +1959,7 @@ extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int6
     unsigned long long *k0 = carve<unsigned long long>(p, n), *k1 = carve<unsigned long long>(p, n);
     acb_match *r1 = carve<acb_match>(p, n);
     void *tmp = carve<char>(p, temp);
-    if ((rc = sort_records<false>(tb, k, d_records, nullptr, r1, n, k0, k1, tmp, temp, s, "sort key"))) return rc;
+    if ((rc = sort_records<kKeyEnd, kKeyEndLow>(tb, k, d_records, nullptr, r1, n, k0, k1, tmp, temp, s, "sort key"))) return rc;
     CUDA_TRY(cudaMemcpyAsync(d_records, r1, (size_t)n * sizeof(acb_match), cudaMemcpyDeviceToDevice, s));
     return scratch_done(&tb->sort_buf.done, s);
 }
@@ -2603,6 +2609,7 @@ struct acb_streams {
     /* leftmost-longest batches (acb_streams_new_leftmost): the tail holds the letters after X, the position up to which
      * every match is decided and emitted; d_hold[s] = pos - X of stream s (<= T).  Per-feed scratch, grown on demand. */
     int leftmost = 0;
+    int kind = ACB_SELECT_LONGEST;                                /* the selection of a leftmost batch */
     long long *d_hold = nullptr;
     long long *d_soff = nullptr; size_t soff_cap = 0;             /* staged byte offsets [n_chunks + 1] */
     long long *d_aux = nullptr; size_t aux_cap = 0;               /* per chunk: last chosen end, new X, window offsets */
@@ -3390,18 +3397,26 @@ extern "C" int acb_last_leftmost_ms(float *ms, int32_t n) {
     return ACB_OK;
 }
 
-extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay,
-                                           int64_t max_hay_letters, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+static bool select_kind_ok(int kind) {
+    if (kind == ACB_SELECT_LONGEST || kind == ACB_SELECT_FIRST) return true;
+    acb_set_error("selection kind %d is neither ACB_SELECT_LONGEST nor ACB_SELECT_FIRST", kind);
+    return false;
+}
+
+/* acb_leftmost_longest_device / acb_leftmost_first_device: the kind picks the sort order of step 1 (the candidate of a
+ * (hay, start) run is its first record), nothing else */
+static int leftmost_select(acb_table *tb, int kind, const acb_match *d_records, int64_t n, int64_t n_hay, int64_t max_hay_letters,
+                           acb_match *d_out, int64_t cap, int64_t *d_count, cudaStream_t s) {
     if (!tb || n < 0 || (n && !d_records) || n_hay < 0 || max_hay_letters < 0 || cap < 0 || (cap > 0 && !d_out) || !d_count) {
         acb_set_error("bad argument");
         return ACB_EINVAL;
     }
+    if (!select_kind_ok(kind)) return ACB_EINVAL;
     if (n > 0x7fffffffLL) { acb_set_error("more than 2^31-1 records to select from"); return ACB_ERANGE; }
     for (float &v : g_ll_ms) v = 0.f;
     if (n == 0) return ACB_OK;
     CUDA_TRY(cudaSetDevice(tb->device));
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    const SortKey k = sort_key(tb, n_hay, max_hay_letters);
+    const SortKey k = sort_key(tb, n_hay, max_hay_letters, kind);
     const int ni = (int)n;
     const long long n_tiles = (n + kLlTile - 1) / kLlTile;
     size_t t_sort = 0, t_sel = 0, t_scan = 0;
@@ -3427,11 +3442,12 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     size_t tb_temp = temp;
     const unsigned grid = blocks(tb, n);
     if ((rc = timing_mark(&tb->l_ev[0], s))) return rc;
-    /* 1. sort by start */
-    if ((rc = sort_records<true>(tb, k, d_records, rb, ra, n, k0, k1, tmp, temp, s, "leftmost sort key")) ||
-        (rc = timing_mark(&tb->l_ev[1], s)))
-        return rc;
-    /* 2. candidates: the longest match at every (hay, start) */
+    /* 1. sort by start, then longest first or smallest key id first */
+    rc = kind == ACB_SELECT_FIRST
+             ? sort_records<kKeyFirst, kKeyFirstLow>(tb, k, d_records, rb, ra, n, k0, k1, tmp, temp, s, "leftmost sort key")
+             : sort_records<kKeyStart, kKeyStartLow>(tb, k, d_records, rb, ra, n, k0, k1, tmp, temp, s, "leftmost sort key");
+    if (rc || (rc = timing_mark(&tb->l_ev[1], s))) return rc;
+    /* 2. candidates: the longest (first) match at every (hay, start) */
     acb_ll_cand_kernel<<<grid, 256, 0, s>>>(ra, n, tb->d_keylen, flag);
     if ((rc = launched("leftmost candidates"))) return rc;
     tb_temp = temp;
@@ -3453,6 +3469,18 @@ extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_rec
     for (int k = 0; k < 5; k++)
         if ((rc = timing_ms(tb->l_ev[k], tb->l_ev[k + 1], &g_ll_ms[k]))) return rc;
     return ACB_OK;
+}
+
+extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay,
+                                           int64_t max_hay_letters, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+    return leftmost_select(tb, ACB_SELECT_LONGEST, d_records, n, n_hay, max_hay_letters, d_out, cap, d_count,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int acb_leftmost_first_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay,
+                                         int64_t max_hay_letters, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+    return leftmost_select(tb, ACB_SELECT_FIRST, d_records, n, n_hay, max_hay_letters, d_out, cap, d_count,
+                           reinterpret_cast<cudaStream_t>(stream));
 }
 
 /* ------------------------------------------------------------ whole-word filter */
@@ -3649,9 +3677,11 @@ extern "C" int acb_scan_host_words(acb_table *tb, const uint8_t *hay, int64_t to
 }
 
 static int scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
-                              int64_t stride_bytes, const WordSet *ws, acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+                              int64_t stride_bytes, const WordSet *ws, acb_match *out, int64_t cap, int64_t *n_found, int algo,
+                              int kind = ACB_SELECT_LONGEST) {
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
+    if (!select_kind_ok(kind)) return ACB_EINVAL;
     if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("leftmost-longest takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
     int rc;
@@ -3669,8 +3699,8 @@ static int scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_b
     if ((rc = ensure(&tb->l_out, &tb->l_out_cap, (size_t)std::max<int64_t>(kept_cap, 1)))) return rc;
     unsigned long long *d_n = tb->l_ctr + 2;
     CUDA_TRY(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s));
-    if ((rc = acb_leftmost_longest_device(tb, rec, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, tb->l_out,
-                                          kept_cap, reinterpret_cast<int64_t *>(d_n), s)))
+    if ((rc = leftmost_select(tb, kind, rec, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, tb->l_out, kept_cap,
+                              reinterpret_cast<int64_t *>(d_n), s)))
         return rc;
     return read_back(tb, d_n, tb->l_out, cap, 0, n_hay, 0, out, n_found, s);
 }
@@ -3685,6 +3715,14 @@ extern "C" int acb_scan_host_leftmost_words(acb_table *tb, const uint8_t *hay, i
                                             int64_t *n_found, int algo) {
     const WordSet ws{bits, n_bits};
     return scan_host_leftmost(tb, hay, total_bytes, offsets, n_hay, stride_bytes, &ws, out, cap, n_found, algo);
+}
+
+extern "C" int acb_scan_host_leftmost_kind(acb_table *tb, int kind, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
+                                           int64_t n_hay, int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out,
+                                           int64_t cap, int64_t *n_found, int algo) {
+    const WordSet ws{bits, n_bits};
+    const bool words = n_bits >= 0 || bits;                 /* n_bits < 0 without a bitmap: no word filter */
+    return scan_host_leftmost(tb, hay, total_bytes, offsets, n_hay, stride_bytes, words ? &ws : nullptr, out, cap, n_found, algo, kind);
 }
 
 /* ------------------------------------------------------------ leftmost-longest replacement */
@@ -3704,6 +3742,7 @@ struct acb_replacer {
     int device = 0;
     int32_t L = 1;
     int64_t n_ids = 0;
+    int kind = ACB_SELECT_LONGEST;                           /* the selection whose matches it rewrites */
     uint8_t *d_rep = nullptr;                                /* replacement bytes, 32 bytes of padding behind */
     long long *d_rep_off = nullptr;                          /* n_ids + 1 byte offsets */
 };
@@ -3862,10 +3901,11 @@ static int rp_fits(const acb_replacer *r, const acb_table *tb) {
     return ACB_OK;
 }
 
-extern "C" int acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets,
-                                int64_t n_ids, acb_replacer **out) {
+extern "C" int acb_replacer_new_kind(const acb_table *tb, int kind, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets,
+                                     int64_t n_ids, acb_replacer **out) {
     if (!tb || !out || rep_bytes < 0 || (rep_bytes && !rep) || !rep_offsets || n_ids < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
+    if (!select_kind_ok(kind)) return ACB_EINVAL;
     if (tb->L != 1 && tb->L != 2 && tb->L != 4) { acb_set_error("not a table"); return ACB_EINVAL; }
     if (n_ids < tb->n_keys) { acb_set_error("%lld replacements for %d key ids", (long long)n_ids, tb->n_keys); return ACB_EINVAL; }
     int rc = check_offsets(tb->L, rep_offsets, n_ids, rep_bytes);
@@ -3873,7 +3913,7 @@ extern "C" int acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t
     CUDA_TRY(cudaSetDevice(tb->device));
     acb_replacer *r = new (std::nothrow) acb_replacer();
     if (!r) { acb_set_error("out of memory"); return ACB_ENOMEM; }
-    r->device = tb->device; r->L = tb->L; r->n_ids = n_ids;
+    r->device = tb->device; r->L = tb->L; r->n_ids = n_ids; r->kind = kind;
     cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&r->d_rep), (size_t)rep_bytes + 32);
     if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&r->d_rep_off), (size_t)(n_ids + 1) * sizeof(long long));
     if (e == cudaSuccess && rep_bytes) e = cudaMemcpy(r->d_rep, rep, (size_t)rep_bytes, cudaMemcpyHostToDevice);
@@ -3885,6 +3925,11 @@ extern "C" int acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t
     }
     *out = r;
     return ACB_OK;
+}
+
+extern "C" int acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets,
+                                int64_t n_ids, acb_replacer **out) {
+    return acb_replacer_new_kind(tb, ACB_SELECT_LONGEST, rep, rep_bytes, rep_offsets, n_ids, out);
 }
 
 extern "C" void acb_replacer_free(acb_replacer *r) {
@@ -4019,8 +4064,8 @@ static int replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int6
     unsigned long long *d_n = tb->l_ctr + 2;
     CUDA_TRY(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), s));
     if (full && (rc = ensure(&tb->l_out, &tb->l_out_cap, (size_t)full))) return rc;
-    if (full && (rc = acb_leftmost_longest_device(tb, rec, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L,
-                                                  tb->l_out, (int64_t)full, reinterpret_cast<int64_t *>(d_n), s)))
+    if (full && (rc = leftmost_select(tb, r->kind, rec, (int64_t)full, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L,
+                                      tb->l_out, (int64_t)full, reinterpret_cast<int64_t *>(d_n), s)))
         return rc;
     RpArgs a;
     rp_args(a, r, tb, tb->w_hay, total_bytes, d_off, n_hay, stride_bytes, tb->l_out, (int64_t)full, reinterpret_cast<int64_t *>(d_n),
@@ -4360,6 +4405,17 @@ extern "C" int acb_streams_new_words(const acb_table *tb, int64_t n_streams, int
     return ACB_OK;
 }
 
+extern "C" int acb_streams_new_leftmost_kind(const acb_table *tb, int64_t n_streams, int kind, const uint32_t *bits, int64_t n_bits,
+                                             acb_streams **out) {
+    if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    if (!select_kind_ok(kind)) return ACB_EINVAL;
+    const bool words = n_bits >= 0 || bits;                 /* n_bits < 0 without a bitmap: no word filter */
+    int rc = words ? acb_streams_new_words(tb, n_streams, 1, bits, n_bits, out) : acb_streams_new_leftmost(tb, n_streams, out);
+    if (rc == ACB_OK) (*out)->kind = kind;
+    return rc;
+}
+
 extern "C" int acb_last_stream_leftmost_ms(float *ms, int32_t n) {
     if (!ms || n < 0 || n > 6) { acb_set_error("bad argument"); return ACB_EINVAL; }
     for (int i = 0; i < n; i++) ms[i] = g_sl_ms[i];
@@ -4383,6 +4439,13 @@ static int sl_check(const acb_streams *ss, const acb_table *tb, int64_t total, c
     if (*algo == ACB_ALGO_AUTO) *algo = ACB_ALGO_FILTER;
     if (*algo != ACB_ALGO_FILTER && *algo != ACB_ALGO_DFA) { acb_set_error("a leftmost-longest feed takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
     return ACB_OK;
+}
+
+/* a replacing feed rewrites what its batch selects: the replacer's kind must be the batch's */
+static int sl_kind_fits(const acb_streams *ss, const acb_replacer *r) {
+    if (r->kind == ss->kind) return ACB_OK;
+    acb_set_error("a replacer of selection kind %d on a stream batch of kind %d", r->kind, ss->kind);
+    return ACB_EINVAL;
 }
 
 /* d_soff[0..n] <- exclusive scan of d_soff[0..n] in place; the total to the host (the one wait of the staging) */
@@ -4441,7 +4504,7 @@ static int sw_order(acb_streams *ss, acb_table *tb, const SlArgs &a, unsigned lo
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, temp, k0, k1, ss->d_settled, ss->d_full, (int)m, 0, 64, s));
     if ((rc = ensure(&ss->d_tmp, &ss->tmp_cap, temp))) return rc;
     acb_match *sorted = k.bits() <= 64 ? ss->d_full : ss->d_settled;      /* two passes go through d_full */
-    if ((rc = sort_records<false>(tb, k, ss->d_settled, ss->d_full, sorted, (long long)m, k0, k1, ss->d_tmp, ss->tmp_cap, s,
+    if ((rc = sort_records<kKeyEnd, kKeyEndLow>(tb, k, ss->d_settled, ss->d_full, sorted, (long long)m, k0, k1, ss->d_tmp, ss->tmp_cap, s,
                                   "stream word sort key")))
         return rc;
     acb_sw_emit_kernel<<<blocks(tb, m), 256, 0, s>>>(a, sorted, (long long)m, d_out, cap, d_count);
@@ -4537,8 +4600,8 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
     if ((rc = timing_mark(&ss->ev[6], s))) return rc;
     if (!ss->leftmost) {                                   /* a find_all word feed returns every kept record, ordered */
         if ((rc = sw_order(ss, tb, a, m, staged, d_out, cap, ccount, s))) return rc;
-    } else if (m && (rc = acb_leftmost_longest_device(tb, ss->d_settled, (int64_t)m, n, max_letters, chosen, ccap,
-                                                      reinterpret_cast<int64_t *>(ccount), s))) {
+    } else if (m && (rc = leftmost_select(tb, ss->kind, ss->d_settled, (int64_t)m, n, max_letters, chosen, ccap,
+                                          reinterpret_cast<int64_t *>(ccount), s))) {
         return rc;
     }
     if ((rc = timing_mark(&ss->ev[7], s))) return rc;
@@ -4602,7 +4665,7 @@ extern "C" int acb_streams_replace_device(acb_streams *ss, acb_replacer *r, acb_
     int rc = sl_check(ss, tb, total_bytes, d_offsets, n_chunks, stride_bytes, &algo);
     if (rc) return rc;
     if (!r || !d_out_offsets || !d_total || out_cap < 0 || (out_cap && !d_out) || (total_bytes && !d_chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
-    if ((rc = rp_fits(r, tb))) return rc;
+    if ((rc = rp_fits(r, tb)) || (rc = sl_kind_fits(ss, r))) return rc;
     if (reinterpret_cast<uintptr_t>(d_out) & 15) { acb_set_error("d_out must be 16-byte aligned"); return ACB_EINVAL; }
     return sl_feed(ss, tb, r, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, nullptr, 0, nullptr,
                    d_out_offsets, d_out, out_cap, d_total, reinterpret_cast<cudaStream_t>(stream), algo);
@@ -4655,7 +4718,7 @@ extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_ta
     int rc = sl_check(ss, tb, total_bytes, offsets, n_chunks, stride_bytes, &algo);
     if (rc) return rc;
     if (!r || !out_offsets || !total || out_cap < 0 || (out_cap && !out) || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
-    if ((rc = rp_fits(r, tb))) return rc;
+    if ((rc = rp_fits(r, tb)) || (rc = sl_kind_fits(ss, r))) return rc;
     *total = 0;
     const int64_t *d_off = nullptr;
     if ((rc = sl_upload(ss, tb, chunks, total_bytes, offsets, n_chunks, ids, &d_off))) return rc;

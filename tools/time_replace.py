@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Time the leftmost-longest replacement stage by stage on device-resident batches.
 
-    python tools/time_replace.py [--reps 10] [--out DIR]
+    python tools/time_replace.py [--reps 10] [--out DIR] [--kinds longest,first]
 
 Workloads (pyahocorasick_b200.synth, C2's 10 k keys): C2 planted (1 M x 256 B), C4 (64 x 16 MiB), and C4's bytes as
 one haystack of 1 GiB; each with three replacement tables: random lengths 0..24 (seeded), the identity (every key
@@ -15,7 +15,9 @@ mapped to itself) and delete-everything.  For each, with the batch resident in H
   call_host_ms   a whole replace_batch from the host array (C2, C4) or (flat, offsets) pair (1 GiB)
 Medians of `reps` runs after 2 warm-up runs.  Every output is checked once, piece by piece, against a numpy build from
 find_leftmost_longest_batch's records.  The card's name, power limit and SM clocks are read in the same run.  Prints one
-JSON line (also written to DIR/replace.json)."""
+JSON line (also written to DIR/replace.json).  --kinds longest,first also times a leftmost-first replacer of the same
+table (Automaton.replacer(leftmost_first=True)), its whole calls alternating with the leftmost-longest ones: each table
+then has "first": {call_cuda_ms, call_host_ms} and "first_over_longest_cuda"."""
 from __future__ import annotations
 
 import argparse
@@ -83,6 +85,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--kinds", default="longest", choices=["longest", "longest,first"])
     a = ap.parse_args()
     import numpy as np
     import torch
@@ -158,16 +161,25 @@ def main():
             check(A, flat, in_off, rep, rep_off, out[:nb].cpu().numpy(), out_off.cpu().numpy())
             row["checked"] = True
             hostform = host if name != "1GiB" else (flat, np.array([0, flat.size], dtype=np.int64))
+            Rs = {"longest": R}
+            if a.kinds == "longest,first":
+                Rs["first"] = A.replacer(table, leftmost_first=True)
             for key_, batch in (("call_cuda_ms", d), ("call_host_ms", hostform)):
-                ts = []
+                ts = {k: [] for k in Rs}
                 for it in range(4):
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    R.replace_batch(batch)
-                    torch.cuda.synchronize()
-                    if it:
-                        ts.append((time.perf_counter() - t0) * 1e3)
-                row[key_] = med(ts)
+                    for k, RR in Rs.items():
+                        torch.cuda.synchronize()
+                        t0 = time.perf_counter()
+                        RR.replace_batch(batch)
+                        torch.cuda.synchronize()
+                        if it:
+                            ts[k].append((time.perf_counter() - t0) * 1e3)
+                row[key_] = med(ts["longest"])
+                if "first" in Rs:
+                    row.setdefault("first", {})[key_] = med(ts["first"])
+            if "first" in Rs:
+                row["first_over_longest_cuda"] = row["first"]["call_cuda_ms"] / row["call_cuda_ms"]
+                del Rs
             res[name][tname] = row
             del R
             out = None
