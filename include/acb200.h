@@ -629,6 +629,43 @@ int acb_streams_feed_words_host(acb_streams *ss, acb_table *tb, const uint8_t *c
                                 const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
                                 acb_match *out, int64_t cap, int64_t *n_found, int algo);
 
+/* ---- ASCII case-insensitive matching: scans of folded text -------------------------------------------------------
+ * A folded table matches keys and text with every ASCII capital made small: a letter whose VALUE is 0x41..0x5A (the
+ * whole letter value: a 4-byte letter U+0141 or U+1F641 is not one) reads as value + 0x20.  Nothing else folds (bytes
+ * 0x80..0xFF and non-ASCII code points stay as they are), so positions and lengths are those of the text.  The trie
+ * holds the folded keys, each under its group's representative: the lowest id among the keys that fold to the same
+ * text.  The alias lists name the group's other ids: alias_ids[alias_ptr[k] .. alias_ptr[k+1]) for representative k,
+ * ascending and above k; alias_ptr has n_keys + 1 entries (n_keys of the trie's flat view), from 0 to n_alias.  Both
+ * may be NULL with n_alias == 0, the key set without case variants.  ACB_EINVAL for lists that break these rules or for
+ * a trie of 2-byte letters.  An alias id has its representative's length; the table's key ids cover the aliases.
+ *
+ * On a folded table, acb_scan_device and every host route that scans (acb_scan_host, acb_scan_host_words, the leftmost
+ * and replacement routes, plain and whole-word) fold the text before the scan: acb_scan_device into a scratch copy it
+ * owns (guarded as the other scratch buffers are: the next call waits for this one's work), the pipelined acb_scan_host
+ * each 32 MiB chunk in place on the device.  The word tests and the rewrites read the caller's text as it is.  Records
+ * carry representative ids.  acb_scan_host and acb_scan_host_words on a table with aliases expand them before the sort
+ * (acb_expand_aliases_device; such a table is not pipelined); the leftmost and replacement routes do not: the
+ * representative is the leftmost-first winner and the leftmost-longest one among keys of one text.  Refused (ACB_EINVAL):
+ * ACB_ALGO_LONG, the white-space scans (*_skip), stream batches (acb_streams_new* and every feed), lookups and key
+ * selections (acb_lookup_*, acb_select_*, acb_table_upload_key_ranges).  A table from acb_table_upload behaves as
+ * before. */
+int acb_table_upload_folded(const acb_trie *t, int device, const int32_t *alias_ptr, const int32_t *alias_ids, int64_t n_alias,
+                            acb_table **out);
+
+/* DEVICE buffers, asynchronous on `stream`; a folded table only (ACB_EINVAL).  Each of the n records of d_in becomes its
+ * own record followed by one per alias of its key id, ascending (key ids without aliases, or outside the lists, stay
+ * one record), at d_out in d_in's order; *d_count is SET to their total and only records below index cap are stored.
+ * d_in and d_out must not overlap.  A sort of the result by acb_sort_matches_device keeps the members of a group in
+ * ascending id (the radix sort is stable).  The scratch space belongs to the table, as for acb_word_filter_device.
+ * ACB_ERANGE for more than 2^31-1 records. */
+int acb_expand_aliases_device(acb_table *tb, const acb_match *d_in, int64_t n, acb_match *d_out, int64_t cap, int64_t *d_count,
+                              void *stream);
+
+/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last fold of acb_scan_device (the pipelined
+ * acb_scan_host's folds are not timed) and of the last alias expansion on this thread (the first n of them, n <= 2), from
+ * CUDA events (the call then waits for them); 0 when timing is off. */
+int acb_last_fold_ms(float *ms, int32_t n);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

@@ -96,6 +96,22 @@ def _space_mask(letters: np.ndarray, bytes_flavour: bool) -> np.ndarray:
 
 
 _WORD_LETTERS_BYTES = b"0123456789ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz_"
+_ASCII_LOWER = {c: c + 0x20 for c in range(0x41, 0x5B)}
+
+
+def _ascii_fold(key):
+    """A key with its 26 ASCII capitals made small and nothing else (bytes.lower() touches ASCII only; str.lower() would
+    fold every letter, so str keys are translated)."""
+    return key.lower() if isinstance(key, bytes) else key.translate(_ASCII_LOWER)
+
+
+class _FoldCore(NamedTuple):
+    """The folded automaton of one letter width (Automaton._fold_host): its host trie, which holds each folded key under
+    its group's representative (the lowest id of the keys that fold to it), and the alias lists of acb_table_upload_folded
+    -- alias_ids[alias_ptr[k]:alias_ptr[k + 1]] are the other ids of representative k's group, ascending."""
+    trie: Any
+    alias_ptr: np.ndarray
+    alias_ids: np.ndarray
 
 
 @functools.lru_cache(maxsize=None)
@@ -215,6 +231,8 @@ class Automaton:
         self._table = None
         self._narrow_trie = None
         self._narrow_table = None
+        self._fold_cores = {}
+        self._fold_tables = {}
         self._configure(store, key_type)
         if len(args) == 7:                # what __reduce__ of the reference produces, src/Automaton.c:106-147
             from . import serialize
@@ -244,6 +262,10 @@ class Automaton:
         self._narrow_table = None
         self._narrow_device = None
         self._narrow_empty = False
+        # ascii_case_insensitive: per letter width (narrow or not) the folded automaton (_FoldCore, or None without a key)
+        # and its table as (acb_table*, device), built lazily
+        self._fold_cores: dict = {}
+        self._fold_tables: dict = {}
         self._match_cap = 0
 
     @staticmethod
@@ -626,6 +648,13 @@ class Automaton:
             self._lib.acb_trie_free(self._narrow_trie)
             self._narrow_trie = None
         self._narrow_empty = False
+        for tb, _ in self._fold_tables.values():
+            self._lib.acb_table_free(tb)
+        self._fold_tables = {}
+        for core in self._fold_cores.values():
+            if core is not None:
+                self._lib.acb_trie_free(core.trie)
+        self._fold_cores = {}
 
     def _uses_narrow(self) -> bool:
         return self._UNICODE and self._key_type == KEY_STRING
@@ -688,13 +717,95 @@ class Automaton:
         self._table_device = device
         return tb
 
-    def _table_for(self, device: Optional[int], narrow: bool):
-        """The table a batch runs on: the latin-1 one for a narrow batch, else the full one.  None when the batch is narrow
-        and no key is latin-1: then nothing matches."""
+    @_locked
+    def _fold_host(self, narrow: bool) -> Optional[_FoldCore]:
+        """The folded automaton of a batch's letter width (narrow: the latin-1 keys at 1 byte per letter), built lazily;
+        None when it has no key.  Keys are added in ascending id, and a key whose folded text is already there is not
+        added but listed as an alias of the id that holds it, so that id is the lowest of its group."""
+        if narrow in self._fold_cores:
+            return self._fold_cores[narrow]
+        t = self._lib.acb_trie_new(1 if narrow else self._L)
+        if not t:
+            raise MemoryError(N.last_error())
+        reps: dict = {}
+        aliases: dict = {}
+        for kid, key in enumerate(self._key_objs):
+            if key is None:
+                continue
+            folded = _ascii_fold(key)
+            if narrow:
+                try:
+                    raw = folded.encode("latin-1")
+                except UnicodeEncodeError:
+                    continue                                    # cannot occur in a latin-1 haystack
+            else:
+                raw, _ = self._raw_key(folded)
+            rep = reps.setdefault(raw, kid)
+            if rep != kid:
+                aliases.setdefault(rep, []).append(kid)
+                continue
+            N.check(self._lib.acb_trie_add_word(t, raw, len(raw), kid, None))
+        if not reps:
+            self._lib.acb_trie_free(t)
+            self._fold_cores[narrow] = None
+            return None
+        built = ctypes.c_int32(0)
+        N.check(self._lib.acb_trie_make_automaton(t, ctypes.byref(built)))
+        alias_ptr = np.zeros(max(reps.values()) + 2, dtype=np.int32)
+        for rep, ids in aliases.items():
+            alias_ptr[rep + 1] = len(ids)
+        np.cumsum(alias_ptr, out=alias_ptr)
+        alias_ids = np.array([k for rep in sorted(aliases) for k in aliases[rep]], dtype=np.int32)
+        core = self._fold_cores[narrow] = _FoldCore(t, alias_ptr, alias_ids)
+        return core
+
+    @_locked
+    def _ensure_folded(self, device: Optional[int], narrow: bool):
+        """The folded table (acb_table_upload_folded) of a batch's letter width on `device`; None when it has no key."""
+        core = self._fold_host(narrow)
+        if core is None:
+            return None
+        if device is None:
+            device = _default_device()
+        have = self._fold_tables.get(narrow)
+        if have is not None and have[1] == device:
+            return have[0]
+        if have is not None:
+            self._lib.acb_table_free(have[0])
+            del self._fold_tables[narrow]
+        tb = ctypes.c_void_p()
+        n = len(core.alias_ids)
+        N.check(self._lib.acb_table_upload_folded(core.trie, device, N.ptr(core.alias_ptr) if n else None,
+                                                  N.ptr(core.alias_ids) if n else None, n, ctypes.byref(tb)))
+        self._fold_tables[narrow] = (tb, device)
+        return tb
+
+    def _table_for(self, device: Optional[int], narrow: bool, fold: bool = False):
+        """The table a batch runs on: the latin-1 one for a narrow batch, else the full one; with fold, the folded table of
+        that width.  None when the batch is narrow and no key is latin-1: then nothing matches."""
+        if fold:
+            return self._ensure_folded(device, narrow)
         if not narrow:
             return self._ensure_table(device)
         core = self._ensure_narrow(device)
         return None if core is None else core[1]
+
+    def _has_aliases(self, narrow: bool) -> bool:
+        """the folded key set of this width has case variants (an alias expansion follows the find_all scans)"""
+        core = self._fold_host(narrow)
+        return core is not None and len(core.alias_ids) > 0
+
+    def _fold_arg(self, ascii_case_insensitive, algo: str = "auto", ignore_white_space: bool = False) -> bool:
+        """The ascii_case_insensitive argument of the batch methods, checked against the others"""
+        if not ascii_case_insensitive:
+            return False
+        if self._key_type == KEY_SEQUENCE:
+            raise ValueError("ascii_case_insensitive needs text: KEY_SEQUENCE letters are integers, not letters")
+        if ignore_white_space:
+            raise ValueError("ascii_case_insensitive cannot be combined with ignore_white_space")
+        if algo == "long":
+            raise ValueError("ascii_case_insensitive cannot be combined with algo='long'")
+        return True
 
     @_locked
     def filter_shape(self) -> dict:
@@ -740,9 +851,10 @@ class Automaton:
     @_locked
     def _scan_flat(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int,
                    algo: str = "auto", sort: bool = True, device: Optional[int] = None, narrow: bool = False,
-                   long_state: Optional[int] = None) -> np.ndarray:
+                   long_state: Optional[int] = None, fold: bool = False) -> np.ndarray:
         """flat uint8 buffer (+ int64 byte offsets or a fixed stride) -> sorted match records.
-        narrow=True: the buffer holds 1-byte letters of a unicode-flavour automaton (latin-1 path).
+        narrow=True: the buffer holds 1-byte letters of a unicode-flavour automaton (latin-1 path).  fold: on the folded
+        table, which folds the text and expands the aliases itself.
         long_state (algo "long", one haystack): the state the walk starts in; the state it ends in is left in
         self._long_state_out (iter_long streaming, acb_table_set_long_state / acb_table_get_long_state)."""
         lib, total = self._lib, int(flat.size)
@@ -757,18 +869,18 @@ class Automaton:
                 N.check(lib.acb_table_get_long_state(tb, ctypes.byref(st)))
                 self._long_state_out = int(st.value)
             return rc
-        return self._host_records(device, narrow, n_hay, scan)
+        return self._host_records(device, narrow, n_hay, scan, fold)
 
     def _record_room(self, n_hay: int) -> int:
         """The first guess of the records a batch of n_hay haystacks gives; _match_cap remembers the largest overflow."""
         return max(self._match_cap, 1 << 12, 2 * n_hay)
 
-    def _host_records(self, device: Optional[int], narrow: bool, n_hay: int, call) -> np.ndarray:
+    def _host_records(self, device: Optional[int], narrow: bool, n_hay: int, call, fold: bool = False) -> np.ndarray:
         """The records of one host-buffer call, which leaves them in its table's pinned buffer.  call(tb, cap, found_ref)
         makes the native call with room for cap records and returns its status.  On ACB_EOVERFLOW it runs once more with
         room for the exact count (+1024, kept in _match_cap); a second overflow raises.  The records are handed over
-        without a copy (_take_records)."""
-        tb = self._table_for(device, narrow)
+        without a copy (_take_records).  fold: on the folded table (_table_for)."""
+        tb = self._table_for(device, narrow, fold)
         if tb is None:
             return np.empty(0, dtype=N.MATCH_DTYPE)
         found = ctypes.c_int64(0)
@@ -819,7 +931,8 @@ class Automaton:
 
     @_locked
     def _words_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str, sort: bool,
-                    device: Optional[int], narrow: bool, words: tuple, leftmost: bool, select: int = N.SELECT_LONGEST) -> np.ndarray:
+                    device: Optional[int], narrow: bool, words: tuple, leftmost: bool, select: int = N.SELECT_LONGEST,
+                    fold: bool = False) -> np.ndarray:
         """acb_scan_host_words / acb_scan_host_leftmost_words (acb_scan_host_leftmost_kind for leftmost-first): upload,
         scan, keep the whole-word matches, then sort or select, copy back (_host_records)."""
         lib = self._lib
@@ -833,7 +946,7 @@ class Automaton:
             if leftmost:
                 return lib.acb_scan_host_leftmost_words(tb, *args, cap, found_ref, N.ALGOS[algo])
             return lib.acb_scan_host_words(tb, *args, cap, found_ref, N.ALGOS[algo], int(sort))
-        return self._host_records(device, narrow, n_hay, scan)
+        return self._host_records(device, narrow, n_hay, scan, fold)
 
     def _filter_words_device(self, tb, t, n: int, stride: int, full, m: int, words: tuple, stream):
         """The whole-word records among the first m of the device buffer `full` (a scan of the aligned device batch t),
@@ -849,18 +962,28 @@ class Automaton:
 
     @_locked
     def _scan_device_tensor(self, batch, algo: str, sort: bool, words: Optional[tuple] = None,
-                            white_space: bool = False) -> np.ndarray:
+                            white_space: bool = False, fold: bool = False) -> np.ndarray:
         """Batch already resident in HBM: a C-contiguous uint8 torch CUDA tensor [n, stride].  No host copy of
         the haystacks; the scan runs on torch's current stream, only the records come back.  words: keep the
         whole-word matches (_filter_words_device) before the sort.  white_space: the scan skips the white space
-        (acb_scan_device_skip)."""
+        (acb_scan_device_skip).  fold: on the folded table, with the aliases expanded after the word filter; the stable
+        sort keeps each group's records in ascending id."""
         t = _aligned(batch.data)
         dev = _device_of(t)
-        tb = self._ensure_table(dev)
+        tb = self._table_for(dev, False, fold)
         skip = self._skip_set(False) if white_space else None
         with _on_device(dev) as stream:
             out, found = self._device_matches(tb, t, batch.n, batch.stride, algo, stream, words, skip)
+            if fold and found and self._has_aliases(False):
+                out, found = self._expand_device(tb, t, batch.n, out, found, stream)
             return self._device_records(tb, out, found, batch.n, batch.stride // self._L, stream, sort)
+
+    def _expand_device(self, tb, t, n: int, full, m: int, stream):
+        """The first m records of the device buffer `full` with every alias of their key added (acb_expand_aliases_device),
+        left on the device (_device_scan)."""
+        def expand(out, cap, cnt):
+            N.check(self._lib.acb_expand_aliases_device(tb, full.data_ptr(), m, out.data_ptr(), cap, cnt.data_ptr(), stream))
+        return self._device_scan(t, n, expand)
 
     def _device_matches(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None,
                         skip: Optional[np.ndarray] = None):
@@ -999,13 +1122,16 @@ class Automaton:
         start, end = _parse_start_end(args, 1, 2, 0, len(letters))
         return AutomatonSearchIterLong(self, letters, start, end)
 
-    def find_long_batch(self, haystacks, *, sort: bool = True, device: Optional[int] = None, whole_words=False) -> "Matches":
-        """iter_long() over a whole batch (same input forms and result type as find_all_batch).  whole_words is refused
-        (ValueError): iter_long's walk picks its matches itself, so a filter after it has no clear meaning."""
-        return self.find_all_batch(haystacks, algo="long", sort=sort, device=device, whole_words=whole_words)
+    def find_long_batch(self, haystacks, *, sort: bool = True, device: Optional[int] = None, whole_words=False,
+                        ascii_case_insensitive: bool = False) -> "Matches":
+        """iter_long() over a whole batch (same input forms and result type as find_all_batch).  whole_words and
+        ascii_case_insensitive are refused (ValueError): iter_long's walk picks its matches itself, so a filter after it
+        has no clear meaning, and its walk follows the automaton of the keys as given."""
+        return self.find_all_batch(haystacks, algo="long", sort=sort, device=device, whole_words=whole_words,
+                                   ascii_case_insensitive=ascii_case_insensitive)
 
     def find_leftmost_longest_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
-                                    whole_words=False) -> "Matches":
+                                    whole_words=False, ascii_case_insensitive: bool = False) -> "Matches":
         """Leftmost-longest non-overlapping matches of a whole batch, selected on the GPU (input forms and result type
         of find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or
         after p, take the smallest such start, the longest match there, and continue after its end.  Records come in
@@ -1015,24 +1141,32 @@ class Automaton:
 
         whole_words (see find_all_batch): the same rule over the whole-word matches only, so a longer match inside a
         word does not hide a shorter whole word: keys ``new`` and ``new york`` on ``new yorker`` give ``new``.  A CUDA
-        tensor batch then waits once more, for the number of whole-word matches."""
+        tensor batch then waits once more, for the number of whole-word matches.
+
+        ascii_case_insensitive (see find_all_batch): the same rule over the folded text.  Of the keys that fold to the
+        same text, only the one added first is reported."""
         self._require_automaton()
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-longest takes 'auto', 'filter' or 'dfa'")
         words = self._words(whole_words)
+        fold = self._fold_arg(ascii_case_insensitive)
         b = self._batch_input(haystacks)
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
         elif b.kind == "device":
-            rec = self._leftmost_device(b, algo, words)
+            rec = self._leftmost_device(b, algo, words, fold=fold)
+        elif words is not None and fold:
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, fold=True)
         elif words is not None:
             rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True)
+        elif fold:
+            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, fold=True)
         else:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow)
         return Matches(rec, self._values)
 
     def find_leftmost_first_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
-                                  whole_words=False) -> "Matches":
+                                  whole_words=False, ascii_case_insensitive: bool = False) -> "Matches":
         """Leftmost-first non-overlapping matches of a whole batch, selected on the GPU (input forms and result type of
         find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or after
         p, take the smallest such start, the match there whose key was added first, and continue after its end.  This is
@@ -1040,27 +1174,34 @@ class Automaton:
         at a start, but a match further left always wins.  Priority is the order in which add_word first added each key:
         add_word of a key already present keeps its place, removing a key and adding it again moves it to the end.  An
         automaton read back from pickle or save numbers its keys afresh, so its priority can differ.  Records come in
-        haystack order, then end_index ascending; algo and whole_words as for find_leftmost_longest_batch."""
+        haystack order, then end_index ascending; algo, whole_words and ascii_case_insensitive as for
+        find_leftmost_longest_batch (the key added first wins among keys of one folded text, as at any start)."""
         self._require_automaton()
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-first takes 'auto', 'filter' or 'dfa'")
         words = self._words(whole_words)
+        fold = self._fold_arg(ascii_case_insensitive)
         b = self._batch_input(haystacks)
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
         elif b.kind == "device":
-            rec = self._leftmost_device(b, algo, words, N.SELECT_FIRST)
+            rec = self._leftmost_device(b, algo, words, N.SELECT_FIRST, fold)
+        elif words is not None and fold:
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, select=N.SELECT_FIRST,
+                                   fold=True)
         elif words is not None:
             rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, select=N.SELECT_FIRST)
+        elif fold:
+            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST, fold=True)
         else:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST)
         return Matches(rec, self._values)
 
     @_locked
     def _leftmost_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str,
-                       device: Optional[int], narrow: bool, select: int = N.SELECT_LONGEST) -> np.ndarray:
+                       device: Optional[int], narrow: bool, select: int = N.SELECT_LONGEST, fold: bool = False) -> np.ndarray:
         """acb_scan_host_leftmost (acb_scan_host_leftmost_kind for leftmost-first): upload, scan, select, copy back
-        (_host_records)."""
+        (_host_records).  fold: on the folded table, whose representatives are the winners; no alias expansion."""
         lib = self._lib
         args = (N.ptr(flat), int(flat.size), N.ptr(offsets) if offsets is not None else None, n_hay, stride_bytes)
 
@@ -1068,15 +1209,16 @@ class Automaton:
             if select != N.SELECT_LONGEST:
                 return lib.acb_scan_host_leftmost_kind(tb, select, *args, None, -1, None, cap, found_ref, N.ALGOS[algo])
             return lib.acb_scan_host_leftmost(tb, *args, None, cap, found_ref, N.ALGOS[algo])
-        return self._host_records(device, narrow, n_hay, scan)
+        return self._host_records(device, narrow, n_hay, scan, fold)
 
     @_locked
-    def _leftmost_device(self, batch, algo: str, words: Optional[tuple] = None, select: int = N.SELECT_LONGEST) -> np.ndarray:
+    def _leftmost_device(self, batch, algo: str, words: Optional[tuple] = None, select: int = N.SELECT_LONGEST,
+                         fold: bool = False) -> np.ndarray:
         """A CUDA tensor batch: the full scan into a device buffer, then the selection, both on torch's current stream;
-        only the chosen records come back."""
+        only the chosen records come back.  fold: on the folded table."""
         t = _aligned(batch.data)
         dev = _device_of(t)
-        tb = self._ensure_table(dev)
+        tb = self._table_for(dev, False, fold)
         with _on_device(dev) as stream:
             out, cnt, _ = self._leftmost_chosen(tb, t, batch.n, batch.stride, algo, stream, words, select)
             found = int(cnt.item())
@@ -1124,7 +1266,7 @@ class Automaton:
 
     # ------------------------------------------------------------------ the batch entry (new)
     def find_all_batch(self, haystacks, *, algo: str = "auto", sort: bool = True, device: Optional[int] = None,
-                       ignore_white_space: bool = False, whole_words=False) -> Matches:
+                       ignore_white_space: bool = False, whole_words=False, ascii_case_insensitive: bool = False) -> Matches:
         """Search a whole batch on the GPU.
 
         haystacks: a sequence of bytes / str / tuple objects (as `iter` accepts), or a 2-D
@@ -1145,6 +1287,13 @@ class Automaton:
         flavour.  bytes (bytes flavour) or str (unicode flavour): exactly these word letters; empty: none, every match
         is kept.  The matches are filtered on the GPU after the scan; a CUDA tensor batch then waits once more, for
         their number.  ValueError with ignore_white_space, algo="long" or a KEY_SEQUENCE automaton.
+
+        ascii_case_insensitive: the 26 ASCII letters match either case and nothing else folds -- a byte 0x41-0x5A equals
+        itself + 0x20 (bytes flavour), a code point 0x41-0x5A equals itself + 0x20 (unicode flavour; É and é, or Ł and
+        š, stay distinct).  Every key whose folded text occurs is reported, so keys ``abc`` and ``ABC`` both match in
+        ``xAbCx``; keys of one length at one end (case variants of each other) come in ascending key id.  end_index and
+        the whole-word test are those of the text as given.  The text is folded on the GPU; the caller's copy is not
+        changed.  ValueError with ignore_white_space, algo="long" or a KEY_SEQUENCE automaton.
         """
         self._require_automaton()
         if ignore_white_space and algo == "long":
@@ -1154,15 +1303,20 @@ class Automaton:
             raise ValueError("whole_words cannot be combined with ignore_white_space")
         if words is not None and algo == "long":
             raise ValueError("whole_words cannot be combined with algo='long': iter_long's walk picks its matches itself")
+        fold = self._fold_arg(ascii_case_insensitive, algo, ignore_white_space)
         b = self._batch_input(haystacks, narrow_ok=algo != "long")
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
         elif b.kind == "device":
-            rec = self._scan_device_tensor(b, algo, sort, words, ignore_white_space)
+            rec = self._scan_device_tensor(b, algo, sort, words, ignore_white_space, fold)
+        elif words is not None and fold:
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, sort, device, b.narrow, words, False, fold=True)
         elif words is not None:
             rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, sort, device, b.narrow, words, False)
         elif ignore_white_space:
             rec = self._scan_skip(b, algo, sort, device)
+        elif fold:
+            rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow, fold=True)
         else:
             rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow)
         return Matches(rec, self._values)
@@ -1742,13 +1896,16 @@ class Replacer:
             self._native[(narrow, device)] = r
         return r
 
-    def replace_batch(self, haystacks, *, algo: str = "auto", whole_words=False):
+    def replace_batch(self, haystacks, *, algo: str = "auto", whole_words=False, ascii_case_insensitive: bool = False):
         """The batch with every leftmost-longest match replaced.  `haystacks` takes the input forms of find_all_batch;
         a list gives a list of the same item type, uint8[n, stride] or (flat, offsets) gives (flat uint8, offsets
         int64[n+1]), a CUDA tensor gives that pair as CUDA tensors computed on torch's current stream (the call
         synchronises once to size the output).  algo ("auto", "filter", "dfa") only picks the scan.  whole_words (see
         find_all_batch): replace the matches that find_leftmost_longest_batch chooses with the same option, so a key
-        inside a longer word is left alone; a CUDA tensor batch then synchronises once more."""
+        inside a longer word is left alone; a CUDA tensor batch then synchronises once more.  ascii_case_insensitive
+        (see find_all_batch): replace the matches the find_leftmost_*_batch method of this replacer's rule chooses with
+        the same option, each by the replacement of its key -- the one added first among keys that fold to the same
+        text; every other letter is copied as given, in its own case."""
         A = self._A
         with A._gpu_lock:
             if self._version != A._version:
@@ -1757,10 +1914,11 @@ class Replacer:
             if algo not in ("auto", "filter", "dfa"):
                 raise ValueError(f"algo {algo!r}: replace_batch takes 'auto', 'filter' or 'dfa'")
             words = A._words(whole_words)
+            fold = A._fold_arg(ascii_case_insensitive)
             pair = isinstance(haystacks, np.ndarray) or _is_pair(haystacks)
             batch = A._batch_input(haystacks)
             if batch.kind == "device":
-                return self._run_device(batch, algo, words)
+                return self._run_device(batch, algo, words, fold)
             _, flat, offs, n, stride, narrow = batch
             if narrow and True not in self._tables:         # a replacement outside latin-1: 4 bytes per letter
                 flat = flat.astype("<u4").view(np.uint8)
@@ -1770,6 +1928,8 @@ class Replacer:
                 offs = np.arange(n + 1, dtype=np.int64) * stride
             if batch.empty:
                 out, out_offs = flat[:0].copy(), np.zeros(n + 1, dtype=np.int64)
+            elif fold:
+                out, out_offs = self._run_host(flat, offs, n, narrow, algo, words, fold=True)
             elif words is None:
                 out, out_offs = self._run_host(flat, offs, n, narrow, algo)
             else:
@@ -1812,11 +1972,12 @@ class Replacer:
         s = raw.decode("utf-32-le", "surrogatepass")
         return [s[b[i] // 4:b[i + 1] // 4] for i in range(len(b) - 1)]
 
-    def _run_host(self, flat: np.ndarray, offs: np.ndarray, n: int, narrow: bool, algo: str, words: Optional[tuple] = None):
+    def _run_host(self, flat: np.ndarray, offs: np.ndarray, n: int, narrow: bool, algo: str, words: Optional[tuple] = None,
+                  fold: bool = False):
         """acb_replace_host (acb_replace_host_words with a word set) -> (output bytes, output offsets int64[n+1]); a
-        second call when the first guess of the output size was too small (_host_bytes)"""
+        second call when the first guess of the output size was too small (_host_bytes).  fold: on the folded table."""
         A = self._A
-        tb = A._table_for(self._device, narrow)
+        tb = A._table_for(self._device, narrow, fold)
         if tb is None:                                      # no latin-1 key: nothing matches
             return flat.copy(), offs.copy()
         r = self._replacer(tb, narrow, self._device)
@@ -1832,7 +1993,7 @@ class Replacer:
             return A._lib.acb_replace_host_words(*batch, N.ptr(bits) if n_bits else None, n_bits, *result)
         return _host_bytes(int(flat.size) * 5 // 4 + 4096, replace), out_offs
 
-    def _run_device(self, batch, algo: str, words: Optional[tuple] = None):
+    def _run_device(self, batch, algo: str, words: Optional[tuple] = None, fold: bool = False):
         """A CUDA tensor batch: scan, select and rewrite on torch's current stream; (flat, offsets) CUDA tensors"""
         import torch
         A = self._A
@@ -1841,7 +2002,7 @@ class Replacer:
             return torch.empty(0, dtype=torch.uint8, device=t.device), torch.zeros(n + 1, dtype=torch.int64, device=t.device)
         t = _aligned(t)
         dev = _device_of(t)
-        tb = A._ensure_table(dev)
+        tb = A._table_for(dev, False, fold)
         with _on_device(dev) as stream:
             chosen, cnt, cap = A._leftmost_chosen(tb, t, n, stride, algo, stream, words, self._select)
             r = self._replacer(tb, False, dev)

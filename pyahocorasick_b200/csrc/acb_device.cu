@@ -1399,6 +1399,15 @@ struct acb_table {
     acb_match *ww_out = nullptr; size_t ww_out_cap = 0;  /* the host routes: the whole-word records */
     cudaEvent_t ww_ev[2] = {};                           /* kernel timing of the filter */
     int cta_limit = 0;                       /* acb_table_set_cta_limit: 0, or the SMs the launches act as if the device had */
+    /* ASCII case folding (acb_table_upload_folded): every scan reads a folded copy of the text */
+    int fold = 0;
+    int32_t n_rep = 0;                                   /* ids the alias CSR covers: the trie's n_keys */
+    int64_t n_alias = 0;                                 /* alias ids; 0: no key set member has a case variant */
+    int32_t *d_alias_ptr = nullptr, *d_alias_ids = nullptr;   /* per representative id, its other ids, ascending */
+    Scratch f_buf;                                       /* acb_scan_device: the folded copy of the batch */
+    Scratch x_buf;                                       /* the alias expansion: per-record positions, cub scratch */
+    acb_match *x_out = nullptr; size_t x_out_cap = 0;    /* the host routes: the expanded records */
+    cudaEvent_t f_ev[4] = {};                            /* kernel timing of the fold and of the expansion */
 };
 
 extern "C" int acb_device_count(int32_t *n) {
@@ -1451,6 +1460,8 @@ extern "C" void acb_table_free(acb_table *tb) {
     if (tb->k_done) cudaEventDestroy(tb->k_done);
     if (tb->k_t0) cudaEventDestroy(tb->k_t0);
     if (tb->k_t1) cudaEventDestroy(tb->k_t1);
+    cudaFree(tb->d_alias_ptr); cudaFree(tb->d_alias_ids); tb->f_buf.release(); tb->x_buf.release(); cudaFree(tb->x_out);
+    for (cudaEvent_t e : tb->f_ev) if (e) cudaEventDestroy(e);
     delete tb;
 }
 
@@ -1596,6 +1607,13 @@ static int check_stride(int32_t L, int64_t total, int64_t n, int64_t stride, int
     return ACB_EINVAL;
 }
 
+/* a table uploaded by acb_table_upload_folded: refused by the entries that do not fold their text */
+static int refuse_folded(const acb_table *tb, const char *what) {
+    if (!tb || !tb->fold) return ACB_OK;
+    acb_set_error("%s does not take a case-folded table", what);
+    return ACB_EINVAL;
+}
+
 /* ------------------------------------------------------------- launching */
 
 constexpr int kMaxDevices = 64;                              /* opt-in caches below are per device */
@@ -1711,6 +1729,130 @@ static void fill_params(const acb_table *tb, ScanParams &p, const uint8_t *d_hay
     p.letter_shift = tb->L == 4 ? 2 : (tb->L == 2 ? 1 : 0);
 }
 
+/* ------------------------------------------------------------- ASCII case folding */
+/* A folded table's scans read the text with every ASCII capital (letter value 0x41..0x5A) made small (+0x20); nothing
+ * else changes, so positions and lengths are those of the text.  1-byte letters: four per 32-bit word, tested together
+ * (SWAR); 4-byte letters: the whole letter value is compared, so U+0141 or U+1F641 never fold. */
+namespace {
+thread_local float g_fold_ms[2] = {};                      /* kernel timing: fold, alias expansion */
+
+/* the bytes of x with 0x41..0x5A made small: h + 0x3f carries into bit 7 iff h >= 0x41, h + 0x25 iff h >= 0x5b (h <= 0x7f,
+ * so no byte carries into the next); a byte with bit 7 set is never a capital */
+__device__ __forceinline__ uint32_t fold_bytes(uint32_t x) {
+    const uint32_t h = x & 0x7f7f7f7fu;
+    const uint32_t upper = (h + 0x3f3f3f3fu) & ~(h + 0x25252525u) & ~x & 0x80808080u;
+    return x | upper >> 2;
+}
+
+template <int L>
+__device__ __forceinline__ uint32_t fold_word(uint32_t v) {
+    return L == 1 ? fold_bytes(v) : (v - 0x41u < 26u ? v + 0x20u : v);
+}
+
+template <int L>
+__device__ __forceinline__ uint4 fold_block(uint4 v) {
+    return make_uint4(fold_word<L>(v.x), fold_word<L>(v.y), fold_word<L>(v.z), fold_word<L>(v.w));
+}
+
+/* out = the n16 16-byte blocks of in folded, then `tail` (< 16, a multiple of L) more bytes; in == out is allowed.  Each
+ * thread keeps four blocks in flight per turn of the grid-stride loop. */
+template <int L>
+__global__ void __launch_bounds__(256) acb_fold_kernel(const uint4 *in, uint4 *out, long long n16, int tail) {
+    const long long step = (long long)gridDim.x * blockDim.x;
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (; i + 3 * step < n16; i += 4 * step) {
+        uint4 v[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) v[k] = in[i + k * step];
+#pragma unroll
+        for (int k = 0; k < 4; k++) out[i + k * step] = fold_block<L>(v[k]);
+    }
+    for (; i < n16; i += step) out[i] = fold_block<L>(in[i]);
+    if (blockIdx.x == 0 && (int)threadIdx.x * L < tail) {
+        if (L == 1) {
+            const uint8_t b = reinterpret_cast<const uint8_t *>(in + n16)[threadIdx.x];
+            reinterpret_cast<uint8_t *>(out + n16)[threadIdx.x] = (uint8_t)(b - 0x41u < 26u ? b + 0x20u : b);
+        } else {
+            reinterpret_cast<uint32_t *>(out + n16)[threadIdx.x] = fold_word<L>(reinterpret_cast<const uint32_t *>(in + n16)[threadIdx.x]);
+        }
+    }
+}
+} // namespace
+
+/* the fold of `bytes` bytes at in (16-byte aligned) to out (16-byte aligned, may be in), on s: one launch */
+static int fold_text(const acb_table *tb, const uint8_t *in, uint8_t *out, long long bytes, cudaStream_t s) {
+    const long long n16 = bytes / 16;
+    const int tail = (int)(bytes % 16);
+    const unsigned grid = std::max(blocks(tb, n16), 1u);
+    auto *i4 = reinterpret_cast<const uint4 *>(in);
+    auto *o4 = reinterpret_cast<uint4 *>(out);
+    if (tb->L == 1) acb_fold_kernel<1><<<grid, 256, 0, s>>>(i4, o4, n16, tail);
+    else acb_fold_kernel<4><<<grid, 256, 0, s>>>(i4, o4, n16, tail);
+    return launched("case fold");
+}
+
+extern "C" int acb_table_upload_folded(const acb_trie *t, int device, const int32_t *alias_ptr, const int32_t *alias_ids,
+                                       int64_t n_alias, acb_table **out) {
+    if (!t || !out || n_alias < 0 || (n_alias && (!alias_ptr || !alias_ids))) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    acb_flat_view f;
+    int rc = acb_trie_flat_view(t, &f);
+    if (rc != ACB_OK) return rc;
+    if (f.letter_bytes != 1 && f.letter_bytes != 4) { acb_set_error("case folding takes 1- or 4-byte letters, not %d", f.letter_bytes); return ACB_EINVAL; }
+    /* the alias lists: alias_ptr[0 .. n_keys] from 0 to n_alias, each list ascending above its representative, which is a
+     * live key of the trie */
+    int32_t max_id = f.n_keys - 1;
+    if (alias_ptr) {
+        bool ok = alias_ptr[0] == 0 && alias_ptr[f.n_keys] == n_alias;
+        for (int32_t k = 0; ok && k < f.n_keys; k++) {
+            ok = alias_ptr[k + 1] >= alias_ptr[k] && (alias_ptr[k + 1] == alias_ptr[k] || f.key_len[k] > 0);
+            for (int32_t j = alias_ptr[k]; ok && j < alias_ptr[k + 1]; j++) {
+                ok = alias_ids[j] > (j == alias_ptr[k] ? k : alias_ids[j - 1]) && alias_ids[j] < 0x7fffffff;
+                if (ok) max_id = std::max(max_id, alias_ids[j]);
+            }
+        }
+        if (!ok) {
+            acb_set_error("alias lists must run from 0 to n_alias over n_keys + 1 offsets, each ascending above its live key id");
+            return ACB_EINVAL;
+        }
+    }
+    if ((rc = acb_table_upload(t, device, out))) return rc;
+    acb_table *tb = *out;
+    tb->fold = 1;
+    tb->n_rep = f.n_keys;
+    tb->n_alias = n_alias;
+    do {
+        if (!n_alias) break;
+        try {                                              /* an alias has its representative's length */
+            tb->key_len.resize((size_t)max_id + 1, 0);
+            for (int32_t k = 0; k < f.n_keys; k++)
+                for (int32_t j = alias_ptr[k]; j < alias_ptr[k + 1]; j++) tb->key_len[alias_ids[j]] = f.key_len[k];
+        } catch (const std::exception &) {
+            acb_set_error("out of host memory while staging the tables");
+            rc = ACB_ENOMEM;
+            break;
+        }
+        cudaFree(tb->d_keylen);                            /* replaced by the longer list, as upload() sized it */
+        tb->d_keylen = nullptr;
+        tb->dev_bytes -= (long long)(((size_t)std::max(f.n_keys, 1) * sizeof(int32_t) + 15) & ~(size_t)15);
+        tb->n_keys = max_id + 1;
+        if ((rc = upload(&tb->d_keylen, tb->key_len.data(), tb->key_len.size(), tb->dev_bytes))) break;
+        if ((rc = upload(&tb->d_alias_ptr, alias_ptr, (size_t)f.n_keys + 1, tb->dev_bytes))) break;
+        rc = upload(&tb->d_alias_ids, alias_ids, (size_t)n_alias, tb->dev_bytes);
+    } while (0);
+    if (rc != ACB_OK) { acb_table_free(tb); *out = nullptr; }
+    return rc;
+}
+
+extern "C" int acb_last_fold_ms(float *ms, int32_t n) {
+    if (!ms || n < 0 || n > 2) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    for (int i = 0; i < n; i++) ms[i] = g_fold_ms[i];
+    return ACB_OK;
+}
+
+static int scratch_take(Scratch &sc, size_t need, cudaStream_t s);
+static int scratch_done(cudaEvent_t *done, cudaStream_t s);
+
 /* an ACB_ALGO_LONG scan with no text or no keys launches nothing: haystack 0 ends in the state it starts in, and the
  * one-shot start state is consumed as by any other scan */
 static void long_scan_without_launch(acb_table *tb) {
@@ -1722,6 +1864,7 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
                                const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
                                acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
     if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (algo == ACB_ALGO_LONG && refuse_folded(tb, "ACB_ALGO_LONG")) return ACB_EINVAL;
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
     if (!d_offsets) {
         int rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1);
@@ -1744,8 +1887,15 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
         if (algo == ACB_ALGO_LONG) long_scan_without_launch(tb);
         return ACB_OK;
     }
-    int rc = timing_mark(&tb->ev0, s);
-    if (rc != ACB_OK) return rc;
+    int rc;
+    if (tb->fold) {                                         /* the scan reads a folded copy; d_hay stays as the caller gave it */
+        g_fold_ms[0] = 0.f;
+        if ((rc = scratch_take(tb->f_buf, (size_t)total_bytes + 64, s)) || (rc = timing_mark(&tb->f_ev[0], s)) ||
+            (rc = fold_text(tb, d_hay, static_cast<uint8_t *>(tb->f_buf.buf), total_bytes, s)) || (rc = timing_mark(&tb->f_ev[1], s)))
+            return rc;
+        p.hay = static_cast<const uint8_t *>(tb->f_buf.buf);
+    }
+    if ((rc = timing_mark(&tb->ev0, s))) return rc;
     if (algo == ACB_ALGO_FILTER) {
         if ((rc = launch_filter_range(tb, p, 0, total_bytes, s))) return rc;
     } else if (algo == ACB_ALGO_DFA) {
@@ -1768,6 +1918,7 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
         return ACB_EINVAL;
     }
     if ((rc = timing_mark(&tb->ev1, s))) return rc;
+    if (tb->fold && ((rc = scratch_done(&tb->f_buf.done, s)) || (rc = timing_ms(tb->f_ev[0], tb->f_ev[1], &g_fold_ms[0])))) return rc;
     return timing_ms(tb->ev0, tb->ev1, &g_last_ms);
 }
 
@@ -2034,7 +2185,8 @@ struct RefOrder {
     bool operator()(const acb_match &a, const acb_match &b) const {
         if (a.hay_id != b.hay_id) return a.hay_id < b.hay_id;
         if (a.end_index != b.end_index) return a.end_index < b.end_index;
-        return key_len[a.key_id] > key_len[b.key_id];
+        if (key_len[a.key_id] != key_len[b.key_id]) return key_len[a.key_id] > key_len[b.key_id];
+        return a.key_id < b.key_id;                            /* equal lengths at one end: case variants (alias expansion) */
     }
 };
 
@@ -2116,6 +2268,10 @@ static int scan_host_pipelined(acb_table *tb, const uint8_t *hay, int64_t total,
     auto cut = [&](int c) { return c <= 0 ? 0LL : (c >= nch ? (long long)total : std::max<long long>(0, (long long)c * kChunk - reach)); };
     for (int c = 0; c < nch; c++) {
         CUDA_TRY(cudaStreamWaitEvent(sc, tb->ev_h2d[c], 0));
+        if (tb->fold) {                                         /* in place: only this scan reads the batch's copy */
+            const long long b0 = (long long)c * kChunk, b1 = std::min<long long>(b0 + kChunk, total);
+            if ((rc = fold_text(tb, tb->w_hay + b0, tb->w_hay + b0, b1 - b0, sc))) return rc;
+        }
         if (cut(c + 1) > cut(c) && (rc = launch_filter_range(tb, p, cut(c), cut(c + 1), sc))) return rc;
         CUDA_TRY(cudaMemcpyAsync(tb->h_counts + c, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, sc));
         CUDA_TRY(cudaEventRecord(tb->ev_scan[c], sc));
@@ -2154,10 +2310,17 @@ static int scan_host_pipelined(acb_table *tb, const uint8_t *hay, int64_t total,
     return ACB_OK;
 }
 
+struct WordSet;
+static int scan_host_full(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                          int64_t stride_bytes, const WordSet *ws, acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort);
+
 extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_bytes,
                              const int64_t *offsets, int64_t n_hay, int64_t stride_bytes,
                              acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort) {
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (algo == ACB_ALGO_LONG && refuse_folded(tb, "ACB_ALGO_LONG")) return ACB_EINVAL;
+    if (tb->n_alias)                                             /* the full list, expanded; not pipelined */
+        return scan_host_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, nullptr, out, cap, n_found, algo, sort);
     *n_found = 0;
     tb->h_out_n = 0;
     if (total_bytes == 0 || n_hay == 0) {
@@ -2437,6 +2600,7 @@ extern "C" int acb_scan_device_skip(acb_table *tb, const uint8_t *d_hay, int64_t
                                     acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo,
                                     const uint32_t *skip, int64_t n_skip) {
     if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (refuse_folded(tb, "a white-space scan")) return ACB_EINVAL;
     int rc = check_skip(skip, n_skip, algo);
     if (rc != ACB_OK) return rc;
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
@@ -2461,6 +2625,7 @@ extern "C" int acb_scan_host_skip(acb_table *tb, const uint8_t *hay, int64_t tot
                                   acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort,
                                   const uint32_t *skip, int64_t n_skip) {
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (refuse_folded(tb, "a white-space scan")) return ACB_EINVAL;
     *n_found = 0;
     int rc = check_skip(skip, n_skip, algo);
     if (rc != ACB_OK) return rc;
@@ -2634,6 +2799,7 @@ struct acb_streams {
 static int32_t tail_letters(const acb_table *tb) { return std::max<int32_t>(tb->max_key_bytes / tb->L - 1, 0); }
 
 static int streams_check_table(const acb_streams *ss, const acb_table *tb) {
+    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
     if (tb->device != ss->device || tb->L != ss->L || (!ss->long_mode && tail_letters(tb) != ss->T) || (ss->long_mode && tb->S != ss->S)) {
         acb_set_error("the table does not belong to this stream batch (device %d/%d, letter bytes %d/%d, tail %d/%d, states %d/%d)",
                       tb->device, ss->device, tb->L, ss->L, ss->long_mode ? 0 : tail_letters(tb), ss->T, tb->S, ss->S);
@@ -2665,6 +2831,7 @@ extern "C" void acb_streams_free(acb_streams *ss) {
 extern "C" int acb_streams_new(const acb_table *tb, int64_t n_streams, int long_mode, acb_streams **out) {
     if (!tb || !out || n_streams < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
+    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
     if (n_streams > 0x7fffffffLL) { acb_set_error("more than 2^31-1 streams"); return ACB_ERANGE; }
     CUDA_TRY(cudaSetDevice(tb->device));
     acb_streams *ss = new (std::nothrow) acb_streams();
@@ -2917,6 +3084,7 @@ __global__ void __launch_bounds__(kLookupThreads) acb_lookup_kernel(const __grid
 
 extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t total_bytes, const int64_t *d_offsets,
                                  int64_t n_keys, int64_t stride_bytes, int32_t *d_key_id, int32_t *d_prefix, void *stream) {
+    if (refuse_folded(tb, "a lookup")) return ACB_EINVAL;
     if (!tb || total_bytes < 0 || n_keys < 0 || (total_bytes && !d_keys) || (n_keys && (!d_key_id || !d_prefix))) {
         acb_set_error("bad argument");
         return ACB_EINVAL;
@@ -2940,6 +3108,7 @@ extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t t
 
 extern "C" int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total_bytes, const int64_t *offsets,
                                int64_t n_keys, int64_t stride_bytes, int32_t *key_id, int32_t *prefix) {
+    if (refuse_folded(tb, "a lookup")) return ACB_EINVAL;
     if (!tb || total_bytes < 0 || n_keys < 0 || (total_bytes && !keys) || (n_keys && (!key_id || !prefix))) {
         acb_set_error("bad argument");
         return ACB_EINVAL;
@@ -3083,6 +3252,7 @@ __global__ void __launch_bounds__(kSelectThreads) acb_select_kernel(const __grid
 
 extern "C" int acb_table_upload_key_ranges(acb_table *tb, const acb_trie *t) {
     if (!tb || !t) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (refuse_folded(tb, "a key selection")) return ACB_EINVAL;
     if (tb->d_order) return ACB_OK;
     acb_flat_view f;
     int rc = acb_trie_flat_view(t, &f);
@@ -3168,6 +3338,7 @@ static int select_fill(acb_table *tb, const SelectParams &p, int64_t n, cudaStre
 
 static int select_common_checks(const acb_table *tb, const void *pat, int64_t total_bytes, int64_t n, const void *out_off,
                                 const void *key_id, int64_t cap, const void *total, int64_t wildcard, int how) {
+    if (refuse_folded(tb, "a key selection")) return ACB_EINVAL;
     if (!tb || total_bytes < 0 || n < 0 || (total_bytes && !pat) || !out_off || !total || cap < 0 || (cap && !key_id)) {
         acb_set_error("bad argument");
         return ACB_EINVAL;
@@ -3601,6 +3772,101 @@ extern "C" int acb_word_filter_device(acb_table *tb, const uint8_t *d_hay, int64
     return timing_ms(tb->ww_ev[0], tb->ww_ev[1], &g_ww_ms);
 }
 
+/* ------------------------------------------------------------ alias expansion */
+/* A folded table's scan reports each match under its group's representative, the lowest id of the keys that fold to the
+ * same text.  The find_all routes then give every member of the group: record i becomes 1 + aliases(key_id) records,
+ * the representative first and its aliases after it, ascending.  Count per record, exclusive sum, scatter. */
+namespace {
+struct XpArgs {
+    const acb_match *rec;
+    long long n;
+    const int32_t *alias_ptr, *alias_ids;                  /* the table's alias CSR over n_rep ids (nullptr: no aliases) */
+    int32_t n_rep;
+};
+
+__device__ __forceinline__ int32_t xp_aliases(const XpArgs &a, int32_t k, int32_t *first) {
+    if (!a.alias_ptr || k < 0 || k >= a.n_rep) { *first = 0; return 0; }
+    *first = __ldg(a.alias_ptr + k);
+    return __ldg(a.alias_ptr + k + 1) - *first;
+}
+
+/* pos[i] = the records record i becomes; pos[n] = 0 (the exclusive sum then leaves the total there) */
+__global__ void acb_xp_count_kernel(const __grid_constant__ XpArgs a, long long *pos) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= a.n; i += (long long)gridDim.x * blockDim.x) {
+        int32_t first;
+        pos[i] = i < a.n ? 1 + xp_aliases(a, a.rec[i].key_id, &first) : 0;
+    }
+}
+
+/* the expanded records at out[pos[i] ..], those at or past cap not stored; *count = pos[n], the total */
+__global__ void acb_xp_scatter_kernel(const __grid_constant__ XpArgs a, const long long *pos, acb_match *out, long long cap,
+                                      long long *count) {
+    const long long first_i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (first_i == 0) *count = pos[a.n];
+    for (long long i = first_i; i < a.n; i += (long long)gridDim.x * blockDim.x) {
+        acb_match m = a.rec[i];
+        long long o = pos[i];
+        int32_t first;
+        const int32_t k = xp_aliases(a, m.key_id, &first);
+        if (o < cap) out[o] = m;
+        for (int32_t j = 0; j < k && ++o < cap; j++) {
+            m.key_id = __ldg(a.alias_ids + first + j);
+            out[o] = m;
+        }
+    }
+}
+} // namespace
+
+extern "C" int acb_expand_aliases_device(acb_table *tb, const acb_match *d_in, int64_t n, acb_match *d_out, int64_t cap,
+                                         int64_t *d_count, void *stream) {
+    if (!tb || n < 0 || (n && !d_in) || cap < 0 || (cap > 0 && !d_out) || !d_count) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (!tb->fold) { acb_set_error("alias expansion needs a case-folded table (acb_table_upload_folded)"); return ACB_EINVAL; }
+    if (n > 0x7fffffffLL) { acb_set_error("more than 2^31-1 records to expand"); return ACB_ERANGE; }
+    g_fold_ms[1] = 0.f;
+    CUDA_TRY(cudaSetDevice(tb->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (n == 0) {
+        CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
+        return ACB_OK;
+    }
+    const size_t N = (size_t)n + 1;
+    size_t temp = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, (long long *)nullptr, (long long *)nullptr, (int)N, s));
+    int rc;
+    if ((rc = scratch_take(tb->x_buf, 2 * 256 + N * sizeof(long long) + temp, s))) return rc;
+    char *p = static_cast<char *>(tb->x_buf.buf);
+    long long *pos = carve<long long>(p, N);
+    void *tmp = carve<char>(p, temp);
+    const XpArgs a{d_in, (long long)n, tb->d_alias_ptr, tb->d_alias_ids, tb->n_rep};
+    if ((rc = timing_mark(&tb->f_ev[2], s))) return rc;
+    acb_xp_count_kernel<<<blocks(tb, n + 1), 256, 0, s>>>(a, pos);
+    if ((rc = launched("alias count"))) return rc;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, temp, pos, pos, (int)N, s));
+    acb_xp_scatter_kernel<<<blocks(tb, n), 256, 0, s>>>(a, pos, d_out, cap, reinterpret_cast<long long *>(d_count));
+    if ((rc = launched("alias scatter")) || (rc = timing_mark(&tb->f_ev[3], s)) || (rc = scratch_done(&tb->x_buf.done, s))) return rc;
+    return timing_ms(tb->f_ev[2], tb->f_ev[3], &g_fold_ms[1]);
+}
+
+/* The host find_all routes on a table with aliases: the n records at *rec expanded into tb->x_out, grown to fit; then
+ * *rec, *n and tb->w_count describe the expanded list.  Nothing without aliases.  On tb->stream, left synchronised. */
+static int expand_host(acb_table *tb, acb_match **rec, unsigned long long *n) {
+    if (!tb->n_alias || *n == 0) return ACB_OK;
+    cudaStream_t s = tb->stream;
+    int rc = ensure(&tb->x_out, &tb->x_out_cap, (size_t)*n);
+    for (; rc == ACB_OK;) {
+        if ((rc = acb_expand_aliases_device(tb, *rec, (int64_t)*n, tb->x_out, (int64_t)tb->x_out_cap, reinterpret_cast<int64_t *>(tb->w_count), s)))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(tb->h_count, tb->w_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (*tb->h_count <= tb->x_out_cap) break;
+        rc = ensure(&tb->x_out, &tb->x_out_cap, (size_t)*tb->h_count);
+    }
+    if (rc != ACB_OK) return rc;
+    *rec = tb->x_out;
+    *n = *tb->h_count;
+    return ACB_OK;
+}
+
 /* The word set of a host route that filters (acb_*_words): a host bitmap */
 struct WordSet {
     const uint32_t *bits;
@@ -3656,24 +3922,34 @@ static int check_words_route(const acb_table *tb, const uint32_t *bits, int64_t 
     return rc;
 }
 
-extern "C" int acb_scan_host_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
-                                   int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap,
-                                   int64_t *n_found, int algo, int sort) {
+/* acb_scan_host_words, and without a word set (ws == nullptr) acb_scan_host on a table with aliases: the full list, its
+ * whole-word records, expanded (expand_host), sorted and copied back */
+static int scan_host_full(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                          int64_t stride_bytes, const WordSet *ws, acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort) {
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
     if (algo != ACB_ALGO_AUTO && algo != ACB_ALGO_FILTER && algo != ACB_ALGO_DFA) { acb_set_error("a whole-word scan takes ACB_ALGO_AUTO, _FILTER or _DFA"); return ACB_EINVAL; }
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
     int rc;
-    if ((rc = check_words_route(tb, bits, n_bits, offsets, n_hay, total_bytes))) return rc;
+    if (ws && (rc = check_words_route(tb, ws->bits, ws->n_bits, offsets, n_hay, total_bytes))) return rc;
+    if (!ws && offsets && (rc = check_offsets(tb->L, offsets, n_hay, total_bytes))) return rc;
     if (!offsets && (rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1))) return rc;
     tb->h_out_n = 0;
     if (total_bytes == 0 || n_hay == 0) return ACB_OK;
-    const WordSet ws{bits, n_bits};
     const int64_t *d_off = nullptr;
     unsigned long long full = 0;
     acb_match *rec = nullptr;
-    if ((rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, &ws, &d_off, &full, &rec))) return rc;
+    if ((rc = upload_and_scan_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, algo, ws, &d_off, &full, &rec)) ||
+        (rc = expand_host(tb, &rec, &full)))
+        return rc;
     return read_back(tb, tb->w_count, rec, cap, sort, n_hay, (offsets ? total_bytes : stride_bytes) / tb->L, out, n_found, tb->stream);
+}
+
+extern "C" int acb_scan_host_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
+                                   int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap,
+                                   int64_t *n_found, int algo, int sort) {
+    const WordSet ws{bits, n_bits};
+    return scan_host_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, &ws, out, cap, n_found, algo, sort);
 }
 
 static int scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
