@@ -646,9 +646,9 @@ int acb_streams_feed_words_host(acb_streams *ss, acb_table *tb, const uint8_t *c
  * carry representative ids.  acb_scan_host and acb_scan_host_words on a table with aliases expand them before the sort
  * (acb_expand_aliases_device; such a table is not pipelined); the leftmost and replacement routes do not: the
  * representative is the leftmost-first winner and the leftmost-longest one among keys of one text.  Refused (ACB_EINVAL):
- * ACB_ALGO_LONG, the white-space scans (*_skip), stream batches (acb_streams_new* and every feed), lookups and key
- * selections (acb_lookup_*, acb_select_*, acb_table_upload_key_ranges).  A table from acb_table_upload behaves as
- * before. */
+ * ACB_ALGO_LONG, the white-space scans (*_skip), the stream batch constructors other than acb_streams_new_folded (and
+ * every feed of a batch they made), lookups and key selections (acb_lookup_*, acb_select_*, acb_table_upload_key_ranges).
+ * A table from acb_table_upload behaves as before. */
 int acb_table_upload_folded(const acb_trie *t, int device, const int32_t *alias_ptr, const int32_t *alias_ids, int64_t n_alias,
                             acb_table **out);
 
@@ -661,9 +661,28 @@ int acb_table_upload_folded(const acb_trie *t, int device, const int32_t *alias_
 int acb_expand_aliases_device(acb_table *tb, const acb_match *d_in, int64_t n, acb_match *d_out, int64_t cap, int64_t *d_count,
                               void *stream);
 
-/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last fold of acb_scan_device (the pipelined
- * acb_scan_host's folds are not timed) and of the last alias expansion on this thread (the first n of them, n <= 2), from
- * CUDA events (the call then waits for them); 0 when timing is off. */
+/* A case-folded stream batch: every stream's text matched as a folded table's scans match a whole haystack.  tb must
+ * come from acb_table_upload_folded (else ACB_EINVAL).  leftmost = 0: a find_all batch, fed by acb_streams_feed_device /
+ * _host, or with a word set by acb_streams_feed_words_*; leftmost = 1: a leftmost batch of selection `kind`
+ * (ACB_SELECT_LONGEST or ACB_SELECT_FIRST; checked in both cases), fed by acb_streams_feed_leftmost_* and
+ * acb_streams_replace_*, with or without a word set.  bits / n_bits: the word set, as for acb_streams_new_words; no word
+ * set is bits == NULL with n_bits < 0.  No long mode and no skip set.  Each feed reports and releases exactly what the
+ * same feed of a batch from acb_streams_new / _new_words / _new_leftmost_kind reports over the folded text (the fold maps
+ * each letter alone, so folding chunk by chunk folds the stream), with the word tests and the rewrites on the text as
+ * given: held letters keep their case.  A find_all feed reports every alias of each key found, after it and ascending, and
+ * the capacity test of the feed is on that expanded count: a feed that overflows still changes no stream.  On a key set
+ * with aliases the plain find_all feed waits once for the unexpanded count; without aliases it stays asynchronous.  The
+ * feeds of a folded batch refuse any other table, and the feeds of any other batch refuse a folded table (ACB_EINVAL).
+ * The device find_all feed folds into a copy the batch owns; the host feeds fold their upload in place: caller memory is
+ * never written.  A find_all feed refuses what acb_scan_device refuses (ACB_ERANGE for a fixed stride past 2^31-1
+ * letters) before it folds or launches anything, as the plain feed does. */
+int acb_streams_new_folded(const acb_table *tb, int64_t n_streams, int leftmost, int kind, const uint32_t *bits, int64_t n_bits,
+                           acb_streams **out);
+
+/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last fold of acb_scan_device or of a folded
+ * find_all stream feed (the pipelined acb_scan_host's folds are not timed) and of the last alias expansion on this thread
+ * (the first n of them, n <= 2), from CUDA events (the call then waits for them); 0 when timing is off, and a folded stream
+ * feed zeroes both before it runs. */
 int acb_last_fold_ms(float *ms, int32_t n);
 
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */

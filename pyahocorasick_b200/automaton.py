@@ -820,12 +820,16 @@ class Automaton:
     def flat(self, narrow: bool = False) -> dict:
         """White-box view of the flattened automaton (numpy copies) -- used by tests and docs.
         narrow=True: the latin-1 automaton of a unicode-flavour Automaton (None if it has no latin-1 key)."""
-        fv = N.FlatView()
         trie = self._trie
         if narrow:
             trie = self._narrow_host()
             if trie is None:
                 return None
+        return self._flat_view(trie)
+
+    def _flat_view(self, trie) -> dict:
+        """flat() of a host trie of this automaton (also the folded ones of _fold_host)"""
+        fv = N.FlatView()
         N.check(self._lib.acb_trie_flat_view(trie, ctypes.byref(fv)))
         S, K = fv.n_states, fv.n_classes
 
@@ -883,6 +887,10 @@ class Automaton:
         tb = self._table_for(device, narrow, fold)
         if tb is None:
             return np.empty(0, dtype=N.MATCH_DTYPE)
+        return self._host_records_on(tb, n_hay, call)
+
+    def _host_records_on(self, tb, n_hay: int, call) -> np.ndarray:
+        """_host_records on the table tb"""
         found = ctypes.c_int64(0)
         rc = call(tb, self._record_room(n_hay), ctypes.byref(found))
         if rc == N.ACB_EOVERFLOW:
@@ -1390,7 +1398,26 @@ class Automaton:
 
         Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
         wider chunks, so the latin-1 automaton is not used)."""
+        return self._stream_batch(n_streams, long, algo, device, ignore_white_space, leftmost_longest, whole_words,
+                                  leftmost_first, False)
+
+    def ascii_case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
+                                            leftmost_longest: bool = False, leftmost_first: bool = False,
+                                            whole_words=False) -> "StreamBatch":
+        """`stream_batch` with ASCII case-insensitive matching: over all feeds (and `finish`) of a stream, what
+        find_all_batch, find_leftmost_longest_batch or find_leftmost_first_batch reports for its whole text with
+        ascii_case_insensitive=True and the same whole_words.  A find_all batch reports every key whose folded text
+        occurs, keys of one length at one end in ascending id; a leftmost batch reports, of the keys that fold to one
+        text, the one added first.  Matches are released at the same points as by the stream_batch of the same options,
+        and the word test reads the letters as given.  Takes neither long nor ignore_white_space; not for KEY_SEQUENCE
+        automata.  The returned StreamBatch has ``ascii_case_insensitive`` True."""
+        return self._stream_batch(n_streams, False, algo, device, False, leftmost_longest, whole_words, leftmost_first, True)
+
+    def _stream_batch(self, n_streams: int, long: bool, algo: str, device: Optional[int], ignore_white_space: bool,
+                      leftmost_longest: bool, whole_words, leftmost_first: bool, fold: bool) -> "StreamBatch":
+        """The argument check and constructor of stream_batch and ascii_case_insensitive_stream_batch (fold)"""
         self._require_automaton()
+        self._fold_arg(fold)
         n_streams = operator.index(n_streams)
         if n_streams < 0:
             raise ValueError("n_streams must not be negative")
@@ -1407,7 +1434,7 @@ class Automaton:
             raise ValueError("iter_long has no ignore_white_space option")
         skip = self._skip_set(False) if ignore_white_space else None
         return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip,
-                           bool(leftmost_longest), words, bool(leftmost_first))
+                           bool(leftmost_longest), words, bool(leftmost_first), fold)
 
     # ------------------------------------------------------------------ batch lookups (new)
     # exists / match / longest_prefix / get for a whole batch of keys, in one GPU call (acb_lookup_*).  `keys` takes the
@@ -1631,6 +1658,14 @@ class _Streams:
         N.check(lib.acb_streams_positions(self._ss, N.ptr(out), self.n_streams))
         return out[:self.n_streams]
 
+    def _table(self):
+        """(the table every call of this batch runs on, whether it is folded): the automaton's full table, or for an
+        ascii_case_insensitive batch its folded one -- the full one when there is no key, which matches nothing either
+        way"""
+        A = self._A
+        tb = A._table_for(self._device, False, True) if self.ascii_case_insensitive else None
+        return (A._ensure_table(self._device), False) if tb is None else (tb, True)
+
     def _ids(self, ids, n: int) -> Optional[np.ndarray]:
         if ids is None:
             if n > self.n_streams:
@@ -1690,11 +1725,17 @@ class StreamBatch(_Streams):
     chunk; a leftmost_longest match by the first feed after which it starts before ``position - longest_word``.
 
     A leftmost_first batch is a leftmost_longest batch under the leftmost-first rule: it reports what
-    `find_leftmost_first_batch` reports (with the same whole_words), at the same points."""
+    `find_leftmost_first_batch` reports (with the same whole_words), at the same points.
+
+    A batch from `Automaton.ascii_case_insensitive_stream_batch` (``ascii_case_insensitive`` True) reports what the
+    batch of the same options reports, with keys and text compared ASCII case-insensitively: what the whole-batch
+    method reports with ascii_case_insensitive=True for each stream's whole text."""
 
     def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None,
-                 leftmost_longest: bool = False, words: Optional[tuple] = None, leftmost_first: bool = False):
+                 leftmost_longest: bool = False, words: Optional[tuple] = None, leftmost_first: bool = False,
+                 fold: bool = False):
         self._A = A
+        self.ascii_case_insensitive = fold
         self._version = A._version
         self.n_streams = n_streams
         self.long = long
@@ -1726,12 +1767,16 @@ class StreamBatch(_Streams):
         A = self._A
         if op == "new":
             ss = ctypes.c_void_p()
-            N.check(A._lib.acb_streams_new(A._ensure_table(self._device), self.n_streams, int(self.long), ctypes.byref(ss)))
+            tb, folded = self._table()
+            if folded:
+                N.check(A._lib.acb_streams_new_folded(tb, self.n_streams, 0, N.SELECT_LONGEST, None, -1, ctypes.byref(ss)))
+            else:
+                N.check(A._lib.acb_streams_new(tb, self.n_streams, int(self.long), ctypes.byref(ss)))
             return ss
         if op == "new_leftmost":
-            return _new_leftmost_streams(A, self.n_streams, self._device, self._select)
+            return _new_leftmost_streams(A, self._table(), self.n_streams, self._select)
         if op == "new_words":
-            return _new_word_streams(A, self.n_streams, self._device, self.leftmost_longest or self.leftmost_first, self._words,
+            return _new_word_streams(A, self._table(), self.n_streams, self.leftmost_longest or self.leftmost_first, self._words,
                                      self._select)
         if op == "new_skip":
             skip, = args
@@ -1758,10 +1803,10 @@ class StreamBatch(_Streams):
                 if op == "feed_words":
                     return lib.acb_streams_feed_words_host(*args, int(flag), None, cap, found_ref, algo)
                 return lib.acb_streams_feed_host(*args, None, cap, found_ref, algo, int(flag))
-            return A._host_records(self._device, False, n, feed)
+            return A._host_records_on(self._table()[0], n, feed)
         import torch
         t = _stream_tensor(data, n, stride, self._device)
-        tb = A._ensure_table(self._device)
+        tb = self._table()[0]
         with _on_device(self._device) as stream:
             d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
             args = (self._ss, tb, t.data_ptr() if n and stride else None, n * stride, None, n, stride,
@@ -1943,17 +1988,30 @@ class Replacer:
         """`n_streams` streams rewritten chunk by chunk (ReplaceStream.feed): over all feeds and `finish` of a stream,
         the output is exactly what `replace_batch` gives for its whole text, with the same whole_words.  Streams run at
         the automaton's full letter width (unicode: 4 bytes per letter), as every stream batch does."""
+        return self._stream_batch(n_streams, algo, device, whole_words, False)
+
+    def ascii_case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
+                                            whole_words=False) -> "ReplaceStream":
+        """`stream_batch` with ASCII case-insensitive matching: over all feeds and `finish` of a stream, the output is
+        exactly what `replace_batch` gives for its whole text with ascii_case_insensitive=True and the same whole_words.
+        Each match takes the replacement of the key added first among those that fold to its text; every other letter,
+        held ones included, keeps its own case.  The returned ReplaceStream has ``ascii_case_insensitive`` True."""
+        return self._stream_batch(n_streams, algo, device, whole_words, True)
+
+    def _stream_batch(self, n_streams: int, algo: str, device: Optional[int], whole_words, fold: bool) -> "ReplaceStream":
+        """The argument check and constructor of stream_batch and ascii_case_insensitive_stream_batch (fold)"""
         A = self._A
         if self._version != A._version:
             raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
         A._require_automaton()
+        A._fold_arg(fold)
         n_streams = operator.index(n_streams)
         if n_streams < 0:
             raise ValueError("n_streams must not be negative")
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: a replacing stream batch takes 'auto', 'filter' or 'dfa'")
         words = A._words(whole_words)
-        return ReplaceStream(self, n_streams, algo, self._device if device is None else device, words)
+        return ReplaceStream(self, n_streams, algo, self._device if device is None else device, words, fold)
 
     def _items(self, out: np.ndarray, offs: np.ndarray, narrow: bool) -> list:
         """the output haystacks as objects of the input's type"""
@@ -2023,10 +2081,13 @@ class ReplaceStream(_Streams):
     letter before ``position - (longest_word - 1)`` and every replacement that starts there); ``finish(ids=None)``
     returns the rest and returns those streams to their start.  Concatenated, a stream's outputs are what
     `Replacer.replace_batch` gives for its whole text.  Stale (ValueError) when the replacer is.  With whole_words, a
-    stream holds back one letter more: the output before ``position - longest_word`` is released."""
+    stream holds back one letter more: the output before ``position - longest_word`` is released.  From
+    `Replacer.ascii_case_insensitive_stream_batch` (``ascii_case_insensitive`` True), the output is what replace_batch
+    gives with ascii_case_insensitive=True, released at the same points."""
 
-    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int, words: Optional[tuple] = None):
+    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int, words: Optional[tuple] = None, fold: bool = False):
         self._R = R
+        self.ascii_case_insensitive = fold
         self._A = R._A
         self._version = R._version
         self.n_streams = n_streams
@@ -2045,12 +2106,12 @@ class ReplaceStream(_Streams):
         lib = A._lib
         if op == "new":
             if self._words is not None:
-                return _new_word_streams(A, self.n_streams, self._device, True, self._words, self._R._select)
-            return _new_leftmost_streams(A, self.n_streams, self._device, self._R._select)
+                return _new_word_streams(A, self._table(), self.n_streams, True, self._words, self._R._select)
+            return _new_leftmost_streams(A, self._table(), self.n_streams, self._R._select)
         if op != "feed":
             return super()._native(op, *args)
         kind, data, offs, n, stride, ids, final = args
-        tb = A._ensure_table(self._device)
+        tb = self._table()[0]
         r = self._R._replacer(tb, False, self._device)
         algo = N.ALGOS[self._algo]
         held = n * max(int(lib.acb_trie_longest_word(A._trie)) - 1 + self.whole_words, 0) * A._L   # at most what is held back
@@ -2382,23 +2443,30 @@ def _host_bytes(cap: int, call) -> np.ndarray:
     return out[:total.value]
 
 
-def _new_leftmost_streams(A: Automaton, n_streams: int, device: int, select: int = N.SELECT_LONGEST):
+def _new_leftmost_streams(A: Automaton, table, n_streams: int, select: int = N.SELECT_LONGEST):
+    """a leftmost stream batch on table = (tb, folded) (_Streams._table)"""
     ss = ctypes.c_void_p()
-    tb = A._ensure_table(device)
-    if select == N.SELECT_LONGEST:
+    tb, folded = table
+    if folded:
+        N.check(A._lib.acb_streams_new_folded(tb, n_streams, 1, select, None, -1, ctypes.byref(ss)))
+    elif select == N.SELECT_LONGEST:
         N.check(A._lib.acb_streams_new_leftmost(tb, n_streams, ctypes.byref(ss)))
     else:
         N.check(A._lib.acb_streams_new_leftmost_kind(tb, n_streams, select, None, -1, ctypes.byref(ss)))
     return ss
 
 
-def _new_word_streams(A: Automaton, n_streams: int, device: int, leftmost: bool, words: tuple, select: int = N.SELECT_LONGEST):
-    """a whole-word stream batch (acb_streams_new_words; acb_streams_new_leftmost_kind for leftmost-first) with the
-    word set at the streams' full letter width"""
+def _new_word_streams(A: Automaton, table, n_streams: int, leftmost: bool, words: tuple, select: int = N.SELECT_LONGEST):
+    """a whole-word stream batch (acb_streams_new_words; acb_streams_new_leftmost_kind for leftmost-first;
+    acb_streams_new_folded on a folded table) on table = (tb, folded) (_Streams._table) with the word set at the
+    streams' full letter width"""
     bits, n_bits = _word_bits(words, A._L)
     ss = ctypes.c_void_p()
-    tb = A._ensure_table(device)
-    if leftmost and select != N.SELECT_LONGEST:
+    tb, folded = table
+    if folded:
+        N.check(A._lib.acb_streams_new_folded(tb, n_streams, int(leftmost), select, N.ptr(bits) if n_bits else None, n_bits,
+                                              ctypes.byref(ss)))
+    elif leftmost and select != N.SELECT_LONGEST:
         N.check(A._lib.acb_streams_new_leftmost_kind(tb, n_streams, select, N.ptr(bits) if n_bits else None, n_bits,
                                                      ctypes.byref(ss)))
     else:

@@ -1860,17 +1860,54 @@ static void long_scan_without_launch(acb_table *tb) {
     tb->long_init = 0;
 }
 
-extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
-                               const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
-                               acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
-    if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
-    if (algo == ACB_ALGO_LONG && refuse_folded(tb, "ACB_ALGO_LONG")) return ACB_EINVAL;
+/* the scan launches of acb_scan_device over p, whose text a folded table's caller has already folded: timed by ev0 / ev1
+ * into g_last_ms */
+static int scan_text(acb_table *tb, ScanParams &p, int64_t total_bytes, int64_t n_hay, int algo, cudaStream_t s) {
+    int rc;
+    if ((rc = timing_mark(&tb->ev0, s))) return rc;
+    if (algo == ACB_ALGO_FILTER) {
+        if ((rc = launch_filter_range(tb, p, 0, total_bytes, s))) return rc;
+    } else if (algo == ACB_ALGO_DFA) {
+        long long spans = (total_bytes + kDfaSpan - 1) / kDfaSpan;
+        long long grid = (spans + kDfaThreads - 1) / kDfaThreads;
+        if (grid > 0x7fffffffLL) { acb_set_error("batch too large for one launch"); return ACB_ERANGE; }
+        acb_dfa_kernel<<<(unsigned)grid, kDfaThreads, 0, s>>>(p);
+        if ((rc = launched("DFA kernel"))) return rc;
+    } else if (algo == ACB_ALGO_LONG) {
+        if (!tb->d_long_final) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->d_long_final), sizeof(int32_t)));
+        p.long_init = tb->long_init;
+        p.long_final = tb->d_long_final;
+        tb->long_init = 0;                                      /* one shot */
+        tb->long_final_host = -1;                               /* the kernel writes the final state */
+        long long grid = (n_hay + kDfaThreads - 1) / kDfaThreads;
+        acb_long_kernel<<<(unsigned)grid, kDfaThreads, 0, s>>>(p);
+        if ((rc = launched("iter_long kernel"))) return rc;
+    } else {
+        acb_set_error("unknown algo %d", algo);
+        return ACB_EINVAL;
+    }
+    if ((rc = timing_mark(&tb->ev1, s))) return rc;
+    return timing_ms(tb->ev0, tb->ev1, &g_last_ms);
+}
+
+/* the batch shapes a scan's records can describe (int32 hay_id and end_index): at most 2^31-1 haystacks, and a fixed
+ * stride of at most 2^31-1 letters; checked before anything is launched */
+static int check_scan_shape(const acb_table *tb, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes) {
     if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
     if (!d_offsets) {
         int rc = check_stride(tb->L, total_bytes, n_hay, stride_bytes, 1);
         if (rc != ACB_OK) return rc;
         if (stride_bytes / tb->L > 0x7fffffffLL) { acb_set_error("haystack longer than 2^31-1 letters"); return ACB_ERANGE; }
     }
+    return ACB_OK;
+}
+
+extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
+                               const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
+                               acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (algo == ACB_ALGO_LONG && refuse_folded(tb, "ACB_ALGO_LONG")) return ACB_EINVAL;
+    if (int rc = check_scan_shape(tb, total_bytes, d_offsets, n_hay, stride_bytes)) return rc;
     if (total_bytes == 0 || n_hay == 0) {
         if (algo == ACB_ALGO_LONG) long_scan_without_launch(tb);
         return ACB_OK;
@@ -1895,31 +1932,9 @@ extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t tota
             return rc;
         p.hay = static_cast<const uint8_t *>(tb->f_buf.buf);
     }
-    if ((rc = timing_mark(&tb->ev0, s))) return rc;
-    if (algo == ACB_ALGO_FILTER) {
-        if ((rc = launch_filter_range(tb, p, 0, total_bytes, s))) return rc;
-    } else if (algo == ACB_ALGO_DFA) {
-        long long spans = (total_bytes + kDfaSpan - 1) / kDfaSpan;
-        long long grid = (spans + kDfaThreads - 1) / kDfaThreads;
-        if (grid > 0x7fffffffLL) { acb_set_error("batch too large for one launch"); return ACB_ERANGE; }
-        acb_dfa_kernel<<<(unsigned)grid, kDfaThreads, 0, s>>>(p);
-        if ((rc = launched("DFA kernel"))) return rc;
-    } else if (algo == ACB_ALGO_LONG) {
-        if (!tb->d_long_final) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&tb->d_long_final), sizeof(int32_t)));
-        p.long_init = tb->long_init;
-        p.long_final = tb->d_long_final;
-        tb->long_init = 0;                                      /* one shot */
-        tb->long_final_host = -1;                               /* the kernel writes the final state */
-        long long grid = (n_hay + kDfaThreads - 1) / kDfaThreads;
-        acb_long_kernel<<<(unsigned)grid, kDfaThreads, 0, s>>>(p);
-        if ((rc = launched("iter_long kernel"))) return rc;
-    } else {
-        acb_set_error("unknown algo %d", algo);
-        return ACB_EINVAL;
-    }
-    if ((rc = timing_mark(&tb->ev1, s))) return rc;
+    if ((rc = scan_text(tb, p, total_bytes, n_hay, algo, s))) return rc;
     if (tb->fold && ((rc = scratch_done(&tb->f_buf.done, s)) || (rc = timing_ms(tb->f_ev[0], tb->f_ev[1], &g_fold_ms[0])))) return rc;
-    return timing_ms(tb->ev0, tb->ev1, &g_last_ms);
+    return ACB_OK;
 }
 
 extern "C" int acb_table_set_long_state(acb_table *tb, int32_t state) {
@@ -2794,12 +2809,20 @@ struct acb_streams {
     uint8_t *d_left = nullptr;
     uint32_t *d_bits = nullptr; long long n_bits = 0;
     unsigned long long *d_keys = nullptr; size_t keys_cap = 0;    /* find_all word feeds: sort keys, 2 per kept record */
+    /* case-folded batches (acb_streams_new_folded): fed with the folded table only.  The find_all feed folds the chunks
+     * once, into d_fold (the device feed) or in place (the host feed's upload), and with aliases scans into d_full. */
+    int fold = 0;
+    uint8_t *d_fold = nullptr; size_t fold_cap = 0;
 };
 
 static int32_t tail_letters(const acb_table *tb) { return std::max<int32_t>(tb->max_key_bytes / tb->L - 1, 0); }
 
 static int streams_check_table(const acb_streams *ss, const acb_table *tb) {
-    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
+    if (tb->fold != ss->fold) {                    /* both tables can share L and T: the check below would not tell them apart */
+        acb_set_error(ss->fold ? "a case-folded stream batch takes the folded table (acb_table_upload_folded)"
+                               : "a stream batch does not take a case-folded table");
+        return ACB_EINVAL;
+    }
     if (tb->device != ss->device || tb->L != ss->L || (!ss->long_mode && tail_letters(tb) != ss->T) || (ss->long_mode && tb->S != ss->S)) {
         acb_set_error("the table does not belong to this stream batch (device %d/%d, letter bytes %d/%d, tail %d/%d, states %d/%d)",
                       tb->device, ss->device, tb->L, ss->L, ss->long_mode ? 0 : tail_letters(tb), ss->T, tb->S, ss->S);
@@ -2822,21 +2845,21 @@ extern "C" void acb_streams_free(acb_streams *ss) {
     cudaFree(ss->d_start); cudaFree(ss->d_end); cudaFree(ss->d_ids); cudaFree(ss->d_kept);
     cudaFree(ss->d_hold); cudaFree(ss->d_soff); cudaFree(ss->d_aux); cudaFree(ss->d_stage); cudaFree(ss->d_win); cudaFree(ss->d_ts);
     cudaFree(ss->d_full); cudaFree(ss->d_settled); cudaFree(ss->d_flag); cudaFree(ss->d_chosen); cudaFree(ss->d_tmp);
-    cudaFree(ss->d_ctr); cudaFree(ss->d_left); cudaFree(ss->d_bits); cudaFree(ss->d_keys);
+    cudaFree(ss->d_ctr); cudaFree(ss->d_left); cudaFree(ss->d_bits); cudaFree(ss->d_keys); cudaFree(ss->d_fold);
     if (ss->h_ctr) cudaFreeHost(ss->h_ctr);
     for (cudaEvent_t e : ss->ev) if (e) cudaEventDestroy(e);
     delete ss;
 }
 
-extern "C" int acb_streams_new(const acb_table *tb, int64_t n_streams, int long_mode, acb_streams **out) {
+/* a find_all or iter_long batch of the table's kind (folded or not); the public constructors refuse a folded table */
+static int streams_new(const acb_table *tb, int64_t n_streams, int long_mode, acb_streams **out) {
     if (!tb || !out || n_streams < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
-    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
     if (n_streams > 0x7fffffffLL) { acb_set_error("more than 2^31-1 streams"); return ACB_ERANGE; }
     CUDA_TRY(cudaSetDevice(tb->device));
     acb_streams *ss = new (std::nothrow) acb_streams();
     if (!ss) { acb_set_error("out of memory"); return ACB_ENOMEM; }
-    ss->device = tb->device; ss->L = tb->L; ss->S = tb->S; ss->long_mode = long_mode ? 1 : 0;
+    ss->device = tb->device; ss->L = tb->L; ss->S = tb->S; ss->long_mode = long_mode ? 1 : 0; ss->fold = tb->fold;
     ss->T = ss->long_mode ? 0 : tail_letters(tb);
     ss->n = n_streams;
     const size_t n = (size_t)std::max<int64_t>(n_streams, 1);
@@ -2854,10 +2877,67 @@ extern "C" int acb_streams_new(const acb_table *tb, int64_t n_streams, int long_
     return ACB_OK;
 }
 
-/* the device feed; d_count is zeroed here, on `s` */
+extern "C" int acb_streams_new(const acb_table *tb, int64_t n_streams, int long_mode, acb_streams **out) {
+    if (out) *out = nullptr;
+    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
+    return streams_new(tb, n_streams, long_mode, out);
+}
+
+/* A folded find_all feed's scan and seam walk (DESIGN section 4.18): the chunks folded once -- in place when `in_place`
+ * (the host feed's upload, the library's own copy), else into ss->d_fold -- then the scan and the seam kernel over the
+ * folded copy, so the staged tails hold folded letters (a find_all tail is only walked, never output).  Without aliases
+ * the records go to p's buffer as in the plain feed.  With aliases they go to ss->d_full, grown until the full list
+ * fits (one wait for its size), and are expanded into p's buffer, *p.count = the expanded total: the commit's fit test
+ * then sees what the caller receives. */
+static int streams_scan_folded(acb_streams *ss, acb_table *tb, ScanParams &p, StreamsArgs &a, bool in_place, unsigned grid,
+                               cudaStream_t s, int algo) {
+    int rc;
+    const long long total = p.total;
+    /* acb_scan_device's checks, before the fold: the plain feed gets the same refusals through it */
+    if ((rc = check_scan_shape(tb, total, reinterpret_cast<const int64_t *>(p.offsets), p.n_hay, p.stride_bytes))) return rc;
+    uint8_t *folded = const_cast<uint8_t *>(p.hay);
+    if (!in_place) {
+        if ((rc = ensure(&ss->d_fold, &ss->fold_cap, (size_t)total + 64))) return rc;
+        folded = ss->d_fold;
+    }
+    if ((rc = timing_mark(&tb->f_ev[0], s)) || (rc = fold_text(tb, p.hay, folded, total, s)) || (rc = timing_mark(&tb->f_ev[1], s)) ||
+        (rc = timing_ms(tb->f_ev[0], tb->f_ev[1], &g_fold_ms[0])))
+        return rc;
+    ScanParams q = p;
+    q.hay = folded;
+    if (ss->T > 0) {
+        if ((rc = ensure(&ss->d_next_tail, &ss->next_tail_cap, (size_t)p.n_hay * ss->T * ss->L))) return rc;
+        a.next_tail = ss->d_next_tail;
+    }
+    for (;;) {
+        if (tb->n_alias) {
+            size_t fcap = std::max<size_t>(ss->full_cap, 4096);
+            if ((rc = ensure(&ss->d_full, &ss->full_cap, fcap))) return rc;
+            q.out = ss->d_full;
+            q.cap = (long long)std::min<size_t>(ss->full_cap, 0x7fffffffULL);
+            q.count = ss->d_ctr;
+            CUDA_TRY(cudaMemsetAsync(ss->d_ctr, 0, sizeof(unsigned long long), s));
+        }
+        if (tb->n_keys > 0 && (rc = scan_text(tb, q, total, p.n_hay, algo, s))) return rc;
+        if (ss->T > 0) {
+            acb_seam_kernel<<<grid, kDfaThreads, 0, s>>>(q, a);
+            if ((rc = launched("seam kernel"))) return rc;
+        }
+        if (!tb->n_alias) return ACB_OK;
+        CUDA_TRY(cudaMemcpyAsync(ss->h_ctr, ss->d_ctr, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (ss->h_ctr[0] <= (unsigned long long)q.cap) break;
+        if (ss->h_ctr[0] > 0x7fffffffULL) { acb_set_error("more than 2^31-1 matches in one feed"); return ACB_ERANGE; }
+        if ((rc = ensure(&ss->d_full, &ss->full_cap, (size_t)ss->h_ctr[0]))) return rc;
+    }
+    return acb_expand_aliases_device(tb, ss->d_full, (int64_t)ss->h_ctr[0], p.out, p.cap, reinterpret_cast<int64_t *>(p.count), s);
+}
+
+/* the device feed; d_count is zeroed here, on `s`.  in_place: d_chunks is the library's own upload (a folded batch may
+ * fold it in place) */
 static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total, const int64_t *d_off,
                         int64_t n_chunks, int64_t stride, const int32_t *d_ids, acb_match *d_out, int64_t cap,
-                        int64_t *d_count, cudaStream_t s, int algo) {
+                        int64_t *d_count, cudaStream_t s, int algo, bool in_place = false) {
     if (!ss || !tb || !d_count || total < 0 || n_chunks < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (ss->leftmost) { acb_set_error("a leftmost-longest stream batch takes acb_streams_feed_leftmost_* or acb_streams_replace_*"); return ACB_EINVAL; }
     if (ss->words) { acb_set_error("a whole-word stream batch takes acb_streams_feed_words_*"); return ACB_EINVAL; }
@@ -2872,6 +2952,7 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
     }
     CUDA_TRY(cudaSetDevice(ss->device));
     CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
+    if (ss->fold) g_fold_ms[0] = g_fold_ms[1] = 0.f;
     if (total == 0 || n_chunks == 0) return ACB_OK;              /* empty chunks move no stream */
     if (reinterpret_cast<uintptr_t>(d_chunks) & 15) { acb_set_error("d_chunks must be 16-byte aligned"); return ACB_EINVAL; }
     ScanParams p;
@@ -2903,6 +2984,8 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
             if ((rc = launched("seam kernel"))) return rc;
         }
         if ((rc = launch_remap(tb, meta, d_off, stride, d_out, cap, d_count, s))) return rc;
+    } else if (ss->fold) {
+        if ((rc = streams_scan_folded(ss, tb, p, a, in_place, grid, s, algo))) return rc;
     } else {
         if (tb->n_keys > 0 && (rc = acb_scan_device(tb, d_chunks, total, d_off, n_chunks, stride, d_out, cap, d_count, s, algo))) return rc;
         if (ss->T > 0) {
@@ -2959,6 +3042,7 @@ extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8
     if (ids && (rc = check_ids(ss, ids, n_chunks))) return rc;
     if ((rc = streams_check_table(ss, tb))) return rc;
     if (n_chunks > ss->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, ss->n); return ACB_EINVAL; }
+    if (ss->fold) g_fold_ms[0] = g_fold_ms[1] = 0.f;
     if (total_bytes == 0 || n_chunks == 0) return ACB_OK;
     const int64_t *d_off = nullptr;
     if ((rc = upload_batch(tb, chunks, total_bytes, offsets, n_chunks, &d_off)) || (rc = upload_ids(ss, ids, n_chunks, tb->stream)) ||
@@ -2966,7 +3050,7 @@ extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8
         return rc;
     cudaStream_t s = tb->stream;
     if ((rc = streams_feed(ss, tb, tb->w_hay, total_bytes, d_off, n_chunks, stride_bytes, ids ? ss->d_ids : nullptr, tb->w_out, cap,
-                           reinterpret_cast<int64_t *>(tb->w_count), s, algo)))
+                           reinterpret_cast<int64_t *>(tb->w_count), s, algo, true)))
         return rc;
     return read_back(tb, tb->w_count, tb->w_out, cap, sort, n_chunks, (offsets ? total_bytes : stride_bytes) / tb->L, out, n_found, s);
 }
@@ -4634,17 +4718,23 @@ __global__ void acb_sw_left_kernel(const __grid_constant__ SwArgs w, const unsig
 }
 } // namespace
 
-extern "C" int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out) {
+/* the feed counters d_ctr (device) and h_ctr (pinned) */
+static cudaError_t streams_alloc_counters(acb_streams *ss) {
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ss->d_ctr), 4 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void **>(&ss->h_ctr), 4 * sizeof(unsigned long long));
+    return e;
+}
+
+static int streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out) {
     if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
-    int rc = acb_streams_new(tb, n_streams, 0, out);
+    int rc = streams_new(tb, n_streams, 0, out);
     if (rc != ACB_OK) return rc;
     acb_streams *ss = *out;
     ss->leftmost = 1;
     const size_t n = (size_t)std::max<int64_t>(n_streams, 1);
     cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&ss->d_hold), n * sizeof(long long));
     if (e == cudaSuccess) e = cudaMemset(ss->d_hold, 0, n * sizeof(long long));
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&ss->d_ctr), 4 * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void **>(&ss->h_ctr), 4 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = streams_alloc_counters(ss);
     if (e != cudaSuccess) {
         acb_set_error("allocating %lld streams: %s", (long long)n_streams, cudaGetErrorString(e));
         acb_streams_free(ss);
@@ -4654,12 +4744,18 @@ extern "C" int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, 
     return ACB_OK;
 }
 
-extern "C" int acb_streams_new_words(const acb_table *tb, int64_t n_streams, int leftmost, const uint32_t *bits, int64_t n_bits,
-                                     acb_streams **out) {
+extern "C" int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out) {
+    if (out) *out = nullptr;
+    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
+    return streams_new_leftmost(tb, n_streams, out);
+}
+
+static int streams_new_words(const acb_table *tb, int64_t n_streams, int leftmost, const uint32_t *bits, int64_t n_bits,
+                             acb_streams **out) {
     if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
     int rc = check_words(tb, bits, n_bits);
-    if (rc != ACB_OK || (rc = acb_streams_new_leftmost(tb, n_streams, out))) return rc;
+    if (rc != ACB_OK || (rc = streams_new_leftmost(tb, n_streams, out))) return rc;
     acb_streams *ss = *out;
     ss->leftmost = leftmost ? 1 : 0;
     ss->words = 1;
@@ -4681,15 +4777,50 @@ extern "C" int acb_streams_new_words(const acb_table *tb, int64_t n_streams, int
     return ACB_OK;
 }
 
-extern "C" int acb_streams_new_leftmost_kind(const acb_table *tb, int64_t n_streams, int kind, const uint32_t *bits, int64_t n_bits,
-                                             acb_streams **out) {
+extern "C" int acb_streams_new_words(const acb_table *tb, int64_t n_streams, int leftmost, const uint32_t *bits, int64_t n_bits,
+                                     acb_streams **out) {
+    if (out) *out = nullptr;
+    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
+    return streams_new_words(tb, n_streams, leftmost, bits, n_bits, out);
+}
+
+/* a leftmost batch of selection `kind` (leftmost = 1) or a find_all batch (leftmost = 0), whole-word unless n_bits < 0
+ * without a bitmap; of the table's kind, folded or not */
+static int streams_new_kind(const acb_table *tb, int64_t n_streams, int leftmost, int kind, const uint32_t *bits, int64_t n_bits,
+                            acb_streams **out) {
     if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
     if (!select_kind_ok(kind)) return ACB_EINVAL;
     const bool words = n_bits >= 0 || bits;                 /* n_bits < 0 without a bitmap: no word filter */
-    int rc = words ? acb_streams_new_words(tb, n_streams, 1, bits, n_bits, out) : acb_streams_new_leftmost(tb, n_streams, out);
+    int rc;
+    if (words) rc = streams_new_words(tb, n_streams, leftmost, bits, n_bits, out);
+    else if (leftmost) rc = streams_new_leftmost(tb, n_streams, out);
+    else if ((rc = streams_new(tb, n_streams, 0, out)) == ACB_OK && tb->fold) {    /* a folded find_all feed counts its full list */
+        cudaError_t e = streams_alloc_counters(*out);
+        if (e != cudaSuccess) {
+            acb_set_error("allocating %lld streams: %s", (long long)n_streams, cudaGetErrorString(e));
+            acb_streams_free(*out);
+            *out = nullptr;
+            return ACB_ECUDA;
+        }
+    }
     if (rc == ACB_OK) (*out)->kind = kind;
     return rc;
+}
+
+extern "C" int acb_streams_new_leftmost_kind(const acb_table *tb, int64_t n_streams, int kind, const uint32_t *bits, int64_t n_bits,
+                                             acb_streams **out) {
+    if (out) *out = nullptr;
+    if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
+    return streams_new_kind(tb, n_streams, 1, kind, bits, n_bits, out);
+}
+
+extern "C" int acb_streams_new_folded(const acb_table *tb, int64_t n_streams, int leftmost, int kind, const uint32_t *bits, int64_t n_bits,
+                                      acb_streams **out) {
+    if (!tb || !out || (leftmost != 0 && leftmost != 1)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    if (!tb->fold) { acb_set_error("acb_streams_new_folded takes a case-folded table (acb_table_upload_folded)"); return ACB_EINVAL; }
+    return streams_new_kind(tb, n_streams, leftmost, kind, bits, n_bits, out);
 }
 
 extern "C" int acb_last_stream_leftmost_ms(float *ms, int32_t n) {
@@ -4767,20 +4898,46 @@ static int sw_flags(acb_streams *ss, acb_table *tb, const SlArgs &a, long long f
     return launched("stream word flags");
 }
 
-/* a find_all word feed's m kept records (ss->d_settled, staged coordinates) in the reference order -- chunk, end, longest
- * key first -- and rebased to their chunks into d_out (the first cap of them); *d_count = m */
+/* A folded word feed's m kept records (ss->d_settled) with every alias of their key added, into ss->d_full, grown until
+ * they fit (one wait for their number, counted in d_ctr[2]); *m becomes that number */
+static int sw_expand(acb_streams *ss, acb_table *tb, unsigned long long *m, cudaStream_t s) {
+    int rc = ensure(&ss->d_full, &ss->full_cap, (size_t)*m);
+    for (; rc == ACB_OK;) {
+        const int64_t cap = (int64_t)std::min<size_t>(ss->full_cap, 0x7fffffffULL);
+        if ((rc = acb_expand_aliases_device(tb, ss->d_settled, (int64_t)*m, ss->d_full, cap, reinterpret_cast<int64_t *>(ss->d_ctr + 2), s)))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(ss->h_ctr + 2, ss->d_ctr + 2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (ss->h_ctr[2] <= (unsigned long long)cap) break;
+        if (ss->h_ctr[2] > 0x7fffffffULL) { acb_set_error("more than 2^31-1 matches in one feed"); return ACB_ERANGE; }
+        rc = ensure(&ss->d_full, &ss->full_cap, (size_t)ss->h_ctr[2]);
+    }
+    if (rc != ACB_OK) return rc;
+    *m = ss->h_ctr[2];
+    return ensure(&ss->d_settled, &ss->settled_cap, (size_t)*m);        /* the sort's second buffer */
+}
+
+/* a find_all word feed's m kept records (ss->d_settled, staged coordinates; on a folded table with aliases, expanded
+ * first) in the reference order -- chunk, end, longest key first, a group of case variants in ascending id (the sort is
+ * stable) -- and rebased to their chunks into d_out (the first cap of them); *d_count = their number */
 static int sw_order(acb_streams *ss, acb_table *tb, const SlArgs &a, unsigned long long m, long long staged, acb_match *d_out,
                     int64_t cap, unsigned long long *d_count, cudaStream_t s) {
     if (m == 0) return ACB_OK;                             /* *d_count is 0 already */
+    acb_match *in = ss->d_settled, *mid = ss->d_full;
+    int rc;
+    if (tb->n_alias) {
+        if ((rc = sw_expand(ss, tb, &m, s))) return rc;
+        in = ss->d_full;
+        mid = ss->d_settled;
+    }
     const SortKey k = sort_key(tb, a.n, staged / a.L);
-    int rc = ensure(&ss->d_keys, &ss->keys_cap, 2 * (size_t)m);
-    if (rc) return rc;
+    if ((rc = ensure(&ss->d_keys, &ss->keys_cap, 2 * (size_t)m))) return rc;
     unsigned long long *k0 = ss->d_keys, *k1 = ss->d_keys + m;
     size_t temp = 0;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, temp, k0, k1, ss->d_settled, ss->d_full, (int)m, 0, 64, s));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, temp, k0, k1, in, mid, (int)m, 0, 64, s));
     if ((rc = ensure(&ss->d_tmp, &ss->tmp_cap, temp))) return rc;
-    acb_match *sorted = k.bits() <= 64 ? ss->d_full : ss->d_settled;      /* two passes go through d_full */
-    if ((rc = sort_records<kKeyEnd, kKeyEndLow>(tb, k, ss->d_settled, ss->d_full, sorted, (long long)m, k0, k1, ss->d_tmp, ss->tmp_cap, s,
+    acb_match *sorted = k.bits() <= 64 ? mid : in;          /* two passes go through mid */
+    if ((rc = sort_records<kKeyEnd, kKeyEndLow>(tb, k, in, mid, sorted, (long long)m, k0, k1, ss->d_tmp, ss->tmp_cap, s,
                                   "stream word sort key")))
         return rc;
     acb_sw_emit_kernel<<<blocks(tb, m), 256, 0, s>>>(a, sorted, (long long)m, d_out, cap, d_count);
@@ -4803,6 +4960,7 @@ static int sl_feed(acb_streams *ss, acb_table *tb, acb_replacer *r, const uint8_
                    int64_t *d_rout_off, uint8_t *d_rout, int64_t out_cap, int64_t *d_rtotal, cudaStream_t s, int algo) {
     int rc;
     for (float &v : g_sl_ms) v = 0.f;
+    if (ss->fold) g_fold_ms[0] = g_fold_ms[1] = 0.f;
     CUDA_TRY(cudaSetDevice(ss->device));
     if (!r) CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), s));
     if (n == 0) {
