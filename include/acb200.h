@@ -657,7 +657,7 @@ int acb_table_upload_folded(const acb_trie *t, int device, const int32_t *alias_
  * one record), at d_out in d_in's order; *d_count is SET to their total and only records below index cap are stored.
  * d_in and d_out must not overlap.  A sort of the result by acb_sort_matches_device keeps the members of a group in
  * ascending id (the radix sort is stable).  The scratch space belongs to the table, as for acb_word_filter_device.
- * ACB_ERANGE for more than 2^31-1 records. */
+ * ACB_ERANGE for n >= 2^31-1 (its exclusive sum runs over n + 1 counts), before anything is allocated or launched. */
 int acb_expand_aliases_device(acb_table *tb, const acb_match *d_in, int64_t n, acb_match *d_out, int64_t cap, int64_t *d_count,
                               void *stream);
 

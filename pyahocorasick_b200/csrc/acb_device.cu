@@ -3905,7 +3905,8 @@ extern "C" int acb_expand_aliases_device(acb_table *tb, const acb_match *d_in, i
                                          int64_t *d_count, void *stream) {
     if (!tb || n < 0 || (n && !d_in) || cap < 0 || (cap > 0 && !d_out) || !d_count) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (!tb->fold) { acb_set_error("alias expansion needs a case-folded table (acb_table_upload_folded)"); return ACB_EINVAL; }
-    if (n > 0x7fffffffLL) { acb_set_error("more than 2^31-1 records to expand"); return ACB_ERANGE; }
+    /* the exclusive sum runs over n + 1 counts in an int */
+    if (n >= 0x7fffffffLL) { acb_set_error("more than 2^31-2 records to expand"); return ACB_ERANGE; }
     g_fold_ms[1] = 0.f;
     CUDA_TRY(cudaSetDevice(tb->device));
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
