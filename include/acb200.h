@@ -20,6 +20,9 @@
  *     its TRIE_LETTER_TYPE array (src/common.h:51-67).
  *   - the library never falls back to a CPU search: acb_scan_* fail with
  *     ACB_ECUDA when no device / kernel image is available.
+ *   - an entry point that runs on the device of its table, stream batch or replacer
+ *     leaves the calling thread's current CUDA device as it found it, on every
+ *     return path, errors included.
  */
 #ifndef ACB200_H_INCLUDED
 #define ACB200_H_INCLUDED

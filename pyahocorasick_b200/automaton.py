@@ -178,7 +178,8 @@ class _PinnedRecords:
 
 class Matches:
     """Result of a batch search: parallel int32 arrays in the reference's order
-    (hay_id, then end_index ascending, then longest key first)."""
+    (hay_id, then end_index ascending, then longest key first).  Its values are those of the key set at call time:
+    later changes of the automaton do not reach them (Automaton._result_values)."""
 
     __slots__ = ("hay_id", "end_index", "key_id", "_values")
 
@@ -253,6 +254,7 @@ class Automaton:
         self._key_ids: dict = {}          # key object -> key_id
         self._key_objs: list = []         # key_id -> key object (None once removed)
         self._values: list = []           # key_id -> value
+        self._values_shared = False       # a result reads _values later: copy it before changing an entry (_own_values)
         self._version = 0
         self._table = None                # acb_table* (device), created lazily
         self._table_device = None
@@ -399,6 +401,7 @@ class Automaton:
             self._values.append(value)
             self._version += 1                                  # :283-284
             return True
+        self._own_values()
         self._values[kid] = value                               # replaced, version unchanged (A10)
         return False
 
@@ -448,6 +451,7 @@ class Automaton:
         value = self._values[k]
         self._key_ids.pop(self._hashable(self._key_objs[k]), None)
         self._key_objs[k] = None
+        self._own_values()
         self._values[k] = None
         self._version += 1
         self._drop_table()
@@ -470,8 +474,22 @@ class Automaton:
         self._key_ids.clear()
         self._key_objs = []
         self._values = []
+        self._values_shared = False
         self._version += 1
         self._drop_table()
+
+    def _result_values(self):
+        """_values for a result that reads them after the call (Matches), taken under the lock of the scan: from then on
+        the list is copied before an entry of it changes (_own_values), so the result keeps the values of the key set it
+        was computed on.  Adding keys appends to the list and needs no copy."""
+        self._values_shared = True
+        return self._values
+
+    def _own_values(self):
+        """before an entry of _values changes in place: a fresh copy of the list when a result holds it"""
+        if self._values_shared:
+            self._values = list(self._values)
+            self._values_shared = False
 
     # keys / values / items (src/AutomatonItemsIter.c) -- host enumeration; keys_batch & co. run on the GPU
     def _select_args(self, args):
@@ -1069,6 +1087,7 @@ class Automaton:
                                  "make_automaton to convert the trie to an automaton.")
 
     # ------------------------------------------------------------------ search API of the reference
+    @_locked
     def iter(self, *args, **kwargs):
         """src/Automaton.c:875-966: iter(string, [start, [end]], ignore_white_space=False)."""
         self._require_automaton()
@@ -1119,6 +1138,7 @@ class Automaton:
                 callback(e + start, values[k])
         return None
 
+    @_locked
     def iter_long(self, *args):
         """src/Automaton.c:968-1040 + src/AutomatonSearchIterLong.c:89-153: iter_long(string, [start, [end]]) --
         longest, non-overlapping matches.  One GPU lane replays the reference's state machine per haystack."""
@@ -1138,6 +1158,7 @@ class Automaton:
         return self.find_all_batch(haystacks, algo="long", sort=sort, device=device, whole_words=whole_words,
                                    ascii_case_insensitive=ascii_case_insensitive)
 
+    @_locked
     def find_leftmost_longest_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
                                     whole_words=False, ascii_case_insensitive: bool = False) -> "Matches":
         """Leftmost-longest non-overlapping matches of a whole batch, selected on the GPU (input forms and result type
@@ -1171,8 +1192,9 @@ class Automaton:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, fold=True)
         else:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow)
-        return Matches(rec, self._values)
+        return Matches(rec, self._result_values())
 
+    @_locked
     def find_leftmost_first_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
                                   whole_words=False, ascii_case_insensitive: bool = False) -> "Matches":
         """Leftmost-first non-overlapping matches of a whole batch, selected on the GPU (input forms and result type of
@@ -1203,7 +1225,7 @@ class Automaton:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST, fold=True)
         else:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST)
-        return Matches(rec, self._values)
+        return Matches(rec, self._result_values())
 
     @_locked
     def _leftmost_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str,
@@ -1247,6 +1269,7 @@ class Automaton:
         N.check(fn(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap, cnt.data_ptr(), stream))
         return out, cnt, cap
 
+    @_locked
     def replacer(self, replacements=None, *, device: Optional[int] = None, leftmost_first: bool = False) -> "Replacer":
         """A `Replacer` that rewrites whole batches with the leftmost-longest matches replaced (Replacer.replace_batch);
         leftmost_first=True: the matches find_leftmost_first_batch chooses.
@@ -1273,6 +1296,7 @@ class Automaton:
         return nodes, edges, fail
 
     # ------------------------------------------------------------------ the batch entry (new)
+    @_locked
     def find_all_batch(self, haystacks, *, algo: str = "auto", sort: bool = True, device: Optional[int] = None,
                        ignore_white_space: bool = False, whole_words=False, ascii_case_insensitive: bool = False) -> Matches:
         """Search a whole batch on the GPU.
@@ -1327,7 +1351,7 @@ class Automaton:
             rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow, fold=True)
         else:
             rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow)
-        return Matches(rec, self._values)
+        return Matches(rec, self._result_values())
 
     def _batch_input(self, haystacks, narrow_ok: bool = True, required: bool = True) -> "_Batch":
         """The input forms of find_all_batch, checked and laid out for a scan (_Batch).  narrow: the buffer holds the
@@ -1413,6 +1437,7 @@ class Automaton:
         automata.  The returned StreamBatch has ``ascii_case_insensitive`` True."""
         return self._stream_batch(n_streams, False, algo, device, False, leftmost_longest, whole_words, leftmost_first, True)
 
+    @_locked
     def _stream_batch(self, n_streams: int, long: bool, algo: str, device: Optional[int], ignore_white_space: bool,
                       leftmost_longest: bool, whole_words, leftmost_first: bool, fold: bool) -> "StreamBatch":
         """The argument check and constructor of stream_batch and ascii_case_insensitive_stream_batch (fold)"""
@@ -1461,17 +1486,18 @@ class Automaton:
         KeyError of the first key that is missing."""
         if not isinstance(keys, (list, tuple, np.ndarray)) and not type(keys).__module__.startswith("torch"):
             keys = list(keys)                                   # an iterator: kept, for the KeyError
-        key_id, _, _ = self._lookup_batch(keys, device)
-        if not isinstance(key_id, np.ndarray):
-            key_id = key_id.cpu().numpy()                      # synchronises torch's current stream
-        values = self._values
-        if default is Automaton._MISSING:
-            miss = np.flatnonzero(key_id < 0)
-            if miss.size:
-                raise KeyError(self._batch_key(keys, int(miss[0])))
-        else:
-            values = values + [default]                         # key_id -1 picks it
-        return list(map(values.__getitem__, key_id.tolist()))
+        with self._gpu_lock:                                    # the ids and the values of one key set
+            key_id, _, _ = self._lookup_batch(keys, device)
+            if not isinstance(key_id, np.ndarray):
+                key_id = key_id.cpu().numpy()                  # synchronises torch's current stream
+            values = self._values
+            if default is Automaton._MISSING:
+                miss = np.flatnonzero(key_id < 0)
+                if miss.size:
+                    raise KeyError(self._batch_key(keys, int(miss[0])))
+            else:
+                values = values + [default]                     # key_id -1 picks it
+            return list(map(values.__getitem__, key_id.tolist()))
 
     @_locked
     def _lookup_batch(self, keys, device: Optional[int]):
@@ -1533,18 +1559,21 @@ class Automaton:
     # the full table, as the lookups do: the latin-1 table lacks the nodes of keys that are not latin-1.
     def keys_batch(self, patterns, wildcard=None, how=MATCH_EXACT_LENGTH, *, device: Optional[int] = None) -> list:
         """``[list(A.keys(p, wildcard, how)) for p in patterns]``, read when the call returns."""
-        ko = self._key_objs
-        return [list(map(ko.__getitem__, ids)) for ids in self._select_lists(patterns, wildcard, how, device)]
+        with self._gpu_lock:                                    # the ids and the keys of one key set
+            ko = self._key_objs
+            return [list(map(ko.__getitem__, ids)) for ids in self._select_lists(patterns, wildcard, how, device)]
 
     def values_batch(self, patterns, wildcard=None, how=MATCH_EXACT_LENGTH, *, device: Optional[int] = None) -> list:
         """``[list(A.values(p, wildcard, how)) for p in patterns]``, read when the call returns."""
-        vals = self._values
-        return [list(map(vals.__getitem__, ids)) for ids in self._select_lists(patterns, wildcard, how, device)]
+        with self._gpu_lock:
+            vals = self._values
+            return [list(map(vals.__getitem__, ids)) for ids in self._select_lists(patterns, wildcard, how, device)]
 
     def items_batch(self, patterns, wildcard=None, how=MATCH_EXACT_LENGTH, *, device: Optional[int] = None) -> list:
         """``[list(A.items(p, wildcard, how)) for p in patterns]``, read when the call returns."""
-        ko, vals = self._key_objs, self._values
-        return [[(ko[k], vals[k]) for k in ids] for ids in self._select_lists(patterns, wildcard, how, device)]
+        with self._gpu_lock:
+            ko, vals = self._key_objs, self._values
+            return [[(ko[k], vals[k]) for k in ids] for ids in self._select_lists(patterns, wildcard, how, device)]
 
     def _select_lists(self, patterns, wildcard, how, device):
         """the key ids of every pattern, as lists"""
@@ -1828,7 +1857,7 @@ class StreamBatch(_Streams):
         """A feed's records (hay_id = chunk index, end_index in the chunk) -> (Matches with stream ids and positions in
         the whole stream, the stream of every chunk)"""
         sid = np.arange(n, dtype=np.int64) if ids32 is None else ids32.astype(np.int64)
-        m = Matches(rec, self._A._values)
+        m = Matches(rec, self._A._result_values())
         m.hay_id = sid[rec["hay_id"]]
         m.end_index = rec["end_index"].astype(np.int64) + self._pos[m.hay_id]
         return m, sid
@@ -2001,17 +2030,18 @@ class Replacer:
     def _stream_batch(self, n_streams: int, algo: str, device: Optional[int], whole_words, fold: bool) -> "ReplaceStream":
         """The argument check and constructor of stream_batch and ascii_case_insensitive_stream_batch (fold)"""
         A = self._A
-        if self._version != A._version:
-            raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
-        A._require_automaton()
-        A._fold_arg(fold)
-        n_streams = operator.index(n_streams)
-        if n_streams < 0:
-            raise ValueError("n_streams must not be negative")
-        if algo not in ("auto", "filter", "dfa"):
-            raise ValueError(f"algo {algo!r}: a replacing stream batch takes 'auto', 'filter' or 'dfa'")
-        words = A._words(whole_words)
-        return ReplaceStream(self, n_streams, algo, self._device if device is None else device, words, fold)
+        with A._gpu_lock:
+            if self._version != A._version:
+                raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
+            A._require_automaton()
+            A._fold_arg(fold)
+            n_streams = operator.index(n_streams)
+            if n_streams < 0:
+                raise ValueError("n_streams must not be negative")
+            if algo not in ("auto", "filter", "dfa"):
+                raise ValueError(f"algo {algo!r}: a replacing stream batch takes 'auto', 'filter' or 'dfa'")
+            words = A._words(whole_words)
+            return ReplaceStream(self, n_streams, algo, self._device if device is None else device, words, fold)
 
     def _items(self, out: np.ndarray, offs: np.ndarray, narrow: bool) -> list:
         """the output haystacks as objects of the input's type"""

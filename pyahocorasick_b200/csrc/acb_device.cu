@@ -1410,6 +1410,22 @@ struct acb_table {
     cudaEvent_t f_ev[4] = {};                            /* kernel timing of the fold and of the expansion */
 };
 
+/* The calling thread's current device, saved when an exported entry point starts and made current again on every return
+ * path.  Entry points switch to the device of their table, stream batch or replacer (cudaSetDevice); without this the
+ * caller's next CUDA work -- its own allocations, or the next call that reads the current device -- would land there.
+ * An entry point that calls another one after switching gets the switched device back from it. */
+class DeviceRestore {
+    int prev_ = -1;
+public:
+    DeviceRestore() { if (cudaGetDevice(&prev_) != cudaSuccess) prev_ = -1; }
+    ~DeviceRestore() {
+        int cur = -1;
+        if (prev_ >= 0 && cudaGetDevice(&cur) == cudaSuccess && cur != prev_) cudaSetDevice(prev_);
+    }
+    DeviceRestore(const DeviceRestore &) = delete;
+    DeviceRestore &operator=(const DeviceRestore &) = delete;
+};
+
 extern "C" int acb_device_count(int32_t *n) {
     int c = 0;
     cudaError_t e = cudaGetDeviceCount(&c);
@@ -1430,6 +1446,7 @@ static int upload(T **dst, const T *src, size_t n, long long &acc) {
 }
 
 extern "C" void acb_table_free(acb_table *tb) {
+    DeviceRestore keep_device;
     if (!tb) return;
     cudaSetDevice(tb->device);
     cudaFree(tb->d_lfail); cudaFree(tb->d_cls); cudaFree(tb->d_goto); cudaFree(tb->d_fail); cudaFree(tb->d_keyof);
@@ -1466,6 +1483,7 @@ extern "C" void acb_table_free(acb_table *tb) {
 }
 
 extern "C" int acb_table_upload(const acb_trie *t, int device, acb_table **out) {
+    DeviceRestore keep_device;
     if (!t || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
     acb_flat_view f;
@@ -1618,18 +1636,33 @@ static int refuse_folded(const acb_table *tb, const char *what) {
 
 constexpr int kMaxDevices = 64;                              /* opt-in caches below are per device */
 
+/* Opts the current device's kernels into `smem` bytes of dynamic shared memory once: `opted` is the largest size they were
+ * set to so far (per instantiation and device) and only grows.  Check, set and store happen under one lock, so the cache
+ * is never ahead of the attribute: two threads that opt in to sizes a < b at once otherwise can leave the cache at b and
+ * the attribute at a, and every later launch that needs b fails.  The load before the lock keeps the common path free. */
+template <class SetAll>
+static int opt_in_smem(std::atomic<size_t> &opted, size_t smem, SetAll &&set_all) {
+    if (opted.load(std::memory_order_acquire) >= smem) return ACB_OK;
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lk(mu);
+    if (opted.load(std::memory_order_relaxed) >= smem) return ACB_OK;
+    int rc = set_all(smem);
+    if (rc == ACB_OK) opted.store(smem, std::memory_order_release);
+    return rc;
+}
+
 template <int NW, int STRIDE, int MODE>
 static int launch_stream_m(const ScanParams &p, int grid, cudaStream_t s) {
     auto kern = acb_stream_kernel<NW, STRIDE, MODE>;
     const size_t smem = stream_smem(p.log1).total;
-    static std::atomic<size_t> opted_dev[kMaxDevices];       /* per instantiation and device: the largest size opted into so far */
+    static std::atomic<size_t> opted_dev[kMaxDevices];
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));                           /* the attribute belongs to the current device's context */
-    std::atomic<size_t> &opted = opted_dev[dev % kMaxDevices];
-    if (opted.load(std::memory_order_relaxed) < smem) {
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        opted.store(smem, std::memory_order_relaxed);
-    }
+    int rc = opt_in_smem(opted_dev[dev % kMaxDevices], smem, [&](size_t n) {
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n));
+        return ACB_OK;
+    });
+    if (rc != ACB_OK) return rc;
     kern<<<grid, kFThreads, smem, s>>>(p);
     return launched("stream kernel");
 }
@@ -1639,12 +1672,12 @@ static int launch_pair(const ScanParams &p, int grid, cudaStream_t s) {
     static std::atomic<size_t> opted_dev[kMaxDevices];
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
-    std::atomic<size_t> &opted = opted_dev[dev % kMaxDevices];
-    if (opted.load(std::memory_order_relaxed) < smem) {
-        CUDA_TRY(cudaFuncSetAttribute(acb_pair_kernel<17>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(acb_pair_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        opted.store(smem, std::memory_order_relaxed);
-    }
+    int rc = opt_in_smem(opted_dev[dev % kMaxDevices], smem, [](size_t n) {
+        CUDA_TRY(cudaFuncSetAttribute(acb_pair_kernel<17>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n));
+        CUDA_TRY(cudaFuncSetAttribute(acb_pair_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n));
+        return ACB_OK;
+    });
+    if (rc != ACB_OK) return rc;
     if (p.log2b == 17) acb_pair_kernel<17><<<grid, kPairThreads, smem, s>>>(p);      /* the 2^20-bit level 1 of 10 k keys and more */
     else acb_pair_kernel<0><<<grid, kPairThreads, smem, s>>>(p);
     return launched("pair kernel");
@@ -1793,6 +1826,7 @@ static int fold_text(const acb_table *tb, const uint8_t *in, uint8_t *out, long 
 
 extern "C" int acb_table_upload_folded(const acb_trie *t, int device, const int32_t *alias_ptr, const int32_t *alias_ids,
                                        int64_t n_alias, acb_table **out) {
+    DeviceRestore keep_device;
     if (!t || !out || n_alias < 0 || (n_alias && (!alias_ptr || !alias_ids))) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
     acb_flat_view f;
@@ -1823,6 +1857,11 @@ extern "C" int acb_table_upload_folded(const acb_trie *t, int device, const int3
     tb->n_alias = n_alias;
     do {
         if (!n_alias) break;
+        if (cudaSetDevice(device) != cudaSuccess) {        /* acb_table_upload gave the caller's device back */
+            acb_set_error("cudaSetDevice(%d) failed", device);
+            rc = ACB_ECUDA;
+            break;
+        }
         try {                                              /* an alias has its representative's length */
             tb->key_len.resize((size_t)max_id + 1, 0);
             for (int32_t k = 0; k < f.n_keys; k++)
@@ -1905,6 +1944,7 @@ static int check_scan_shape(const acb_table *tb, int64_t total_bytes, const int6
 extern "C" int acb_scan_device(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes,
                                const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
                                acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    DeviceRestore keep_device;
     if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (algo == ACB_ALGO_LONG && refuse_folded(tb, "ACB_ALGO_LONG")) return ACB_EINVAL;
     if (int rc = check_scan_shape(tb, total_bytes, d_offsets, n_hay, stride_bytes)) return rc;
@@ -1944,6 +1984,7 @@ extern "C" int acb_table_set_long_state(acb_table *tb, int32_t state) {
 }
 
 extern "C" int acb_table_get_long_state(acb_table *tb, int32_t *state) {
+    DeviceRestore keep_device;
     if (!tb || !state) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *state = 0;
     if (tb->long_final_host >= 0) { *state = tb->long_final_host; return ACB_OK; }
@@ -2110,6 +2151,7 @@ static size_t sort_scratch_bytes(int64_t n, int bits, cudaStream_t s, size_t *te
 
 extern "C" int acb_sort_matches_device(acb_table *tb, acb_match *d_records, int64_t n, int64_t n_hay,
                                        int64_t max_hay_letters, void *stream) {
+    DeviceRestore keep_device;
     if (!tb || n < 0 || (n && !d_records)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (n <= 1) return ACB_OK;
     /* before any allocation: scratch for this many records may not exist, and the caller sorts on the host on ERANGE */
@@ -2332,6 +2374,7 @@ static int scan_host_full(acb_table *tb, const uint8_t *hay, int64_t total_bytes
 extern "C" int acb_scan_host(acb_table *tb, const uint8_t *hay, int64_t total_bytes,
                              const int64_t *offsets, int64_t n_hay, int64_t stride_bytes,
                              acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort) {
+    DeviceRestore keep_device;
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (algo == ACB_ALGO_LONG && refuse_folded(tb, "ACB_ALGO_LONG")) return ACB_EINVAL;
     if (tb->n_alias)                                             /* the full list, expanded; not pipelined */
@@ -2614,6 +2657,7 @@ extern "C" int acb_scan_device_skip(acb_table *tb, const uint8_t *d_hay, int64_t
                                     const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
                                     acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo,
                                     const uint32_t *skip, int64_t n_skip) {
+    DeviceRestore keep_device;
     if (!tb || !d_count || total_bytes < 0 || n_hay < 0 || cap < 0 || (cap > 0 && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (refuse_folded(tb, "a white-space scan")) return ACB_EINVAL;
     int rc = check_skip(skip, n_skip, algo);
@@ -2639,6 +2683,7 @@ extern "C" int acb_scan_host_skip(acb_table *tb, const uint8_t *hay, int64_t tot
                                   const int64_t *offsets, int64_t n_hay, int64_t stride_bytes,
                                   acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort,
                                   const uint32_t *skip, int64_t n_skip) {
+    DeviceRestore keep_device;
     if (!tb || !n_found || total_bytes < 0 || n_hay < 0 || cap < 0 || (total_bytes && !hay)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (refuse_folded(tb, "a white-space scan")) return ACB_EINVAL;
     *n_found = 0;
@@ -2839,6 +2884,7 @@ static StreamsArgs streams_args(const acb_streams *ss, const int32_t *d_ids) {
 }
 
 extern "C" void acb_streams_free(acb_streams *ss) {
+    DeviceRestore keep_device;
     if (!ss) return;
     cudaSetDevice(ss->device);
     cudaFree(ss->d_pos); cudaFree(ss->d_tail); cudaFree(ss->d_state); cudaFree(ss->d_next_tail);
@@ -2878,6 +2924,7 @@ static int streams_new(const acb_table *tb, int64_t n_streams, int long_mode, ac
 }
 
 extern "C" int acb_streams_new(const acb_table *tb, int64_t n_streams, int long_mode, acb_streams **out) {
+    DeviceRestore keep_device;
     if (out) *out = nullptr;
     if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
     return streams_new(tb, n_streams, long_mode, out);
@@ -3006,6 +3053,7 @@ static int streams_feed(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks,
 extern "C" int acb_streams_feed_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
                                        const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
                                        acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    DeviceRestore keep_device;
     return streams_feed(ss, tb, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, d_out, cap, d_count,
                         reinterpret_cast<cudaStream_t>(stream), algo);
 }
@@ -3033,6 +3081,7 @@ static int upload_ids(acb_streams *ss, const int32_t *ids, int64_t n, cudaStream
 extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
                                      const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids,
                                      acb_match *out, int64_t cap, int64_t *n_found, int algo, int sort) {
+    DeviceRestore keep_device;
     if (!ss || !tb || !n_found || total_bytes < 0 || n_chunks < 0 || cap < 0 || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *n_found = 0;
     tb->h_out_n = 0;
@@ -3056,6 +3105,7 @@ extern "C" int acb_streams_feed_host(acb_streams *ss, acb_table *tb, const uint8
 }
 
 extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n) {
+    DeviceRestore keep_device;
     if (!ss || n < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
     int rc;
     if (ids && (rc = check_ids(ss, ids, n))) return rc;
@@ -3084,6 +3134,7 @@ extern "C" int acb_streams_reset(acb_streams *ss, const int32_t *ids, int64_t n)
 }
 
 extern "C" int acb_streams_positions(acb_streams *ss, int64_t *out, int64_t cap) {
+    DeviceRestore keep_device;
     if (!ss || cap < ss->n || (ss->n && !out)) { acb_set_error("bad argument (capacity %lld for %lld streams)", (long long)cap, ss ? ss->n : 0LL); return ACB_EINVAL; }
     CUDA_TRY(cudaSetDevice(ss->device));
     CUDA_TRY(cudaDeviceSynchronize());
@@ -3092,10 +3143,12 @@ extern "C" int acb_streams_positions(acb_streams *ss, int64_t *out, int64_t cap)
 }
 
 extern "C" int acb_streams_new_skip(const acb_table *tb, int64_t n_streams, const uint32_t *skip, int64_t n_skip, acb_streams **out) {
+    DeviceRestore keep_device;
     if (!tb || !out) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
     int rc = check_skip(skip, n_skip, ACB_ALGO_FILTER);
     if (rc != ACB_OK) return rc;
+    CUDA_TRY(cudaSetDevice(tb->device));                    /* for the allocation below: acb_streams_new restores it */
     if ((rc = acb_streams_new(tb, n_streams, 0, out))) return rc;
     acb_streams *ss = *out;
     const size_t n = (size_t)std::max<int64_t>(n_streams, 1);
@@ -3168,6 +3221,7 @@ __global__ void __launch_bounds__(kLookupThreads) acb_lookup_kernel(const __grid
 
 extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t total_bytes, const int64_t *d_offsets,
                                  int64_t n_keys, int64_t stride_bytes, int32_t *d_key_id, int32_t *d_prefix, void *stream) {
+    DeviceRestore keep_device;
     if (refuse_folded(tb, "a lookup")) return ACB_EINVAL;
     if (!tb || total_bytes < 0 || n_keys < 0 || (total_bytes && !d_keys) || (n_keys && (!d_key_id || !d_prefix))) {
         acb_set_error("bad argument");
@@ -3192,6 +3246,7 @@ extern "C" int acb_lookup_device(acb_table *tb, const uint8_t *d_keys, int64_t t
 
 extern "C" int acb_lookup_host(acb_table *tb, const uint8_t *keys, int64_t total_bytes, const int64_t *offsets,
                                int64_t n_keys, int64_t stride_bytes, int32_t *key_id, int32_t *prefix) {
+    DeviceRestore keep_device;
     if (refuse_folded(tb, "a lookup")) return ACB_EINVAL;
     if (!tb || total_bytes < 0 || n_keys < 0 || (total_bytes && !keys) || (n_keys && (!key_id || !prefix))) {
         acb_set_error("bad argument");
@@ -3335,6 +3390,7 @@ __global__ void __launch_bounds__(kSelectThreads) acb_select_kernel(const __grid
 } // namespace
 
 extern "C" int acb_table_upload_key_ranges(acb_table *tb, const acb_trie *t) {
+    DeviceRestore keep_device;
     if (!tb || !t) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (refuse_folded(tb, "a key selection")) return ACB_EINVAL;
     if (tb->d_order) return ACB_OK;
@@ -3439,6 +3495,7 @@ static int select_view_ok(const acb_table *tb) {
 extern "C" int acb_select_device(acb_table *tb, const uint8_t *d_patterns, int64_t total_bytes, const int64_t *d_offsets,
                                  int64_t n, int64_t stride_bytes, int64_t wildcard, int how, int64_t *d_out_offsets,
                                  int32_t *d_key_id, int64_t cap, int64_t *d_total, void *stream) {
+    DeviceRestore keep_device;
     int rc = select_common_checks(tb, d_patterns, total_bytes, n, d_out_offsets, d_key_id, cap, d_total, wildcard, how);
     if (rc != ACB_OK) return rc;
     if (!d_offsets && (rc = check_stride(tb->L, total_bytes, n, stride_bytes, 0))) return rc;
@@ -3456,6 +3513,7 @@ extern "C" int acb_select_device(acb_table *tb, const uint8_t *d_patterns, int64
 extern "C" int acb_select_host(acb_table *tb, const uint8_t *patterns, int64_t total_bytes, const int64_t *offsets,
                                int64_t n, int64_t stride_bytes, int64_t wildcard, int how, int64_t *out_offsets,
                                int32_t *key_id, int64_t cap, int64_t *total) {
+    DeviceRestore keep_device;
     int rc = select_common_checks(tb, patterns, total_bytes, n, out_offsets, key_id, cap, total, wildcard, how);
     if (rc != ACB_OK) return rc;
     if ((rc = offsets ? check_offsets(tb->L, offsets, n, total_bytes) : check_stride(tb->L, total_bytes, n, stride_bytes, 0))) return rc;
@@ -3728,12 +3786,14 @@ static int leftmost_select(acb_table *tb, int kind, const acb_match *d_records, 
 
 extern "C" int acb_leftmost_longest_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay,
                                            int64_t max_hay_letters, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+    DeviceRestore keep_device;
     return leftmost_select(tb, ACB_SELECT_LONGEST, d_records, n, n_hay, max_hay_letters, d_out, cap, d_count,
                            reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int acb_leftmost_first_device(acb_table *tb, const acb_match *d_records, int64_t n, int64_t n_hay,
                                          int64_t max_hay_letters, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+    DeviceRestore keep_device;
     return leftmost_select(tb, ACB_SELECT_FIRST, d_records, n, n_hay, max_hay_letters, d_out, cap, d_count,
                            reinterpret_cast<cudaStream_t>(stream));
 }
@@ -3821,6 +3881,7 @@ static int check_words(const acb_table *tb, const uint32_t *bits, int64_t n_bits
 extern "C" int acb_word_filter_device(acb_table *tb, const uint8_t *d_hay, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
                                       int64_t stride_bytes, const acb_match *d_records, int64_t n, const uint32_t *d_bits, int64_t n_bits,
                                       acb_match *d_out, int64_t cap, int64_t *d_count, void *stream) {
+    DeviceRestore keep_device;
     if (!tb || total_bytes < 0 || (total_bytes && !d_hay) || n_hay < 0 || n < 0 || (n && !d_records) || cap < 0 || (cap > 0 && !d_out) ||
         !d_count) {
         acb_set_error("bad argument");
@@ -3903,6 +3964,7 @@ __global__ void acb_xp_scatter_kernel(const __grid_constant__ XpArgs a, const lo
 
 extern "C" int acb_expand_aliases_device(acb_table *tb, const acb_match *d_in, int64_t n, acb_match *d_out, int64_t cap,
                                          int64_t *d_count, void *stream) {
+    DeviceRestore keep_device;
     if (!tb || n < 0 || (n && !d_in) || cap < 0 || (cap > 0 && !d_out) || !d_count) { acb_set_error("bad argument"); return ACB_EINVAL; }
     if (!tb->fold) { acb_set_error("alias expansion needs a case-folded table (acb_table_upload_folded)"); return ACB_EINVAL; }
     /* the exclusive sum runs over n + 1 counts in an int */
@@ -4033,6 +4095,7 @@ static int scan_host_full(acb_table *tb, const uint8_t *hay, int64_t total_bytes
 extern "C" int acb_scan_host_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
                                    int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap,
                                    int64_t *n_found, int algo, int sort) {
+    DeviceRestore keep_device;
     const WordSet ws{bits, n_bits};
     return scan_host_full(tb, hay, total_bytes, offsets, n_hay, stride_bytes, &ws, out, cap, n_found, algo, sort);
 }
@@ -4068,12 +4131,14 @@ static int scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_b
 
 extern "C" int acb_scan_host_leftmost(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
                                       int64_t stride_bytes, acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    DeviceRestore keep_device;
     return scan_host_leftmost(tb, hay, total_bytes, offsets, n_hay, stride_bytes, nullptr, out, cap, n_found, algo);
 }
 
 extern "C" int acb_scan_host_leftmost_words(acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets, int64_t n_hay,
                                             int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out, int64_t cap,
                                             int64_t *n_found, int algo) {
+    DeviceRestore keep_device;
     const WordSet ws{bits, n_bits};
     return scan_host_leftmost(tb, hay, total_bytes, offsets, n_hay, stride_bytes, &ws, out, cap, n_found, algo);
 }
@@ -4081,6 +4146,7 @@ extern "C" int acb_scan_host_leftmost_words(acb_table *tb, const uint8_t *hay, i
 extern "C" int acb_scan_host_leftmost_kind(acb_table *tb, int kind, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
                                            int64_t n_hay, int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, acb_match *out,
                                            int64_t cap, int64_t *n_found, int algo) {
+    DeviceRestore keep_device;
     const WordSet ws{bits, n_bits};
     const bool words = n_bits >= 0 || bits;                 /* n_bits < 0 without a bitmap: no word filter */
     return scan_host_leftmost(tb, hay, total_bytes, offsets, n_hay, stride_bytes, words ? &ws : nullptr, out, cap, n_found, algo, kind);
@@ -4264,6 +4330,7 @@ static int rp_fits(const acb_replacer *r, const acb_table *tb) {
 
 extern "C" int acb_replacer_new_kind(const acb_table *tb, int kind, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets,
                                      int64_t n_ids, acb_replacer **out) {
+    DeviceRestore keep_device;
     if (!tb || !out || rep_bytes < 0 || (rep_bytes && !rep) || !rep_offsets || n_ids < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
     if (!select_kind_ok(kind)) return ACB_EINVAL;
@@ -4290,10 +4357,12 @@ extern "C" int acb_replacer_new_kind(const acb_table *tb, int kind, const uint8_
 
 extern "C" int acb_replacer_new(const acb_table *tb, const uint8_t *rep, int64_t rep_bytes, const int64_t *rep_offsets,
                                 int64_t n_ids, acb_replacer **out) {
+    DeviceRestore keep_device;
     return acb_replacer_new_kind(tb, ACB_SELECT_LONGEST, rep, rep_bytes, rep_offsets, n_ids, out);
 }
 
 extern "C" void acb_replacer_free(acb_replacer *r) {
+    DeviceRestore keep_device;
     if (!r) return;
     cudaSetDevice(r->device);
     cudaFree(r->d_rep);
@@ -4380,6 +4449,7 @@ extern "C" int acb_replace_device(acb_replacer *r, acb_table *tb, const uint8_t 
                                   int64_t n_hay, int64_t stride_bytes, const acb_match *d_chosen, int64_t chosen_cap,
                                   const int64_t *d_n_chosen, int64_t *d_out_offsets, uint8_t *d_out, int64_t out_cap,
                                   int64_t *d_total, void *stream) {
+    DeviceRestore keep_device;
     int rc = rp_check(r, tb, total_bytes, n_hay, stride_bytes, d_offsets != nullptr, out_cap);
     if (rc) return rc;
     if ((total_bytes && !d_hay) || chosen_cap < 0 || (chosen_cap && !d_chosen) || !d_n_chosen || !d_out_offsets || !d_total ||
@@ -4451,12 +4521,14 @@ static int replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int6
 extern "C" int acb_replace_host(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
                                 int64_t n_hay, int64_t stride_bytes, int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap,
                                 int64_t *total) {
+    DeviceRestore keep_device;
     return replace_host(r, tb, hay, total_bytes, offsets, n_hay, stride_bytes, nullptr, algo, out_offsets, out, out_cap, total);
 }
 
 extern "C" int acb_replace_host_words(acb_replacer *r, acb_table *tb, const uint8_t *hay, int64_t total_bytes, const int64_t *offsets,
                                       int64_t n_hay, int64_t stride_bytes, const uint32_t *bits, int64_t n_bits, int algo, int64_t *out_offsets,
                                       uint8_t *out, int64_t out_cap, int64_t *total) {
+    DeviceRestore keep_device;
     const WordSet ws{bits, n_bits};
     return replace_host(r, tb, hay, total_bytes, offsets, n_hay, stride_bytes, &ws, algo, out_offsets, out, out_cap, total);
 }
@@ -4746,6 +4818,7 @@ static int streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_stre
 }
 
 extern "C" int acb_streams_new_leftmost(const acb_table *tb, int64_t n_streams, acb_streams **out) {
+    DeviceRestore keep_device;
     if (out) *out = nullptr;
     if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
     return streams_new_leftmost(tb, n_streams, out);
@@ -4780,6 +4853,7 @@ static int streams_new_words(const acb_table *tb, int64_t n_streams, int leftmos
 
 extern "C" int acb_streams_new_words(const acb_table *tb, int64_t n_streams, int leftmost, const uint32_t *bits, int64_t n_bits,
                                      acb_streams **out) {
+    DeviceRestore keep_device;
     if (out) *out = nullptr;
     if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
     return streams_new_words(tb, n_streams, leftmost, bits, n_bits, out);
@@ -4811,6 +4885,7 @@ static int streams_new_kind(const acb_table *tb, int64_t n_streams, int leftmost
 
 extern "C" int acb_streams_new_leftmost_kind(const acb_table *tb, int64_t n_streams, int kind, const uint32_t *bits, int64_t n_bits,
                                              acb_streams **out) {
+    DeviceRestore keep_device;
     if (out) *out = nullptr;
     if (refuse_folded(tb, "a stream batch")) return ACB_EINVAL;
     return streams_new_kind(tb, n_streams, 1, kind, bits, n_bits, out);
@@ -4818,6 +4893,7 @@ extern "C" int acb_streams_new_leftmost_kind(const acb_table *tb, int64_t n_stre
 
 extern "C" int acb_streams_new_folded(const acb_table *tb, int64_t n_streams, int leftmost, int kind, const uint32_t *bits, int64_t n_bits,
                                       acb_streams **out) {
+    DeviceRestore keep_device;
     if (!tb || !out || (leftmost != 0 && leftmost != 1)) { acb_set_error("bad argument"); return ACB_EINVAL; }
     *out = nullptr;
     if (!tb->fold) { acb_set_error("acb_streams_new_folded takes a case-folded table (acb_table_upload_folded)"); return ACB_EINVAL; }
@@ -5083,6 +5159,7 @@ static int sl_feed_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunk
 extern "C" int acb_streams_feed_leftmost_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
                                                 const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
                                                 int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    DeviceRestore keep_device;
     return sl_feed_device(ss, tb, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, d_out, cap, d_count, stream,
                           algo, false);
 }
@@ -5090,6 +5167,7 @@ extern "C" int acb_streams_feed_leftmost_device(acb_streams *ss, acb_table *tb, 
 extern "C" int acb_streams_feed_words_device(acb_streams *ss, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
                                              const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids,
                                              int final, acb_match *d_out, int64_t cap, int64_t *d_count, void *stream, int algo) {
+    DeviceRestore keep_device;
     return sl_feed_device(ss, tb, d_chunks, total_bytes, d_offsets, n_chunks, stride_bytes, d_ids, final, d_out, cap, d_count, stream,
                           algo, true);
 }
@@ -5097,6 +5175,7 @@ extern "C" int acb_streams_feed_words_device(acb_streams *ss, acb_table *tb, con
 extern "C" int acb_streams_replace_device(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *d_chunks, int64_t total_bytes,
                                           const int64_t *d_offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids, int final,
                                           int64_t *d_out_offsets, uint8_t *d_out, int64_t out_cap, int64_t *d_total, void *stream, int algo) {
+    DeviceRestore keep_device;
     int rc = sl_check(ss, tb, total_bytes, d_offsets, n_chunks, stride_bytes, &algo);
     if (rc) return rc;
     if (!r || !d_out_offsets || !d_total || out_cap < 0 || (out_cap && !d_out) || (total_bytes && !d_chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
@@ -5138,18 +5217,21 @@ static int sl_feed_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, i
 extern "C" int acb_streams_feed_leftmost_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
                                               const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
                                               acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    DeviceRestore keep_device;
     return sl_feed_host(ss, tb, chunks, total_bytes, offsets, n_chunks, stride_bytes, ids, final, out, cap, n_found, algo, false);
 }
 
 extern "C" int acb_streams_feed_words_host(acb_streams *ss, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
                                            const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
                                            acb_match *out, int64_t cap, int64_t *n_found, int algo) {
+    DeviceRestore keep_device;
     return sl_feed_host(ss, tb, chunks, total_bytes, offsets, n_chunks, stride_bytes, ids, final, out, cap, n_found, algo, true);
 }
 
 extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_table *tb, const uint8_t *chunks, int64_t total_bytes,
                                         const int64_t *offsets, int64_t n_chunks, int64_t stride_bytes, const int32_t *ids, int final,
                                         int algo, int64_t *out_offsets, uint8_t *out, int64_t out_cap, int64_t *total) {
+    DeviceRestore keep_device;
     int rc = sl_check(ss, tb, total_bytes, offsets, n_chunks, stride_bytes, &algo);
     if (rc) return rc;
     if (!r || !out_offsets || !total || out_cap < 0 || (out_cap && !out) || (total_bytes && !chunks)) { acb_set_error("bad argument"); return ACB_EINVAL; }
