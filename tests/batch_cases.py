@@ -1,7 +1,10 @@
 """Cases, input forms, references and C-entry checks shared by the batch-feature tests (leftmost-longest, replacement,
 whole words, white space, lookups, selects, stream batches).  Not a test module: tests/conftest.py puts tests/ on the
 path, and the test modules import from here, never from each other."""
+import collections
 import ctypes
+import random
+import string
 
 import numpy as np
 import pytest
@@ -147,6 +150,41 @@ def np_greedy(full: np.ndarray, key_len: np.ndarray) -> np.ndarray:
             i = nx[i]
     chosen = np.array(sorted(chosen), dtype=np.int64)
     return np.stack([hay[chosen], end[chosen], key[chosen]], axis=1)
+
+
+# ------------------------------------------------------------------ the reference's published benchmark shape
+PUBLISHED_CHARS = string.ascii_letters + string.digits
+
+
+Published = collections.namedtuple("Published", "words text missing")
+
+
+def _published_word(rng):
+    return "".join(rng.choice(PUBLISHED_CHARS) for _ in range(rng.randint(3, 32)))
+
+
+def published(n, text_length=0, n_missing=0):
+    """the reference's published benchmark shape (etc/benchmarks/benchmark.py), drawn in one pass of random.Random(0):
+    n distinct words of 3..32 characters over [A-Za-z0-9] as str, in generation order (not a set's order, which changes
+    with PYTHONHASHSEED and with it the key ids); then the haystack of text_length characters, drawn right after the
+    words as tools/published_benchmark.py draws it; then n_missing distinct words of the same shape that are not keys.
+    Nothing is cached: the caller decides how long the million strings live."""
+    rng = random.Random(0)
+    seen = {}
+    while len(seen) < n:
+        seen.setdefault(_published_word(rng))
+    text = "".join(rng.choice(PUBLISHED_CHARS) for _ in range(text_length))
+    missing = {}
+    while len(missing) < n_missing:
+        w = _published_word(rng)
+        if w not in seen:
+            missing.setdefault(w)
+    return Published(list(seen), text, list(missing))
+
+
+def published_words(n):
+    """published(n).words"""
+    return published(n).words
 
 
 # ------------------------------------------------------------------ random and structured cases of more than one file

@@ -5,8 +5,6 @@ The answer is always the drop-in's per-key method (the host trie, which test_api
 reference) and, where oracle/_ref is built, the reference extension itself.  Every randomised test has a CPU form on the
 numpy restatement of the kernel (tests/emul_lookup.py) and a gpu-marked twin on the real kernel."""
 import ctypes
-import random
-import string
 
 import numpy as np
 import pytest
@@ -14,7 +12,7 @@ import pytest
 import emul_lookup
 import oracle
 import pyahocorasick_b200 as pkg
-from batch_cases import DT, fake_table, obj, skip_if_device
+from batch_cases import DT, fake_table, obj, published, skip_if_device
 from pyahocorasick_b200 import _native as N
 from pyahocorasick_b200 import automaton as am
 
@@ -458,27 +456,13 @@ def test_queries_past_2_31_bytes():
         assert (bool(kid[i] >= 0), int(lp[i])) == (A.exists(k), A.longest_prefix(k)), i
 
 
-def _published_words(n):
-    rng = random.Random(0)
-    chars = string.ascii_letters + string.digits
-    seen = set()
-    while len(seen) < n:
-        seen.add("".join(rng.choice(chars) for _ in range(rng.randint(3, 32))))
-    words = list(seen)
-    missing = set()
-    while len(missing) < n:
-        w = "".join(rng.choice(chars) for _ in range(rng.randint(3, 32)))
-        if w not in seen:
-            missing.add(w)
-    return words, list(missing)
-
-
 @pytest.mark.gpu
 def test_published_lookup_shape_in_full():
     """1 M words of 3..32 characters over [a-zA-Z0-9], each its own value; 1 M present and 1 M absent lookups"""
-    words, missing = _published_words(1_000_000)
-    words = [w.encode() for w in words]
-    missing = [w.encode() for w in missing]
+    pw = published(1_000_000, n_missing=1_000_000)
+    words = [w.encode() for w in pw.words]
+    missing = [w.encode() for w in pw.missing]
+    del pw
     A = pkg.flavour("bytes").Automaton()
     for w in words:
         A.add_word(w, w)

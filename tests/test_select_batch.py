@@ -7,7 +7,6 @@ form on the Python restatement of the kernel (tests/emul_select.py) and a gpu-ma
 import ctypes
 import os
 import pickle
-import random
 import string
 
 import numpy as np
@@ -16,7 +15,7 @@ import pytest
 import emul_select
 import oracle
 import pyahocorasick_b200 as pkg
-from batch_cases import DT, fake_table, obj, skip_if_device
+from batch_cases import DT, fake_table, obj, published_words, skip_if_device
 from pyahocorasick_b200 import _native as N
 
 EXACT, AT_MOST, AT_LEAST = pkg.MATCH_EXACT_LENGTH, pkg.MATCH_AT_MOST_PREFIX, pkg.MATCH_AT_LEAST_PREFIX
@@ -415,18 +414,9 @@ def test_cuda_tensors_on_a_side_stream(fl):
             assert [[ko[x] for x in k[o[i]:o[i + 1]]] for i in range(len(objs))] == want
 
 
-def _published_words(n):
-    rng = random.Random(0)
-    chars = string.ascii_letters + string.digits
-    seen = set()
-    while len(seen) < n:
-        seen.add("".join(rng.choice(chars) for _ in range(rng.randint(3, 32))))
-    return list(seen)
-
-
 @pytest.fixture(scope="module")
 def published():
-    words = [w.encode() for w in _published_words(1_000_000)]
+    words = [w.encode() for w in published_words(1_000_000)]
     A = pkg.flavour("bytes").Automaton(pkg.STORE_INTS)
     for i, w in enumerate(words):
         A.add_word(w, i)
