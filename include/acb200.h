@@ -655,6 +655,20 @@ int acb_streams_feed_words_host(acb_streams *ss, acb_table *tb, const uint8_t *c
 int acb_table_upload_folded(const acb_trie *t, int device, const int32_t *alias_ptr, const int32_t *alias_ids, int64_t n_alias,
                             acb_table **out);
 
+/* ---- case-insensitive matching through a letter map (the package's Unicode simple case folding) -------------------
+ * acb_table_upload_folded with the fold given as a map: letter map_from[j] reads as map_to[j], every other letter as
+ * itself.  The trie, the alias lists and everything the folded table does (scans, expansion, refusals, streams through
+ * acb_streams_new_folded) are as for acb_table_upload_folded; only the fold differs.  The map's rules (ACB_EINVAL
+ * otherwise): map_from strictly ascending and below 0x110000, map_to[j] < map_from[j], no map_to value among map_from
+ * (the fold is idempotent), and on a trie of 1-byte letters every map_from below 256 maps below 256 (entries from 256 up
+ * do not apply to 1-byte letters).  4-byte letters from 0x110000 up (not code points) read as themselves.  A 4-byte map
+ * may change letters in at most 42 blocks of 256 code points (Unicode 15's simple folding uses 24); a 2-byte trie is
+ * refused.  The fold is one kernel per scan with the map staged in shared memory (DESIGN section 4.19).  A stream batch
+ * made on one fold refuses a table of the other (ACB_EINVAL).  Both may be NULL with n_map == 0: nothing folds. */
+int acb_table_upload_folded_map(const acb_trie *t, int device, const int32_t *alias_ptr, const int32_t *alias_ids,
+                                int64_t n_alias, const uint32_t *map_from, const uint32_t *map_to, int64_t n_map,
+                                acb_table **out);
+
 /* DEVICE buffers, asynchronous on `stream`; a folded table only (ACB_EINVAL).  Each of the n records of d_in becomes its
  * own record followed by one per alias of its key id, ascending (key ids without aliases, or outside the lists, stay
  * one record), at d_out in d_in's order; *d_count is SET to their total and only records below index cap are stored.

@@ -146,6 +146,7 @@ def lib() -> ctypes.CDLL:
         "acb_streams_feed_words_host": (ctypes.c_int, [vp, vp, vp, i64, vp, i64, i64, vp, ctypes.c_int, vp, i64, pi64,
                                                        ctypes.c_int]),
         "acb_table_upload_folded": (ctypes.c_int, [vp, ctypes.c_int, vp, vp, i64, ctypes.POINTER(vp)]),
+        "acb_table_upload_folded_map": (ctypes.c_int, [vp, ctypes.c_int, vp, vp, i64, vp, vp, i64, ctypes.POINTER(vp)]),
         "acb_expand_aliases_device": (ctypes.c_int, [vp, vp, i64, vp, i64, vp, vp]),
         "acb_last_fold_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), i32]),
         "acb_streams_new_folded": (ctypes.c_int, [vp, i64, ctypes.c_int, ctypes.c_int, vp, i64, ctypes.POINTER(vp)]),
@@ -185,7 +186,7 @@ EXPORTED_SYMBOLS = [
     "acb_scan_host_leftmost_words", "acb_replace_host_words", "acb_last_words_ms", "acb_streams_new_words",
     "acb_streams_feed_words_device", "acb_streams_feed_words_host", "acb_leftmost_first_device", "acb_scan_host_leftmost_kind",
     "acb_replacer_new_kind", "acb_streams_new_leftmost_kind", "acb_table_upload_folded", "acb_expand_aliases_device",
-    "acb_last_fold_ms", "acb_streams_new_folded", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_last_fold_ms", "acb_table_upload_folded_map", "acb_streams_new_folded", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

@@ -105,6 +105,54 @@ def _ascii_fold(key):
     return key.lower() if isinstance(key, bytes) else key.translate(_ASCII_LOWER)
 
 
+# the case folds of the batch methods, as a folded table records them (acb_table's fold): ascii_case_insensitive folds
+# A-Z only (acb_table_upload_folded), case_insensitive folds through _unicode_fold_map (acb_table_upload_folded_map)
+_FOLD_NONE, _FOLD_ASCII, _FOLD_UNICODE = 0, 1, 2
+
+
+def _sfold(ch: str) -> str:
+    """Unicode simple case folding of one letter: its casefold() when that is one letter, else its lower() when that is
+    one letter, else itself"""
+    f = ch.casefold()
+    if len(f) == 1:
+        return f
+    f = ch.lower()
+    return f if len(f) == 1 else ch
+
+
+@functools.lru_cache(maxsize=None)
+def _unicode_fold_map() -> Tuple[np.ndarray, np.ndarray]:
+    """The fold of case_insensitive as (from, to): two sorted uint32 arrays of every code point that changes and the
+    one it folds to.  Letters with equal _sfold (Unicode simple case folding) match each other, and each such class
+    folds to its lowest code point, so every latin-1 letter folds into latin-1 (µ stays µ; Μ and μ fold to it) and the
+    map restricted to from < 256 is the fold of 1-byte letters.  One letter maps to one letter: ß and ss, or ﬁ and fi,
+    stay apart, and ΐ stays itself.  No Turkic rule: ı and İ match neither i nor I.  No normalisation: é and e + U+0301
+    stay apart.  Surrogates and letter values above U+10FFFF fold to themselves.  The classes follow the Unicode version
+    of the running Python's unicodedata (unicodedata.unidata_version).  About 1.1 M calls: built on first use, once
+    per process."""
+    classes: dict = {}
+    for c in range(0x110000):
+        classes.setdefault(_sfold(chr(c)), []).append(c)
+    pairs = sorted((c, members[0]) for members in classes.values() if len(members) > 1 for c in members[1:])
+    frm = np.array([a for a, _ in pairs], dtype=np.uint32)
+    to = np.array([b for _, b in pairs], dtype=np.uint32)
+    frm.flags.writeable = False
+    to.flags.writeable = False
+    return frm, to
+
+
+@functools.lru_cache(maxsize=None)
+def _unicode_fold_table() -> dict:
+    """_unicode_fold_map as a str.translate table"""
+    frm, to = _unicode_fold_map()
+    return dict(zip(frm.tolist(), to.tolist()))
+
+
+def _fold_key(key, kind: int):
+    """A key folded as a table of fold kind _FOLD_ASCII or _FOLD_UNICODE folds its text"""
+    return _ascii_fold(key) if kind == _FOLD_ASCII else key.translate(_unicode_fold_table())
+
+
 class _FoldCore(NamedTuple):
     """The folded automaton of one letter width (Automaton._fold_host): its host trie, which holds each folded key under
     its group's representative (the lowest id of the keys that fold to it), and the alias lists of acb_table_upload_folded
@@ -264,8 +312,8 @@ class Automaton:
         self._narrow_table = None
         self._narrow_device = None
         self._narrow_empty = False
-        # ascii_case_insensitive: per letter width (narrow or not) the folded automaton (_FoldCore, or None without a key)
-        # and its table as (acb_table*, device), built lazily
+        # case folding: per (fold kind, narrow) the folded automaton (_FoldCore, or None without a key) and its table as
+        # (acb_table*, device), built lazily
         self._fold_cores: dict = {}
         self._fold_tables: dict = {}
         self._match_cap = 0
@@ -736,12 +784,13 @@ class Automaton:
         return tb
 
     @_locked
-    def _fold_host(self, narrow: bool) -> Optional[_FoldCore]:
-        """The folded automaton of a batch's letter width (narrow: the latin-1 keys at 1 byte per letter), built lazily;
-        None when it has no key.  Keys are added in ascending id, and a key whose folded text is already there is not
-        added but listed as an alias of the id that holds it, so that id is the lowest of its group."""
-        if narrow in self._fold_cores:
-            return self._fold_cores[narrow]
+    def _fold_host(self, narrow: bool, kind: int = _FOLD_ASCII) -> Optional[_FoldCore]:
+        """The folded automaton of a fold kind (_FOLD_ASCII or _FOLD_UNICODE) and a batch's letter width (narrow: the
+        keys whose folded text is latin-1, at 1 byte per letter), built lazily; None when it has no key.  Keys are added in
+        ascending id, and a key whose folded text is already there is not added but listed as an alias of the id that
+        holds it, so that id is the lowest of its group."""
+        if (kind, narrow) in self._fold_cores:
+            return self._fold_cores[(kind, narrow)]
         t = self._lib.acb_trie_new(1 if narrow else self._L)
         if not t:
             raise MemoryError(N.last_error())
@@ -750,7 +799,7 @@ class Automaton:
         for kid, key in enumerate(self._key_objs):
             if key is None:
                 continue
-            folded = _ascii_fold(key)
+            folded = _fold_key(key, kind)
             if narrow:
                 try:
                     raw = folded.encode("latin-1")
@@ -765,7 +814,7 @@ class Automaton:
             N.check(self._lib.acb_trie_add_word(t, raw, len(raw), kid, None))
         if not reps:
             self._lib.acb_trie_free(t)
-            self._fold_cores[narrow] = None
+            self._fold_cores[(kind, narrow)] = None
             return None
         built = ctypes.c_int32(0)
         N.check(self._lib.acb_trie_make_automaton(t, ctypes.byref(built)))
@@ -774,56 +823,71 @@ class Automaton:
             alias_ptr[rep + 1] = len(ids)
         np.cumsum(alias_ptr, out=alias_ptr)
         alias_ids = np.array([k for rep in sorted(aliases) for k in aliases[rep]], dtype=np.int32)
-        core = self._fold_cores[narrow] = _FoldCore(t, alias_ptr, alias_ids)
+        core = self._fold_cores[(kind, narrow)] = _FoldCore(t, alias_ptr, alias_ids)
         return core
 
     @_locked
-    def _ensure_folded(self, device: Optional[int], narrow: bool):
-        """The folded table (acb_table_upload_folded) of a batch's letter width on `device`; None when it has no key."""
-        core = self._fold_host(narrow)
+    def _ensure_folded(self, device: Optional[int], narrow: bool, kind: int = _FOLD_ASCII):
+        """The folded table of a fold kind and a batch's letter width on `device` (acb_table_upload_folded, or
+        acb_table_upload_folded_map with _unicode_fold_map); None when it has no key."""
+        core = self._fold_host(narrow, kind)
         if core is None:
             return None
         if device is None:
             device = _default_device()
-        have = self._fold_tables.get(narrow)
+        have = self._fold_tables.get((kind, narrow))
         if have is not None and have[1] == device:
             return have[0]
         if have is not None:
             self._lib.acb_table_free(have[0])
-            del self._fold_tables[narrow]
+            del self._fold_tables[(kind, narrow)]
         tb = ctypes.c_void_p()
         n = len(core.alias_ids)
-        N.check(self._lib.acb_table_upload_folded(core.trie, device, N.ptr(core.alias_ptr) if n else None,
-                                                  N.ptr(core.alias_ids) if n else None, n, ctypes.byref(tb)))
-        self._fold_tables[narrow] = (tb, device)
+        aliases = (core.trie, device, N.ptr(core.alias_ptr) if n else None, N.ptr(core.alias_ids) if n else None, n)
+        if kind == _FOLD_ASCII:
+            N.check(self._lib.acb_table_upload_folded(*aliases, ctypes.byref(tb)))
+        else:
+            frm, to = _unicode_fold_map()
+            if narrow:
+                frm, to = np.ascontiguousarray(frm[frm < 256]), np.ascontiguousarray(to[frm < 256])
+            N.check(self._lib.acb_table_upload_folded_map(*aliases, N.ptr(frm), N.ptr(to), len(frm), ctypes.byref(tb)))
+        self._fold_tables[(kind, narrow)] = (tb, device)
         return tb
 
-    def _table_for(self, device: Optional[int], narrow: bool, fold: bool = False):
-        """The table a batch runs on: the latin-1 one for a narrow batch, else the full one; with fold, the folded table of
-        that width.  None when the batch is narrow and no key is latin-1: then nothing matches."""
+    def _table_for(self, device: Optional[int], narrow: bool, fold: int = _FOLD_NONE):
+        """The table a batch runs on: the latin-1 one for a narrow batch, else the full one; with a fold kind, the folded
+        table of that kind and width.  None when the batch is narrow and no key is latin-1: then nothing matches."""
         if fold:
-            return self._ensure_folded(device, narrow)
+            return self._ensure_folded(device, narrow, fold)
         if not narrow:
             return self._ensure_table(device)
         core = self._ensure_narrow(device)
         return None if core is None else core[1]
 
-    def _has_aliases(self, narrow: bool) -> bool:
-        """the folded key set of this width has case variants (an alias expansion follows the find_all scans)"""
-        core = self._fold_host(narrow)
+    def _has_aliases(self, narrow: bool, kind: int = _FOLD_ASCII) -> bool:
+        """the folded key set of this kind and width has case variants (an alias expansion follows the find_all scans)"""
+        core = self._fold_host(narrow, kind)
         return core is not None and len(core.alias_ids) > 0
 
-    def _fold_arg(self, ascii_case_insensitive, algo: str = "auto", ignore_white_space: bool = False) -> bool:
-        """The ascii_case_insensitive argument of the batch methods, checked against the others"""
-        if not ascii_case_insensitive:
-            return False
+    def _fold_arg(self, ascii_case_insensitive, algo: str = "auto", ignore_white_space: bool = False,
+                  case_insensitive: bool = False) -> int:
+        """The fold kind that the ascii_case_insensitive and case_insensitive arguments of the batch methods ask for
+        (_FOLD_NONE, _FOLD_ASCII or _FOLD_UNICODE), checked against the others"""
+        if not ascii_case_insensitive and not case_insensitive:
+            return _FOLD_NONE
+        name = "case_insensitive" if case_insensitive else "ascii_case_insensitive"
         if self._key_type == KEY_SEQUENCE:
-            raise ValueError("ascii_case_insensitive needs text: KEY_SEQUENCE letters are integers, not letters")
+            raise ValueError(f"{name} needs text: KEY_SEQUENCE letters are integers, not letters")
+        if ascii_case_insensitive and case_insensitive:
+            raise ValueError("case_insensitive and ascii_case_insensitive are two different folds: pass one of them")
+        if case_insensitive and not self._UNICODE:
+            raise ValueError("case_insensitive folds code points, and bytes have no known encoding: the bytes flavour "
+                             "takes ascii_case_insensitive")
         if ignore_white_space:
-            raise ValueError("ascii_case_insensitive cannot be combined with ignore_white_space")
+            raise ValueError(f"{name} cannot be combined with ignore_white_space")
         if algo == "long":
-            raise ValueError("ascii_case_insensitive cannot be combined with algo='long'")
-        return True
+            raise ValueError(f"{name} cannot be combined with algo='long'")
+        return _FOLD_UNICODE if case_insensitive else _FOLD_ASCII
 
     @_locked
     def filter_shape(self) -> dict:
@@ -873,7 +937,7 @@ class Automaton:
     @_locked
     def _scan_flat(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int,
                    algo: str = "auto", sort: bool = True, device: Optional[int] = None, narrow: bool = False,
-                   long_state: Optional[int] = None, fold: bool = False) -> np.ndarray:
+                   long_state: Optional[int] = None, fold: int = _FOLD_NONE) -> np.ndarray:
         """flat uint8 buffer (+ int64 byte offsets or a fixed stride) -> sorted match records.
         narrow=True: the buffer holds 1-byte letters of a unicode-flavour automaton (latin-1 path).  fold: on the folded
         table, which folds the text and expands the aliases itself.
@@ -897,7 +961,7 @@ class Automaton:
         """The first guess of the records a batch of n_hay haystacks gives; _match_cap remembers the largest overflow."""
         return max(self._match_cap, 1 << 12, 2 * n_hay)
 
-    def _host_records(self, device: Optional[int], narrow: bool, n_hay: int, call, fold: bool = False) -> np.ndarray:
+    def _host_records(self, device: Optional[int], narrow: bool, n_hay: int, call, fold: int = _FOLD_NONE) -> np.ndarray:
         """The records of one host-buffer call, which leaves them in its table's pinned buffer.  call(tb, cap, found_ref)
         makes the native call with room for cap records and returns its status.  On ACB_EOVERFLOW it runs once more with
         room for the exact count (+1024, kept in _match_cap); a second overflow raises.  The records are handed over
@@ -958,7 +1022,7 @@ class Automaton:
     @_locked
     def _words_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str, sort: bool,
                     device: Optional[int], narrow: bool, words: tuple, leftmost: bool, select: int = N.SELECT_LONGEST,
-                    fold: bool = False) -> np.ndarray:
+                    fold: int = _FOLD_NONE) -> np.ndarray:
         """acb_scan_host_words / acb_scan_host_leftmost_words (acb_scan_host_leftmost_kind for leftmost-first): upload,
         scan, keep the whole-word matches, then sort or select, copy back (_host_records)."""
         lib = self._lib
@@ -988,7 +1052,7 @@ class Automaton:
 
     @_locked
     def _scan_device_tensor(self, batch, algo: str, sort: bool, words: Optional[tuple] = None,
-                            white_space: bool = False, fold: bool = False) -> np.ndarray:
+                            white_space: bool = False, fold: int = _FOLD_NONE) -> np.ndarray:
         """Batch already resident in HBM: a C-contiguous uint8 torch CUDA tensor [n, stride].  No host copy of
         the haystacks; the scan runs on torch's current stream, only the records come back.  words: keep the
         whole-word matches (_filter_words_device) before the sort.  white_space: the scan skips the white space
@@ -1000,7 +1064,7 @@ class Automaton:
         skip = self._skip_set(False) if white_space else None
         with _on_device(dev) as stream:
             out, found = self._device_matches(tb, t, batch.n, batch.stride, algo, stream, words, skip)
-            if fold and found and self._has_aliases(False):
+            if fold and found and self._has_aliases(False, fold):
                 out, found = self._expand_device(tb, t, batch.n, out, found, stream)
             return self._device_records(tb, out, found, batch.n, batch.stride // self._L, stream, sort)
 
@@ -1151,16 +1215,17 @@ class Automaton:
         return AutomatonSearchIterLong(self, letters, start, end)
 
     def find_long_batch(self, haystacks, *, sort: bool = True, device: Optional[int] = None, whole_words=False,
-                        ascii_case_insensitive: bool = False) -> "Matches":
-        """iter_long() over a whole batch (same input forms and result type as find_all_batch).  whole_words and
-        ascii_case_insensitive are refused (ValueError): iter_long's walk picks its matches itself, so a filter after it
-        has no clear meaning, and its walk follows the automaton of the keys as given."""
+                        ascii_case_insensitive: bool = False, case_insensitive: bool = False) -> "Matches":
+        """iter_long() over a whole batch (same input forms and result type as find_all_batch).  whole_words,
+        ascii_case_insensitive and case_insensitive are refused (ValueError): iter_long's walk picks its matches itself,
+        so a filter after it has no clear meaning, and its walk follows the automaton of the keys as given."""
         return self.find_all_batch(haystacks, algo="long", sort=sort, device=device, whole_words=whole_words,
-                                   ascii_case_insensitive=ascii_case_insensitive)
+                                   ascii_case_insensitive=ascii_case_insensitive, case_insensitive=case_insensitive)
 
     @_locked
     def find_leftmost_longest_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
-                                    whole_words=False, ascii_case_insensitive: bool = False) -> "Matches":
+                                    whole_words=False, ascii_case_insensitive: bool = False,
+                                    case_insensitive: bool = False) -> "Matches":
         """Leftmost-longest non-overlapping matches of a whole batch, selected on the GPU (input forms and result type
         of find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or
         after p, take the smallest such start, the longest match there, and continue after its end.  Records come in
@@ -1172,31 +1237,32 @@ class Automaton:
         word does not hide a shorter whole word: keys ``new`` and ``new york`` on ``new yorker`` give ``new``.  A CUDA
         tensor batch then waits once more, for the number of whole-word matches.
 
-        ascii_case_insensitive (see find_all_batch): the same rule over the folded text.  Of the keys that fold to the
-        same text, only the one added first is reported."""
+        ascii_case_insensitive and case_insensitive (see find_all_batch): the same rule over the folded text.  Of the keys
+        that fold to the same text, only the one added first is reported."""
         self._require_automaton()
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-longest takes 'auto', 'filter' or 'dfa'")
         words = self._words(whole_words)
-        fold = self._fold_arg(ascii_case_insensitive)
+        fold = self._fold_arg(ascii_case_insensitive, case_insensitive=case_insensitive)
         b = self._batch_input(haystacks)
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
         elif b.kind == "device":
             rec = self._leftmost_device(b, algo, words, fold=fold)
         elif words is not None and fold:
-            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, fold=True)
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, fold=fold)
         elif words is not None:
             rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True)
         elif fold:
-            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, fold=True)
+            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, fold=fold)
         else:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow)
         return Matches(rec, self._result_values())
 
     @_locked
     def find_leftmost_first_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
-                                  whole_words=False, ascii_case_insensitive: bool = False) -> "Matches":
+                                  whole_words=False, ascii_case_insensitive: bool = False,
+                                  case_insensitive: bool = False) -> "Matches":
         """Leftmost-first non-overlapping matches of a whole batch, selected on the GPU (input forms and result type of
         find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or after
         p, take the smallest such start, the match there whose key was added first, and continue after its end.  This is
@@ -1204,13 +1270,13 @@ class Automaton:
         at a start, but a match further left always wins.  Priority is the order in which add_word first added each key:
         add_word of a key already present keeps its place, removing a key and adding it again moves it to the end.  An
         automaton read back from pickle or save numbers its keys afresh, so its priority can differ.  Records come in
-        haystack order, then end_index ascending; algo, whole_words and ascii_case_insensitive as for
+        haystack order, then end_index ascending; algo, whole_words, ascii_case_insensitive and case_insensitive as for
         find_leftmost_longest_batch (the key added first wins among keys of one folded text, as at any start)."""
         self._require_automaton()
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-first takes 'auto', 'filter' or 'dfa'")
         words = self._words(whole_words)
-        fold = self._fold_arg(ascii_case_insensitive)
+        fold = self._fold_arg(ascii_case_insensitive, case_insensitive=case_insensitive)
         b = self._batch_input(haystacks)
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
@@ -1218,18 +1284,18 @@ class Automaton:
             rec = self._leftmost_device(b, algo, words, N.SELECT_FIRST, fold)
         elif words is not None and fold:
             rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, select=N.SELECT_FIRST,
-                                   fold=True)
+                                   fold=fold)
         elif words is not None:
             rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, False, device, b.narrow, words, True, select=N.SELECT_FIRST)
         elif fold:
-            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST, fold=True)
+            rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST, fold=fold)
         else:
             rec = self._leftmost_host(b.data, b.offsets, b.n, b.stride, algo, device, b.narrow, select=N.SELECT_FIRST)
         return Matches(rec, self._result_values())
 
     @_locked
     def _leftmost_host(self, flat: np.ndarray, offsets: Optional[np.ndarray], n_hay: int, stride_bytes: int, algo: str,
-                       device: Optional[int], narrow: bool, select: int = N.SELECT_LONGEST, fold: bool = False) -> np.ndarray:
+                       device: Optional[int], narrow: bool, select: int = N.SELECT_LONGEST, fold: int = _FOLD_NONE) -> np.ndarray:
         """acb_scan_host_leftmost (acb_scan_host_leftmost_kind for leftmost-first): upload, scan, select, copy back
         (_host_records).  fold: on the folded table, whose representatives are the winners; no alias expansion."""
         lib = self._lib
@@ -1243,7 +1309,7 @@ class Automaton:
 
     @_locked
     def _leftmost_device(self, batch, algo: str, words: Optional[tuple] = None, select: int = N.SELECT_LONGEST,
-                         fold: bool = False) -> np.ndarray:
+                         fold: int = _FOLD_NONE) -> np.ndarray:
         """A CUDA tensor batch: the full scan into a device buffer, then the selection, both on torch's current stream;
         only the chosen records come back.  fold: on the folded table."""
         t = _aligned(batch.data)
@@ -1298,7 +1364,8 @@ class Automaton:
     # ------------------------------------------------------------------ the batch entry (new)
     @_locked
     def find_all_batch(self, haystacks, *, algo: str = "auto", sort: bool = True, device: Optional[int] = None,
-                       ignore_white_space: bool = False, whole_words=False, ascii_case_insensitive: bool = False) -> Matches:
+                       ignore_white_space: bool = False, whole_words=False, ascii_case_insensitive: bool = False,
+                       case_insensitive: bool = False) -> Matches:
         """Search a whole batch on the GPU.
 
         haystacks: a sequence of bytes / str / tuple objects (as `iter` accepts), or a 2-D
@@ -1326,6 +1393,16 @@ class Automaton:
         ``xAbCx``; keys of one length at one end (case variants of each other) come in ascending key id.  end_index and
         the whole-word test are those of the text as given.  The text is folded on the GPU; the caller's copy is not
         changed.  ValueError with ignore_white_space, algo="long" or a KEY_SEQUENCE automaton.
+
+        case_insensitive (unicode flavour): letters match when Unicode simple case folding maps them to the same letter
+        (`_unicode_fold_map`, from the running Python's unicodedata): ``Müller`` matches ``MÜLLER``, ``Σοφία`` matches
+        ``ΣΟΦΊΑ``, ``Straße`` matches ``STRAẞE``, and K, k and the Kelvin sign match each other, also in a latin-1 batch.
+        One letter folds to one letter only: ``ß`` does not match ``ss`` nor ``ﬁ`` ``fi``; there is no Turkic rule (``ı``
+        and ``İ`` match neither ``i`` nor ``I``) and no normalisation (``é`` does not match ``e`` + U+0301).  Everything
+        else is as for ascii_case_insensitive: every key whose folded text occurs, case variants in ascending key id,
+        end_index and whole words of the text as given, the text folded on the GPU and the caller's copy unchanged.
+        ValueError for the bytes flavour (bytes have no known encoding: use ascii_case_insensitive), together with
+        ascii_case_insensitive, with ignore_white_space, algo="long" or a KEY_SEQUENCE automaton.
         """
         self._require_automaton()
         if ignore_white_space and algo == "long":
@@ -1335,20 +1412,20 @@ class Automaton:
             raise ValueError("whole_words cannot be combined with ignore_white_space")
         if words is not None and algo == "long":
             raise ValueError("whole_words cannot be combined with algo='long': iter_long's walk picks its matches itself")
-        fold = self._fold_arg(ascii_case_insensitive, algo, ignore_white_space)
+        fold = self._fold_arg(ascii_case_insensitive, algo, ignore_white_space, case_insensitive)
         b = self._batch_input(haystacks, narrow_ok=algo != "long")
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
         elif b.kind == "device":
             rec = self._scan_device_tensor(b, algo, sort, words, ignore_white_space, fold)
         elif words is not None and fold:
-            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, sort, device, b.narrow, words, False, fold=True)
+            rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, sort, device, b.narrow, words, False, fold=fold)
         elif words is not None:
             rec = self._words_host(b.data, b.offsets, b.n, b.stride, algo, sort, device, b.narrow, words, False)
         elif ignore_white_space:
             rec = self._scan_skip(b, algo, sort, device)
         elif fold:
-            rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow, fold=True)
+            rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow, fold=fold)
         else:
             rec = self._scan_flat(b.data, b.offsets, b.n, b.stride, algo=algo, sort=sort, device=device, narrow=b.narrow)
         return Matches(rec, self._result_values())
@@ -1423,7 +1500,7 @@ class Automaton:
         Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
         wider chunks, so the latin-1 automaton is not used)."""
         return self._stream_batch(n_streams, long, algo, device, ignore_white_space, leftmost_longest, whole_words,
-                                  leftmost_first, False)
+                                  leftmost_first, _FOLD_NONE)
 
     def ascii_case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
                                             leftmost_longest: bool = False, leftmost_first: bool = False,
@@ -1435,14 +1512,29 @@ class Automaton:
         text, the one added first.  Matches are released at the same points as by the stream_batch of the same options,
         and the word test reads the letters as given.  Takes neither long nor ignore_white_space; not for KEY_SEQUENCE
         automata.  The returned StreamBatch has ``ascii_case_insensitive`` True."""
-        return self._stream_batch(n_streams, False, algo, device, False, leftmost_longest, whole_words, leftmost_first, True)
+        return self._stream_batch(n_streams, False, algo, device, False, leftmost_longest, whole_words, leftmost_first,
+                                  _FOLD_ASCII)
+
+    def case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
+                                      leftmost_longest: bool = False, leftmost_first: bool = False,
+                                      whole_words=False) -> "StreamBatch":
+        """`stream_batch` with Unicode case-insensitive matching (unicode flavour): over all feeds (and `finish`) of a
+        stream, what find_all_batch, find_leftmost_longest_batch or find_leftmost_first_batch reports for its whole text
+        with case_insensitive=True and the same whole_words.  A find_all batch reports every key whose folded text occurs,
+        keys of one length at one end in ascending id; a leftmost batch reports, of the keys that fold to one text, the
+        one added first.  Matches are released at the same points as by the stream_batch of the same options, and the
+        word test reads the letters as given.  Takes neither long nor ignore_white_space; not for the bytes flavour or
+        KEY_SEQUENCE automata.  The returned StreamBatch has ``case_insensitive`` True."""
+        return self._stream_batch(n_streams, False, algo, device, False, leftmost_longest, whole_words, leftmost_first,
+                                  _FOLD_UNICODE)
 
     @_locked
     def _stream_batch(self, n_streams: int, long: bool, algo: str, device: Optional[int], ignore_white_space: bool,
-                      leftmost_longest: bool, whole_words, leftmost_first: bool, fold: bool) -> "StreamBatch":
-        """The argument check and constructor of stream_batch and ascii_case_insensitive_stream_batch (fold)"""
+                      leftmost_longest: bool, whole_words, leftmost_first: bool, fold: int) -> "StreamBatch":
+        """The argument check and constructor of stream_batch, ascii_case_insensitive_stream_batch and
+        case_insensitive_stream_batch (fold: the fold kind)"""
         self._require_automaton()
-        self._fold_arg(fold)
+        self._fold_arg(fold == _FOLD_ASCII, case_insensitive=fold == _FOLD_UNICODE)
         n_streams = operator.index(n_streams)
         if n_streams < 0:
             raise ValueError("n_streams must not be negative")
@@ -1688,11 +1780,11 @@ class _Streams:
         return out[:self.n_streams]
 
     def _table(self):
-        """(the table every call of this batch runs on, whether it is folded): the automaton's full table, or for an
-        ascii_case_insensitive batch its folded one -- the full one when there is no key, which matches nothing either
-        way"""
+        """(the table every call of this batch runs on, whether it is folded): the automaton's full table, or for a
+        case-insensitive batch the folded one of its fold kind -- the full one when there is no key, which matches
+        nothing either way"""
         A = self._A
-        tb = A._table_for(self._device, False, True) if self.ascii_case_insensitive else None
+        tb = A._table_for(self._device, False, self._fold) if self._fold else None
         return (A._ensure_table(self._device), False) if tb is None else (tb, True)
 
     def _ids(self, ids, n: int) -> Optional[np.ndarray]:
@@ -1758,13 +1850,16 @@ class StreamBatch(_Streams):
 
     A batch from `Automaton.ascii_case_insensitive_stream_batch` (``ascii_case_insensitive`` True) reports what the
     batch of the same options reports, with keys and text compared ASCII case-insensitively: what the whole-batch
-    method reports with ascii_case_insensitive=True for each stream's whole text."""
+    method reports with ascii_case_insensitive=True for each stream's whole text.  One from
+    `Automaton.case_insensitive_stream_batch` (``case_insensitive`` True) does the same with case_insensitive=True."""
 
     def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None,
                  leftmost_longest: bool = False, words: Optional[tuple] = None, leftmost_first: bool = False,
-                 fold: bool = False):
+                 fold: int = _FOLD_NONE):
         self._A = A
-        self.ascii_case_insensitive = fold
+        self._fold = fold
+        self.ascii_case_insensitive = fold == _FOLD_ASCII
+        self.case_insensitive = fold == _FOLD_UNICODE
         self._version = A._version
         self.n_streams = n_streams
         self.long = long
@@ -1970,7 +2065,8 @@ class Replacer:
             self._native[(narrow, device)] = r
         return r
 
-    def replace_batch(self, haystacks, *, algo: str = "auto", whole_words=False, ascii_case_insensitive: bool = False):
+    def replace_batch(self, haystacks, *, algo: str = "auto", whole_words=False, ascii_case_insensitive: bool = False,
+                      case_insensitive: bool = False):
         """The batch with every leftmost-longest match replaced.  `haystacks` takes the input forms of find_all_batch;
         a list gives a list of the same item type, uint8[n, stride] or (flat, offsets) gives (flat uint8, offsets
         int64[n+1]), a CUDA tensor gives that pair as CUDA tensors computed on torch's current stream (the call
@@ -1979,7 +2075,8 @@ class Replacer:
         inside a longer word is left alone; a CUDA tensor batch then synchronises once more.  ascii_case_insensitive
         (see find_all_batch): replace the matches the find_leftmost_*_batch method of this replacer's rule chooses with
         the same option, each by the replacement of its key -- the one added first among keys that fold to the same
-        text; every other letter is copied as given, in its own case."""
+        text; every other letter is copied as given, in its own case.  case_insensitive (unicode flavour; see
+        find_all_batch): the same with Unicode simple case folding."""
         A = self._A
         with A._gpu_lock:
             if self._version != A._version:
@@ -1988,7 +2085,7 @@ class Replacer:
             if algo not in ("auto", "filter", "dfa"):
                 raise ValueError(f"algo {algo!r}: replace_batch takes 'auto', 'filter' or 'dfa'")
             words = A._words(whole_words)
-            fold = A._fold_arg(ascii_case_insensitive)
+            fold = A._fold_arg(ascii_case_insensitive, case_insensitive=case_insensitive)
             pair = isinstance(haystacks, np.ndarray) or _is_pair(haystacks)
             batch = A._batch_input(haystacks)
             if batch.kind == "device":
@@ -2003,7 +2100,7 @@ class Replacer:
             if batch.empty:
                 out, out_offs = flat[:0].copy(), np.zeros(n + 1, dtype=np.int64)
             elif fold:
-                out, out_offs = self._run_host(flat, offs, n, narrow, algo, words, fold=True)
+                out, out_offs = self._run_host(flat, offs, n, narrow, algo, words, fold=fold)
             elif words is None:
                 out, out_offs = self._run_host(flat, offs, n, narrow, algo)
             else:
@@ -2017,7 +2114,7 @@ class Replacer:
         """`n_streams` streams rewritten chunk by chunk (ReplaceStream.feed): over all feeds and `finish` of a stream,
         the output is exactly what `replace_batch` gives for its whole text, with the same whole_words.  Streams run at
         the automaton's full letter width (unicode: 4 bytes per letter), as every stream batch does."""
-        return self._stream_batch(n_streams, algo, device, whole_words, False)
+        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_NONE)
 
     def ascii_case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
                                             whole_words=False) -> "ReplaceStream":
@@ -2025,16 +2122,26 @@ class Replacer:
         exactly what `replace_batch` gives for its whole text with ascii_case_insensitive=True and the same whole_words.
         Each match takes the replacement of the key added first among those that fold to its text; every other letter,
         held ones included, keeps its own case.  The returned ReplaceStream has ``ascii_case_insensitive`` True."""
-        return self._stream_batch(n_streams, algo, device, whole_words, True)
+        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_ASCII)
 
-    def _stream_batch(self, n_streams: int, algo: str, device: Optional[int], whole_words, fold: bool) -> "ReplaceStream":
-        """The argument check and constructor of stream_batch and ascii_case_insensitive_stream_batch (fold)"""
+    def case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
+                                      whole_words=False) -> "ReplaceStream":
+        """`stream_batch` with Unicode case-insensitive matching (unicode flavour): over all feeds and `finish` of a
+        stream, the output is exactly what `replace_batch` gives for its whole text with case_insensitive=True and the
+        same whole_words.  Each match takes the replacement of the key added first among those that fold to its text;
+        every other letter, held ones included, keeps its own case.  The returned ReplaceStream has ``case_insensitive``
+        True."""
+        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_UNICODE)
+
+    def _stream_batch(self, n_streams: int, algo: str, device: Optional[int], whole_words, fold: int) -> "ReplaceStream":
+        """The argument check and constructor of stream_batch, ascii_case_insensitive_stream_batch and
+        case_insensitive_stream_batch (fold: the fold kind)"""
         A = self._A
         with A._gpu_lock:
             if self._version != A._version:
                 raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
             A._require_automaton()
-            A._fold_arg(fold)
+            A._fold_arg(fold == _FOLD_ASCII, case_insensitive=fold == _FOLD_UNICODE)
             n_streams = operator.index(n_streams)
             if n_streams < 0:
                 raise ValueError("n_streams must not be negative")
@@ -2061,7 +2168,7 @@ class Replacer:
         return [s[b[i] // 4:b[i + 1] // 4] for i in range(len(b) - 1)]
 
     def _run_host(self, flat: np.ndarray, offs: np.ndarray, n: int, narrow: bool, algo: str, words: Optional[tuple] = None,
-                  fold: bool = False):
+                  fold: int = _FOLD_NONE):
         """acb_replace_host (acb_replace_host_words with a word set) -> (output bytes, output offsets int64[n+1]); a
         second call when the first guess of the output size was too small (_host_bytes).  fold: on the folded table."""
         A = self._A
@@ -2081,7 +2188,7 @@ class Replacer:
             return A._lib.acb_replace_host_words(*batch, N.ptr(bits) if n_bits else None, n_bits, *result)
         return _host_bytes(int(flat.size) * 5 // 4 + 4096, replace), out_offs
 
-    def _run_device(self, batch, algo: str, words: Optional[tuple] = None, fold: bool = False):
+    def _run_device(self, batch, algo: str, words: Optional[tuple] = None, fold: int = _FOLD_NONE):
         """A CUDA tensor batch: scan, select and rewrite on torch's current stream; (flat, offsets) CUDA tensors"""
         import torch
         A = self._A
@@ -2113,11 +2220,14 @@ class ReplaceStream(_Streams):
     `Replacer.replace_batch` gives for its whole text.  Stale (ValueError) when the replacer is.  With whole_words, a
     stream holds back one letter more: the output before ``position - longest_word`` is released.  From
     `Replacer.ascii_case_insensitive_stream_batch` (``ascii_case_insensitive`` True), the output is what replace_batch
-    gives with ascii_case_insensitive=True, released at the same points."""
+    gives with ascii_case_insensitive=True, released at the same points; from `Replacer.case_insensitive_stream_batch`
+    (``case_insensitive`` True), what it gives with case_insensitive=True."""
 
-    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int, words: Optional[tuple] = None, fold: bool = False):
+    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int, words: Optional[tuple] = None, fold: int = _FOLD_NONE):
         self._R = R
-        self.ascii_case_insensitive = fold
+        self._fold = fold
+        self.ascii_case_insensitive = fold == _FOLD_ASCII
+        self.case_insensitive = fold == _FOLD_UNICODE
         self._A = R._A
         self._version = R._version
         self.n_streams = n_streams

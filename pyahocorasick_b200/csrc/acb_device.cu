@@ -1399,8 +1399,10 @@ struct acb_table {
     acb_match *ww_out = nullptr; size_t ww_out_cap = 0;  /* the host routes: the whole-word records */
     cudaEvent_t ww_ev[2] = {};                           /* kernel timing of the filter */
     int cta_limit = 0;                       /* acb_table_set_cta_limit: 0, or the SMs the launches act as if the device had */
-    /* ASCII case folding (acb_table_upload_folded): every scan reads a folded copy of the text */
+    /* case folding: every scan reads a folded copy of the text.  fold: 0 none, 1 ASCII (acb_table_upload_folded), 2 a
+     * letter map (acb_table_upload_folded_map), whose device tables are d_fold_map, fold_map16 16-byte blocks */
     int fold = 0;
+    uint4 *d_fold_map = nullptr; int fold_map16 = 0;
     int32_t n_rep = 0;                                   /* ids the alias CSR covers: the trie's n_keys */
     int64_t n_alias = 0;                                 /* alias ids; 0: no key set member has a case variant */
     int32_t *d_alias_ptr = nullptr, *d_alias_ids = nullptr;   /* per representative id, its other ids, ascending */
@@ -1478,6 +1480,7 @@ extern "C" void acb_table_free(acb_table *tb) {
     if (tb->k_t0) cudaEventDestroy(tb->k_t0);
     if (tb->k_t1) cudaEventDestroy(tb->k_t1);
     cudaFree(tb->d_alias_ptr); cudaFree(tb->d_alias_ids); tb->f_buf.release(); tb->x_buf.release(); cudaFree(tb->x_out);
+    cudaFree(tb->d_fold_map);
     for (cudaEvent_t e : tb->f_ev) if (e) cudaEventDestroy(e);
     delete tb;
 }
@@ -1810,15 +1813,75 @@ __global__ void __launch_bounds__(256) acb_fold_kernel(const uint4 *in, uint4 *o
         }
     }
 }
+
+/* ------------------------------------------------------------- mapped case folding (acb_table_upload_folded_map) */
+/* A letter map folds each letter alone: 1-byte letters through a 256-byte table; 4-byte letters below 0x110000 through
+ * two levels -- page[v >> 8] picks one of the 256-entry blocks, whose entry is the drop (v - folded v), block 0 all zero
+ * -- and letters from 0x110000 up (not code points) stay as they are.  The device buffer holds the blocks, then the
+ * 4352 page indices; every CTA stages it in shared memory before it reads the text. */
+constexpr int kFoldPages = 0x110000 >> 8;
+constexpr int kFoldMaxBlocks = (48 * 1024 - kFoldPages) / 1024;   /* the tables fit the 48 KiB a launch gets without opt-in */
+
+template <int L>
+__device__ __forceinline__ uint32_t map_word(uint32_t v, const uint32_t *drop, const uint8_t *page) {
+    if (L == 1) {
+        const uint8_t *m = page;
+        return m[v & 255] | (uint32_t)m[(v >> 8) & 255] << 8 | (uint32_t)m[(v >> 16) & 255] << 16 | (uint32_t)m[v >> 24] << 24;
+    }
+    return v < 0x110000u ? v - drop[(uint32_t)page[v >> 8] << 8 | (v & 255)] : v;
+}
+
+template <int L>
+__device__ __forceinline__ uint4 map_block(uint4 v, const uint32_t *drop, const uint8_t *page) {
+    return make_uint4(map_word<L>(v.x, drop, page), map_word<L>(v.y, drop, page), map_word<L>(v.z, drop, page),
+                      map_word<L>(v.w, drop, page));
+}
+
+/* acb_fold_kernel's loop with the letter map `map` (map16 16-byte blocks) staged in shared memory; in == out is allowed */
+template <int L>
+__global__ void __launch_bounds__(256) acb_map_fold_kernel(const uint4 *in, uint4 *out, long long n16, int tail,
+                                                          const uint4 *__restrict__ map, int map16) {
+    extern __shared__ uint4 s_map[];
+    for (int j = threadIdx.x; j < map16; j += blockDim.x) s_map[j] = map[j];
+    __syncthreads();
+    const uint32_t *drop = reinterpret_cast<const uint32_t *>(s_map);
+    const uint8_t *page = L == 1 ? reinterpret_cast<const uint8_t *>(s_map)
+                                 : reinterpret_cast<const uint8_t *>(s_map + map16) - kFoldPages;
+    const long long step = (long long)gridDim.x * blockDim.x;
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (; i + 3 * step < n16; i += 4 * step) {
+        uint4 v[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) v[k] = in[i + k * step];
+#pragma unroll
+        for (int k = 0; k < 4; k++) out[i + k * step] = map_block<L>(v[k], drop, page);
+    }
+    for (; i < n16; i += step) out[i] = map_block<L>(in[i], drop, page);
+    if (blockIdx.x == 0 && (int)threadIdx.x * L < tail) {
+        if (L == 1) {
+            const uint8_t b = reinterpret_cast<const uint8_t *>(in + n16)[threadIdx.x];
+            reinterpret_cast<uint8_t *>(out + n16)[threadIdx.x] = page[b];
+        } else {
+            reinterpret_cast<uint32_t *>(out + n16)[threadIdx.x] = map_word<L>(reinterpret_cast<const uint32_t *>(in + n16)[threadIdx.x], drop, page);
+        }
+    }
+}
 } // namespace
 
 /* the fold of `bytes` bytes at in (16-byte aligned) to out (16-byte aligned, may be in), on s: one launch */
 static int fold_text(const acb_table *tb, const uint8_t *in, uint8_t *out, long long bytes, cudaStream_t s) {
     const long long n16 = bytes / 16;
     const int tail = (int)(bytes % 16);
-    const unsigned grid = std::max(blocks(tb, n16), 1u);
     auto *i4 = reinterpret_cast<const uint4 *>(in);
     auto *o4 = reinterpret_cast<uint4 *>(out);
+    if (tb->fold == 2) {        /* every CTA stages the map: four per SM keep enough loads in flight and stage it less often */
+        const unsigned grid = (unsigned)std::max<long long>(std::min<long long>(blocks(tb, n16), grid_sms(tb) * 4), 1);
+        const size_t smem = (size_t)tb->fold_map16 * 16;
+        if (tb->L == 1) acb_map_fold_kernel<1><<<grid, 256, smem, s>>>(i4, o4, n16, tail, tb->d_fold_map, tb->fold_map16);
+        else acb_map_fold_kernel<4><<<grid, 256, smem, s>>>(i4, o4, n16, tail, tb->d_fold_map, tb->fold_map16);
+        return launched("case fold");
+    }
+    const unsigned grid = std::max(blocks(tb, n16), 1u);
     if (tb->L == 1) acb_fold_kernel<1><<<grid, 256, 0, s>>>(i4, o4, n16, tail);
     else acb_fold_kernel<4><<<grid, 256, 0, s>>>(i4, o4, n16, tail);
     return launched("case fold");
@@ -1879,6 +1942,65 @@ extern "C" int acb_table_upload_folded(const acb_trie *t, int device, const int3
         if ((rc = upload(&tb->d_alias_ptr, alias_ptr, (size_t)f.n_keys + 1, tb->dev_bytes))) break;
         rc = upload(&tb->d_alias_ids, alias_ids, (size_t)n_alias, tb->dev_bytes);
     } while (0);
+    if (rc != ACB_OK) { acb_table_free(tb); *out = nullptr; }
+    return rc;
+}
+
+extern "C" int acb_table_upload_folded_map(const acb_trie *t, int device, const int32_t *alias_ptr, const int32_t *alias_ids,
+                                           int64_t n_alias, const uint32_t *map_from, const uint32_t *map_to, int64_t n_map,
+                                           acb_table **out) {
+    DeviceRestore keep_device;
+    if (!t || !out || n_map < 0 || (n_map && (!map_from || !map_to))) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    acb_flat_view f;
+    int rc = acb_trie_flat_view(t, &f);
+    if (rc != ACB_OK) return rc;
+    /* the map: from strictly ascending, each to below its from and not itself mapped (a fold applied twice changes nothing),
+     * every from a code point; a 1-byte trie reads the entries below 256, which must stay there */
+    bool ok = true;
+    for (int64_t j = 0; ok && j < n_map; j++)
+        ok = (j == 0 || map_from[j] > map_from[j - 1]) && map_to[j] < map_from[j] && map_from[j] < 0x110000u &&
+             !std::binary_search(map_from, map_from + n_map, map_to[j]) && (f.letter_bytes != 1 || map_from[j] >= 256 || map_to[j] < 256);
+    if (!ok) {
+        acb_set_error("a letter map needs ascending code points, each mapped below itself to a letter the map leaves alone "
+                      "(below 256 for a 1-byte trie)");
+        return ACB_EINVAL;
+    }
+    std::vector<uint8_t> map;
+    try {
+        if (f.letter_bytes == 1) {
+            map.resize(256);
+            for (int b = 0; b < 256; b++) map[b] = (uint8_t)b;
+            for (int64_t j = 0; j < n_map && map_from[j] < 256; j++) map[map_from[j]] = (uint8_t)map_to[j];
+        } else {
+            std::vector<uint8_t> page(kFoldPages, 0);
+            int nb = 1;
+            for (int64_t j = 0; j < n_map; j++)
+                if (!page[map_from[j] >> 8]) page[map_from[j] >> 8] = (uint8_t)std::min(nb++, 255);
+            if (nb > kFoldMaxBlocks) {
+                acb_set_error("a letter map may change letters in at most %d blocks of 256 code points, not %d", kFoldMaxBlocks - 1, nb - 1);
+                return ACB_EINVAL;
+            }
+            map.resize((size_t)nb * 1024 + kFoldPages, 0);
+            auto *drop = reinterpret_cast<uint32_t *>(map.data());
+            for (int64_t j = 0; j < n_map; j++)
+                drop[(size_t)page[map_from[j] >> 8] << 8 | (map_from[j] & 255)] = map_from[j] - map_to[j];
+            std::copy(page.begin(), page.end(), map.begin() + (size_t)nb * 1024);
+        }
+    } catch (const std::exception &) {
+        acb_set_error("out of host memory while staging the tables");
+        return ACB_ENOMEM;
+    }
+    if ((rc = acb_table_upload_folded(t, device, alias_ptr, alias_ids, n_alias, out))) return rc;
+    acb_table *tb = *out;
+    tb->fold = 2;
+    tb->fold_map16 = (int)(map.size() / 16);
+    if (cudaSetDevice(device) != cudaSuccess) {            /* acb_table_upload_folded gave the caller's device back */
+        acb_set_error("cudaSetDevice(%d) failed", device);
+        rc = ACB_ECUDA;
+    } else {
+        rc = upload(&tb->d_fold_map, reinterpret_cast<const uint4 *>(map.data()), map.size() / 16, tb->dev_bytes);
+    }
     if (rc != ACB_OK) { acb_table_free(tb); *out = nullptr; }
     return rc;
 }
@@ -2863,9 +2985,10 @@ struct acb_streams {
 static int32_t tail_letters(const acb_table *tb) { return std::max<int32_t>(tb->max_key_bytes / tb->L - 1, 0); }
 
 static int streams_check_table(const acb_streams *ss, const acb_table *tb) {
-    if (tb->fold != ss->fold) {                    /* both tables can share L and T: the check below would not tell them apart */
-        acb_set_error(ss->fold ? "a case-folded stream batch takes the folded table (acb_table_upload_folded)"
-                               : "a stream batch does not take a case-folded table");
+    if (tb->fold != ss->fold) {                    /* the tables can share L and T: the check below would not tell them apart */
+        acb_set_error(!ss->fold ? "a stream batch does not take a case-folded table"
+                      : !tb->fold ? "a case-folded stream batch takes the folded table (acb_table_upload_folded)"
+                                  : "a case-folded stream batch takes a table of its own fold (ASCII or letter map)");
         return ACB_EINVAL;
     }
     if (tb->device != ss->device || tb->L != ss->L || (!ss->long_mode && tail_letters(tb) != ss->T) || (ss->long_mode && tb->S != ss->S)) {
