@@ -702,6 +702,42 @@ int acb_streams_new_folded(const acb_table *tb, int64_t n_streams, int leftmost,
  * feed zeroes both before it runs. */
 int acb_last_fold_ms(float *ms, int32_t n);
 
+/* ---- UTF-8 batches: decoded to letters on the GPU, letters encoded back (DESIGN section 4.20) ----------------------
+ * A batch of UTF-8 haystacks (d_in, 16-byte aligned: d_offsets' n_hay + 1 int64 byte offsets, any values, or rows of
+ * stride_bytes with d_offsets NULL) becomes letters of 1 or 4 bytes in two passes.  A byte starts a letter unless it is
+ * a continuation byte (0x80-0xBF) that the nearest other byte at most 3 bytes before it, in its haystack, covers with its
+ * maximal valid prefix (Unicode Table 3-7: the second byte narrowed after E0, ED, F0 and F4; C0, C1 and F5-FF never
+ * lead; never past the haystack's end).  A letter whose maximal prefix is not a whole sequence is invalid and decodes to
+ * U+FFFD.  Per haystack that is CPython's bytes.decode("utf-8", "replace"); the first invalid letter is the strict
+ * error, from the letter's first byte to the end of its prefix.  DEVICE buffers, asynchronous on `stream`, on `device`.
+ *
+ * acb_utf8_work_bytes: the workspace a batch of total_bytes and n_hay haystacks needs, for the decode and for an encode
+ * of n_hay haystacks.  acb_utf8_decode_device (pass 1, two launches) fills the workspace and d_info[5]: letters in the
+ * batch, largest letter, longest haystack in letters, and the first invalid letter's byte start and end in the batch
+ * (-1 and -1 when there is none or errors is ACB_UTF8_REPLACE).  acb_utf8_write_device (pass 2, one launch; the same
+ * batch and workspace, after the decode) stores every letter at `width` (1 or 4) bytes from d_out (16-byte aligned, room
+ * for width * letters bytes; width 1 needs every letter below 256) and d_out_offsets[n_hay + 1] in output bytes.
+ * acb_utf8_encode_device: letters of `width` bytes in d_in at d_offsets' byte offsets (n_hay + 1, multiples of width,
+ * as acb_replace_device writes them) -> UTF-8: *d_total and d_out_offsets[n_hay + 1] always written, d_out when
+ * *d_total <= out_cap (checked on the device); surrogates encode to 3 bytes and letters from 0x110000 up to U+FFFD.
+ * Two launches, one with out_cap 0.  ACB_EINVAL for NULL buffers with non-zero sizes, a width other than 1 or 4, an
+ * errors kind other than these two, a workspace smaller than acb_utf8_work_bytes gives, or an unaligned buffer;
+ * ACB_ERANGE for more than 2^31 - 2 haystacks. */
+enum { ACB_UTF8_STRICT = 0, ACB_UTF8_REPLACE = 1 };
+int acb_utf8_work_bytes(int64_t total_bytes, int64_t n_hay, int64_t *bytes);
+int acb_utf8_decode_device(int device, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                           int64_t stride_bytes, int errors, void *d_work, int64_t work_bytes, int64_t *d_info, void *stream);
+int acb_utf8_write_device(int device, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                          int64_t stride_bytes, const void *d_work, int64_t work_bytes, int width, uint8_t *d_out,
+                          int64_t *d_out_offsets, void *stream);
+int acb_utf8_encode_device(int device, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                           int width, void *d_work, int64_t work_bytes, uint8_t *d_out, int64_t out_cap,
+                           int64_t *d_out_offsets, int64_t *d_total, void *stream);
+
+/* With kernel timing on (acb_set_kernel_timing), the milliseconds of the last UTF-8 decode pass 1, pass 2 and encode on
+ * this thread (the first n, n <= 3), from CUDA events made for the call (which then waits for them); 0 when timing is off. */
+int acb_last_utf8_ms(float *ms, int32_t n);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

@@ -16,6 +16,7 @@ ALGO_AUTO, ALGO_FILTER, ALGO_DFA, ALGO_LONG = 0, 1, 2, 3
 ALGOS = {"auto": ALGO_AUTO, "filter": ALGO_FILTER, "dfa": ALGO_DFA, "long": ALGO_LONG}
 SELECT_LONGEST, SELECT_FIRST = 0, 1     # ACB_SELECT_*: the match a leftmost selection takes at a start
 MAX_SKIP = 1024            # ACB_MAX_SKIP: largest skip set of the white-space scans
+UTF8_STRICT, UTF8_REPLACE = 0, 1        # ACB_UTF8_*: the errors kind of acb_utf8_decode_device
 
 MATCH_DTYPE = np.dtype([("hay_id", "<i4"), ("end_index", "<i4"), ("key_id", "<i4")])
 
@@ -150,6 +151,11 @@ def lib() -> ctypes.CDLL:
         "acb_expand_aliases_device": (ctypes.c_int, [vp, vp, i64, vp, i64, vp, vp]),
         "acb_last_fold_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), i32]),
         "acb_streams_new_folded": (ctypes.c_int, [vp, i64, ctypes.c_int, ctypes.c_int, vp, i64, ctypes.POINTER(vp)]),
+        "acb_utf8_work_bytes": (ctypes.c_int, [i64, i64, pi64]),
+        "acb_utf8_decode_device": (ctypes.c_int, [ctypes.c_int, vp, i64, vp, i64, i64, ctypes.c_int, vp, i64, vp, vp]),
+        "acb_utf8_write_device": (ctypes.c_int, [ctypes.c_int, vp, i64, vp, i64, i64, vp, i64, ctypes.c_int, vp, vp, vp]),
+        "acb_utf8_encode_device": (ctypes.c_int, [ctypes.c_int, vp, i64, vp, i64, ctypes.c_int, vp, i64, vp, i64, vp, vp, vp]),
+        "acb_last_utf8_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), i32]),
         "acb_launch_count": (i64, []),
         "acb_set_kernel_timing": (ctypes.c_int, [ctypes.c_int]),
         "acb_last_kernel_ms": (ctypes.c_float, []),
@@ -186,7 +192,8 @@ EXPORTED_SYMBOLS = [
     "acb_scan_host_leftmost_words", "acb_replace_host_words", "acb_last_words_ms", "acb_streams_new_words",
     "acb_streams_feed_words_device", "acb_streams_feed_words_host", "acb_leftmost_first_device", "acb_scan_host_leftmost_kind",
     "acb_replacer_new_kind", "acb_streams_new_leftmost_kind", "acb_table_upload_folded", "acb_expand_aliases_device",
-    "acb_last_fold_ms", "acb_table_upload_folded_map", "acb_streams_new_folded", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_last_fold_ms", "acb_table_upload_folded_map", "acb_streams_new_folded", "acb_utf8_work_bytes", "acb_utf8_decode_device",
+    "acb_utf8_write_device", "acb_utf8_encode_device", "acb_last_utf8_ms", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

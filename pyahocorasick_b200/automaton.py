@@ -10,6 +10,7 @@ Reference semantics are cited as file:line relative to /root/reference.
 """
 from __future__ import annotations
 
+import codecs
 import contextlib
 import ctypes
 import functools
@@ -18,6 +19,7 @@ import os
 import operator
 import pickle
 import threading
+import warnings
 from typing import Any, Iterable, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
@@ -1038,14 +1040,16 @@ class Automaton:
             return lib.acb_scan_host_words(tb, *args, cap, found_ref, N.ALGOS[algo], int(sort))
         return self._host_records(device, narrow, n_hay, scan, fold)
 
-    def _filter_words_device(self, tb, t, n: int, stride: int, full, m: int, words: tuple, stream):
+    def _filter_words_device(self, tb, t, n: int, stride: int, full, m: int, words: tuple, stream, offs=None, narrow: bool = False):
         """The whole-word records among the first m of the device buffer `full` (a scan of the aligned device batch t),
-        on `stream`: (records [max(m, 1), 3] int32 CUDA tensor, their number).  Waits once, for that number."""
+        on `stream`: (records [max(m, 1), 3] int32 CUDA tensor, their number).  Waits once, for that number.  offs: the
+        batch's int64 CUDA byte offsets instead of rows of `stride` bytes; narrow: its letters are 1 byte each."""
         import torch
-        bits, n_bits = _word_bits_device(words, self._L, t.device.index)
+        bits, n_bits = _word_bits_device(words, 1 if narrow else self._L, t.device.index)
         out = torch.empty((max(m, 1), 3), dtype=torch.int32, device=t.device)
         cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
-        N.check(self._lib.acb_word_filter_device(tb, t.data_ptr(), n * stride, None, n, stride, full.data_ptr(), m,
+        N.check(self._lib.acb_word_filter_device(tb, t.data_ptr(), t.numel(), None if offs is None else offs.data_ptr(), n, stride,
+                                                 full.data_ptr(), m,
                                                  bits.data_ptr() if n_bits else None, n_bits, out.data_ptr(), m, cnt.data_ptr(),
                                                  stream))
         return out, int(cnt.item())
@@ -1076,17 +1080,19 @@ class Automaton:
         return self._device_scan(t, n, expand)
 
     def _device_matches(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None,
-                        skip: Optional[np.ndarray] = None):
+                        skip: Optional[np.ndarray] = None, offs=None, narrow: bool = False):
         """Every match of the aligned device batch t, left on the device (_device_scan): (int32 [cap, 3] CUDA tensor,
-        their number).  skip: the scan skips these letters; words: only the whole-word matches (_filter_words_device)."""
+        their number).  skip: the scan skips these letters; words: only the whole-word matches (_filter_words_device).
+        offs, narrow: as for _filter_words_device."""
         lib = self._lib
+        d_off = None if offs is None else offs.data_ptr()
 
         def scan(out, cap, cnt):
-            args = (tb, t.data_ptr(), n * stride, None, n, stride, out.data_ptr(), cap, cnt.data_ptr(), stream, N.ALGOS[algo])
+            args = (tb, t.data_ptr(), t.numel(), d_off, n, stride, out.data_ptr(), cap, cnt.data_ptr(), stream, N.ALGOS[algo])
             N.check(lib.acb_scan_device(*args) if skip is None else lib.acb_scan_device_skip(*args, N.ptr(skip), len(skip)))
         out, found = self._device_scan(t, n, scan)
         if words is not None:
-            out, found = self._filter_words_device(tb, t, n, stride, out, found, words, stream)
+            out, found = self._filter_words_device(tb, t, n, stride, out, found, words, stream, offs, narrow)
         return out, found
 
     def _device_records(self, tb, out, found: int, n_hay: int, max_letters: int, stream, sort: bool) -> np.ndarray:
@@ -1215,17 +1221,21 @@ class Automaton:
         return AutomatonSearchIterLong(self, letters, start, end)
 
     def find_long_batch(self, haystacks, *, sort: bool = True, device: Optional[int] = None, whole_words=False,
-                        ascii_case_insensitive: bool = False, case_insensitive: bool = False) -> "Matches":
+                        ascii_case_insensitive: bool = False, case_insensitive: bool = False, encoding: Optional[str] = None,
+                        errors: str = "strict") -> "Matches":
         """iter_long() over a whole batch (same input forms and result type as find_all_batch).  whole_words,
         ascii_case_insensitive and case_insensitive are refused (ValueError): iter_long's walk picks its matches itself,
-        so a filter after it has no clear meaning, and its walk follows the automaton of the keys as given."""
+        so a filter after it has no clear meaning, and its walk follows the automaton of the keys as given.  encoding and
+        errors: UTF-8 haystacks, as for find_all_batch (always at 4 bytes per letter)."""
         return self.find_all_batch(haystacks, algo="long", sort=sort, device=device, whole_words=whole_words,
-                                   ascii_case_insensitive=ascii_case_insensitive, case_insensitive=case_insensitive)
+                                   ascii_case_insensitive=ascii_case_insensitive, case_insensitive=case_insensitive,
+                                   encoding=encoding, errors=errors)
 
     @_locked
     def find_leftmost_longest_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
                                     whole_words=False, ascii_case_insensitive: bool = False,
-                                    case_insensitive: bool = False) -> "Matches":
+                                    case_insensitive: bool = False, encoding: Optional[str] = None,
+                                    errors: str = "strict") -> "Matches":
         """Leftmost-longest non-overlapping matches of a whole batch, selected on the GPU (input forms and result type
         of find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or
         after p, take the smallest such start, the longest match there, and continue after its end.  Records come in
@@ -1238,12 +1248,19 @@ class Automaton:
         tensor batch then waits once more, for the number of whole-word matches.
 
         ascii_case_insensitive and case_insensitive (see find_all_batch): the same rule over the folded text.  Of the keys
-        that fold to the same text, only the one added first is reported."""
+        that fold to the same text, only the one added first is reported.
+
+        encoding and errors (see find_all_batch): UTF-8 haystacks, decoded on the GPU; the result is that of the same
+        call on the decoded list of str."""
         self._require_automaton()
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-longest takes 'auto', 'filter' or 'dfa'")
         words = self._words(whole_words)
         fold = self._fold_arg(ascii_case_insensitive, case_insensitive=case_insensitive)
+        u8 = self._utf8_arg(encoding, errors)
+        if u8 is not None:
+            return Matches(self._leftmost_utf8(self._utf8_batch(haystacks, u8, device), algo, words, N.SELECT_LONGEST, fold),
+                           self._result_values())
         b = self._batch_input(haystacks)
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
@@ -1262,7 +1279,8 @@ class Automaton:
     @_locked
     def find_leftmost_first_batch(self, haystacks, *, algo: str = "auto", device: Optional[int] = None,
                                   whole_words=False, ascii_case_insensitive: bool = False,
-                                  case_insensitive: bool = False) -> "Matches":
+                                  case_insensitive: bool = False, encoding: Optional[str] = None,
+                                  errors: str = "strict") -> "Matches":
         """Leftmost-first non-overlapping matches of a whole batch, selected on the GPU (input forms and result type of
         find_all_batch).  Per haystack, from the matches ``iter()`` reports: p = 0; while some match starts at or after
         p, take the smallest such start, the match there whose key was added first, and continue after its end.  This is
@@ -1271,12 +1289,17 @@ class Automaton:
         add_word of a key already present keeps its place, removing a key and adding it again moves it to the end.  An
         automaton read back from pickle or save numbers its keys afresh, so its priority can differ.  Records come in
         haystack order, then end_index ascending; algo, whole_words, ascii_case_insensitive and case_insensitive as for
-        find_leftmost_longest_batch (the key added first wins among keys of one folded text, as at any start)."""
+        find_leftmost_longest_batch (the key added first wins among keys of one folded text, as at any start).  encoding
+        and errors (see find_all_batch): UTF-8 haystacks, with the result of the same call on the decoded list of str."""
         self._require_automaton()
         if algo not in ("auto", "filter", "dfa"):
             raise ValueError(f"algo {algo!r}: leftmost-first takes 'auto', 'filter' or 'dfa'")
         words = self._words(whole_words)
         fold = self._fold_arg(ascii_case_insensitive, case_insensitive=case_insensitive)
+        u8 = self._utf8_arg(encoding, errors)
+        if u8 is not None:
+            return Matches(self._leftmost_utf8(self._utf8_batch(haystacks, u8, device), algo, words, N.SELECT_FIRST, fold),
+                           self._result_values())
         b = self._batch_input(haystacks)
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
@@ -1321,19 +1344,142 @@ class Automaton:
             return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
 
     def _leftmost_chosen(self, tb, t, n: int, stride: int, algo: str, stream, words: Optional[tuple] = None,
-                         select: int = N.SELECT_LONGEST):
+                         select: int = N.SELECT_LONGEST, offs=None, max_letters: Optional[int] = None, narrow: bool = False):
         """The chosen records of an aligned device batch, left on the device: (records [cap, 3] int32 CUDA tensor,
         their count as an int64 CUDA tensor, cap).  Synchronises once, to size the full list; with words, the
         selection runs on the whole-word matches and a second wait sizes them (_device_matches).  select: the rule,
-        acb_leftmost_longest_device or acb_leftmost_first_device."""
+        acb_leftmost_longest_device or acb_leftmost_first_device.  offs, narrow: as for _device_matches, with
+        max_letters the longest haystack."""
         import torch
-        full, m = self._device_matches(tb, t, n, stride, algo, stream, words)
+        if max_letters is None:
+            max_letters = stride // self._L
+        full, m = self._device_matches(tb, t, n, stride, algo, stream, words, offs=offs, narrow=narrow)
         cap = max(m, 1)
         out = torch.empty((cap, 3), dtype=torch.int32, device=t.device)
         cnt = torch.zeros(1, dtype=torch.int64, device=t.device)
         fn = self._lib.acb_leftmost_longest_device if select == N.SELECT_LONGEST else self._lib.acb_leftmost_first_device
-        N.check(fn(tb, full.data_ptr(), m, n, stride // self._L, out.data_ptr(), cap, cnt.data_ptr(), stream))
+        N.check(fn(tb, full.data_ptr(), m, n, max_letters, out.data_ptr(), cap, cnt.data_ptr(), stream))
         return out, cnt, cap
+
+    # ------------------------------------------------------------------ UTF-8 batches (DESIGN section 4.20)
+    def _utf8_arg(self, encoding, errors) -> Optional[int]:
+        """The encoding and errors arguments of the batch methods: None for haystacks of letters, else the errors kind
+        of a UTF-8 batch (N.UTF8_STRICT or N.UTF8_REPLACE), checked against the automaton"""
+        if errors not in ("strict", "replace"):
+            raise ValueError(f"errors {errors!r}: a UTF-8 batch takes 'strict' or 'replace'")
+        if encoding is None:
+            if errors != "strict":
+                raise ValueError("errors applies to UTF-8 haystacks: pass encoding='utf-8'")
+            return None
+        try:
+            name = codecs.lookup(encoding).name
+        except (LookupError, TypeError):
+            name = None
+        if name != "utf-8":
+            raise ValueError(f"encoding {encoding!r}: haystacks are decoded from UTF-8 only")
+        if not self._UNICODE:
+            raise ValueError("encoding is for the unicode flavour: the bytes flavour matches bytes as they are, and its keys "
+                             "can be UTF-8 bytes already")
+        if self._key_type == KEY_SEQUENCE:
+            raise ValueError("encoding needs text: KEY_SEQUENCE letters are integers, not letters")
+        return N.UTF8_STRICT if errors == "strict" else N.UTF8_REPLACE
+
+    @staticmethod
+    def _utf8_upload(haystacks, device: Optional[int]):
+        """The input forms of a UTF-8 batch on the GPU: (flat uint8 CUDA tensor, int64 CUDA byte offsets or None for rows
+        of `stride` bytes, n, stride, the host batch as (flat, offsets or None) or None for a CUDA tensor).  A host batch
+        is uploaded once, to `device`."""
+        import torch
+        if type(haystacks).__module__.startswith("torch") and getattr(haystacks, "is_cuda", False):
+            t = haystacks
+            if t.dtype != torch.uint8 or t.dim() != 2 or not t.is_contiguous():
+                raise TypeError("device batches must be 2-D contiguous uint8 tensors [n_haystacks, stride_bytes]")
+            return _aligned(t).reshape(-1), None, int(t.shape[0]), int(t.shape[1]), None
+        if isinstance(haystacks, np.ndarray):
+            if haystacks.dtype != np.uint8 or haystacks.ndim != 2 or not haystacks.flags.c_contiguous:
+                raise TypeError("array batches must be 2-D C-contiguous uint8 [n_haystacks, stride_bytes]")
+            (n, stride), flat, offs = haystacks.shape, haystacks.reshape(-1), None
+        elif _is_pair(haystacks):
+            flat = np.ascontiguousarray(haystacks[0], dtype=np.uint8).reshape(-1)
+            offs = np.ascontiguousarray(haystacks[1], dtype=np.int64)
+            if offs.ndim != 1 or len(offs) < 1 or offs[0] != 0 or offs[-1] != flat.size or np.any(np.diff(offs) < 0):
+                raise ValueError("offsets must be non-decreasing, start at 0 and end at len(flat)")
+            n, stride = len(offs) - 1, 0
+        elif isinstance(haystacks, (list, tuple)):
+            types = set(map(type, haystacks))
+            if not types <= {bytes, bytearray}:
+                if str in types:
+                    raise TypeError("a UTF-8 batch holds bytes, and a str is already decoded: pass it without encoding")
+                raise TypeError("a UTF-8 batch is a list or tuple of bytes or bytearray, a uint8 array [n, stride], a "
+                                "(flat, offsets) pair or a uint8 CUDA tensor [n, stride]")
+            n, stride = len(haystacks), 0
+            offs = np.zeros(n + 1, dtype=np.int64)
+            np.cumsum(np.fromiter(map(len, haystacks), dtype=np.int64, count=n), out=offs[1:])
+            flat = np.frombuffer(bytearray().join(haystacks), dtype=np.uint8)
+        else:
+            raise TypeError("a UTF-8 batch is a list or tuple of bytes or bytearray, a uint8 array [n, stride], a "
+                            "(flat, offsets) pair or a uint8 CUDA tensor [n, stride]")
+        dev = f"cuda:{_default_device() if device is None else device}"
+        with warnings.catch_warnings():                      # a read-only array is only read: the upload copies it
+            warnings.simplefilter("ignore", UserWarning)
+            t = torch.from_numpy(flat).to(dev)
+            d_offs = None if offs is None else torch.from_numpy(offs).to(dev)
+        return t, d_offs, n, stride, (flat, offs)
+
+    def _utf8_batch(self, haystacks, errors: int, device: Optional[int], narrow_ok: bool = True) -> "_Utf8Batch":
+        """A UTF-8 batch decoded on the GPU (acb_utf8_decode_device, acb_utf8_write_device) on torch's current stream of
+        its device: at 1 byte per letter when narrow_ok and every letter is below 256, else at 4.  Waits once, for the
+        info block; under "strict" an invalid sequence raises UnicodeDecodeError before pass 2."""
+        import torch
+        t, offs, n, stride, host = self._utf8_upload(haystacks, device)
+        lib, dev, total = self._lib, _device_of(t), int(t.numel())
+        need = ctypes.c_int64(0)
+        N.check(lib.acb_utf8_work_bytes(total, n, ctypes.byref(need)))
+        with _on_device(dev) as stream:
+            work = torch.empty(int(need.value), dtype=torch.uint8, device=t.device)
+            info = torch.empty(5, dtype=torch.int64, device=t.device)
+            batch = (t.data_ptr() if total else None, total, None if offs is None else offs.data_ptr(), n, stride)
+            N.check(lib.acb_utf8_decode_device(dev, *batch, errors, work.data_ptr(), work.numel(), info.data_ptr(), stream))
+            letters, top, longest, err_start, err_end = info.tolist()
+            if err_start >= 0:
+                raise _utf8_error(t, host, stride, err_start, err_end)
+            narrow = narrow_ok and top < 256
+            width = 1 if narrow else 4
+            out = torch.empty(max(letters * width, 16), dtype=torch.uint8, device=t.device)
+            out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+            N.check(lib.acb_utf8_write_device(dev, *batch, work.data_ptr(), work.numel(), width, out.data_ptr(),
+                                              out_offs.data_ptr(), stream))
+        return _Utf8Batch(out[:letters * width], out_offs, n, longest, narrow)
+
+    @_locked
+    def _scan_utf8(self, b: "_Utf8Batch", algo: str, sort: bool, words: Optional[tuple], white_space: bool,
+                   fold: int) -> np.ndarray:
+        """find_all over a decoded UTF-8 batch: scan (skipping white space), word filter, alias expansion and sort on the
+        device, as _scan_device_tensor does for a batch of rows"""
+        t = b.data
+        dev = _device_of(t)
+        tb = self._table_for(dev, b.narrow, fold)
+        if tb is None or b.n == 0 or t.numel() == 0:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        skip = self._skip_set(b.narrow) if white_space else None
+        with _on_device(dev) as stream:
+            out, found = self._device_matches(tb, t, b.n, 0, algo, stream, words, skip, b.offsets, b.narrow)
+            if fold and found and self._has_aliases(b.narrow, fold):
+                out, found = self._expand_device(tb, t, b.n, out, found, stream)
+            return self._device_records(tb, out, found, b.n, b.max_letters, stream, sort)
+
+    @_locked
+    def _leftmost_utf8(self, b: "_Utf8Batch", algo: str, words: Optional[tuple], select: int, fold: int) -> np.ndarray:
+        """a leftmost selection over a decoded UTF-8 batch, as _leftmost_device"""
+        t = b.data
+        dev = _device_of(t)
+        tb = self._table_for(dev, b.narrow, fold)
+        if tb is None or b.n == 0 or t.numel() == 0:
+            return np.empty(0, dtype=N.MATCH_DTYPE)
+        with _on_device(dev) as stream:
+            out, cnt, _ = self._leftmost_chosen(tb, t, b.n, 0, algo, stream, words, select, b.offsets, b.max_letters, b.narrow)
+            found = int(cnt.item())
+            return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
 
     @_locked
     def replacer(self, replacements=None, *, device: Optional[int] = None, leftmost_first: bool = False) -> "Replacer":
@@ -1365,7 +1511,7 @@ class Automaton:
     @_locked
     def find_all_batch(self, haystacks, *, algo: str = "auto", sort: bool = True, device: Optional[int] = None,
                        ignore_white_space: bool = False, whole_words=False, ascii_case_insensitive: bool = False,
-                       case_insensitive: bool = False) -> Matches:
+                       case_insensitive: bool = False, encoding: Optional[str] = None, errors: str = "strict") -> Matches:
         """Search a whole batch on the GPU.
 
         haystacks: a sequence of bytes / str / tuple objects (as `iter` accepts), or a 2-D
@@ -1403,6 +1549,19 @@ class Automaton:
         end_index and whole words of the text as given, the text folded on the GPU and the caller's copy unchanged.
         ValueError for the bytes flavour (bytes have no known encoding: use ascii_case_insensitive), together with
         ascii_case_insensitive, with ignore_white_space, algo="long" or a KEY_SEQUENCE automaton.
+
+        encoding="utf-8" (unicode flavour, KEY_STRING keys; any name codecs.lookup gives as utf-8): the haystacks are
+        UTF-8 bytes -- a list or tuple of bytes or bytearray (a str item raises TypeError), a (flat uint8, int64 byte
+        offsets) pair, a C-contiguous uint8 array [n, stride] of one haystack per row (NUL bytes included) or a
+        contiguous uint8 CUDA tensor [n, stride] -- decoded on the GPU.  The result is exactly that of the same call on
+        ``[h.decode("utf-8", errors) for h in haystacks]``: end_index counts letters (code points).  errors="strict"
+        raises the UnicodeDecodeError CPython raises for the first haystack with an invalid sequence (its bytes, start
+        and end) before anything is scanned; errors="replace" decodes each invalid sequence to one U+FFFD, as CPython
+        does, so a key holding U+FFFD matches it.  A batch whose letters are all below 256 runs on the latin-1 automaton
+        at 1 byte per letter (not with algo="long"); the width changes speed, never results.  Host input is uploaded
+        once and searched unpipelined.  ValueError for the bytes flavour (it matches the bytes themselves), KEY_SEQUENCE
+        automata, another encoding, or errors other than "strict" and "replace"; errors other than "strict" also needs
+        an encoding.
         """
         self._require_automaton()
         if ignore_white_space and algo == "long":
@@ -1413,6 +1572,10 @@ class Automaton:
         if words is not None and algo == "long":
             raise ValueError("whole_words cannot be combined with algo='long': iter_long's walk picks its matches itself")
         fold = self._fold_arg(ascii_case_insensitive, algo, ignore_white_space, case_insensitive)
+        u8 = self._utf8_arg(encoding, errors)
+        if u8 is not None:
+            b = self._utf8_batch(haystacks, u8, device, narrow_ok=algo != "long")
+            return Matches(self._scan_utf8(b, algo, sort, words, ignore_white_space, fold), self._result_values())
         b = self._batch_input(haystacks, narrow_ok=algo != "long")
         if b.empty:
             rec = np.empty(0, dtype=N.MATCH_DTYPE)
@@ -2066,7 +2229,7 @@ class Replacer:
         return r
 
     def replace_batch(self, haystacks, *, algo: str = "auto", whole_words=False, ascii_case_insensitive: bool = False,
-                      case_insensitive: bool = False):
+                      case_insensitive: bool = False, encoding: Optional[str] = None, errors: str = "strict"):
         """The batch with every leftmost-longest match replaced.  `haystacks` takes the input forms of find_all_batch;
         a list gives a list of the same item type, uint8[n, stride] or (flat, offsets) gives (flat uint8, offsets
         int64[n+1]), a CUDA tensor gives that pair as CUDA tensors computed on torch's current stream (the call
@@ -2076,7 +2239,13 @@ class Replacer:
         (see find_all_batch): replace the matches the find_leftmost_*_batch method of this replacer's rule chooses with
         the same option, each by the replacement of its key -- the one added first among keys that fold to the same
         text; every other letter is copied as given, in its own case.  case_insensitive (unicode flavour; see
-        find_all_batch): the same with Unicode simple case folding."""
+        find_all_batch): the same with Unicode simple case folding.
+
+        encoding and errors (see find_all_batch): UTF-8 haystacks, decoded on the GPU, and UTF-8 output, encoded on the
+        GPU: exactly ``[s.encode("utf-8") for s in R.replace_batch(decoded)]`` with the same options, where decoded is
+        ``[h.decode("utf-8", errors) for h in haystacks]``.  A list gives a list of bytes, uint8[n, stride] or (flat,
+        offsets) gives (flat uint8, int64 byte offsets[n+1]), a CUDA tensor gives that pair as CUDA tensors.  A
+        replacement that UTF-8 cannot encode (a lone surrogate) raises UnicodeEncodeError."""
         A = self._A
         with A._gpu_lock:
             if self._version != A._version:
@@ -2087,6 +2256,17 @@ class Replacer:
             words = A._words(whole_words)
             fold = A._fold_arg(ascii_case_insensitive, case_insensitive=case_insensitive)
             pair = isinstance(haystacks, np.ndarray) or _is_pair(haystacks)
+            u8 = A._utf8_arg(encoding, errors)
+            if u8 is not None:
+                self._check_utf8_replacements()
+                b = A._utf8_batch(haystacks, u8, self._device, narrow_ok=True in self._tables)
+                out, out_offs = self._run_utf8(b, algo, words, fold)
+                if out.device.type == "cuda" and (pair or isinstance(haystacks, (list, tuple))):
+                    out, out_offs = out.cpu().numpy(), out_offs.cpu().numpy()
+                    if not pair:
+                        raw, o = out.tobytes(), out_offs.tolist()
+                        return [raw[o[i]:o[i + 1]] for i in range(len(o) - 1)]
+                return out, out_offs
             batch = A._batch_input(haystacks)
             if batch.kind == "device":
                 return self._run_device(batch, algo, words, fold)
@@ -2108,6 +2288,52 @@ class Replacer:
             if pair:
                 return out, out_offs
             return self._items(out, out_offs, narrow)
+
+    def _check_utf8_replacements(self) -> None:
+        """UnicodeEncodeError, as str.encode("utf-8") raises it, for a replacement with a lone surrogate"""
+        flat, offs = self._tables[False]
+        v = flat.view("<u4")
+        bad = np.flatnonzero((v >= 0xD800) & (v <= 0xDFFF))
+        if bad.size:
+            k = int(np.searchsorted(offs, 4 * int(bad[0]), side="right")) - 1
+            flat[offs[k]:offs[k + 1]].tobytes().decode("utf-32-le", "surrogatepass").encode("utf-8")
+
+    def _run_utf8(self, b, algo: str, words: Optional[tuple], fold: int):
+        """A decoded UTF-8 batch (Automaton._utf8_batch): select and rewrite as _run_device does, then encode the output
+        letters to UTF-8 on the GPU (acb_utf8_encode_device); (flat, offsets) CUDA tensors.  Waits twice: for the size of
+        the rewritten letters and for that of the UTF-8 output."""
+        import torch
+        A = self._A
+        t, n = b.data, b.n
+        dev = _device_of(t)
+        width = 1 if b.narrow else 4
+        tb = A._table_for(dev, b.narrow, fold) if n and t.numel() else None
+        with _on_device(dev) as stream:
+            letters, offs = t, b.offsets                    # nothing to replace: the decoded text
+            if tb is not None:
+                chosen, cnt, cap = A._leftmost_chosen(tb, t, n, 0, algo, stream, words, self._select, b.offsets, b.max_letters,
+                                                      b.narrow)
+                r = self._replacer(tb, b.narrow, dev)
+                offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+                total = torch.empty(1, dtype=torch.int64, device=t.device)
+                args = (r, tb, t.data_ptr(), t.numel(), b.offsets.data_ptr(), n, 0, chosen.data_ptr(), cap, cnt.data_ptr(),
+                        offs.data_ptr())
+                N.check(A._lib.acb_replace_device(*args, None, 0, total.data_ptr(), stream))
+                m = int(total.item())
+                letters = torch.empty(max(m, 16), dtype=torch.uint8, device=t.device)[:m]
+                if m:
+                    N.check(A._lib.acb_replace_device(*args, letters.data_ptr(), m, total.data_ptr(), stream))
+            need = ctypes.c_int64(0)
+            N.check(A._lib.acb_utf8_work_bytes(0, n, ctypes.byref(need)))
+            work = torch.empty(int(need.value), dtype=torch.uint8, device=t.device)
+            cap = letters.numel() // width * (2 if width == 1 else 4)     # the most UTF-8 bytes a letter takes at this width
+            out = torch.empty(max(cap, 1), dtype=torch.uint8, device=t.device)
+            out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+            total = torch.empty(1, dtype=torch.int64, device=t.device)
+            N.check(A._lib.acb_utf8_encode_device(dev, letters.data_ptr() if letters.numel() else None, letters.numel(),
+                                                  offs.data_ptr(), n, width, work.data_ptr(), work.numel(), out.data_ptr(),
+                                                  cap, out_offs.data_ptr(), total.data_ptr(), stream))
+            return out[:int(total.item())], out_offs
 
     def stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
                      whole_words=False) -> "ReplaceStream":
@@ -2512,6 +2738,37 @@ def _take_records(lib, tb, found: int) -> np.ndarray:
     if not ptr.value or n.value != found:
         raise N.NativeError("acb_take_records: no records to take")
     return np.asarray(_PinnedRecords(lib, ptr.value, n.value, room.value))
+
+
+class _Utf8Batch(NamedTuple):
+    """A UTF-8 batch decoded on the GPU (Automaton._utf8_batch): data, its letters (1-D uint8 CUDA tensor, 16-byte
+    aligned); offsets, their int64 CUDA byte offsets [n + 1]; max_letters, the longest haystack; narrow: 1 byte per
+    letter."""
+    data: Any
+    offsets: Any
+    n: int
+    max_letters: int
+    narrow: bool
+
+
+def _utf8_error(t, host, stride: int, start: int, end: int) -> UnicodeDecodeError:
+    """CPython's UnicodeDecodeError for the invalid sequence at bytes [start, end) of a UTF-8 batch: the haystack that
+    holds it, and the sequence's place in it"""
+    if host is not None and host[1] is not None:
+        flat, offs = host
+        h = int(np.searchsorted(offs, start, side="right")) - 1
+        hs, he = int(offs[h]), int(offs[h + 1])
+    else:
+        hs = start // stride * stride
+        he = hs + stride
+    hay = bytes((host[0][hs:he] if host is not None else t[hs:he].cpu().numpy()).tobytes())
+    if not 0xC2 <= hay[start - hs] <= 0xF4:
+        reason = "invalid start byte"
+    elif end - hs == len(hay):
+        reason = "unexpected end of data"
+    else:
+        reason = "invalid continuation byte"
+    return UnicodeDecodeError("utf-8", hay, start - hs, end - hs, reason)
 
 
 class _Batch(NamedTuple):

@@ -5386,3 +5386,547 @@ extern "C" int acb_streams_replace_host(acb_streams *ss, acb_replacer *r, acb_ta
     CUDA_TRY(cudaStreamSynchronize(s));
     return ACB_OK;
 }
+
+/* ------------------------------------------------------------ UTF-8 batches (DESIGN section 4.20) */
+/* A batch of UTF-8 haystacks decoded to letters of 1 or 4 bytes, byte by byte and in parallel: a byte starts a letter
+ * unless it is a continuation byte (0x80-0xBF) that the nearest non-continuation byte at most 3 bytes before it, in its
+ * haystack, covers with its maximal valid prefix (Unicode Table 3-7, never past the haystack's end).  A letter whose
+ * maximal prefix is not a whole sequence is invalid and decodes to U+FFFD.  Haystack by haystack this is CPython's
+ * bytes.decode("utf-8", "replace"), and the first invalid letter is its strict error: start at the letter, end after
+ * its prefix.
+ * Pass 1 (acb_utf8_decode_kernel) keeps the white-space compaction's metadata -- a start mask per 32-byte group, uint16
+ * group prefixes within a tile, int64 tile prefixes from a decoupled look-back (CompactMeta, kept_before) -- and
+ * reduces the largest letter and the first error; acb_utf8_offsets_kernel gives each haystack's first letter, the
+ * longest haystack and the letter total.  Pass 2 (acb_utf8_write_kernel) classifies the bytes again, decodes every
+ * start and stores it at its rank, staged per tile in shared memory so the stores are coalesced. */
+namespace {
+constexpr int kU8Stage = 1024;                            /* haystack offsets around a tile staged in shared memory */
+constexpr int kU8Look = 36;                               /* bytes past a group whose haystack starts a group needs */
+
+struct U8Args {
+    const uint8_t *in;            /* 16-byte aligned */
+    long long total;
+    const long long *off;         /* n_hay + 1 byte offsets, or nullptr: rows of `stride` bytes */
+    long long stride, n_hay;
+    uint32_t *mask;
+    uint16_t *gpre;
+    long long *tile_pre;          /* [n_tiles + 1] */
+    unsigned long long *status;   /* [n_tiles], zeroed */
+    unsigned int *ctr;            /* zeroed */
+    unsigned long long *err;      /* first invalid letter: start << 2 | (prefix length - 1); all ones for none */
+    long long *loff;              /* [n_hay + 1]: first letter of each haystack */
+    long long *info;              /* [5]: letters, largest letter, longest haystack in letters, error start, error end */
+    long long n_tiles;
+    int strict;
+};
+
+/* byte i (-4 <= i < 36) of a group's window: w[0] holds the 4 bytes before the group, w[1..8] its 32, w[9] the 4 after */
+__device__ __forceinline__ uint32_t u8_at(const uint32_t (&w)[10], int i) { return (w[(i + 4) >> 2] >> (8 * ((i + 4) & 3))) & 255u; }
+
+/* the window of the group at p0 (a multiple of 32), zero outside the batch */
+__device__ __forceinline__ void u8_load(const uint8_t *in, long long total, long long p0, uint32_t (&w)[10]) {
+    if (p0 >= 4 && p0 + 36 <= total) {
+        const uint4 *src = reinterpret_cast<const uint4 *>(in + p0);
+        const uint4 v0 = src[0], v1 = src[1];
+        w[0] = __ldg(reinterpret_cast<const uint32_t *>(in + p0) - 1);
+        w[1] = v0.x; w[2] = v0.y; w[3] = v0.z; w[4] = v0.w; w[5] = v1.x; w[6] = v1.y; w[7] = v1.z; w[8] = v1.w;
+        w[9] = __ldg(reinterpret_cast<const uint32_t *>(in + p0 + 32));
+        return;
+    }
+#pragma unroll
+    for (int k = 0; k < 10; k++) w[k] = 0;
+#pragma unroll
+    for (int i = -4; i < 36; i++)                          /* unrolled: w stays in registers */
+        if (p0 + i >= 0 && p0 + i < total) w[(i + 4) >> 2] |= (uint32_t)in[p0 + i] << (8 * ((i + 4) & 3));
+}
+
+/* haystack offsets read from the tile's staged copy when it fits, else from global memory */
+struct U8Offs {
+    const long long *s, *g;
+    long long base;
+    bool staged;
+    __device__ __forceinline__ long long at(long long h) const { return staged ? s[h - base] : __ldg(g + h); }
+    /* the first h in [lo, hi) with at(h) > x (upper) or >= x (lower), else hi */
+    __device__ __forceinline__ long long first(long long lo, long long hi, long long x, bool upper) const {
+        while (lo < hi) {
+            const long long mid = (lo + hi) >> 1, v = at(mid);
+            if (v < x || (upper && v == x)) lo = mid + 1; else hi = mid;
+        }
+        return lo;
+    }
+};
+
+/* The haystack starts among bytes p0 - 3 .. p0 + 36 as bits 1 .. 40 (bit 4 + i: a haystack starts at byte p0 + i); the
+ * batch's end counts as one.  o: the tile's offsets, holding every offset in [t0 - 3, t0 + kCmpTile + kU8Look] in
+ * [lo, hi) */
+__device__ __forceinline__ unsigned long long u8_bounds(const U8Args &a, const U8Offs &o, long long lo, long long hi, long long p0) {
+    unsigned long long b = 0;
+    if (!a.off) {
+        for (long long x = (max(p0 - 3, 0LL) + a.stride - 1) / a.stride * a.stride; x <= p0 + kU8Look && x <= a.total; x += a.stride)
+            b |= 1ULL << (x - p0 + 4);
+        return b;
+    }
+    for (long long h = o.first(lo, hi, p0 - 3, false); h < hi;) {
+        const long long x = o.at(h);
+        if (x > p0 + kU8Look) break;
+        b |= 1ULL << (x - p0 + 4);
+        h = o.first(h + 1, hi, x, true);                   /* past the empty haystacks that start there too */
+    }
+    return b;
+}
+
+/* The tile's haystack offsets, staged in shared memory when they fit (ragged batches; block-wide, every thread calls) */
+__device__ __forceinline__ U8Offs u8_stage(const U8Args &a, long long t0, long long *s_off, long long *s_range, long long *lo, long long *hi) {
+    U8Offs o{s_off, a.off, 0, false};
+    if (!a.off) return o;
+    if (threadIdx.x == 0) {
+        U8Offs g{nullptr, a.off, 0, false};
+        s_range[0] = g.first(0, a.n_hay + 1, max(t0 - 3, 0LL), false);
+        s_range[1] = g.first(s_range[0], a.n_hay + 1, min(t0 + kCmpTile + kU8Look, a.total), true);
+    }
+    __syncthreads();
+    *lo = s_range[0];
+    *hi = s_range[1];
+    if (*hi - *lo <= kU8Stage) {
+        for (long long i = threadIdx.x; i < *hi - *lo; i += blockDim.x) s_off[i] = __ldg(a.off + *lo + i);
+        o.base = *lo;
+        o.staged = true;
+    }
+    __syncthreads();
+    return o;
+}
+
+/* The maximal valid prefix of the sequence that byte i of the window leads (bnd: u8_bounds): its length when it is a
+ * whole sequence, with *cp its code point; minus its length when it is not, with *cp U+FFFD */
+__device__ __forceinline__ int u8_prefix(const uint32_t (&w)[10], int i, unsigned long long bnd, uint32_t *cp) {
+    const uint32_t b0 = u8_at(w, i);
+    if (b0 < 0x80u) { *cp = b0; return 1; }
+    const int need = b0 < 0xC2u ? 0 : b0 < 0xE0u ? 2 : b0 < 0xF0u ? 3 : b0 < 0xF5u ? 4 : 0;
+    *cp = 0xFFFDu;
+    if (!need) return -1;
+    const unsigned long long after = bnd >> (i + 5);       /* haystack starts after byte i */
+    const int avail = after ? __ffsll((long long)after) : 64;
+    const uint32_t b1 = u8_at(w, i + 1), b2 = u8_at(w, i + 2), b3 = u8_at(w, i + 3);
+    const uint32_t lo = b0 == 0xE0u ? 0xA0u : b0 == 0xF0u ? 0x90u : 0x80u, hi = b0 == 0xEDu ? 0x9Fu : b0 == 0xF4u ? 0x8Fu : 0xBFu;
+    int k = 1;
+    if (avail > 1 && b1 >= lo && b1 <= hi) {
+        k = 2;
+        if (need > 2 && avail > 2 && (b2 & 0xC0u) == 0x80u) {
+            k = 3;
+            if (need > 3 && avail > 3 && (b3 & 0xC0u) == 0x80u) k = 4;
+        }
+    }
+    if (k < need) return -k;
+    *cp = need == 2 ? (b0 & 0x1Fu) << 6 | (b1 & 0x3Fu)
+        : need == 3 ? (b0 & 0x0Fu) << 12 | (b1 & 0x3Fu) << 6 | (b2 & 0x3Fu)
+                    : (b0 & 0x07u) << 18 | (b1 & 0x3Fu) << 12 | (b2 & 0x3Fu) << 6 | (b3 & 0x3Fu);
+    return k;
+}
+
+/* bit j: byte j of the group starts a letter; bytes from `valid` on (past the batch) never do */
+__device__ __forceinline__ uint32_t u8_starts(const uint32_t (&w)[10], unsigned long long bnd, int valid) {
+    uint32_t keep = 0;
+#pragma unroll
+    for (int j = 0; j < 32; j++) {
+        bool start = true;
+        if ((u8_at(w, j) & 0xC0u) == 0x80u) {
+#pragma unroll
+            for (int d = 1; d <= 3; d++) {
+                const int q = j - d;
+                if ((bnd >> (q + 5)) & ((1ULL << d) - 1)) break;      /* a haystack starts between the lead and byte j */
+                if ((u8_at(w, q) & 0xC0u) == 0x80u) continue;
+                uint32_t cp;
+                start = abs(u8_prefix(w, q, bnd, &cp)) <= d;
+                break;
+            }
+        }
+        if (start && j < valid) keep |= 1u << j;
+    }
+    return keep;
+}
+
+__device__ __forceinline__ bool u8_ascii(const uint32_t (&w)[10]) {
+    return ((w[1] | w[2] | w[3] | w[4] | w[5] | w[6] | w[7] | w[8]) & 0x80808080u) == 0;
+}
+
+__global__ void __launch_bounds__(kCmpThreads) acb_utf8_decode_kernel(const __grid_constant__ U8Args a) {
+    using Scan = cub::BlockScan<int, kCmpThreads>;
+    __shared__ typename Scan::TempStorage scan_tmp;
+    __shared__ long long s_off[kU8Stage];
+    __shared__ long long s_tile, s_range[2];
+    __shared__ unsigned int s_max;
+    if (threadIdx.x == 0) { s_tile = atomicAdd(a.ctr, 1u); s_max = 0; }   /* in claim order: every earlier tile is running or done */
+    __syncthreads();
+    const long long tile = s_tile, t0 = tile * kCmpTile, p0 = t0 + (long long)threadIdx.x * 32;
+    long long lo = 0, hi = 0;
+    const U8Offs o = u8_stage(a, t0, s_off, s_range, &lo, &hi);
+    uint32_t w[10];
+    u8_load(a.in, a.total, p0, w);
+    const int valid = (int)max(min(32LL, a.total - p0), 0LL);
+    uint32_t keep, mx = 0;
+    unsigned long long err = ~0ULL;
+    if (u8_ascii(w)) {
+        keep = valid == 32 ? ~0u : (1u << valid) - 1u;
+        uint32_t m = __vmaxu4(__vmaxu4(__vmaxu4(w[1], w[2]), __vmaxu4(w[3], w[4])), __vmaxu4(__vmaxu4(w[5], w[6]), __vmaxu4(w[7], w[8])));
+        m = __vmaxu4(m, m >> 16);
+        mx = __vmaxu4(m, m >> 8) & 255u;                   /* bytes past the batch are zero */
+    } else {
+        const unsigned long long bnd = u8_bounds(a, o, lo, hi, p0);
+        keep = u8_starts(w, bnd, valid);
+#pragma unroll
+        for (int j = 0; j < 32; j++) {
+            if (!((keep >> j) & 1)) continue;
+            uint32_t cp;
+            const int k = u8_prefix(w, j, bnd, &cp);
+            mx = max(mx, cp);
+            if (k < 0 && err == ~0ULL) err = (unsigned long long)(p0 + j) << 2 | (unsigned long long)(-k - 1);
+        }
+    }
+    int pre, agg;
+    Scan(scan_tmp).ExclusiveSum(__popc(keep), pre, agg);
+    const long long g = tile * kCmpThreads + threadIdx.x;
+    a.mask[g] = keep;
+    a.gpre[g] = (uint16_t)pre;
+    mx = __reduce_max_sync(kFull, mx);
+    if ((threadIdx.x & 31) == 0 && mx) atomicMax(&s_max, mx);
+    if (a.strict && err != ~0ULL) atomicMin(a.err, err);
+    if (threadIdx.x == 0) {                                /* decoupled look-back over the tiles before this one */
+        long long base = 0;
+        if (tile == 0) {
+            atomicExch(a.status, kLbPre | (unsigned long long)agg);
+        } else {
+            atomicExch(a.status + tile, kLbAgg | (unsigned long long)agg);
+            for (long long i = tile - 1;; --i) {
+                unsigned long long st;
+                while ((st = *reinterpret_cast<volatile unsigned long long *>(a.status + i)) == 0) {}
+                base += (long long)(st & kLbVal);
+                if (st & kLbPre) break;
+            }
+            atomicExch(a.status + tile, kLbPre | (unsigned long long)(base + agg));
+        }
+        a.tile_pre[tile] = base;
+        if (tile == a.n_tiles - 1) a.tile_pre[a.n_tiles] = base + agg;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && s_max) atomicMax(a.info + 1, (long long)s_max);
+}
+} // namespace
+
+namespace {
+/* a.loff[h] = first letter of haystack h (h = 0 .. n_hay); the longest haystack, the letter total and the error into
+ * a.info */
+__global__ void acb_utf8_offsets_kernel(const CompactMeta m, const __grid_constant__ U8Args a) {
+    const long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h > a.n_hay) return;
+    const long long s = kept_before(m, hay_start(a.off, a.stride, h));
+    a.loff[h] = s;
+    if (h < a.n_hay) {
+        const long long len = kept_before(m, hay_start(a.off, a.stride, h + 1)) - s;
+        if (len) atomicMax(a.info + 2, len);
+        return;
+    }
+    a.info[0] = s;
+    const unsigned long long e = *a.err;
+    a.info[3] = e == ~0ULL ? -1 : (long long)(e >> 2);
+    a.info[4] = e == ~0ULL ? -1 : (long long)(e >> 2) + (long long)(e & 3) + 1;
+}
+
+/* Pass 2: the letters of tile blockIdx.x at W bytes each into out (from letter tile_pre[tile] on), and out_off[h] =
+ * W * loff[h] over a grid-stride loop.  Letters of W = 1 must be below 256 (acb_utf8_write_device's caller checks) */
+template <int W>
+__global__ void __launch_bounds__(kCmpThreads) acb_utf8_write_kernel(const __grid_constant__ U8Args a, uint8_t *out, long long *out_off) {
+    using T = std::conditional_t<W == 1, uint8_t, uint32_t>;
+    __shared__ __align__(16) uint8_t s_buf[kCmpTile * W + 16];   /* the tile's letters */
+    __shared__ long long s_off[kU8Stage];
+    __shared__ long long s_range[2];
+    for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h <= a.n_hay; h += (long long)gridDim.x * blockDim.x)
+        out_off[h] = a.loff[h] * W;
+    const long long tile = blockIdx.x;
+    if (tile >= a.n_tiles) return;
+    const long long t0 = tile * kCmpTile, p0 = t0 + (long long)threadIdx.x * 32;
+    long long lo = 0, hi = 0;
+    const U8Offs o = u8_stage(a, t0, s_off, s_range, &lo, &hi);
+    uint32_t w[10];
+    u8_load(a.in, a.total, p0, w);
+    const int valid = (int)max(min(32LL, a.total - p0), 0LL);
+    T *dst = reinterpret_cast<T *>(s_buf) + a.gpre[tile * kCmpThreads + threadIdx.x];
+    if (u8_ascii(w)) {
+#pragma unroll
+        for (int j = 0; j < 32; j++)
+            if (j < valid) dst[j] = (T)u8_at(w, j);
+    } else {
+        const unsigned long long bnd = u8_bounds(a, o, lo, hi, p0);
+        const uint32_t keep = u8_starts(w, bnd, valid);
+        int n = 0;
+#pragma unroll
+        for (int j = 0; j < 32; j++) {
+            if (!((keep >> j) & 1)) continue;
+            uint32_t cp;
+            u8_prefix(w, j, bnd, &cp);
+            dst[n++] = (T)cp;
+        }
+    }
+    __syncthreads();
+    /* coalesced stores: bytes up to a 16-byte boundary of the destination, then 16-byte words, then the rest */
+    const long long first = a.tile_pre[tile];
+    uint8_t *d = out + first * W;
+    const int nb = (int)(a.tile_pre[tile + 1] - first) * W;
+    const int head = min(nb, (int)((16 - (reinterpret_cast<uintptr_t>(d) & 15)) & 15)), nmid = (nb - head) >> 4;
+    if ((int)threadIdx.x < head) d[threadIdx.x] = s_buf[threadIdx.x];
+    const int sh = (head & 3) * 8;
+    const uint32_t *sw = reinterpret_cast<const uint32_t *>(s_buf) + (head >> 2);
+    for (int i = threadIdx.x; i < nmid; i += kCmpThreads) {
+        const uint32_t *q = sw + 4 * i;                    /* unaligned by head bytes in shared memory: funnel shifts */
+        const uint32_t a0 = q[0], a1 = q[1], a2 = q[2], a3 = q[3], a4 = q[4];
+        reinterpret_cast<uint4 *>(d + head)[i] = make_uint4(__funnelshift_r(a0, a1, sh), __funnelshift_r(a1, a2, sh),
+                                                            __funnelshift_r(a2, a3, sh), __funnelshift_r(a3, a4, sh));
+    }
+    for (int i = head + (nmid << 4) + threadIdx.x; i < nb; i += kCmpThreads) d[i] = s_buf[i];
+}
+
+/* UTF-8 bytes of letter c: code points as Unicode encodes them (surrogates at 3 bytes, as "surrogatepass" does);
+ * letters from 0x110000 up become U+FFFD */
+__device__ __forceinline__ int u8_len(uint32_t c) { return c < 0x80u ? 1 : c < 0x800u ? 2 : c < 0x10000u ? 3 : c < 0x110000u ? 4 : 3; }
+
+template <int W>
+__device__ __forceinline__ uint32_t u8_letter(const uint8_t *in, long long i) {
+    return W == 1 ? (uint32_t)in[i] : reinterpret_cast<const uint32_t *>(in)[i];
+}
+
+/* encode, count pass: out_off[h] = UTF-8 bytes of haystack h (one CTA per haystack, grid-stride), out_off[n_hay] = 0 */
+template <int W>
+__global__ void __launch_bounds__(256) acb_utf8_count_kernel(const uint8_t *in, const long long *off, long long n_hay, long long *out_off) {
+    __shared__ unsigned long long s_sum;
+    for (long long h = blockIdx.x; h < n_hay; h += gridDim.x) {
+        if (threadIdx.x == 0) s_sum = 0;
+        __syncthreads();
+        const long long e = __ldg(off + h + 1) / W;
+        unsigned int sum = 0;                              /* < 2^26: at most 2^31 letters of 4 bytes over 256 threads */
+        for (long long i = __ldg(off + h) / W + threadIdx.x; i < e; i += 256) sum += u8_len(u8_letter<W>(in, i));
+        sum = __reduce_add_sync(kFull, sum);
+        if ((threadIdx.x & 31) == 0 && sum) atomicAdd(&s_sum, (unsigned long long)sum);
+        __syncthreads();
+        if (threadIdx.x == 0) out_off[h] = (long long)s_sum;
+        __syncthreads();                                   /* s_sum is set again */
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) out_off[n_hay] = 0;
+}
+
+/* encode, write pass: the UTF-8 bytes of each haystack at out + out_off[h], when the total fits out_cap */
+template <int W>
+__global__ void __launch_bounds__(256) acb_utf8_encode_kernel(const uint8_t *in, const long long *off, long long n_hay,
+                                                              const long long *out_off, uint8_t *out, long long out_cap) {
+    using Scan = cub::BlockScan<int, 256>;
+    __shared__ typename Scan::TempStorage tmp;
+    if (out_off[n_hay] > out_cap) return;
+    for (long long h = blockIdx.x; h < n_hay; h += gridDim.x) {
+        long long base = out_off[h];
+        const long long e = __ldg(off + h + 1) / W;
+        for (long long c0 = __ldg(off + h) / W; c0 < e; c0 += 256) {
+            const long long i = c0 + threadIdx.x;
+            uint32_t c = i < e ? u8_letter<W>(in, i) : 0;
+            if (c >= 0x110000u) c = 0xFFFDu;
+            const int len = i < e ? u8_len(c) : 0;
+            int pre, agg;
+            Scan(tmp).ExclusiveSum(len, pre, agg);
+            uint8_t *d = out + base + pre;
+            if (len == 1) {
+                d[0] = (uint8_t)c;
+            } else if (len == 2) {
+                d[0] = (uint8_t)(0xC0u | c >> 6); d[1] = (uint8_t)(0x80u | (c & 0x3Fu));
+            } else if (len == 3) {
+                d[0] = (uint8_t)(0xE0u | c >> 12); d[1] = (uint8_t)(0x80u | ((c >> 6) & 0x3Fu)); d[2] = (uint8_t)(0x80u | (c & 0x3Fu));
+            } else if (len == 4) {
+                d[0] = (uint8_t)(0xF0u | c >> 18); d[1] = (uint8_t)(0x80u | ((c >> 12) & 0x3Fu));
+                d[2] = (uint8_t)(0x80u | ((c >> 6) & 0x3Fu)); d[3] = (uint8_t)(0x80u | (c & 0x3Fu));
+            }
+            base += agg;
+            __syncthreads();                               /* tmp is used again */
+        }
+    }
+}
+
+thread_local float g_u8_ms[3] = {};                        /* kernel timing: decode pass 1, pass 2, encode */
+
+/* the workspace of acb_utf8_decode_device, carved in this order */
+struct U8Work {
+    long long n_tiles;
+    size_t bytes;
+    U8Work(int64_t total, int64_t n_hay) {
+        n_tiles = (total + kCmpTile - 1) / kCmpTile;
+        const size_t groups = (size_t)n_tiles * kCmpThreads;
+        auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+        bytes = up(groups * 4) + up(groups * 2) + up(((size_t)n_tiles + 1) * 8) + up((size_t)n_tiles * 8) + up(4) + up(8) +
+                up(((size_t)n_hay + 1) * 8);
+    }
+    void carve_into(void *work, U8Args &a) const {
+        char *p = static_cast<char *>(work);
+        const size_t groups = (size_t)n_tiles * kCmpThreads;
+        a.mask = carve<uint32_t>(p, groups);
+        a.gpre = carve<uint16_t>(p, groups);
+        a.tile_pre = carve<long long>(p, (size_t)n_tiles + 1);
+        a.status = carve<unsigned long long>(p, (size_t)n_tiles);
+        a.ctr = carve<unsigned int>(p, 1);
+        a.err = carve<unsigned long long>(p, 1);
+        a.loff = reinterpret_cast<long long *>(p);
+        a.n_tiles = n_tiles;
+    }
+};
+
+/* cub's scratch for the encode's exclusive sum over n_hay + 1 offsets */
+static int u8_scan_bytes(int64_t n_hay, size_t *temp) {
+    *temp = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, *temp, (long long *)nullptr, (long long *)nullptr, (int)(n_hay + 1)));
+    return ACB_OK;
+}
+
+/* f() launched on s; with kernel timing on, *ms is its time from events made for this call (the call waits for them) */
+template <class F>
+static int u8_timed(cudaStream_t s, float *ms, F &&f) {
+    if (!g_timing.load()) return f();
+    cudaEvent_t e[2] = {nullptr, nullptr};
+    int rc = ACB_OK;
+    if (cudaEventCreate(&e[0]) != cudaSuccess || cudaEventCreate(&e[1]) != cudaSuccess || cudaEventRecord(e[0], s) != cudaSuccess) {
+        acb_set_error("kernel timing events failed");
+        rc = ACB_ECUDA;
+    } else if ((rc = f()) == ACB_OK && (cudaEventRecord(e[1], s) != cudaSuccess || cudaEventSynchronize(e[1]) != cudaSuccess ||
+                                        cudaEventElapsedTime(ms, e[0], e[1]) != cudaSuccess)) {
+        acb_set_error("kernel timing events failed");
+        rc = ACB_ECUDA;
+    }
+    for (cudaEvent_t ev : e) if (ev) cudaEventDestroy(ev);
+    return rc;
+}
+
+/* the checks shared by the decode passes: batch shape, buffers, device */
+static int u8_check(int device, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
+                    const void *d_work, int64_t work_bytes) {
+    if (total_bytes < 0 || n_hay < 0 || (total_bytes && !d_in) || work_bytes < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (n_hay > 0x7fffffffLL) { acb_set_error("more than 2^31-1 haystacks in one batch"); return ACB_ERANGE; }
+    if (!d_offsets) {
+        int rc = check_stride(1, total_bytes, n_hay, stride_bytes, 0);
+        if (rc != ACB_OK) return rc;
+    }
+    const U8Work wk(total_bytes, n_hay);
+    if (wk.n_tiles > 0x7fffffffLL) { acb_set_error("batch too large to decode in one launch"); return ACB_ERANGE; }
+    if ((int64_t)wk.bytes > work_bytes || !d_work) {
+        acb_set_error("workspace of %lld bytes at %p, the batch needs %lld (acb_utf8_work_bytes)", (long long)work_bytes, d_work,
+                      (long long)wk.bytes);
+        return ACB_EINVAL;
+    }
+    if (reinterpret_cast<uintptr_t>(d_in) & 15) { acb_set_error("d_in must be 16-byte aligned"); return ACB_EINVAL; }
+    CUDA_TRY(cudaSetDevice(device));
+    return ACB_OK;
+}
+
+static void u8_args(U8Args &a, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay, int64_t stride_bytes,
+                    const void *d_work, int64_t *d_info, int strict) {
+    a = U8Args{};
+    a.in = d_in; a.total = total_bytes; a.off = reinterpret_cast<const long long *>(d_offsets); a.stride = stride_bytes; a.n_hay = n_hay;
+    a.info = reinterpret_cast<long long *>(d_info);
+    a.strict = strict;
+    U8Work(total_bytes, n_hay).carve_into(const_cast<void *>(d_work), a);
+}
+} // namespace
+
+extern "C" int acb_utf8_work_bytes(int64_t total_bytes, int64_t n_hay, int64_t *bytes) {
+    if (!bytes || total_bytes < 0 || n_hay < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (n_hay > 0x7fffffffLL - 1) { acb_set_error("more than 2^31-2 haystacks in one batch"); return ACB_ERANGE; }
+    size_t temp = 0;
+    if (int rc = u8_scan_bytes(n_hay, &temp)) return rc;
+    *bytes = (int64_t)std::max(U8Work(total_bytes, n_hay).bytes, temp + 256);
+    return ACB_OK;
+}
+
+extern "C" int acb_utf8_decode_device(int device, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                                      int64_t stride_bytes, int errors, void *d_work, int64_t work_bytes, int64_t *d_info, void *stream) {
+    DeviceRestore keep_device;
+    if (!d_info || (errors != ACB_UTF8_STRICT && errors != ACB_UTF8_REPLACE)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    int rc = u8_check(device, d_in, total_bytes, d_offsets, n_hay, stride_bytes, d_work, work_bytes);
+    if (rc) return rc;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    U8Args a;
+    u8_args(a, d_in, total_bytes, d_offsets, n_hay, stride_bytes, d_work, d_info, errors == ACB_UTF8_STRICT);
+    g_u8_ms[0] = 0.f;
+    CUDA_TRY(cudaMemsetAsync(d_info, 0, 5 * sizeof(int64_t), s));
+    CUDA_TRY(cudaMemsetAsync(a.err, 0xff, sizeof(unsigned long long), s));
+    CUDA_TRY(cudaMemsetAsync(a.ctr, 0, sizeof(unsigned int), s));
+    CUDA_TRY(cudaMemsetAsync(a.tile_pre, 0, ((size_t)a.n_tiles + 1) * sizeof(long long), s));
+    if (a.n_tiles) CUDA_TRY(cudaMemsetAsync(a.status, 0, (size_t)a.n_tiles * sizeof(unsigned long long), s));
+    const CompactMeta meta{a.mask, a.gpre, a.tile_pre, a.n_tiles};
+    return u8_timed(s, &g_u8_ms[0], [&]() -> int {
+        int r;
+        if (a.n_tiles) {
+            acb_utf8_decode_kernel<<<(unsigned)a.n_tiles, kCmpThreads, 0, s>>>(a);
+            if ((r = launched("UTF-8 decode"))) return r;
+        }
+        acb_utf8_offsets_kernel<<<(unsigned)((n_hay + 1 + 255) / 256), 256, 0, s>>>(meta, a);
+        return launched("UTF-8 offsets");
+    });
+}
+
+extern "C" int acb_utf8_write_device(int device, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                                     int64_t stride_bytes, const void *d_work, int64_t work_bytes, int width, uint8_t *d_out,
+                                     int64_t *d_out_offsets, void *stream) {
+    DeviceRestore keep_device;
+    if ((width != 1 && width != 4) || !d_out_offsets || (total_bytes && !d_out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    int rc = u8_check(device, d_in, total_bytes, d_offsets, n_hay, stride_bytes, d_work, work_bytes);
+    if (rc) return rc;
+    if (reinterpret_cast<uintptr_t>(d_out) & 15) { acb_set_error("d_out must be 16-byte aligned"); return ACB_EINVAL; }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    U8Args a;
+    u8_args(a, d_in, total_bytes, d_offsets, n_hay, stride_bytes, d_work, nullptr, 0);
+    g_u8_ms[1] = 0.f;
+    const unsigned grid = (unsigned)std::max<long long>(a.n_tiles, 1);
+    return u8_timed(s, &g_u8_ms[1], [&]() -> int {
+        auto *oo = reinterpret_cast<long long *>(d_out_offsets);
+        if (width == 1) acb_utf8_write_kernel<1><<<grid, kCmpThreads, 0, s>>>(a, d_out, oo);
+        else acb_utf8_write_kernel<4><<<grid, kCmpThreads, 0, s>>>(a, d_out, oo);
+        return launched("UTF-8 write");
+    });
+}
+
+extern "C" int acb_utf8_encode_device(int device, const uint8_t *d_in, int64_t total_bytes, const int64_t *d_offsets, int64_t n_hay,
+                                      int width, void *d_work, int64_t work_bytes, uint8_t *d_out, int64_t out_cap,
+                                      int64_t *d_out_offsets, int64_t *d_total, void *stream) {
+    DeviceRestore keep_device;
+    if ((width != 1 && width != 4) || total_bytes < 0 || n_hay < 0 || (total_bytes && !d_in) || !d_offsets || !d_out_offsets ||
+        !d_total || out_cap < 0 || (out_cap && !d_out) || work_bytes < 0) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    if (n_hay > 0x7fffffffLL - 1) { acb_set_error("more than 2^31-2 haystacks in one batch"); return ACB_ERANGE; }
+    size_t temp = 0;
+    int rc = u8_scan_bytes(n_hay, &temp);
+    if (rc) return rc;
+    if ((int64_t)temp > work_bytes || (temp && !d_work)) {
+        acb_set_error("workspace of %lld bytes at %p, the encode needs %lld (acb_utf8_work_bytes)", (long long)work_bytes, d_work, (long long)temp);
+        return ACB_EINVAL;
+    }
+    CUDA_TRY(cudaSetDevice(device));
+    int sms = 0;
+    CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    auto *off = reinterpret_cast<const long long *>(d_offsets);
+    auto *oo = reinterpret_cast<long long *>(d_out_offsets);
+    const unsigned grid = (unsigned)std::max<long long>(std::min<long long>(n_hay, (long long)sms * 16), 1);
+    g_u8_ms[2] = 0.f;
+    return u8_timed(s, &g_u8_ms[2], [&]() -> int {
+        int r;
+        if (width == 1) acb_utf8_count_kernel<1><<<grid, 256, 0, s>>>(d_in, off, n_hay, oo);
+        else acb_utf8_count_kernel<4><<<grid, 256, 0, s>>>(d_in, off, n_hay, oo);
+        if ((r = launched("UTF-8 count"))) return r;
+        CUDA_TRY(cub::DeviceScan::ExclusiveSum(d_work, temp, oo, oo, (int)(n_hay + 1), s));
+        CUDA_TRY(cudaMemcpyAsync(d_total, oo + n_hay, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+        if (!out_cap) return ACB_OK;
+        if (width == 1) acb_utf8_encode_kernel<1><<<grid, 256, 0, s>>>(d_in, off, n_hay, oo, d_out, out_cap);
+        else acb_utf8_encode_kernel<4><<<grid, 256, 0, s>>>(d_in, off, n_hay, oo, d_out, out_cap);
+        return launched("UTF-8 encode");
+    });
+}
+
+extern "C" int acb_last_utf8_ms(float *ms, int32_t n) {
+    if (!ms || n < 0 || n > 3) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    for (int i = 0; i < n; i++) ms[i] = g_u8_ms[i];
+    return ACB_OK;
+}
