@@ -738,6 +738,44 @@ int acb_utf8_encode_device(int device, const uint8_t *d_in, int64_t total_bytes,
  * this thread (the first n, n <= 3), from CUDA events made for the call (which then waits for them); 0 when timing is off. */
 int acb_last_utf8_ms(float *ms, int32_t n);
 
+/* ---- UTF-8 stream carries: the unfinished letter of each UTF-8 stream, kept on the GPU (DESIGN section 4.21) -------
+ * An acb_utf8_carry holds, per stream of a stream batch, the bytes (0 to 3) that begin a letter the stream's text has
+ * not finished yet: one 32-bit word in HBM, bytes 0..2 the held bytes and byte 3 their number.  It is separate from the
+ * acb_streams it serves; the caller feeds both with the same ids.  A UTF-8 feed is:
+ *  1. acb_utf8_carry_stage_device: per chunk h of stream s = ids[h] (ids NULL: s = h), stage carry_s || chunk_h without
+ *     its new held tail k_h into a ragged batch (d_staged at d_staged_offsets[n_chunks + 1] byte offsets), and stage
+ *     the new carry, the last k_h bytes of carry_s || chunk_h.  k_h is the length from the last non-continuation byte
+ *     among the last 3 bytes to the end, when that byte's maximal valid prefix (the rule of acb_utf8_decode_device)
+ *     runs to the end and is shorter than its sequence, or when the text ends in ED A0-BF; else 0.  So a valid but
+ *     unfinished letter is held back and a prefix that cannot be continued (E0 80, F0 8F, F4 90, C0, F5) is not: this
+ *     is the buffer CPython's incremental UTF-8 decoder keeps, which also waits for the third byte after ED A0-BF.  final != 0 (the stream's text ends here): k_h = 0, so the decode reads a held prefix as
+ *     the end of a haystack, as the decoder's final=True does.  Bytes from d_staged_offsets[n_chunks] up to total_bytes +
+ *     3 * n_chunks (the "span", at most what the staged batch can need) are set to zero, so the decode can take the span
+ *     as total_bytes without waiting for the staged size: the zeros come after the last haystack and belong to none.
+ *  2. acb_utf8_decode_device / acb_utf8_write_device on (d_staged, span, d_staged_offsets, n_chunks, 0).
+ *  3. a stream feed of the decoded letters, with their offsets.
+ *  4. acb_utf8_carry_commit_device, once that feed has succeeded: the staged carries become the streams' carries.
+ * A stage without a commit changes no carry, and a second stage restages from the committed carries.  The commit takes
+ * the ids and chunk count of the last stage (ACB_EINVAL otherwise).  Streams without a chunk keep their carry.
+ * Chunks as for acb_utf8_decode_device (d_chunks 16-byte aligned; d_offsets, any non-decreasing values, or rows of
+ * stride_bytes); d_ids int32 device ids, distinct and in range (not checked).  d_staged 16-byte aligned with staged_cap
+ * >= total_bytes + 3 * n_chunks.  Stage and commit are asynchronous on `stream`, on the carry's device.
+ * ACB_EINVAL for NULL buffers with non-zero sizes, n_chunks > n_streams, a fixed stride that does not fit, a staged
+ * buffer too small, an unaligned buffer; ACB_ERANGE for more than 2^31 - 2 chunks. */
+typedef struct acb_utf8_carry acb_utf8_carry;
+int  acb_utf8_carry_new(int device, int64_t n_streams, acb_utf8_carry **out);
+void acb_utf8_carry_free(acb_utf8_carry *c);
+/* ids[0..n) (host ids, in range: ACB_EINVAL otherwise; ids NULL: every stream) hold nothing.  Synchronises. */
+int  acb_utf8_carry_reset(acb_utf8_carry *c, const int32_t *ids, int64_t n);
+/* out[s] = the bytes stream s holds (0 to 3), cap >= n_streams.  Synchronises. */
+int  acb_utf8_carry_pending(acb_utf8_carry *c, int64_t *out, int64_t cap);
+/* the bytes stream `id` holds: *n of them in out[0..3).  Synchronises. */
+int  acb_utf8_carry_bytes(acb_utf8_carry *c, int32_t id, uint8_t *out, int32_t *n);
+int  acb_utf8_carry_stage_device(acb_utf8_carry *c, const uint8_t *d_chunks, int64_t total_bytes, const int64_t *d_offsets,
+                                 int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids, int final, uint8_t *d_staged,
+                                 int64_t staged_cap, int64_t *d_staged_offsets, void *stream);
+int  acb_utf8_carry_commit_device(acb_utf8_carry *c, const int32_t *d_ids, int64_t n_chunks, void *stream);
+
 /* number of kernel launches issued by this library so far (bench.py's gpu_launches) */
 int64_t acb_launch_count(void);
 

@@ -156,6 +156,13 @@ def lib() -> ctypes.CDLL:
         "acb_utf8_write_device": (ctypes.c_int, [ctypes.c_int, vp, i64, vp, i64, i64, vp, i64, ctypes.c_int, vp, vp, vp]),
         "acb_utf8_encode_device": (ctypes.c_int, [ctypes.c_int, vp, i64, vp, i64, ctypes.c_int, vp, i64, vp, i64, vp, vp, vp]),
         "acb_last_utf8_ms": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float), i32]),
+        "acb_utf8_carry_new": (ctypes.c_int, [ctypes.c_int, i64, ctypes.POINTER(vp)]),
+        "acb_utf8_carry_free": (None, [vp]),
+        "acb_utf8_carry_reset": (ctypes.c_int, [vp, vp, i64]),
+        "acb_utf8_carry_pending": (ctypes.c_int, [vp, vp, i64]),
+        "acb_utf8_carry_bytes": (ctypes.c_int, [vp, i32, vp, ctypes.POINTER(ctypes.c_int32)]),
+        "acb_utf8_carry_stage_device": (ctypes.c_int, [vp, vp, i64, vp, i64, i64, vp, ctypes.c_int, vp, i64, vp, vp]),
+        "acb_utf8_carry_commit_device": (ctypes.c_int, [vp, vp, i64, vp]),
         "acb_launch_count": (i64, []),
         "acb_set_kernel_timing": (ctypes.c_int, [ctypes.c_int]),
         "acb_last_kernel_ms": (ctypes.c_float, []),
@@ -193,7 +200,9 @@ EXPORTED_SYMBOLS = [
     "acb_streams_feed_words_device", "acb_streams_feed_words_host", "acb_leftmost_first_device", "acb_scan_host_leftmost_kind",
     "acb_replacer_new_kind", "acb_streams_new_leftmost_kind", "acb_table_upload_folded", "acb_expand_aliases_device",
     "acb_last_fold_ms", "acb_table_upload_folded_map", "acb_streams_new_folded", "acb_utf8_work_bytes", "acb_utf8_decode_device",
-    "acb_utf8_write_device", "acb_utf8_encode_device", "acb_last_utf8_ms", "acb_launch_count", "acb_set_kernel_timing",
+    "acb_utf8_write_device", "acb_utf8_encode_device", "acb_last_utf8_ms", "acb_utf8_carry_new",
+    "acb_utf8_carry_free", "acb_utf8_carry_reset", "acb_utf8_carry_pending", "acb_utf8_carry_bytes",
+    "acb_utf8_carry_stage_device", "acb_utf8_carry_commit_device", "acb_launch_count", "acb_set_kernel_timing",
     "acb_last_kernel_ms", "acb_last_error", "acb_abi_version",
 ]
 

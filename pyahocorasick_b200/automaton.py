@@ -1646,7 +1646,8 @@ class Automaton:
 
     def stream_batch(self, n_streams: int, *, long: bool = False, algo: str = "auto",
                      device: Optional[int] = None, ignore_white_space: bool = False,
-                     leftmost_longest: bool = False, whole_words=False, leftmost_first: bool = False) -> "StreamBatch":
+                     leftmost_longest: bool = False, whole_words=False, leftmost_first: bool = False,
+                     encoding: Optional[str] = None, errors: str = "strict") -> "StreamBatch":
         """`n_streams` independent streams searched chunk by chunk, the next chunk of many of them in one GPU call
         (StreamBatch.feed).  long=False: stream s reports what the reference's ``iter(c0)`` ... ``.set(c1)`` ...
         reports over its chunks -- every match, also those across chunk boundaries; long=True: what
@@ -1661,42 +1662,57 @@ class Automaton:
         match is reported once the letter after it has arrived (or by `finish`), so a stream holds back one letter more.
 
         Unicode flavour: streams are always scanned at 4 bytes per letter (a stream can switch between latin-1 and
-        wider chunks, so the latin-1 automaton is not used)."""
+        wider chunks, so the latin-1 automaton is not used).
+
+        encoding="utf-8" (unicode flavour, KEY_STRING keys; errors "strict" or "replace"): the chunks are UTF-8 bytes,
+        decoded on the GPU, in the input forms of find_all_batch's UTF-8 batches.  A letter may be split across chunks:
+        each stream holds back the bytes of a letter it has not finished (``pending``, at most 3) until its next feed or
+        `finish`.  The batch reports exactly what the same batch of `str` reports when each chunk is replaced by
+        ``dec.decode(chunk)`` of an incremental decoder per stream (``codecs.getincrementaldecoder("utf-8")(errors)``)
+        and `finish` is preceded by ``dec.decode(b"", final=True)``; end_index and positions count letters.  So over all
+        feeds and `finish` a stream gets what the whole-batch method with encoding="utf-8" gives for the concatenation
+        of its chunks.  Such a find_all batch (also long=True and ignore_white_space=True) has a `finish` too."""
         return self._stream_batch(n_streams, long, algo, device, ignore_white_space, leftmost_longest, whole_words,
-                                  leftmost_first, _FOLD_NONE)
+                                  leftmost_first, _FOLD_NONE, encoding, errors)
 
     def ascii_case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
                                             leftmost_longest: bool = False, leftmost_first: bool = False,
-                                            whole_words=False) -> "StreamBatch":
+                                            whole_words=False, encoding: Optional[str] = None,
+                                            errors: str = "strict") -> "StreamBatch":
         """`stream_batch` with ASCII case-insensitive matching: over all feeds (and `finish`) of a stream, what
         find_all_batch, find_leftmost_longest_batch or find_leftmost_first_batch reports for its whole text with
         ascii_case_insensitive=True and the same whole_words.  A find_all batch reports every key whose folded text
         occurs, keys of one length at one end in ascending id; a leftmost batch reports, of the keys that fold to one
         text, the one added first.  Matches are released at the same points as by the stream_batch of the same options,
         and the word test reads the letters as given.  Takes neither long nor ignore_white_space; not for KEY_SEQUENCE
-        automata.  The returned StreamBatch has ``ascii_case_insensitive`` True."""
+        automata.  The returned StreamBatch has ``ascii_case_insensitive`` True.  encoding and errors: UTF-8 chunks, as
+        for stream_batch."""
         return self._stream_batch(n_streams, False, algo, device, False, leftmost_longest, whole_words, leftmost_first,
-                                  _FOLD_ASCII)
+                                  _FOLD_ASCII, encoding, errors)
 
     def case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
                                       leftmost_longest: bool = False, leftmost_first: bool = False,
-                                      whole_words=False) -> "StreamBatch":
+                                      whole_words=False, encoding: Optional[str] = None,
+                                      errors: str = "strict") -> "StreamBatch":
         """`stream_batch` with Unicode case-insensitive matching (unicode flavour): over all feeds (and `finish`) of a
         stream, what find_all_batch, find_leftmost_longest_batch or find_leftmost_first_batch reports for its whole text
         with case_insensitive=True and the same whole_words.  A find_all batch reports every key whose folded text occurs,
         keys of one length at one end in ascending id; a leftmost batch reports, of the keys that fold to one text, the
         one added first.  Matches are released at the same points as by the stream_batch of the same options, and the
         word test reads the letters as given.  Takes neither long nor ignore_white_space; not for the bytes flavour or
-        KEY_SEQUENCE automata.  The returned StreamBatch has ``case_insensitive`` True."""
+        KEY_SEQUENCE automata.  The returned StreamBatch has ``case_insensitive`` True.  encoding and errors: UTF-8
+        chunks, as for stream_batch."""
         return self._stream_batch(n_streams, False, algo, device, False, leftmost_longest, whole_words, leftmost_first,
-                                  _FOLD_UNICODE)
+                                  _FOLD_UNICODE, encoding, errors)
 
     @_locked
     def _stream_batch(self, n_streams: int, long: bool, algo: str, device: Optional[int], ignore_white_space: bool,
-                      leftmost_longest: bool, whole_words, leftmost_first: bool, fold: int) -> "StreamBatch":
+                      leftmost_longest: bool, whole_words, leftmost_first: bool, fold: int, encoding: Optional[str] = None,
+                      errors: str = "strict") -> "StreamBatch":
         """The argument check and constructor of stream_batch, ascii_case_insensitive_stream_batch and
         case_insensitive_stream_batch (fold: the fold kind)"""
         self._require_automaton()
+        u8 = self._utf8_arg(encoding, errors)
         self._fold_arg(fold == _FOLD_ASCII, case_insensitive=fold == _FOLD_UNICODE)
         n_streams = operator.index(n_streams)
         if n_streams < 0:
@@ -1714,7 +1730,7 @@ class Automaton:
             raise ValueError("iter_long has no ignore_white_space option")
         skip = self._skip_set(False) if ignore_white_space else None
         return StreamBatch(self, n_streams, bool(long), algo, _default_device() if device is None else device, skip,
-                           bool(leftmost_longest), words, bool(leftmost_first), fold)
+                           bool(leftmost_longest), words, bool(leftmost_first), fold, u8, errors)
 
     # ------------------------------------------------------------------ batch lookups (new)
     # exists / match / longest_prefix / get for a whole batch of keys, in one GPU call (acb_lookup_*).  `keys` takes the
@@ -1913,13 +1929,28 @@ class Automaton:
 
 class _Streams:
     """What StreamBatch and ReplaceStream share: the native stream batch `_ss`, reached only through `_native`, the
-    check that the key set has not changed, stream ids, `reset` and `positions`."""
+    check that the key set has not changed, stream ids, `reset` and `positions`; for UTF-8 batches the carried bytes
+    `_carry` (acb_utf8_carry), `pending` and the staging and decoding of a feed (_utf8_stage)."""
+
+    def _init_utf8(self, u8: Optional[int], errors: str) -> None:
+        """encoding, errors and the native carries of a UTF-8 batch (u8: its errors kind, None for letters)"""
+        self._u8 = u8
+        self.encoding = None if u8 is None else "utf-8"
+        self.errors = errors
+        self._carry = None
+        if u8 is not None:
+            c = ctypes.c_void_p()
+            N.check(self._A._lib.acb_utf8_carry_new(self._device, self.n_streams, ctypes.byref(c)))
+            self._carry = c
 
     def __del__(self):
         try:
             if getattr(self, "_ss", None) is not None:
                 self._native("free")
                 self._ss = None
+            if getattr(self, "_carry", None) is not None:
+                self._A._lib.acb_utf8_carry_free(self._carry)
+                self._carry = None
         except Exception:                                   # interpreter shutdown
             pass
 
@@ -1966,7 +1997,7 @@ class _Streams:
 
     def reset(self, ids=None) -> None:
         """Streams `ids` (default: all) back to their start, as ``set(x, reset=True)`` does: position 0, nothing carried
-        over or held back."""
+        over or held back (for a UTF-8 batch, no pending bytes either)."""
         with self._A._gpu_lock:
             self._check()
             if ids is not None:
@@ -1974,8 +2005,15 @@ class _Streams:
                 if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)) or (a.size and (a.min() < 0 or a.max() >= self.n_streams)):
                     raise ValueError(f"stream ids must be integers in [0, {self.n_streams})")
                 ids = np.unique(a).astype(np.int32)
-            self._native("reset", ids)
-            self._restart(slice(None) if ids is None else ids)
+            self._reset(ids)
+
+    def _reset(self, ids: Optional[np.ndarray]) -> None:
+        """reset of streams ids (int32, distinct; None: all), under the lock"""
+        self._native("reset", ids)
+        if self._carry is not None:
+            N.check(self._A._lib.acb_utf8_carry_reset(self._carry, None if ids is None else N.ptr(ids),
+                                                      0 if ids is None else len(ids)))
+        self._restart(slice(None) if ids is None else ids)
 
     def _restart(self, streams) -> None:
         """`streams` (an index into the streams) are back at position 0: for what the Python side keeps per stream"""
@@ -1986,6 +2024,78 @@ class _Streams:
         copy)."""
         with self._A._gpu_lock:
             return self._native("positions")
+
+    @property
+    def pending(self) -> np.ndarray:
+        """int64[n_streams]: the bytes (0 to 3) each stream of a UTF-8 batch holds back because they begin a letter its
+        text has not finished yet -- what its incremental decoder would keep; not counted in `positions`.  Zeros for a
+        batch of letters.  A copy."""
+        with self._A._gpu_lock:
+            out = np.zeros(max(self.n_streams, 1), dtype=np.int64)
+            if self._carry is not None:
+                N.check(self._A._lib.acb_utf8_carry_pending(self._carry, N.ptr(out), len(out)))
+            return out[:self.n_streams]
+
+    def _utf8_stage(self, chunks, ids, final: bool) -> "_Utf8Feed":
+        """A UTF-8 feed's chunks (the input forms of a UTF-8 batch; in a list, None is an empty chunk) behind their
+        streams' carried bytes, staged (acb_utf8_carry_stage_device) and decoded to 4-byte letters on the GPU, on torch's
+        current stream.  Waits once, for the decode's info block.  Under "strict" an invalid sequence raises
+        UnicodeDecodeError for the first chunk that holds one, as its stream's incremental decoder raises it; nothing is
+        committed until _utf8_commit."""
+        import torch
+        A = self._A
+        lib = A._lib
+        if isinstance(chunks, (list, tuple)) and not _is_pair(chunks):
+            chunks = [b"" if c is None else c for c in chunks]
+        t, offs, n, stride, host = A._utf8_upload(chunks, self._device)
+        if host is None and _device_of(t) != self._device:
+            raise ValueError(f"chunks on cuda:{_device_of(t)} for a stream batch on cuda:{self._device}")
+        ids32 = self._ids(ids, n)
+        total = int(t.numel())
+        span = total + 3 * n                               # the most staged bytes: every chunk behind 3 carried ones
+        with _on_device(self._device) as stream:
+            d_ids = None if ids32 is None else torch.from_numpy(ids32).to(t.device)
+            staged = torch.empty(max(span, 16), dtype=torch.uint8, device=t.device)
+            soffs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+            N.check(lib.acb_utf8_carry_stage_device(self._carry, t.data_ptr() if total else None, total,
+                                                    None if offs is None else offs.data_ptr(), n, stride,
+                                                    None if d_ids is None else d_ids.data_ptr(), int(final),
+                                                    staged.data_ptr(), staged.numel(), soffs.data_ptr(), stream))
+            need = ctypes.c_int64(0)
+            N.check(lib.acb_utf8_work_bytes(span, n, ctypes.byref(need)))
+            work = torch.empty(int(need.value), dtype=torch.uint8, device=t.device)
+            info = torch.empty(6, dtype=torch.int64, device=t.device)
+            batch = (staged.data_ptr(), span, soffs.data_ptr(), n, 0)
+            N.check(lib.acb_utf8_decode_device(self._device, *batch, self._u8, work.data_ptr(), work.numel(), info.data_ptr(),
+                                               stream))
+            info[5:].copy_(soffs[n:])                      # the staged size, read with the info block
+            letters, _, longest, err_start, err_end, staged_total = info.tolist()
+            if err_start >= 0:
+                raise self._utf8_stream_error(t, host, stride, soffs.cpu().numpy(), ids32, err_start, err_end)
+            out = torch.empty(max((letters + span - staged_total) * 4, 16), dtype=torch.uint8, device=t.device)
+            out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
+            N.check(lib.acb_utf8_write_device(self._device, *batch, work.data_ptr(), work.numel(), 4, out.data_ptr(),
+                                              out_offs.data_ptr(), stream))
+        return _Utf8Feed(out[:letters * 4], out_offs, n, longest, ids32, d_ids)
+
+    def _utf8_stream_error(self, t, host, stride: int, soffs: np.ndarray, ids32, start: int, end: int) -> UnicodeDecodeError:
+        """The UnicodeDecodeError of the invalid sequence at staged bytes [start, end): its object is the carried bytes
+        of the chunk's stream followed by the chunk, as the stream's incremental decoder raises it"""
+        h = int(np.searchsorted(soffs, start, side="right")) - 1
+        if host is not None and host[1] is not None:
+            chunk = host[0][host[1][h]:host[1][h + 1]]
+        else:
+            chunk = host[0][h * stride:(h + 1) * stride] if host is not None else t[h * stride:(h + 1) * stride].cpu().numpy()
+        held, k = (ctypes.c_uint8 * 3)(), ctypes.c_int32(0)
+        N.check(self._A._lib.acb_utf8_carry_bytes(self._carry, h if ids32 is None else int(ids32[h]), held, ctypes.byref(k)))
+        base = int(soffs[h])
+        return _decode_error(bytes(held)[:k.value] + chunk.tobytes(), start - base, end - base)
+
+    def _utf8_commit(self, f: "_Utf8Feed") -> None:
+        """After a UTF-8 feed succeeded: the carries it staged become the streams' (acb_utf8_carry_commit_device)"""
+        with _on_device(self._device) as stream:
+            N.check(self._A._lib.acb_utf8_carry_commit_device(self._carry, None if f.d_ids is None else f.d_ids.data_ptr(), f.n,
+                                                              stream))
 
 
 class StreamBatch(_Streams):
@@ -2014,11 +2124,15 @@ class StreamBatch(_Streams):
     A batch from `Automaton.ascii_case_insensitive_stream_batch` (``ascii_case_insensitive`` True) reports what the
     batch of the same options reports, with keys and text compared ASCII case-insensitively: what the whole-batch
     method reports with ascii_case_insensitive=True for each stream's whole text.  One from
-    `Automaton.case_insensitive_stream_batch` (``case_insensitive`` True) does the same with case_insensitive=True."""
+    `Automaton.case_insensitive_stream_batch` (``case_insensitive`` True) does the same with case_insensitive=True.
+
+    A batch made with encoding="utf-8" (``encoding`` "utf-8", ``errors`` "strict" or "replace") takes UTF-8 chunks and
+    reports what the batch of `str` reports for the text each stream's incremental decoder gives (see
+    Automaton.stream_batch); ``pending`` tells the bytes of an unfinished letter each stream holds back."""
 
     def __init__(self, A: Automaton, n_streams: int, long: bool, algo: str, device: int, skip: Optional[np.ndarray] = None,
                  leftmost_longest: bool = False, words: Optional[tuple] = None, leftmost_first: bool = False,
-                 fold: int = _FOLD_NONE):
+                 fold: int = _FOLD_NONE, u8: Optional[int] = None, errors: str = "strict"):
         self._A = A
         self._fold = fold
         self.ascii_case_insensitive = fold == _FOLD_ASCII
@@ -2036,6 +2150,7 @@ class StreamBatch(_Streams):
         self._pos = np.zeros(n_streams, dtype=np.int64)        # host mirror of the positions, for end_index
         self.ignore_white_space = skip is not None
         with A._gpu_lock:
+            self._init_utf8(u8, errors)
             if words is not None:
                 self._ss = self._native("new_words")
             elif leftmost_longest or leftmost_first:
@@ -2074,10 +2189,11 @@ class StreamBatch(_Streams):
             return self._feed(op, *args)
         return super()._native(op, *args)
 
-    def _feed(self, op: str, kind: str, data, offs, n: int, stride: int, ids, flag: bool) -> np.ndarray:
+    def _feed(self, op: str, kind: str, data, offs, n: int, stride: int, ids, flag: bool, longest: Optional[int] = None) -> np.ndarray:
         """acb_streams_feed_* (flag: sort), acb_streams_feed_leftmost_* or acb_streams_feed_words_* (flag: final) -> the
         records (hay_id = chunk index, end_index in the chunk).  Overflow commits nothing: the retry is the same feed
-        again, with room."""
+        again, with room.  kind "letters": a decoded UTF-8 feed, data its letters (a CUDA tensor), offs their int64 CUDA
+        byte offsets and longest its longest chunk in letters."""
         A = self._A
         lib, algo = A._lib, N.ALGOS[self._algo]
         ordered = op != "feed"                                  # the leftmost and word feeds order their records
@@ -2092,11 +2208,14 @@ class StreamBatch(_Streams):
                 return lib.acb_streams_feed_host(*args, None, cap, found_ref, algo, int(flag))
             return A._host_records_on(self._table()[0], n, feed)
         import torch
-        t = _stream_tensor(data, n, stride, self._device)
+        if kind == "letters":
+            t, total, d_off = data, int(data.numel()), offs.data_ptr()
+        else:
+            t, total, d_off, longest = _stream_tensor(data, n, stride, self._device), n * stride, None, stride // A._L
         tb = self._table()[0]
         with _on_device(self._device) as stream:
             d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
-            args = (self._ss, tb, t.data_ptr() if n and stride else None, n * stride, None, n, stride,
+            args = (self._ss, tb, t.data_ptr() if total else None, total, d_off, n, stride,
                     None if d_ids is None else d_ids.data_ptr())
 
             def feed(out, cap, cnt):
@@ -2109,7 +2228,7 @@ class StreamBatch(_Streams):
             out, found = A._device_scan(t, n, feed)
             if ordered:
                 return out[:found].cpu().numpy().view(N.MATCH_DTYPE).reshape(-1)
-            return A._device_records(tb, out, found, n, stride // A._L, stream, flag)
+            return A._device_records(tb, out, found, n, longest, stream, flag)
 
     def _stream_matches(self, rec: np.ndarray, n: int, ids32) -> Tuple[Matches, np.ndarray]:
         """A feed's records (hay_id = chunk index, end_index in the chunk) -> (Matches with stream ids and positions in
@@ -2127,10 +2246,19 @@ class StreamBatch(_Streams):
         """The next chunk of some streams: chunk h continues stream ids[h] (default: stream h).  `chunks` takes the
         input forms of find_all_batch; in a list, None is an empty chunk.  Returns the matches that end inside
         these chunks (see the class); a leftmost_longest or whole_words batch returns the matches this feed settles,
-        already in order (`sort` has no effect)."""
+        already in order (`sort` has no effect).
+
+        A UTF-8 batch takes the UTF-8 forms of find_all_batch (a list or tuple of bytes / bytearray, None an empty
+        chunk; (flat uint8, int64 byte offsets); uint8[n, stride]; a uint8 CUDA tensor [n, stride] on the batch's
+        device) and reports what the batch of `str` reports for ``dec.decode(chunk)`` of each stream's incremental
+        decoder.  Under errors="strict" an invalid sequence raises the UnicodeDecodeError that decoder raises for the
+        first chunk (in call order) holding one -- its object is the stream's pending bytes followed by the chunk --
+        and the feed changes no stream."""
         A = self._A
         with A._gpu_lock:
             self._check()
+            if self._u8 is not None:
+                return self._feed_utf8(chunks, ids, sort, False)
             b, lens = _stream_chunks(A, chunks)
             ids32 = self._ids(ids, b.n)
             leftmost = self.leftmost_longest or self.leftmost_first
@@ -2145,20 +2273,48 @@ class StreamBatch(_Streams):
     def finish(self, ids=None) -> Matches:
         """leftmost_longest, leftmost_first and whole_words batches: the matches streams `ids` (default: all) still hold
         back, as if their text ended here; those streams then start again at position 0 with nothing held.  Other stream
-        batches: ValueError."""
+        batches of letters: ValueError.
+
+        A UTF-8 batch first decodes each stream's pending bytes as the end of its text, as ``dec.decode(b"",
+        final=True)`` does: U+FFFD under errors="replace", UnicodeDecodeError ("unexpected end of data", nothing changed)
+        under "strict".  A UTF-8 find_all batch (plain, long=True or ignore_white_space=True) has a finish too: it returns
+        the matches that end in those last letters, then the streams start again at position 0, as after `reset`."""
         leftmost = self.leftmost_longest or self.leftmost_first
-        if not (leftmost or self.whole_words):
+        if not (leftmost or self.whole_words or self._u8 is not None):
             raise ValueError("finish() belongs to leftmost_longest, leftmost_first and whole_words stream batches")
         A = self._A
         with A._gpu_lock:
             self._check()
             n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
+            if self._u8 is not None:
+                ids32 = self._ids(ids, n)
+                m = self._feed_utf8([b""] * n, ids32, True, True)
+                if leftmost or self.whole_words:           # the final feed returned the streams to their start
+                    self._restart(slice(None) if ids32 is None else ids32)
+                else:                                      # a find_all feed is never final: start again as reset does
+                    self._reset(ids32)
+                return m
             ids32 = self._ids(ids, n)
             rec = self._native("feed_leftmost" if leftmost else "feed_words", "host", np.empty(0, np.uint8),
                                np.zeros(n + 1, np.int64), n, 0, ids32, True)
             m, sid = self._stream_matches(rec, n, ids32)
             self._restart(sid)
             return m
+
+    def _feed_utf8(self, chunks, ids, sort: bool, final: bool) -> Matches:
+        """A feed (final: the last, of finish) of a UTF-8 batch: stage and decode (_utf8_stage), the feed of this batch's
+        form on the letters, then the carries committed and the positions moved"""
+        f = self._utf8_stage(chunks, ids, final)
+        leftmost = self.leftmost_longest or self.leftmost_first
+        if leftmost or self.whole_words:
+            rec = self._native("feed_leftmost" if leftmost else "feed_words", "letters", f.data, f.offsets, f.n, 0, f.ids, final,
+                               f.longest)
+        else:
+            rec = self._native("feed", "letters", f.data, f.offsets, f.n, 0, f.ids, sort, f.longest)
+        self._utf8_commit(f)
+        m, sid = self._stream_matches(rec, f.n, f.ids)
+        self._pos[sid] += np.diff(f.offsets.cpu().numpy()) // 4
+        return m
 
 
 class Replacer:
@@ -2323,43 +2479,41 @@ class Replacer:
                 letters = torch.empty(max(m, 16), dtype=torch.uint8, device=t.device)[:m]
                 if m:
                     N.check(A._lib.acb_replace_device(*args, letters.data_ptr(), m, total.data_ptr(), stream))
-            need = ctypes.c_int64(0)
-            N.check(A._lib.acb_utf8_work_bytes(0, n, ctypes.byref(need)))
-            work = torch.empty(int(need.value), dtype=torch.uint8, device=t.device)
-            cap = letters.numel() // width * (2 if width == 1 else 4)     # the most UTF-8 bytes a letter takes at this width
-            out = torch.empty(max(cap, 1), dtype=torch.uint8, device=t.device)
-            out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
-            total = torch.empty(1, dtype=torch.int64, device=t.device)
-            N.check(A._lib.acb_utf8_encode_device(dev, letters.data_ptr() if letters.numel() else None, letters.numel(),
-                                                  offs.data_ptr(), n, width, work.data_ptr(), work.numel(), out.data_ptr(),
-                                                  cap, out_offs.data_ptr(), total.data_ptr(), stream))
-            return out[:int(total.item())], out_offs
+            return _utf8_encode(A._lib, letters, offs, n, width, dev, stream)
 
     def stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
-                     whole_words=False) -> "ReplaceStream":
+                     whole_words=False, encoding: Optional[str] = None, errors: str = "strict") -> "ReplaceStream":
         """`n_streams` streams rewritten chunk by chunk (ReplaceStream.feed): over all feeds and `finish` of a stream,
         the output is exactly what `replace_batch` gives for its whole text, with the same whole_words.  Streams run at
-        the automaton's full letter width (unicode: 4 bytes per letter), as every stream batch does."""
-        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_NONE)
+        the automaton's full letter width (unicode: 4 bytes per letter), as every stream batch does.
+
+        encoding="utf-8" (see Automaton.stream_batch): UTF-8 chunks in, UTF-8 out; concatenated, a stream's outputs are
+        ``replace_batch([whole text], encoding="utf-8", errors=errors)``.  A replacement UTF-8 cannot encode (a lone
+        surrogate) raises UnicodeEncodeError here."""
+        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_NONE, encoding, errors)
 
     def ascii_case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
-                                            whole_words=False) -> "ReplaceStream":
+                                            whole_words=False, encoding: Optional[str] = None,
+                                            errors: str = "strict") -> "ReplaceStream":
         """`stream_batch` with ASCII case-insensitive matching: over all feeds and `finish` of a stream, the output is
         exactly what `replace_batch` gives for its whole text with ascii_case_insensitive=True and the same whole_words.
         Each match takes the replacement of the key added first among those that fold to its text; every other letter,
-        held ones included, keeps its own case.  The returned ReplaceStream has ``ascii_case_insensitive`` True."""
-        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_ASCII)
+        held ones included, keeps its own case.  The returned ReplaceStream has ``ascii_case_insensitive`` True.
+        encoding and errors: UTF-8 chunks and output, as for stream_batch."""
+        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_ASCII, encoding, errors)
 
     def case_insensitive_stream_batch(self, n_streams: int, *, algo: str = "auto", device: Optional[int] = None,
-                                      whole_words=False) -> "ReplaceStream":
+                                      whole_words=False, encoding: Optional[str] = None,
+                                      errors: str = "strict") -> "ReplaceStream":
         """`stream_batch` with Unicode case-insensitive matching (unicode flavour): over all feeds and `finish` of a
         stream, the output is exactly what `replace_batch` gives for its whole text with case_insensitive=True and the
         same whole_words.  Each match takes the replacement of the key added first among those that fold to its text;
         every other letter, held ones included, keeps its own case.  The returned ReplaceStream has ``case_insensitive``
-        True."""
-        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_UNICODE)
+        True.  encoding and errors: UTF-8 chunks and output, as for stream_batch."""
+        return self._stream_batch(n_streams, algo, device, whole_words, _FOLD_UNICODE, encoding, errors)
 
-    def _stream_batch(self, n_streams: int, algo: str, device: Optional[int], whole_words, fold: int) -> "ReplaceStream":
+    def _stream_batch(self, n_streams: int, algo: str, device: Optional[int], whole_words, fold: int,
+                      encoding: Optional[str] = None, errors: str = "strict") -> "ReplaceStream":
         """The argument check and constructor of stream_batch, ascii_case_insensitive_stream_batch and
         case_insensitive_stream_batch (fold: the fold kind)"""
         A = self._A
@@ -2367,6 +2521,9 @@ class Replacer:
             if self._version != A._version:
                 raise ValueError("underlaying automaton has changed, iterator is not valid anymore")
             A._require_automaton()
+            u8 = A._utf8_arg(encoding, errors)
+            if u8 is not None:
+                self._check_utf8_replacements()
             A._fold_arg(fold == _FOLD_ASCII, case_insensitive=fold == _FOLD_UNICODE)
             n_streams = operator.index(n_streams)
             if n_streams < 0:
@@ -2374,7 +2531,7 @@ class Replacer:
             if algo not in ("auto", "filter", "dfa"):
                 raise ValueError(f"algo {algo!r}: a replacing stream batch takes 'auto', 'filter' or 'dfa'")
             words = A._words(whole_words)
-            return ReplaceStream(self, n_streams, algo, self._device if device is None else device, words, fold)
+            return ReplaceStream(self, n_streams, algo, self._device if device is None else device, words, fold, u8, errors)
 
     def _items(self, out: np.ndarray, offs: np.ndarray, narrow: bool) -> list:
         """the output haystacks as objects of the input's type"""
@@ -2447,9 +2604,11 @@ class ReplaceStream(_Streams):
     stream holds back one letter more: the output before ``position - longest_word`` is released.  From
     `Replacer.ascii_case_insensitive_stream_batch` (``ascii_case_insensitive`` True), the output is what replace_batch
     gives with ascii_case_insensitive=True, released at the same points; from `Replacer.case_insensitive_stream_batch`
-    (``case_insensitive`` True), what it gives with case_insensitive=True."""
+    (``case_insensitive`` True), what it gives with case_insensitive=True.  From a factory with encoding="utf-8", the
+    chunks and the output are UTF-8 (``pending``: the bytes of an unfinished letter each stream holds back)."""
 
-    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int, words: Optional[tuple] = None, fold: int = _FOLD_NONE):
+    def __init__(self, R: Replacer, n_streams: int, algo: str, device: int, words: Optional[tuple] = None, fold: int = _FOLD_NONE,
+                 u8: Optional[int] = None, errors: str = "strict"):
         self._R = R
         self._fold = fold
         self.ascii_case_insensitive = fold == _FOLD_ASCII
@@ -2462,12 +2621,14 @@ class ReplaceStream(_Streams):
         self._words = words
         self.whole_words = words is not None
         with self._A._gpu_lock:
+            self._init_utf8(u8, errors)
             self._ss = self._native("new")
 
     def _native(self, op: str, *args):
         """Every call into the native batch goes through here.  new -> handle;  free;  reset(ids int32 or None);
         positions -> int64[n_streams];  feed(kind, data, offsets, n, stride, ids, final) -> (output bytes, output
-        offsets int64[n+1]), numpy arrays for host chunks, CUDA tensors for a CUDA tensor"""
+        offsets int64[n+1]), numpy arrays for host chunks, CUDA tensors for a CUDA tensor or for kind "letters" (a
+        decoded UTF-8 feed: data its letters, offsets their int64 CUDA byte offsets, stride 0)"""
         A = self._A
         lib = A._lib
         if op == "new":
@@ -2489,16 +2650,19 @@ class ReplaceStream(_Streams):
                 None if ids is None else N.ptr(ids), int(final), algo, N.ptr(out_offs), N.ptr(out), out.size, total_ref))
             return out, out_offs
         import torch
-        t = _stream_tensor(data, n, stride, self._device)
+        if kind == "letters":
+            t, size, d_off = data, int(data.numel()), offs.data_ptr()
+        else:
+            t, size, d_off = _stream_tensor(data, n, stride, self._device), n * stride, None
         with _on_device(self._device) as stream:
             d_ids = None if ids is None else torch.from_numpy(ids).to(t.device)
             out_offs = torch.empty(n + 1, dtype=torch.int64, device=t.device)
             total = torch.empty(1, dtype=torch.int64, device=t.device)
-            cap = (n * stride + held) * 5 // 4 + 4096
+            cap = (size + held) * 5 // 4 + 4096
             for retry in (False, True):
                 out = torch.empty(cap, dtype=torch.uint8, device=t.device)
-                N.check(lib.acb_streams_replace_device(self._ss, r, tb, t.data_ptr() if n and stride else None, n * stride,
-                                                       None, n, stride, None if d_ids is None else d_ids.data_ptr(),
+                N.check(lib.acb_streams_replace_device(self._ss, r, tb, t.data_ptr() if size else None, size,
+                                                       d_off, n, stride, None if d_ids is None else d_ids.data_ptr(),
                                                        int(final), out_offs.data_ptr(), out.data_ptr(), cap,
                                                        total.data_ptr(), stream, algo))
                 m = int(total.item())                       # the size of the output
@@ -2512,10 +2676,18 @@ class ReplaceStream(_Streams):
         """The next chunk of some streams (chunk h continues stream ids[h], default stream h), in the input forms of
         find_all_batch; in a list, None is an empty chunk.  Returns the output each chunk releases: a list gives a list
         of the same item type, uint8[n, stride] or (flat, offsets) gives (flat uint8, offsets int64[n+1]), a CUDA
-        tensor gives that pair as CUDA tensors computed on torch's current stream."""
+        tensor gives that pair as CUDA tensors computed on torch's current stream.
+
+        A UTF-8 batch takes the UTF-8 forms of StreamBatch.feed and returns UTF-8: a list of bytes for a list, (flat
+        uint8, int64 byte offsets[n+1]) for an array or pair, that pair as CUDA tensors for a CUDA tensor.  Errors are
+        raised as by StreamBatch.feed, and a feed that raises changes no stream."""
         A = self._A
         with A._gpu_lock:
             self._check()
+            if self._u8 is not None:
+                form = "pair" if isinstance(chunks, np.ndarray) or _is_pair(chunks) else \
+                    "list" if isinstance(chunks, (list, tuple)) else "device"
+                return self._feed_utf8(chunks, ids, False, form)
             b, _ = _stream_chunks(A, chunks)
             out, offs = self._native("feed", *b[:5], self._ids(ids, b.n), False)
             if isinstance(chunks, np.ndarray) or _is_pair(chunks) or b.kind == "device":
@@ -2524,13 +2696,34 @@ class ReplaceStream(_Streams):
 
     def finish(self, ids=None) -> list:
         """The output streams `ids` (default: all) still hold back, one item of the haystack type per id; those streams
-        then start again at position 0 with nothing held."""
+        then start again at position 0 with nothing held.  A UTF-8 batch decodes each stream's pending bytes as the end
+        of its text first (see StreamBatch.finish) and returns a list of bytes."""
         A = self._A
         with A._gpu_lock:
             self._check()
             n = self.n_streams if ids is None else len(np.asarray(ids).reshape(-1))
+            if self._u8 is not None:
+                return self._feed_utf8([b""] * n, self._ids(ids, n), True, "list")
             out, offs = self._native("feed", "host", np.empty(0, np.uint8), np.zeros(n + 1, np.int64), n, 0, self._ids(ids, n), True)
             return self._R._items(out, offs, False)
+
+
+    def _feed_utf8(self, chunks, ids, final: bool, form: str):
+        """A replacing feed of a UTF-8 batch: stage and decode (_utf8_stage), rewrite, commit the carries, encode the
+        released letters to UTF-8 on the GPU; form "list" (a list of bytes), "pair" (numpy flat and offsets) or "device"
+        (CUDA tensors)"""
+        f = self._utf8_stage(chunks, ids, final)
+        letters, offs = self._native("feed", "letters", f.data, f.offsets, f.n, 0, f.ids, final)
+        self._utf8_commit(f)
+        with _on_device(self._device) as stream:
+            out, offs = _utf8_encode(self._A._lib, letters, offs, f.n, 4, self._device, stream)
+        if form == "device":
+            return out, offs
+        out, offs = out.cpu().numpy(), offs.cpu().numpy()
+        if form == "pair":
+            return out, offs
+        raw, o = out.tobytes(), offs.tolist()
+        return [raw[o[i]:o[i + 1]] for i in range(f.n)]
 
 
 class AutomatonSearchIter:
@@ -2751,6 +2944,18 @@ class _Utf8Batch(NamedTuple):
     narrow: bool
 
 
+class _Utf8Feed(NamedTuple):
+    """A UTF-8 feed staged and decoded on the GPU (_Streams._utf8_stage): data, its 4-byte letters (1-D uint8 CUDA
+    tensor, 16-byte aligned); offsets, their int64 CUDA byte offsets [n + 1]; longest, the longest chunk in letters;
+    ids, the stream ids (int32 or None) and d_ids, their CUDA copy."""
+    data: Any
+    offsets: Any
+    n: int
+    longest: int
+    ids: Optional[np.ndarray]
+    d_ids: Any
+
+
 def _utf8_error(t, host, stride: int, start: int, end: int) -> UnicodeDecodeError:
     """CPython's UnicodeDecodeError for the invalid sequence at bytes [start, end) of a UTF-8 batch: the haystack that
     holds it, and the sequence's place in it"""
@@ -2762,13 +2967,36 @@ def _utf8_error(t, host, stride: int, start: int, end: int) -> UnicodeDecodeErro
         hs = start // stride * stride
         he = hs + stride
     hay = bytes((host[0][hs:he] if host is not None else t[hs:he].cpu().numpy()).tobytes())
-    if not 0xC2 <= hay[start - hs] <= 0xF4:
+    return _decode_error(hay, start - hs, end - hs)
+
+
+def _decode_error(hay: bytes, start: int, end: int) -> UnicodeDecodeError:
+    """CPython's UnicodeDecodeError for the invalid sequence at bytes [start, end) of hay"""
+    if not 0xC2 <= hay[start] <= 0xF4:
         reason = "invalid start byte"
-    elif end - hs == len(hay):
+    elif end == len(hay):
         reason = "unexpected end of data"
     else:
         reason = "invalid continuation byte"
-    return UnicodeDecodeError("utf-8", hay, start - hs, end - hs, reason)
+    return UnicodeDecodeError("utf-8", hay, start, end, reason)
+
+
+def _utf8_encode(lib, letters, offs, n: int, width: int, dev: int, stream):
+    """letters of `width` bytes (a CUDA tensor) at the int64 CUDA byte offsets offs [n + 1] -> their UTF-8, encoded on
+    the GPU (acb_utf8_encode_device) on `stream`: (flat uint8, int64 byte offsets [n + 1]) CUDA tensors.  Waits once,
+    for the size."""
+    import torch
+    need = ctypes.c_int64(0)
+    N.check(lib.acb_utf8_work_bytes(0, n, ctypes.byref(need)))
+    work = torch.empty(int(need.value), dtype=torch.uint8, device=letters.device)
+    cap = letters.numel() // width * (2 if width == 1 else 4)     # the most UTF-8 bytes a letter takes at this width
+    out = torch.empty(max(cap, 1), dtype=torch.uint8, device=letters.device)
+    out_offs = torch.empty(n + 1, dtype=torch.int64, device=letters.device)
+    total = torch.empty(1, dtype=torch.int64, device=letters.device)
+    N.check(lib.acb_utf8_encode_device(dev, letters.data_ptr() if letters.numel() else None, letters.numel(),
+                                       offs.data_ptr(), n, width, work.data_ptr(), work.numel(), out.data_ptr(),
+                                       cap, out_offs.data_ptr(), total.data_ptr(), stream))
+    return out[:int(total.item())], out_offs
 
 
 class _Batch(NamedTuple):

@@ -5930,3 +5930,307 @@ extern "C" int acb_last_utf8_ms(float *ms, int32_t n) {
     for (int i = 0; i < n; i++) ms[i] = g_u8_ms[i];
     return ACB_OK;
 }
+
+/* ------------------------------------------------------------ UTF-8 stream carries (DESIGN section 4.21) */
+/* Per stream, the bytes of an unfinished letter that a UTF-8 stream holds back from one feed to the next, in one 32-bit
+ * word: bytes 0..2 the held bytes, byte 3 their number (0..3).  A stage builds, per chunk h of stream s, carry_s ||
+ * chunk_h without its new held tail into a ragged batch the UTF-8 decode takes as it is, and stages the new tail in a
+ * second word per chunk; a commit copies the staged words to the streams.  The held tail is the one CPython's
+ * incremental decoder keeps: the bytes from the last non-continuation byte among the last 3 to the end, when that
+ * byte's maximal valid prefix (u8_prefix's rule) runs to the end and is shorter than its sequence, and also ED A0-BF,
+ * which CPython keeps until a third byte arrives. */
+namespace {
+constexpr int kU8cTile = 4096;                             /* staged bytes per block turn of the gather */
+constexpr int kU8cHays = 512;                              /* staged offsets a gather block keeps in shared memory */
+
+struct U8cArgs {
+    const uint8_t *in; long long total; const long long *off; long long stride; long long n;   /* the caller's chunks */
+    const int32_t *ids; long long n_streams;
+    const uint32_t *carry; uint32_t *next;                 /* per stream; per chunk */
+    long long *soff;                                       /* staged byte offsets [n + 1] */
+    uint8_t *staged; long long span;                       /* staged bytes, zero from soff[n] to span */
+    int final;
+};
+
+__device__ __forceinline__ long long u8c_stream(const U8cArgs &a, long long h) {
+    const long long s = a.ids ? (long long)__ldg(a.ids + h) : h;
+    return (s >= 0 && s < a.n_streams) ? s : -1;
+}
+
+/* the held tail of a text whose last m (<= 3) bytes are bytes 0..m-1 of v */
+__device__ __forceinline__ int u8c_hold(uint32_t v, int m) {
+    for (int p = m - 1; p >= 0; --p) {
+        const uint32_t b0 = (v >> (8 * p)) & 255u;
+        if ((b0 & 0xC0u) == 0x80u) continue;
+        const int d = m - p, need = b0 < 0xC2u ? 0 : b0 < 0xE0u ? 2 : b0 < 0xF0u ? 3 : b0 < 0xF5u ? 4 : 0;
+        if (d >= need) return 0;
+        const uint32_t b1 = (v >> (8 * (p + 1))) & 255u;   /* the bytes after b0 are continuation bytes */
+        /* as u8_prefix, except that ED A0-BF is held: CPython's decoder waits for a third byte before it calls it invalid */
+        const uint32_t lo = b0 == 0xE0u ? 0xA0u : b0 == 0xF0u ? 0x90u : 0x80u, hi = b0 == 0xF4u ? 0x8Fu : 0xBFu;
+        return d == 1 || (b1 >= lo && b1 <= hi) ? d : 0;
+    }
+    return 0;
+}
+
+/* next[h] = the new held tail of chunk h's stream; soff[h] = bytes of carry || chunk without it (soff[n] = 0), for the
+ * exclusive scan that makes them offsets */
+__global__ void acb_u8c_len_kernel(const __grid_constant__ U8cArgs a) {
+    for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h <= a.n; h += (long long)gridDim.x * blockDim.x) {
+        if (h == a.n) { a.soff[h] = 0; continue; }
+        const long long s = u8c_stream(a, h);
+        const uint32_t c = s < 0 ? 0u : a.carry[s];
+        const int cl = (int)(c >> 24);
+        const long long b0 = hay_start(a.off, a.stride, h), len = cl + hay_start(a.off, a.stride, h + 1) - b0;
+        const int m = (int)min(len, 3LL);
+        uint32_t v = 0;                                    /* the last m bytes of carry || chunk */
+        for (int j = 0; j < m; j++) {
+            const long long i = len - m + j;
+            v |= (i < cl ? (c >> (8 * i)) & 255u : (uint32_t)__ldg(a.in + b0 + i - cl)) << (8 * j);
+        }
+        const int k = a.final ? 0 : u8c_hold(v, m);
+        a.next[h] = (uint32_t)k << 24 | (k ? v >> (8 * (m - k)) : 0u);
+        a.soff[h] = len - k;
+    }
+}
+
+/* last j in [lo, hi] with o(j) <= x, o(lo) <= x */
+template <class O>
+__device__ __forceinline__ long long u8c_find(const O &o, long long lo, long long hi, long long x) {
+    while (lo < hi) {
+        const long long mid = (lo + hi + 1) >> 1;
+        if (o(mid) <= x) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+/* The ragged gather: staged haystack h = [soff[h], soff[h+1]) is its stream's carried bytes, then its chunk, up to its
+ * length; bytes from soff[n] to span are zero.  Blocks take tiles of kU8cTile staged bytes, start at the tile's first
+ * haystack ts[t] (acb_sl_tiles_kernel) and keep the following offsets in shared memory; each thread writes one 16-byte
+ * block, from two aligned 16-byte loads (rp_load16) when it lies in one chunk's bytes, else byte by byte. */
+static_assert(kU8cTile == kSlTile, "the gather's tiles are those acb_sl_tiles_kernel finds");
+__global__ void __launch_bounds__(256) acb_u8c_gather_kernel(const __grid_constant__ U8cArgs a, const long long *ts) {
+    __shared__ long long s_off[kU8cHays + 1];
+    const long long n_tiles = (a.span + kU8cTile - 1) / kU8cTile, total = __ldg(a.soff + a.n);
+    for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const long long c0 = t * kU8cTile, h0 = a.n ? __ldg(ts + t) : 0;
+        __syncthreads();                                   /* the previous tile's readers are done */
+        const int nh = (int)min((long long)kU8cHays, a.n - h0);
+        for (int j = threadIdx.x; j <= nh; j += blockDim.x) s_off[j] = __ldg(a.soff + h0 + j);
+        __syncthreads();
+        const long long c = c0 + (long long)threadIdx.x * 16;
+        if (c >= a.span) continue;
+        if (c >= total) {                                  /* the zeros after the last haystack */
+            if (c + 16 <= a.span) *reinterpret_cast<uint4 *>(a.staged + c) = make_uint4(0u, 0u, 0u, 0u);
+            else for (long long o = c; o < a.span; o++) a.staged[o] = 0;
+            continue;
+        }
+        const auto O = [&](long long j) { return j - h0 <= nh ? s_off[j - h0] : __ldg(a.soff + j); };
+        const auto F = [&](long long from, long long x) { return u8c_find(O, from, x < s_off[nh] ? h0 + nh - 1 : a.n - 1, x); };
+        long long h = F(h0, c), lo = O(h), hi = O(h + 1), src = 0;
+        uint32_t cw = 0;                                   /* the carry of haystack h's stream */
+        const auto enter = [&]() {
+            const long long s = u8c_stream(a, h);
+            cw = s < 0 ? 0u : a.carry[s];
+            src = hay_start(a.off, a.stride, h) - (long long)(cw >> 24);   /* chunk byte of staged byte lo, less the carry */
+        };
+        enter();
+        if (c - lo >= (long long)(cw >> 24) && c + 16 <= hi) {
+            *reinterpret_cast<uint4 *>(a.staged + c) = rp_load16(a.in, src + (c - lo));
+            continue;
+        }
+        uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const long long o = c + j;
+            if (o < total) {
+                if (o >= hi) { h = F(h + 1, o); lo = O(h); hi = O(h + 1); enter(); }
+                const long long rel = o - lo;
+                const uint32_t b = rel < (long long)(cw >> 24) ? (cw >> (8 * rel)) & 255u : (uint32_t)__ldg(a.in + src + rel);
+                w[j >> 2] |= b << (8 * (j & 3));
+            }
+        }
+        if (c + 16 <= a.span) {
+            *reinterpret_cast<uint4 *>(a.staged + c) = make_uint4(w[0], w[1], w[2], w[3]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 16; j++)
+                if (c + j < a.span) a.staged[c + j] = (uint8_t)(w[j >> 2] >> (8 * (j & 3)));
+        }
+    }
+}
+
+/* carry[stream of chunk h] = next[h] */
+__global__ void acb_u8c_commit_kernel(const int32_t *ids, long long n, long long n_streams, const uint32_t *next, uint32_t *carry) {
+    for (long long h = (long long)blockIdx.x * blockDim.x + threadIdx.x; h < n; h += (long long)gridDim.x * blockDim.x) {
+        const long long s = ids ? (long long)__ldg(ids + h) : h;
+        if (s >= 0 && s < n_streams) carry[s] = next[h];
+    }
+}
+
+/* carry[ids[i]] = 0 */
+__global__ void acb_u8c_clear_kernel(const int32_t *ids, long long n, long long n_streams, uint32_t *carry) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long s = ids[i];
+        if (s >= 0 && s < n_streams) carry[s] = 0u;
+    }
+}
+} // namespace
+
+struct acb_utf8_carry {
+    int device = 0;
+    int sm_count = 1;
+    long long n = 0;
+    uint32_t *d_carry = nullptr;                           /* [n]: the committed tails */
+    uint32_t *d_next = nullptr;                            /* [n]: the tails the last stage made, per chunk */
+    long long staged = -1;                                 /* chunks of the last stage, -1 after a commit */
+    long long *d_ts = nullptr; size_t ts_cap = 0;          /* the first staged haystack of every gather tile */
+    int32_t *d_ids = nullptr; size_t ids_cap = 0;          /* the ids of a reset */
+    uint8_t *d_tmp = nullptr; size_t tmp_cap = 0;          /* cub scratch */
+};
+
+/* a grid-stride launch over `items`: a block per 256, at most 16 per SM */
+static unsigned u8c_blocks(const acb_utf8_carry *c, long long items) {
+    return (unsigned)std::max<long long>(std::min<long long>((items + 255) / 256, (long long)c->sm_count * 16), 1);
+}
+
+extern "C" void acb_utf8_carry_free(acb_utf8_carry *c) {
+    DeviceRestore keep_device;
+    if (!c) return;
+    cudaSetDevice(c->device);
+    cudaFree(c->d_carry); cudaFree(c->d_next); cudaFree(c->d_ids); cudaFree(c->d_tmp); cudaFree(c->d_ts);
+    delete c;
+}
+
+extern "C" int acb_utf8_carry_new(int device, int64_t n_streams, acb_utf8_carry **out) {
+    DeviceRestore keep_device;
+    if (!out || n_streams < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    *out = nullptr;
+    if (n_streams > 0x7fffffffLL) { acb_set_error("more than 2^31-1 streams"); return ACB_ERANGE; }
+    CUDA_TRY(cudaSetDevice(device));
+    acb_utf8_carry *c = new (std::nothrow) acb_utf8_carry();
+    if (!c) { acb_set_error("out of memory"); return ACB_ENOMEM; }
+    c->device = device;
+    c->n = n_streams;
+    const size_t n = (size_t)std::max<int64_t>(n_streams, 1);
+    cudaError_t e = cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device);
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&c->d_carry), n * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMemset(c->d_carry, 0, n * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&c->d_next), n * sizeof(uint32_t));
+    if (e != cudaSuccess) {
+        acb_set_error("allocating the carries of %lld streams: %s", (long long)n_streams, cudaGetErrorString(e));
+        acb_utf8_carry_free(c);
+        return ACB_ECUDA;
+    }
+    *out = c;
+    return ACB_OK;
+}
+
+extern "C" int acb_utf8_carry_reset(acb_utf8_carry *c, const int32_t *ids, int64_t n) {
+    DeviceRestore keep_device;
+    if (!c || n < 0 || (n && !ids)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    for (int64_t i = 0; ids && i < n; i++)
+        if (ids[i] < 0 || ids[i] >= c->n) { acb_set_error("stream id %d out of range [0, %lld)", ids[i], c->n); return ACB_EINVAL; }
+    CUDA_TRY(cudaSetDevice(c->device));
+    if (!ids) {
+        CUDA_TRY(cudaMemset(c->d_carry, 0, (size_t)std::max<long long>(c->n, 1) * sizeof(uint32_t)));
+        return ACB_OK;
+    }
+    if (n == 0) return ACB_OK;
+    int rc = ensure(&c->d_ids, &c->ids_cap, (size_t)n);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpy(c->d_ids, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice));
+    acb_u8c_clear_kernel<<<u8c_blocks(c, n), 256>>>(c->d_ids, n, c->n, c->d_carry);
+    if ((rc = launched("UTF-8 carry reset"))) return rc;
+    CUDA_TRY(cudaDeviceSynchronize());
+    return ACB_OK;
+}
+
+extern "C" int acb_utf8_carry_pending(acb_utf8_carry *c, int64_t *out, int64_t cap) {
+    DeviceRestore keep_device;
+    if (!c || cap < c->n || (c->n && !out)) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (!c->n) return ACB_OK;
+    CUDA_TRY(cudaSetDevice(c->device));
+    std::vector<uint32_t> w;
+    try { w.resize((size_t)c->n); } catch (const std::exception &) { acb_set_error("out of host memory"); return ACB_ENOMEM; }
+    CUDA_TRY(cudaMemcpy(w.data(), c->d_carry, (size_t)c->n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (long long s = 0; s < c->n; s++) out[s] = (int64_t)(w[s] >> 24);
+    return ACB_OK;
+}
+
+extern "C" int acb_utf8_carry_bytes(acb_utf8_carry *c, int32_t id, uint8_t *out, int32_t *n) {
+    DeviceRestore keep_device;
+    if (!c || !out || !n || id < 0 || id >= c->n) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    CUDA_TRY(cudaSetDevice(c->device));
+    uint32_t w = 0;
+    CUDA_TRY(cudaMemcpy(&w, c->d_carry + id, sizeof(w), cudaMemcpyDeviceToHost));
+    *n = (int32_t)(w >> 24);
+    for (int j = 0; j < 3; j++) out[j] = (uint8_t)(w >> (8 * j));
+    return ACB_OK;
+}
+
+extern "C" int acb_utf8_carry_stage_device(acb_utf8_carry *c, const uint8_t *d_chunks, int64_t total_bytes, const int64_t *d_offsets,
+                                           int64_t n_chunks, int64_t stride_bytes, const int32_t *d_ids, int final, uint8_t *d_staged,
+                                           int64_t staged_cap, int64_t *d_staged_offsets, void *stream) {
+    DeviceRestore keep_device;
+    if (!c || total_bytes < 0 || n_chunks < 0 || (total_bytes && !d_chunks) || !d_staged_offsets || staged_cap < 0) {
+        acb_set_error("bad argument");
+        return ACB_EINVAL;
+    }
+    if (n_chunks > 0x7fffffffLL - 1) { acb_set_error("more than 2^31-2 chunks in one feed"); return ACB_ERANGE; }
+    if (n_chunks > c->n) { acb_set_error("%lld chunks for %lld streams", (long long)n_chunks, c->n); return ACB_EINVAL; }
+    if (!d_offsets) {
+        int rc = check_stride(1, total_bytes, n_chunks, stride_bytes, 0);
+        if (rc != ACB_OK) return rc;
+    }
+    const long long span = total_bytes + 3 * n_chunks;
+    if (staged_cap < span || (span && !d_staged)) {
+        acb_set_error("staged buffer of %lld bytes, the feed needs %lld (total_bytes + 3 * n_chunks)", (long long)staged_cap, span);
+        return ACB_EINVAL;
+    }
+    if ((reinterpret_cast<uintptr_t>(d_staged) | reinterpret_cast<uintptr_t>(d_chunks)) & 15) {
+        acb_set_error("d_chunks and d_staged must be 16-byte aligned");
+        return ACB_EINVAL;
+    }
+    CUDA_TRY(cudaSetDevice(c->device));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    U8cArgs a;
+    memset(&a, 0, sizeof(a));
+    a.in = d_chunks; a.total = total_bytes; a.off = reinterpret_cast<const long long *>(d_offsets); a.stride = stride_bytes; a.n = n_chunks;
+    a.ids = d_ids; a.n_streams = c->n; a.carry = c->d_carry; a.next = c->d_next;
+    a.soff = reinterpret_cast<long long *>(d_staged_offsets); a.staged = d_staged; a.span = span; a.final = final ? 1 : 0;
+    acb_u8c_len_kernel<<<u8c_blocks(c, n_chunks + 1), 256, 0, s>>>(a);
+    int rc = launched("UTF-8 carry lengths");
+    if (rc) return rc;
+    size_t temp = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, temp, a.soff, a.soff, (int)(n_chunks + 1), s));
+    if ((rc = ensure(&c->d_tmp, &c->tmp_cap, temp))) return rc;
+    temp = c->tmp_cap;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(c->d_tmp, temp, a.soff, a.soff, (int)(n_chunks + 1), s));
+    if (span) {
+        const long long n_tiles = (span + kU8cTile - 1) / kU8cTile;
+        if ((rc = ensure(&c->d_ts, &c->ts_cap, (size_t)n_tiles))) return rc;
+        if (n_chunks) {
+            acb_sl_tiles_kernel<<<u8c_blocks(c, n_tiles), 256, 0, s>>>(a.soff, n_chunks, span, c->d_ts);
+            if ((rc = launched("UTF-8 carry gather tiles"))) return rc;
+        }
+        acb_u8c_gather_kernel<<<(unsigned)std::min<long long>(n_tiles, (long long)c->sm_count * 8), 256, 0, s>>>(a, c->d_ts);
+        if ((rc = launched("UTF-8 carry gather"))) return rc;
+    }
+    c->staged = n_chunks;
+    return ACB_OK;
+}
+
+extern "C" int acb_utf8_carry_commit_device(acb_utf8_carry *c, const int32_t *d_ids, int64_t n_chunks, void *stream) {
+    DeviceRestore keep_device;
+    if (!c || n_chunks < 0) { acb_set_error("bad argument"); return ACB_EINVAL; }
+    if (n_chunks != c->staged) {
+        acb_set_error("a commit of %lld chunks after a stage of %lld (-1: none since the last commit)", (long long)n_chunks, c->staged);
+        return ACB_EINVAL;
+    }
+    CUDA_TRY(cudaSetDevice(c->device));
+    c->staged = -1;
+    if (n_chunks == 0) return ACB_OK;
+    acb_u8c_commit_kernel<<<u8c_blocks(c, n_chunks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(d_ids, n_chunks, c->n, c->d_next,
+                                                                                                          c->d_carry);
+    return launched("UTF-8 carry commit");
+}
